@@ -1,12 +1,16 @@
 """bench.py -- headline metric of BASELINE.json: video frames/s through tokenize + decode_from_code_indices,
 17x128x128 clips, bf16, README config (BASELINE.json configs[1]), data-parallel over N GPUs of one node.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
          bench.py --gpus N --steps K --warmup W
 
 A "step" is one pass of the hot path over one batch of 4 synthetic clips per GPU (weak scaling: the batch
 is sharded by clip, no data-path collective in eval -- SURVEY.md 8e).  Prints ONE JSON line (rank 0).
+
+--dump-outputs DIR writes what the last timed step computed (rank 0) as DIR/<name>.npy: the code indices (float64) and
+the reconstruction (float32) that a caller of tokenize + decode_from_code_indices receives.  Weights and inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 
 --impl reference times the reference's own CPU implementation of the path: the reference is pure Python and
 cannot travel to the GPU box, so this arm runs the restated oracle (oracle/restated.py, pinned bit-for-bit to
@@ -63,11 +67,12 @@ def _peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- upper bounds, not measured rates
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -256,6 +261,21 @@ def cpu_baseline_sample():
                       + ", ".join(f"{k}: {v:.2f}" for k, v in rates.items()) + f"; value = {best}"}
 
 
+def _host_outputs(res):
+    """The arrays a caller of the timed step receives, as float64 (integer codes, exact) or float32 numpy arrays:
+    (codes, recon) for tokenize + decode, the model's output tuple in train mode (tensors only, by position)."""
+    import torch
+    items = res if isinstance(res, (tuple, list)) else (res,)
+    names = ("codes", "recon") if len(items) == 2 else tuple(f"out{i}" for i in range(len(items)))
+    out = {}
+    for name, t in zip(names, items):
+        if not torch.is_tensor(t):
+            continue
+        t = t.detach().cpu()
+        out[name] = t.double().numpy() if not t.is_floating_point() else t.float().numpy()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -267,7 +287,11 @@ def main():
     # consecutive steps (independent batches) are issued round-robin on this many CUDA streams, each replaying its own
     # CUDA-graph instances (magvit2_pytorch_b200.StreamLanes); 1 = strictly serial steps
     ap.add_argument("--lanes", type=int, default=int(os.environ.get("MV2_LANES", "3")))
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (rank 0) as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         if args.steps == 400 and args.warmup == 5:
             args.steps, args.warmup = 3, 1
@@ -325,7 +349,7 @@ def main():
     from magvit2_pytorch_b200 import HostRoundTrip, StreamLanes
     nl = max(1, args.lanes)
     if args.workload == "cfg4" and "MV2_LANES" not in os.environ and args.lanes == 3:
-        nl = 1     # measured (profiles/r02_bench_cfg4*.json): the 256^2 step is power limited (SM clock 1635 MHz with 3 lanes); 1 lane is faster
+        nl = 1     # the 256^2 step is large enough to fill the GPU on its own
     lanes = StreamLanes(model, nl)
     clk = ClockSampler(local)
     if rank == 0:
@@ -341,10 +365,13 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(args.steps):
-        lanes.run(step, dev_batches[i % NB])
+        last, _ = lanes.run(step, dev_batches[i % NB])
     lanes.join()                         # the timing stream waits for every lane: all K steps end inside the timed region
     e1.record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        # copied out before the e2e and profiling passes below replay (and overwrite) the graphs' output buffers
+        dumped = _host_outputs(last)
     ms = e0.elapsed_time(e1)
     launches = eng.launches - l0
     clocks = clk.stop() if rank == 0 else None
@@ -364,7 +391,7 @@ def main():
     # HostRoundTrip (the package's pinned-host front end) runs copy-in / kernels / copy-out on three streams, so the
     # copies of neighbouring steps overlap this step's kernels -- every step still copies its own input and results
     out_bufs = [(out_codes, out_video), (torch.empty_like(out_codes).pin_memory(), torch.empty_like(out_video).pin_memory())]
-    depth = max(2, nl)           # one staging slot per lane (two per lane measured 2 % slower: profiles/README.md)
+    depth = max(2, nl)           # one device staging slot per lane
     out_bufs += [(torch.empty_like(out_codes).pin_memory(), torch.empty_like(out_video).pin_memory()) for _ in range(depth - 2)]
     hrt = HostRoundTrip(model, depth=depth, train_mode_forward=train_mode, lanes=nl)
     cur = torch.cuda.current_stream()
@@ -389,7 +416,7 @@ def main():
     h2d = host_batches[0].numel() * host_batches[0].element_size()
     d2h = out_codes.numel() * out_codes.element_size() + out_video.numel() * 2
 
-    # ---------------- roofline of the dominant kernel (tcgen05 implicit-GEMM conv), timed live ----------
+    # ---------------- roofline of the dominant kernel (wgmma implicit-GEMM conv), timed live ----------
     # instrumented pass: CUDA events around every conv launch of one step, on the launching stream
     peaks, peaks_src = _peaks()
     roofline = None
@@ -400,27 +427,20 @@ def main():
         ms3, n3, fl3 = prof["conv3d"]
         msa, na, fla = prof["all"]
         ach = fl3 / (ms3 / 1e3) / 1e12
-        # which measured peak applies (B200_PROFILING.md): the burst figure while the SM clock holds its maximum (short
+        # which peak applies: the burst figure while the SM clock holds its maximum (short
         # timed region, no power cap seen), the sustained one once the run is long enough to be power limited
         pk_burst, pk_sus = peaks["bf16_tflops"], peaks["bf16_tflops_sustained"]
         sm_now, sm_max = (clocks or {}).get("sm_mhz"), (clocks or {}).get("sm_max_mhz")
-        # (sw_power_cap shows up within milliseconds on this path, but the clock only dips ~2 %: the cuBLAS "sustained" figure
-        #  was taken at a 1387 MHz median and does not describe that regime, so the decision is made on the clock itself)
         power_limited = bool(sm_now and sm_max and sm_now < 0.90 * sm_max)
         pk = pk_sus if power_limited else pk_burst
         traffic = None
-        try:     # dram__bytes_read + write per conv3d launch, from the committed ncu capture of one step (profiles/)
-            if args.workload == "readme":
-                traffic = json.load(open(os.path.join(ROOT, "profiles", "r02_step_metrics_summary.json")))["conv3d"]["avg_dram_bytes"]
-        except Exception:
-            traffic = None
         roofline = {"bound": "tensor", "achieved": ach, "peak": pk, "unit": "TFLOP/s", "frac": ach / pk, "traffic": traffic,
                     "frac_of_burst_peak": ach / pk_burst, "frac_of_sustained_peak": ach / pk_sus,
                     "kernel": "tc_slab_kernel on the causal 3x3x3 Conv3d layers (82% of the step's FLOPs)",
                     "launches_per_step": n3, "kernel_ms_per_step": ms3, "flop_per_launch_avg": fl3 / max(n3, 1),
                     "flops": "algorithmic: 2*B*T*H*W*Co*Ci*kt*kh*kw per launch (conv_in counted with its 3x7x7x7 taps, not the padded K)",
-                    "peak_source": f"MEASURED_PEAKS.json {'bf16_tflops_sustained (SM clock fell below 90% of max: power-limited run)' if power_limited else 'bf16_tflops (burst figure: the SM clock stayed within 10% of its maximum during the timed region)'} ({peaks_src})",
-                    "all_tcgen05_launches": {"launches_per_step": na, "ms_per_step": msa,
+                    "peak_source": f"{peaks_src}: {'bf16_tflops_sustained (SM clock fell below 90% of max: power-limited run)' if power_limited else 'bf16_tflops (burst figure: the SM clock stayed within 10% of its maximum during the timed region)'}",
+                    "all_tensor_core_launches": {"launches_per_step": na, "ms_per_step": msa,
                                              "achieved": fla / (msa / 1e3) / 1e12, "frac": fla / (msa / 1e3) / 1e12 / pk},
                     "whole_step_frac": (FLOP_PER_CLIP_ALL * CLIPS_PER_GPU * world * args.steps / (ms_max / 1e3) / 1e12)
                                        / (pk * world)}
@@ -436,7 +456,7 @@ def main():
                        "global_batch": CLIPS_PER_GPU * world, "parallelism": f"dp{world}",
                        "lanes": f"{nl} CUDA stream lane(s) per GPU: consecutive steps (independent batches) overlap on the device; "
                                 "ms_per_step = timed region / steps",
-                       "l2": f"inputs rotate over {NB} distinct batches per rank ({NB * h2d / 1e6:.0f} MB > 126 MB L2); "
+                       "l2": f"inputs rotate over {NB} distinct batches per rank ({NB * h2d / 1e6:.0f} MB > 50 MB L2); "
                              "per-step activation working set ~2 GB"},
             "clocks": clocks,
             "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
@@ -449,6 +469,11 @@ def main():
         if world == 1 and not args.no_cpu_baseline and args.workload == "readme":
             out["cpu_baseline"] = cpu_baseline_sample()
         print(json.dumps(out), flush=True)
+        if args.dump_outputs:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            import numpy as np
+            for name, arr in dumped.items():
+                np.save(os.path.join(args.dump_outputs, f"{name}.npy"), arr)
     if world > 1:
         dist.destroy_process_group()
 

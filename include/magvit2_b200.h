@@ -1,5 +1,5 @@
 /*
- * magvit2_b200.h -- C ABI of libmagvit2_b200.so, the sm_100a compute library behind
+ * magvit2_b200.h -- C ABI of libmagvit2_b200.so, the sm_90a compute library behind
  * the VideoTokenizer forward path (tokenize / decode_from_code_indices / forward).
  *
  * The reference (lucidrains/magvit2-pytorch @ a00519fa) has NO native / FFI layer of
@@ -20,7 +20,7 @@
  *   - activations are channels-last ("NDHWC"): x[b][t][h][w][c], dtype MV2_F32 or
  *     MV2_BF16; accumulation is always fp32; biases / gammas / tiny SE + quantiser
  *     weights are fp32.
- *   - there is NO CPU fallback: every function launches sm_100a kernels.
+ *   - there is NO CPU fallback: every function launches sm_90a kernels.
  */
 #ifndef MAGVIT2_B200_H
 #define MAGVIT2_B200_H
@@ -47,10 +47,10 @@ enum {
 
 int mv2_abi_version(void);
 const char* mv2_last_error(void);
-/* Compute capability of the current device as major*10+minor (100 on B200), <0 on error. */
+/* Compute capability of the current device as major*10+minor (90 on H100), <0 on error. */
 int mv2_device_arch(void);
 /* Programmatic dependent launch: when on, every kernel is launched with
- * cudaLaunchAttributeProgrammaticStreamSerialization so its prologue (barrier init, TMEM allocation, bias staging,
+ * cudaLaunchAttributeProgrammaticStreamSerialization so its prologue (barrier init, bias staging,
  * block scheduling) overlaps the tail of the previous kernel of the stream; all kernels execute griddepcontrol.wait
  * before touching activations.  Returns the previous setting.  Off by default. */
 int mv2_set_pdl(int on);
@@ -225,11 +225,11 @@ int mv2_gateloop_scan(const void* qkva, const void* res, void* out, int dtype, i
 int mv2_mse(const void* a, int a_dtype, const void* b, int b_dtype, int64_t n, void* workspace, float* out, void* stream);
 size_t mv2_mse_workspace_bytes(void);
 
-/* ---- tcgen05 / TMA implicit-GEMM convolution (bf16 in, fp32 accumulate in TMEM) ------------
+/* ---- wgmma / TMA implicit-GEMM convolution (bf16 in, fp32 accumulate in registers) ------------
  * Same operator family and epilogue as mv2_conv_forward, for bf16 activations, executed on the
- * 5th-generation tensor cores: TMA box loads with out-of-bounds zero fill implement the causal /
+ * Hopper tensor cores (wgmma): TMA box loads with out-of-bounds zero fill implement the causal /
  * spatial halo (no padded copy, reference M:924-928), strided convs read through stride-phase
- * tensor maps, accumulators live in TMEM.  Weights are packed K-major: w[co][tap][ci] (bf16);
+ * tensor maps, accumulators live in registers.  Weights are packed K-major: w[co][tap][ci] (bf16);
  * for depth-to-space / depth-to-time stores the host permutes the Co rows to co' = q*Cy + c
  * (q = p1*2+p2 or p) so that the shuffled stores are channel-contiguous; bias is permuted alike.
  * Requirements (mv2_tc_conv_supported): Ci % 16 == 0, strides in {1,2}, <= 64 taps.            */
@@ -258,8 +258,8 @@ int mv2_tc_conv_supported(const mv2_tc_conv_args* a);
 int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream);
 /* "Slab" variant for stride-1 convs with an in-plane kernel (the causal 3x3x3 residual convs): persistent
  * CTAs, one haloed activation slab per (frame, 64-channel slice) staged in shared memory once and reused by
- * all k_h*k_w in-plane taps, two 128-position M-tiles sharing each weight tile, double-buffered TMEM
- * accumulators.  Requirements (mv2_tc_slab_supported): stride 1, Ci % 64 == 0, Co % 32 == 0, no shuffle.   */
+ * all k_h*k_w in-plane taps, up to four 128-position M-tiles sharing each weight tile (mw * N tile <= 128 columns of
+ * register accumulators).  Requirements (mv2_tc_slab_supported): stride 1, Ci % 64 == 0, Co % 32 == 0, no shuffle.   */
 int mv2_tc_slab_supported(const mv2_tc_conv_args* a);
 int mv2_tc_slab_forward(const mv2_tc_conv_args* a, void* stream);
 /* SpatialDownsample2x (M:770-780: per-frame Conv2d k3 s2 p1) on the slab design: the input is read as (W/2) x (2C) with
@@ -271,7 +271,7 @@ int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream);
 /* Launch plan of mv2_tc_slab_forward for a layer shape on a device with n_sm SMs -- pure host arithmetic (no CUDA call,
  * the pointers in `a` are not dereferenced), exposed so the tiling rule and the static tile schedule can be checked
  * without a GPU.  mv2_tc_slab_plan: out6 = {M-tiles per weight tile (mw), N tile width (bn), N tiles, total tiles,
- * grid size, TMEM accumulator buffers}.  mv2_tc_slab_tile: the k-th tile that persistent CTA `cta` processes:
+ * grid size, activation-slab ring depth}.  mv2_tc_slab_tile: the k-th tile that persistent CTA `cta` processes:
  * out6 = {tile id or -1 when the CTA has no k-th tile, clip b, frame t, h0, w0, first output column n0}. */
 int mv2_tc_slab_plan(const mv2_tc_conv_args* a, int n_sm, int* out6);
 int mv2_tc_slab_tile(const mv2_tc_conv_args* a, int n_sm, int cta, int k, int* out6);
@@ -295,8 +295,8 @@ int mv2_scale_channels(const void* x, const float* scale, void* out, int dtype, 
 /* ---- fused ResidualUnit front half (reference M:937-941 + the pooling half of SqueezeExcite M:229-233) ----------------
  * One launch computes  y = ELU(Conv3d_1x1x1(ELU(CausalConv3d_ktxkhxkw(x))))  for C -> C channels (C = 64 or 128, the
  * HBM-bound levels of the README config): the ELU'd 3x3x3 tile never leaves the SM -- it is written to shared memory as the
- * A operand of a second tcgen05.mma against the 1x1x1 weights -- and the second epilogue emits, next to y, one SqueezeExcite
- * pool record (max logit, sum e, sum e * y[C]; e = exp(logit - max), logit = <y, se_wk> + se_bk) per TMEM lane quarter of a tile,
+ * A operand of a second wgmma against the 1x1x1 weights -- and the second epilogue emits, next to y, one SqueezeExcite
+ * pool record (max logit, sum e, sum e * y[C]; e = exp(logit - max), logit = <y, se_wk> + se_bk) per 32-position quarter of a tile,
  * which mv2_se_gate_records combines (replaces mv2_conv_forward x2 + mv2_se_pool for these layers).
  * w3: bf16 [C][kt*kh*kw*C] (K-major, as mv2_tc_conv_args.w); w1: bf16 [C][C]; b3 / b1 / se_wk: fp32 [C].
  * se_ws: workspace of mv2_tc_ru_workspace_bytes(a) bytes; records per frame = mv2_tc_ru_records(a).                     */

@@ -1,4 +1,4 @@
-"""magvit2_pytorch_b200 -- B200-native (sm_100a) VideoTokenizer forward path.
+"""magvit2_pytorch_b200 -- H100-native (sm_90a) VideoTokenizer forward path.
 
 Drop-in for ``magvit2_pytorch.VideoTokenizer`` inference (tokenize / decode_from_code_indices /
 forward) behind the C ABI of libmagvit2_b200.so.  See DESIGN.md / INTEGRATION.md.

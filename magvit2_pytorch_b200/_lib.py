@@ -46,7 +46,7 @@ class AttnArgs(C.Structure):
 
 
 class TcConvArgs(C.Structure):
-    """mv2_tc_conv_args (tcgen05 implicit-GEMM path; see include/magvit2_b200.h)."""
+    """mv2_tc_conv_args (wgmma implicit-GEMM path; see include/magvit2_b200.h)."""
     _fields_ = [
         ("x", C.c_void_p), ("w", C.c_void_p), ("bias", C.c_void_p), ("res", C.c_void_p), ("y", C.c_void_p),
         ("B", C.c_int32), ("Ti", C.c_int32), ("Hi", C.c_int32), ("Wi", C.c_int32), ("Ci", C.c_int32),

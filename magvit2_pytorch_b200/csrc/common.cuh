@@ -1,4 +1,4 @@
-// Shared helpers for libmagvit2_b200.so (sm_100a only).
+// Shared helpers for libmagvit2_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -92,7 +92,7 @@ struct PerDeviceOnce {
 };
 
 // ---- programmatic dependent launch (PDL) ---------------------------------------------------------------------
-// Every kernel of the library starts with pdl_wait() (everything before it -- barrier init, TMEM allocation, bias
+// Every kernel of the library starts with pdl_wait() (everything before it -- barrier init, bias
 // staging -- may overlap the tail of the previous kernel in the stream) and signals pdl_launch_dependents() right
 // after, so the next kernel's CTAs move in as this kernel's CTAs retire.  Without the launch attribute both
 // instructions are no-ops.  mv2_set_pdl(1) turns the attribute on for all launches.

@@ -3,7 +3,7 @@
 // These cover every operator of the VideoTokenizer forward path for ANY shape and for both
 // activation dtypes.  They are (a) the whole fp32 parity path (fp32 storage + fp32 FMA, no
 // TF32), (b) the memory-bound operators of the bf16 path (SqueezeExcite, norms, attention
-// cores, GEGLU, quantisers, layout), and (c) the on-device cross-check for the tcgen05
+// cores, GEGLU, quantisers, layout), and (c) the on-device cross-check for the wgmma
 // implicit-GEMM kernels in tc_conv.cu, which take over the dense contractions in bf16.
 //
 // Reference semantics are cited per entry point in include/magvit2_b200.h.
@@ -16,6 +16,18 @@
 namespace mv2 {
 
 int g_pdl = 0;
+
+// Cap for the grid of a grid-stride elementwise kernel: `per_sm` blocks on every SM of the current device.
+static int grid_cap(int per_sm) {
+  static thread_local int dev_cached = -1, n_sm = 132;
+  int dev = 0;
+  if (cudaGetDevice(&dev) == cudaSuccess && dev != dev_cached) {
+    int v = 0;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) n_sm = v;
+    dev_cached = dev;
+  }
+  return n_sm * per_sm;
+}
 static thread_local char g_err[512] = "";
 void set_error(const char* fmt, ...) {
   va_list ap;
@@ -108,7 +120,7 @@ static int dispatch_transpose(const void* src, int sd, void* dst, int dd, int B,
 }
 
 
-// Video ingest for the tcgen05 conv_in: packs the k_w taps of the (tiny-channel) input into the channel axis so the
+// Video ingest for the tensor-core conv_in: packs the k_w taps of the (tiny-channel) input into the channel axis so the
 // 7x7x7, C_in = 3 conv becomes a (7x7x1)-tap conv over 32 "channels":
 //   dst[b][t + t_pad][h][w][dw * C + c] = src[b][c][t][h][w + dw - pw]   (0 outside the image / for padded channels)
 // One block per (b, t, h) image row: the C source rows are staged in shared memory with a zero halo (coalesced
@@ -433,7 +445,11 @@ __global__ void __launch_bounds__(256) se_pool_online_kernel(const __nv_bfloat16
 #pragma unroll
       for (int u = 0; u < VEC / 8; ++u) raw[uu][u] = ok[uu] ? src[u] : make_uint4(0, 0, 0, 0);
     }
-    __syncthreads();                                // every thread has its rows in registers: the stage can be refilled
+    // every thread has its rows in registers: the stage can be refilled.  The refill is an async-proxy write, so the
+    // generic-proxy reads above must be ordered before it explicitly; without the fence the bulk copy may overwrite rows
+    // that have not been read yet.
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
     if (tid == 0 && bi + SE_STAGES < n_batches) issue(bi + SE_STAGES);
     // the U rows are folded in together: one running-max update, one rescale of the accumulators and U + 1 exponentials
     // per batch (the row-at-a-time recurrence serialised 2 exponentials and a full rescale per row)
@@ -588,7 +604,6 @@ __global__ void __launch_bounds__(256) se_out_kernel(const float* __restrict__ h
 #pragma unroll
   for (int u = 0; u < 8; ++u) acc[u] = 0.f;
   // unrolled so that the weight loads of 8 steps are in flight together: the kernel is a chain of load latencies
-  // (measured 11.8 -> 6.5 us at C = 512; the same pragma on se_hidden_kernel's loops made that kernel slower)
 #pragma unroll 8
   for (int j = lane; j < Hd; j += 32) {
     const float hv = sm[j];
@@ -1635,7 +1650,7 @@ __global__ void __launch_bounds__(128) linattn_reduce_mma_kernel(const __nv_bflo
   // Token-major staging [token][feature] (one token per thread, 16-byte stores: a 176-byte row pitch puts the 32 rows of a warp
   // in 8 distinct bank groups = the minimal 4 wavefronts per store); the MMA wants A = phi^T [feature][token], which
   // ldmatrix.trans delivers straight from the token-major tile.  (The former feature-major layout needed 160 two-byte stores
-  // per token and was shared-memory wavefront bound: ncu L1/shared 80 %.)
+  // per token and was bound by shared-memory wavefronts.)
   extern __shared__ __align__(16) unsigned char lam_dyn[];
   __nv_bfloat16 (*phi_s)[LAM_RS] = reinterpret_cast<__nv_bfloat16 (*)[LAM_RS]>(lam_dyn);                                // [token][feature] hi
   __nv_bfloat16 (*phi_l)[LAM_RS] = reinterpret_cast<__nv_bfloat16 (*)[LAM_RS]>(lam_dyn + (size_t)LAM_TB * LAM_RS * 2);  // lo
@@ -2330,8 +2345,8 @@ static int se_rows_per_block(int dtype, int F, int P, int C) {
     const int v = atoi(env);
     if (v >= SE_MIN_ROWS && v <= 4096 && (v & (v - 1)) == 0) return v;
   }
-  // measured (profiles/r02_sweep_small.json, r01 se_pool notes): L2-resident small frames want 64 - 128-row chunks (fewer, longer
-  // bulk-copy pipelines, fewer records to merge than 32-row chunks: -15 .. -30 %); large frames amortise the per-block merge
+  // small (L2-resident) frames take 64 - 128-row chunks: fewer, longer bulk-copy pipelines and fewer records to merge than
+  // 32-row chunks; large frames amortise the per-block merge over longer chunks
   if (P <= 256) return 64;
   if (P <= 1024) return 128;
   if (P <= 4096) return 512;
@@ -2472,7 +2487,7 @@ int mv2_scale_channels(const void* x, const float* scale, void* out, int dtype, 
                        void* stream) {
   MV2_CHECK_ARG(x && scale && out && B > 0 && positions_per_clip > 0 && C > 0);
   const int64_t per_clip = positions_per_clip * C, total = per_clip * B;
-  const int blocks = (int)std::min<int64_t>((total + 255) / 256, 148 * 32);
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, grid_cap(32));
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32) launch_k(scale_channels_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)x, scale, (float*)out, total, per_clip, C);
   else if (dtype == MV2_BF16) launch_k(scale_channels_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, scale, (__nv_bfloat16*)out, total, per_clip, C);
@@ -2501,7 +2516,7 @@ int mv2_pad_cl(const void* src, void* dst, int dtype, int B, int T, int H, int W
   if (mode == 1) MV2_CHECK_ARG(pt < T && ph < H && pw < W);          // torch's reflection padding requires pad < size
   if (mode == 3) MV2_CHECK_ARG(pt <= T && ph <= H && pw <= W);
   const int64_t total = (int64_t)B * (T + pt) * (H + 2 * ph) * (W + 2 * pw) * C;
-  const int blocks = (int)std::min<int64_t>((total + 255) / 256, 148 * 32);
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, grid_cap(32));
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32) launch_k(pad_cl_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)src, (float*)dst, B, T, H, W, C, pt, ph, pw, mode);
   else if (dtype == MV2_BF16) launch_k(pad_cl_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)src, (__nv_bfloat16*)dst, B, T, H, W, C, pt, ph, pw, mode);
@@ -2514,13 +2529,13 @@ int mv2_gate_residual(const void* y, const void* x, const float* gates, void* ou
                       void* stream) {
   MV2_CHECK_ARG(y && x && gates && out && F > 0 && P > 0 && C > 0);
   const int64_t total = (int64_t)F * P * C;
-  const int blocks = (int)((total + 255) / 256 > 148 * 32 ? 148 * 32 : (total + 255) / 256);
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, grid_cap(32));
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32)
     launch_k(gate_residual_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)y, (const float*)x, gates, (float*)out, total, (int64_t)P * C, C);
   else if (dtype == MV2_BF16 && C % 8 == 0) {
     const int64_t total8 = total / 8;
-    const int b8 = (int)std::min<int64_t>((total8 + 255) / 256, 148 * 16);
+    const int b8 = (int)std::min<int64_t>((total8 + 255) / 256, grid_cap(16));
     launch_k(gate_residual_bf16x8_kernel, dim3(b8), dim3(256), 0, st, (const uint4*)y, (const uint4*)x, gates, (uint4*)out, total8, (int64_t)P * C / 8, C / 8);
   } else if (dtype == MV2_BF16)
     launch_k(gate_residual_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)y, (const __nv_bfloat16*)x, gates, (__nv_bfloat16*)out, total, (int64_t)P * C, C);
@@ -2541,7 +2556,7 @@ int mv2_rmsnorm(const void* x, void* out, int dtype, const float* gamma, int B, 
     {
       const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
       __nv_bfloat16* ob = (__nv_bfloat16*)out;
-      int tpw = 1;      // measured on the (L2-resident) README shapes, profiles/r02_sweep_small.json: 1 token per warp 23.7 / 14.4 us, 4: 27.7 / 20.3 us
+      int tpw = 1;      // tokens per warp; 1 keeps the most warps in flight on the small README shapes
       if (const char* env = getenv("MV2_RN_TPW")) { const int v = atoi(env); if (v == 1 || v == 2 || v == 4) tpw = v; }   // tuning override
       if (C <= 256 && tpw == 1) launch_k(rmsnorm_bf16x8_kernel<1, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
       else if (C <= 256 && tpw == 2) launch_k(rmsnorm_bf16x8_kernel<1, 2>, dim3(ceil_div(n_tok, 8 * 2)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
@@ -2627,7 +2642,7 @@ int mv2_linear_attention(const void* q, const void* kv, void* out, int dtype, in
 int mv2_geglu(const void* in, void* out, int dtype, int64_t N, int I, void* stream) {
   MV2_CHECK_ARG(in && out && N > 0 && I > 0);
   const int64_t total = N * I;
-  const int blocks = (int)((total + 255) / 256 > 148 * 32 ? 148 * 32 : (total + 255) / 256);
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, grid_cap(32));
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32) launch_k(geglu_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)in, (float*)out, N, I);
   else if (dtype == MV2_BF16) launch_k(geglu_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)in, (__nv_bfloat16*)out, N, I);

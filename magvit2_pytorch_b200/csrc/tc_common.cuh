@@ -1,5 +1,5 @@
-// Shared device-side PTX wrappers (mbarrier / TMA / tcgen05 / TMEM) and host-side tensor-map helpers for the
-// tcgen05 kernels (tc_conv.cu, tc_slab.cu).  sm_100a only.
+// Shared device-side PTX wrappers (mbarrier / TMA / wgmma) and host-side tensor-map helpers for the Hopper
+// tensor-core kernels (tc_conv.cu, tc_slab.cu).  sm_90a only.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -32,8 +32,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_5d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2,
                                             int c3, int c4) {
@@ -55,125 +53,72 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]   (kind::f16: bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// ---- wgmma (sm_90a warpgroup MMA): D[regs] (+)= A[smem] * B[smem], bf16 in, fp32 accumulate ----
+// Every wgmma instruction is issued by all 128 threads of a warpgroup; the 64 x N fp32 accumulator lives in their
+// registers (m64nNk16 fragment: thread t holds rows 16 (t / 32) + (t % 32) / 4 (+ 8), columns 8 j + 2 (t % 4) (+ 1)).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_bf16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-// ---- 2-CTA cluster helpers (weight-tile multicast) ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// 3-D box load delivered to the same shared-memory offset (and mbarrier offset) of every CTA in cta_mask
-__device__ __forceinline__ void tma_load_3d_mcast(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2,
-                                                  uint16_t cta_mask) {
+template <> __device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tma_load_2d_mcast(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1,
-                                                  uint16_t cta_mask) {
+template <> __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask) : "memory");
-}
-// tcgen05.commit arriving on the barrier at the same offset in every CTA of cta_mask
-__device__ __forceinline__ void umma_commit_mcast(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(cta_mask) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
 
-// warp-uniform leader election (all 32 lanes must execute it); returns 1 in exactly one lane
-__device__ __forceinline__ uint32_t elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t"
-      "}" : "=r"(pred));
-  return pred;
+// wgmma shared-memory matrix descriptor, K-major operand with hardware swizzle (128 B rows -> SWIZZLE_128B, 64 B ->
+// SWIZZLE_64B, 32 B -> SWIZZLE_32B), without the start address:
+//   bits [0,14) start address >> 4      bits [16,30) leading byte offset >> 4 (unused for swizzled K-major)
+//   bits [32,46) stride byte offset >> 4 (distance between 8-row core groups)      bits [62,64) swizzle: 1 = 128B, 2 = 64B, 3 = 32B
+// The swizzle is a function of the absolute shared-memory address (as for TMA), so a start address moved by whole rows
+// or by 32-byte K steps inside a 1024-byte-aligned tile still addresses what TMA wrote; the base-offset field stays 0.
+__host__ __device__ __forceinline__ uint64_t gmma_desc_hi(uint32_t sbo, uint32_t row_bytes) {
+  const uint64_t layout = row_bytes == 128 ? 1 : (row_bytes == 64 ? 2 : 3);
+  return ((uint64_t)1 << 16) | ((uint64_t)(sbo >> 4) << 32) | (layout << 62);
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return (saddr & 0x3FFFF) >> 4; }
 
-// UMMA shared-memory matrix descriptor, K-major operand with hardware swizzle.
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (ignored for swizzled K-major)
-//   bits [32,46) stride byte offset >> 4   (8 rows x row bytes)     bits [46,48) version = 1 (sm_100)
-//   bits [61,64) layout: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B
-__device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t saddr, uint32_t row_bytes) {
-  const uint32_t sbo = 8 * row_bytes;
-  const uint64_t layout = row_bytes == 128 ? 2 : (row_bytes == 64 ? 4 : 6);
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(sbo >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= layout << 61;
-  return d;
+// Accumulator staging: a warpgroup writes its 64 x N fragment to shared memory ([64][N + 4] fp32: the padding makes the
+// row-per-thread reads below conflict-free), so that the epilogue can work on one output row per thread.
+template <int N> __device__ __forceinline__ void stage_acc(const float (&d)[N / 2], float* stg, int t) {
+  const int r = 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    *reinterpret_cast<float2*>(stg + r * (N + 4) + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(stg + (r + 8) * (N + 4) + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
 }
-
-
-// general: explicit SBO and row width (128 B rows -> SWIZZLE_128B, 64 B -> SWIZZLE_64B, 32 B -> SWIZZLE_32B)
-__device__ __forceinline__ uint64_t make_kmajor_desc_rb(uint32_t saddr, uint32_t sbo, uint32_t row_bytes) {
-  const uint64_t layout = row_bytes == 128 ? 2 : (row_bytes == 64 ? 4 : 6);
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(sbo >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= layout << 61;
-  return d;
+// 32 (or, at the end of a 16-column-wide tile, 16) consecutive accumulator columns of one staged row
+__device__ __forceinline__ void load_row32(const float* src, int ncols, uint32_t (&r)[32]) {
+#pragma unroll
+  for (int g = 0; g < 8; ++g) {
+    if (g * 4 >= ncols) break;
+    const float4 v = *reinterpret_cast<const float4*>(src + 4 * g);
+    r[4 * g] = __float_as_uint(v.x); r[4 * g + 1] = __float_as_uint(v.y);
+    r[4 * g + 2] = __float_as_uint(v.z); r[4 * g + 3] = __float_as_uint(v.w);
+  }
 }
-
-// same, with an explicit stride-byte-offset (distance between consecutive 8-row core groups), SWIZZLE_128B
-__device__ __forceinline__ uint64_t make_kmajor_desc_sbo(uint32_t saddr, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(sbo >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
@@ -212,7 +157,7 @@ __device__ __forceinline__ void store8_bf16(__nv_bfloat16* dst, const float (&v)
 // and act(conv + bias) + res is summed in fp32 and rounded to bf16 ONCE (the reference's bf16 `fn(x) + x` rounds twice; the
 // single rounding is strictly closer to the fp32 result).
 // EPI_FUSED_RU (slab kernel only): the whole conv half of a ResidualUnit in one launch -- the ELU'd 3x3x3 tile goes to
-// shared memory as the A operand of a second tcgen05.mma against the 1x1x1 weights, and the second epilogue emits the
+// shared memory as the A operand of a second wgmma against the 1x1x1 weights, and the second epilogue emits the
 // SqueezeExcite online-softmax pool partials next to y (see tc_slab.cu).
 // EPI_SHUFFLE_ST (slab kernel only): depth-to-space / depth-to-time stores through the same shared-memory transpose as
 // EPI_PLAIN (64 contiguous bytes per output position and store instruction); needs Cy % 32 == 0 so that a 32-column chunk
@@ -251,7 +196,7 @@ __device__ __forceinline__ float erf_fast(float x) {
 // (|error| <= 1.5e-7): with q = 0.5 * t * poly(t) * exp(-g^2 / 2), t = 1 / (1 + 0.3275911 z),
 //   Phi(g) = 1 - q (g >= 0), q (g < 0)   =>   gelu(g) = max(g, 0) - |g| * q.
 // All constant factors (1 / sqrt 2, 0.5, log2 e) are folded into the coefficients: 2 MUFU + 12 FP32 instructions per value
-// (the erf_fast form above costs 16); the fc1 + GEGLU epilogue is issue bound (ncu: ~39 instructions per output in total).
+// (the erf_fast form above costs 16); the fc1 + GEGLU epilogue is bound by instruction issue.
 __device__ __forceinline__ float gelu_fast(float g) {
   const float ag = fabsf(g);
   const float t = rcp_approx(fmaf(0.3275911f * 0.70710678118654752440f, ag, 1.f));

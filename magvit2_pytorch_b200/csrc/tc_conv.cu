@@ -1,4 +1,4 @@
-// tcgen05 / TMA implicit-GEMM convolution for sm_100a (bf16 in, fp32 accumulate in TMEM).
+// wgmma / TMA implicit-GEMM convolution for sm_90a (bf16 in, fp32 accumulate in registers).
 //
 // One kernel covers the whole dense-contraction family of the VideoTokenizer forward path:
 // causal 3x3x3 convs, 1x1x1 convs / Linear layers, the strided compress_space / compress_time
@@ -6,7 +6,7 @@
 //
 // GEMM view:  D[m][n] = sum_{tap, c} X[pos(m) + off(tap)][c] * W[n][tap][c]
 //   M = 128 output positions per CTA, laid out as a (bt, bh, bw) box of the output volume
-//   N = up to 256 output channels per CTA
+//   N = 32, 64 or 128 output channels per CTA
 //   K = taps x Ci, walked in BK-channel slices of one tap at a time
 // Operand staging: one TMA box load per (tap, slice) for A -- the box {BK, bw, bh, bt, 1} of the
 // channels-last activation tensor shifted by the tap offset; out-of-bounds elements (the causal
@@ -14,8 +14,9 @@
 // copy of the activations is ever materialised (the reference does F.pad + conv, M:924-928).
 // Strided convs read through "parity view" tensor maps (one per stride phase).  Both operands are
 // K-major in shared memory with the hardware 128B/64B/32B swizzle (BK = 64/32/16 channels).
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread
-// tcgen05.mma issuer, warps 2-5 = epilogue (tcgen05.ld -> bias/activation/residual -> global).
+// Warp roles (384 threads): warp 0 = TMA producer, warps 4-11 = two consumer warpgroups (rows 0-63 / 64-127 of the
+// tile): wgmma into registers, then the epilogue (accumulator -> shared-memory staging -> bias/activation/residual
+// -> global, one output row per thread and 32-column chunk).
 #include "common.cuh"
 #include "tc_common.cuh"
 #include <cuda.h>
@@ -39,25 +40,26 @@ struct alignas(64) TcParams {
   int ntaps, kchunks, ci_pad, bk;
   int B, To, Ho, Wo, Co;
   int bt, bh, bw, tt, th, tw;
-  int bn, stages, tmem_cols;
+  int bn, stages;
   TcEpi epi;
 };
 
-template <int MODE>
-__global__ void __launch_bounds__(192, 2) tc_conv_kernel(const __grid_constant__ TcParams p) {
+template <int MODE, int BN>
+__global__ void __launch_bounds__(384, 1) tc_conv_kernel(const __grid_constant__ TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int bk = p.bk;
   const uint32_t row_bytes = bk * 2;
   const uint32_t a_bytes = TC_BM * row_bytes;
-  const uint32_t b_bytes = p.bn * row_bytes;
-  const uint32_t stage_bytes = a_bytes + b_bytes;   // both multiples of 1024 when bn % 16 == 0 and bk >= 32; see host
+  const uint32_t b_bytes = BN * row_bytes;
+  const uint32_t stage_bytes = a_bytes + b_bytes;   // both multiples of 1024 (BN >= 32, bk >= 16)
   const uint32_t bar_base = smem_base + p.stages * stage_bytes;
-  // barriers: full[s] at +8s, empty[s] at +8(S+s), tmem_full at +16S, tmem slot at +16S+8
-  const uint32_t full0 = bar_base, empty0 = bar_base + 8 * p.stages, tfull = bar_base + 16 * p.stages;
-  const uint32_t tslot = tfull + 8;
-  float* sbias = reinterpret_cast<float*>(smem_raw + (((tslot + 8 + 15) & ~15u) - smem_u32(smem_raw)));   // bn floats, 16-byte aligned
+  // barriers: full[s] at +8s, empty[s] at +8(S+s)
+  const uint32_t full0 = bar_base, empty0 = bar_base + 8 * p.stages;
+  const uint32_t sbias_u = (empty0 + 8 * p.stages + 15) & ~15u;
+  float* sbias = reinterpret_cast<float*>(smem_raw + (sbias_u - smem_u32(smem_raw)));   // BN floats, 16-byte aligned
+  float* stg_all = sbias + BN;                                                            // 2 x [64][BN + 4] fp32 staging
 
   // tile coordinates
   int tile = blockIdx.x;
@@ -66,28 +68,22 @@ __global__ void __launch_bounds__(192, 2) tc_conv_kernel(const __grid_constant__
   const int it = tile % p.tt; tile /= p.tt;
   const int b = tile;
   const int w0 = iw * p.bw, h0 = ih * p.bh, t0 = it * p.bt;
-  const int n0 = blockIdx.y * p.bn;
+  const int n0 = blockIdx.y * BN;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, 8);     // one arrival per consumer warp
     }
-    mbar_init(tfull, 1);
     fence_barrier_init();
   }
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.wmap);
     tma_prefetch_desc(&p.amap[0]);
   }
-  if (warp == 1) tmem_alloc(tslot, p.tmem_cols);
-  if (warp >= 2)
-    for (int i = threadIdx.x - 64; i < p.bn; i += 128) sbias[i] = (p.epi.bias && n0 + i < p.Co) ? p.epi.bias[n0 + i] : 0.f;
-  tc_fence_before();
+  if (warp >= 4)
+    for (int i = threadIdx.x - 128; i < BN; i += 256) sbias[i] = (p.epi.bias && n0 + i < p.Co) ? p.epi.bias[n0 + i] : 0.f;
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tslot));
   // everything above overlapped the previous kernel's tail (PDL); activations may only be touched from here on
   pdl_wait();
   pdl_launch_dependents();
@@ -109,57 +105,49 @@ __global__ void __launch_bounds__(192, 2) tc_conv_kernel(const __grid_constant__
         if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // whole warp runs the loop (uniform operands); one elected lane issues the tcgen05 instructions
-    // instruction descriptor: D=f32 (bits 4-5 = 1), A=B=bf16 (bits 7-9, 10-12 = 1), K-major both, N>>3 at 17, M>>4 at 24
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.bn >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-    const uint32_t leader = elect_one();
+  } else if (warp >= 4) {
+    // ---------------- consumer warpgroups: wgmma main loop ----------------
+    const int wg = (warp - 4) >> 2, t = threadIdx.x & 127;
+    const uint64_t d_hi = gmma_desc_hi(8 * row_bytes, row_bytes);
     const int ksteps = bk >> 4;
-    const uint64_t d_hi = make_kmajor_desc(0, row_bytes);     // descriptor with a zero start address
-    const uint32_t stage16 = stage_bytes >> 4, a16 = a_bytes >> 4, base16 = (smem_base & 0x3FFFF) >> 4;
-    uint32_t s = 0, ph = 0, lo = base16;
+    // this warpgroup's 64 rows start 64 rows into the A tile; advancing 16 bf16 along K = +32 bytes = +2 address units
+    const uint32_t stage16 = stage_bytes >> 4, a16 = a_bytes >> 4, wg16 = (uint32_t)wg * ((64 * row_bytes) >> 4);
+    uint32_t s = 0, ph = 0, lo = desc_lo(smem_base);
+    float acc[BN / 2];
     for (int i = 0; i < n_iters; ++i) {
       mbar_wait(full0 + 8 * s, ph);
-      tc_fence_after();
-      const uint64_t ad = d_hi | (uint64_t)lo;
+      wgmma_fence();
+      const uint64_t ad = d_hi | (uint64_t)(lo + wg16);
       const uint64_t bd = d_hi | (uint64_t)(lo + a16);
-      if (leader) {
-        // advancing 16 bf16 along K = +32 bytes = +2 in the (addr >> 4) field
-        umma_bf16(tmem_base, ad, bd, idesc, i > 0 ? 1u : 0u);
-        if (ksteps > 1) umma_bf16(tmem_base, ad + 2, bd + 2, idesc, 1u);
-        if (ksteps > 2) {
-          umma_bf16(tmem_base, ad + 4, bd + 4, idesc, 1u);
-          umma_bf16(tmem_base, ad + 6, bd + 6, idesc, 1u);
-        }
-        umma_commit(empty0 + 8 * s);   // frees the smem slot once these MMAs retire
+      wgmma_bf16<BN>(acc, ad, bd, i > 0 ? 1u : 0u);
+      if (ksteps > 1) wgmma_bf16<BN>(acc, ad + 2, bd + 2, 1u);
+      if (ksteps > 2) {
+        wgmma_bf16<BN>(acc, ad + 4, bd + 4, 1u);
+        wgmma_bf16<BN>(acc, ad + 6, bd + 6, 1u);
       }
-      if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1; lo = base16; } else { lo += stage16; }
+      wgmma_commit();
+      wgmma_wait_all();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty0 + 8 * s);   // frees the smem slot: these MMAs have read it
+      if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1; lo = desc_lo(smem_base); } else { lo += stage16; }
     }
-    if (leader) umma_commit(tfull);    // accumulator complete
-  } else {
-    // ---------------- epilogue warps 2..5 : TMEM lanes 32*(warp%4) .. +31 ----------------
-    const int sub = warp & 3;
+    // ---------------- epilogue: one output row per thread, the two warps of a 32-row quarter split the columns ----------------
+    float* stg = stg_all + wg * 64 * (BN + 4);
+    stage_acc<BN>(acc, stg, t);
+    named_bar_sync(1 + wg, 128);
+    const int wq = warp & 3;
+    const int sub = 2 * wg + (wq & 1), half = wq >> 1;
     const int row = sub * 32 + lane;
     const int lw = row % p.bw, lh = (row / p.bw) % p.bh, lt = row / (p.bw * p.bh);
     const int wo = w0 + lw, ho = h0 + lh, to = t0 + lt;
     const bool row_ok = wo < p.Wo && ho < p.Ho && to < p.To;
-    mbar_wait(tfull, 0);
-    tc_fence_after();
-    const uint32_t tlane = tmem_base + ((uint32_t)(sub * 32) << 16);
     const int64_t row_base = ((((int64_t)b * p.To + to) * p.Ho + ho) * p.Wo + wo) * p.Co;
-    for (int c0 = 0; c0 < p.bn; c0 += 32) {
+    const float* srow = stg + (row - 64 * wg) * (BN + 4);
+    for (int c0 = half * 32; c0 < BN; c0 += 64) {
       uint32_t r[32];
-      if (p.bn - c0 >= 32) tmem_ld_32x32b_x32(tlane + c0, r);
-      else tmem_ld_32x32b_x16(tlane + c0, r);
-      tmem_ld_wait();
-      if (row_ok) epi_chunk32<MODE>(p.epi, r, min(32, p.bn - c0), n0 + c0, sbias + c0, b, to, ho, wo, row_base);
+      load_row32(srow + c0, 32, r);
+      if (row_ok) epi_chunk32<MODE>(p.epi, r, 32, n0 + c0, sbias + c0, b, to, ho, wo, row_base);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
   }
 }
 
@@ -205,18 +193,16 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) {
   p.bh = std::min(128 / p.bw, pow2_ceil(a->Ho));
   p.bt = 128 / (p.bw * p.bh);
   p.tw = ceil_div(a->Wo, p.bw); p.th = ceil_div(a->Ho, p.bh); p.tt = ceil_div(a->To, p.bt);
-  // N tile: multiple of 16 (UMMA M=128 constraint), rows of B must keep 1024 B stage alignment
-  int bn = std::min(256, (a->Co + 15) / 16 * 16);
+  // N tile: 32, 64 or 128 columns (a wgmma N, 64 fp32 accumulator registers per thread at 128); wider outputs take
+  // several N tiles, a ragged last one reads zero-filled weight rows and stores nothing for them
+  const int bn = a->Co <= 32 ? 32 : (a->Co <= 64 ? 64 : 128);
   const int row_bytes = bk * 2;
-  while ((bn * row_bytes) % 1024 != 0) bn += 16;      // bk=16 -> bn % 32 == 0, bk >= 32: already fine
-  MV2_CHECK_ARG(bn <= 256);
   p.bn = bn;
-  p.tmem_cols = std::max(32, pow2_ceil(bn));
   const int stage_bytes = TC_BM * row_bytes + bn * row_bytes;
-  MV2_CHECK_ARG((TC_BM * row_bytes) % 1024 == 0);
-  // ring depth: no deeper than the K loop (short-K layers then fit several CTAs per SM, overlapping one CTA's
-  // epilogue with another's loads)
-  int stages = (200 * 1024) / stage_bytes;
+  MV2_CHECK_ARG((TC_BM * row_bytes) % 1024 == 0 && (bn * row_bytes) % 1024 == 0);
+  const int stg_bytes = 2 * 64 * (bn + 4) * 4;         // accumulator staging of the two consumer warpgroups
+  // ring depth: no deeper than the K loop
+  int stages = (200 * 1024 - stg_bytes) / stage_bytes;
   stages = std::max(2, std::min(stages, 8));
   stages = std::max(1, std::min(stages, a->kt * a->kh * a->kw * (a->Ci / bk)));
   p.stages = stages;
@@ -271,20 +257,27 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) {
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(weights) failed: %d", (int)r); return MV2_E_CUDA; }
   }
-  const size_t smem = (size_t)stages * stage_bytes + 16 * stages + 32 + (size_t)bn * 4 + 1024;
+  const size_t smem = 1024 + (size_t)stages * stage_bytes + 16 * stages + 16 + (size_t)bn * 4 + stg_bytes;
   static PerDeviceOnce attr_once;
   const cudaError_t attr_err = attr_once.run([] {
-    cudaError_t e = cudaFuncSetAttribute(tc_conv_kernel<EPI_RAGGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_conv_kernel<EPI_GEGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_conv_kernel<EPI_SHUFFLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaSuccess;
+    for (auto k : {tc_conv_kernel<EPI_RAGGED, 32>, tc_conv_kernel<EPI_RAGGED, 64>, tc_conv_kernel<EPI_RAGGED, 128>,
+                   tc_conv_kernel<EPI_GEGLU, 32>, tc_conv_kernel<EPI_GEGLU, 64>, tc_conv_kernel<EPI_GEGLU, 128>,
+                   tc_conv_kernel<EPI_SHUFFLE, 32>, tc_conv_kernel<EPI_SHUFFLE, 64>, tc_conv_kernel<EPI_SHUFFLE, 128>})
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     return e;
   });
   if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
   MV2_CHECK_ARG(smem <= 227 * 1024);
   dim3 grid((unsigned)((int64_t)a->B * p.tt * p.th * p.tw), (unsigned)ceil_div(a->Co, bn));
-  if (a->epi_mode == 1) launch_k(tc_conv_kernel<EPI_GEGLU>, dim3(grid), dim3(192), smem, (cudaStream_t)stream, p);
-  else if (a->shuffle != MV2_SHUFFLE_NONE) launch_k(tc_conv_kernel<EPI_SHUFFLE>, dim3(grid), dim3(192), smem, (cudaStream_t)stream, p);
-  else launch_k(tc_conv_kernel<EPI_RAGGED>, dim3(grid), dim3(192), smem, (cudaStream_t)stream, p);
+  const int mode = a->epi_mode == 1 ? EPI_GEGLU : (a->shuffle != MV2_SHUFFLE_NONE ? EPI_SHUFFLE : EPI_RAGGED);
+  void (*k)(TcParams) = nullptr;
+#define MV2_PICK(M) k = bn == 32 ? tc_conv_kernel<M, 32> : (bn == 64 ? tc_conv_kernel<M, 64> : tc_conv_kernel<M, 128>)
+  if (mode == EPI_GEGLU) MV2_PICK(EPI_GEGLU);
+  else if (mode == EPI_SHUFFLE) MV2_PICK(EPI_SHUFFLE);
+  else MV2_PICK(EPI_RAGGED);
+#undef MV2_PICK
+  launch_k(k, grid, dim3(384), smem, (cudaStream_t)stream, p);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }

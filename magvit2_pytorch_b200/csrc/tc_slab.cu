@@ -1,26 +1,25 @@
-// tcgen05 "slab" implicit-GEMM kernel for stride-1 k_t x k_h x k_w convolutions (the causal 3x3x3 residual
-// convs = 82 % of the path's FLOPs), bf16 in / fp32 accumulate in TMEM, persistent CTAs.
+// wgmma / TMA "slab" implicit-GEMM kernel for stride-1 k_t x k_h x k_w convolutions (the causal 3x3x3 residual
+// convs carry most of the path's FLOPs), bf16 in / fp32 accumulate in registers, persistent CTAs, sm_90a.
 //
-// Why a second kernel: tc_conv.cu reloads the activation tile from L2 once per tap (27x) and the weight tile
-// once per 128 output positions; on B200 that makes the C=64/128 levels L2-bandwidth bound (measured 171 / 343
-// TFLOP/s).  Here
-//   * one TMA box load brings a haloed activation slab  {64 ch, 8*mw+2, 16+2} (one frame, one 64-channel
-//     slice) into shared memory ONCE and all k_h*k_w in-plane taps are fed from it: the UMMA A-descriptor is
-//     simply started (dh*pitch + dw) rows further into the slab (128-byte rows, hardware SWIZZLE_128B is a
-//     function of the absolute smem address, so row-shifted starts stay consistent with what TMA wrote;
-//     8-row core groups are 8 consecutive w positions, group stride (SBO) = slab row pitch);
-//   * a macro tile is mw (1|2|4) M-tiles of 16(h) x 8(w) positions side by side; all of them consume the same
-//     weight tile from smem (mw accumulators in TMEM), dividing weight traffic by mw;
+// Why a second kernel: tc_conv.cu reloads the activation tile from L2 once per tap (27x) and the weight tile once per
+// 128 output positions.  Here
+//   * one TMA box load brings a haloed activation slab {64 ch, 8*mw + kw - 1, 16 + kh - 1} (one frame, one 64-channel
+//     slice) into shared memory ONCE and all k_h*k_w in-plane taps are fed from it: the wgmma A descriptor is simply
+//     started (dh*pitch + dw) rows further into the slab (128-byte rows; the hardware SWIZZLE_128B is a function of the
+//     absolute shared-memory address, so row-shifted starts stay consistent with what TMA wrote; 8-row core groups are
+//     8 consecutive w positions, group stride (SBO) = slab row pitch);
+//   * a macro tile is mw (1|2|4) M-tiles of 16(h) x 8(w) positions side by side; all of them consume the same weight
+//     tile from shared memory, dividing weight traffic by mw (mw * bn <= 128: the mw accumulators of a consumer
+//     warpgroup fit 64 fp32 registers per thread);
 //   * CTAs are persistent with a static, cost-sorted serpentine tile schedule (slab_frame_of / slab_tile_of);
-//     accumulators are double-buffered in TMEM when they fit (2 * mw * BN <= 512 columns) so the epilogue of
-//     tile i overlaps the MMAs of tile i+1;
 //   * causal frames in front of the clip (t + dt - pt < 0) are all-zero and are skipped outright;
-//   * N tiles need not divide Co (plain / GEGLU epilogues guard every stored column): deep wide layers choose
-//     their tile width with a makespan model (choose_ragged_tiles);
-//   * the kernel is instantiated per epilogue flavour (tc_common.cuh: EPI_*); the plain flavour transposes each
-//     32 x 32 chunk through shared memory so stores / residual loads are 64-byte contiguous per row.
-// Warp roles (384 threads): w0 slab TMA producer, w1 MMA issuer (+TMEM alloc), w2 weight TMA producer,
-// w4-11 epilogue (TMEM lanes 32*(w%4)..+31; the two warps of a lane quarter split the column chunks).
+//   * N tiles need not divide Co (the plain / GEGLU epilogues guard every stored column): wide outputs without a
+//     128-column divisor take 128-column tiles with a ragged last one;
+//   * the kernel is instantiated per epilogue flavour (tc_common.cuh: EPI_*) and N tile (32 / 64 / 128); the plain
+//     flavour transposes each 32 x 32 chunk through shared memory so stores / residual loads are 64-byte contiguous per row.
+// Warp roles (384 threads): w0 slab TMA producer, w2 weight TMA producer, w3 resident 1x1x1 weights (fused ResidualUnit
+// only), w4-7 / w8-11 two consumer warpgroups: each issues the wgmma of 64 of the 128 positions of every M-tile, stages
+// its accumulators in shared memory and runs the epilogue on them (one output row per thread and 32-column chunk).
 #include "common.cuh"
 #include "tc_common.cuh"
 #include <cuda.h>
@@ -43,11 +42,9 @@ struct alignas(64) SlabParams {
   int B, T, H, W, Co;
   int mw, pitch, slab_h, slab_bytes, slab_stride;
   int bn, n_tiles_n, tiles_w, tiles_h, total_tiles;
-  int slab_stages, w_stages, nbuf;
-  int acc_stride;        // TMEM columns between the two accumulator buffers (256 when double buffered)
+  int slab_stages, w_stages;
   int tpw;               // in-plane taps per weight stage (one 3-D TMA box {bk, bn, tpw})
   int geglu_staged;      // EPI_GEGLU: 64-column chunks through the transpose buffers (1) or direct 16-byte row pieces (0)
-  int cluster;           // 1, or 2: CTA pairs on neighbouring tiles multicast each other half of every weight tile
   TcEpi epi;
   // ---- EPI_FUSED_RU only (mv2_tc_ru_forward) ----
   CUtensorMap w1map;     // 1x1x1 weights [Co][Ci] as {ci, co}: 2-D boxes {64, bn}
@@ -60,20 +57,14 @@ struct alignas(64) SlabParams {
   int dn_e_off;          // byte offset of the even-row sub-slab inside a slab stage
   int dn_aoff[6];        // per tap' = dh * 2 + (dw2 + 1): A-descriptor start offset inside the stage, in 16-byte units
   int dn_lower;          // K-chunks of the lower (pw = 0) half of the 2C axis: they only see the dw2 = 0 taps
-  int nh;                // shared-memory H buffers (ELU'd 3x3x3 tile of one M-tile, A operand of the second MMA): 1 or 2
-  int h_stride;          // bytes per H buffer = kchunks * 16 KB
+  int h_stride;          // bytes of the shared-memory H buffer (ELU'd 3x3x3 tile of one M-tile) = kchunks * 16 KB
 };
-
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
 
 // Frames are enumerated most-expensive first: the B * (T - pt) frames that see all kt frame taps, then the frames
 // t = pt-1, pt-2, ..., 0 of every clip (their leading taps fall into the causal padding and are skipped, so their tiles
 // cost (kt-1)/kt ... 1/kt of a full one).  Together with the serpentine CTA assignment (slab_tile_of) a static schedule
-// then behaves like longest-processing-time-first list scheduling: with few tiles per CTA (C = 512 at T = 20: 320 tiles
-// for 148 CTAs) no CTA gets three full tiles while others get two.  Pure index arithmetic, so the tile id stays warp
-// uniform in the MMA-issuing warp (a schedule table read from memory does not: measured 5 % slower overall).
+// then behaves like longest-processing-time-first list scheduling: with few tiles per CTA no CTA gets three full tiles
+// while others get two.  Pure index arithmetic, shared by every warp of the CTA and by the host-side tests.
 __host__ __device__ __forceinline__ void slab_frame_of(const SlabParams& p, int slot, int& b, int& t) {
   const int ptc = p.pt > 0 ? (p.pt + p.st - 1) / p.st : 0;   // output frames whose leading taps fall into the causal padding
                                                               // (pt < 0: cropped conv_out output, none)
@@ -85,7 +76,6 @@ __host__ __device__ __forceinline__ void slab_frame_of(const SlabParams& p, int 
 // k-th tile of CTA `cta` of `grid`: waves alternate direction (serpentine) so the CTAs that finish a wave first start the
 // next one first.  (mv2_tc_slab_tile exposes the same function to the host-side tests.)
 __host__ __device__ __forceinline__ int slab_tile_of_cta(const SlabParams& p, int k, int cta, int grid) {
-  if (p.cluster > 1) { const int tile = cta + k * grid; return tile < p.total_tiles ? tile : -1; }
   const int tile = k * grid + ((k & 1) ? grid - 1 - cta : cta);
   return tile < p.total_tiles ? tile : -1;
 }
@@ -94,81 +84,42 @@ __device__ __forceinline__ int slab_tile_of(const SlabParams& p, int k) { return
 struct TileCoord { int b, t, h0, w0, n0; };
 __host__ __device__ __forceinline__ TileCoord decode_tile(const SlabParams& p, int tile) {
   TileCoord c;
-  int nt, tw, th;
-  if (p.cluster == 1) {      // n-tile fastest: CTAs running side by side share the activation slab through L2
-    nt = tile % p.n_tiles_n; tile /= p.n_tiles_n;
-    tw = tile % p.tiles_w; tile /= p.tiles_w;
-    th = tile % p.tiles_h; tile /= p.tiles_h;
-  } else {                   // w-tile fastest: the two CTAs of a cluster work on neighbouring tiles of the same (b, t, n-tile)
-    tw = tile % p.tiles_w; tile /= p.tiles_w;
-    th = tile % p.tiles_h; tile /= p.tiles_h;
-    nt = tile % p.n_tiles_n; tile /= p.n_tiles_n;
-  }
-  if (p.cluster == 1) slab_frame_of(p, tile, c.b, c.t);
-  else { c.t = tile % p.T; c.b = tile / p.T; }
+  // n-tile fastest: CTAs running side by side share the activation slab through L2
+  const int nt = tile % p.n_tiles_n; tile /= p.n_tiles_n;
+  const int tw = tile % p.tiles_w; tile /= p.tiles_w;
+  const int th = tile % p.tiles_h; tile /= p.tiles_h;
+  slab_frame_of(p, tile, c.b, c.t);
   c.h0 = th * 16;
   c.w0 = tw * 8 * p.mw;
   c.n0 = nt * p.bn;
   return c;
 }
 
-// EPI_FUSED_RU, warp 3: issuer of the second GEMM (the 1x1x1 conv of a tile), which runs while the main MMA warp is already
-// issuing the next tile's 3x3x3 taps.  One M-tile at a time, as soon as the epilogue warps have written that M-tile's ELU'd
-// 3x3x3 result to shared memory (h_full): A = that H tile, B = the 1x1x1 weights (resident in shared memory, loaded once
-// here), D = the TMEM columns that held the M-tile's 3x3x3 accumulator (fully drained once h_full completes).
-// Lane 0 issues (no second elect.sync in the kernel): with a second elect_one() instance -- or a real call -- the compiler
-// moved the MAIN MMA warp's loop nest out of uniform registers (R2UR in front of every tcgen05.mma group; tests/test_abi.py
-// guards the SASS).
-__device__ __forceinline__ void ru_second_gemm_issuer(const SlabParams& p, uint32_t tmem_base, uint32_t h_full, uint32_t m2_done,
-                                                   uint32_t w1_full, uint32_t hbuf0, uint32_t w1buf, uint32_t w_tile, uint32_t bk,
-                                                   int lane) {
-  if (lane == 0) {
-    mbar_expect_tx(w1_full, (uint32_t)p.kchunks * w_tile);
-    for (int kc2 = 0; kc2 < p.kchunks; ++kc2) tma_load_2d(w1buf + kc2 * w_tile, &p.w1map, w1_full, kc2 * (int)bk, 0);
-  }
-  mbar_wait(w1_full, 0);
-  const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.bn >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  const uint64_t d_hi = ((uint64_t)((8 * 128) >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)1 << 16) | ((uint64_t)2 << 61);
-  const uint32_t leader = lane == 0;
-  const uint32_t b0 = (w1buf & 0x3FFFF) >> 4;
-  uint32_t buf = 0;
-  for (int tk = 0; slab_tile_of(p, tk) >= 0; ++tk) {
-    const uint32_t par = (uint32_t)tk & 1u;
-    for (int j = 0; j < p.mw; ++j) {
-      mbar_wait(h_full + 8 * j, par);
-      tc_fence_after();
-      if (leader) {
-        const uint32_t d2 = tmem_base + buf * p.acc_stride + (uint32_t)j * p.bn;
-        uint32_t a2 = ((hbuf0 + (uint32_t)((p.nh == 2) ? (j & 1) : 0) * p.h_stride) & 0x3FFFF) >> 4, b2 = b0;
-        for (int kc2 = 0; kc2 < p.kchunks; ++kc2) {
-          const uint64_t ad = d_hi | (uint64_t)a2, bd = d_hi | (uint64_t)b2;
-          umma_bf16(d2, ad, bd, idesc, kc2 > 0 ? 1u : 0u);
-          umma_bf16(d2, ad + 2, bd + 2, idesc, 1u);
-          umma_bf16(d2, ad + 4, bd + 4, idesc, 1u);
-          umma_bf16(d2, ad + 6, bd + 6, idesc, 1u);
-          a2 += 16384 >> 4;
-          b2 += w_tile >> 4;
-        }
-        umma_commit(m2_done + 8 * j);
-      }
-      __syncwarp();
-    }
-    if (++buf == (uint32_t)p.nbuf) buf = 0;
-  }
+// Shared-memory layout behind the two TMA rings (host and kernel must agree): barriers, bias, the eight 2 KB
+// epilogue transpose buffers, [fused: logit partials], the fp32 accumulator staging of both consumer warpgroups
+// (mw M-tiles x 64 rows x (bn + 4) each), [fused: the H buffer and the resident 1x1x1 weights].
+struct SlabSmem { uint32_t sbias, stage0, lpart, accstg, hbuf, w1buf, end; };
+__host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& p, uint32_t bar0, bool fused) {
+  SlabSmem m;
+  m.sbias = (bar0 + 8 * (2 * p.slab_stages + 2 * p.w_stages + 1) + 15) & ~15u;
+  m.stage0 = m.sbias + (uint32_t)(p.n_tiles_n * p.bn) * 4 * (fused ? 3 : 1);   // fused: [conv3 bias][conv1 bias][SE to_k weight]
+  m.lpart = m.stage0 + (fused ? 0 : 8 * 2048);   // fused: the transposes reuse the accumulator staging
+  m.accstg = m.lpart + (fused ? 2048 : 0);
+  m.hbuf = m.accstg + 2u * p.mw * 64 * (p.bn + 4) * 4;
+  if (fused) m.hbuf = (m.hbuf + 1023u) & ~1023u;        // SWIZZLE_128B operand tiles: 1024-byte aligned
+  m.w1buf = m.hbuf + (fused ? (uint32_t)p.h_stride : 0);
+  m.end = m.w1buf + (fused ? (uint32_t)(p.kchunks * p.bn * p.row_bytes) : 0);
+  return m;
 }
 
-// Epilogue warps per instantiation: 8 (two per TMEM lane quarter).  The fc1 + GEGLU flavour was also measured with 16 (its epilogue
-// is ~35 instructions per output and the kernel is bound by their issue: ncu 472 k warp instructions per SM at IPC 2.4, tensor pipe
-// 27 % active): no gain at C = 512, -8 % at C = 256 (profiles/r02_sweep_ff.json), so it stays at 8.
-template <int MODE> struct SlabEpiWarps { static constexpr int value = 8; };
-
-// Every instantiation declares 512 threads per block (they are launched with 384): that caps the kernel at 128 registers per
-// thread, i.e. 48 k of the SM's 64 k registers, so that another stream lane's small kernels can be co-resident with a persistent conv
-// CTA (DESIGN.md 3.9).  ptxas: no spills anywhere; fused ResidualUnit 162 -> 128, residual epilogue 164 -> 128, GEGLU 151 -> 127,
-// down-space 151 -> 123, staged shuffle 145 -> 123 registers.  Measured: the tcgen05 launches of a step 5.81 -> 5.73 ms.
-template <int MODE>
-__global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__ SlabParams p) {
-  constexpr int NEPI = SlabEpiWarps<MODE>::value;
+// Every instantiation runs 384 threads: warp 0 slab TMA producer, warp 2 weight TMA producer, warp 3 (fused ResidualUnit
+// only) loads the resident 1x1x1 weights, warps 4-11 are two consumer warpgroups.  Consumer warpgroup g issues the wgmma
+// of output rows h0 + 8g .. h0 + 8g + 7 of every M-tile (64 positions) against all bn columns, keeping mw accumulators of
+// 64 x bn in registers (mw * bn <= 128: at most 64 fp32 registers per thread), then runs the epilogue on them.
+template <int MODE, int BN>
+__global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__ SlabParams p) {
+  constexpr int MWMAX = 128 / BN;
+  constexpr int NEPI = 8;                            // epilogue warps
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -182,47 +133,33 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
   // barrier table (8 bytes each)
   const uint32_t slab_full = bar0, slab_empty = slab_full + 8 * p.slab_stages;
   const uint32_t w_full = slab_empty + 8 * p.slab_stages, w_empty = w_full + 8 * p.w_stages;
-  const uint32_t t_full = w_empty + 8 * p.w_stages, t_empty = t_full + 8 * 2;
-  const uint32_t h_full = t_empty + 8 * 2, m2_done = h_full + 8 * 4;       // EPI_FUSED_RU: per M-tile, once per tile each
-  const uint32_t w1_full = m2_done + 8 * 4;                                // EPI_FUSED_RU: 1x1x1 weights landed (once)
-  const uint32_t tslot = w1_full + 8;
-  const uint32_t sbias_u = (tslot + 8 + 15) & ~15u;
-  float* sbias = reinterpret_cast<float*>(smem_raw + (sbias_u - smem_u32(smem_raw)));   // Co floats, 16-byte aligned
-  // EPI_PLAIN: one 2 KB transpose buffer per epilogue warp (32 rows x 64 B, 16-byte pieces XOR-swizzled)
+  const uint32_t w1_full = w_empty + 8 * p.w_stages;                       // EPI_FUSED_RU: 1x1x1 weights landed (once)
+  const SlabSmem L = slab_smem_layout(p, bar0, MODE == EPI_FUSED_RU);
+  auto gen = [&](uint32_t u) { return smem_raw + (u - smem_u32(smem_raw)); };
+  float* sbias = reinterpret_cast<float*>(gen(L.sbias));   // padded Co floats, 16-byte aligned
   const uint32_t nbias = (uint32_t)(p.n_tiles_n * p.bn);
-  const uint32_t stage0 = sbias_u + nbias * 4 * (MODE == EPI_FUSED_RU ? 3 : 1);   // fused: [conv3 bias][conv1 bias][SE to_k weight]
-  // fused: no separate transpose buffers -- the H buffers double as them once every second GEMM of the tile is done
-  const uint32_t lpart_u = stage0;                                                 // fused: logit partials [2][8 warps][32] fp32
-  const uint32_t hbuf0 = (lpart_u + 2048 + 1023u) & ~1023u;                        // fused: H buffers (SWIZZLE_128B atoms: 1024-aligned)
-  const uint32_t w1buf = hbuf0 + (uint32_t)p.nh * p.h_stride;                      // fused: 1x1x1 weights, kchunks K-major tiles [bn][64]
+  const uint32_t stage0 = L.stage0;                        // one 2 KB transpose buffer per epilogue warp (32 rows x 64 B)
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.slab_stages; ++s) { mbar_init(slab_full + 8 * s, 1); mbar_init(slab_empty + 8 * s, 1); }
-    for (int s = 0; s < p.w_stages; ++s) { mbar_init(w_full + 8 * s, 1); mbar_init(w_empty + 8 * s, p.cluster); }
-    for (int s = 0; s < 2; ++s) { mbar_init(t_full + 8 * s, 1); mbar_init(t_empty + 8 * s, NEPI); }
-    for (int s = 0; s < 4; ++s) { mbar_init(h_full + 8 * s, 8); mbar_init(m2_done + 8 * s, 1); }
+    // empty barriers: one arrival per consumer warp once its wgmma of the stage have completed
+    for (int s = 0; s < p.slab_stages; ++s) { mbar_init(slab_full + 8 * s, 1); mbar_init(slab_empty + 8 * s, 8); }
+    for (int s = 0; s < p.w_stages; ++s) { mbar_init(w_full + 8 * s, 1); mbar_init(w_empty + 8 * s, 8); }
     mbar_init(w1_full, 1);
     fence_barrier_init();
   }
   if (warp == 0 && lane == 0) { tma_prefetch_desc(&p.amap); if (MODE == EPI_DOWN_SPACE) tma_prefetch_desc(&p.amap_odd); }
   if (warp == 2 && lane == 0) { tma_prefetch_desc(&p.wmap); tma_prefetch_desc(&p.wmap2); }
   if (MODE == EPI_FUSED_RU && warp == 3 && lane == 0) tma_prefetch_desc(&p.w1map);
-  if (warp == 1) tmem_alloc(tslot, 512);
   if (warp >= 4) {
     const int nb = p.n_tiles_n * p.bn;   // >= Co; padded columns read zeros
-    for (int i = threadIdx.x - 128; i < nb; i += 32 * NEPI) sbias[i] = (p.epi.bias && i < p.Co) ? p.epi.bias[i] : 0.f;
+    for (int i = threadIdx.x - 128; i < nb; i += 256) sbias[i] = (p.epi.bias && i < p.Co) ? p.epi.bias[i] : 0.f;
     if (MODE == EPI_FUSED_RU)
       for (int i = threadIdx.x - 128; i < nb; i += 256) {
         sbias[nb + i] = (p.bias1 && i < p.Co) ? p.bias1[i] : 0.f;
         sbias[2 * nb + i] = i < p.Co ? p.se_wk[i] : 0.f;
       }
   }
-  tc_fence_before();
   __syncthreads();
-  if (p.cluster > 1) cluster_sync_all();     // peer barriers must be initialised before any multicast / remote arrive
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tslot));
   // everything above overlapped the previous kernel's tail (PDL); activations may only be touched from here on
   pdl_wait();
   pdl_launch_dependents();
@@ -291,175 +228,154 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
             for (int tp = 0; tp < taps2d; tp += p.tpw) {
               mbar_wait(w_empty + 8 * s, ph ^ 1);
               mbar_expect_tx(w_full + 8 * s, w_bytes);
-              if (p.cluster == 1) {
-                if (p.tpw == 1) tma_load_2d(wst0 + s * w_bytes, &p.wmap2, w_full + 8 * s, (dt * taps2d + tp) * p.Ci + kc * bk, c.n0);
-                else tma_load_3d(wst0 + s * w_bytes, &p.wmap, w_full + 8 * s, kc * bk, c.n0, dt * taps2d + tp);
-              } else {   // my half of the rows goes to both CTAs; the peer sends the other half (tpw == 1 here)
-                const uint32_t rank = cluster_ctarank();
-                const uint32_t half_rows = p.bn >> 1;
-                tma_load_2d_mcast(wst0 + s * w_bytes + rank * half_rows * row_bytes, &p.wmap2, w_full + 8 * s,
-                                  (dt * taps2d + tp) * p.Ci + kc * bk, c.n0 + rank * half_rows, (uint16_t)0x3);
-              }
+              if (p.tpw == 1) tma_load_2d(wst0 + s * w_bytes, &p.wmap2, w_full + 8 * s, (dt * taps2d + tp) * p.Ci + kc * bk, c.n0);
+              else tma_load_3d(wst0 + s * w_bytes, &p.wmap, w_full + 8 * s, kc * bk, c.n0, dt * taps2d + tp);
               if (++s == (uint32_t)p.w_stages) { s = 0; ph ^= 1; }
             }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    // The whole warp runs the loop (warp-uniform control flow and operands, so descriptors live in uniform
-    // registers); only the tcgen05 instructions themselves are issued by one elected lane.
-    {
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(p.bn >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      const uint32_t sbo = (uint32_t)p.pitch * row_bytes;
-      const uint64_t lay = (uint64_t)(row_bytes == 128 ? 2 : 4) << 61;
-      const uint64_t a_hi = ((uint64_t)(sbo >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)1 << 16) | lay;
-      const uint64_t b_hi = ((uint64_t)((8 * row_bytes) >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)1 << 16) | lay;
-      const bool k4 = bk == 64;
-      const uint32_t leader = elect_one();
-      // All ring bookkeeping is incremental (stage index, parity, descriptor low words): the per-tap issue path holds no
-      // integer division / modulo and only a handful of uniform adds.
-      const uint32_t a_row = row_bytes >> 4;                       // descriptor-address units per slab row
-      const uint32_t a_next_dh = (uint32_t)(p.pitch - p.kw + 1) * a_row;
-      const uint32_t a_mtile = 8 * a_row;                          // next M-tile: 8 positions further along w
-      const uint32_t w_tile16 = w_tile >> 4, w_stage16 = w_bytes >> 4;
-      const uint32_t b_lo0 = (wst0 & 0x3FFFF) >> 4;
-      uint32_t s_idx = 0, s_par = 0;                               // slab ring
-      uint32_t w_idx = 0, w_par = 0, b_lo = b_lo0;                 // weight ring
-      uint32_t t_idx = 0, t_par = 0;                               // TMEM accumulator ring
-      const int tiles_per_frame = p.n_tiles_n * p.tiles_w * p.tiles_h;
-      // same sequence as slab_tile_of, written with plain induction variables: the compiler only keeps this warp's loop
-      // nest (descriptors, ring indices) in uniform registers when the tile id is an obviously uniform recurrence
-      const int fwd = blockIdx.x, rev = p.cluster == 1 ? (int)gridDim.x - 1 - (int)blockIdx.x : (int)blockIdx.x;
+  } else if (warp == 3) {
+    // ------------------------------ EPI_FUSED_RU: the 1x1x1 weights, resident for the whole kernel ------------------------------
+    if (MODE == EPI_FUSED_RU && lane == 0) {
+      mbar_expect_tx(w1_full, (uint32_t)p.kchunks * w_tile);
+      for (int kc2 = 0; kc2 < p.kchunks; ++kc2) tma_load_2d(L.w1buf + kc2 * w_tile, &p.w1map, w1_full, kc2 * (int)bk, 0);
+    }
+  } else if (warp >= 4) {
+    // ------------------------------ consumer warpgroups: wgmma main loop + epilogue ------------------------------
+    const int wg = (warp - 4) >> 2, wq = warp & 3, tid = threadIdx.x & 127;
+    // epilogue roles: 32-row quarter `sub` of the M-tile (rows sub*32 .. +31 = output rows h0 + 4 sub .. +3, all 8 w) and
+    // column half `half`; ew numbers the 8 epilogue warps (transpose buffer, logit exchange)
+    const int sub = 2 * wg + (wq & 1), half = wq >> 1, ew = sub + 4 * half;
+    const int row = sub * 32 + lane;
+    const int lh = row >> 3, lw = row & 7;
+    float* stg = reinterpret_cast<float*>(gen(L.accstg)) + (size_t)wg * p.mw * 64 * (BN + 4);   // [mw][64][BN + 4]
+    const uint32_t wg_bar = 5 + wg;                          // named barrier of this warpgroup (1..4: logit exchange pairs)
+    const uint32_t sbo = (uint32_t)p.pitch * row_bytes;
+    const uint64_t a_hi = gmma_desc_hi(sbo, row_bytes);
+    const uint64_t b_hi = gmma_desc_hi(8 * row_bytes, row_bytes);
+    const bool k4 = bk == 64;
+    // All ring bookkeeping is incremental (stage index, parity, descriptor low words).
+    const uint32_t a_row = row_bytes >> 4;                       // descriptor-address units per slab row
+    const uint32_t a_wg = (uint32_t)wg * 8 * (sbo >> 4);         // this warpgroup's first output row: 8 slab rows (h) down
+    const uint32_t a_next_dh = (uint32_t)(p.pitch - p.kw + 1) * a_row;
+    const uint32_t a_mtile = 8 * a_row;                          // next M-tile: 8 positions further along w
+    const uint32_t w_tile16 = w_tile >> 4, w_stage16 = w_bytes >> 4;
+    const uint32_t b_lo0 = desc_lo(wst0);
+    uint32_t s_idx = 0, s_par = 0;                               // slab ring
+    uint32_t w_idx = 0, w_par = 0, b_lo = b_lo0;                 // weight ring
+    uint32_t ecount = 0;       // EPI_FUSED_RU: M-tiles processed (selects the logit exchange buffer)
+    if (MODE == EPI_FUSED_RU) mbar_wait(w1_full, 0);
+    float acc[MWMAX][BN / 2];
+    for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
+      const TileCoord c = decode_tile(p, tile);
+      uint32_t accum = 0;
       if (MODE == EPI_DOWN_SPACE) {
-        for (int tk = 0, base = 0;; ++tk, base += gridDim.x) {
-          const int tile = base + ((tk & 1) ? rev : fwd);
-          if (tile >= p.total_tiles) break;
-          mbar_wait(t_empty + 8 * t_idx, t_par ^ 1);
-          tc_fence_after();
-          const uint32_t acc = tmem_base + t_idx * p.acc_stride;
-          uint32_t accum = 0;
-          for (int kc = 0; kc < p.kchunks; ++kc) {
-            mbar_wait(slab_full + 8 * s_idx, s_par);
-            const uint32_t a_base = ((slab0 + s_idx * p.slab_stride) & 0x3FFFF) >> 4;
-            const int t0 = kc < p.dn_lower ? 1 : 0, tstep = kc < p.dn_lower ? 2 : 1;
-            for (int tap = t0; tap < 6; tap += tstep) {
-              mbar_wait(w_full + 8 * w_idx, w_par);
-              tc_fence_after();
-              if (leader) {
-                uint32_t a_j = a_base + (uint32_t)p.dn_aoff[tap], d = acc;
-                for (int j = 0; j < p.mw; ++j) {
-                  const uint64_t ad = a_hi | (uint64_t)a_j, bd = b_hi | (uint64_t)b_lo;
-                  umma_bf16(d, ad, bd, idesc, accum);
-                  umma_bf16(d, ad + 2, bd + 2, idesc, 1u);
-                  umma_bf16(d, ad + 4, bd + 4, idesc, 1u);
-                  umma_bf16(d, ad + 6, bd + 6, idesc, 1u);
-                  a_j += a_mtile;
-                  d += p.bn;
-                }
-                umma_commit(w_empty + 8 * w_idx);
-              }
-              accum = 1;
-              if (++w_idx == (uint32_t)p.w_stages) { w_idx = 0; w_par ^= 1; b_lo = b_lo0; } else { b_lo += w_stage16; }
+        for (int kc = 0; kc < p.kchunks; ++kc) {
+          mbar_wait(slab_full + 8 * s_idx, s_par);
+          const uint32_t a_base = desc_lo(slab0 + s_idx * p.slab_stride) + a_wg;
+          const int t0 = kc < p.dn_lower ? 1 : 0, tstep = kc < p.dn_lower ? 2 : 1;
+          for (int tap = t0; tap < 6; tap += tstep) {
+            mbar_wait(w_full + 8 * w_idx, w_par);
+            wgmma_fence();
+            const uint64_t bd = b_hi | (uint64_t)b_lo;
+#pragma unroll
+            for (int j = 0; j < MWMAX; ++j) {
+              if (j >= p.mw) break;
+              const uint64_t ad = a_hi | (uint64_t)(a_base + (uint32_t)p.dn_aoff[tap] + j * a_mtile);
+              wgmma_bf16<BN>(acc[j], ad, bd, accum);
+              wgmma_bf16<BN>(acc[j], ad + 2, bd + 2, 1u);
+              wgmma_bf16<BN>(acc[j], ad + 4, bd + 4, 1u);
+              wgmma_bf16<BN>(acc[j], ad + 6, bd + 6, 1u);
             }
-            if (leader) umma_commit(slab_empty + 8 * s_idx);
-            if (++s_idx == (uint32_t)p.slab_stages) { s_idx = 0; s_par ^= 1; }
+            wgmma_commit();
+            wgmma_wait_all();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(w_empty + 8 * w_idx);
+            accum = 1;
+            if (++w_idx == (uint32_t)p.w_stages) { w_idx = 0; w_par ^= 1; b_lo = b_lo0; } else { b_lo += w_stage16; }
           }
-          if (leader) umma_commit(t_full + 8 * t_idx);
-          if (++t_idx == (uint32_t)p.nbuf) { t_idx = 0; t_par ^= 1; }
+          if (lane == 0) mbar_arrive(slab_empty + 8 * s_idx);
+          if (++s_idx == (uint32_t)p.slab_stages) { s_idx = 0; s_par ^= 1; }
         }
-      } else
-      for (int tk = 0, base = 0;; ++tk, base += gridDim.x) {
-        const int tile = base + ((tk & 1) ? rev : fwd);
-        if (tile >= p.total_tiles) break;
-        int b_of_tile, t_of_tile;                                  // once per tile (hundreds of taps)
-        if (p.cluster == 1) slab_frame_of(p, tile / tiles_per_frame, b_of_tile, t_of_tile);
-        else t_of_tile = (tile / tiles_per_frame) % p.T;
-        const int dt0 = max(0, p.pt - t_of_tile * p.st);
-        mbar_wait(t_empty + 8 * t_idx, t_par ^ 1);
-        tc_fence_after();
-        const uint32_t acc = tmem_base + t_idx * p.acc_stride;
-        uint32_t accum = 0;
+      } else {
+        const int dt0 = max(0, p.pt - c.t * p.st);
         for (int dt = dt0; dt < p.kt; ++dt)
           for (int kc = 0; kc < p.kchunks; ++kc) {
             mbar_wait(slab_full + 8 * s_idx, s_par);
-            uint32_t a_lo = ((slab0 + s_idx * p.slab_stride) & 0x3FFFF) >> 4;   // descriptor low word of tap (0, 0)
+            uint32_t a_lo = desc_lo(slab0 + s_idx * p.slab_stride) + a_wg;   // descriptor low word of tap (0, 0)
             int dw = 0;
             for (int tp0 = 0; tp0 < taps2d; tp0 += p.tpw) {
               mbar_wait(w_full + 8 * w_idx, w_par);
-              tc_fence_after();
+              wgmma_fence();
               uint32_t b_cur = b_lo;
               for (int u = 0; u < p.tpw; ++u) {
-                if (leader) {
-                  uint32_t a_j = a_lo, d = acc;
-                  for (int j = 0; j < p.mw; ++j) {
-                    const uint64_t ad = a_hi | (uint64_t)a_j, bd = b_hi | (uint64_t)b_cur;
-                    umma_bf16(d, ad, bd, idesc, accum);
-                    umma_bf16(d, ad + 2, bd + 2, idesc, 1u);
-                    if (k4) {
-                      umma_bf16(d, ad + 4, bd + 4, idesc, 1u);
-                      umma_bf16(d, ad + 6, bd + 6, idesc, 1u);
-                    }
-                    a_j += a_mtile;
-                    d += p.bn;
+                const uint64_t bd = b_hi | (uint64_t)b_cur;
+#pragma unroll
+                for (int j = 0; j < MWMAX; ++j) {
+                  if (j >= p.mw) break;
+                  const uint64_t ad = a_hi | (uint64_t)(a_lo + j * a_mtile);
+                  wgmma_bf16<BN>(acc[j], ad, bd, accum);
+                  wgmma_bf16<BN>(acc[j], ad + 2, bd + 2, 1u);
+                  if (k4) {
+                    wgmma_bf16<BN>(acc[j], ad + 4, bd + 4, 1u);
+                    wgmma_bf16<BN>(acc[j], ad + 6, bd + 6, 1u);
                   }
                 }
                 accum = 1;
                 b_cur += w_tile16;
                 if (++dw == p.kw) { dw = 0; a_lo += a_next_dh; } else { a_lo += a_row; }
               }
-              if (leader) {
-                if (p.cluster == 1) umma_commit(w_empty + 8 * w_idx);
-                else umma_commit_mcast(w_empty + 8 * w_idx, (uint16_t)0x3);   // the slot is free once BOTH CTAs consumed it
-              }
+              wgmma_commit();
+              wgmma_wait_all();
+              __syncwarp();
+              if (lane == 0) mbar_arrive(w_empty + 8 * w_idx);   // the weight slot is free once these MMAs have read it
               if (++w_idx == (uint32_t)p.w_stages) { w_idx = 0; w_par ^= 1; b_lo = b_lo0; } else { b_lo += w_stage16; }
             }
-            if (leader) umma_commit(slab_empty + 8 * s_idx);
+            if (lane == 0) mbar_arrive(slab_empty + 8 * s_idx);
             if (++s_idx == (uint32_t)p.slab_stages) { s_idx = 0; s_par ^= 1; }
           }
-        if (leader) umma_commit(t_full + 8 * t_idx);
-        if (++t_idx == (uint32_t)p.nbuf) { t_idx = 0; t_par ^= 1; }
       }
-    }
-  } else if (warp == 3) {
-    // ------------------------------ EPI_FUSED_RU: second-GEMM issuer ------------------------------
-    // The 1x1x1 conv of a tile runs while the main MMA warp is already issuing the next tile's 3x3x3 taps: this warp
-    // issues it, one M-tile at a time, as soon as the epilogue warps have written that M-tile's ELU'd 3x3x3 result to
-    // shared memory (h_full).  A = that H tile, B = the 1x1x1 weights (resident in shared memory, loaded once below),
-    // D = the TMEM columns that held the M-tile's 3x3x3 accumulator (fully drained once h_full completes).  Keeping this
-    // out of the main MMA warp leaves that warp's loop nest (and its uniform-register allocation) exactly as in the
-    // plain kernel.
-    if (MODE == EPI_FUSED_RU) ru_second_gemm_issuer(p, tmem_base, h_full, m2_done, w1_full, hbuf0, w1buf, w_tile, bk, lane);
-  } else if (warp >= 4) {
-    // ------------------------------ epilogue ------------------------------
-    // 8 epilogue warps: TMEM lane quarter = warp % 4 (hardware rule), column half = (warp - 4) / 4
-    const int sub = warp & 3, half = (warp - 4) >> 2;
-    const int row = sub * 32 + lane;
-    const int lh = row >> 3, lw = row & 7;
-    uint32_t buf = 0, bpar = 0;
-    uint32_t ecount = 0;       // EPI_FUSED_RU: M-tiles processed (selects the logit exchange buffer)
-    for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
-      const TileCoord c = decode_tile(p, tile);
-      mbar_wait(t_full + 8 * buf, bpar);
-      tc_fence_after();
+      // ---- accumulators -> shared-memory staging (one [64][BN + 4] block per M-tile), once the previous tile's epilogue
+      //      of this warpgroup has read its staging ----
+      named_bar_sync(wg_bar, 128);
+#pragma unroll
+      for (int j = 0; j < MWMAX; ++j) {
+        if (j >= p.mw) break;
+        stage_acc<BN>(acc[j], stg + j * 64 * (BN + 4), tid);
+      }
+      named_bar_sync(wg_bar, 128);
       const int h = c.h0 + lh;
       if (MODE == EPI_FUSED_RU) {
         // ---------------- fused ResidualUnit epilogue (reference M:937-941 + the pooling half of M:229-233) ----------------
-        const uint32_t par = (uint32_t)tk & 1u;
-        // every epilogue warp has finished the previous tile's transposes (they alias the H buffers written below)
-        if (tk > 0) asm volatile("bar.sync 5, 256;" ::: "memory");
         const float* sb1 = sbias + nbias;
         const float* swk = sbias + 2 * nbias;
-        float* lpart = reinterpret_cast<float*>(smem_raw + (lpart_u - smem_u32(smem_raw)));
-        const uint32_t tl0 = tmem_base + buf * p.acc_stride + ((uint32_t)(sub * 32) << 16);
-        // E1: h = ELU(conv3 + b3) -> bf16 -> shared memory, K-major SWIZZLE_128B (128 rows x 64 channels per 16 KB K-chunk):
-        //     the A operand of the 1x1x1 GEMM.  One M-tile at a time; buffer j % nh is free once the GEMM of M-tile j - nh is done.
+        float* lpart = reinterpret_cast<float*>(gen(L.lpart));
+        const int64_t kstride = (int64_t)p.W * p.Co;
+        const uint32_t wsw = (lane >> 1) & 3;
+        const int rl = lane >> 2, piece = lane & 3;
+        const int h20 = c.h0 + sub * 4;
+        // one record per (tile, lane quarter): the M-tiles of the tile are folded in registers (online softmax over j)
+        const int recs_per_frame = p.tiles_h * p.tiles_w * 4;
+        float* rec = p.se_ws + ((int64_t)(c.b * p.T + c.t) * recs_per_frame + ((c.h0 >> 4) * p.tiles_w + c.w0 / (8 * p.mw)) * 4 + sub) * (p.Co + 2);
+        float run_m = -INFINITY, run_s = 0.f, run_acc[2][8];
+#pragma unroll
+        for (int q = 0; q < 2; ++q)
+#pragma unroll
+          for (int i = 0; i < 8; ++i) run_acc[q][i] = 0.f;
+        const uint64_t h_hi = gmma_desc_hi(1024, 128);
+        const uint32_t h_lo = desc_lo(L.hbuf) + (uint32_t)wg * ((64 * 128) >> 4), w1_lo = desc_lo(L.w1buf);
         for (int j = 0; j < p.mw; ++j) {
-          if (j >= p.nh) mbar_wait(m2_done + 8 * (j - p.nh), par);
-          const uint32_t hb = hbuf0 + (uint32_t)((p.nh == 2) ? (j & 1) : 0) * p.h_stride + (uint32_t)row * 128;
-          for (int c0 = half * 32; c0 < p.bn; c0 += 64) {      // fused: a warp owns the same columns in every M-tile
+          const float* srow = stg + (j * 64 + row - 64 * wg) * (BN + 4);
+          // E2's transpose buffers: 2 KB per warp inside the staging rows of this warp pair, which both warps have read
+          // by the time they exchange their logit partials
+          const uint32_t stg2 = smem_u32(stg + (j * 64 + (sub & 1) * 32) * (BN + 4)) + (uint32_t)half * 2048;
+          const uint32_t wr = stg2 + lane * 64, rd = stg2 + rl * 64;
+          // E1: h = ELU(conv3 + b3) -> bf16 -> shared memory, K-major SWIZZLE_128B (128 rows x 64 channels per 16 KB K-chunk):
+          //     the A operand of the 1x1x1 GEMM; each warpgroup writes (and multiplies) its own 64 rows
+          const uint32_t hb = L.hbuf + (uint32_t)row * 128;
+          for (int c0 = half * 32; c0 < p.bn; c0 += 64) {
             uint32_t r[32], pk[16];
-            tmem_ld_32x32b_x32(tl0 + j * p.bn + c0, r);
-            tmem_ld_wait();
+            load_row32(srow + c0, 32, r);
             epi_pack32_t<MV2_ACT_ELU>(r, sbias + c0, pk);
             const uint32_t hrow = hb + (uint32_t)(c0 >> 6) * 16384;
             const uint32_t p0 = (uint32_t)(c0 & 63) >> 3;
@@ -469,32 +385,22 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
                            "r"(pk[4 * g]), "r"(pk[4 * g + 1]), "r"(pk[4 * g + 2]), "r"(pk[4 * g + 3]) : "memory");
           }
           fence_proxy_async();      // generic-proxy writes -> visible to the tensor core's async-proxy reads
-          tc_fence_before();        // this warp's TMEM reads of M-tile j are complete before the GEMM overwrites those columns
-          __syncwarp();
-          if (lane == 0) mbar_arrive(h_full + 8 * j);
-        }
-        // E2: y = ELU(conv1 + b1) -> bf16 -> global (64-byte row pieces through the transpose buffer), and per 32-position
-        //     row group (this warp's TMEM lane quarter) one SE pool record (max, sum e, sum e * y[C]) with e = exp(logit - max).
-        //     The transpose buffers live in the H region: free once the LAST second GEMM of the tile has completed
-        //     (tcgen05.commit covers every earlier MMA of the issuing thread).
-        mbar_wait(m2_done + 8 * (p.mw - 1), par);
-        const uint32_t stg = hbuf0 + (uint32_t)(warp - 4) * 2048;
-        const uint32_t wr = stg + lane * 64, wsw = (lane >> 1) & 3;
-        const int rl = lane >> 2, piece = lane & 3;
-        const uint32_t rd = stg + rl * 64;
-        const int h20 = c.h0 + sub * 4;
-        const int64_t kstride = (int64_t)p.W * p.Co;
-        // one record per (tile, lane quarter): the M-tiles of the tile are folded in registers (online softmax over j)
-        const int recs_per_frame = p.tiles_h * p.tiles_w * 4;
-        float* rec = p.se_ws + ((int64_t)(c.b * p.T + c.t) * recs_per_frame + ((c.h0 >> 4) * p.tiles_w + c.w0 / (8 * p.mw)) * 4 + sub) * (p.Co + 2);
-        float run_m = -INFINITY, run_s = 0.f, run_acc[2][8];
-#pragma unroll
-        for (int q = 0; q < 2; ++q)
-#pragma unroll
-          for (int i = 0; i < 8; ++i) run_acc[q][i] = 0.f;
-        for (int j = 0; j < p.mw; ++j) {
-          mbar_wait(m2_done + 8 * j, par);
-          tc_fence_after();
+          named_bar_sync(wg_bar, 128);
+          // second GEMM: acc[0] = H (this warpgroup's 64 rows) x W1^T; the staging of M-tile j is free again afterwards
+          wgmma_fence();
+          for (int kc2 = 0; kc2 < p.kchunks; ++kc2) {
+            const uint64_t ad = h_hi | (uint64_t)(h_lo + kc2 * (16384 >> 4)), bd = h_hi | (uint64_t)(w1_lo + kc2 * (w_tile >> 4));
+            wgmma_bf16<BN>(acc[0], ad, bd, kc2 > 0 ? 1u : 0u);
+            wgmma_bf16<BN>(acc[0], ad + 2, bd + 2, 1u);
+            wgmma_bf16<BN>(acc[0], ad + 4, bd + 4, 1u);
+            wgmma_bf16<BN>(acc[0], ad + 6, bd + 6, 1u);
+          }
+          wgmma_commit();
+          wgmma_wait_all();
+          stage_acc<BN>(acc[0], stg + j * 64 * (BN + 4), tid);
+          named_bar_sync(wg_bar, 128);
+          // E2: y = ELU(conv1 + b1) -> bf16 -> global (64-byte row pieces through the transpose buffer), and per 32-position
+          //     row group (this warp's lane quarter) one SE pool record (max, sum e, sum e * y[C]) with e = exp(logit - max).
           const int w = c.w0 + 8 * j + lw;
           const bool row_ok = h < p.H && w < p.W;
           uint32_t pk2[2][16];
@@ -504,8 +410,7 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
             const int c0 = half * 32 + 64 * q;
             if (c0 < p.bn) {
               uint32_t r[32];
-              tmem_ld_32x32b_x32(tl0 + j * p.bn + c0, r);
-              tmem_ld_wait();
+              load_row32(srow + c0, 32, r);
               epi_pack32_t<MV2_ACT_ELU>(r, sb1 + c0, pk2[q]);
 #pragma unroll
               for (int i = 0; i < 16; i += 2) {          // SE logit on the bf16-rounded y, like the unfused path reads it
@@ -520,7 +425,7 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
           // the two warps of this lane quarter hold the two halves of every row's channels: exchange the logit partials
           float* lpb = lpart + (ecount & 1u) * 256;
           ++ecount;
-          lpb[(warp - 4) * 32 + lane] = lp;
+          lpb[ew * 32 + lane] = lp;
           asm volatile("bar.sync %0, 64;" ::"r"(1 + sub) : "memory");
           float lg = lpb[sub * 32 + lane] + lpb[(sub + 4) * 32 + lane] + p.se_bk;
           lg = row_ok ? lg : -INFINITY;
@@ -592,14 +497,14 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
       for (int j = 0; j < p.mw; ++j) {
         const int w = c.w0 + 8 * j + lw;
         const bool row_ok = h < p.H && w < p.W;
-        const uint32_t tl = tmem_base + buf * p.acc_stride + j * p.bn + ((uint32_t)(sub * 32) << 16);
+        const float* srow = stg + (j * 64 + row - 64 * wg) * (BN + 4);
         const int64_t row_base = ((((int64_t)c.b * p.T + c.t) * p.H + h) * p.W + w) * p.Co;
         // column chunks are dealt round-robin to the two warps that share this lane quarter
         if (MODE == EPI_PLAIN || MODE == EPI_PLAIN_RES || MODE == EPI_SHUFFLE_ST || MODE == EPI_DOWN_SPACE) {
           // Row-per-lane results are transposed through shared memory so that every store instruction writes 8 rows
           // x 64 contiguous bytes (full sectors; the 8 rows are neighbours along w, i.e. one contiguous run when the
           // tile spans all of Co) instead of 32 scattered 16-byte pieces.  The residual is read with the same mapping.
-          const uint32_t stg = stage0 + (uint32_t)(warp - 4) * 2048;
+          const uint32_t stg = stage0 + (uint32_t)ew * 2048;
           const uint32_t wr = stg + lane * 64, wsw = (lane >> 1) & 3;
           const int rl = lane >> 2, piece = lane & 3;                 // read side: row within an 8-row group, 16-byte piece
           const int w2 = c.w0 + 8 * j + rl;
@@ -614,15 +519,14 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
             uint32_t r[32], pk[16];
             uint4 rv[4];
             if (MODE == EPI_PLAIN_RES) {
-              // residual: this lane's own row, 64 contiguous bytes (two full sectors), requested before the TMEM load returns;
+              // residual: this lane's own row, 64 contiguous bytes (two full sectors), requested before the staged accumulators are read;
               // it is added in fp32 BEFORE the single rounding to bf16 (the reference's bf16 `fn(x) + x` rounds twice)
               const __nv_bfloat16* rr = p.epi.res + row_base + c.n0 + c0;
 #pragma unroll
               for (int g = 0; g < 4; ++g)
                 rv[g] = (row_ok && c.n0 + c0 + g * 8 < p.Co && c0 + g * 8 < p.bn) ? *reinterpret_cast<const uint4*>(rr + g * 8) : make_uint4(0, 0, 0, 0);
             }
-            tmem_ld_32x32b_x32(tl + c0, r);
-            tmem_ld_wait();
+            load_row32(srow + c0, 32, r);
             if ((MODE == EPI_PLAIN || MODE == EPI_PLAIN_RES) && p.epi.oscale) {   // Conv3DMod demodulation (M:741-742)
               const float* os = p.epi.oscale + (int64_t)c.b * p.Co + c.n0 + c0;
 #pragma unroll
@@ -678,10 +582,10 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
         } else if (MODE == EPI_GEGLU && p.geglu_staged) {
           // fc1 + GEGLU (M:466-469, M:492): 64 accumulator columns (packed [8 x | 8 gate] groups) give 32 outputs = 64 bytes per
           // row, staged through the same transpose buffer as the plain epilogue so that every store instruction writes 8 rows x
-          // 64 contiguous bytes instead of 32 scattered 16-byte pieces.  Opt-in (MV2_GEGLU_STAGED): measured 3 % slower than the
-          // direct path -- the kernel is bound by the instruction issue of the GELU math, not by the stores.  The two warps of a
+          // 64 contiguous bytes instead of 32 scattered 16-byte pieces.  Opt-in (MV2_GEGLU_STAGED): the
+          // GELU math, not the stores, sets the pace of this epilogue, so the direct path is the default.  The two warps of a
           // lane quarter alternate 64-column chunks (bn % 64 == 0: the packed width is a multiple of 128).
-          const uint32_t stg = stage0 + (uint32_t)(warp - 4) * 2048;
+          const uint32_t stg = stage0 + (uint32_t)ew * 2048;
           const uint32_t wr = stg + lane * 64, wsw = (lane >> 1) & 3;
           const int rl = lane >> 2, piece = lane & 3;
           const int w2 = c.w0 + 8 * j + rl;
@@ -695,9 +599,8 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
           for (int c0 = 0; c0 < p.bn; c0 += 64) {
             if (((j * nch + (c0 >> 6)) & (NEPI / 4 - 1)) != half) continue;
             uint32_t r0[32], r1[32], pk[16];
-            tmem_ld_32x32b_x32(tl + c0, r0);
-            tmem_ld_32x32b_x32(tl + c0 + 32, r1);
-            tmem_ld_wait();
+            load_row32(srow + c0, 32, r0);
+            load_row32(srow + c0 + 32, 32, r1);
             epi_geglu_pack32(r0, sbias + c.n0 + c0, pk);
             epi_geglu_pack32(r1, sbias + c.n0 + c0 + 32, pk + 8);
 #pragma unroll
@@ -720,24 +623,12 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
         } else {
           for (int c0 = ((j + half) & 1) * 32; c0 < p.bn; c0 += 64) {
             uint32_t r[32];
-            tmem_ld_32x32b_x32(tl + c0, r);
-            tmem_ld_wait();
+            load_row32(srow + c0, 32, r);
             if (row_ok) epi_chunk32<MODE>(p.epi, r, min(32, p.bn - c0), c.n0 + c0, sbias + c.n0 + c0, c.b, c.t, h, w, row_base);
           }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(t_empty + 8 * buf);
-      if (++buf == (uint32_t)p.nbuf) { buf = 0; bpar ^= 1; }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (p.cluster > 1) cluster_sync_all();     // the peer may still multicast into / arrive on this CTA's shared memory
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -745,64 +636,24 @@ __global__ void __launch_bounds__(512, 1) tc_slab_kernel(const __grid_constant__
 
 using namespace mv2;
 
-
-// ---- N-tile width for deep, wide layers (Co > 256, few positions) -------------------------------------------------------
-// With 128 x 256 tiles a 512-channel 16x16 layer has only 80 .. 320 tiles for 148 persistent CTAs, so up to half of the
-// SMs idle in the last wave.  Narrower, possibly ragged N tiles (e.g. 3 x 176 columns for Co = 512) trade a little MMA
-// efficiency for a full wave.  The choice comes from a small makespan model calibrated on profiles/r01_sweep_ragged.json:
-//   tile cost  = live frame taps(t) * kchunks * kh*kw * mw * 4 MMAs * max(bn/2, 1.28 * (32 + bn/4)) cycles
-//                (tensor pipe vs the shared-memory operand bandwidth of one 128 x bn x 16 MMA) + per-tile overhead,
-//   assignment = the kernel's static schedule (slab_frame_of / slab_tile_of: cost-sorted frames, serpentine over the CTAs).
-// A ragged candidate must beat the power-of-two default by 8 % in the model; results are cached per layer shape.
-static double slab_model_cycles(const mv2_tc_conv_args* a, int n_sm, int mw, int bn) {
-  const int tiles_per_frame = ceil_div(a->Ho, 16) * ceil_div(a->Wo, 8 * mw) * ceil_div(a->Co, bn);
-  const double t_mma = std::max(bn / 2.0, 1.28 * (32.0 + bn / 4.0));
-  const double per_tap_frame = (double)(a->Ci / 64) * a->kh * a->kw * mw * 4.0 * t_mma;
-  const double fixed = 3000.0 + (2 * mw * bn > 512 ? mw * bn * 10.0 : 0.0);   // + unoverlapped epilogue when single buffered
-  const int64_t total = (int64_t)a->B * a->To * tiles_per_frame;
-  const int G = (int)std::min<int64_t>(total, n_sm);
-  std::vector<double> load(G, 0.0);
-  int64_t idx = 0;
-  // same enumeration as the kernel: full-cost frames first, then t = pt-1 ... 0 of every clip; serpentine over the CTAs
-  const int n_cheap = std::max(0, std::min(a->pt, a->To)), n_full = a->To - n_cheap;
-  auto deal = [&](int frames, int live) {
-    const double cost = live * per_tap_frame + fixed;
-    for (int64_t i = 0; i < (int64_t)frames * tiles_per_frame; ++i, ++idx) {
-      const int64_t k = idx / G, pos = idx % G;
-      load[(k & 1) ? G - 1 - pos : pos] += cost;
-    }
-  };
-  deal(a->B * n_full, a->kt);
-  for (int level = 0; level < n_cheap; ++level) deal(a->B, a->kt - (a->pt - (n_cheap - 1 - level)));
-  return *std::max_element(load.begin(), load.end());
+// kernel instance per (epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared memory
+#define MV2_SLAB_BN(M) {tc_slab_kernel<M, 32>, tc_slab_kernel<M, 64>, tc_slab_kernel<M, 128>}
+static void (*const g_slab_kernels[8][3])(SlabParams) = {
+    MV2_SLAB_BN(EPI_PLAIN), MV2_SLAB_BN(EPI_GEGLU), MV2_SLAB_BN(EPI_SHUFFLE), MV2_SLAB_BN(EPI_RAGGED),
+    MV2_SLAB_BN(EPI_PLAIN_RES), MV2_SLAB_BN(EPI_FUSED_RU), MV2_SLAB_BN(EPI_SHUFFLE_ST), MV2_SLAB_BN(EPI_DOWN_SPACE)};
+#undef MV2_SLAB_BN
+static void (*slab_kernel_for(int mode, int bn))(SlabParams) { return g_slab_kernels[mode][bn == 32 ? 0 : (bn == 64 ? 1 : 2)]; }
+static cudaError_t slab_set_smem_attr() {
+  static PerDeviceOnce once;
+  return once.run([] {
+    cudaError_t e = cudaSuccess;
+    for (auto& row : g_slab_kernels)
+      for (auto k : row)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    return e;
+  });
 }
 
-static void choose_ragged_tiles(const mv2_tc_conv_args* a, int n_sm, int* mw_io, int* bn_io) {
-  struct Key { int v[10]; bool operator<(const Key& o) const { return memcmp(v, o.v, sizeof(v)) < 0; } };
-  static std::mutex mu;
-  static std::map<Key, std::pair<int, int>> cache;
-  const Key key = {{a->B, a->To, a->Ho, a->Wo, a->Ci, a->Co, a->kt, a->kh, a->kw, n_sm}};
-  std::lock_guard<std::mutex> lk(mu);
-  auto it = cache.find(key);
-  if (it == cache.end()) {
-    int mw = *mw_io, bn = *bn_io;
-    const double base = slab_model_cycles(a, n_sm, mw, bn);
-    double best = base * 0.92;
-    for (int j = ceil_div(a->Co, 256) + 1; j <= ceil_div(a->Co, 128); ++j) {
-      const int cbn = (ceil_div(a->Co, j) + 15) / 16 * 16;
-      if (cbn > 256 || cbn < 128) continue;
-      for (int cmw = 1; cmw <= 2; ++cmw) {
-        if (cmw == 2 && (a->Wo <= 8 || cmw * cbn > 512)) continue;
-        // two M-tiles per weight tile halve the weight stream, which the model does not see: worth ~3 %
-        const double c = slab_model_cycles(a, n_sm, cmw, cbn) * (cmw == 2 ? 0.97 : 1.0);
-        if (c < best) { best = c; mw = cmw; bn = cbn; }
-      }
-    }
-    it = cache.emplace(key, std::make_pair(mw, bn)).first;
-  }
-  *mw_io = it->second.first;
-  *bn_io = it->second.second;
-}
 
 extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
   if (!a) return 0;
@@ -842,64 +693,52 @@ static int slab_fill_plan(const mv2_tc_conv_args* a, int n_sm, SlabParams& p, in
   p.epi.act = a->act; p.epi.shuffle = a->shuffle; p.epi.mode = a->epi_mode; p.epi.Co = a->Co;
   p.epi.To = a->To; p.epi.Ho = a->Ho; p.epi.Wo = a->Wo; p.epi.out_cf = a->out_layout == 1; p.epi.oscale = a->oscale;
 
-  // ---- tiling (profiles/r01_sweep_slab_v*.json): widest N tile; two M-tiles per weight tile whenever both
-  //      accumulator sets still double-buffer in TMEM (2 * mw * bn <= 512), which also halves weight traffic ----
+  // ---- tiling: widest N tile (<= 128 columns); M-tiles side by side share each weight tile while their accumulators
+  //      fit 64 fp32 registers per consumer thread (mw * bn <= 128), which divides the weight traffic by mw ----
   const int tiles_h = ceil_div(a->Ho, 16);
   const int co_pad = (a->Co + 31) / 32 * 32;
   int best_bn = 32;
-  for (int bn = 256; bn >= 32; bn >>= 1)
-    if (bn <= co_pad && co_pad % bn == 0) { best_bn = bn; break; }
-  int best_mw = (best_bn <= 128 && a->Wo > 8) ? 2 : 1;
-  if (best_bn <= 64 && a->Wo > 16) best_mw = 4;   // narrow N: four M-tiles per weight tile still double-buffer in TMEM
-  // EPI_PLAIN guards every stored column, so N tiles need not divide Co: deep wide layers pick the width that fills
-  // the 148 SMs best (choose_ragged_tiles)
-  const bool ragged_ok = a->epi_mode == 0 && a->shuffle == MV2_SHUFFLE_NONE && a->Co % 8 == 0;
-  if (ragged_ok && a->Co > 256 && a->kt * a->kh * a->kw > 1 && a->st == 1) choose_ragged_tiles(a, n_sm, &best_mw, &best_bn);
+  for (int bn = 128; bn >= 32; bn >>= 1)
+    if (co_pad % bn == 0) { best_bn = bn; break; }
   // wide outputs whose width has no large power-of-two divisor (the GEGLU feed-forward: 2 * 1365 -> 2752 packed columns
-  // would run 43 tiles of 64): 64-column MMAs are shared-memory bound, so take wide tiles and let the last one be ragged
-  // (the GEGLU epilogue guards its 16-column groups against Co like the plain one guards its 8-column pieces)
-  if ((ragged_ok || a->epi_mode == 1) && best_bn <= 64 && co_pad >= 512) {
-    for (int bn : {256, 192, 128}) {
-      const int padded = (co_pad + bn - 1) / bn * bn;
-      if (padded * 100 <= co_pad * 108) { best_bn = bn; best_mw = (bn <= 128 && a->Wo > 8) ? 2 : 1; break; }
-    }
-  }
+  // would run 43 tiles of 64): take 128-column tiles and let the last one be ragged (the plain and GEGLU epilogues guard
+  // every stored column against Co)
+  const bool ragged_ok = a->epi_mode == 0 && a->shuffle == MV2_SHUFFLE_NONE && a->Co % 8 == 0;
+  if ((ragged_ok || a->epi_mode == 1) && best_bn <= 64 && co_pad >= 512 && (co_pad + 127) / 128 * 128 * 100 <= co_pad * 108)
+    best_bn = 128;
+  int best_mw = 1;
+  if (a->Wo > 8 && best_bn <= 64) best_mw = 2;
+  if (a->Wo > 16 && best_bn == 32) best_mw = 4;
   if (const char* env = getenv("MV2_SLAB_CFG")) {   // debug / tuning override: "mw,bn"
     int emw = 0, ebn = 0;
-    if (sscanf(env, "%d,%d", &emw, &ebn) == 2 && (emw == 1 || emw == 2 || emw == 4) && ebn >= 32 && ebn <= 256 && ebn % 16 == 0 &&
-        (a->epi_mode == 1 ? ebn % 64 == 0 : (co_pad % ebn == 0 || ragged_ok)) && emw * ebn <= 512 && !(emw >= 2 && a->Wo <= 8)) { best_mw = emw; best_bn = ebn; }
+    if (sscanf(env, "%d,%d", &emw, &ebn) == 2 && (emw == 1 || emw == 2 || emw == 4) && (ebn == 32 || ebn == 64 || ebn == 128) &&
+        (a->epi_mode == 1 ? ebn % 64 == 0 : (co_pad % ebn == 0 || ragged_ok)) && emw * ebn <= 128 && !(emw >= 2 && a->Wo <= 8)) { best_mw = emw; best_bn = ebn; }
   }
   p.mw = best_mw; p.bn = best_bn;
-  // measured inside a README step (profiles/r02_sweep_ff.json, CUPTI): fc1 + GEGLU 329 us with the direct row-piece stores, 339 us
-  // staged -- the epilogue is bound by the issue of its ~35 instructions per output, not by its stores -- so staged is opt-in
   p.geglu_staged = (a->epi_mode == 1 && p.bn % 64 == 0 && getenv("MV2_GEGLU_STAGED")) ? 1 : 0;
   p.n_tiles_n = (co_pad + p.bn - 1) / p.bn;   // a ragged last tile reads zero-filled weight rows and stores nothing for them
-  // weight multicast across CTA pairs: when one M-tile per CTA cannot amortise the weight stream (mw == 1, deep
-  // layers) two CTAs on neighbouring tiles fetch half of every weight tile each and multicast it to both
-  // (measured: no gain on B200 at these shapes -- the deep layers are wave-quantisation bound, not weight-stream bound --
-  //  so it is off unless MV2_SLAB_CLUSTER=2)
-  p.cluster = 1;
-  if (const char* env = getenv("MV2_SLAB_CLUSTER")) p.cluster = (atoi(env) == 2 && p.mw == 1 && ceil_div(a->Wo, 8) % 2 == 0 && p.bn >= 64 && a->Co % p.bn == 0) ? 2 : 1;
   p.tiles_h = tiles_h;
+  p.slab_h = 16 + a->kh - 1;
+  const int nb_pad = p.n_tiles_n * p.bn;   // bias staging covers the padded column range
+  int budget;
+  for (;; p.mw >>= 1) {     // a wide macro tile whose two slab stages and accumulator staging do not fit: narrow it
+    p.pitch = 8 * p.mw + a->kw - 1;
+    p.slab_bytes = p.pitch * p.slab_h * p.row_bytes;
+    p.slab_stride = (p.slab_bytes + 1023) / 1024 * 1024;
+    p.slab_stages = 3; p.w_stages = 12;      // upper bounds for the barrier table
+    // 227 KB minus what follows the rings (barriers, bias, transpose buffers, accumulator staging) and alignment slack
+    budget = 227 * 1024 - 2048 - (int)slab_smem_layout(p, 0, false).end;
+    if (p.mw == 1 || 2 * p.slab_stride + 2 * p.bn * p.row_bytes <= budget) break;
+  }
   p.tiles_w = ceil_div(a->Wo, 8 * p.mw);
   p.total_tiles = (int)((int64_t)a->B * a->To * p.tiles_h * p.tiles_w * p.n_tiles_n);
-  p.pitch = 8 * p.mw + a->kw - 1;
-  p.slab_h = 16 + a->kh - 1;
-  p.slab_bytes = p.pitch * p.slab_h * p.row_bytes;
-  p.slab_stride = (p.slab_bytes + 1023) / 1024 * 1024;
-  p.nbuf = (2 * p.mw * p.bn <= 512) ? 2 : 1;
-  p.acc_stride = p.nbuf == 2 ? 256 : 0;
   // weight ring stage = tpw consecutive in-plane taps (fewer barrier round trips for small tiles), <= 32 KB
   const int taps2d = a->kh * a->kw;
   p.tpw = 1;
   for (int d = taps2d; d >= 1; --d)
     if (taps2d % d == 0 && d * p.bn * p.row_bytes <= 32 * 1024) { p.tpw = d; break; }
-  if (p.cluster > 1) p.tpw = 1;
   if (const char* env = getenv("MV2_SLAB_TPW")) { const int v = atoi(env); if (v >= 1 && taps2d % v == 0 && v * p.bn * p.row_bytes <= 64 * 1024) p.tpw = v; }
   int w_bytes = p.bn * p.row_bytes * p.tpw;
-  const int nb_pad = p.n_tiles_n * p.bn;   // bias staging covers the padded column range
-  // 227 KB minus the epilogue transpose buffers (2 KB per epilogue warp: 16 KB, 32 KB for fc1 + GEGLU), barriers, alignment slack
-  const int budget = 204 * 1024 - nb_pad * 4 - (a->epi_mode == 1 ? (SlabEpiWarps<EPI_GEGLU>::value - 8) * 2048 : 0);
   p.slab_stages = p.slab_stride * 3 + w_bytes * 3 <= budget ? 3 : 2;
   if (const char* env = getenv("MV2_SLAB_STAGES")) {   // tuning override: activation-slab ring depth
     const int v = atoi(env);
@@ -907,7 +746,7 @@ static int slab_fill_plan(const mv2_tc_conv_args* a, int n_sm, SlabParams& p, in
   }
   p.w_stages = std::min(12, (budget - p.slab_stages * p.slab_stride) / w_bytes);
   if (p.w_stages < 2 && p.slab_stages > 2) { p.slab_stages = 2; p.w_stages = std::min(12, (budget - 2 * p.slab_stride) / w_bytes); }
-  while (p.w_stages < 2 && p.tpw > 1) {   // wide slabs (mw = 4) + the fp32 residual staging: fall back to fewer taps per weight stage
+  while (p.w_stages < 2 && p.tpw > 1) {   // wide slabs: fall back to fewer taps per weight stage
     int d = p.tpw - 1;
     while (d > 1 && taps2d % d != 0) --d;
     p.tpw = d;
@@ -927,9 +766,8 @@ extern "C" int mv2_tc_slab_plan(const mv2_tc_conv_args* a, int n_sm, int* out6) 
   int bk, w_bytes, co_pad, nb_pad;
   const int rc = slab_fill_plan(a, n_sm, p, &bk, &w_bytes, &co_pad, &nb_pad);
   if (rc != MV2_OK) return rc;
-  int grid = std::min(p.total_tiles, n_sm);
-  if (p.cluster > 1) grid &= ~1;
-  out6[0] = p.mw; out6[1] = p.bn; out6[2] = p.n_tiles_n; out6[3] = p.total_tiles; out6[4] = grid; out6[5] = p.nbuf;
+  const int grid = std::min(p.total_tiles, n_sm);
+  out6[0] = p.mw; out6[1] = p.bn; out6[2] = p.n_tiles_n; out6[3] = p.total_tiles; out6[4] = grid; out6[5] = p.slab_stages;
   return MV2_OK;
 }
 
@@ -940,8 +778,7 @@ extern "C" int mv2_tc_slab_tile(const mv2_tc_conv_args* a, int n_sm, int cta, in
   int bk, w_bytes, co_pad, nb_pad;
   const int rc = slab_fill_plan(a, n_sm, p, &bk, &w_bytes, &co_pad, &nb_pad);
   if (rc != MV2_OK) return rc;
-  int grid = std::min(p.total_tiles, n_sm);
-  if (p.cluster > 1) grid &= ~1;
+  const int grid = std::min(p.total_tiles, n_sm);
   MV2_CHECK_ARG(cta < grid);
   const int tile = slab_tile_of_cta(p, k, cta, grid);
   out6[0] = tile;                                // -1: this CTA has no k-th tile
@@ -957,7 +794,7 @@ extern "C" int mv2_tc_slab_forward(const mv2_tc_conv_args* a, void* stream) {
   if (!mv2_tc_slab_supported(a)) { set_error("mv2_tc_slab_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return MV2_E_CUDA; }
-  int dev = 0, n_sm = 148;
+  int dev = 0, n_sm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
 
@@ -985,7 +822,7 @@ extern "C" int mv2_tc_slab_forward(const mv2_tc_conv_args* a, void* stream) {
     const int64_t K = ntaps * a->Ci;
     cuuint64_t dims[3] = {(cuuint64_t)a->Ci, (cuuint64_t)a->Co, (cuuint64_t)ntaps};
     cuuint64_t strides[2] = {(cuuint64_t)(K * 2), (cuuint64_t)(a->Ci * 2)};
-    cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)(p.bn / p.cluster), (cuuint32_t)p.tpw};
+    cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)p.bn, (cuuint32_t)p.tpw};
     cuuint32_t es[3] = {1, 1, 1};
     CUresult r = enc(&p.wmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)a->w, dims, strides, box, es,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -993,36 +830,24 @@ extern "C" int mv2_tc_slab_forward(const mv2_tc_conv_args* a, void* stream) {
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(weights) failed: %d", (int)r); return MV2_E_CUDA; }
     cuuint64_t dims2[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
     cuuint64_t strides2[1] = {(cuuint64_t)(K * 2)};
-    cuuint32_t box2[2] = {(cuuint32_t)bk, (cuuint32_t)(p.bn / p.cluster)};
+    cuuint32_t box2[2] = {(cuuint32_t)bk, (cuuint32_t)p.bn};
     cuuint32_t es2[2] = {1, 1};
     r = enc(&p.wmap2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)a->w, dims2, strides2, box2, es2,
             CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(weights 2-D) failed: %d", (int)r); return MV2_E_CUDA; }
   }
-  const size_t smem = (size_t)p.slab_stages * p.slab_stride + (size_t)p.w_stages * w_bytes + 8 * (2 * p.slab_stages + 2 * p.w_stages + 4) + 32 + (size_t)nb_pad * 4 +
-                      (size_t)(a->epi_mode == 1 ? SlabEpiWarps<EPI_GEGLU>::value : 8) * 2048 + 1024;
+  const size_t smem = 1024 + slab_smem_layout(p, (uint32_t)(p.slab_stages * p.slab_stride + p.w_stages * w_bytes), false).end;
   MV2_CHECK_ARG(smem <= 227 * 1024);
-  static PerDeviceOnce attr_once;
-  const cudaError_t attr_err = attr_once.run([] {
-    cudaError_t e = cudaFuncSetAttribute(tc_slab_kernel<EPI_PLAIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_slab_kernel<EPI_GEGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_slab_kernel<EPI_SHUFFLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_slab_kernel<EPI_RAGGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_slab_kernel<EPI_PLAIN_RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_slab_kernel<EPI_FUSED_RU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_slab_kernel<EPI_SHUFFLE_ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    return e;
-  });
+  const cudaError_t attr_err = slab_set_smem_attr();
   if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
-  int grid = std::min(p.total_tiles, n_sm);
-  if (p.cluster > 1) grid &= ~1;
-  if (a->epi_mode == 1) launch_kc(tc_slab_kernel<EPI_GEGLU>, dim3(grid), dim3(128 + 32 * SlabEpiWarps<EPI_GEGLU>::value), smem, (cudaStream_t)stream, p.cluster, p);
-  else if (a->shuffle != MV2_SHUFFLE_NONE && (a->Co / (a->shuffle == MV2_SHUFFLE_SPACE ? 4 : 2)) % 32 == 0 && !getenv("MV2_NO_SHUFFLE_ST"))
-    launch_kc(tc_slab_kernel<EPI_SHUFFLE_ST>, dim3(grid), dim3(384), smem, (cudaStream_t)stream, p.cluster, p);
-  else if (a->shuffle != MV2_SHUFFLE_NONE) launch_kc(tc_slab_kernel<EPI_SHUFFLE>, dim3(grid), dim3(384), smem, (cudaStream_t)stream, p.cluster, p);
-  else if (a->Co % 8 != 0) launch_kc(tc_slab_kernel<EPI_RAGGED>, dim3(grid), dim3(384), smem, (cudaStream_t)stream, p.cluster, p);
-  else if (a->res) launch_kc(tc_slab_kernel<EPI_PLAIN_RES>, dim3(grid), dim3(384), smem, (cudaStream_t)stream, p.cluster, p);
-  else launch_kc(tc_slab_kernel<EPI_PLAIN>, dim3(grid), dim3(384), smem, (cudaStream_t)stream, p.cluster, p);
+  const int grid = std::min(p.total_tiles, n_sm);
+  int mode = EPI_PLAIN;
+  if (a->epi_mode == 1) mode = EPI_GEGLU;
+  else if (a->shuffle != MV2_SHUFFLE_NONE && (a->Co / (a->shuffle == MV2_SHUFFLE_SPACE ? 4 : 2)) % 32 == 0 && !getenv("MV2_NO_SHUFFLE_ST")) mode = EPI_SHUFFLE_ST;
+  else if (a->shuffle != MV2_SHUFFLE_NONE) mode = EPI_SHUFFLE;
+  else if (a->Co % 8 != 0) mode = EPI_RAGGED;
+  else if (a->res) mode = EPI_PLAIN_RES;
+  launch_k(slab_kernel_for(mode, p.bn), dim3(grid), dim3(384), smem, (cudaStream_t)stream, p);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }
@@ -1042,8 +867,8 @@ static void ru_as_conv_args(const mv2_tc_ru_args* a, mv2_tc_conv_args* c) {
 
 extern "C" int mv2_tc_ru_supported(const mv2_tc_ru_args* a) {
   if (!a) return 0;
-  if (a->C != 64 && a->C != 128) return 0;            // all of Co in one N tile (bn = C), mw * C = 256 TMEM columns per buffer
-  if (a->W <= 8) return 0;                            // needs mw >= 2 M-tiles side by side
+  if (a->C != 64 && a->C != 128) return 0;            // all of Co in one N tile (bn = C)
+  if (a->W <= 8) return 0;                            // narrow frames take the unfused path
   if (a->kt < 1 || a->kt > 8 || a->kh < 1 || a->kh > 7 || a->kw < 1 || a->kw > 3) return 0;
   if ((a->kh & 1) == 0 || (a->kw & 1) == 0) return 0;
   mv2_tc_conv_args c;
@@ -1058,32 +883,28 @@ static int ru_fill_plan(const mv2_tc_ru_args* a, int n_sm, SlabParams& p, size_t
   int bk, w_bytes, co_pad, nb_pad;
   const int rc = slab_fill_plan(&c, n_sm, p, &bk, &w_bytes, &co_pad, &nb_pad);
   if (rc != MV2_OK) return rc;
-  MV2_CHECK_ARG(p.bn == a->C && p.n_tiles_n == 1 && p.cluster == 1 && p.row_bytes == 128);
-  // defaults (profiles/r02_sweep_ru.json): C = 128: 2 M-tiles, one H buffer; C = 64: 4 M-tiles (W > 16), two H buffers
-  int mw = (a->C == 64 && a->W > 16) ? 4 : 2, nh = a->C == 64 ? 2 : 1, tpw = 1, slab_stages = 2, w_stages = 0;
-  if (const char* env = getenv("MV2_RU_CFG")) {      // tuning override: "mw,nh,tpw,slab_stages,w_stages" (0 = derive)
-    int v[5] = {0, 0, 0, 0, 0};
-    if (sscanf(env, "%d,%d,%d,%d,%d", &v[0], &v[1], &v[2], &v[3], &v[4]) >= 1) {
-      if ((v[0] == 2 || v[0] == 4) && v[0] * a->C <= 256 && !(v[0] == 4 && a->W <= 16)) mw = v[0];
-      if (v[1] == 1 || v[1] == 2) nh = v[1];
-      if (v[2] >= 1 && (a->kh * a->kw) % v[2] == 0) tpw = v[2];
-      if (v[3] == 2 || v[3] == 3) slab_stages = v[3];
-      if (v[4] >= 2) w_stages = v[4];
+  MV2_CHECK_ARG(p.bn == a->C && p.n_tiles_n == 1 && p.row_bytes == 128);
+  // defaults: as many M-tiles as the 64-register accumulator budget allows (C = 64: 2, C = 128: 1)
+  int mw = a->C == 64 ? 2 : 1, tpw = 1, slab_stages = 2, w_stages = 0;
+  if (const char* env = getenv("MV2_RU_CFG")) {      // tuning override: "mw,tpw,slab_stages,w_stages" (0 = derive)
+    int v[4] = {0, 0, 0, 0};
+    if (sscanf(env, "%d,%d,%d,%d", &v[0], &v[1], &v[2], &v[3]) >= 1) {
+      if ((v[0] == 1 || v[0] == 2) && v[0] * a->C <= 128) mw = v[0];
+      if (v[1] >= 1 && (a->kh * a->kw) % v[1] == 0) tpw = v[1];
+      if (v[2] == 2 || v[2] == 3) slab_stages = v[2];
+      if (v[3] >= 2) w_stages = v[3];
     }
   }
-  p.mw = mw; p.nh = nh; p.tpw = tpw;
+  p.mw = mw; p.tpw = tpw;
   p.tiles_w = ceil_div(a->W, 8 * p.mw);
   p.total_tiles = (int)((int64_t)a->B * a->T * p.tiles_h * p.tiles_w);
   p.pitch = 8 * p.mw + a->kw - 1;
   p.slab_bytes = p.pitch * p.slab_h * p.row_bytes;
   p.slab_stride = (p.slab_bytes + 1023) / 1024 * 1024;
-  p.nbuf = 2; p.acc_stride = 256;
   p.h_stride = p.kchunks * 16384;
   const int wb = p.bn * p.row_bytes * p.tpw;
-  const size_t fixed = 1024 /* base alignment */ + 8 * (2 * 3 + 2 * 16 + 4 + 9) + 64 /* barriers, tmem slot */ + (size_t)3 * nb_pad * 4 +
-                       2048 /* logit partials */ + 1024 /* H alignment */ + (size_t)p.nh * p.h_stride /* H buffers = transpose buffers */ +
-                       (size_t)p.kchunks * p.bn * p.row_bytes /* resident 1x1x1 weights */;
-  MV2_CHECK_ARG(p.nh * p.h_stride >= 8 * 2048);
+  p.slab_stages = 3; p.w_stages = 12;      // upper bounds for the barrier table
+  const size_t fixed = 2048 /* base and H alignment */ + slab_smem_layout(p, 0, true).end;
   const size_t total = 227 * 1024;
   p.slab_stages = slab_stages;
   while (p.slab_stages > 2 && fixed + (size_t)p.slab_stages * p.slab_stride + 2 * (size_t)wb > total) --p.slab_stages;
@@ -1091,7 +912,7 @@ static int ru_fill_plan(const mv2_tc_ru_args* a, int n_sm, SlabParams& p, size_t
   p.w_stages = (int)std::min<int64_t>(12, room / wb);
   if (w_stages >= 2 && w_stages <= p.w_stages) p.w_stages = w_stages;
   MV2_CHECK_ARG(p.w_stages >= 2);
-  *smem_out = fixed + (size_t)p.slab_stages * p.slab_stride + (size_t)p.w_stages * wb;
+  *smem_out = 1024 + slab_smem_layout(p, (uint32_t)(p.slab_stages * p.slab_stride + p.w_stages * wb), true).end;
   p.bias1 = a->b1; p.se_wk = a->se_wk; p.se_bk = a->se_bk; p.se_ws = a->se_ws;
   return MV2_OK;
 }
@@ -1100,7 +921,7 @@ extern "C" int mv2_tc_ru_records(const mv2_tc_ru_args* a) {
   if (!mv2_tc_ru_supported(a)) { set_error("mv2_tc_ru_records: unsupported shape"); return MV2_E_UNSUPPORTED; }
   SlabParams p;
   size_t smem;
-  const int rc = ru_fill_plan(a, 148, p, &smem);
+  const int rc = ru_fill_plan(a, 132, p, &smem);   // the record count does not depend on the SM count
   if (rc != MV2_OK) return rc;
   return p.tiles_h * p.tiles_w * 4;
 }
@@ -1117,7 +938,7 @@ extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, void* stream) {
   if (!mv2_tc_ru_supported(a)) { set_error("mv2_tc_ru_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return MV2_E_CUDA; }
-  int dev = 0, n_sm = 148;
+  int dev = 0, n_sm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   SlabParams p;
@@ -1160,13 +981,10 @@ extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, void* stream) {
             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(w1) failed: %d", (int)r); return MV2_E_CUDA; }
   }
-  static PerDeviceOnce attr_once;
-  const cudaError_t attr_err = attr_once.run([] {
-    return cudaFuncSetAttribute(tc_slab_kernel<EPI_FUSED_RU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  });
+  const cudaError_t attr_err = slab_set_smem_attr();
   if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
   const int grid = std::min(p.total_tiles, n_sm);
-  launch_kc(tc_slab_kernel<EPI_FUSED_RU>, dim3(grid), dim3(384), smem, (cudaStream_t)stream, 1, p);
+  launch_k(slab_kernel_for(EPI_FUSED_RU, p.bn), dim3(grid), dim3(384), smem, (cudaStream_t)stream, p);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }
@@ -1196,7 +1014,7 @@ extern "C" int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream
   if (!mv2_tc_down_space_supported(a)) { set_error("mv2_tc_down_space_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }
   EncodeTiledFn enc = get_encode_fn();
   if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return MV2_E_CUDA; }
-  int dev = 0, n_sm = 148;
+  int dev = 0, n_sm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   SlabParams p;
@@ -1208,24 +1026,26 @@ extern "C" int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream
   p.epi.bias = a->bias; p.epi.res = nullptr; p.epi.y = (__nv_bfloat16*)a->y; p.epi.act = a->act; p.epi.shuffle = MV2_SHUFFLE_NONE;
   p.epi.mode = 0; p.epi.Co = a->Co; p.epi.To = a->To; p.epi.Ho = a->Ho; p.epi.Wo = a->Wo; p.epi.out_cf = 0; p.epi.oscale = nullptr;
   int bn = 32;
-  for (int c = 256; c >= 32; c >>= 1) if (a->Co % c == 0) { bn = c; break; }
-  int mw = (bn <= 128 && a->Wo > 8) ? 2 : 1;
-  if (bn <= 64 && a->Wo > 16) mw = 4;
+  for (int c = 128; c >= 32; c >>= 1) if (a->Co % c == 0) { bn = c; break; }
+  int mw = (bn <= 64 && a->Wo > 8) ? 2 : 1;
+  if (bn == 32 && a->Wo > 16) mw = 4;
   if (const char* env = getenv("MV2_DOWN_CFG")) {
     int emw = 0, ebn = 0;
-    if (sscanf(env, "%d,%d", &emw, &ebn) == 2 && (emw == 1 || emw == 2 || emw == 4) && ebn >= 32 && ebn <= 256 && a->Co % ebn == 0 && emw * ebn <= 512 && !(emw >= 2 && a->Wo <= 8)) { mw = emw; bn = ebn; }
+    if (sscanf(env, "%d,%d", &emw, &ebn) == 2 && (emw == 1 || emw == 2 || emw == 4) && (ebn == 32 || ebn == 64 || ebn == 128) && a->Co % ebn == 0 && emw * ebn <= 128 && !(emw >= 2 && a->Wo <= 8)) { mw = emw; bn = ebn; }
   }
-  const int w_bytes = bn * 128, nb_pad = (a->Co / bn) * bn;
-  const int budget = 204 * 1024 - nb_pad * 4;
-  int o_bytes, e_bytes;
+  const int w_bytes = bn * 128;
+  p.bn = bn; p.n_tiles_n = a->Co / bn; p.tpw = 1;
+  int o_bytes, e_bytes, budget;
   for (;; mw >>= 1) {           // the two row-parity sub-slabs of a 4-M-tile macro tile do not fit twice: narrow the macro tile
+    p.mw = mw;
+    p.slab_stages = 3; p.w_stages = 12;      // upper bounds for the barrier table
+    budget = 227 * 1024 - 2048 - (int)slab_smem_layout(p, 0, false).end;
     p.pitch = 8 * mw + 1;
     o_bytes = 17 * p.pitch * 128; e_bytes = 16 * p.pitch * 128;
     p.dn_e_off = (o_bytes + 1023) / 1024 * 1024;
     p.slab_stride = p.dn_e_off + (e_bytes + 1023) / 1024 * 1024;
     if (mw == 1 || 2 * p.slab_stride + 3 * w_bytes <= budget) break;
   }
-  p.mw = mw; p.bn = bn; p.n_tiles_n = a->Co / bn; p.cluster = 1; p.tpw = 1;
   p.tiles_h = ceil_div(a->Ho, 16); p.tiles_w = ceil_div(a->Wo, 8 * mw);
   p.total_tiles = (int)((int64_t)a->B * a->To * p.tiles_h * p.tiles_w * p.n_tiles_n);
   p.slab_h = 17;
@@ -1233,8 +1053,6 @@ extern "C" int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream
   for (int dh = 0; dh < 3; ++dh)
     for (int q = 0; q < 2; ++q)      // q = dw2 + 1
       p.dn_aoff[dh * 2 + q] = ((dh == 1 ? p.dn_e_off : 0) + ((dh == 2 ? p.pitch : 0) + q) * 128) >> 4;
-  p.nbuf = (2 * mw * bn <= 512) ? 2 : 1;
-  p.acc_stride = p.nbuf == 2 ? 256 : 0;
   p.slab_stages = p.slab_stride * 3 + w_bytes * 4 <= budget ? 3 : 2;
   p.w_stages = std::min(12, (budget - p.slab_stages * p.slab_stride) / w_bytes);
   MV2_CHECK_ARG(p.w_stages >= 2);
@@ -1260,16 +1078,12 @@ extern "C" int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(weights) failed: %d", (int)r); return MV2_E_CUDA; }
     p.wmap = p.wmap2;
   }
-  const size_t smem = (size_t)p.slab_stages * p.slab_stride + (size_t)p.w_stages * w_bytes + 8 * (2 * p.slab_stages + 2 * p.w_stages + 4 + 9) + 32 +
-                      (size_t)nb_pad * 4 + 8 * 2048 + 1024;
+  const size_t smem = 1024 + slab_smem_layout(p, (uint32_t)(p.slab_stages * p.slab_stride + p.w_stages * w_bytes), false).end;
   MV2_CHECK_ARG(smem <= 227 * 1024);
-  static PerDeviceOnce attr_once;
-  const cudaError_t attr_err = attr_once.run([] {
-    return cudaFuncSetAttribute(tc_slab_kernel<EPI_DOWN_SPACE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  });
+  const cudaError_t attr_err = slab_set_smem_attr();
   if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
   const int grid = std::min(p.total_tiles, n_sm);
-  launch_kc(tc_slab_kernel<EPI_DOWN_SPACE>, dim3(grid), dim3(384), smem, (cudaStream_t)stream, 1, p);
+  launch_k(slab_kernel_for(EPI_DOWN_SPACE, p.bn), dim3(grid), dim3(384), smem, (cudaStream_t)stream, p);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }

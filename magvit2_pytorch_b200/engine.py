@@ -1,9 +1,9 @@
-"""Host-side executor: walks the VideoTokenizer layer schedule and launches the sm_100a
+"""Host-side executor: walks the VideoTokenizer layer schedule and launches the sm_90a
 kernels of libmagvit2_b200.so through the C ABI (ctypes).  PyTorch is used only for device
 memory (caching allocator), streams and parameter storage.
 
 Activations are channels-last (B, T, H, W, C) tensors in the compute dtype (fp32 -> CUDA-core
-path, bf16 -> tcgen05 tensor-core path for the dense contractions).  There is no eager / CPU
+path, bf16 -> wgmma tensor-core path for the dense contractions).  There is no eager / CPU
 fallback: every op is a library call and a missing library is an error.
 """
 from __future__ import annotations
@@ -44,9 +44,9 @@ class ConvPack:
     k: Tuple[int, int, int]
     Ci: int
     Co: int
-    w_tc: Optional[torch.Tensor] = None      # [Co][taps*Ci] bf16, K-major (tcgen05 path); rows permuted for shuffles
+    w_tc: Optional[torch.Tensor] = None      # [Co][taps*Ci] bf16, K-major (wgmma path); rows permuted for shuffles
     bias_tc: Optional[torch.Tensor] = None   # bias in w_tc's row order
-    Ci_tc: int = 0                           # GEMM dims of the tcgen05 call (may be padded / re-paired)
+    Ci_tc: int = 0                           # GEMM dims of the wgmma call (may be padded / re-paired)
     Co_tc: int = 0
     epi_mode: int = 0                        # 1: fused GEGLU (output has Co_tc // 2 channels)
     k_tc: Optional[Tuple[int, int, int]] = None
@@ -56,7 +56,7 @@ class ConvPack:
 
 def pack_conv(weight: torch.Tensor, bias: Optional[torch.Tensor], dtype, k=None, shuffle_q: int = 1) -> ConvPack:
     """weight: torch layout (Co, Ci, *kernel).  Kernel dims are mapped onto (kt, kh, kw) by `k`.
-    shuffle_q = 4 / 2 for the depth-to-space / depth-to-time up-samplers: the tcgen05 kernel wants output
+    shuffle_q = 4 / 2 for the depth-to-space / depth-to-time up-samplers: the wgmma kernel wants output
     rows ordered (q, c) instead of the reference's (c, q) so shuffled stores are channel-contiguous."""
     Co, Ci = weight.shape[:2]
     if k is None:
@@ -99,7 +99,7 @@ def _round_up(v, m):
 
 
 def pack_ff(fc1_w, fc1_b, fc2_w, fc2_b, dtype):
-    """FeedForward weights (reference M:492-496).  tcgen05 layout: the hidden width I is padded to a multiple of 64,
+    """FeedForward weights (reference M:492-496).  wgmma layout: the hidden width I is padded to a multiple of 64,
     fc1's rows are re-paired as [8 x-rows, their 8 gate-rows] per group of 16 so GEGLU (M:466-469) fuses into fc1's
     epilogue, and fc2's K is zero-padded to match."""
     fc1 = pack_conv(fc1_w, fc1_b, dtype)
@@ -128,7 +128,7 @@ def pack_ff(fc1_w, fc1_b, fc2_w, fc2_b, dtype):
 
 
 def pack_conv_in_kwpack(weight, bias, cpack=32):
-    """conv_in (M:1109) for the tcgen05 path: (Co, Cin, kt, kh, kw) -> [Co][(dt, dh)][dw * Cin + c], zero padded to
+    """conv_in (M:1109) for the wgmma path: (Co, Cin, kt, kh, kw) -> [Co][(dt, dh)][dw * Cin + c], zero padded to
     `cpack` channels -- pairs with mv2_ingest_kwpack."""
     Co, Cin, kt, kh, kw = weight.shape
     if Cin * kw > cpack:
@@ -155,13 +155,12 @@ class Engine:
         self._sig = None
         self._sig_id = 0             # bumped whenever parameters are re-packed (invalidates cached CUDA graphs)
         self.launches = 0            # kernels launched through the C ABI (bench's gpu_launches)
-        self.use_tc = True           # bf16: dense contractions on tcgen05 (False -> CUDA-core cross-check path)
+        self.use_tc = True           # bf16: dense contractions on wgmma (False -> CUDA-core cross-check path)
         self.tc_variant = "auto"     # "auto" | "tap" (tc_conv.cu only) | "slab" (prefer tc_slab.cu)
-        self.fuse_ru = True          # bf16: conv3x3x3 + ELU + conv1x1x1 + ELU + SE pool partials in one tcgen05 launch (C = 64 / 128)
+        self.fuse_ru = True          # bf16: conv3x3x3 + ELU + conv1x1x1 + ELU + SE pool partials in one wgmma launch (C = 64 / 128)
         self.fused_ru_calls = 0
-        # bf16, small frames: SE pool + gate MLP + gate/residual in ONE launch (mv2_se_tail).  Off by default: measured 38 us per
-        # unit at C = 512 / 16x16 (one CTA per frame is instruction-issue bound: ncu issue-active 49 %, 7.7 k warp instructions
-        # per warp) against 36 us for the four small launches under graph replay (profiles/r02_se_tail.json)
+        # bf16, small frames: SE pool + gate MLP + gate/residual in ONE launch (mv2_se_tail).  Off by default (an unmeasured
+        # default on this GPU): one CTA per frame leaves most of the SMs idle at the small frame counts of the README config
         self.se_tail = False
         self.se_tail_calls = 0
         self.fuse_conv_out = True    # bf16: conv_out stores torch's (B,C,T,H,W) directly and skips the time_padding frames
@@ -169,8 +168,8 @@ class Engine:
         self.slab_calls = 0
         self.simt_conv_calls = 0
         self.taps: Optional[dict] = None  # when set, per-stage activations are recorded (tests)
-        self._prof: Optional[list] = None  # when set, (event0, event1, flops) per tcgen05 conv launch
-        self.conv_log: Optional[list] = None  # when set, one shape record per tcgen05 conv launch (tools/step_breakdown.py)
+        self._prof: Optional[list] = None  # when set, (event0, event1, flops) per wgmma conv launch
+        self.conv_log: Optional[list] = None  # when set, one shape record per tensor-core conv launch
 
     # ------------------------------------------------------------------ parameters
     def _signature(self):
@@ -185,13 +184,13 @@ class Engine:
         m = self.model
         p0 = m.conv_in.conv.weight
         if p0.device.type != "cuda":
-            raise RuntimeError("magvit2_pytorch_b200.VideoTokenizer runs on CUDA (sm_100a) only; "
+            raise RuntimeError("magvit2_pytorch_b200.VideoTokenizer runs on CUDA (sm_90a) only; "
                                "move the model with .cuda() -- there is no CPU fallback")
         if p0.dtype not in (torch.float32, torch.bfloat16):
             raise TypeError("parameters must be float32 or bfloat16")
         arch = self.lib.mv2_device_arch()
-        if arch < 100:
-            raise RuntimeError(f"libmagvit2_b200.so targets sm_100a; device reports sm_{arch}")
+        if arch != 90:
+            raise RuntimeError(f"libmagvit2_b200.so targets sm_90a (H100); device reports sm_{arch}")
         self.dtype = p0.dtype
         self.device = p0.device
         dt = self.dtype
@@ -299,7 +298,7 @@ class Engine:
     def conv(self, x, pk: ConvPack, *, stride=(1, 1, 1), pad=None, out_spatial=None, act=ACT_NONE,
              res=None, shuffle=SHUFFLE_NONE, token_shift=False, out_cf=False, oscale=None):
         """x: (B,T,H,W,Ci) channels-last.  `pad` = leading (pt,ph,pw); causal default (kt-1, kh//2, kw//2).
-        out_cf (tcgen05 slab path, Co % 8 != 0 only): write torch's (B,Co,To,Ho,Wo) layout directly."""
+        out_cf (wgmma slab path, Co % 8 != 0 only): write torch's (B,Co,To,Ho,Wo) layout directly."""
         B, Ti, Hi, Wi, Ci = x.shape
         tc_ok = (self.dtype == torch.bfloat16 and self.use_tc and pk.w_tc is not None and not token_shift
                  and Ci == pk.Ci_tc)
@@ -327,9 +326,8 @@ class Engine:
                             kt=kt, kh=kh, kw=kw, st=stride[0], sh=stride[1], sw=stride[2],
                             pt=pad[0], ph=pad[1], pw=pad[2], act=act, shuffle=shuffle, epi_mode=pk.epi_mode,
                             oscale=_ptr(oscale), out_layout=int(out_cf))
-            # measured policy (profiles/r01_sweep_slab_v*.json): the persistent slab kernel wins on every layer it supports
-            # (incl. the 64-byte-row conv_in once it runs 4 M-tiles and 7 taps per weight stage); the tap-wise kernel
-            # keeps the strided down-samplers.  tc_variant = "tap" forces the tap-wise kernel (tests / sweeps).
+            # policy: the persistent slab kernel reuses each activation slab for all in-plane taps, so it takes every layer it
+            # supports (incl. the 64-byte-row conv_in); the tap-wise kernel keeps the strided down-samplers.  tc_variant = "tap" forces the tap-wise kernel (tests / sweeps).
             use_slab = self.tc_variant != "tap" and bool(self.lib.mv2_tc_slab_supported(C.byref(ta)))
             use_down = (not use_slab and self.tc_variant != "tap" and pk.w_down is not None and stride == (1, 2, 2)
                         and bool(self.lib.mv2_tc_down_space_supported(C.byref(ta))))
@@ -358,8 +356,8 @@ class Engine:
                 self.launches += 1
                 self.tc_calls += 1
                 return y
-            assert not out_cf, "channels-first output is a tcgen05 slab-kernel feature"
-            assert pk.w is not None and pk.epi_mode == 0 and Ci == pk.Ci, "tcgen05-only weight pack has no CUDA-core fallback"
+            assert not out_cf, "channels-first output is a wgmma slab-kernel feature"
+            assert pk.w is not None and pk.epi_mode == 0 and Ci == pk.Ci, "wgmma-only weight pack has no CUDA-core fallback"
             kt, kh, kw = pk.k
         assert Ci == pk.Ci, (Ci, pk.Ci)
         assert pk.w is not None and not out_cf
@@ -478,7 +476,7 @@ class Engine:
         """Residual(FeedForward) (M:471-508, M:1191): x + fc2(geglu(fc1(rmsnorm(shift(x)))))."""
         B, T, H, W, Cc = x.shape
         xn = self.rmsnorm(x, p["gamma"], token_shift)
-        # fused fc1 + GEGLU pack is tcgen05-only (K = C must be a multiple of 16); other widths take the unfused
+        # fused fc1 + GEGLU pack is wgmma-only (K = C must be a multiple of 16); other widths take the unfused
         # CUDA-core convs + mv2_geglu below, like the fp32 path
         if self.dtype == torch.bfloat16 and self.use_tc and p["fc1"].epi_mode == 1 and Cc % 16 == 0:
             g = self.conv(xn, p["fc1"])                       # fc1 + bias + GEGLU fused, hidden width padded to 64
@@ -546,10 +544,10 @@ class Engine:
         return out
 
     def profile_convs(self, fn, steps: int = 3):
-        """Runs fn() `steps` times with CUDA events around every tcgen05 conv launch (on the launching stream).
+        """Runs fn() `steps` times with CUDA events around every wgmma conv launch (on the launching stream).
         A long spin kernel is queued first so the host runs ahead of the GPU and the event pairs bracket pure
         kernel time, not host launch gaps.  Returns {class: (kernel ms per step, launches per step, FLOPs per step)}
-        for class in 'conv3d' (taps > 1 convs in tc_slab_kernel: the causal Conv3d path) and 'all' (every tcgen05 launch)."""
+        for class in 'conv3d' (taps > 1 convs in tc_slab_kernel: the causal Conv3d path) and 'all' (every wgmma launch)."""
         fn()
         torch.cuda.synchronize(self.device)
         self._prof = []

@@ -1,4 +1,4 @@
-"""Parameter containers of the B200 VideoTokenizer.
+"""Parameter containers of the H100 VideoTokenizer.
 
 These ``nn.Module`` classes hold parameters under exactly the attribute paths of the reference
 model so that ``state_dict()`` keys are interchangeable with reference checkpoints
@@ -313,7 +313,7 @@ class CausalConvTranspose3d(nn.Module):
         assert x.ndim == 5
         w = self.conv.weight
         if w.device.type != "cuda" or x.device != w.device:
-            raise RuntimeError("CausalConvTranspose3d runs on CUDA (sm_100a) only, input and parameters on the same device")
+            raise RuntimeError("CausalConvTranspose3d runs on CUDA (sm_90a) only, input and parameters on the same device")
         if w.dtype not in (torch.float32, torch.bfloat16):
             raise TypeError("parameters must be float32 or bfloat16")
         sig = (w.data_ptr(), w._version, w.dtype, w.device, None if self.conv.bias is None else self.conv.bias._version)

@@ -4,7 +4,7 @@ model(video, return_loss=True); loss.backward()`` for tokenizers without the GAN
 (reference trainer.py:356-363).
 
 Division of labour
-  * FORWARD: the hand-written sm_100a kernels of the inference path (engine.Engine / libmagvit2_b200.so), with the
+  * FORWARD: the hand-written sm_90a kernels of the inference path (engine.Engine / libmagvit2_b200.so), with the
     ResidualUnit run unfused so that its intermediate activations exist.  The activations the backward needs are kept as
     they come out of the kernels (channels-last).
   * BACKWARD: the DATA gradient of the stride-1 causal convs (the 3x3x3 and 1x1x1 convs of every ResidualUnit, conv_out: about

@@ -1,4 +1,4 @@
-"""B200-native drop-in for the reference ``VideoTokenizer`` inference path.
+"""H100-native drop-in for the reference ``VideoTokenizer`` inference path.
 
 Mirrors the reference class's public surface (magvit2_pytorch/magvit2_pytorch.py:1045-1720 =
 M:): the keyword-only constructor and ``layers=(...)`` spec (M:1047-1092, M:1138-1318),
@@ -7,9 +7,9 @@ M:): the keyword-only constructor and ``layers=(...)`` spec (M:1047-1092, M:1138
 ``state_dict`` key layout (SURVEY.md 8b), ``save`` / ``load`` / ``init_and_load_from``
 (M:1447-1458, M:1495-1520), ``copy_for_eval`` (M:1476), ``device`` (M:1443).
 
-All arithmetic runs in hand-written sm_100a kernels behind the C ABI of libmagvit2_b200.so;
+All arithmetic runs in hand-written sm_90a kernels behind the C ABI of libmagvit2_b200.so;
 the compute dtype follows the parameters' dtype (``.float()`` -> fp32 CUDA-core path,
-``.bfloat16()`` -> bf16 tcgen05 path).  There is no CPU / eager fallback.
+``.bfloat16()`` -> bf16 wgmma path).  There is no CPU / eager fallback.
 
 ``cond_residual`` layers (ResidualUnitMod / Conv3DMod, M:680-753, M:946-988) run on the device through the
 factorisation in include/magvit2_b200.h; the other ``cond_*`` types raise in the reference itself.

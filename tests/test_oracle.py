@@ -160,7 +160,7 @@ def test_restated_separate_first_frame_encoding_matches_reference_golden():
 
 
 def test_modulated_conv_factorises_into_shared_weight_conv():
-    """The mapping the B200 path will use for Conv3DMod (M:736-751): per-clip weights w * (cond + 1) * inv_norm never need
+    """The mapping the GPU path uses for Conv3DMod (M:736-751): per-clip weights w * (cond + 1) * inv_norm never need
     to be materialised --  y[b, o] = inv_norm[b, o] * conv(x[b] * (cond[b] + 1), w)[o]  with
     inv_norm[b, o] = rsqrt(max(sum_i (cond[b, i] + 1)^2 * S[o, i], eps)),  S[o, i] = sum_taps w[o, i, :]^2 --
     i.e. the shared-weight causal conv with a per-(clip, channel) input scale and a per-(clip, channel) output scale."""

@@ -1,4 +1,4 @@
-"""Host-side launch planning of the tcgen05 slab conv (tiling rule + static tile schedule), through the C ABI without a
+"""Host-side launch planning of the wgmma slab conv (tiling rule + static tile schedule), through the C ABI without a
 GPU: mv2_tc_slab_plan / mv2_tc_slab_tile run the same code mv2_tc_slab_forward and the kernel use."""
 import ctypes as C
 
@@ -6,7 +6,7 @@ import pytest
 
 from magvit2_pytorch_b200 import _lib
 
-N_SM = 148
+N_SM = 132
 
 
 def _args(B, T, H, W, Ci, Co, k=(3, 3, 3), epi_mode=0, shuffle=0):
@@ -26,7 +26,7 @@ def _args(B, T, H, W, Ci, Co, k=(3, 3, 3), epi_mode=0, shuffle=0):
 def _plan(lib, a, n_sm=N_SM):
     out = (C.c_int32 * 6)()
     assert lib.mv2_tc_slab_plan(C.byref(a), n_sm, out) == 0, lib.mv2_last_error()
-    return dict(zip(("mw", "bn", "n_tiles_n", "total", "grid", "nbuf"), out))
+    return dict(zip(("mw", "bn", "n_tiles_n", "total", "grid", "slab_stages"), out))
 
 
 def _tiles_of(lib, a, cta, n_sm=N_SM):
@@ -50,9 +50,9 @@ def test_plan_is_well_formed(shape):
     lib = _lib.load()
     B, T, H, W, Ci, Co = shape
     p = _plan(lib, _args(*shape))
-    assert p["mw"] in (1, 2, 4) and p["bn"] % 16 == 0 and 32 <= p["bn"] <= 256
-    assert p["mw"] * p["bn"] <= 512                                   # both M-tile accumulators fit TMEM
-    assert p["nbuf"] == (2 if 2 * p["mw"] * p["bn"] <= 512 else 1)
+    assert p["mw"] in (1, 2, 4) and p["bn"] in (32, 64, 128)
+    assert p["mw"] * p["bn"] <= 128                                   # the M-tile accumulators fit 64 registers per thread
+    assert p["slab_stages"] in (2, 3)                               # the ring fits next to the staging at least double-buffered
     assert p["n_tiles_n"] * p["bn"] >= Co > (p["n_tiles_n"] - 1) * p["bn"]   # N tiles cover Co, last one may be ragged
     tiles_per_frame = -(-H // 16) * -(-W // (8 * p["mw"])) * p["n_tiles_n"]
     assert p["total"] == B * T * tiles_per_frame
@@ -62,16 +62,15 @@ def test_plan_is_well_formed(shape):
 def test_tiling_rule_on_readme_layers():
     lib = _lib.load()
     got = [(_plan(lib, _args(*s))["mw"], _plan(lib, _args(*s))["bn"]) for s in README_CONV3]
-    # narrow layers share each weight tile between 4 / 2 M-tiles; Co >= 256 takes the widest MMA
-    assert got[:3] == [(4, 64), (2, 128), (1, 256)]
-    assert got[3] == (1, 256) and got[4] == (1, 256)
-    assert got[5][0] == 1 and got[5][1] in (128, 176, 256)            # 80 tiles for 148 CTAs: the makespan model may narrow N
-    # GEGLU feed-forward: 2 * 1408 packed columns -> 11 tiles of 256
+    # narrow layers share each weight tile between 2 M-tiles; Co >= 128 takes the widest MMA
+    assert got[:3] == [(2, 64), (1, 128), (1, 128)]
+    assert got[3:] == [(1, 128)] * 3
+    # GEGLU feed-forward: 2 * 1408 packed columns -> 22 tiles of 128
     ff = _plan(lib, _args(4, 20, 16, 16, 512, 2816, k=(1, 1, 1), epi_mode=1))
-    assert (ff["mw"], ff["bn"], ff["n_tiles_n"]) == (1, 256, 11)
+    assert (ff["mw"], ff["bn"], ff["n_tiles_n"]) == (1, 128, 22)
     # a width with no large power-of-two divisor takes wide tiles with a ragged last one instead of 64-column tiles
     odd = _plan(lib, _args(4, 20, 16, 16, 512, 2752, k=(1, 1, 1), epi_mode=1))
-    assert odd["bn"] == 256 and odd["n_tiles_n"] == 11
+    assert odd["bn"] == 128 and odd["n_tiles_n"] == 22
 
 
 @pytest.mark.parametrize("shape", [(4, 20, 16, 16, 512, 512), (4, 10, 16, 16, 512, 512), (4, 5, 16, 16, 512, 512),
@@ -96,12 +95,12 @@ def test_schedule_visits_every_tile_exactly_once(shape):
 
 
 def test_schedule_is_longest_first_and_balanced():
-    """C = 512, T = 20: 320 tiles on 148 CTAs.  Frames t = 0 / 1 see 1 / 2 of the 3 frame taps; the static schedule must
-    start every CTA on full-cost tiles and leave no CTA with three full tiles (the plain round robin did)."""
+    """C = 512, T = 20: 640 tiles on 132 CTAs.  Frames t = 0 / 1 see 1 / 2 of the 3 frame taps; the static schedule must
+    start every CTA on full-cost tiles and run the cheap tiles in the last, partial wave."""
     lib = _lib.load()
     a = _args(4, 20, 16, 16, 512, 512)
     p = _plan(lib, a)
-    assert (p["total"], p["grid"]) == (320, 148)
+    assert (p["total"], p["grid"]) == (640, 132)
     cost = lambda t: 3 - max(0, 2 - t)
     loads = []
     for cta in range(p["grid"]):
@@ -110,9 +109,9 @@ def test_schedule_is_longest_first_and_balanced():
         assert costs == sorted(costs, reverse=True)                   # each CTA runs its expensive tiles first
         assert costs[0] == 3
         loads.append(sum(costs))
-    total = 4 * (18 * 3 + 2 + 1) * 4                                  # clips * per-clip frame cost * tiles per frame
+    total = 4 * (18 * 3 + 2 + 1) * 8                                  # clips * per-clip frame cost * tiles per frame
     assert sum(loads) == total
-    assert max(loads) == 7                                            # 2 full tiles + at most one third-cost remainder
+    assert max(loads) == 15                                           # 576 full tiles: no CTA runs more than 5 of them
     assert max(loads) <= -(-total // p["grid"]) + 2
 
 

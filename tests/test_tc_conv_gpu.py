@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM convolution, shape by shape, through the engine's conv() entry (C ABI underneath), against
+"""wgmma implicit-GEMM convolution, shape by shape, through the engine's conv() entry (C ABI underneath), against
 (a) the CPU oracle's building blocks (oracle/restated.py: plain torch fp32 functional ops on the same bf16-representable
 inputs and weights) and (b) the library's own CUDA-core kernel on identical bf16 inputs (both accumulate in fp32)."""
 import pytest
@@ -116,7 +116,7 @@ def test_tc_matches_cuda_core(case):
     eng.tc_calls = 0
     eng.tc_variant = "tap"
     y_tc = run(True)
-    assert eng.tc_calls == 1, "tcgen05 path was not taken"
+    assert eng.tc_calls == 1, "wgmma path was not taken"
     y_ref = run(False)
     torch.cuda.synchronize()
     res_o = None
@@ -191,7 +191,7 @@ def test_slab_matches_cuda_core(case):
 
 @pytest.mark.parametrize("C_,tshift", [(256, False), (512, True), (64, False)])
 def test_fused_geglu_feed_forward_matches_cuda_core(C_, tshift):
-    """fc1 + GEGLU fused in the tcgen05 epilogue (hidden width padded to 64) + fc2 vs the unfused CUDA-core path."""
+    """fc1 + GEGLU fused in the wgmma epilogue (hidden width padded to 64) + fc2 vs the unfused CUDA-core path."""
     from magvit2_pytorch_b200.engine import pack_ff
     assert torch.cuda.is_available()
     g = torch.Generator(device="cpu").manual_seed(C_)
@@ -219,7 +219,7 @@ def test_fused_geglu_feed_forward_matches_cuda_core(C_, tshift):
 
 @pytest.mark.parametrize("variant", ["tap", "slab"])
 def test_conv_in_kwpack_matches_cuda_core(variant):
-    """conv_in (7x7x7, C_in=3) through mv2_ingest_kwpack + tcgen05 (49 taps x 32 packed channels) vs the CUDA-core conv."""
+    """conv_in (7x7x7, C_in=3) through mv2_ingest_kwpack + wgmma (49 taps x 32 packed channels) vs the CUDA-core conv."""
     assert torch.cuda.is_available()
     m = VideoTokenizer(image_size=32, init_dim=64, codebook_size=1024, layers=("residual",)).cuda().bfloat16()
     eng = m.engine
@@ -348,7 +348,7 @@ def _ru_pack(C_, g):
 
 @pytest.mark.parametrize("case", RU_CASES, ids=[c[0] for c in RU_CASES])
 def test_fused_residual_unit(case):
-    """mv2_tc_ru_forward (conv3x3x3 + ELU + conv1x1x1 + ELU + SE pool records in one tcgen05 launch) + gate + residual
+    """mv2_tc_ru_forward (conv3x3x3 + ELU + conv1x1x1 + ELU + SE pool records in one wgmma launch) + gate + residual
     against (a) the unfused kernels on identical inputs and (b) the CPU oracle's residual_unit (M:930-944)."""
     assert torch.cuda.is_available()
     name, C_, (B, T, H, W) = case

@@ -69,19 +69,25 @@ def test_own_dgrad_kernels_agree_with_the_library_dgrad():
     g = load_golden("mini_train")
     video = golden_video(g).cuda()
     grads = []
-    for own in (True, False):
-        model = build_product(g["kwargs"], g["wseed"]).cuda()
-        orig = T.TrainRunner.__init__
+    # the library side in true fp32: TF32 convolutions (cuDNN's default on this GPU) would round far above fp32 round-off
+    tf32 = torch.backends.cudnn.allow_tf32
+    torch.backends.cudnn.allow_tf32 = False
+    try:
+        for own in (True, False):
+            model = build_product(g["kwargs"], g["wseed"]).cuda()
+            orig = T.TrainRunner.__init__
 
-        def patched(self, m, _own=own, _orig=orig):
-            _orig(self, m)
-            self.own_dgrad = _own
-        T.TrainRunner.__init__ = patched
-        try:
-            _train_step(model, video)
-        finally:
-            T.TrainRunner.__init__ = orig
-        grads.append({k: p.grad.clone() for k, p in model.named_parameters() if p.grad is not None})
+            def patched(self, m, _own=own, _orig=orig):
+                _orig(self, m)
+                self.own_dgrad = _own
+            T.TrainRunner.__init__ = patched
+            try:
+                _train_step(model, video)
+            finally:
+                T.TrainRunner.__init__ = orig
+            grads.append({k: p.grad.clone() for k, p in model.named_parameters() if p.grad is not None})
+    finally:
+        torch.backends.cudnn.allow_tf32 = tf32
     worst = 0.0
     gnorm = sum(float(b.double().pow(2).sum()) for b in grads[1].values()) ** 0.5
     for k, a in grads[0].items():
@@ -120,7 +126,7 @@ def test_optimizer_step_changes_the_loss_and_repacks_the_weights():
 
 
 def test_bf16_gradients_agree_with_fp32():
-    """bf16 training path (tcgen05 forward, cuDNN bf16 backward) against the fp32 path on the reconstruction loss.  (With the LFQ
+    """bf16 training path (wgmma forward, cuDNN bf16 backward) against the fp32 path on the reconstruction loss.  (With the LFQ
     auxiliary loss the comparison is meaningless: its logits are 200 x the pre-sign values, so bf16 round-off of the encoder
     output changes the code probabilities by O(1) -- in the reference's own bf16 run as well.)"""
     _require_cuda()
