@@ -36,7 +36,8 @@ extern "C" {
 
 enum { MV2_F32 = 0, MV2_BF16 = 1,
        MV2_U8 = 2   /* source dtype of the two layout-in entry points only: decoded uint8 frames, normalised x / 255 */ };
-enum { MV2_ACT_NONE = 0, MV2_ACT_ELU = 1, MV2_ACT_SILU = 2 };
+enum { MV2_ACT_NONE = 0, MV2_ACT_ELU = 1, MV2_ACT_SILU = 2,
+       MV2_ACT_LEAKY_RELU = 3   /* LeakyReLU(0.1), the discriminator's activation (M:117-118) */ };
 enum { MV2_SHUFFLE_NONE = 0, MV2_SHUFFLE_SPACE = 1, MV2_SHUFFLE_TIME = 2 };
 enum {
   MV2_OK = 0,
@@ -247,7 +248,9 @@ typedef struct mv2_tc_conv_args {
   int32_t act;
   int32_t shuffle;
   int32_t epi_mode;    /* 0 plain; 1 fused GEGLU (M:466-469): packed columns come in groups of 16 = 8 x-columns then
-                          their 8 gate-columns, output has Co/2 channels: y = gelu_erf(gate) * x */
+                          their 8 gate-columns, output has Co/2 channels: y = gelu_erf(gate) * x;
+                          2 scaled residual (needs res, no shuffle): y = (act(acc + bias) + res) * 2^-0.5, the
+                          DiscriminatorBlock output (M:585), rounded to bf16 once */
   const float* oscale; /* as mv2_conv_args.oscale (plain / ragged epilogues only) */
   int32_t out_layout;  /* 0: y is channels-last (B,To,Ho,Wo,Co).  1: y is torch's channels-first (B,Co,To,Ho,Wo) -- the slab
                           kernel's conv_out (Co % 8 != 0) writes the reconstruction directly in the caller's layout; with

@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MV2_LIB_PATH") or os.path.join(_HERE, "libmagvit2_b200.so")   # env override: A/B builds
 
 MV2_F32, MV2_BF16, MV2_U8 = 0, 1, 2
-ACT_NONE, ACT_ELU, ACT_SILU = 0, 1, 2
+ACT_NONE, ACT_ELU, ACT_SILU, ACT_LEAKY_RELU = 0, 1, 2, 3
 SHUFFLE_NONE, SHUFFLE_SPACE, SHUFFLE_TIME = 0, 1, 2
 
 

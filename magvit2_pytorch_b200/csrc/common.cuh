@@ -56,6 +56,7 @@ __device__ __forceinline__ float act_silu(float v) { return v / (1.f + expf(-v))
 __device__ __forceinline__ float apply_act(float v, int act) {
   if (act == MV2_ACT_ELU) return act_elu(v);
   if (act == MV2_ACT_SILU) return act_silu(v);
+  if (act == MV2_ACT_LEAKY_RELU) return v > 0.f ? v : 0.1f * v;
   return v;
 }
 

@@ -135,7 +135,8 @@ struct TcEpi {
   const float* bias;             // global, packed column order (only used to decide has-bias; values come from smem)
   const __nv_bfloat16* res;
   __nv_bfloat16* y;
-  int act, shuffle, mode;        // mode 0 plain; 1 GEGLU: packed cols [16g, 16g+8) = x, [16g+8, 16g+16) = gate (M:466-469)
+  int act, shuffle, mode;        // mode 0 plain; 1 GEGLU: packed cols [16g, 16g+8) = x, [16g+8, 16g+16) = gate (M:466-469);
+                                 // 2 scaled residual: (act(acc + bias) + res) * 2^-0.5 (DiscriminatorBlock, M:585)
   int Co;                        // packed GEMM output columns
   int To, Ho, Wo;                // output volume before any depth-to-space/time shuffle
   int out_cf;                    // 1: y is channels-first (B, Co, To, Ho, Wo) -- EPI_RAGGED scalar stores only (conv_out)
@@ -216,6 +217,7 @@ __device__ __forceinline__ float act_ct(float x) {
     return x > 0.f ? x : e;
   }
   if (ACT == MV2_ACT_SILU) return x * rcp_approx(1.f + ex2_approx(-1.4426950408889634f * x));
+  if (ACT == MV2_ACT_LEAKY_RELU) return x > 0.f ? x : 0.1f * x;
   return x;
 }
 
@@ -274,6 +276,7 @@ __device__ __forceinline__ void epi_chunk32_t(const TcEpi& e, const uint32_t (&r
     } else {
       off = row_base + ng;
     }
+    const float rscale = e.mode == 2 ? 0.70710678118654752440f : 1.f;
     if (vec_ok && ng + 8 <= e.Co) {
       if (e.res) {
         const uint4 rv = *reinterpret_cast<const uint4*>(e.res + off);
@@ -281,8 +284,8 @@ __device__ __forceinline__ void epi_chunk32_t(const TcEpi& e, const uint32_t (&r
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const float2 f = __bfloat1622float2(rb[q]);
-          v[2 * q] += f.x;
-          v[2 * q + 1] += f.y;
+          v[2 * q] = (v[2 * q] + f.x) * rscale;
+          v[2 * q + 1] = (v[2 * q + 1] + f.y) * rscale;
         }
       }
       store8_bf16(e.y + off, v);
@@ -294,7 +297,7 @@ __device__ __forceinline__ void epi_chunk32_t(const TcEpi& e, const uint32_t (&r
       } else
       for (int q = 0; q < 8 && ng + q < e.Co; ++q) {   // scalar tail (Co % 8 != 0, e.g. conv_out's 3 channels)
         float x = v[q];
-        if (e.res) x += __bfloat162float(e.res[off + q]);
+        if (e.res) x = (x + __bfloat162float(e.res[off + q])) * rscale;
         e.y[off + q] = __float2bfloat16_rn(x);
       }
     }
@@ -342,11 +345,13 @@ __device__ __forceinline__ void epi_act32_t(uint32_t (&r)[32], const float* sb) 
 __device__ __forceinline__ void epi_act32(int act, uint32_t (&r)[32], const float* sb) {
   if (act == MV2_ACT_ELU) epi_act32_t<MV2_ACT_ELU>(r, sb);
   else if (act == MV2_ACT_SILU) epi_act32_t<MV2_ACT_SILU>(r, sb);
+  else if (act == MV2_ACT_LEAKY_RELU) epi_act32_t<MV2_ACT_LEAKY_RELU>(r, sb);
   else epi_act32_t<MV2_ACT_NONE>(r, sb);
 }
 __device__ __forceinline__ void epi_pack32(int act, const uint32_t (&r)[32], const float* sb, uint32_t (&pk)[16]) {
   if (act == MV2_ACT_ELU) epi_pack32_t<MV2_ACT_ELU>(r, sb, pk);
   else if (act == MV2_ACT_SILU) epi_pack32_t<MV2_ACT_SILU>(r, sb, pk);
+  else if (act == MV2_ACT_LEAKY_RELU) epi_pack32_t<MV2_ACT_LEAKY_RELU>(r, sb, pk);
   else epi_pack32_t<MV2_ACT_NONE>(r, sb, pk);
 }
 
@@ -357,6 +362,7 @@ __device__ __forceinline__ void epi_chunk32(const TcEpi& e, const uint32_t (&r)[
   if (MODE == EPI_GEGLU) { epi_chunk32_t<EPI_GEGLU, MV2_ACT_NONE>(e, r, ncols, n, sb, b, to, ho, wo, row_base); return; }
   if (e.act == MV2_ACT_ELU) epi_chunk32_t<MODE, MV2_ACT_ELU>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
   else if (e.act == MV2_ACT_SILU) epi_chunk32_t<MODE, MV2_ACT_SILU>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
+  else if (e.act == MV2_ACT_LEAKY_RELU) epi_chunk32_t<MODE, MV2_ACT_LEAKY_RELU>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
   else epi_chunk32_t<MODE, MV2_ACT_NONE>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
 }
 

@@ -168,7 +168,8 @@ int mv2_tc_conv_supported(const mv2_tc_conv_args* a) {
   if (a->shuffle != MV2_SHUFFLE_NONE && ((a->shuffle == MV2_SHUFFLE_SPACE ? a->Co / 4 : a->Co / 2) % 8 != 0)) return 0;
   if (a->res && a->Co % 8 != 0) return 0;
   if (a->epi_mode == 1 && (a->Co % 32 != 0 || a->shuffle != MV2_SHUFFLE_NONE || a->res)) return 0;   // GEGLU pairs
-  if (a->epi_mode != 0 && a->epi_mode != 1) return 0;
+  if (a->epi_mode == 2 && (!a->res || a->shuffle != MV2_SHUFFLE_NONE)) return 0;   // scaled residual
+  if (a->epi_mode < 0 || a->epi_mode > 2) return 0;
   if (a->out_layout != 0) return 0;
   if (a->oscale && (a->epi_mode != 0 || a->shuffle != MV2_SHUFFLE_NONE)) return 0;
   return 1;

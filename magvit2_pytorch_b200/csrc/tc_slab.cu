@@ -534,13 +534,14 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
             }
             if (MODE == EPI_PLAIN_RES) {
               epi_act32(p.epi.act, r, sbias + c.n0 + c0);
+              const float rs = p.epi.mode == 2 ? 0.70710678118654752440f : 1.f;     // scaled residual (DiscriminatorBlock, M:585)
 #pragma unroll
               for (int g = 0; g < 4; ++g) {
                 const uint32_t w4[4] = {rv[g].x, rv[g].y, rv[g].z, rv[g].w};
 #pragma unroll
                 for (int q = 0; q < 4; ++q)
-                  pk[4 * g + q] = pack_bf16x2(__uint_as_float(r[8 * g + 2 * q]) + __uint_as_float(w4[q] << 16),
-                                              __uint_as_float(r[8 * g + 2 * q + 1]) + __uint_as_float(w4[q] & 0xffff0000u));
+                  pk[4 * g + q] = pack_bf16x2((__uint_as_float(r[8 * g + 2 * q]) + __uint_as_float(w4[q] << 16)) * rs,
+                                              (__uint_as_float(r[8 * g + 2 * q + 1]) + __uint_as_float(w4[q] & 0xffff0000u)) * rs);
               }
             } else
             epi_pack32(p.epi.act, r, sbias + c.n0 + c0, pk);
@@ -665,7 +666,8 @@ extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
   if (a->Ci % 32 != 0 || a->Co > 4096) return 0;
   if (a->oscale && (a->epi_mode != 0 || a->shuffle != MV2_SHUFFLE_NONE)) return 0;   // demodulation: plain / ragged epilogues only
   if (a->epi_mode == 1 && (a->Co % 64 != 0 || a->shuffle != MV2_SHUFFLE_NONE || a->res)) return 0;   // fused GEGLU (64-column epilogue chunks)
-  if (a->epi_mode != 0 && a->epi_mode != 1) return 0;
+  if (a->epi_mode == 2 && (!a->res || a->shuffle != MV2_SHUFFLE_NONE)) return 0;   // scaled residual
+  if (a->epi_mode < 0 || a->epi_mode > 2) return 0;
   if (a->Co % 32 != 0 && a->Co > 32) return 0;           // ragged N only as a single (zero padded) 32-column tile
   if (a->Ci % 64 != 0 && a->kw != 1) return 0;           // 64-byte rows (32 channels): only h-shifted taps (1024 B multiples)
   if (a->res && a->Co % 8 != 0) return 0;

@@ -48,7 +48,7 @@ class ConvPack:
     bias_tc: Optional[torch.Tensor] = None   # bias in w_tc's row order
     Ci_tc: int = 0                           # GEMM dims of the wgmma call (may be padded / re-paired)
     Co_tc: int = 0
-    epi_mode: int = 0                        # 1: fused GEGLU (output has Co_tc // 2 channels)
+    epi_mode: int = 0                        # 1: fused GEGLU (output has Co_tc // 2 channels); 2: (act(conv) + res) * 2^-0.5
     k_tc: Optional[Tuple[int, int, int]] = None
     macs: int = 0                            # algorithmic multiply-accumulates per output position (Co * Ci * taps, unpadded)
     w_down: Optional[torch.Tensor] = None    # SpatialDownsample2x pack for mv2_tc_down_space_forward ([Co][6][2*Ci] bf16)
@@ -125,6 +125,21 @@ def pack_ff(fc1_w, fc1_b, fc2_w, fc2_b, dtype):
         fc2.w_tc = w2p.contiguous().to(torch.bfloat16)
         fc2.Ci_tc, fc2.Co_tc = Ip, int(w2.shape[0])
     return fc1, fc2
+
+
+def pack_linear_attention(la, dt):
+    """LinearSpaceAttention (M:390-442) for Engine.linear_attention."""
+    return dict(gamma=la.norm.gamma.detach().float().contiguous(),
+                q=pack_conv(la.attn.to_q[0].weight[:, :, None, None, None], None, dt),
+                kv=pack_conv(la.attn.to_kv[0].weight[:, :, None, None, None], None, dt),
+                out=pack_conv(la.attn.to_out[0].weight[:, :, None, None, None], None, dt),
+                heads=la.heads, dim_head=la.dim_head)
+
+
+def pack_feed_forward(ff, dt):
+    """FeedForward (M:471-496) for Engine.feed_forward."""
+    fc1, fc2 = pack_ff(ff.net[0].weight, ff.net[0].bias, ff.net[2].weight, ff.net[2].bias, dt)
+    return dict(gamma=ff.norm.gamma.detach().float().reshape(-1).contiguous(), fc1=fc1, fc2=fc2, inner=ff.dim_inner)
 
 
 def pack_conv_in_kwpack(weight, bias, cpack=32):
@@ -222,8 +237,7 @@ class Engine:
                 P[key]["w2b"] = P[key]["w2"].to(torch.bfloat16).contiguous()
 
         def pack_ffn(ff, key):
-            fc1, fc2 = pack_ff(ff.net[0].weight, ff.net[0].bias, ff.net[2].weight, ff.net[2].bias, dt)
-            P[key] = dict(gamma=f32(ff.norm.gamma.reshape(-1)), fc1=fc1, fc2=fc2, inner=ff.dim_inner)
+            P[key] = pack_feed_forward(ff, dt)
 
         def pack_attn(at, key):
             P[key] = dict(gamma=f32(at.norm.gamma), qkv=pack_conv(at.to_qkv[0].weight[:, :, None, None, None], None, dt),
@@ -232,11 +246,7 @@ class Engine:
                           heads=at.heads, dim_head=at.dim_head, n_mem=int(at.mem_kv.shape[2]))
 
         def pack_lin(la, key):
-            P[key] = dict(gamma=f32(la.norm.gamma),
-                          q=pack_conv(la.attn.to_q[0].weight[:, :, None, None, None], None, dt),
-                          kv=pack_conv(la.attn.to_kv[0].weight[:, :, None, None, None], None, dt),
-                          out=pack_conv(la.attn.to_out[0].weight[:, :, None, None, None], None, dt),
-                          heads=la.heads, dim_head=la.dim_head)
+            P[key] = pack_linear_attention(la, dt)
 
         for side, layers in (("enc", m.encoder_layers), ("dec", m.decoder_layers)):
             stages = m.stages if side == "enc" else list(reversed(m.stages))
@@ -352,12 +362,13 @@ class Engine:
                                        "slab" if use_slab else "tap", pk.k[1] * pk.k[2] * pk.k[0]))
                 if self.conv_log is not None:
                     self.conv_log.append(dict(kind="slab" if use_slab else "tap", Ci=Ci, Co=co_out, k=tuple(pk.k), out=(B, To, Ho, Wo),
-                                              geglu=pk.epi_mode == 1, shuffle=shuffle, res=res is not None))
+                                              geglu=pk.epi_mode == 1, shuffle=shuffle, res=res is not None, act=act,
+                                              epi_mode=pk.epi_mode, stride=tuple(stride)))
                 self.launches += 1
                 self.tc_calls += 1
                 return y
             assert not out_cf, "channels-first output is a wgmma slab-kernel feature"
-            assert pk.w is not None and pk.epi_mode == 0 and Ci == pk.Ci, "wgmma-only weight pack has no CUDA-core fallback"
+            assert pk.w is not None and pk.epi_mode in (0, 2) and Ci == pk.Ci, "wgmma-only weight pack has no CUDA-core fallback"
             kt, kh, kw = pk.k
         assert Ci == pk.Ci, (Ci, pk.Ci)
         assert pk.w is not None and not out_cf
@@ -377,6 +388,12 @@ class Engine:
                      oscale=_ptr(oscale))
         check(self.lib.mv2_conv_forward(C.byref(a), self._stream()), "mv2_conv_forward")
         self.launches += 1
+        if pk.epi_mode == 2:          # scaled residual: the residual epilogue, then * 2^-0.5 (the reference's add-then-multiply)
+            assert res is not None and shuffle == SHUFFLE_NONE
+            scale = torch.full((B, pk.Co), 2 ** -0.5, device=self.device, dtype=torch.float32)
+            check(self.lib.mv2_scale_channels(_ptr(y), _ptr(scale), _ptr(y), _dt(self.dtype), B, To * Ho * Wo, pk.Co, self._stream()),
+                  "mv2_scale_channels")
+            self.launches += 1
         return y
 
     def residual_unit(self, x, p):

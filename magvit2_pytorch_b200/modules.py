@@ -154,12 +154,12 @@ class TimeUpsample2x(_NoForward):
 
 
 class RMSNorm(_NoForward):
-    """M:258-273: gamma is (C,) channel-last or (C,1,1,1) channel-first."""
+    """M:258-273: gamma is (C,) channel-last or (C,1,1,1) channel-first ((C,1,1) for images)."""
 
-    def __init__(self, dim, channel_first=False):
+    def __init__(self, dim, channel_first=False, images=False):
         super().__init__()
         self.channel_first = channel_first
-        self.gamma = nn.Parameter(torch.ones((dim, 1, 1, 1) if channel_first else (dim,)))
+        self.gamma = nn.Parameter(torch.ones(((dim, 1, 1) if images else (dim, 1, 1, 1)) if channel_first else (dim,)))
 
 
 class Attention(_NoForward):
@@ -216,14 +216,71 @@ class ToTimeSequence(_NoForward):
 
 
 class FeedForward(_NoForward):
-    """M:471-496: channel-first RMSNorm, Conv3d C->2I 1x1x1, GEGLU, Conv3d I->C; I = int(C*4*2/3)."""
+    """M:471-496: channel-first RMSNorm, Conv3d C->2I 1x1x1, GEGLU, Conv3d I->C; I = int(C*4*2/3).
+    images=True (the discriminator's blocks): Conv2d and a (C, 1, 1) gamma."""
 
-    def __init__(self, dim, mult=4):
+    def __init__(self, dim, mult=4, images=False):
         super().__init__()
         inner = int(dim * mult * 2 / 3)
         self.dim, self.dim_inner = dim, inner
-        self.norm = RMSNorm(dim, channel_first=True)
-        self.net = nn.Sequential(nn.Conv3d(dim, inner * 2, 1), Marker("GEGLU"), nn.Conv3d(inner, dim, 1))
+        self.norm = RMSNorm(dim, channel_first=True, images=images)
+        conv = nn.Conv2d if images else nn.Conv3d
+        self.net = nn.Sequential(conv(dim, inner * 2, 1), Marker("GEGLU"), conv(inner, dim, 1))
+
+
+class DiscriminatorBlock(_NoForward):
+    """M:549-586 (antialiased_downsample=False): conv_res 1x1 (stride 2 when downsampling), net = 3x3 conv, LeakyReLU,
+    3x3 conv, LeakyReLU, downsample = pixel-unshuffle + 1x1 conv; output (downsample(net(x)) + conv_res(x)) * 2^-0.5."""
+
+    def __init__(self, input_channels, filters, downsample=True):
+        super().__init__()
+        self.conv_res = nn.Conv2d(input_channels, filters, 1, stride=(2 if downsample else 1))
+        self.net = nn.Sequential(nn.Conv2d(input_channels, filters, 3, padding=1), Marker("LeakyReLU(0.1)"),
+                                 nn.Conv2d(filters, filters, 3, padding=1), Marker("LeakyReLU(0.1)"))
+        self.downsample = nn.Sequential(Marker("'b c (h p1) (w p2) -> b (c p1 p2) h w'"),
+                                        nn.Conv2d(filters * 4, filters, 1)) if downsample else None
+
+
+class Discriminator(_NoForward):
+    """M:588-675: the image discriminator of the GAN loss.  Parameters only -- ``VideoTokenizer.discr`` runs it on the
+    device (gan.py).  Blur (antialiased_downsample) needs kornia's filter3d and is not supported; the linear attention
+    kernel takes dim_head 8 only."""
+
+    def __init__(self, *, dim, image_size, channels=3, max_dim=512, attn_heads=8, attn_dim_head=32, linear_attn_dim_head=8,
+                 linear_attn_heads=16, ff_mult=4, antialiased_downsample=False):
+        super().__init__()
+        if antialiased_downsample:
+            raise NotImplementedError("Discriminator(antialiased_downsample=True): Blur needs kornia's filter3d, which is "
+                                      "not supported")
+        if linear_attn_dim_head != 8:
+            raise NotImplementedError("Discriminator: the linear attention kernel takes linear_attn_dim_head = 8 only")
+        hw = tuple(image_size) if isinstance(image_size, (tuple, list)) else (image_size, image_size)
+        num_layers = int(math.log2(min(hw)) - 2)
+        layer_dims = [channels] + [(dim * 4) * (2 ** i) for i in range(num_layers + 1)]
+        layer_dims = [min(d, max_dim) for d in layer_dims]
+        dims_in_out = list(zip(layer_dims[:-1], layer_dims[1:]))
+        self.image_size, self.channels = hw, channels
+        self.blocks = nn.ModuleList([])
+        for ind, (cin, cout) in enumerate(dims_in_out):
+            block = DiscriminatorBlock(cin, cout, downsample=ind != len(dims_in_out) - 1)
+            attn = nn.Sequential(Residual(LinearSpaceAttention(cout, linear_attn_dim_head, linear_attn_heads)),
+                                 Residual(FeedForward(cout, mult=ff_mult, images=True)))
+            self.blocks.append(nn.ModuleList([block, attn]))
+        dim_last = layer_dims[-1]
+        self.last_fmap = tuple(n // 2 ** num_layers for n in hw)
+        latent = self.last_fmap[0] * self.last_fmap[1] * dim_last
+        self.to_logits = nn.Sequential(nn.Conv2d(dim_last, dim_last, 3, padding=1), Marker("LeakyReLU(0.1)"),
+                                       Marker("'b ... -> b (...)'"), nn.Linear(latent, 1), Marker("'b 1 -> b'"))
+        self._pack = None         # (parameter signature, engine, weight packs) of the device path (gan.py)
+
+    def __getstate__(self):       # the packs and the engine belong to this instance: copies and pickles re-pack on first use
+        st = dict(self.__dict__)
+        st["_pack"] = None
+        return st
+
+    def forward(self, images):
+        from .gan import discriminator_forward
+        return discriminator_forward(self, images)
 
 
 class LFQ(_NoForward):

@@ -17,8 +17,11 @@ factorisation in include/magvit2_b200.h; the other ``cond_*`` types raise in the
 ``forward(return_loss=True)`` (reconstruction + quantiser auxiliary loss; models built with ``use_gan=False,
 perceptual_loss_weight=0``) runs on the device; in ``model.train()`` with gradients enabled it returns a loss with a
 ``grad_fn`` (train.py: forward by the same kernels, backward by library code).
-Out of scope (raise at construction / call; SURVEY.md 8f): the
-GAN / perceptual training losses (``return_discr_loss``, ``return_loss`` with a discriminator or VGG).
+Models without a perceptual (VGG) term that use the GAN (``use_gan=True, adversarial_loss_weight > 0``) build the image
+discriminator ``discr`` (M:1415-1422) and run it on the device (gan.py): ``return_discr_loss`` (M:1731-1786) and the
+adversarial generator term of ``return_loss`` (M:1826-1843).
+Out of scope (raise at construction / call; SURVEY.md 8f): the perceptual (VGG) loss and adaptive weighting, multiscale
+discriminators, and the discriminator's antialiased (Blur) downsampling.
 """
 from __future__ import annotations
 
@@ -32,6 +35,7 @@ from pathlib import Path
 from typing import List, Optional, Tuple
 
 import torch
+import torch.nn.functional as F
 from torch import nn
 
 from . import modules as M
@@ -251,12 +255,18 @@ class VideoTokenizer(nn.Module):
         self.quantizer_aux_loss_weight = quantizer_aux_loss_weight
         self.register_buffer("zero", torch.tensor(0.), persistent=False)
 
-        # training-only branches of the reference are not built (SURVEY.md 2 rows 13-15)
+        # training-only branches of the reference: the VGG and multiscale discriminators are not built (SURVEY.md 2 rows
+        # 13-15); the image discriminator is, for models whose loss has no perceptual term (M:1415-1427, gan.py)
         self.vgg = None
         self.use_vgg = False
         self.perceptual_loss_weight = perceptual_loss_weight
         self.use_gan = use_gan
         self.has_gan = False
+        self.discr = None
+        if use_gan and adversarial_loss_weight > 0. and not self._has_vgg():
+            kw = dict(dim=dim, image_size=image_size, channels=channels, max_dim=512) if discr_kwargs is None else dict(discr_kwargs)
+            self.discr = M.Discriminator(**kw)
+            self.has_gan = True
         self.has_multiscale_gan = False
         self.has_multiscale_discrs = False
         self.multiscale_discrs = nn.ModuleList([])
@@ -291,12 +301,13 @@ class VideoTokenizer(nn.Module):
                 *self.quantizers.parameters()]
 
     def discr_parameters(self):
-        return []
+        return [] if self.discr is None else list(self.discr.parameters())
 
     def load_state_dict(self, state_dict, strict: bool = True, **kw):
-        # reference checkpoints carry discriminator weights (always constructed, M:1422); they are
-        # not part of the inference path and are dropped here.
-        sd = {k: v for k, v in state_dict.items() if not (k.startswith("discr.") or k.startswith("multiscale_discrs."))}
+        # reference checkpoints carry discriminator weights (always constructed, M:1422); a model that built no
+        # discriminator drops them, as it drops the multiscale discriminators'.
+        sd = {k: v for k, v in state_dict.items()
+              if not ((self.discr is None and k.startswith("discr.")) or k.startswith("multiscale_discrs."))}
         return super().load_state_dict(sd, strict=strict, **kw)
 
     def __deepcopy__(self, memo):
@@ -545,15 +556,19 @@ class VideoTokenizer(nn.Module):
         for models without the GAN / perceptual branches (``use_gan=False, perceptual_loss_weight=0``) -- ``return_loss``:
         ``(total_loss, LossBreakdown)`` with ``total_loss = recon_loss + aux_loss * quantizer_aux_loss_weight`` (M:1868-1896)."""
         assert (return_loss + return_codes + return_discr_loss) <= 1               # M:1674
-        if return_discr_loss:
-            raise NotImplementedError("the GAN discriminator losses (reference M:1728-1786) are outside the accelerated path "
-                                      "(SURVEY.md 8f N2)")
+        if return_discr_loss and self.discr is None:
+            raise NotImplementedError("return_discr_loss needs the image discriminator, which is built for use_gan=True, "
+                                      "adversarial_loss_weight > 0 and no perceptual (VGG) term (SURVEY.md 8f N2)")
         if return_loss and self._needs_gan_or_vgg():
             raise NotImplementedError(
-                "return_loss with the GAN / perceptual / adaptive-weighting terms (reference M:1788-1866) is outside the "
-                "accelerated path (SURVEY.md 8f N2): construct with use_gan=False, perceptual_loss_weight=0.")
+                "return_loss with the perceptual / adaptive-weighting terms or multiscale discriminators (reference "
+                "M:1788-1866) is outside the accelerated path (SURVEY.md 8f N2): construct with perceptual_loss_weight=0.")
         video, ff = self._check_video(video_or_images, video_contains_first_frame)
         cond = self._check_cond(cond, video.shape[0])
+        if adversarial_loss_weight is None:                                        # the call-site weight wins (M:1674-1680)
+            adversarial_loss_weight = self.adversarial_loss_weight
+        if return_discr_loss:
+            return self._discr_loss(video, ff, cond, apply_gradient_penalty)
         if return_loss and self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             # the trainer's generator step (T:356-363): loss with a grad_fn.  Forward = the same kernels; backward = train.py
             from .train import train_forward
@@ -563,27 +578,14 @@ class VideoTokenizer(nn.Module):
             self.quantizer_loss_breakdown, self.quantizer_aux_loss = qlb, aux.detach()
             aux_losses = aux.to(recon_loss.dtype)
             total_loss = recon_loss + aux_losses * self.quantizer_aux_loss_weight                # M:1868-1871
-            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, self.zero, self.zero, 0., [], [])
+            gen_loss, adaptive_weight = self._gen_loss(recon)
+            if self.has_gan:
+                total_loss = total_loss + gen_loss * adaptive_weight * adversarial_loss_weight   # M:1872-1875
+            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, self.zero, gen_loss, adaptive_weight, [], [])
         with torch.no_grad():
             eng = self.engine
             need_recon = return_recon or return_recon_loss_only or return_loss or not return_codes
-            aux = None
-
-            def run(v, cd=None):
-                x = eng.encode_cl(v, ff, cd)
-                q, codes_, _ = eng.quantize_cl(x, want_quantized=need_recon)
-                if not need_recon:
-                    return codes_
-                return codes_, eng.decode_cl(q, ff, cd)
-
-            if cond is not None:
-                out = self._graph_call(("fwd_recon_cond" if need_recon else "fwd_codes_cond") + ("" if ff else "_noff"), run,
-                                       video.contiguous(), cond.contiguous())
-            elif self.training and not self.use_fsq:
-                out = self._forward_train_mode(eng, video.contiguous(), need_recon, ff)
-                aux = self.quantizer_aux_loss
-            else:
-                out = self._graph_call(("fwd_recon" if need_recon else "fwd_codes") + ("" if ff else "_noff"), run, video.contiguous())
+            out, aux = self._no_grad_forward(eng, video, ff, cond, need_recon)
             if return_codes and not return_recon:
                 return out                                                         # M:1707-1708
             codes, recon = out
@@ -594,17 +596,82 @@ class VideoTokenizer(nn.Module):
             recon_loss = eng.mse(video, recon).to(self.dtype)                      # M:1722
             if return_recon_loss_only:                                             # M:1726-1727
                 return recon_loss, recon
-            # M:1868-1896 with perceptual_loss = gen_loss = zero, adaptive_weight = 0., no multiscale discriminators
+            # M:1868-1896 with perceptual_loss = zero, no multiscale discriminators; gen_loss = zero, adaptive_weight = 0.
+            # without a discriminator
             zero = self.zero
             aux_losses = zero if aux is None else aux.to(recon_loss.dtype)         # eval mode / FSQ: M:1700-1703
             total_loss = recon_loss + aux_losses * self.quantizer_aux_loss_weight
+            gen_loss, adaptive_weight = self._gen_loss(recon)
+            if self.has_gan:
+                total_loss = total_loss + gen_loss * adaptive_weight * adversarial_loss_weight
             qlb = None if (self.use_fsq or aux is None) else self.quantizer_loss_breakdown
-            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, zero, zero, 0., [], [])
+            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, zero, gen_loss, adaptive_weight, [], [])
+
+    def _no_grad_forward(self, eng, video, ff, cond, need_recon):
+        """The tokenizer forward without gradients -> (codes | (codes, recon), train-mode LFQ aux loss | None)."""
+        aux = None
+
+        def run(v, cd=None):
+            x = eng.encode_cl(v, ff, cd)
+            q, codes_, _ = eng.quantize_cl(x, want_quantized=need_recon)
+            if not need_recon:
+                return codes_
+            return codes_, eng.decode_cl(q, ff, cd)
+
+        if cond is not None:
+            out = self._graph_call(("fwd_recon_cond" if need_recon else "fwd_codes_cond") + ("" if ff else "_noff"), run,
+                                   video.contiguous(), cond.contiguous())
+        elif self.training and not self.use_fsq:
+            out = self._forward_train_mode(eng, video.contiguous(), need_recon, ff)
+            aux = self.quantizer_aux_loss
+        else:
+            out = self._graph_call(("fwd_recon" if need_recon else "fwd_codes") + ("" if ff else "_noff"), run, video.contiguous())
+        return out, aux
+
+    @staticmethod
+    def _pick_frames(video, frame_indices):
+        """pick_video_frame (M:91-98): (B, C, F, H, W), indices (B, 1) -> (B, C, H, W)."""
+        b = torch.arange(video.shape[0], device=video.device)[:, None]
+        return video.transpose(1, 2)[b, frame_indices.to(video.device)][:, 0]
+
+    def _gen_loss(self, recon):
+        """The adversarial generator term (M:1826-1844): -discr(frames).mean() on one random frame per clip, drawn from the
+        default CPU generator as the reference does; (zero, 0.) without a discriminator."""
+        if not self.has_gan:
+            return self.zero, 0.
+        frame_indices = torch.randn((recon.shape[0], recon.shape[2])).topk(1, dim=-1).indices
+        return -self.discr(self._pick_frames(recon, frame_indices)).mean(), 1.
+
+    def _discr_loss(self, video, ff, cond, apply_gradient_penalty):
+        """``return_discr_loss`` (M:1731-1786): the tokenizer runs without gradients (as the no-grad forward, including the
+        train-mode LFQ all-reduce), then the hinge loss of the device discriminator on one real and one reconstructed frame
+        per clip, plus the gradient penalty (gan.gradient_penalty) when asked for."""
+        from .gan import DiscrLossBreakdown, gradient_penalty
+        with torch.no_grad():
+            (_, recon), _ = self._no_grad_forward(self.engine, video, ff, cond, True)
+        frame_indices = torch.randn((video.shape[0], video.shape[2])).topk(1, dim=-1).indices
+        frames = video.float() / 255. if video.dtype == torch.uint8 else video
+        real = self._pick_frames(frames, frame_indices).to(self.dtype).contiguous()
+        fake = self._pick_frames(recon, frame_indices).detach().contiguous()
+        real_logits, fake_logits = self.discr(real), self.discr(fake)
+        discr_loss = (F.relu(1 + fake_logits) + F.relu(1 - real_logits)).mean()           # hinge_discr_loss (M:120-121)
+        if apply_gradient_penalty:
+            gp = gradient_penalty(self.discr, real) + gradient_penalty(self.discr, fake)
+        else:
+            gp = self.zero
+        multiscale = [self.zero]
+        total = discr_loss + gp * self.grad_penalty_loss_weight + sum(multiscale) * self.multiscale_adversarial_loss_weight
+        return total, DiscrLossBreakdown(discr_loss, multiscale, gp)
+
+    def _has_vgg(self) -> bool:
+        """True when the reference constructor would have built a VGG (M:1392)."""
+        return bool(self.channels in {1, 3, 4} and self.perceptual_loss_weight > 0.)
 
     def _needs_gan_or_vgg(self) -> bool:
-        """True when the reference constructor would have built a VGG (M:1392) or discriminators (M:1427, M:1435)."""
-        return bool((self.channels in {1, 3, 4} and self.perceptual_loss_weight > 0.)
-                    or (self.use_gan and self.adversarial_loss_weight > 0.) or self.has_multiscale_discrs)
+        """True when the loss needs a term this package does not build: the VGG (M:1392), multiscale discriminators (M:1435),
+        or the GAN term of a model that built no discriminator (M:1427)."""
+        return bool(self._has_vgg() or (self.use_gan and self.adversarial_loss_weight > 0. and self.discr is None)
+                    or self.has_multiscale_discrs)
 
     @property
     def dtype(self):

@@ -63,6 +63,16 @@ def fill_state_dict_(module, seed: int = 0):
     return module
 
 
+@torch.no_grad()
+def fill_discr_(module, seed: int = 0):
+    """Overwrite every floating-point ``discr.*`` tensor (the GAN's image discriminator) of a tokenizer in place;
+    ``fill_state_dict_`` leaves them alone so that the generator's weights do not depend on whether one is built."""
+    for k, v in module.state_dict().items():
+        if k.startswith("discr.") and v.is_floating_point():
+            v.copy_(synth_tensor(k, v.shape, seed).to(v.dtype))
+    return module
+
+
 def synth_video(batch, channels, frames, size, seed=1234):
     g = torch.Generator(device="cpu")
     g.manual_seed(seed)
