@@ -32,7 +32,9 @@
 extern "C" {
 #endif
 
-#define MV2_ABI_VERSION 3   /* 2: mv2_conv_args.oscale, mv2_tc_conv_args.{oscale,out_layout}; 3: num_codebooks / spherical in the quantiser entry points */
+#define MV2_ABI_VERSION 4   /* 2: mv2_conv_args.oscale, mv2_tc_conv_args.{oscale,out_layout}; 3: num_codebooks / spherical in the quantiser entry points;
+                               4: the two entry points of the one-launch SqueezeExcite tail for small frames are removed: the
+                               engine never enabled it by default, so the separate pool / gate / gate_residual calls are the only SE path */
 
 enum { MV2_F32 = 0, MV2_BF16 = 1,
        MV2_U8 = 2   /* source dtype of the two layout-in entry points only: decoded uint8 frames, normalised x / 255 */ };
@@ -134,13 +136,6 @@ int mv2_se_gate(const void* workspace, int dtype /* of the y passed to mv2_se_po
                 float* gates, void* stream);
 int mv2_gate_residual(const void* y, const void* x, const float* gates, void* out, int dtype,
                       int F, int P, int C, void* stream);
-
-/* SqueezeExcite + residual for small frames in ONE launch (bf16 activations; P * C <= 131072 elements per frame, C and Hd
- * multiples of 8, <= 1024): pool, gate MLP and  out = gate * y + x  (M:221-240 + M:174) by one CTA per frame.  The gate MLP
- * weights are passed as bf16 (w1 [Hd][C], w2 [C][Hd]; exact for a bf16 model); wk / b1 / b2 fp32.                          */
-int mv2_se_tail_supported(int F, int P, int C, int Hd);
-int mv2_se_tail(const void* y, const void* x, void* out, int F, int P, int C, int Hd, const float* wk, float bk,
-                const void* w1_bf16, const float* b1, const void* w2_bf16, const float* b2, void* stream);
 
 /* ---- RMSNorm (M:275-276): out = x / max(||x||_2, 1e-12) * sqrt(C) * gamma over the channel
  * axis of channels-last tokens; token_shift as in mv2_conv_args (M:250-254).               */

@@ -86,8 +86,6 @@ SIGNATURES = {
     "mv2_se_pool": (_I, [_VP, _I, _I, _I, _I, _VP, _F, _VP, _VP]),
     "mv2_se_gate": (_I, [_VP, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
     "mv2_gate_residual": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
-    "mv2_se_tail_supported": (_I, [_I, _I, _I, _I]),
-    "mv2_se_tail": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _VP, _F, _VP, _VP, _VP, _VP, _VP]),
     "mv2_rmsnorm": (_I, [_VP, _VP, _I, _VP, _I, _I, _I, _I, _I, _VP]),
     "mv2_attention": (_I, [C.POINTER(AttnArgs), _VP]),
     "mv2_linattn_workspace_bytes": (_SZ, [_I, _I, _I]),
@@ -141,8 +139,8 @@ def load():
         fn.restype = res
         fn.argtypes = args
     ver = lib.mv2_abi_version()
-    if ver != 3:
-        raise Mv2Error(f"ABI version mismatch: library {ver}, binding 3")
+    if ver != 4:
+        raise Mv2Error(f"ABI version mismatch: library {ver}, binding 4")
     _lib = lib
     return lib
 

@@ -660,237 +660,6 @@ __global__ void gate_residual_bf16x8_kernel(const uint4* __restrict__ y, const u
 
 
 // ------------------------------------------------------------------------------------------
-// SqueezeExcite + residual for SMALL frames in one launch (the deep 16x16 levels: a frame of y is <= 256 KB and the four
-// launches of the general path -- pool, hidden, out, gate/residual -- are pure launch + L2 latency there).
-// One CTA (512 threads) per frame f:
-//   1. pooled[c] = sum_n softmax_n(<y[n,:], wk> + bk) y[n,c]     one warp per position row, online softmax, merged via smem
-//   2. hidden    = leaky_relu_0.1(W1 pooled + b1)                one warp per output, bf16 weight rows (exact: the SE
-//   3. gate      = sigmoid(W2 hidden + b2)                        weights of a bf16 model are bf16 values), fp32 accumulate
-//   4. out[n,c]  = gate[c] * y[n,c] + x[n,c]                      (M:240 + M:174), y re-read from L2
-// NU = 16-byte pieces per lane and row (C <= 256 * NU), HU likewise for the hidden width.
-// ------------------------------------------------------------------------------------------
-constexpr int ST_WARPS = 16;
-template <int NU, int HU>
-__global__ void __launch_bounds__(ST_WARPS * 32) se_tail_kernel(const __nv_bfloat16* __restrict__ y, const __nv_bfloat16* __restrict__ x,
-                                                                __nv_bfloat16* __restrict__ out, int P, int C, int Hd,
-                                                                const float* __restrict__ wk, float bk,
-                                                                const __nv_bfloat16* __restrict__ w1, const float* __restrict__ b1,
-                                                                const __nv_bfloat16* __restrict__ w2, const float* __restrict__ b2) {
-  extern __shared__ __align__(16) float st_sm[];
-  float* wacc = st_sm;                       // [ST_WARPS][C]
-  float* pooled = wacc + ST_WARPS * C;       // [C]
-  float* hidden = pooled + C;                // [Hd]
-  float* gates = hidden + Hd;                // [C]
-  __shared__ float wm[ST_WARPS], wsum[ST_WARPS];
-  const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const __nv_bfloat16* yf = y + (int64_t)f * P * C;
-  pdl_wait();
-  pdl_launch_dependents();
-  // ---- 1. pooling ----
-  float wv[NU][8];
-#pragma unroll
-  for (int u = 0; u < NU; ++u) {
-    const int c = (u * 32 + lane) * 8;
-#pragma unroll
-    for (int q = 0; q < 8; ++q) wv[u][q] = c + q < C ? wk[c + q] : 0.f;
-  }
-  float m = -INFINITY, ssum = 0.f, acc[NU][8];
-#pragma unroll
-  for (int u = 0; u < NU; ++u)
-#pragma unroll
-    for (int q = 0; q < 8; ++q) acc[u][q] = 0.f;
-  // two rows per iteration, software pipelined: the loads of the next pair are issued before the current pair is folded, so
-  // every lane keeps 4 * NU 16-byte loads in flight (the whole kernel is a chain of L2 round trips otherwise)
-  uint4 q0[NU], q1[NU];
-  auto fetch = [&](int n0, uint4 (&a)[NU], uint4 (&b)[NU]) {
-    const int n1 = n0 + ST_WARPS;
-#pragma unroll
-    for (int u = 0; u < NU; ++u) {
-      const int c = (u * 32 + lane) * 8;
-      a[u] = (c < C && n0 < P) ? *reinterpret_cast<const uint4*>(yf + (int64_t)n0 * C + c) : make_uint4(0, 0, 0, 0);
-      b[u] = (c < C && n1 < P) ? *reinterpret_cast<const uint4*>(yf + (int64_t)n1 * C + c) : make_uint4(0, 0, 0, 0);
-    }
-  };
-  fetch(warp, q0, q1);
-  for (int n0 = warp; n0 < P; n0 += 2 * ST_WARPS) {
-    const int n1 = n0 + ST_WARPS;
-    uint4 r0[NU], r1[NU];
-#pragma unroll
-    for (int u = 0; u < NU; ++u) { r0[u] = q0[u]; r1[u] = q1[u]; }
-    fetch(n0 + 2 * ST_WARPS, q0, q1);
-    float v0[NU][8], v1[NU][8], d0 = 0.f, d1 = 0.f;
-#pragma unroll
-    for (int u = 0; u < NU; ++u) {
-      const uint32_t a[4] = {r0[u].x, r0[u].y, r0[u].z, r0[u].w}, b[4] = {r1[u].x, r1[u].y, r1[u].z, r1[u].w};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        v0[u][2 * q] = __uint_as_float(a[q] << 16); v0[u][2 * q + 1] = __uint_as_float(a[q] & 0xffff0000u);
-        v1[u][2 * q] = __uint_as_float(b[q] << 16); v1[u][2 * q + 1] = __uint_as_float(b[q] & 0xffff0000u);
-      }
-#pragma unroll
-      for (int q = 0; q < 8; ++q) { d0 = fmaf(v0[u][q], wv[u][q], d0); d1 = fmaf(v1[u][q], wv[u][q], d1); }
-    }
-    d0 = warp_sum(d0);
-    d1 = warp_sum(d1);
-    const float l0 = d0 + bk, l1 = n1 < P ? d1 + bk : -INFINITY;
-    const float mn = fmaxf(m, fmaxf(l0, l1));
-    const float sc = se_exp(m - mn), e0 = se_exp(l0 - mn), e1 = se_exp(l1 - mn);     // exp(-inf) = 0
-    ssum = fmaf(ssum, sc, e0 + e1);
-#pragma unroll
-    for (int u = 0; u < NU; ++u)
-#pragma unroll
-      for (int q = 0; q < 8; ++q) acc[u][q] = fmaf(e1, v1[u][q], fmaf(e0, v0[u][q], acc[u][q] * sc));
-    m = mn;
-  }
-  if (lane == 0) { wm[warp] = m; wsum[warp] = ssum; }
-#pragma unroll
-  for (int u = 0; u < NU; ++u) {
-    const int c = (u * 32 + lane) * 8;
-    if (c < C) {
-      *reinterpret_cast<float4*>(wacc + warp * C + c) = make_float4(acc[u][0], acc[u][1], acc[u][2], acc[u][3]);
-      *reinterpret_cast<float4*>(wacc + warp * C + c + 4) = make_float4(acc[u][4], acc[u][5], acc[u][6], acc[u][7]);
-    }
-  }
-  __syncthreads();
-  {
-    float M = -INFINITY;
-#pragma unroll
-    for (int w = 0; w < ST_WARPS; ++w) M = fmaxf(M, wm[w]);
-    float cf[ST_WARPS], S = 0.f;
-#pragma unroll
-    for (int w = 0; w < ST_WARPS; ++w) { cf[w] = wm[w] > -INFINITY ? __expf(wm[w] - M) : 0.f; S = fmaf(cf[w], wsum[w], S); }
-    const float inv = 1.f / S;
-    for (int c = tid; c < C; c += ST_WARPS * 32) {
-      float t = 0.f;
-#pragma unroll
-      for (int w = 0; w < ST_WARPS; ++w) t = fmaf(cf[w], wacc[w * C + c], t);
-      pooled[c] = t * inv;
-    }
-  }
-  __syncthreads();
-  // ---- 2. hidden layer: warp per output, 4 outputs in flight ----
-  {
-    float pv[NU][8];
-#pragma unroll
-    for (int u = 0; u < NU; ++u) {
-      const int c = (u * 32 + lane) * 8;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) pv[u][q] = c + q < C ? pooled[c + q] : 0.f;
-    }
-    // every CTA (frame) walks the same weight matrix: start each one at a different row group, so that the ~80 CTAs of a
-    // launch do not all pull the same L2 lines at the same moment
-    const int ng2 = (Hd + ST_WARPS * 4 - 1) / (ST_WARPS * 4);
-    for (int gi = 0; gi < ng2; ++gi) {
-      const int j0 = ((gi + f) % ng2) * (ST_WARPS * 4) + warp * 4;
-      if (j0 >= Hd) continue;
-      uint4 r[4][NU];
-#pragma unroll
-      for (int t = 0; t < 4; ++t)
-#pragma unroll
-        for (int u = 0; u < NU; ++u) {
-          const int c = (u * 32 + lane) * 8;
-          r[t][u] = (j0 + t < Hd && c < C) ? *reinterpret_cast<const uint4*>(w1 + (int64_t)(j0 + t) * C + c) : make_uint4(0, 0, 0, 0);
-        }
-#pragma unroll
-      for (int t = 0; t < 4; ++t) {
-        float d = 0.f;
-#pragma unroll
-        for (int u = 0; u < NU; ++u) {
-          const uint32_t a[4] = {r[t][u].x, r[t][u].y, r[t][u].z, r[t][u].w};
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            d = fmaf(__uint_as_float(a[q] << 16), pv[u][2 * q], d);
-            d = fmaf(__uint_as_float(a[q] & 0xffff0000u), pv[u][2 * q + 1], d);
-          }
-        }
-        d = warp_sum(d);
-        if (lane == 0 && j0 + t < Hd) {
-          const float h = d + b1[j0 + t];
-          hidden[j0 + t] = h > 0.f ? h : 0.1f * h;
-        }
-      }
-    }
-  }
-  __syncthreads();
-  // ---- 3. gates ----
-  {
-    float hv[HU][8];
-#pragma unroll
-    for (int u = 0; u < HU; ++u) {
-      const int j = (u * 32 + lane) * 8;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) hv[u][q] = j + q < Hd ? hidden[j + q] : 0.f;
-    }
-    constexpr int GB = HU == 1 ? 8 : 4;          // outputs per batch: GB * HU 16-byte loads in flight per lane
-    const int ng3 = (C + ST_WARPS * GB - 1) / (ST_WARPS * GB);
-    for (int gi = 0; gi < ng3; ++gi) {
-      const int c0 = ((gi + f) % ng3) * (ST_WARPS * GB) + warp * GB;
-      if (c0 >= C) continue;
-      uint4 r[GB][HU];
-#pragma unroll
-      for (int t = 0; t < GB; ++t)
-#pragma unroll
-        for (int u = 0; u < HU; ++u) {
-          const int j = (u * 32 + lane) * 8;
-          r[t][u] = (c0 + t < C && j < Hd) ? *reinterpret_cast<const uint4*>(w2 + (int64_t)(c0 + t) * Hd + j) : make_uint4(0, 0, 0, 0);
-        }
-#pragma unroll
-      for (int t = 0; t < GB; ++t) {
-        float d = 0.f;
-#pragma unroll
-        for (int u = 0; u < HU; ++u) {
-          const uint32_t a[4] = {r[t][u].x, r[t][u].y, r[t][u].z, r[t][u].w};
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            d = fmaf(__uint_as_float(a[q] << 16), hv[u][2 * q], d);
-            d = fmaf(__uint_as_float(a[q] & 0xffff0000u), hv[u][2 * q + 1], d);
-          }
-        }
-        d = warp_sum(d);
-        if (lane == 0 && c0 + t < C) gates[c0 + t] = 1.f / (1.f + expf(-(d + b2[c0 + t])));
-      }
-    }
-  }
-  __syncthreads();
-  // ---- 4. out = gate * y + x ----
-  {
-    const uint4* y8 = reinterpret_cast<const uint4*>(yf);
-    const uint4* x8 = reinterpret_cast<const uint4*>(x + (int64_t)f * P * C);
-    uint4* o8 = reinterpret_cast<uint4*>(out + (int64_t)f * P * C);
-    const int C8 = C >> 3, total = P * C8;
-    constexpr int PB = 4, NT = ST_WARPS * 32;         // 2 * PB 16-byte loads in flight per thread
-    for (int i0 = tid; i0 < total; i0 += PB * NT) {
-      uint4 yv[PB], xv[PB];
-#pragma unroll
-      for (int b = 0; b < PB; ++b) {
-        const int i = i0 + b * NT;
-        yv[b] = i < total ? y8[i] : make_uint4(0, 0, 0, 0);
-        xv[b] = i < total ? x8[i] : make_uint4(0, 0, 0, 0);
-      }
-#pragma unroll
-      for (int b = 0; b < PB; ++b) {
-        const int i = i0 + b * NT;
-        if (i >= total) break;
-        const int c = (i % C8) * 8;
-        const float4 g0 = *reinterpret_cast<const float4*>(gates + c), g1 = *reinterpret_cast<const float4*>(gates + c + 4);
-        const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-        const __nv_bfloat162* yb = reinterpret_cast<const __nv_bfloat162*>(&yv[b]);
-        const __nv_bfloat162* xb = reinterpret_cast<const __nv_bfloat162*>(&xv[b]);
-        uint4 o;
-        uint32_t* ob = reinterpret_cast<uint32_t*>(&o);
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float2 yf2 = __bfloat1622float2(yb[q]), xf2 = __bfloat1622float2(xb[q]);
-          __nv_bfloat162 r = __floats2bfloat162_rn(fmaf(gg[2 * q], yf2.x, xf2.x), fmaf(gg[2 * q + 1], yf2.y, xf2.y));
-          ob[q] = *reinterpret_cast<uint32_t*>(&r);
-        }
-        o8[i] = o;
-      }
-    }
-  }
-}
-
-// ------------------------------------------------------------------------------------------
 // conditioning helpers (cond_residual; reference M:680-753, M:946-988, M:1344-1352)
 // ------------------------------------------------------------------------------------------
 // y[b][n] = act(sum_k x[b][k] w[n][k] + bias[n]); one warp per output, grid (ceil(N / 8), B)
@@ -2341,10 +2110,6 @@ static int se_rows_per_block(int dtype, int F, int P, int C) {
   (void)F;   // deliberately NOT a function of the frame count: the chunking fixes the summation order of the pooled vector, and
              // a clip's tokens must not depend on how many other clips share its batch (tests: ..._batch_independence)
   if (!(dtype == MV2_BF16 && se_online_vec(C) != 0)) return SE_CHUNK;
-  if (const char* env = getenv("MV2_SE_ROWS")) {     // tuning override (power of two, >= SE_MIN_ROWS)
-    const int v = atoi(env);
-    if (v >= SE_MIN_ROWS && v <= 4096 && (v & (v - 1)) == 0) return v;
-  }
   // small (L2-resident) frames take 64 - 128-row chunks: fewer, longer bulk-copy pipelines and fewer records to merge than
   // 32-row chunks; large frames amortise the per-block merge over longer chunks
   if (P <= 256) return 64;
@@ -2424,46 +2189,6 @@ int mv2_se_gate_records(const void* workspace, int nrec, int F, int C, int Hd, c
     launch_k(se_hidden_kernel<false>, dim3(dim3(F, ceil_div(Hd, 32))), dim3(256), smem1, st, (const float*)workspace, nrec, C, Hd, w1, b1, hidden);
   MV2_CHECK_LAUNCH();
   launch_k(se_out_kernel, dim3(dim3(F, ceil_div(C, 64))), dim3(256), smem2, st, hidden, C, Hd, w2, b2, gates);
-  MV2_CHECK_LAUNCH();
-  return MV2_OK;
-}
-
-int mv2_se_tail_supported(int F, int P, int C, int Hd) {
-  if (F <= 0 || P <= 0 || C <= 0 || Hd <= 0) return 0;
-  if (C % 8 != 0 || C > 1024 || Hd % 8 != 0 || Hd > 1024) return 0;
-  if ((int64_t)P * C > 131072) return 0;                 // frame of y <= 256 KB: the latency-bound deep levels
-  return 1;
-}
-
-int mv2_se_tail(const void* y, const void* x, void* out, int F, int P, int C, int Hd, const float* wk, float bk,
-                const void* w1_bf16, const float* b1, const void* w2_bf16, const float* b2, void* stream) {
-  MV2_CHECK_ARG(y && x && out && wk && w1_bf16 && b1 && w2_bf16 && b2);
-  if (!mv2_se_tail_supported(F, P, C, Hd)) { set_error("mv2_se_tail: unsupported shape F=%d P=%d C=%d Hd=%d", F, P, C, Hd); return MV2_E_UNSUPPORTED; }
-  const size_t smem = ((size_t)ST_WARPS * C + 2 * (size_t)C + Hd) * sizeof(float);
-  MV2_CHECK_ARG(smem <= 96 * 1024);
-  static PerDeviceOnce once;
-  const cudaError_t e = once.run([] {
-    cudaError_t err = cudaSuccess;
-    auto set = [&](const void* fn) { if (err == cudaSuccess) err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024); };
-    set((const void*)se_tail_kernel<1, 1>); set((const void*)se_tail_kernel<2, 1>); set((const void*)se_tail_kernel<2, 2>);
-    set((const void*)se_tail_kernel<4, 1>); set((const void*)se_tail_kernel<4, 2>); set((const void*)se_tail_kernel<4, 4>);
-    set((const void*)se_tail_kernel<1, 2>); set((const void*)se_tail_kernel<1, 4>); set((const void*)se_tail_kernel<2, 4>);
-    return err;
-  });
-  MV2_CHECK_CUDA(e);
-  const int nu = C <= 256 ? 1 : (C <= 512 ? 2 : 4), hu = Hd <= 256 ? 1 : (Hd <= 512 ? 2 : 4);
-  cudaStream_t st = (cudaStream_t)stream;
-  const __nv_bfloat16* yb = (const __nv_bfloat16*)y;
-  const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
-  __nv_bfloat16* ob = (__nv_bfloat16*)out;
-  const __nv_bfloat16* w1b = (const __nv_bfloat16*)w1_bf16;
-  const __nv_bfloat16* w2b = (const __nv_bfloat16*)w2_bf16;
-#define MV2_ST_CASE(N, H) \
-  else if (nu == N && hu == H) launch_k(se_tail_kernel<N, H>, dim3(F), dim3(ST_WARPS * 32), smem, st, yb, xb, ob, P, C, Hd, wk, bk, w1b, b1, w2b, b2)
-  if (false) {}
-  MV2_ST_CASE(1, 1); MV2_ST_CASE(1, 2); MV2_ST_CASE(1, 4); MV2_ST_CASE(2, 1); MV2_ST_CASE(2, 2); MV2_ST_CASE(2, 4);
-  MV2_ST_CASE(4, 1); MV2_ST_CASE(4, 2); MV2_ST_CASE(4, 4);
-#undef MV2_ST_CASE
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }
@@ -2556,14 +2281,9 @@ int mv2_rmsnorm(const void* x, void* out, int dtype, const float* gamma, int B, 
     {
       const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
       __nv_bfloat16* ob = (__nv_bfloat16*)out;
-      int tpw = 1;      // tokens per warp; 1 keeps the most warps in flight on the small README shapes
-      if (const char* env = getenv("MV2_RN_TPW")) { const int v = atoi(env); if (v == 1 || v == 2 || v == 4) tpw = v; }   // tuning override
-      if (C <= 256 && tpw == 1) launch_k(rmsnorm_bf16x8_kernel<1, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
-      else if (C <= 256 && tpw == 2) launch_k(rmsnorm_bf16x8_kernel<1, 2>, dim3(ceil_div(n_tok, 8 * 2)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
-      else if (C <= 256) launch_k(rmsnorm_bf16x8_kernel<1, 4>, dim3(ceil_div(n_tok, 8 * 4)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
-      else if (C <= 512 && tpw == 1) launch_k(rmsnorm_bf16x8_kernel<2, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
-      else if (C <= 512 && tpw == 2) launch_k(rmsnorm_bf16x8_kernel<2, 2>, dim3(ceil_div(n_tok, 8 * 2)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
-      else if (C <= 512) launch_k(rmsnorm_bf16x8_kernel<2, 4>, dim3(ceil_div(n_tok, 8 * 4)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
+      // one token per warp up to C = 512 keeps the most warps in flight on the small README shapes; the widest rows take 4
+      if (C <= 256) launch_k(rmsnorm_bf16x8_kernel<1, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
+      else if (C <= 512) launch_k(rmsnorm_bf16x8_kernel<2, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
       else launch_k(rmsnorm_bf16x8_kernel<4, 4>, dim3(ceil_div(n_tok, 8 * 4)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
     }
   else if (dtype == MV2_BF16)

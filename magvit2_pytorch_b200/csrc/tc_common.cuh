@@ -314,22 +314,6 @@ __device__ __forceinline__ void epi_pack32_t(const uint32_t (&r)[32], const floa
     pk[2 * g + 1] = pack_bf16x2(act_ct<ACT>(__uint_as_float(r[4 * g + 2]) + b.z), act_ct<ACT>(__uint_as_float(r[4 * g + 3]) + b.w));
   }
 }
-// GEGLU of one packed 32-column chunk ([8 x | 8 gate] twice, M:466-469): 16 outputs -> 8 bf16x2 words
-__device__ __forceinline__ void epi_geglu_pack32(const uint32_t (&r)[32], const float* sb, uint32_t* pk) {
-#pragma unroll
-  for (int g = 0; g < 2; ++g) {
-    float bx[8], bg[8], v[8];
-    *reinterpret_cast<float4*>(bx) = *reinterpret_cast<const float4*>(sb + g * 16);
-    *reinterpret_cast<float4*>(bx + 4) = *reinterpret_cast<const float4*>(sb + g * 16 + 4);
-    *reinterpret_cast<float4*>(bg) = *reinterpret_cast<const float4*>(sb + g * 16 + 8);
-    *reinterpret_cast<float4*>(bg + 4) = *reinterpret_cast<const float4*>(sb + g * 16 + 12);
-#pragma unroll
-    for (int q = 0; q < 8; ++q)
-      v[q] = gelu_fast(__uint_as_float(r[g * 16 + 8 + q]) + bg[q]) * (__uint_as_float(r[g * 16 + q]) + bx[q]);
-    pk[4 * g] = pack_bf16x2(v[0], v[1]); pk[4 * g + 1] = pack_bf16x2(v[2], v[3]);
-    pk[4 * g + 2] = pack_bf16x2(v[4], v[5]); pk[4 * g + 3] = pack_bf16x2(v[6], v[7]);
-  }
-}
 // bias + activation of one 32-column chunk, kept in fp32 (for the fp32-staged residual epilogue)
 template <int ACT>
 __device__ __forceinline__ void epi_act32_t(uint32_t (&r)[32], const float* sb) {
@@ -381,6 +365,33 @@ static inline EncodeTiledFn get_encode_fn() {
       fn = (EncodeTiledFn)f;
   });
   return fn;
+}
+
+// Hardware swizzle of a K-major operand tile with rows of row_bytes (128 / 64 / 32 bytes), as gmma_desc_hi describes it
+static inline CUtensorMapSwizzle swizzle_of_row(int row_bytes) {
+  return row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+}
+
+// One bf16 tiled tensor map: dims and box innermost first, byte strides of dims 1 .. rank-1, unit element strides,
+// 256-byte L2 promotion; box elements outside the tensor are zero-filled.  `what` names the map in the error message.
+static inline int encode_bf16_map(CUtensorMap* map, int rank, const void* base, const cuuint64_t* dims,
+                                  const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swz, const char* what) {
+  const EncodeTiledFn enc = get_encode_fn();
+  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return MV2_E_CUDA; }
+  const cuuint32_t es[5] = {1, 1, 1, 1, 1};
+  const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, es,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r); return MV2_E_CUDA; }
+  return MV2_OK;
+}
+
+// Epilogue arguments of a tensor-core conv launch
+static inline TcEpi tc_epi_of(const mv2_tc_conv_args* a) {
+  TcEpi e = {};
+  e.bias = a->bias; e.res = (const __nv_bfloat16*)a->res; e.y = (__nv_bfloat16*)a->y;
+  e.act = a->act; e.shuffle = a->shuffle; e.mode = a->epi_mode; e.Co = a->Co;
+  e.To = a->To; e.Ho = a->Ho; e.Wo = a->Wo; e.out_cf = a->out_layout == 1; e.oscale = a->oscale;
+  return e;
 }
 
 static inline int pow2_ceil(int v) { int r = 1; while (r < v) r <<= 1; return r; }

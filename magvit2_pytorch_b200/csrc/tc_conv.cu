@@ -154,6 +154,12 @@ __global__ void __launch_bounds__(384, 1) tc_conv_kernel(const __grid_constant__
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
+// kernel instance per (epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared memory.
+// Rows: ragged (plain) stores, GEGLU, depth-to-space / depth-to-time shuffle.
+#define MV2_TC_BN(M) {tc_conv_kernel<M, 32>, tc_conv_kernel<M, 64>, tc_conv_kernel<M, 128>}
+static void (*const g_tc_kernels[3][3])(TcParams) = {MV2_TC_BN(EPI_RAGGED), MV2_TC_BN(EPI_GEGLU), MV2_TC_BN(EPI_SHUFFLE)};
+#undef MV2_TC_BN
+
 }  // namespace mv2
 
 using namespace mv2;
@@ -178,13 +184,11 @@ int mv2_tc_conv_supported(const mv2_tc_conv_args* a) {
 int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) {
   MV2_CHECK_ARG(a && a->x && a->w && a->y);
   if (!mv2_tc_conv_supported(a)) { set_error("mv2_tc_conv_forward: unsupported shape (Ci=%d Co=%d)", a->Ci, a->Co); return MV2_E_UNSUPPORTED; }
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return MV2_E_CUDA; }
 
   TcParams p;
   memset(&p, 0, sizeof(p));
   const int bk = (a->Ci % 64 == 0) ? 64 : ((a->Ci % 32 == 0) ? 32 : 16);
-  const CUtensorMapSwizzle swz = bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+  const CUtensorMapSwizzle swz = swizzle_of_row(bk * 2);
   p.bk = bk;
   p.ci_pad = a->Ci;
   p.kchunks = a->Ci / bk;
@@ -207,9 +211,7 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) {
   stages = std::max(2, std::min(stages, 8));
   stages = std::max(1, std::min(stages, a->kt * a->kh * a->kw * (a->Ci / bk)));
   p.stages = stages;
-  p.epi.bias = a->bias; p.epi.res = (const __nv_bfloat16*)a->res; p.epi.y = (__nv_bfloat16*)a->y;
-  p.epi.act = a->act; p.epi.shuffle = a->shuffle; p.epi.mode = a->epi_mode; p.epi.Co = a->Co;
-  p.epi.To = a->To; p.epi.Ho = a->Ho; p.epi.Wo = a->Wo; p.epi.out_cf = 0; p.epi.oscale = a->oscale;
+  p.epi = tc_epi_of(a);
 
   // ---- activation tensor maps: one per stride-parity phase ----
   const int st = a->st, sh = a->sh, sw = a->sw;
@@ -222,16 +224,14 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) {
         const int id = (pt * sh + ph) * sw + pw;
         const int64_t nW = (W - pw + sw - 1) / sw, nH = (H - ph + sh - 1) / sh, nT = (T - pt + st - 1) / st;
         if (nW <= 0 || nH <= 0 || nT <= 0) { set_error("empty stride phase (dimension smaller than stride)"); return MV2_E_UNSUPPORTED; }
-        cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)nW, (cuuint64_t)nH, (cuuint64_t)nT, (cuuint64_t)a->B};
-        cuuint64_t strides[4] = {(cuuint64_t)(sw * C * 2), (cuuint64_t)(sh * W * C * 2), (cuuint64_t)(st * H * W * C * 2),
-                                 (cuuint64_t)(T * H * W * C * 2)};
-        cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)p.bw, (cuuint32_t)p.bh, (cuuint32_t)p.bt, 1};
-        cuuint32_t es[5] = {1, 1, 1, 1, 1};
-        char* base = (char*)a->x + ((int64_t)pt * H * W + (int64_t)ph * W + pw) * C * 2;
-        CUresult r = enc(&p.amap[id], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, base, dims, strides, box, es,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(activations, phase %d) failed: %d", id, (int)r); return MV2_E_CUDA; }
+        const cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)nW, (cuuint64_t)nH, (cuuint64_t)nT, (cuuint64_t)a->B};
+        const cuuint64_t strides[4] = {(cuuint64_t)(sw * C * 2), (cuuint64_t)(sh * W * C * 2), (cuuint64_t)(st * H * W * C * 2),
+                                       (cuuint64_t)(T * H * W * C * 2)};
+        const cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)p.bw, (cuuint32_t)p.bh, (cuuint32_t)p.bt, 1};
+        const char* base = (const char*)a->x + ((int64_t)pt * H * W + (int64_t)ph * W + pw) * C * 2;
+        char what[32];
+        snprintf(what, sizeof(what), "activations, phase %d", id);
+        if (const int rc = encode_bf16_map(&p.amap[id], 5, base, dims, strides, box, swz, what)) return rc;
       }
   // ---- taps ----
   p.ntaps = a->kt * a->kh * a->kw;
@@ -247,38 +247,26 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) {
         p.tap_dw[tap] = (int8_t)floor_div(ow, sw);
       }
   // ---- weights map: [Co][taps * Ci] K-major ----
-  {
-    const int64_t K = (int64_t)p.ntaps * a->Ci;
-    cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
-    cuuint64_t strides[1] = {(cuuint64_t)(K * 2)};
-    cuuint32_t box[2] = {(cuuint32_t)bk, (cuuint32_t)bn};
-    cuuint32_t es[2] = {1, 1};
-    CUresult r = enc(&p.wmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)a->w, dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(weights) failed: %d", (int)r); return MV2_E_CUDA; }
-  }
+  const int64_t K = (int64_t)p.ntaps * a->Ci;
+  const cuuint64_t wdims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
+  const cuuint64_t wstrides[1] = {(cuuint64_t)(K * 2)};
+  const cuuint32_t wbox[2] = {(cuuint32_t)bk, (cuuint32_t)bn};
+  if (const int rc = encode_bf16_map(&p.wmap, 2, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
+
   const size_t smem = 1024 + (size_t)stages * stage_bytes + 16 * stages + 16 + (size_t)bn * 4 + stg_bytes;
   static PerDeviceOnce attr_once;
   const cudaError_t attr_err = attr_once.run([] {
     cudaError_t e = cudaSuccess;
-    for (auto k : {tc_conv_kernel<EPI_RAGGED, 32>, tc_conv_kernel<EPI_RAGGED, 64>, tc_conv_kernel<EPI_RAGGED, 128>,
-                   tc_conv_kernel<EPI_GEGLU, 32>, tc_conv_kernel<EPI_GEGLU, 64>, tc_conv_kernel<EPI_GEGLU, 128>,
-                   tc_conv_kernel<EPI_SHUFFLE, 32>, tc_conv_kernel<EPI_SHUFFLE, 64>, tc_conv_kernel<EPI_SHUFFLE, 128>})
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    for (auto& row : g_tc_kernels)
+      for (auto k : row)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     return e;
   });
   if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
   MV2_CHECK_ARG(smem <= 227 * 1024);
   dim3 grid((unsigned)((int64_t)a->B * p.tt * p.th * p.tw), (unsigned)ceil_div(a->Co, bn));
-  const int mode = a->epi_mode == 1 ? EPI_GEGLU : (a->shuffle != MV2_SHUFFLE_NONE ? EPI_SHUFFLE : EPI_RAGGED);
-  void (*k)(TcParams) = nullptr;
-#define MV2_PICK(M) k = bn == 32 ? tc_conv_kernel<M, 32> : (bn == 64 ? tc_conv_kernel<M, 64> : tc_conv_kernel<M, 128>)
-  if (mode == EPI_GEGLU) MV2_PICK(EPI_GEGLU);
-  else if (mode == EPI_SHUFFLE) MV2_PICK(EPI_SHUFFLE);
-  else MV2_PICK(EPI_RAGGED);
-#undef MV2_PICK
-  launch_k(k, grid, dim3(384), smem, (cudaStream_t)stream, p);
+  const int flavour = a->epi_mode == 1 ? 1 : (a->shuffle != MV2_SHUFFLE_NONE ? 2 : 0);   // row of g_tc_kernels
+  launch_k(g_tc_kernels[flavour][bn == 32 ? 0 : (bn == 64 ? 1 : 2)], grid, dim3(384), smem, (cudaStream_t)stream, p);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }

@@ -28,7 +28,6 @@
 #include <map>
 #include <vector>
 #include <string.h>
-#include <stdlib.h>
 
 namespace mv2 {
 
@@ -44,7 +43,6 @@ struct alignas(64) SlabParams {
   int bn, n_tiles_n, tiles_w, tiles_h, total_tiles;
   int slab_stages, w_stages;
   int tpw;               // in-plane taps per weight stage (one 3-D TMA box {bk, bn, tpw})
-  int geglu_staged;      // EPI_GEGLU: 64-column chunks through the transpose buffers (1) or direct 16-byte row pieces (0)
   TcEpi epi;
   // ---- EPI_FUSED_RU only (mv2_tc_ru_forward) ----
   CUtensorMap w1map;     // 1x1x1 weights [Co][Ci] as {ci, co}: 2-D boxes {64, bn}
@@ -119,7 +117,6 @@ __host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& 
 template <int MODE, int BN>
 __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__ SlabParams p) {
   constexpr int MWMAX = 128 / BN;
-  constexpr int NEPI = 8;                            // epilogue warps
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -580,47 +577,6 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
             }
             __syncwarp();
           }
-        } else if (MODE == EPI_GEGLU && p.geglu_staged) {
-          // fc1 + GEGLU (M:466-469, M:492): 64 accumulator columns (packed [8 x | 8 gate] groups) give 32 outputs = 64 bytes per
-          // row, staged through the same transpose buffer as the plain epilogue so that every store instruction writes 8 rows x
-          // 64 contiguous bytes instead of 32 scattered 16-byte pieces.  Opt-in (MV2_GEGLU_STAGED): the
-          // GELU math, not the stores, sets the pace of this epilogue, so the direct path is the default.  The two warps of a
-          // lane quarter alternate 64-column chunks (bn % 64 == 0: the packed width is a multiple of 128).
-          const uint32_t stg = stage0 + (uint32_t)ew * 2048;
-          const uint32_t wr = stg + lane * 64, wsw = (lane >> 1) & 3;
-          const int rl = lane >> 2, piece = lane & 3;
-          const int w2 = c.w0 + 8 * j + rl;
-          const uint32_t rd = stg + rl * 64;
-          const int h20 = c.h0 + sub * 4;
-          const int I = p.Co >> 1;
-          const int64_t row0 = ((((int64_t)c.b * p.T + c.t) * p.H + h20) * p.W + w2) * I + (c.n0 >> 1) + piece * 8;
-          const int64_t ks = (int64_t)p.W * I;
-          const int kmax = w2 < p.W ? p.H - h20 : 0;
-          const int nch = p.bn >> 6;                 // 64-column chunks per M-tile, dealt round-robin over the NEPI / 4 warps of a quarter
-          for (int c0 = 0; c0 < p.bn; c0 += 64) {
-            if (((j * nch + (c0 >> 6)) & (NEPI / 4 - 1)) != half) continue;
-            uint32_t r0[32], r1[32], pk[16];
-            load_row32(srow + c0, 32, r0);
-            load_row32(srow + c0 + 32, 32, r1);
-            epi_geglu_pack32(r0, sbias + c.n0 + c0, pk);
-            epi_geglu_pack32(r1, sbias + c.n0 + c0 + 32, pk + 8);
-#pragma unroll
-            for (int g = 0; g < 4; ++g)
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(wr + ((g ^ wsw) << 4)), "r"(pk[4 * g]),
-                           "r"(pk[4 * g + 1]), "r"(pk[4 * g + 2]), "r"(pk[4 * g + 3]) : "memory");
-            __syncwarp();
-            const bool col_ok = c.n0 + c0 + piece * 16 < p.Co && c0 + piece * 16 < p.bn;
-            const int klim = col_ok ? kmax : 0;
-            __nv_bfloat16* yp = p.epi.y + row0 + (c0 >> 1);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              uint4 v;
-              asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
-                           : "r"(rd + k * 512 + ((piece ^ (((8 * k + rl) >> 1) & 3)) << 4)));
-              if (k < klim) *reinterpret_cast<uint4*>(yp + k * ks) = v;
-            }
-            __syncwarp();
-          }
         } else {
           for (int c0 = ((j + half) & 1) * 32; c0 < p.bn; c0 += 64) {
             uint32_t r[32];
@@ -636,25 +592,6 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
 }  // namespace mv2
 
 using namespace mv2;
-
-// kernel instance per (epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared memory
-#define MV2_SLAB_BN(M) {tc_slab_kernel<M, 32>, tc_slab_kernel<M, 64>, tc_slab_kernel<M, 128>}
-static void (*const g_slab_kernels[8][3])(SlabParams) = {
-    MV2_SLAB_BN(EPI_PLAIN), MV2_SLAB_BN(EPI_GEGLU), MV2_SLAB_BN(EPI_SHUFFLE), MV2_SLAB_BN(EPI_RAGGED),
-    MV2_SLAB_BN(EPI_PLAIN_RES), MV2_SLAB_BN(EPI_FUSED_RU), MV2_SLAB_BN(EPI_SHUFFLE_ST), MV2_SLAB_BN(EPI_DOWN_SPACE)};
-#undef MV2_SLAB_BN
-static void (*slab_kernel_for(int mode, int bn))(SlabParams) { return g_slab_kernels[mode][bn == 32 ? 0 : (bn == 64 ? 1 : 2)]; }
-static cudaError_t slab_set_smem_attr() {
-  static PerDeviceOnce once;
-  return once.run([] {
-    cudaError_t e = cudaSuccess;
-    for (auto& row : g_slab_kernels)
-      for (auto k : row)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    return e;
-  });
-}
-
 
 extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
   if (!a) return 0;
@@ -681,23 +618,44 @@ extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
   return 1;
 }
 
+// Shared memory left for the two TMA rings of a launch: 227 KB minus what follows them (barrier table sized for the deepest
+// rings, bias, transpose buffers, accumulator staging, [fused: H buffer, resident 1x1x1 weights]) and the alignment slack.
+static int slab_ring_budget(const SlabParams& p, bool fused) {
+  SlabParams q = p;
+  q.slab_stages = 3; q.w_stages = 12;      // upper bounds for the barrier table
+  return 227 * 1024 - 2048 - (int)slab_smem_layout(q, 0, fused).end;
+}
+// Dynamic shared memory of a launch: alignment slack, the slab and weight rings, then slab_smem_layout
+static size_t slab_smem_bytes(const SlabParams& p, bool fused) {
+  const uint32_t rings = (uint32_t)(p.slab_stages * p.slab_stride + p.w_stages * p.bn * p.row_bytes * p.tpw);
+  return 1024 + slab_smem_layout(p, rings, fused).end;
+}
+// M-tiles side by side per weight tile: as many as the frame width uses, while their accumulators fit 64 fp32 registers
+// per consumer thread (mw * bn <= 128); this divides the weight traffic by mw
+static int slab_default_mw(int bn, int Wo) { return bn == 32 && Wo > 16 ? 4 : (bn <= 64 && Wo > 8 ? 2 : 1); }
+// Slab geometry of a macro tile of mw M-tiles: slab row pitch, bytes of one slab (slab_h rows) and its 1024-byte aligned
+// ring stride, tile counts.  Needs kw, slab_h, row_bytes, B, T, W, tiles_h and n_tiles_n.
+static void slab_set_geometry(SlabParams& p, int mw) {
+  p.mw = mw;
+  p.pitch = 8 * mw + p.kw - 1;
+  p.slab_bytes = p.pitch * p.slab_h * p.row_bytes;
+  p.slab_stride = (p.slab_bytes + 1023) / 1024 * 1024;
+  p.tiles_w = ceil_div(p.W, 8 * mw);
+  p.total_tiles = (int)((int64_t)p.B * p.T * p.tiles_h * p.tiles_w * p.n_tiles_n);
+}
+
 // Everything the launch derives from the layer shape alone (tiling, ring depths, tile count): pure host arithmetic, no
 // CUDA calls -- also reachable through mv2_tc_slab_plan / mv2_tc_slab_tile for the CPU-side tests.
-static int slab_fill_plan(const mv2_tc_conv_args* a, int n_sm, SlabParams& p, int* bk_out, int* w_bytes_out, int* co_pad_out, int* nb_pad_out) {
+static int slab_fill_plan(const mv2_tc_conv_args* a, SlabParams& p) {
   memset(&p, 0, sizeof(p));
   p.kt = a->kt; p.kh = a->kh; p.kw = a->kw; p.pt = a->pt; p.ph = a->ph; p.pw = a->pw;
   p.st = a->st;
   p.row_bytes = (a->Ci % 64 == 0) ? 128 : 64;
-  const int bk = p.row_bytes / 2;
-  p.Ci = a->Ci; p.kchunks = a->Ci / bk;
+  p.Ci = a->Ci; p.kchunks = a->Ci / (p.row_bytes / 2);
   p.B = a->B; p.T = a->To; p.H = a->Ho; p.W = a->Wo; p.Co = a->Co;
-  p.epi.bias = a->bias; p.epi.res = (const __nv_bfloat16*)a->res; p.epi.y = (__nv_bfloat16*)a->y;
-  p.epi.act = a->act; p.epi.shuffle = a->shuffle; p.epi.mode = a->epi_mode; p.epi.Co = a->Co;
-  p.epi.To = a->To; p.epi.Ho = a->Ho; p.epi.Wo = a->Wo; p.epi.out_cf = a->out_layout == 1; p.epi.oscale = a->oscale;
+  p.epi = tc_epi_of(a);
 
-  // ---- tiling: widest N tile (<= 128 columns); M-tiles side by side share each weight tile while their accumulators
-  //      fit 64 fp32 registers per consumer thread (mw * bn <= 128), which divides the weight traffic by mw ----
-  const int tiles_h = ceil_div(a->Ho, 16);
+  // ---- tiling: widest N tile (<= 128 columns), then as many M-tiles per weight tile as slab_default_mw allows ----
   const int co_pad = (a->Co + 31) / 32 * 32;
   int best_bn = 32;
   for (int bn = 128; bn >= 32; bn >>= 1)
@@ -708,44 +666,23 @@ static int slab_fill_plan(const mv2_tc_conv_args* a, int n_sm, SlabParams& p, in
   const bool ragged_ok = a->epi_mode == 0 && a->shuffle == MV2_SHUFFLE_NONE && a->Co % 8 == 0;
   if ((ragged_ok || a->epi_mode == 1) && best_bn <= 64 && co_pad >= 512 && (co_pad + 127) / 128 * 128 * 100 <= co_pad * 108)
     best_bn = 128;
-  int best_mw = 1;
-  if (a->Wo > 8 && best_bn <= 64) best_mw = 2;
-  if (a->Wo > 16 && best_bn == 32) best_mw = 4;
-  if (const char* env = getenv("MV2_SLAB_CFG")) {   // debug / tuning override: "mw,bn"
-    int emw = 0, ebn = 0;
-    if (sscanf(env, "%d,%d", &emw, &ebn) == 2 && (emw == 1 || emw == 2 || emw == 4) && (ebn == 32 || ebn == 64 || ebn == 128) &&
-        (a->epi_mode == 1 ? ebn % 64 == 0 : (co_pad % ebn == 0 || ragged_ok)) && emw * ebn <= 128 && !(emw >= 2 && a->Wo <= 8)) { best_mw = emw; best_bn = ebn; }
-  }
-  p.mw = best_mw; p.bn = best_bn;
-  p.geglu_staged = (a->epi_mode == 1 && p.bn % 64 == 0 && getenv("MV2_GEGLU_STAGED")) ? 1 : 0;
+  p.bn = best_bn;
   p.n_tiles_n = (co_pad + p.bn - 1) / p.bn;   // a ragged last tile reads zero-filled weight rows and stores nothing for them
-  p.tiles_h = tiles_h;
+  p.tiles_h = ceil_div(a->Ho, 16);
   p.slab_h = 16 + a->kh - 1;
-  const int nb_pad = p.n_tiles_n * p.bn;   // bias staging covers the padded column range
   int budget;
-  for (;; p.mw >>= 1) {     // a wide macro tile whose two slab stages and accumulator staging do not fit: narrow it
-    p.pitch = 8 * p.mw + a->kw - 1;
-    p.slab_bytes = p.pitch * p.slab_h * p.row_bytes;
-    p.slab_stride = (p.slab_bytes + 1023) / 1024 * 1024;
-    p.slab_stages = 3; p.w_stages = 12;      // upper bounds for the barrier table
-    // 227 KB minus what follows the rings (barriers, bias, transpose buffers, accumulator staging) and alignment slack
-    budget = 227 * 1024 - 2048 - (int)slab_smem_layout(p, 0, false).end;
-    if (p.mw == 1 || 2 * p.slab_stride + 2 * p.bn * p.row_bytes <= budget) break;
+  for (int mw = slab_default_mw(p.bn, a->Wo);; mw >>= 1) {   // two slab stages and the staging of a wide macro tile do not fit: narrow it
+    slab_set_geometry(p, mw);
+    budget = slab_ring_budget(p, false);
+    if (mw == 1 || 2 * p.slab_stride + 2 * p.bn * p.row_bytes <= budget) break;
   }
-  p.tiles_w = ceil_div(a->Wo, 8 * p.mw);
-  p.total_tiles = (int)((int64_t)a->B * a->To * p.tiles_h * p.tiles_w * p.n_tiles_n);
   // weight ring stage = tpw consecutive in-plane taps (fewer barrier round trips for small tiles), <= 32 KB
   const int taps2d = a->kh * a->kw;
   p.tpw = 1;
   for (int d = taps2d; d >= 1; --d)
     if (taps2d % d == 0 && d * p.bn * p.row_bytes <= 32 * 1024) { p.tpw = d; break; }
-  if (const char* env = getenv("MV2_SLAB_TPW")) { const int v = atoi(env); if (v >= 1 && taps2d % v == 0 && v * p.bn * p.row_bytes <= 64 * 1024) p.tpw = v; }
   int w_bytes = p.bn * p.row_bytes * p.tpw;
   p.slab_stages = p.slab_stride * 3 + w_bytes * 3 <= budget ? 3 : 2;
-  if (const char* env = getenv("MV2_SLAB_STAGES")) {   // tuning override: activation-slab ring depth
-    const int v = atoi(env);
-    if (v >= 2 && v <= 12 && v * p.slab_stride + 2 * w_bytes <= budget) p.slab_stages = v;
-  }
   p.w_stages = std::min(12, (budget - p.slab_stages * p.slab_stride) / w_bytes);
   if (p.w_stages < 2 && p.slab_stages > 2) { p.slab_stages = 2; p.w_stages = std::min(12, (budget - 2 * p.slab_stride) / w_bytes); }
   while (p.w_stages < 2 && p.tpw > 1) {   // wide slabs: fall back to fewer taps per weight stage
@@ -756,8 +693,51 @@ static int slab_fill_plan(const mv2_tc_conv_args* a, int n_sm, SlabParams& p, in
     p.w_stages = std::min(12, (budget - p.slab_stages * p.slab_stride) / w_bytes);
   }
   MV2_CHECK_ARG(p.w_stages >= 2);
+  return MV2_OK;
+}
 
-  *bk_out = bk; *w_bytes_out = w_bytes; *co_pad_out = co_pad; *nb_pad_out = nb_pad;
+// TMA maps of a stride-1 slab conv: the activation slab (box {bk, pitch, slab_h, 1, 1} of x as {Ci, Wi, Hi, Ti, B}) and the
+// weights [Co][tap][Ci] as {ci, co, tap} (box {bk, bn, tpw}: tpw consecutive K-major tiles) and as {k, co} (box {bk, bn}).
+static int slab_encode_maps(SlabParams& p, const mv2_tc_conv_args* a) {
+  const CUtensorMapSwizzle swz = swizzle_of_row(p.row_bytes);
+  const int64_t C = a->Ci, W = a->Wi, H = a->Hi, T = a->Ti;
+  const cuuint64_t xdims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)T, (cuuint64_t)a->B};
+  const cuuint64_t xstrides[4] = {(cuuint64_t)(C * 2), (cuuint64_t)(W * C * 2), (cuuint64_t)(H * W * C * 2), (cuuint64_t)(T * H * W * C * 2)};
+  const cuuint32_t xbox[5] = {(cuuint32_t)p.row_bytes / 2, (cuuint32_t)p.pitch, (cuuint32_t)p.slab_h, 1, 1};
+  if (const int rc = encode_bf16_map(&p.amap, 5, a->x, xdims, xstrides, xbox, swz, "slab")) return rc;
+  const int64_t ntaps = (int64_t)a->kt * a->kh * a->kw, K = ntaps * C;
+  const cuuint64_t wdims[3] = {(cuuint64_t)C, (cuuint64_t)a->Co, (cuuint64_t)ntaps}, kdims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
+  const cuuint64_t wstrides[2] = {(cuuint64_t)(K * 2), (cuuint64_t)(C * 2)};
+  const cuuint32_t wbox[3] = {(cuuint32_t)p.row_bytes / 2, (cuuint32_t)p.bn, (cuuint32_t)p.tpw};
+  if (const int rc = encode_bf16_map(&p.wmap, 3, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
+  return encode_bf16_map(&p.wmap2, 2, a->w, kdims, wstrides, wbox, swz, "weights 2-D");
+}
+
+// Launches one slab-kernel flavour: persistent CTAs, one per SM of the current device (fewer when there are fewer tiles)
+static int slab_launch(int mode, const SlabParams& p, void* stream) {
+  // kernel instance per (epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared memory
+#define MV2_SLAB_BN(M) {tc_slab_kernel<M, 32>, tc_slab_kernel<M, 64>, tc_slab_kernel<M, 128>}
+  static void (*const kernels[8][3])(SlabParams) = {
+      MV2_SLAB_BN(EPI_PLAIN), MV2_SLAB_BN(EPI_GEGLU), MV2_SLAB_BN(EPI_SHUFFLE), MV2_SLAB_BN(EPI_RAGGED),
+      MV2_SLAB_BN(EPI_PLAIN_RES), MV2_SLAB_BN(EPI_FUSED_RU), MV2_SLAB_BN(EPI_SHUFFLE_ST), MV2_SLAB_BN(EPI_DOWN_SPACE)};
+#undef MV2_SLAB_BN
+  static PerDeviceOnce attr_once;
+  const cudaError_t attr_err = attr_once.run([] {
+    cudaError_t e = cudaSuccess;
+    for (auto& row : kernels)
+      for (auto k : row)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    return e;
+  });
+  if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
+  const size_t smem = slab_smem_bytes(p, mode == EPI_FUSED_RU);
+  MV2_CHECK_ARG(smem <= 227 * 1024);
+  int dev = 0, n_sm = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+  launch_k(kernels[mode][p.bn == 32 ? 0 : (p.bn == 64 ? 1 : 2)], dim3(std::min(p.total_tiles, n_sm)), dim3(384), smem,
+           (cudaStream_t)stream, p);
+  MV2_CHECK_LAUNCH();
   return MV2_OK;
 }
 
@@ -765,9 +745,7 @@ extern "C" int mv2_tc_slab_plan(const mv2_tc_conv_args* a, int n_sm, int* out6) 
   MV2_CHECK_ARG(a && out6 && n_sm > 0);
   if (!mv2_tc_slab_supported(a)) { set_error("mv2_tc_slab_plan: unsupported shape"); return MV2_E_UNSUPPORTED; }
   SlabParams p;
-  int bk, w_bytes, co_pad, nb_pad;
-  const int rc = slab_fill_plan(a, n_sm, p, &bk, &w_bytes, &co_pad, &nb_pad);
-  if (rc != MV2_OK) return rc;
+  if (const int rc = slab_fill_plan(a, p)) return rc;
   const int grid = std::min(p.total_tiles, n_sm);
   out6[0] = p.mw; out6[1] = p.bn; out6[2] = p.n_tiles_n; out6[3] = p.total_tiles; out6[4] = grid; out6[5] = p.slab_stages;
   return MV2_OK;
@@ -777,9 +755,7 @@ extern "C" int mv2_tc_slab_tile(const mv2_tc_conv_args* a, int n_sm, int cta, in
   MV2_CHECK_ARG(a && out6 && n_sm > 0 && cta >= 0 && k >= 0);
   if (!mv2_tc_slab_supported(a)) { set_error("mv2_tc_slab_tile: unsupported shape"); return MV2_E_UNSUPPORTED; }
   SlabParams p;
-  int bk, w_bytes, co_pad, nb_pad;
-  const int rc = slab_fill_plan(a, n_sm, p, &bk, &w_bytes, &co_pad, &nb_pad);
-  if (rc != MV2_OK) return rc;
+  if (const int rc = slab_fill_plan(a, p)) return rc;
   const int grid = std::min(p.total_tiles, n_sm);
   MV2_CHECK_ARG(cta < grid);
   const int tile = slab_tile_of_cta(p, k, cta, grid);
@@ -794,64 +770,16 @@ extern "C" int mv2_tc_slab_tile(const mv2_tc_conv_args* a, int n_sm, int cta, in
 extern "C" int mv2_tc_slab_forward(const mv2_tc_conv_args* a, void* stream) {
   MV2_CHECK_ARG(a && a->x && a->w && a->y);
   if (!mv2_tc_slab_supported(a)) { set_error("mv2_tc_slab_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return MV2_E_CUDA; }
-  int dev = 0, n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-
   SlabParams p;
-  int bk, w_bytes, co_pad, nb_pad;
-  {
-    const int rc = slab_fill_plan(a, n_sm, p, &bk, &w_bytes, &co_pad, &nb_pad);
-    if (rc != MV2_OK) return rc;
-  }
-  const CUtensorMapSwizzle swz = p.row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
-  {
-    const int64_t C = a->Ci, W = a->Wi, H = a->Hi, T = a->Ti;
-    cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)T, (cuuint64_t)a->B};
-    cuuint64_t strides[4] = {(cuuint64_t)(C * 2), (cuuint64_t)(W * C * 2), (cuuint64_t)(H * W * C * 2), (cuuint64_t)(T * H * W * C * 2)};
-    cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)p.pitch, (cuuint32_t)p.slab_h, 1, 1};
-    cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(&p.amap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)a->x, dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(slab) failed: %d", (int)r); return MV2_E_CUDA; }
-  }
-  {
-    // weights [Co][tap][Ci] viewed as {ci, co, tap}: a box {bk, bn, tpw} lands as tpw consecutive K-major tiles
-    const int64_t ntaps = (int64_t)a->kt * a->kh * a->kw;
-    const int64_t K = ntaps * a->Ci;
-    cuuint64_t dims[3] = {(cuuint64_t)a->Ci, (cuuint64_t)a->Co, (cuuint64_t)ntaps};
-    cuuint64_t strides[2] = {(cuuint64_t)(K * 2), (cuuint64_t)(a->Ci * 2)};
-    cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)p.bn, (cuuint32_t)p.tpw};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(&p.wmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)a->w, dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(weights) failed: %d", (int)r); return MV2_E_CUDA; }
-    cuuint64_t dims2[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
-    cuuint64_t strides2[1] = {(cuuint64_t)(K * 2)};
-    cuuint32_t box2[2] = {(cuuint32_t)bk, (cuuint32_t)p.bn};
-    cuuint32_t es2[2] = {1, 1};
-    r = enc(&p.wmap2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)a->w, dims2, strides2, box2, es2,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(weights 2-D) failed: %d", (int)r); return MV2_E_CUDA; }
-  }
-  const size_t smem = 1024 + slab_smem_layout(p, (uint32_t)(p.slab_stages * p.slab_stride + p.w_stages * w_bytes), false).end;
-  MV2_CHECK_ARG(smem <= 227 * 1024);
-  const cudaError_t attr_err = slab_set_smem_attr();
-  if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
-  const int grid = std::min(p.total_tiles, n_sm);
+  if (const int rc = slab_fill_plan(a, p)) return rc;
+  if (const int rc = slab_encode_maps(p, a)) return rc;
   int mode = EPI_PLAIN;
   if (a->epi_mode == 1) mode = EPI_GEGLU;
-  else if (a->shuffle != MV2_SHUFFLE_NONE && (a->Co / (a->shuffle == MV2_SHUFFLE_SPACE ? 4 : 2)) % 32 == 0 && !getenv("MV2_NO_SHUFFLE_ST")) mode = EPI_SHUFFLE_ST;
+  else if (a->shuffle != MV2_SHUFFLE_NONE && (a->Co / (a->shuffle == MV2_SHUFFLE_SPACE ? 4 : 2)) % 32 == 0) mode = EPI_SHUFFLE_ST;
   else if (a->shuffle != MV2_SHUFFLE_NONE) mode = EPI_SHUFFLE;
   else if (a->Co % 8 != 0) mode = EPI_RAGGED;
   else if (a->res) mode = EPI_PLAIN_RES;
-  launch_k(slab_kernel_for(mode, p.bn), dim3(grid), dim3(384), smem, (cudaStream_t)stream, p);
-  MV2_CHECK_LAUNCH();
-  return MV2_OK;
+  return slab_launch(mode, p, stream);
 }
 
 
@@ -878,43 +806,20 @@ extern "C" int mv2_tc_ru_supported(const mv2_tc_ru_args* a) {
   return mv2_tc_slab_supported(&c);
 }
 
-// tiling + shared-memory plan of the fused kernel (host arithmetic only)
-static int ru_fill_plan(const mv2_tc_ru_args* a, int n_sm, SlabParams& p, size_t* smem_out) {
+// tiling + shared-memory plan of the fused kernel (host arithmetic only): the slab plan of the 3x3x3 conv (one N tile of
+// bn = C; its M-tile rule gives mw = 2 at C = 64 and 1 at C = 128), one tap per weight stage, two slab stages and as many
+// weight stages as the H buffer and the resident 1x1x1 weights leave room for
+static int ru_fill_plan(const mv2_tc_ru_args* a, SlabParams& p) {
   mv2_tc_conv_args c;
   ru_as_conv_args(a, &c);
-  int bk, w_bytes, co_pad, nb_pad;
-  const int rc = slab_fill_plan(&c, n_sm, p, &bk, &w_bytes, &co_pad, &nb_pad);
-  if (rc != MV2_OK) return rc;
+  if (const int rc = slab_fill_plan(&c, p)) return rc;
   MV2_CHECK_ARG(p.bn == a->C && p.n_tiles_n == 1 && p.row_bytes == 128);
-  // defaults: as many M-tiles as the 64-register accumulator budget allows (C = 64: 2, C = 128: 1)
-  int mw = a->C == 64 ? 2 : 1, tpw = 1, slab_stages = 2, w_stages = 0;
-  if (const char* env = getenv("MV2_RU_CFG")) {      // tuning override: "mw,tpw,slab_stages,w_stages" (0 = derive)
-    int v[4] = {0, 0, 0, 0};
-    if (sscanf(env, "%d,%d,%d,%d", &v[0], &v[1], &v[2], &v[3]) >= 1) {
-      if ((v[0] == 1 || v[0] == 2) && v[0] * a->C <= 128) mw = v[0];
-      if (v[1] >= 1 && (a->kh * a->kw) % v[1] == 0) tpw = v[1];
-      if (v[2] == 2 || v[2] == 3) slab_stages = v[2];
-      if (v[3] >= 2) w_stages = v[3];
-    }
-  }
-  p.mw = mw; p.tpw = tpw;
-  p.tiles_w = ceil_div(a->W, 8 * p.mw);
-  p.total_tiles = (int)((int64_t)a->B * a->T * p.tiles_h * p.tiles_w);
-  p.pitch = 8 * p.mw + a->kw - 1;
-  p.slab_bytes = p.pitch * p.slab_h * p.row_bytes;
-  p.slab_stride = (p.slab_bytes + 1023) / 1024 * 1024;
+  p.tpw = 1;
   p.h_stride = p.kchunks * 16384;
-  const int wb = p.bn * p.row_bytes * p.tpw;
-  p.slab_stages = 3; p.w_stages = 12;      // upper bounds for the barrier table
-  const size_t fixed = 2048 /* base and H alignment */ + slab_smem_layout(p, 0, true).end;
-  const size_t total = 227 * 1024;
-  p.slab_stages = slab_stages;
-  while (p.slab_stages > 2 && fixed + (size_t)p.slab_stages * p.slab_stride + 2 * (size_t)wb > total) --p.slab_stages;
-  const int64_t room = (int64_t)total - (int64_t)fixed - (int64_t)p.slab_stages * p.slab_stride;
-  p.w_stages = (int)std::min<int64_t>(12, room / wb);
-  if (w_stages >= 2 && w_stages <= p.w_stages) p.w_stages = w_stages;
+  const int budget = slab_ring_budget(p, true);
+  p.slab_stages = 2;
+  p.w_stages = std::min(12, (budget - 2 * p.slab_stride) / (p.bn * p.row_bytes));
   MV2_CHECK_ARG(p.w_stages >= 2);
-  *smem_out = 1024 + slab_smem_layout(p, (uint32_t)(p.slab_stages * p.slab_stride + p.w_stages * wb), true).end;
   p.bias1 = a->b1; p.se_wk = a->se_wk; p.se_bk = a->se_bk; p.se_ws = a->se_ws;
   return MV2_OK;
 }
@@ -922,9 +827,7 @@ static int ru_fill_plan(const mv2_tc_ru_args* a, int n_sm, SlabParams& p, size_t
 extern "C" int mv2_tc_ru_records(const mv2_tc_ru_args* a) {
   if (!mv2_tc_ru_supported(a)) { set_error("mv2_tc_ru_records: unsupported shape"); return MV2_E_UNSUPPORTED; }
   SlabParams p;
-  size_t smem;
-  const int rc = ru_fill_plan(a, 132, p, &smem);   // the record count does not depend on the SM count
-  if (rc != MV2_OK) return rc;
+  if (const int rc = ru_fill_plan(a, p)) return rc;
   return p.tiles_h * p.tiles_w * 4;
 }
 
@@ -938,57 +841,16 @@ extern "C" size_t mv2_tc_ru_workspace_bytes(const mv2_tc_ru_args* a) {
 extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, void* stream) {
   MV2_CHECK_ARG(a && a->x && a->w3 && a->w1 && a->y && a->se_wk && a->se_ws);
   if (!mv2_tc_ru_supported(a)) { set_error("mv2_tc_ru_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return MV2_E_CUDA; }
-  int dev = 0, n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   SlabParams p;
-  size_t smem = 0;
-  {
-    const int rc = ru_fill_plan(a, n_sm, p, &smem);
-    if (rc != MV2_OK) return rc;
-  }
-  MV2_CHECK_ARG(smem <= 227 * 1024);
-  const int bk = 64;
-  {
-    const int64_t C = a->C, W = a->W, H = a->H, T = a->T;
-    cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)T, (cuuint64_t)a->B};
-    cuuint64_t strides[4] = {(cuuint64_t)(C * 2), (cuuint64_t)(W * C * 2), (cuuint64_t)(H * W * C * 2), (cuuint64_t)(T * H * W * C * 2)};
-    cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)p.pitch, (cuuint32_t)p.slab_h, 1, 1};
-    cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    CUresult r = enc(&p.amap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)a->x, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(slab) failed: %d", (int)r); return MV2_E_CUDA; }
-  }
-  {
-    const int64_t ntaps = (int64_t)a->kt * a->kh * a->kw, K = ntaps * a->C;
-    cuuint64_t dims[3] = {(cuuint64_t)a->C, (cuuint64_t)a->C, (cuuint64_t)ntaps};
-    cuuint64_t strides[2] = {(cuuint64_t)(K * 2), (cuuint64_t)(a->C * 2)};
-    cuuint32_t box[3] = {(cuuint32_t)bk, (cuuint32_t)p.bn, (cuuint32_t)p.tpw};
-    cuuint32_t es[3] = {1, 1, 1};
-    CUresult r = enc(&p.wmap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, (void*)a->w3, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(w3) failed: %d", (int)r); return MV2_E_CUDA; }
-    cuuint64_t dims2[2] = {(cuuint64_t)K, (cuuint64_t)a->C};
-    cuuint64_t strides2[1] = {(cuuint64_t)(K * 2)};
-    cuuint32_t box2[2] = {(cuuint32_t)bk, (cuuint32_t)p.bn};
-    cuuint32_t es2[2] = {1, 1};
-    r = enc(&p.wmap2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)a->w3, dims2, strides2, box2, es2, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(w3 2-D) failed: %d", (int)r); return MV2_E_CUDA; }
-    cuuint64_t dims1[2] = {(cuuint64_t)a->C, (cuuint64_t)a->C};
-    cuuint64_t strides1[1] = {(cuuint64_t)(a->C * 2)};
-    r = enc(&p.w1map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)a->w1, dims1, strides1, box2, es2, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(w1) failed: %d", (int)r); return MV2_E_CUDA; }
-  }
-  const cudaError_t attr_err = slab_set_smem_attr();
-  if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
-  const int grid = std::min(p.total_tiles, n_sm);
-  launch_k(slab_kernel_for(EPI_FUSED_RU, p.bn), dim3(grid), dim3(384), smem, (cudaStream_t)stream, p);
-  MV2_CHECK_LAUNCH();
-  return MV2_OK;
+  if (const int rc = ru_fill_plan(a, p)) return rc;
+  mv2_tc_conv_args c;
+  ru_as_conv_args(a, &c);
+  if (const int rc = slab_encode_maps(p, &c)) return rc;
+  const cuuint64_t dims1[2] = {(cuuint64_t)a->C, (cuuint64_t)a->C};
+  const cuuint64_t strides1[1] = {(cuuint64_t)a->C * 2};
+  const cuuint32_t box1[2] = {64, (cuuint32_t)p.bn};
+  if (const int rc = encode_bf16_map(&p.w1map, 2, a->w1, dims1, strides1, box1, CU_TENSOR_MAP_SWIZZLE_128B, "w1")) return rc;
+  return slab_launch(EPI_FUSED_RU, p, stream);
 }
 
 
@@ -1014,78 +876,47 @@ extern "C" int mv2_tc_down_space_supported(const mv2_tc_conv_args* a) {
 extern "C" int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream) {
   MV2_CHECK_ARG(a && a->x && a->w && a->y);
   if (!mv2_tc_down_space_supported(a)) { set_error("mv2_tc_down_space_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }
-  EncodeTiledFn enc = get_encode_fn();
-  if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return MV2_E_CUDA; }
-  int dev = 0, n_sm = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   SlabParams p;
   memset(&p, 0, sizeof(p));
   const int C2 = 2 * a->Ci, bk = 64;
   p.kt = 1; p.kh = 3; p.kw = 2; p.pt = 0; p.ph = 1; p.pw = 1; p.st = 1;
   p.row_bytes = 128; p.Ci = C2; p.kchunks = C2 / bk; p.dn_lower = a->Ci / bk;
   p.B = a->B; p.T = a->To; p.H = a->Ho; p.W = a->Wo; p.Co = a->Co;
-  p.epi.bias = a->bias; p.epi.res = nullptr; p.epi.y = (__nv_bfloat16*)a->y; p.epi.act = a->act; p.epi.shuffle = MV2_SHUFFLE_NONE;
-  p.epi.mode = 0; p.epi.Co = a->Co; p.epi.To = a->To; p.epi.Ho = a->Ho; p.epi.Wo = a->Wo; p.epi.out_cf = 0; p.epi.oscale = nullptr;
+  p.epi = tc_epi_of(a);
   int bn = 32;
   for (int c = 128; c >= 32; c >>= 1) if (a->Co % c == 0) { bn = c; break; }
-  int mw = (bn <= 64 && a->Wo > 8) ? 2 : 1;
-  if (bn == 32 && a->Wo > 16) mw = 4;
-  if (const char* env = getenv("MV2_DOWN_CFG")) {
-    int emw = 0, ebn = 0;
-    if (sscanf(env, "%d,%d", &emw, &ebn) == 2 && (emw == 1 || emw == 2 || emw == 4) && (ebn == 32 || ebn == 64 || ebn == 128) && a->Co % ebn == 0 && emw * ebn <= 128 && !(emw >= 2 && a->Wo <= 8)) { mw = emw; bn = ebn; }
-  }
   const int w_bytes = bn * 128;
   p.bn = bn; p.n_tiles_n = a->Co / bn; p.tpw = 1;
-  int o_bytes, e_bytes, budget;
-  for (;; mw >>= 1) {           // the two row-parity sub-slabs of a 4-M-tile macro tile do not fit twice: narrow the macro tile
-    p.mw = mw;
-    p.slab_stages = 3; p.w_stages = 12;      // upper bounds for the barrier table
-    budget = 227 * 1024 - 2048 - (int)slab_smem_layout(p, 0, false).end;
-    p.pitch = 8 * mw + 1;
-    o_bytes = 17 * p.pitch * 128; e_bytes = 16 * p.pitch * 128;
-    p.dn_e_off = (o_bytes + 1023) / 1024 * 1024;
-    p.slab_stride = p.dn_e_off + (e_bytes + 1023) / 1024 * 1024;
+  p.tiles_h = ceil_div(a->Ho, 16);
+  p.slab_h = 17;       // the odd-row sub-slab (input rows 2 ho - 1: 17 rows for 16 output rows) is an ordinary slab ...
+  int budget;
+  for (int mw = slab_default_mw(bn, a->Wo);; mw >>= 1) {   // the two sub-slabs of a wide macro tile do not fit twice: narrow it
+    slab_set_geometry(p, mw);
+    p.dn_e_off = p.slab_stride;    // ... and the 16-row even-row sub-slab follows it at the next 1024-byte boundary
+    const int e_bytes = 16 * p.pitch * 128;
+    p.slab_bytes += e_bytes;
+    p.slab_stride += (e_bytes + 1023) / 1024 * 1024;
+    budget = slab_ring_budget(p, false);
     if (mw == 1 || 2 * p.slab_stride + 3 * w_bytes <= budget) break;
   }
-  p.tiles_h = ceil_div(a->Ho, 16); p.tiles_w = ceil_div(a->Wo, 8 * mw);
-  p.total_tiles = (int)((int64_t)a->B * a->To * p.tiles_h * p.tiles_w * p.n_tiles_n);
-  p.slab_h = 17;
-  p.slab_bytes = o_bytes + e_bytes;
   for (int dh = 0; dh < 3; ++dh)
     for (int q = 0; q < 2; ++q)      // q = dw2 + 1
       p.dn_aoff[dh * 2 + q] = ((dh == 1 ? p.dn_e_off : 0) + ((dh == 2 ? p.pitch : 0) + q) * 128) >> 4;
   p.slab_stages = p.slab_stride * 3 + w_bytes * 4 <= budget ? 3 : 2;
   p.w_stages = std::min(12, (budget - p.slab_stages * p.slab_stride) / w_bytes);
   MV2_CHECK_ARG(p.w_stages >= 2);
-  {
-    const int64_t W2 = a->Wi / 2, H2 = a->Hi / 2, T = a->Ti, rowb = (int64_t)a->Wi * a->Ci * 2;
-    cuuint64_t dims[5] = {(cuuint64_t)C2, (cuuint64_t)W2, (cuuint64_t)H2, (cuuint64_t)T, (cuuint64_t)a->B};
-    cuuint64_t strides[4] = {(cuuint64_t)(C2 * 2), (cuuint64_t)(2 * rowb), (cuuint64_t)(a->Hi * rowb), (cuuint64_t)(T * a->Hi * rowb)};
-    cuuint32_t es[5] = {1, 1, 1, 1, 1};
-    cuuint32_t box_e[5] = {(cuuint32_t)bk, (cuuint32_t)p.pitch, 16, 1, 1}, box_o[5] = {(cuuint32_t)bk, (cuuint32_t)p.pitch, 17, 1, 1};
-    CUresult r = enc(&p.amap, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (void*)a->x, dims, strides, box_e, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(even rows) failed: %d", (int)r); return MV2_E_CUDA; }
-    r = enc(&p.amap_odd, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, (char*)a->x + rowb, dims, strides, box_o, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(odd rows) failed: %d", (int)r); return MV2_E_CUDA; }
-    const int64_t K = 6 * (int64_t)C2;
-    cuuint64_t dims2[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
-    cuuint64_t strides2[1] = {(cuuint64_t)(K * 2)};
-    cuuint32_t box2[2] = {(cuuint32_t)bk, (cuuint32_t)bn};
-    cuuint32_t es2[2] = {1, 1};
-    r = enc(&p.wmap2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, (void*)a->w, dims2, strides2, box2, es2, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(weights) failed: %d", (int)r); return MV2_E_CUDA; }
-    p.wmap = p.wmap2;
-  }
-  const size_t smem = 1024 + slab_smem_layout(p, (uint32_t)(p.slab_stages * p.slab_stride + p.w_stages * w_bytes), false).end;
-  MV2_CHECK_ARG(smem <= 227 * 1024);
-  const cudaError_t attr_err = slab_set_smem_attr();
-  if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
-  const int grid = std::min(p.total_tiles, n_sm);
-  launch_k(slab_kernel_for(EPI_DOWN_SPACE, p.bn), dim3(grid), dim3(384), smem, (cudaStream_t)stream, p);
-  MV2_CHECK_LAUNCH();
-  return MV2_OK;
+
+  const int64_t rowb = (int64_t)a->Wi * a->Ci * 2;
+  const cuuint64_t dims[5] = {(cuuint64_t)C2, (cuuint64_t)(a->Wi / 2), (cuuint64_t)(a->Hi / 2), (cuuint64_t)a->Ti, (cuuint64_t)a->B};
+  const cuuint64_t strides[4] = {(cuuint64_t)(C2 * 2), (cuuint64_t)(2 * rowb), (cuuint64_t)(a->Hi * rowb), (cuuint64_t)(a->Ti * a->Hi * rowb)};
+  const cuuint32_t box_e[5] = {(cuuint32_t)bk, (cuuint32_t)p.pitch, 16, 1, 1}, box_o[5] = {(cuuint32_t)bk, (cuuint32_t)p.pitch, 17, 1, 1};
+  if (const int rc = encode_bf16_map(&p.amap, 5, a->x, dims, strides, box_e, CU_TENSOR_MAP_SWIZZLE_128B, "even rows")) return rc;
+  if (const int rc = encode_bf16_map(&p.amap_odd, 5, (const char*)a->x + rowb, dims, strides, box_o, CU_TENSOR_MAP_SWIZZLE_128B, "odd rows")) return rc;
+  const int64_t K = 6 * (int64_t)C2;
+  const cuuint64_t wdims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
+  const cuuint64_t wstrides[1] = {(cuuint64_t)(K * 2)};
+  const cuuint32_t wbox[2] = {(cuuint32_t)bk, (cuuint32_t)bn};
+  if (const int rc = encode_bf16_map(&p.wmap2, 2, a->w, wdims, wstrides, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "weights")) return rc;
+  p.wmap = p.wmap2;
+  return slab_launch(EPI_DOWN_SPACE, p, stream);
 }

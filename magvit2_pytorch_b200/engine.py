@@ -174,10 +174,6 @@ class Engine:
         self.tc_variant = "auto"     # "auto" | "tap" (tc_conv.cu only) | "slab" (prefer tc_slab.cu)
         self.fuse_ru = True          # bf16: conv3x3x3 + ELU + conv1x1x1 + ELU + SE pool partials in one wgmma launch (C = 64 / 128)
         self.fused_ru_calls = 0
-        # bf16, small frames: SE pool + gate MLP + gate/residual in ONE launch (mv2_se_tail).  Off by default (an unmeasured
-        # default on this GPU): one CTA per frame leaves most of the SMs idle at the small frame counts of the README config
-        self.se_tail = False
-        self.se_tail_calls = 0
         self.fuse_conv_out = True    # bf16: conv_out stores torch's (B,C,T,H,W) directly and skips the time_padding frames
         self.tc_calls = 0
         self.slab_calls = 0
@@ -232,9 +228,6 @@ class Engine:
                 w2=f32(se.net[2].weight.reshape(C_, -1)), b2=f32(se.net[2].bias),
                 hidden=int(se.net[0].weight.shape[0]),
             )
-            if dt == torch.bfloat16:      # bf16 copies of the gate MLP for the one-launch SE tail (exact: the parameters are bf16)
-                P[key]["w1b"] = P[key]["w1"].to(torch.bfloat16).contiguous()
-                P[key]["w2b"] = P[key]["w2"].to(torch.bfloat16).contiguous()
 
         def pack_ffn(ff, key):
             P[key] = pack_feed_forward(ff, dt)
@@ -434,14 +427,6 @@ class Engine:
                 return out
         h = self.conv(x, c3, act=ACT_ELU)
         y = self.conv(h, c1, act=ACT_ELU)
-        if (self.dtype == torch.bfloat16 and self.se_tail and "w1b" in p
-                and self.lib.mv2_se_tail_supported(F_, Pn, Cc, p["hidden"])):
-            out = self._new(x.shape)
-            check(self.lib.mv2_se_tail(_ptr(y), _ptr(x), _ptr(out), F_, Pn, Cc, p["hidden"], _ptr(p["wk"]), p["bk"],
-                                       _ptr(p["w1b"]), _ptr(p["b1"]), _ptr(p["w2b"]), _ptr(p["b2"]), st), "mv2_se_tail")
-            self.launches += 1
-            self.se_tail_calls += 1
-            return out
         ws = self._new((self.lib.mv2_se_workspace_bytes(F_, Pn, Cc) // 4,), torch.float32)
         gates = self._new((F_, Cc), torch.float32)
         check(self.lib.mv2_se_pool(_ptr(y), dt, F_, Pn, Cc, _ptr(p["wk"]), p["bk"], _ptr(ws), st), "mv2_se_pool")
