@@ -127,7 +127,8 @@ int mv2_conv_forward(const mv2_conv_args* a, void* stream);
  *            done as chunk partials (online softmax) + a combine fused into se_gate.
  * se_gate  : gate[f,:] = sigmoid(W2 leaky_relu_0.1(W1 pooled + b1) + b2)   (fp32 [F][C])
  * gate_residual : out = gate[f(m), c] * y[m, c] + x[m, c]                    (M:240 + M:174)
- * workspace for se_pool: mv2_se_workspace_bytes(F, P, C).                                   */
+ * workspace for se_pool: mv2_se_workspace_bytes(F, P, C).  se_gate keeps its F * Hd hidden activations in the same
+ * workspace, which reserves F * (C + 16) floats for them: Hd <= C + 16, else MV2_E_ARG.                             */
 size_t mv2_se_workspace_bytes(int F, int P, int C);
 int mv2_se_pool(const void* y, int dtype, int F, int P, int C, const float* wk, float bk,
                 void* workspace, void* stream);
@@ -313,7 +314,8 @@ int mv2_tc_ru_records(const mv2_tc_ru_args* a);
 size_t mv2_tc_ru_workspace_bytes(const mv2_tc_ru_args* a);
 int mv2_tc_ru_forward(const mv2_tc_ru_args* a, void* stream);
 /* SE gate from pool records in the (max, sum, acc[C]) format, nrec records per frame laid out [F][nrec][C + 2], with the
- * hidden layer scratch (F * Hd floats) right behind them: gate[f,:] = sigmoid(W2 leaky_relu_0.1(W1 pooled + b1) + b2).   */
+ * hidden layer scratch (F * Hd floats) right behind them: gate[f,:] = sigmoid(W2 leaky_relu_0.1(W1 pooled + b1) + b2).
+ * mv2_tc_ru_workspace_bytes reserves F * (C + 16) floats for that scratch: Hd <= C + 16, else MV2_E_ARG.                  */
 int mv2_se_gate_records(const void* workspace, int nrec, int F, int C, int Hd,
                         const float* w1, const float* b1, const float* w2, const float* b2,
                         float* gates, void* stream);

@@ -2163,6 +2163,7 @@ int mv2_se_pool(const void* y, int dtype, int F, int P, int C, const float* wk, 
 int mv2_se_gate(const void* workspace, int dtype, int F, int P, int C, int Hd, const float* w1, const float* b1,
                 const float* w2, const float* b2, float* gates, void* stream) {
   MV2_CHECK_ARG(workspace && w1 && b1 && w2 && b2 && gates && F > 0 && P > 0 && C > 0 && Hd > 0);
+  MV2_CHECK_ARG(Hd <= C + 16);     // the hidden layer scratch mv2_se_workspace_bytes reserves: F * (C + 16) floats
   const int nc = ceil_div(P, se_rows_per_block(dtype, F, P, C));   // chunk records se_pool wrote per frame
   const size_t smem1 = (size_t)(C + nc + 256) * sizeof(float), smem2 = (size_t)Hd * sizeof(float);
   MV2_CHECK_ARG(smem1 <= 48 * 1024 && smem2 <= 48 * 1024);
@@ -2179,6 +2180,7 @@ int mv2_se_gate(const void* workspace, int dtype, int F, int P, int C, int Hd, c
 int mv2_se_gate_records(const void* workspace, int nrec, int F, int C, int Hd, const float* w1, const float* b1,
                         const float* w2, const float* b2, float* gates, void* stream) {
   MV2_CHECK_ARG(workspace && w1 && b1 && w2 && b2 && gates && F > 0 && nrec > 0 && C > 0 && Hd > 0);
+  MV2_CHECK_ARG(Hd <= C + 16);     // the hidden layer scratch mv2_tc_ru_workspace_bytes reserves: F * (C + 16) floats
   const size_t smem1 = (size_t)(C + nrec + 256) * sizeof(float), smem2 = (size_t)Hd * sizeof(float);
   MV2_CHECK_ARG(smem1 <= 48 * 1024 && smem2 <= 48 * 1024);
   float* hidden = (float*)workspace + (size_t)F * nrec * (C + 2);

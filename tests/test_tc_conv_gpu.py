@@ -239,10 +239,11 @@ def test_conv_in_kwpack_matches_cuda_core(variant):
     assert (a - b).abs().max().item() <= 0.008 * b.abs().max().item() + 1e-3
 
 
-@pytest.mark.parametrize("L,D,heads,nseq", [(256, 32, 8, 6), (100, 32, 4, 3), (1024, 32, 2, 2), (128, 64, 4, 2)])
+@pytest.mark.parametrize("L,D,heads,nseq", [(256, 32, 8, 6), (100, 32, 4, 3), (1024, 32, 2, 2), (128, 64, 4, 2),
+                                            (64, 32, 4, 2), (65, 64, 2, 3), (129, 32, 3, 2)])
 def test_attention_tensor_core_kernel_matches_fp32_cuda_core(L, D, heads, nseq):
     """bf16 mma.sync flash-attention kernel (space attention) vs the fp32 CUDA-core attention kernel on the same
-    (bf16-representable) inputs."""
+    (bf16-representable) inputs; L = 64 is the smallest sequence it takes, 65 and 129 leave a partial 128-query block."""
     import ctypes as C
     from magvit2_pytorch_b200 import _lib
     from magvit2_pytorch_b200._lib import AttnArgs, check
@@ -275,7 +276,7 @@ def test_attention_tensor_core_kernel_matches_fp32_cuda_core(L, D, heads, nseq):
     assert (a_.cpu() - o_).abs().mean().item() < 0.006 * o_.abs().mean().item() + 1e-3
 
 
-@pytest.mark.parametrize("L,heads,nseq", [(1024, 16, 3), (200, 4, 2), (4096, 2, 1)])
+@pytest.mark.parametrize("L,heads,nseq", [(1024, 16, 3), (200, 4, 2), (4096, 2, 1), (1, 4, 3), (257, 8, 2)])
 def test_linear_attention_tensor_core_kernels_match_fp32_cuda_core(L, heads, nseq):
     """bf16 mma.sync Taylor-linear-attention kernels vs the fp32 CUDA-core kernels on the same bf16-representable inputs."""
     import ctypes as C
@@ -477,11 +478,18 @@ def test_slab_space_downsample(Ci, Co, shape):
         _check_vs_oracle("slab_down_space", y_slab, _oracle_conv(w, bias, x, None, dict(stride=(1, 2, 2))))
 
 
-@pytest.mark.parametrize("T,HW,D,heads,causal", [(5, 64, 32, 8, 1), (1, 16, 32, 4, 1), (8, 24, 64, 2, 1), (3, 10, 32, 3, 0)])
-def test_attention_small_sequences_kernel(T, HW, D, heads, causal):
-    """Short-sequence attention kernel (time attention: one warp per (pixel, head), right-aligned causal mask over 4 memory
-    key/values + the frames so far, A:46-47 / A:123-129; masking off when L == 1, A:209-210) vs the fp32 general kernel and
-    the CPU oracle, with the strided token addressing of TimeAttention (M:456-464)."""
+@pytest.mark.parametrize("T,HW,D,heads,causal,n_mem", [
+    pytest.param(5, 64, 32, 8, 1, 4, id="5-64-32-8-1"), pytest.param(1, 16, 32, 4, 1, 4, id="1-16-32-4-1"),
+    pytest.param(8, 24, 64, 2, 1, 4, id="8-24-64-2-1"), pytest.param(3, 10, 32, 3, 0, 4, id="3-10-32-3-0"),
+    # more than 8 frames or memory slots, or dim_head 96: the general kernel (attention_kernel<bf16, D / 32>)
+    pytest.param(9, 16, 32, 4, 1, 0, id="9-16-32-4-1-nmem0"), pytest.param(33, 8, 64, 2, 1, 9, id="33-8-64-2-1-nmem9"),
+    pytest.param(5, 12, 96, 2, 1, 4, id="5-12-96-2-1"), pytest.param(9, 6, 96, 3, 1, 9, id="9-6-96-3-1-nmem9"),
+])
+def test_attention_small_sequences_kernel(T, HW, D, heads, causal, n_mem):
+    """Short-sequence attention kernel (time attention: one warp per (pixel, head), right-aligned causal mask over n_mem
+    memory key/values + the frames so far, A:46-47 / A:123-129; masking off when L == 1, A:209-210) vs the fp32 general
+    kernel and the CPU oracle, with the strided token addressing of TimeAttention (M:456-464).  Sequences the short kernel
+    cannot hold take the general kernel in bf16 as well."""
     import ctypes as C
     from magvit2_pytorch_b200 import _lib
     from magvit2_pytorch_b200._lib import AttnArgs, check
@@ -490,13 +498,15 @@ def test_attention_small_sequences_kernel(T, HW, D, heads, causal):
     g = torch.Generator(device="cpu").manual_seed(T * 10 + D)
     HDm = heads * D
     qkv = (torch.randn((B * T * HW, 3 * HDm), generator=g) * 1.2).to(torch.bfloat16).cuda()
-    mem = torch.randn((2, heads, 4, D), generator=g).to(torch.bfloat16).float().cuda()
+    mem = torch.randn((2, heads, n_mem, D), generator=g).to(torch.bfloat16).float().cuda()
+    mem_buf = mem if n_mem > 0 else torch.zeros(1, device="cuda")       # the library takes a non-null mem_kv pointer
     outs = {}
     for dt, code in ((torch.bfloat16, 1), (torch.float32, 0)):
         x = qkv.to(dt).contiguous()
         o = torch.zeros((B * T * HW, HDm), device="cuda", dtype=dt)
-        a = AttnArgs(qkv=x.data_ptr(), out=o.data_ptr(), mem_kv=mem.data_ptr(), dtype=code, heads=heads, dim_head=D, n_mem=4,
-                     causal=causal, n_outer=B, n_inner=HW, L=T, outer_stride=T * HW, inner_stride=1, tok_stride=HW)
+        a = AttnArgs(qkv=x.data_ptr(), out=o.data_ptr(), mem_kv=mem_buf.data_ptr(), dtype=code, heads=heads, dim_head=D,
+                     n_mem=n_mem, causal=causal, n_outer=B, n_inner=HW, L=T, outer_stride=T * HW, inner_stride=1,
+                     tok_stride=HW)
         check(lib.mv2_attention(C.byref(a), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "mv2_attention")
         outs[dt] = o.float().cpu()
     torch.cuda.synchronize()
