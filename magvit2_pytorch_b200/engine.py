@@ -160,6 +160,12 @@ def pack_conv_in_kwpack(weight, bias, cpack=32):
     return pk
 
 
+def param_signature(module):
+    """Identity of a module's parameter storage: changes on load_state_dict, .to(), optimizer steps and in-place edits."""
+    ps = list(module.parameters())
+    return (tuple((p.data_ptr(), p._version) for p in ps), ps[0].dtype, ps[0].device)
+
+
 class Engine:
     """Executes the inference path of one VideoTokenizer on its parameters' device/dtype."""
 
@@ -174,7 +180,6 @@ class Engine:
         self.tc_variant = "auto"     # "auto" | "tap" (tc_conv.cu only) | "slab" (prefer tc_slab.cu)
         self.fuse_ru = True          # bf16: conv3x3x3 + ELU + conv1x1x1 + ELU + SE pool partials in one wgmma launch (C = 64 / 128)
         self.fused_ru_calls = 0
-        self.fuse_conv_out = True    # bf16: conv_out stores torch's (B,C,T,H,W) directly and skips the time_padding frames
         self.tc_calls = 0
         self.slab_calls = 0
         self.simt_conv_calls = 0
@@ -183,20 +188,11 @@ class Engine:
         self.conv_log: Optional[list] = None  # when set, one shape record per tensor-core conv launch
 
     # ------------------------------------------------------------------ parameters
-    def _signature(self):
-        ps = list(self.model.parameters())
-        return (tuple((p.data_ptr(), p._version) for p in ps), ps[0].dtype, ps[0].device)
-
-    def prepare(self):
-        """(Re)pack parameters into kernel layouts when they changed (load_state_dict, .to(), ...)."""
-        sig = self._signature()
-        if sig == self._sig:
-            return
-        m = self.model
-        p0 = m.conv_in.conv.weight
+    def bind(self, p0: torch.Tensor, what: str):
+        """Runs on the device and in the dtype of parameter p0, after checking that they are an sm_90 CUDA device and
+        fp32 / bf16.  `what` names the model in the error messages."""
         if p0.device.type != "cuda":
-            raise RuntimeError("magvit2_pytorch_b200.VideoTokenizer runs on CUDA (sm_90a) only; "
-                               "move the model with .cuda() -- there is no CPU fallback")
+            raise RuntimeError(f"{what} runs on CUDA (sm_90a) only; move the model with .cuda() -- there is no CPU fallback")
         if p0.dtype not in (torch.float32, torch.bfloat16):
             raise TypeError("parameters must be float32 or bfloat16")
         arch = self.lib.mv2_device_arch()
@@ -204,6 +200,14 @@ class Engine:
             raise RuntimeError(f"libmagvit2_b200.so targets sm_90a (H100); device reports sm_{arch}")
         self.dtype = p0.dtype
         self.device = p0.device
+
+    def prepare(self):
+        """(Re)pack parameters into kernel layouts when they changed (load_state_dict, .to(), ...)."""
+        sig = param_signature(self.model)
+        if sig == self._sig:
+            return
+        m = self.model
+        self.bind(m.conv_in.conv.weight, "magvit2_pytorch_b200.VideoTokenizer")
         dt = self.dtype
         P: Dict[str, object] = {}
         P["conv_in"] = pack_conv(m.conv_in.conv.weight, m.conv_in.conv.bias, dt)
@@ -427,6 +431,14 @@ class Engine:
                 return out
         h = self.conv(x, c3, act=ACT_ELU)
         y = self.conv(h, c1, act=ACT_ELU)
+        return self.squeeze_excite_residual(y, x, p)
+
+    def squeeze_excite_residual(self, y, x, p):
+        """x + SqueezeExcite(y) (M:221-240) of an unfused ResidualUnit: softmax pool of y per frame, gate MLP, gated residual."""
+        B, T, H, W, Cc = x.shape
+        F_, Pn = B * T, H * W
+        st = self._stream()
+        dt = _dt(self.dtype)
         ws = self._new((self.lib.mv2_se_workspace_bytes(F_, Pn, Cc) // 4,), torch.float32)
         gates = self._new((F_, Cc), torch.float32)
         check(self.lib.mv2_se_pool(_ptr(y), dt, F_, Pn, Cc, _ptr(p["wk"]), p["bk"], _ptr(ws), st), "mv2_se_pool")
@@ -682,9 +694,9 @@ class Engine:
         return out[0]
 
     # ------------------------------------------------------------------ the path
-    def encode_cl(self, video: torch.Tensor, first_frame: bool = True, cond=None):
-        """video (B,C,T,H,W) on device -> encoder output, channels-last.  Reference encode M:1523-1576; the time_padding
-        zero frames are only prepended when the clip starts with a first frame (video_contains_first_frame, M:1534-1537)."""
+    def conv_in(self, video: torch.Tensor, first_frame: bool = True):
+        """video (B,C,T,H,W) on device -> conv_in's output (B,T+t_pad,H,W,C) channels-last.  The time_padding zero frames
+        are only prepended when the clip starts with a first frame (video_contains_first_frame, M:1534-1537)."""
         m = self.model
         t_pad = m.time_padding if first_frame else 0
         pin = self._packs.get("conv_in_tc")
@@ -707,6 +719,12 @@ class Engine:
         else:
             x = self.to_channels_last(video, t_pad)
             x = self.conv(x, self._packs["conv_in"])
+        return x
+
+    def encode_cl(self, video: torch.Tensor, first_frame: bool = True, cond=None):
+        """video (B,C,T,H,W) on device -> encoder output, channels-last.  Reference encode M:1523-1576."""
+        m = self.model
+        x = self.conv_in(video, first_frame)
         self._tap("conv_in", x)
         cond_e = self.cond_stem(cond, "enc") if (m.has_cond and cond is not None) else None     # M:1544-1548
         for i, st in enumerate(m.stages):
@@ -715,14 +733,19 @@ class Engine:
         return x
 
     def decode_cl(self, q: torch.Tensor, first_frame: bool = True, cond=None):
-        """quantized channels-last (B,T',H',W',C) -> video (B,3,T,H,W).  Reference decode M:1598-1649; the leading
-        time_padding frames are dropped only for clips that contain a first frame (M:1646-1647)."""
+        """quantized channels-last (B,T',H',W',C) -> video (B,3,T,H,W).  Reference decode M:1598-1649."""
         m = self.model
         x = q
         cond_e = self.cond_stem(cond, "dec") if (m.has_cond and cond is not None) else None     # M:1612-1616
         for j, st in enumerate(reversed(m.stages)):
             x = self._stage(x, st, f"dec{j}", decoder=True, cond_e=cond_e)
             self._tap(f"dec{j}", x)
+        return self.conv_out(x, first_frame)
+
+    def conv_out(self, x: torch.Tensor, first_frame: bool = True):
+        """decoder output (B,T,H,W,C) channels-last -> reconstruction (B,3,T-t_pad,H,W).  The leading time_padding frames
+        are dropped only for clips that contain a first frame (M:1646-1647)."""
+        m = self.model
         pk = self._packs["conv_out"]
         B, T, H, W, Cc = x.shape
         tp = m.time_padding if first_frame else 0
@@ -737,8 +760,8 @@ class Engine:
             return self.to_channels_first(out)
         if m.conv_out.pad_mode != "constant":
             return self.to_channels_first(self.causal_conv_padded(x, pk, m.conv_out.pad_mode), t_crop=tp)
-        if (self.dtype == torch.bfloat16 and self.use_tc and self.tc_variant != "tap" and self.fuse_conv_out and pk.w_tc is not None
-                and pk.Co % 8 != 0 and Cc % 64 == 0 and pk.k[2] <= 3 and T > tp):
+        if (self.dtype == torch.bfloat16 and self.use_tc and self.tc_variant != "tap" and pk.w_tc is not None and pk.Co % 8 != 0
+                and Cc % 64 == 0 and pk.k[2] <= 3 and T > tp):
             # conv_out writes the reconstruction in torch's (B,C,T,H,W) layout itself and never computes the time_padding
             # frames the reference drops afterwards (M:1642-1647)
             return self.conv(x, pk, pad=(pk.k[0] - 1 - tp, pk.k[1] // 2, pk.k[2] // 2), out_spatial=(T - tp, H, W), out_cf=True)

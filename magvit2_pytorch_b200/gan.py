@@ -27,8 +27,8 @@ import torch.nn.functional as F
 from torch.autograd.function import once_differentiable
 
 from ._lib import ACT_LEAKY_RELU, ACT_NONE, SHUFFLE_SPACE
-from .engine import Engine, pack_conv, pack_conv_in_kwpack, pack_feed_forward, pack_linear_attention
-from .train import TrainRunner, _feed_forward_block, _linear_attention_block
+from .engine import Engine, pack_conv, pack_conv_in_kwpack, pack_feed_forward, pack_linear_attention, param_signature
+from .train import TapeRunner, _feed_forward_block, _linear_attention_block
 
 # reference M:1039-1043
 DiscrLossBreakdown = namedtuple("DiscrLossBreakdown", ["discr_loss", "multiscale_discr_losses", "gradient_penalty"])
@@ -101,27 +101,14 @@ def gradient_penalty(d, images):
 # --------------------------------------------------------------------------------------------
 # device path
 # --------------------------------------------------------------------------------------------
-def _signature(d):
-    ps = list(d.parameters())
-    return (tuple((p.data_ptr(), p._version) for p in ps), ps[0].dtype, ps[0].device)
-
-
 def _packs(d):
     """(engine, packs) of the Discriminator, re-packed when its parameters changed."""
-    w0 = d.to_logits[0].weight
-    if w0.device.type != "cuda":
-        raise RuntimeError("the discriminator runs on CUDA (sm_90a) only; move the model with .cuda() -- there is no CPU fallback")
-    if w0.dtype not in (torch.float32, torch.bfloat16):
-        raise TypeError("parameters must be float32 or bfloat16")
-    sig = _signature(d)
+    sig = param_signature(d)
     if d._pack is not None and d._pack[0] == sig:
         return d._pack[1], d._pack[2]
     eng = d._pack[1] if d._pack is not None else Engine(None)
-    arch = eng.lib.mv2_device_arch()
-    if arch != 90:
-        raise RuntimeError(f"libmagvit2_b200.so targets sm_90a (H100); device reports sm_{arch}")
-    dt = w0.dtype
-    eng.dtype, eng.device = dt, w0.device
+    eng.bind(d.to_logits[0].weight, "the discriminator")
+    dt = eng.dtype
     P = []
     with torch.no_grad():
         for block, attn in d.blocks:
@@ -152,27 +139,13 @@ def _leaky_grad(g, y):
     return g * torch.where(y > 0, torch.ones_like(y), torch.full_like(y, 0.1))
 
 
-class DiscrRunner(TrainRunner):
+class DiscrRunner(TapeRunner):
     """One discriminator forward through the engine's kernels, recording what the backward needs."""
 
     def __init__(self, d):
+        eng, (self.P, self.logits_pk) = _packs(d)
+        super().__init__(eng)
         self.d = d
-        self.eng, (self.P, self.logits_pk) = _packs(d)
-        self.tape = []
-        self.grads = {}
-        self.own_dgrad = True
-        self.own_dgrad_calls = 0
-
-    def _wgrad(self, g, x, weight, bias, w5, stride, pad=(0, 0, 0)):
-        """Weight / bias gradients of a conv run as y = conv(x; w5, stride, pad) on channels-last tensors."""
-        if not (weight.requires_grad or (bias is not None and bias.requires_grad)):
-            return
-        _, gw, gb = torch.ops.aten.convolution_backward(
-            g.permute(0, 4, 1, 2, 3), x.permute(0, 4, 1, 2, 3), w5, [w5.shape[0]] if bias is not None else None, list(stride),
-            list(pad), [1, 1, 1], False, [0, 0, 0], 1, [False, weight.requires_grad, bias is not None and bias.requires_grad])
-        self._acc(weight, gw)
-        if bias is not None:
-            self._acc(bias, gb)
 
     def _dgrad_s2(self, g, wd, x_shape):
         """Data gradient of a stride-2 conv whose dgrad weights `wd` (4 Ci, Co, 1, 1) feed the depth-to-space store."""
@@ -205,9 +178,10 @@ class DiscrRunner(TrainRunner):
 
         def bwd(g):
             g = g * _RES_SCALE                     # d out / d (branch) for both branches
+            res_stride = (1, 2, 2) if down else (1, 1, 1)
             if down:
-                ds = block.downsample[1]
-                self._wgrad(g, h2, ds.weight, ds.bias, unshuffle_conv_weight(ds.weight)[:, :, None], (1, 2, 2))
+                ds = block.downsample[1]          # pixel-unshuffle + 1x1 conv as the 2x2 stride-2 conv (unshuffle_conv_weight)
+                self._wgrad(g, h2.permute(0, 4, 1, 2, 3), ds.weight, ds.bias, (1, 2, 2), (1, 2, 2), (0, 0, 0))
                 gz2 = _leaky_grad(self._dgrad_s2(g, unshuffle_dgrad_weight(ds.weight.detach()), h2.shape), h2)
             else:
                 gz2 = _leaky_grad(g, h2)
@@ -217,28 +191,19 @@ class DiscrRunner(TrainRunner):
                 v = images.to(eng.dtype)
                 # the first block's input is the images (channels-first): weight gradients on them, data gradients optional
                 self._conv_bwd(gz1, v[:, :, None], n0.weight, n0.bias, (1, 3, 3), pad=(0, 1, 1), need_gx=False, x_is_cf=True)
-                self._wgrad(g, x, cr.weight, cr.bias, cr.weight[:, :, None], (1, 2, 2) if down else (1, 1, 1))
+                self._wgrad(g, x.permute(0, 4, 1, 2, 3), cr.weight, cr.bias, (1, 1, 1), res_stride, (0, 0, 0))
                 if not need_gx:
                     return None
-                gx = self._conv_bwd_data(gz1, n0.weight, x.shape)
+                gx = self._dgrad(gz1, n0.weight, (1, 3, 3), x.shape[1:4])
             else:
                 gx = self._conv_bwd(gz1, x, n0.weight, n0.bias, (1, 3, 3))
-                self._wgrad(g, x, cr.weight, cr.bias, cr.weight[:, :, None], (1, 2, 2) if down else (1, 1, 1))
+                self._wgrad(g, x.permute(0, 4, 1, 2, 3), cr.weight, cr.bias, (1, 1, 1), res_stride, (0, 0, 0))
             if down:
                 return gx + self._dgrad_s2(g, stride2_1x1_dgrad_weight(cr.weight.detach()), x.shape)
-            return gx + self._conv_bwd_data(g, cr.weight, x.shape)
+            return gx + self._dgrad(g, cr.weight, (1, 1, 1), x.shape[1:4])
 
         self.tape.append(bwd)
         return out
-
-    def _conv_bwd_data(self, g, weight, x_shape):
-        """Data gradient of a stride-1 'same' conv (3x3 pad 1 or 1x1) on the engine's kernels."""
-        kh, kw = weight.shape[2:]
-        wt = weight.detach().reshape(weight.shape[0], weight.shape[1], 1, kh, kw).flip(2, 3, 4).transpose(0, 1).contiguous()
-        gx = self.eng.conv(g.contiguous(), pack_conv(wt, None, self.eng.dtype), pad=(0, kh // 2, kw // 2),
-                           out_spatial=tuple(x_shape[1:4]))
-        self.own_dgrad_calls += 1
-        return gx
 
     def forward(self, images, need_image_grad=False):
         """images (B, C, H, W) -> logits (B,) in the compute dtype."""
@@ -262,14 +227,10 @@ class DiscrRunner(TrainRunner):
         logits = eng.conv(h, self.logits_pk["lin"], pad=(0, 0, 0), out_spatial=(1, 1, 1), act=ACT_NONE)
 
         def bwd_logits(g):       # g: (B,) -> gradient wrt the last feature map (channels-last)
-            lin = tl[3]
-            w5 = logits_conv_weight(lin, h.shape[-1], d.last_fmap)[:, :, None]
+            lin = tl[3]          # the Linear as the conv covering the last feature map (logits_conv_weight)
             g5 = g.reshape(-1, 1, 1, 1, 1).to(h.dtype)
-            gh, gw, gb = torch.ops.aten.convolution_backward(
-                g5.permute(0, 4, 1, 2, 3), h.permute(0, 4, 1, 2, 3), w5.to(h.dtype), [1], [1, 1, 1], [0, 0, 0], [1, 1, 1], False,
-                [0, 0, 0], 1, [True, lin.weight.requires_grad, lin.bias.requires_grad])
-            self._acc(lin.weight, gw)
-            self._acc(lin.bias, gb)
+            gh = self._wgrad(g5, h.permute(0, 4, 1, 2, 3), lin.weight, lin.bias, (1,) + tuple(d.last_fmap), (1, 1, 1), (0, 0, 0),
+                             need_gx=True)
             gz = _leaky_grad(gh.permute(0, 2, 3, 4, 1).contiguous(), h)
             return self._conv_bwd(gz, xl, tl[0].weight, tl[0].bias, (1, 3, 3))
 

@@ -26,8 +26,8 @@ from typing import Callable, Dict, List, Sequence
 import torch
 import torch.nn.functional as F
 
-from ._lib import ACT_ELU, check
-from .engine import _dt, _ptr
+from ._lib import ACT_ELU
+from .engine import pack_conv
 
 
 # --------------------------------------------------------------------------------------------
@@ -216,18 +216,14 @@ def _elu_grad(g, y):
     return g * torch.where(y > 0, torch.ones_like(y), y + 1)
 
 
-class TrainRunner:
-    """One training-mode forward through the engine's kernels, recording what the backward needs."""
+class TapeRunner:
+    """A forward through the engine's kernels that records its backward on a tape, with the gradient pieces shared by the
+    generator's runner (TrainRunner) and the discriminator's (gan.DiscrRunner)."""
 
-    def __init__(self, model):
-        m = model
-        self.g_cond: Dict[str, torch.Tensor] = {}      # gradient wrt the cond stems' outputs, summed over the cond_residual stages
-        self.m = m
-        self.eng = m.engine
+    def __init__(self, eng):
+        self.eng = eng
         self.tape: List[Callable] = []
         self.grads: Dict[torch.nn.Parameter, torch.Tensor] = {}
-        self.codes = None
-        self.breakdown = None
         self.own_dgrad = True            # data gradient of the stride-1 convs through the engine's own conv kernels
         self.own_dgrad_calls = 0
 
@@ -254,45 +250,67 @@ class TrainRunner:
             return gs[0], gs[1 + len(params):]
         return gs[0]
 
+    # ---- conv gradients
+    def _dgrad(self, g, weight, k, out_spatial):
+        """Data gradient of a stride-1 conv with leading pad (kt - 1, kh // 2, kw // 2) on the engine's conv kernels: the
+        transposed conv is the same implicit GEMM with the weights flipped in (t, h, w) and transposed in (co, ci), and no
+        leading pad in time (gx[t] = sum_e W'[e] g[t + e]; frames past the clip are the kernels' out-of-bounds zeros).
+        g: (B,To,Ho,Wo,Co) channels-last; returns (B,*out_spatial,Ci) channels-last."""
+        kt, kh, kw = k
+        wt = weight.detach().reshape(weight.shape[0], -1, kt, kh, kw).flip(2, 3, 4).transpose(0, 1).contiguous()
+        self.own_dgrad_calls += 1
+        return self.eng.conv(g.contiguous(), pack_conv(wt, None, self.eng.dtype), pad=(0, kh // 2, kw // 2),
+                             out_spatial=tuple(out_spatial))
+
+    def _wgrad(self, g, x_cf, weight, bias, k, stride, pad, need_gx=False):
+        """aten.convolution_backward (cuDNN) of y = conv(x_cf; weight, stride, symmetric pad): accumulates the weight / bias
+        gradients and returns the data gradient (B,C,T,H,W) if need_gx.  g: (B,To,Ho,Wo,Co) channels-last."""
+        w_grad, b_grad = weight.requires_grad, bias is not None and bias.requires_grad
+        if not (need_gx or w_grad or b_grad):
+            return None
+        w5 = weight.reshape(weight.shape[0], -1, *k)
+        gx, gw, gb = torch.ops.aten.convolution_backward(
+            g.permute(0, 4, 1, 2, 3), x_cf, w5, [w5.shape[0]] if bias is not None else None, list(stride), list(pad), [1, 1, 1],
+            False, [0, 0, 0], 1, [need_gx, w_grad, b_grad])
+        self._acc(weight, gw)
+        if bias is not None:
+            self._acc(bias, gb)
+        return gx
+
     def _conv_bwd(self, g, x, weight, bias, k, stride=(1, 1, 1), pad=None, need_gx=True, x_is_cf=False):
         """Backward of a conv the engine ran as  y = conv(x; leading pad (pt, ph, pw), stride).
         g: (B,To,Ho,Wo,Co) channels-last grad of the pre-activation output; x: the saved channels-last input (or, x_is_cf,
         a (B,C,T,H,W) tensor).  Returns grad wrt x (channels-last) or None.
-          * data gradient of the stride-1 causal convs (every ResidualUnit conv, conv_out): OUR conv kernels -- the transposed
-            conv is the same implicit GEMM with the weights flipped in (t, h, w) and transposed in (co, ci), no leading pad in
-            time (gx[t] = sum_e W'[e] g[t + e]; frames past the clip are the kernels' out-of-bounds zeros);
-          * weight / bias gradients, and the data gradient of the strided down-samplers: aten.convolution_backward (cuDNN).  The
-            time axis is padded at the FRONT only (causal, M:913-928): those zero frames are materialised; H / W use the
-            symmetric padding natively."""
+          * data gradient of the stride-1 causal convs (every ResidualUnit conv, conv_out): _dgrad, on our conv kernels;
+          * weight / bias gradients, and the data gradient of the strided down-samplers: _wgrad (cuDNN).  The time axis is
+            padded at the FRONT only (causal, M:913-928): those zero frames are materialised; H / W use the symmetric padding
+            natively."""
         kt, kh, kw = k
         causal_default = pad is None
         if pad is None:
             pad = (kt - 1, kh // 2, kw // 2)
         pt, ph, pw = pad
-        w5 = weight.reshape(weight.shape[0], weight.shape[1], kt, kh, kw)
-        gx = None
         own_dgrad = need_gx and self.own_dgrad and causal_default and tuple(stride) == (1, 1, 1) and not x_is_cf
-        if own_dgrad:
-            from .engine import pack_conv
-            wt = w5.detach().flip(2, 3, 4).transpose(0, 1).contiguous()          # (Ci, Co, kt, kh, kw): dgrad weights
-            gx = self.eng.conv(g.contiguous(), pack_conv(wt, None, self.eng.dtype), pad=(0, ph, pw), out_spatial=tuple(x.shape[1:4]))
-            self.own_dgrad_calls += 1
+        gx = self._dgrad(g, weight, k, x.shape[1:4]) if own_dgrad else None
         if x_is_cf:
             x_cf = F.pad(x, (0, 0, 0, 0, pt, 0)) if pt > 0 else x
         else:       # pad the (contiguous) channels-last tensor along T, then view it as (B,C,T,H,W) in channels_last_3d strides
             x_cf = (F.pad(x, (0, 0, 0, 0, 0, 0, pt, 0)) if pt > 0 else x).permute(0, 4, 1, 2, 3)
-        lib_gx = need_gx and not own_dgrad
-        gxl, gw, gb = torch.ops.aten.convolution_backward(
-            g.permute(0, 4, 1, 2, 3), x_cf, w5, [w5.shape[0]] if bias is not None else None, list(stride), [0, ph, pw],
-            [1, 1, 1], False, [0, 0, 0], 1, [lib_gx, weight.requires_grad, bias is not None and bias.requires_grad])
-        self._acc(weight, gw)
-        if bias is not None:
-            self._acc(bias, gb)
-        if not need_gx:
-            return None
-        if own_dgrad:
+        gxl = self._wgrad(g, x_cf, weight, bias, k, stride, (0, ph, pw), need_gx=need_gx and not own_dgrad)
+        if not need_gx or own_dgrad:
             return gx
         return gxl[:, :, pt:].permute(0, 2, 3, 4, 1).contiguous()
+
+
+class TrainRunner(TapeRunner):
+    """One training-mode forward of the tokenizer through the engine's kernels, recording what the backward needs."""
+
+    def __init__(self, model):
+        super().__init__(model.engine)
+        self.m = model
+        self.g_cond: Dict[str, torch.Tensor] = {}      # gradient wrt the cond stems' outputs, summed over the cond_residual stages
+        self.codes = None
+        self.breakdown = None
 
     def _conv_bwd_padmode(self, g, x, weight, bias, k, pad_mode, need_gx=True):
         """Backward of Engine.causal_conv_padded (CausalConv3d with pad_mode reflect / replicate / circular, M:925-927): the padding
@@ -304,13 +322,7 @@ class TrainRunner:
         x_ = x.detach().permute(0, 4, 1, 2, 3).requires_grad_(need_gx)
         with torch.enable_grad():
             xp = F.pad(x_, (kw // 2, kw // 2, kh // 2, kh // 2, kt - 1, 0), mode=pad_mode)
-        w5 = weight.reshape(weight.shape[0], weight.shape[1], kt, kh, kw)
-        gxp, gw, gb = torch.ops.aten.convolution_backward(
-            g.permute(0, 4, 1, 2, 3), xp.detach(), w5, [w5.shape[0]] if bias is not None else None, [1, 1, 1], [0, 0, 0], [1, 1, 1],
-            False, [0, 0, 0], 1, [need_gx, weight.requires_grad, bias is not None and bias.requires_grad])
-        self._acc(weight, gw)
-        if bias is not None:
-            self._acc(bias, gb)
+        gxp = self._wgrad(g, xp.detach(), weight, bias, k, (1, 1, 1), (0, 0, 0), need_gx=need_gx)
         if not need_gx:
             return None
         gx, = torch.autograd.grad(xp, x_, gxp)
@@ -318,23 +330,13 @@ class TrainRunner:
 
     # ---- forward pieces (engine kernels) that record their backward
     def _residual_unit(self, x, p, ru):
-        """ResidualUnit (M:930-944) unfused: both conv outputs and the SE gates are kept for the backward."""
-        eng, lib = self.eng, self.eng.lib
+        """ResidualUnit (M:930-944) unfused: both conv outputs are kept for the backward."""
+        eng = self.eng
         seq = ru.fn
         c3m, c1m, se = seq[0].conv, seq[2], seq[4]
-        B, T, H, W, Cc = x.shape
-        F_, Pn = B * T, H * W
-        st, dt = eng._stream(), _dt(eng.dtype)
         h = eng.conv(x, p["conv3"], act=ACT_ELU)
         y = eng.conv(h, p["conv1"], act=ACT_ELU)
-        ws = eng._new((lib.mv2_se_workspace_bytes(F_, Pn, Cc) // 4,), torch.float32)
-        gates = eng._new((F_, Cc), torch.float32)
-        check(lib.mv2_se_pool(_ptr(y), dt, F_, Pn, Cc, _ptr(p["wk"]), p["bk"], _ptr(ws), st), "mv2_se_pool")
-        check(lib.mv2_se_gate(_ptr(ws), dt, F_, Pn, Cc, p["hidden"], _ptr(p["w1"]), _ptr(p["b1"]), _ptr(p["w2"]), _ptr(p["b2"]),
-                              _ptr(gates), st), "mv2_se_gate")
-        out = eng._new(x.shape)
-        check(lib.mv2_gate_residual(_ptr(y), _ptr(x), _ptr(gates), _ptr(out), dt, F_, Pn, Cc, st), "mv2_gate_residual")
-        eng.launches += 3
+        out = eng.squeeze_excite_residual(y, x, p)
         k3 = tuple(c3m.weight.shape[2:])
 
         def bwd(g):
@@ -414,37 +416,19 @@ class TrainRunner:
         """-> (recon (B,C,T,H,W), aux_loss 0-d fp32); codes / the LFQ breakdown are left in .codes / .breakdown."""
         from .dist import LfqBatchEntropy
         m, eng = self.m, self.eng
-        P = eng._packs
         self.cond = cond
         ce_enc = eng.cond_stem(cond, "enc") if m.has_cond else None            # M:1544-1548 (Linear + SiLU stems)
         ce_dec = eng.cond_stem(cond, "dec") if m.has_cond else None            # M:1612-1616
         t_pad = m.time_padding if first_frame else 0
         cin, cout = m.conv_in.conv, m.conv_out.conv
         kin = tuple(cin.weight.shape[2:])
-        pin = P.get("conv_in_tc")
         sff = bool(m.separate_first_frame_encoding and first_frame)
         mode_in, mode_out = m.conv_in.pad_mode, m.conv_out.pad_mode
         vid = video
-        if sff:
-            # M:1553-1561: the first frame through its own 2-D conv, frames 1.. through the causal conv_in on their own
-            Bv, _, Tv, Hv, Wv = video.shape
-            v_cl = eng.to_channels_last(video, 0)
-            first = eng.conv(eng.copy_frames(v_cl, 0, 1), P["conv_in_ff"])
-            x = eng._new((Bv, Tv + t_pad, Hv, Wv, first.shape[-1]))
-            eng.copy_frames(first, 0, 1, dst=x, dst_t0=t_pad, zero_front=True)
-            rest_in = eng.copy_frames(v_cl, 1, Tv - 1) if Tv > 1 else None
-            if Tv > 1:
-                rest = eng.causal_conv_padded(rest_in, P["conv_in"], mode_in)
-                eng.copy_frames(rest, 0, Tv - 1, dst=x, dst_t0=t_pad + 1)
-        elif mode_in != "constant":
-            padded_in = eng.to_channels_last(video, t_pad)               # time_padding zero frames first (M:1537), then the mode's pad
-            x = eng.causal_conv_padded(padded_in, P["conv_in"], mode_in)
-        elif eng.dtype == torch.bfloat16 and eng.use_tc and pin is not None:
-            x = eng.conv(eng.ingest_kwpack(video, t_pad, pin), pin, pad=(pin.k_tc[0] - 1, pin.k_tc[1] // 2, 0))
-        else:
-            x = eng.conv(eng.to_channels_last(video, t_pad), P["conv_in"])
+        x = eng.conv_in(video, first_frame)
 
         def bwd_conv_in(g):     # the video needs no gradient: weight / bias only
+            # the causal conv_in's input in the pad modes: channels-last, from the same layout kernel as in the forward
             v = (vid.float() / 255. if vid.dtype == torch.uint8 else vid).to(eng.dtype)
             if sff:
                 ff = m.conv_in_first_frame
@@ -452,10 +436,11 @@ class TrainRunner:
                 self._conv_bwd(g[:, t_pad:t_pad + 1].contiguous(), v[:, :, 0:1], ff.weight, ff.bias, kff, pad=(0, kff[1] // 2, kff[2] // 2),
                                need_gx=False, x_is_cf=True)
                 if v.shape[2] > 1:
-                    self._conv_bwd_padmode(g[:, t_pad + 1:].contiguous(), rest_in, cin.weight, cin.bias, kin, mode_in, need_gx=False)
+                    self._conv_bwd_padmode(g[:, t_pad + 1:].contiguous(), eng.to_channels_last(vid[:, :, 1:]), cin.weight, cin.bias, kin,
+                                           mode_in, need_gx=False)
                 return None
             if mode_in != "constant":
-                self._conv_bwd_padmode(g, padded_in, cin.weight, cin.bias, kin, mode_in, need_gx=False)
+                self._conv_bwd_padmode(g, eng.to_channels_last(vid, t_pad), cin.weight, cin.bias, kin, mode_in, need_gx=False)
                 return None
             self._conv_bwd(g, v, cin.weight, cin.bias, kin, pad=(t_pad + kin[0] - 1, kin[1] // 2, kin[2] // 2),
                            need_gx=False, x_is_cf=True)
@@ -490,19 +475,7 @@ class TrainRunner:
             x = self._stage(x, st, f"dec{j}", m.decoder_layers[j], decoder=True, cond_e=ce_dec)
         xo = x
         kout = tuple(cout.weight.shape[2:])
-        if sff:
-            # M:1633-1639: conv_out_first_frame on frame t_pad, the causal conv_out on the frames after it, re-attached
-            Bx, Tx, Hx, Wx, _ = x.shape
-            first = eng.conv(eng.copy_frames(x, t_pad, 1), P["conv_out_ff"])
-            y = eng._new((Bx, Tx - t_pad, Hx, Wx, first.shape[-1]))
-            eng.copy_frames(first, 0, 1, dst=y, dst_t0=0)
-            rest_out = eng.copy_frames(x, t_pad + 1, Tx - t_pad - 1) if Tx - t_pad > 1 else None
-            if Tx - t_pad > 1:
-                eng.copy_frames(eng.causal_conv_padded(rest_out, P["conv_out"], mode_out), 0, Tx - t_pad - 1, dst=y, dst_t0=1)
-            recon = eng.to_channels_first(y)
-        else:
-            y = eng.causal_conv_padded(x, P["conv_out"], mode_out)
-            recon = eng.to_channels_first(y, t_crop=t_pad)
+        recon = eng.conv_out(xo, first_frame)
 
         def bwd_conv_out(g_recon):    # (B,C,T,H,W) -> channels-last with zero gradient on the cropped time_padding frames
             g = g_recon.permute(0, 2, 3, 4, 1)
@@ -513,7 +486,8 @@ class TrainRunner:
                 gx[:, t_pad:t_pad + 1] = self._conv_bwd(g[:, 0:1].contiguous(), xo[:, t_pad:t_pad + 1].contiguous(), off.weight, off.bias, kff,
                                                         pad=(0, kff[1] // 2, kff[2] // 2))
                 if xo.shape[1] - t_pad > 1:
-                    gx[:, t_pad + 1:] = self._conv_bwd_padmode(g[:, 1:].contiguous(), rest_out, cout.weight, cout.bias, kout, mode_out)
+                    gx[:, t_pad + 1:] = self._conv_bwd_padmode(g[:, 1:].contiguous(), xo[:, t_pad + 1:].contiguous(), cout.weight, cout.bias,
+                                                               kout, mode_out)
                 return gx
             if t_pad:
                 g = F.pad(g, (0, 0, 0, 0, 0, 0, t_pad, 0))
