@@ -39,7 +39,8 @@ extern "C" {
 enum { MV2_F32 = 0, MV2_BF16 = 1,
        MV2_U8 = 2   /* source dtype of the two layout-in entry points only: decoded uint8 frames, normalised x / 255 */ };
 enum { MV2_ACT_NONE = 0, MV2_ACT_ELU = 1, MV2_ACT_SILU = 2,
-       MV2_ACT_LEAKY_RELU = 3   /* LeakyReLU(0.1), the discriminator's activation (M:117-118) */ };
+       MV2_ACT_LEAKY_RELU = 3,  /* LeakyReLU(0.1), the discriminator's activation (M:117-118) */
+       MV2_ACT_RELU = 4         /* ReLU, the activation of a VGG feature extractor (perceptual loss, M:1397-1405) */ };
 enum { MV2_SHUFFLE_NONE = 0, MV2_SHUFFLE_SPACE = 1, MV2_SHUFFLE_TIME = 2 };
 enum {
   MV2_OK = 0,
@@ -221,6 +222,15 @@ int mv2_gateloop_scan(const void* qkva, const void* res, void* out, int dtype, i
  * Deterministic (fixed-order two-stage reduction); workspace: mv2_mse_workspace_bytes() bytes.                          */
 int mv2_mse(const void* a, int a_dtype, const void* b, int b_dtype, int64_t n, void* workspace, float* out, void* stream);
 size_t mv2_mse_workspace_bytes(void);
+
+/* ---- 2x2 max-pool of a VGG feature extractor (nn.MaxPool2d(2, 2), floor mode) over channels-last maps ------------------
+ * mv2_maxpool2x2         : x (N, H, W, C) -> y (N, H/2, W/2, C), y = max of each 2x2 window (NaN propagates, as in torch).
+ * mv2_maxpool2x2_backward: gy (N, H/2, W/2, C) and the saved pool input x (N, H, W, C), the output of a conv with ReLU in its
+ *   epilogue -> gx (N, H, W, C), dense: each window's gradient goes to its first maximum in row-major order (torch's tie
+ *   rule) and is masked by x > 0 (the ReLU's gradient); every other element, including the row / column that floor mode
+ *   drops for odd H / W, is zero.  Windows do not overlap: no atomics.  dtype MV2_F32 or MV2_BF16.                      */
+int mv2_maxpool2x2(const void* x, void* y, int dtype, int N, int H, int W, int C, void* stream);
+int mv2_maxpool2x2_backward(const void* gy, const void* x, void* gx, int dtype, int N, int H, int W, int C, void* stream);
 
 /* ---- wgmma / TMA implicit-GEMM convolution (bf16 in, fp32 accumulate in registers) ------------
  * Same operator family and epilogue as mv2_conv_forward, for bf16 activations, executed on the

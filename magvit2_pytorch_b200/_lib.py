@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MV2_LIB_PATH") or os.path.join(_HERE, "libmagvit2_b200.so")   # env override: A/B builds
 
 MV2_F32, MV2_BF16, MV2_U8 = 0, 1, 2
-ACT_NONE, ACT_ELU, ACT_SILU, ACT_LEAKY_RELU = 0, 1, 2, 3
+ACT_NONE, ACT_ELU, ACT_SILU, ACT_LEAKY_RELU, ACT_RELU = 0, 1, 2, 3, 4
 SHUFFLE_NONE, SHUFFLE_SPACE, SHUFFLE_TIME = 0, 1, 2
 
 
@@ -100,6 +100,8 @@ SIGNATURES = {
     "mv2_gateloop_scan": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
     "mv2_mse": (_I, [_VP, _I, _VP, _I, _I64, _VP, _VP, _VP]),
     "mv2_mse_workspace_bytes": (C.c_size_t, []),
+    "mv2_maxpool2x2": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
+    "mv2_maxpool2x2_backward": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
     "mv2_tc_conv_supported": (_I, [C.POINTER(TcConvArgs)]),
     "mv2_tc_conv_forward": (_I, [C.POINTER(TcConvArgs), _VP]),
     "mv2_tc_slab_supported": (_I, [C.POINTER(TcConvArgs)]),

@@ -57,6 +57,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   if (act == MV2_ACT_ELU) return act_elu(v);
   if (act == MV2_ACT_SILU) return act_silu(v);
   if (act == MV2_ACT_LEAKY_RELU) return v > 0.f ? v : 0.1f * v;
+  if (act == MV2_ACT_RELU) return v < 0.f ? 0.f : v;     // NaN passes, as torch.relu
   return v;
 }
 

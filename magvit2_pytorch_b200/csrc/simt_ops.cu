@@ -1996,6 +1996,102 @@ __global__ void __launch_bounds__(256) lfq_aux_final_kernel(const float* __restr
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// 2x2 max-pool of a VGG feature extractor (nn.MaxPool2d(2, 2), floor mode), channels-last, VEC channels per thread
+// ------------------------------------------------------------------------------------------
+template <typename T, int VEC>
+struct alignas(sizeof(T) * VEC) VecT { T v[VEC]; };
+
+// torch's rule (max_pool2d): a later element replaces the running maximum only when strictly larger or NaN, so ties go to
+// the first element in row-major window order and a NaN, once taken, stays
+__device__ __forceinline__ bool pool_takes(float v, float m) { return v > m || isnan(v); }
+
+template <typename T, int VEC>
+__global__ void __launch_bounds__(256) maxpool2x2_kernel(const T* __restrict__ x, T* __restrict__ y, int N, int H, int W, int C) {
+  pdl_wait();
+  pdl_launch_dependents();
+  using V = VecT<T, VEC>;
+  const int Ho = H >> 1, Wo = W >> 1, Cv = C / VEC;
+  const int64_t total = (int64_t)N * Ho * Wo * Cv;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    int64_t r = i;
+    const int cv = (int)(r % Cv); r /= Cv;
+    const int wo = (int)(r % Wo); r /= Wo;
+    const int ho = (int)(r % Ho);
+    const int64_t n = r / Ho;
+    const int64_t p0 = ((n * H + 2 * ho) * W + 2 * wo) * C + (int64_t)cv * VEC, row = (int64_t)W * C;
+    const int64_t off[4] = {p0, p0 + C, p0 + row, p0 + row + C};
+    float m[VEC];
+    {
+      const V a = *reinterpret_cast<const V*>(x + off[0]);
+#pragma unroll
+      for (int q = 0; q < VEC; ++q) m[q] = to_f32<T>(a.v[q]);
+    }
+#pragma unroll
+    for (int k = 1; k < 4; ++k) {
+      const V a = *reinterpret_cast<const V*>(x + off[k]);
+#pragma unroll
+      for (int q = 0; q < VEC; ++q) {
+        const float v = to_f32<T>(a.v[q]);
+        if (pool_takes(v, m[q])) m[q] = v;
+      }
+    }
+    V o;
+#pragma unroll
+    for (int q = 0; q < VEC; ++q) o.v[q] = from_f32<T>(m[q]);      // exact: m is one of the inputs
+    *reinterpret_cast<V*>(y + ((n * Ho + ho) * Wo + wo) * C + (int64_t)cv * VEC) = o;
+  }
+}
+
+// one thread per (window, VEC channels) over ceil(H/2) x ceil(W/2) windows: the windows past the floor-mode output (odd H / W)
+// only write zeros, so gx is written densely without a separate memset
+template <typename T, int VEC>
+__global__ void __launch_bounds__(256) maxpool2x2_backward_kernel(const T* __restrict__ gy, const T* __restrict__ x, T* __restrict__ gx,
+                                                                  int N, int H, int W, int C) {
+  pdl_wait();
+  pdl_launch_dependents();
+  using V = VecT<T, VEC>;
+  const int Ho = H >> 1, Wo = W >> 1, Hw = (H + 1) >> 1, Ww = (W + 1) >> 1, Cv = C / VEC;
+  const int64_t total = (int64_t)N * Hw * Ww * Cv;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    int64_t r = i;
+    const int cv = (int)(r % Cv); r /= Cv;
+    const int ww = (int)(r % Ww); r /= Ww;
+    const int hh = (int)(r % Hw);
+    const int64_t n = r / Hw;
+    const bool pooled = hh < Ho && ww < Wo;
+    const int64_t p0 = ((n * H + 2 * hh) * W + 2 * ww) * C + (int64_t)cv * VEC, row = (int64_t)W * C;
+    const int64_t off[4] = {p0, p0 + C, p0 + row, p0 + row + C};
+    float g[VEC];
+    int arg[VEC];
+#pragma unroll
+    for (int q = 0; q < VEC; ++q) { g[q] = 0.f; arg[q] = -1; }
+    if (pooled) {
+      const V gv = *reinterpret_cast<const V*>(gy + ((n * Ho + hh) * Wo + ww) * C + (int64_t)cv * VEC);
+      float m[VEC] = {};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const V a = *reinterpret_cast<const V*>(x + off[k]);
+#pragma unroll
+        for (int q = 0; q < VEC; ++q) {
+          const float v = to_f32<T>(a.v[q]);
+          if (k == 0 || pool_takes(v, m[q])) { m[q] = v; arg[q] = k; }
+        }
+      }
+#pragma unroll
+      for (int q = 0; q < VEC; ++q) g[q] = m[q] <= 0.f ? 0.f : to_f32<T>(gv.v[q]);   // ReLU mask of the pooled conv (torch's threshold_backward)
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (2 * hh + (k >> 1) >= H || 2 * ww + (k & 1) >= W) continue;
+      V o;
+#pragma unroll
+      for (int q = 0; q < VEC; ++q) o.v[q] = from_f32<T>(arg[q] == k ? g[q] : 0.f);
+      *reinterpret_cast<V*>(gx + off[k]) = o;
+    }
+  }
+}
+
 }  // namespace mv2
 
 // ==========================================================================================
@@ -2496,6 +2592,52 @@ int mv2_gateloop_scan(const void* qkva, const void* res, void* out, int dtype, i
   else if (dtype == MV2_BF16)
     launch_k(gateloop_scan_kernel<__nv_bfloat16>, dim3((unsigned)blocks), dim3(256), 0, st, (const __nv_bfloat16*)qkva, (const __nv_bfloat16*)res, (__nv_bfloat16*)out, T, (int64_t)P * C, C, total);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
+  MV2_CHECK_LAUNCH();
+  return MV2_OK;
+}
+
+// 16-byte vectors over C when every pointer and the channel count allow them, else one channel per thread
+static bool pool_vec_ok(int C, int vec, std::initializer_list<const void*> ps) {
+  if (C % vec != 0) return false;
+  for (const void* p : ps)
+    if ((uintptr_t)p % 16 != 0) return false;
+  return true;
+}
+
+int mv2_maxpool2x2(const void* x, void* y, int dtype, int N, int H, int W, int C, void* stream) {
+  MV2_CHECK_ARG(x && y && N > 0 && H >= 2 && W >= 2 && C > 0);
+  const int vec = dtype == MV2_BF16 ? 8 : 4;
+  const bool v = pool_vec_ok(C, vec, {x, y});
+  const int64_t total = (int64_t)N * (H / 2) * (W / 2) * (v ? C / vec : C);
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, grid_cap(32));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == MV2_F32) {
+    if (v) launch_k(maxpool2x2_kernel<float, 4>, dim3(blocks), dim3(256), 0, st, (const float*)x, (float*)y, N, H, W, C);
+    else launch_k(maxpool2x2_kernel<float, 1>, dim3(blocks), dim3(256), 0, st, (const float*)x, (float*)y, N, H, W, C);
+  } else if (dtype == MV2_BF16) {
+    using B16 = __nv_bfloat16;
+    if (v) launch_k(maxpool2x2_kernel<B16, 8>, dim3(blocks), dim3(256), 0, st, (const B16*)x, (B16*)y, N, H, W, C);
+    else launch_k(maxpool2x2_kernel<B16, 1>, dim3(blocks), dim3(256), 0, st, (const B16*)x, (B16*)y, N, H, W, C);
+  } else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
+  MV2_CHECK_LAUNCH();
+  return MV2_OK;
+}
+
+int mv2_maxpool2x2_backward(const void* gy, const void* x, void* gx, int dtype, int N, int H, int W, int C, void* stream) {
+  MV2_CHECK_ARG(gy && x && gx && N > 0 && H >= 2 && W >= 2 && C > 0);
+  const int vec = dtype == MV2_BF16 ? 8 : 4;
+  const bool v = pool_vec_ok(C, vec, {gy, x, gx});
+  const int64_t total = (int64_t)N * ((H + 1) / 2) * ((W + 1) / 2) * (v ? C / vec : C);
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, grid_cap(32));
+  cudaStream_t st = (cudaStream_t)stream;
+  if (dtype == MV2_F32) {
+    if (v) launch_k(maxpool2x2_backward_kernel<float, 4>, dim3(blocks), dim3(256), 0, st, (const float*)gy, (const float*)x, (float*)gx, N, H, W, C);
+    else launch_k(maxpool2x2_backward_kernel<float, 1>, dim3(blocks), dim3(256), 0, st, (const float*)gy, (const float*)x, (float*)gx, N, H, W, C);
+  } else if (dtype == MV2_BF16) {
+    using B16 = __nv_bfloat16;
+    if (v) launch_k(maxpool2x2_backward_kernel<B16, 8>, dim3(blocks), dim3(256), 0, st, (const B16*)gy, (const B16*)x, (B16*)gx, N, H, W, C);
+    else launch_k(maxpool2x2_backward_kernel<B16, 1>, dim3(blocks), dim3(256), 0, st, (const B16*)gy, (const B16*)x, (B16*)gx, N, H, W, C);
+  } else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }

@@ -210,14 +210,15 @@ __device__ __forceinline__ float gelu_fast(float g) {
   return fmaf(-ag, q, fmaxf(g, 0.f));
 }
 
+// ReLU shares the LeakyReLU instantiation (a runtime flag), so the epilogues carry no extra code path
 template <int ACT>
-__device__ __forceinline__ float act_ct(float x) {
+__device__ __forceinline__ float act_ct(float x, bool relu = false) {
   if (ACT == MV2_ACT_ELU) {
     const float e = ex2_approx(x * 1.4426950408889634f) - 1.f;
     return x > 0.f ? x : e;
   }
   if (ACT == MV2_ACT_SILU) return x * rcp_approx(1.f + ex2_approx(-1.4426950408889634f * x));
-  if (ACT == MV2_ACT_LEAKY_RELU) return x > 0.f ? x : 0.1f * x;
+  if (ACT == MV2_ACT_LEAKY_RELU) return x > 0.f ? x : (relu ? 0.f * x : 0.1f * x);   // ReLU: NaN * 0 passes NaN, as torch
   return x;
 }
 
@@ -226,7 +227,7 @@ __device__ __forceinline__ float act_ct(float x) {
 // row_base = linear position index * Co (plain mode), computed once per row by the caller.
 template <int MODE, int ACT>
 __device__ __forceinline__ void epi_chunk32_t(const TcEpi& e, const uint32_t (&r)[32], int ncols, int n, const float* sb,
-                                              int b, int to, int ho, int wo, int64_t row_base) {
+                                              int b, int to, int ho, int wo, int64_t row_base, bool relu = false) {
   if (MODE == EPI_GEGLU) {
     const int I = e.Co >> 1;
     const int64_t pos = (((int64_t)b * e.To + to) * e.Ho + ho) * e.Wo + wo;
@@ -258,11 +259,11 @@ __device__ __forceinline__ void epi_chunk32_t(const TcEpi& e, const uint32_t (&r
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
           const float os = ng + q < e.Co ? e.oscale[(int64_t)b * e.Co + ng + q] : 0.f;
-          v[q] = act_ct<ACT>(__uint_as_float(r[g * 8 + q]) * os + bb[q]);
+          v[q] = act_ct<ACT>(__uint_as_float(r[g * 8 + q]) * os + bb[q], relu);
         }
       } else
 #pragma unroll
-      for (int q = 0; q < 8; ++q) v[q] = act_ct<ACT>(__uint_as_float(r[g * 8 + q]) + bb[q]);
+      for (int q = 0; q < 8; ++q) v[q] = act_ct<ACT>(__uint_as_float(r[g * 8 + q]) + bb[q], relu);
     }
     int64_t off;
     if (MODE == EPI_SHUFFLE) {
@@ -306,36 +307,36 @@ __device__ __forceinline__ void epi_chunk32_t(const TcEpi& e, const uint32_t (&r
 
 // bias + activation + bf16 packing of one 32-column chunk (row-per-lane), for the staged epilogue
 template <int ACT>
-__device__ __forceinline__ void epi_pack32_t(const uint32_t (&r)[32], const float* sb, uint32_t (&pk)[16]) {
+__device__ __forceinline__ void epi_pack32_t(const uint32_t (&r)[32], const float* sb, uint32_t (&pk)[16], bool relu = false) {
 #pragma unroll
   for (int g = 0; g < 8; ++g) {
     const float4 b = *reinterpret_cast<const float4*>(sb + g * 4);
-    pk[2 * g] = pack_bf16x2(act_ct<ACT>(__uint_as_float(r[4 * g]) + b.x), act_ct<ACT>(__uint_as_float(r[4 * g + 1]) + b.y));
-    pk[2 * g + 1] = pack_bf16x2(act_ct<ACT>(__uint_as_float(r[4 * g + 2]) + b.z), act_ct<ACT>(__uint_as_float(r[4 * g + 3]) + b.w));
+    pk[2 * g] = pack_bf16x2(act_ct<ACT>(__uint_as_float(r[4 * g]) + b.x, relu), act_ct<ACT>(__uint_as_float(r[4 * g + 1]) + b.y, relu));
+    pk[2 * g + 1] = pack_bf16x2(act_ct<ACT>(__uint_as_float(r[4 * g + 2]) + b.z, relu), act_ct<ACT>(__uint_as_float(r[4 * g + 3]) + b.w, relu));
   }
 }
 // bias + activation of one 32-column chunk, kept in fp32 (for the fp32-staged residual epilogue)
 template <int ACT>
-__device__ __forceinline__ void epi_act32_t(uint32_t (&r)[32], const float* sb) {
+__device__ __forceinline__ void epi_act32_t(uint32_t (&r)[32], const float* sb, bool relu = false) {
 #pragma unroll
   for (int g = 0; g < 8; ++g) {
     const float4 b = *reinterpret_cast<const float4*>(sb + g * 4);
-    r[4 * g] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g]) + b.x));
-    r[4 * g + 1] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g + 1]) + b.y));
-    r[4 * g + 2] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g + 2]) + b.z));
-    r[4 * g + 3] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g + 3]) + b.w));
+    r[4 * g] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g]) + b.x, relu));
+    r[4 * g + 1] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g + 1]) + b.y, relu));
+    r[4 * g + 2] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g + 2]) + b.z, relu));
+    r[4 * g + 3] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g + 3]) + b.w, relu));
   }
 }
 __device__ __forceinline__ void epi_act32(int act, uint32_t (&r)[32], const float* sb) {
   if (act == MV2_ACT_ELU) epi_act32_t<MV2_ACT_ELU>(r, sb);
   else if (act == MV2_ACT_SILU) epi_act32_t<MV2_ACT_SILU>(r, sb);
-  else if (act == MV2_ACT_LEAKY_RELU) epi_act32_t<MV2_ACT_LEAKY_RELU>(r, sb);
+  else if (act == MV2_ACT_LEAKY_RELU || act == MV2_ACT_RELU) epi_act32_t<MV2_ACT_LEAKY_RELU>(r, sb, act == MV2_ACT_RELU);
   else epi_act32_t<MV2_ACT_NONE>(r, sb);
 }
 __device__ __forceinline__ void epi_pack32(int act, const uint32_t (&r)[32], const float* sb, uint32_t (&pk)[16]) {
   if (act == MV2_ACT_ELU) epi_pack32_t<MV2_ACT_ELU>(r, sb, pk);
   else if (act == MV2_ACT_SILU) epi_pack32_t<MV2_ACT_SILU>(r, sb, pk);
-  else if (act == MV2_ACT_LEAKY_RELU) epi_pack32_t<MV2_ACT_LEAKY_RELU>(r, sb, pk);
+  else if (act == MV2_ACT_LEAKY_RELU || act == MV2_ACT_RELU) epi_pack32_t<MV2_ACT_LEAKY_RELU>(r, sb, pk, act == MV2_ACT_RELU);
   else epi_pack32_t<MV2_ACT_NONE>(r, sb, pk);
 }
 
@@ -346,7 +347,8 @@ __device__ __forceinline__ void epi_chunk32(const TcEpi& e, const uint32_t (&r)[
   if (MODE == EPI_GEGLU) { epi_chunk32_t<EPI_GEGLU, MV2_ACT_NONE>(e, r, ncols, n, sb, b, to, ho, wo, row_base); return; }
   if (e.act == MV2_ACT_ELU) epi_chunk32_t<MODE, MV2_ACT_ELU>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
   else if (e.act == MV2_ACT_SILU) epi_chunk32_t<MODE, MV2_ACT_SILU>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
-  else if (e.act == MV2_ACT_LEAKY_RELU) epi_chunk32_t<MODE, MV2_ACT_LEAKY_RELU>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
+  else if (e.act == MV2_ACT_LEAKY_RELU || e.act == MV2_ACT_RELU)
+    epi_chunk32_t<MODE, MV2_ACT_LEAKY_RELU>(e, r, ncols, n, sb, b, to, ho, wo, row_base, e.act == MV2_ACT_RELU);
   else epi_chunk32_t<MODE, MV2_ACT_NONE>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
 }
 

@@ -693,6 +693,26 @@ class Engine:
         self.launches += 2
         return out[0]
 
+    def maxpool2x2(self, x):
+        """nn.MaxPool2d(2, 2) (floor mode) of a channels-last (B, T, H, W, C) map -> (B, T, H // 2, W // 2, C)."""
+        B, T, H, W, Cc = x.shape
+        y = self._new((B, T, H // 2, W // 2, Cc), x.dtype)
+        check(self.lib.mv2_maxpool2x2(_ptr(x), _ptr(y), _dt(x.dtype), B * T, H, W, Cc, self._stream()), "mv2_maxpool2x2")
+        self.launches += 1
+        return y
+
+    def maxpool2x2_backward(self, g, x):
+        """Gradient wrt the pool's input x (the output of a conv with ReLU in its epilogue) from the pool output's gradient g:
+        each window's gradient goes to its first maximum, masked by x > 0; dense (B, T, H, W, C)."""
+        B, T, H, W, Cc = x.shape
+        g = g.to(x.dtype).contiguous()
+        assert tuple(g.shape) == (B, T, H // 2, W // 2, Cc), (g.shape, x.shape)
+        gx = self._new(x.shape, x.dtype)
+        check(self.lib.mv2_maxpool2x2_backward(_ptr(g), _ptr(x), _ptr(gx), _dt(x.dtype), B * T, H, W, Cc, self._stream()),
+              "mv2_maxpool2x2_backward")
+        self.launches += 1
+        return gx
+
     # ------------------------------------------------------------------ the path
     def conv_in(self, video: torch.Tensor, first_frame: bool = True):
         """video (B,C,T,H,W) on device -> conv_in's output (B,T+t_pad,H,W,C) channels-last.  The time_padding zero frames

@@ -1,5 +1,6 @@
 """The image discriminator of the GAN loss (reference M:549-675) on the device, and the loss terms built on it
-(``return_discr_loss``, M:1731-1786; the adversarial generator term, M:1826-1843).
+(``return_discr_loss``, M:1731-1786; the adversarial generator term, M:1826-1843, ``generator_term``: its image gradient is
+computed in the forward, so that the adaptive adversarial weight can use it before the total backward).
 
 Division of labour (as in train.py)
   * FORWARD: the engine's sm_90a kernels.  Every 3x3 conv carries LeakyReLU(0.1) in its epilogue; the block output
@@ -266,14 +267,56 @@ class _DiscriminatorFn(torch.autograd.Function):
         return (None, gx) + tuple(grads[p] if p in grads else torch.zeros_like(p) for p in ctx.params)
 
 
-def discriminator_forward(d, images):
-    """Discriminator(images): (B, C, H, W) on the device -> logits (B,) in the model dtype, differentiable (first order)
-    wrt the images and every discriminator parameter."""
+class _GeneratorTermFn(torch.autograd.Function):
+    """(images, *parameters) -> hinge_gen_loss = -logits.mean() (M:123-124).  When a gradient is needed, the tape runs in
+    the forward: the image gradient is then available to the adaptive adversarial weight (M:1837) before the total
+    backward, and the backward only scales it and the discriminator's parameter gradients by grad_out."""
+
+    @staticmethod
+    def forward(ctx, runner, info, images, *params):
+        logits = runner.forward(images, need_image_grad=info["image_grad"])
+        loss = -logits.mean()
+        ctx.gx, ctx.grads, ctx.params = None, None, params
+        if info["need_grad"]:
+            gx, grads = runner.backward(torch.full_like(logits, -1. / logits.numel()))
+            ctx.gx, ctx.grads = gx, [grads.get(p) for p in params]
+            info["grad_images"] = gx
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        gx = None if ctx.gx is None else ctx.gx * g.to(ctx.gx.dtype)
+        return (None, None, gx) + tuple(torch.zeros_like(p) if gp is None else gp * g.to(gp.dtype)
+                                        for p, gp in zip(ctx.params, ctx.grads))
+
+
+def _check_images(d, images):
     if images.ndim != 4 or images.shape[1] != d.channels or tuple(images.shape[-2:]) != tuple(d.image_size):
         raise ValueError(f"images must be (B, {d.channels}, {d.image_size[0]}, {d.image_size[1]}), got {tuple(images.shape)}")
     w0 = d.to_logits[0].weight
     if images.device != w0.device:
         raise RuntimeError(f"images are on {images.device} but the discriminator is on {w0.device}")
+    return w0.device
+
+
+def discriminator_forward(d, images):
+    """Discriminator(images): (B, C, H, W) on the device -> logits (B,) in the model dtype, differentiable (first order)
+    wrt the images and every discriminator parameter."""
+    dev = _check_images(d, images)
     runner = DiscrRunner(d)
-    with torch.cuda.device(w0.device):
+    with torch.cuda.device(dev):
         return _DiscriminatorFn.apply(runner, images, *[p for p in d.parameters()])
+
+
+def generator_term(d, images):
+    """The adversarial generator term -discr(images).mean() (M:1826-1831) -> (loss 0-d, info): differentiable (first order)
+    wrt the images and every discriminator parameter, like -discriminator_forward(d, images).mean(); info["grad_images"] is
+    d loss / d images, present when the images need a gradient."""
+    dev = _check_images(d, images)
+    params = list(d.parameters())
+    info = dict(image_grad=images.requires_grad,
+                need_grad=torch.is_grad_enabled() and (images.requires_grad or any(p.requires_grad for p in params)))
+    runner = DiscrRunner(d)
+    with torch.cuda.device(dev):
+        return _GeneratorTermFn.apply(runner, info, images, *params), info

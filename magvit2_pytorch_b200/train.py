@@ -311,6 +311,7 @@ class TrainRunner(TapeRunner):
         self.g_cond: Dict[str, torch.Tensor] = {}      # gradient wrt the cond stems' outputs, summed over the cond_residual stages
         self.codes = None
         self.breakdown = None
+        self._bwd_conv_out = None
 
     def _conv_bwd_padmode(self, g, x, weight, bias, k, pad_mode, need_gx=True):
         """Backward of Engine.causal_conv_padded (CausalConv3d with pad_mode reflect / replicate / circular, M:925-927): the padding
@@ -477,25 +478,46 @@ class TrainRunner(TapeRunner):
         kout = tuple(cout.weight.shape[2:])
         recon = eng.conv_out(xo, first_frame)
 
-        def bwd_conv_out(g_recon):    # (B,C,T,H,W) -> channels-last with zero gradient on the cropped time_padding frames
+        def bwd_conv_out(g_recon, need_gx=True):    # (B,C,T,H,W) -> channels-last with zero gradient on the cropped time_padding frames
+            # need_gx=False: conv_out's weight / bias gradients only (last_layer_weight_grad), the first frame's conv is skipped
             g = g_recon.permute(0, 2, 3, 4, 1)
             if sff:
                 off = m.conv_out_first_frame
                 kff = (1,) + tuple(off.weight.shape[2:])
-                gx = torch.zeros_like(xo)
-                gx[:, t_pad:t_pad + 1] = self._conv_bwd(g[:, 0:1].contiguous(), xo[:, t_pad:t_pad + 1].contiguous(), off.weight, off.bias, kff,
-                                                        pad=(0, kff[1] // 2, kff[2] // 2))
+                gx = torch.zeros_like(xo) if need_gx else None
+                if need_gx:
+                    gx[:, t_pad:t_pad + 1] = self._conv_bwd(g[:, 0:1].contiguous(), xo[:, t_pad:t_pad + 1].contiguous(), off.weight, off.bias,
+                                                            kff, pad=(0, kff[1] // 2, kff[2] // 2))
                 if xo.shape[1] - t_pad > 1:
-                    gx[:, t_pad + 1:] = self._conv_bwd_padmode(g[:, 1:].contiguous(), xo[:, t_pad + 1:].contiguous(), cout.weight, cout.bias,
-                                                               kout, mode_out)
+                    g1 = self._conv_bwd_padmode(g[:, 1:].contiguous(), xo[:, t_pad + 1:].contiguous(), cout.weight, cout.bias, kout, mode_out,
+                                                need_gx=need_gx)
+                    if need_gx:
+                        gx[:, t_pad + 1:] = g1
                 return gx
             if t_pad:
                 g = F.pad(g, (0, 0, 0, 0, 0, 0, t_pad, 0))
-            return self._conv_bwd_padmode(g.contiguous(), xo, cout.weight, cout.bias, kout, mode_out)
+            return self._conv_bwd_padmode(g.contiguous(), xo, cout.weight, cout.bias, kout, mode_out, need_gx=need_gx)
 
         self.tape.append(bwd_conv_out)
+        self._bwd_conv_out = bwd_conv_out
         self._recon_shape = tuple(recon.shape)
         return recon, aux
+
+    def last_layer_weight_grad(self, g_recon):
+        """The gradient of ``conv_out.conv.weight`` for a reconstruction gradient g_recon (B,C,T,H,W): the adaptive adversarial
+        weight's gradient norms at the last decoder layer (M:1812-1841).  Runs conv_out's weight-gradient piece of the tape on the
+        saved decoder output; the tape stays intact for the backward and ``self.grads`` is left untouched."""
+        if self._bwd_conv_out is None:
+            raise RuntimeError("the tokenizer's backward ran already: its saved activations are released")
+        w = self.m.conv_out.conv.weight
+        grads, self.grads = self.grads, {}
+        try:
+            with torch.no_grad():
+                self._bwd_conv_out(g_recon.to(self.eng.dtype), need_gx=False)
+            gw = self.grads.get(w)
+        finally:
+            self.grads = grads
+        return torch.zeros_like(w) if gw is None else gw
 
     def backward(self, g_recon, g_aux):
         """Runs the tape in reverse; returns {Parameter: grad}.  g_recon (B,C,T,H,W) or None, g_aux 0-d or None."""
@@ -522,7 +544,10 @@ class TrainRunner(TapeRunner):
                     lin = stem[0]
                     self._vjp(lambda t, lin=lin: F.silu(F.linear(t, lin.weight.float(), lin.bias.float())), self.cond.float(),
                               list(lin.parameters()), self.g_cond[side].float())
+        # the tape's closures and conv_out's piece of it refer to this runner: dropping them here breaks the reference cycle,
+        # so the saved activations are freed with the loss graph, not at a later cyclic collection
         self.tape = []
+        self._bwd_conv_out = None
         return self.grads
 
 
@@ -554,9 +579,10 @@ def live_parameters(model, first_frame=True):
     return [p for p in model.parameters() if p.requires_grad and id(p) not in dead]
 
 
-def train_forward(model, video, first_frame=True, cond=None):
-    """-> (recon with grad_fn, aux_loss with grad_fn, codes, lfq breakdown | None)."""
-    runner = TrainRunner(model)
+def train_forward(model, video, first_frame=True, cond=None, runner=None):
+    """-> (recon with grad_fn, aux_loss with grad_fn, codes, lfq breakdown | None).  `runner`: a fresh TrainRunner of the model
+    to run on (the caller keeps it for last_layer_weight_grad)."""
+    runner = runner or TrainRunner(model)
     params = live_parameters(model, first_frame)
     recon, aux = _TokenizerTrainFn.apply(runner, first_frame, cond, video, *params)
     return recon, aux, runner.codes, runner.breakdown

@@ -17,11 +17,15 @@ factorisation in include/magvit2_b200.h; the other ``cond_*`` types raise in the
 ``forward(return_loss=True)`` (reconstruction + quantiser auxiliary loss; models built with ``use_gan=False,
 perceptual_loss_weight=0``) runs on the device; in ``model.train()`` with gradients enabled it returns a loss with a
 ``grad_fn`` (train.py: forward by the same kernels, backward by library code).
-Models without a perceptual (VGG) term that use the GAN (``use_gan=True, adversarial_loss_weight > 0``) build the image
-discriminator ``discr`` (M:1415-1422) and run it on the device (gan.py): ``return_discr_loss`` (M:1731-1786) and the
-adversarial generator term of ``return_loss`` (M:1826-1843).
-Out of scope (raise at construction / call; SURVEY.md 8f): the perceptual (VGG) loss and adaptive weighting, multiscale
-discriminators, and the discriminator's antialiased (Blur) downsampling.
+Models that use the GAN (``use_gan=True, adversarial_loss_weight > 0``) build the image discriminator ``discr``
+(M:1415-1422) and run it on the device (gan.py): ``return_discr_loss`` (M:1731-1786) and the adversarial generator term of
+``return_loss`` (M:1826-1843).  The perceptual term (``perceptual_loss_weight > 0``, ``channels`` in {1, 3, 4}) needs a
+user-supplied VGG module (``vgg=``, M:1081; nothing is downloaded): the perceptual loss and the adaptive adversarial weight
+(M:1788-1841) then run on the device (vgg.py).  Without one (``vgg=None``) the model builds no discriminator and
+``return_loss`` / ``return_discr_loss`` raise.  The VGG is left out of ``state_dict``, ``copy_for_eval`` and the pickled
+config, so ``init_and_load_from`` gives a model without it.
+Out of scope (raise at construction / call; SURVEY.md 8f): multiscale discriminators and the discriminator's antialiased
+(Blur) downsampling.
 """
 from __future__ import annotations
 
@@ -255,15 +259,22 @@ class VideoTokenizer(nn.Module):
         self.quantizer_aux_loss_weight = quantizer_aux_loss_weight
         self.register_buffer("zero", torch.tensor(0.), persistent=False)
 
-        # training-only branches of the reference: the VGG and multiscale discriminators are not built (SURVEY.md 2 rows
-        # 13-15); the image discriminator is, for models whose loss has no perceptual term (M:1415-1427, gan.py)
+        # training-only branches of the reference.  The perceptual term runs when a VGG module is passed (vgg.py; this
+        # package never downloads torchvision's weights, M:1397-1405); the image discriminator is built for the GAN term unless
+        # the loss has a perceptual term without a VGG module (M:1415-1427, gan.py); multiscale discriminators are not built
         self.vgg = None
         self.use_vgg = False
+        self._vgg_cache = {}                    # the VGG's weight packs (vgg.vgg_packs): per model, like _engine
         self.perceptual_loss_weight = perceptual_loss_weight
+        if isinstance(vgg, nn.Module) and self._has_vgg():
+            from .vgg import check_vgg
+            check_vgg(vgg)
+            self.vgg = vgg
+            self.use_vgg = True
         self.use_gan = use_gan
         self.has_gan = False
         self.discr = None
-        if use_gan and adversarial_loss_weight > 0. and not self._has_vgg():
+        if use_gan and adversarial_loss_weight > 0. and (self.use_vgg or not self._has_vgg()):
             kw = dict(dim=dim, image_size=image_size, channels=channels, max_dim=512) if discr_kwargs is None else dict(discr_kwargs)
             self.discr = M.Discriminator(**kw)
             self.has_gan = True
@@ -303,11 +314,24 @@ class VideoTokenizer(nn.Module):
     def discr_parameters(self):
         return [] if self.discr is None else list(self.discr.parameters())
 
+    def state_dict(self, *args, destination=None, prefix="", keep_vars=False):
+        # the VGG is left out of checkpoints, as the reference's remove_vgg does (M:141-155, M:1487-1489); filtering the
+        # result keeps the module tree itself untouched
+        if len(args) > 1:                       # torch's deprecated positional form (destination, prefix, keep_vars)
+            prefix = args[1]
+        sd = super().state_dict(*args, destination=destination, prefix=prefix, keep_vars=keep_vars)
+        for k in [k for k in sd if k.startswith(prefix + "vgg.")]:
+            del sd[k]
+        return sd
+
     def load_state_dict(self, state_dict, strict: bool = True, **kw):
         # reference checkpoints carry discriminator weights (always constructed, M:1422); a model that built no
-        # discriminator drops them, as it drops the multiscale discriminators'.
+        # discriminator drops them, as it drops the multiscale discriminators'.  Checkpoints carry no VGG weights (M:1491-1493):
+        # any in `state_dict` are ignored and the VGG keeps its own, which stand in for its keys under strict loading.
         sd = {k: v for k, v in state_dict.items()
-              if not ((self.discr is None and k.startswith("discr.")) or k.startswith("multiscale_discrs."))}
+              if not ((self.discr is None and k.startswith("discr.")) or k.startswith("multiscale_discrs.") or k.startswith("vgg."))}
+        if self.vgg is not None:
+            sd.update(("vgg." + k, v) for k, v in self.vgg.state_dict(keep_vars=True).items())
         return super().load_state_dict(sd, strict=strict, **kw)
 
     def __deepcopy__(self, memo):
@@ -315,6 +339,7 @@ class VideoTokenizer(nn.Module):
         # to THIS instance: a copy starts without them and re-packs / re-captures on first use
         eng, self._engine = self._engine, None
         graphs, self._graphs = self._graphs, {}
+        vgg_cache, self._vgg_cache = self._vgg_cache, {}
         try:
             cls = self.__class__
             new = cls.__new__(cls)
@@ -324,18 +349,23 @@ class VideoTokenizer(nn.Module):
         finally:
             self._engine = eng
             self._graphs = graphs
+            self._vgg_cache = vgg_cache
         return new
 
     def __getstate__(self):
         st = dict(self.__dict__)
         st["_engine"] = None
         st["_graphs"] = {}
+        st["_vgg_cache"] = {}
         return st
 
     def copy_for_eval(self):
+        """An eval-mode copy without the VGG (M:1476-1485): its return_loss raises like a model built with vgg=None."""
         dev = self.device
-        c = copy.deepcopy(self.cpu())
+        memo = {} if self.vgg is None else {id(self.vgg): None}      # the copy's `vgg` entry is None: the VGG is not copied
+        c = copy.deepcopy(self.cpu(), memo)
         self.to(dev)
+        c.vgg, c.use_vgg = None, False
         c.eval()
         return c.to(dev)
 
@@ -346,7 +376,8 @@ class VideoTokenizer(nn.Module):
         pkg = torch.load(str(path), map_location="cpu", weights_only=False)
         assert "config" in pkg, "model configs were not found in this saved checkpoint"
         config = pickle.loads(pkg["config"])
-        # reference checkpoints pickle module-valued kwargs we do not build
+        # reference checkpoints pickle module-valued kwargs we do not build; the VGG is never saved, so a model loaded here
+        # has none (vgg=None): pass the VGG module to the constructor and load_state_dict to train with the perceptual term
         for k in ("vgg", "lfq_activation"):
             config[k] = None
         config["multiscale_discrs"] = tuple()
@@ -552,36 +583,53 @@ class VideoTokenizer(nn.Module):
                 return_discr_loss=False, return_recon_loss_only=False, apply_gradient_penalty=True,
                 video_contains_first_frame=True, adversarial_loss_weight=None,
                 multiscale_adversarial_loss_weight=None):
-        """The reference forward (M:1657-1896): inference returns (codes / reconstruction), ``return_recon_loss_only`` and --
-        for models without the GAN / perceptual branches (``use_gan=False, perceptual_loss_weight=0``) -- ``return_loss``:
-        ``(total_loss, LossBreakdown)`` with ``total_loss = recon_loss + aux_loss * quantizer_aux_loss_weight`` (M:1868-1896)."""
+        """The reference forward (M:1657-1896): inference returns (codes / reconstruction), ``return_recon_loss_only``,
+        ``return_discr_loss`` and ``return_loss``: ``(total_loss, LossBreakdown)`` with ``total_loss = recon_loss + aux_loss *
+        quantizer_aux_loss_weight + perceptual_loss * perceptual_loss_weight + gen_loss * adaptive_weight *
+        adversarial_loss_weight`` (M:1868-1896).  The perceptual term needs a ``vgg=`` module; the adaptive weight is the ratio
+        of the perceptual and adversarial terms' gradient norms at ``conv_out.conv.weight`` in a train-mode step (M:1812-1841),
+        1 in eval mode."""
         assert (return_loss + return_codes + return_discr_loss) <= 1               # M:1674
         if return_discr_loss and self.discr is None:
             raise NotImplementedError("return_discr_loss needs the image discriminator, which is built for use_gan=True, "
-                                      "adversarial_loss_weight > 0 and no perceptual (VGG) term (SURVEY.md 8f N2)")
+                                      "adversarial_loss_weight > 0 and a `vgg=` module when the loss has a perceptual term "
+                                      "(SURVEY.md 8f N2)")
         if return_loss and self._needs_gan_or_vgg():
             raise NotImplementedError(
-                "return_loss with the perceptual / adaptive-weighting terms or multiscale discriminators (reference "
-                "M:1788-1866) is outside the accelerated path (SURVEY.md 8f N2): construct with perceptual_loss_weight=0.")
+                "return_loss with the perceptual term needs a `vgg=` module (this package downloads no VGG weights), and "
+                "multiscale discriminators (reference M:1846-1866) are outside the accelerated path (SURVEY.md 8f N2): pass "
+                "vgg=<module> or construct with perceptual_loss_weight=0.")
+        grad_step = (return_loss and self.training and torch.is_grad_enabled()
+                     and any(p.requires_grad for p in self.parameters()))
+        if return_loss and self.training and self.use_vgg and self.has_gan and not grad_step:
+            raise RuntimeError("a train-mode return_loss with a VGG and a GAN needs gradients: the adaptive adversarial weight is "
+                               "a ratio of gradient norms (M:1812-1841; the reference fails in torch.autograd.grad here)")
         video, ff = self._check_video(video_or_images, video_contains_first_frame)
         cond = self._check_cond(cond, video.shape[0])
         if adversarial_loss_weight is None:                                        # the call-site weight wins (M:1674-1680)
             adversarial_loss_weight = self.adversarial_loss_weight
         if return_discr_loss:
             return self._discr_loss(video, ff, cond, apply_gradient_penalty)
-        if return_loss and self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        if grad_step:
             # the trainer's generator step (T:356-363): loss with a grad_fn.  Forward = the same kernels; backward = train.py
-            from .train import train_forward
-            recon, aux, _, qlb = train_forward(self, video.contiguous(), ff, cond)
+            from .train import TrainRunner, train_forward
+            runner = TrainRunner(self)
+            recon, aux, _, qlb = train_forward(self, video.contiguous(), ff, cond, runner=runner)
             target = video.float() / 255. if video.dtype == torch.uint8 else video
             recon_loss = torch.nn.functional.mse_loss(target.to(recon.dtype), recon)          # M:1722
             self.quantizer_loss_breakdown, self.quantizer_aux_loss = qlb, aux.detach()
             aux_losses = aux.to(recon_loss.dtype)
             total_loss = recon_loss + aux_losses * self.quantizer_aux_loss_weight                # M:1868-1871
-            gen_loss, adaptive_weight = self._gen_loss(recon)
+            perceptual_loss, g_perc = self._perceptual_loss(target, recon)
+            gen_loss, g_gen = self._gen_loss(recon)
+            adaptive_weight = 0.
+            if self.has_gan:
+                adaptive_weight = self._adaptive_weight(runner, recon, g_perc, g_gen) if self.use_vgg else 1.
+            if self.use_vgg:
+                total_loss = total_loss + perceptual_loss * self.perceptual_loss_weight
             if self.has_gan:
                 total_loss = total_loss + gen_loss * adaptive_weight * adversarial_loss_weight   # M:1872-1875
-            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, self.zero, gen_loss, adaptive_weight, [], [])
+            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, perceptual_loss, gen_loss, adaptive_weight, [], [])
         with torch.no_grad():
             eng = self.engine
             need_recon = return_recon or return_recon_loss_only or return_loss or not return_codes
@@ -596,16 +644,20 @@ class VideoTokenizer(nn.Module):
             recon_loss = eng.mse(video, recon).to(self.dtype)                      # M:1722
             if return_recon_loss_only:                                             # M:1726-1727
                 return recon_loss, recon
-            # M:1868-1896 with perceptual_loss = zero, no multiscale discriminators; gen_loss = zero, adaptive_weight = 0.
-            # without a discriminator
+            # M:1868-1896 without multiscale discriminators: perceptual_loss = zero without a VGG; gen_loss = zero and
+            # adaptive_weight = 0. without a discriminator, adaptive_weight = 1. with one (no gradients here, M:1833)
             zero = self.zero
             aux_losses = zero if aux is None else aux.to(recon_loss.dtype)         # eval mode / FSQ: M:1700-1703
             total_loss = recon_loss + aux_losses * self.quantizer_aux_loss_weight
-            gen_loss, adaptive_weight = self._gen_loss(recon)
+            perceptual_loss, _ = self._perceptual_loss(video.float() / 255. if video.dtype == torch.uint8 else video, recon)
+            if self.use_vgg:
+                total_loss = total_loss + perceptual_loss * self.perceptual_loss_weight
+            gen_loss, _ = self._gen_loss(recon)
+            adaptive_weight = 1. if self.has_gan else 0.
             if self.has_gan:
                 total_loss = total_loss + gen_loss * adaptive_weight * adversarial_loss_weight
             qlb = None if (self.use_fsq or aux is None) else self.quantizer_loss_breakdown
-            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, zero, gen_loss, adaptive_weight, [], [])
+            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, perceptual_loss, gen_loss, adaptive_weight, [], [])
 
     def _no_grad_forward(self, eng, video, ff, cond, need_recon):
         """The tokenizer forward without gradients -> (codes | (codes, recon), train-mode LFQ aux loss | None)."""
@@ -635,12 +687,42 @@ class VideoTokenizer(nn.Module):
         return video.transpose(1, 2)[b, frame_indices.to(video.device)][:, 0]
 
     def _gen_loss(self, recon):
-        """The adversarial generator term (M:1826-1844): -discr(frames).mean() on one random frame per clip, drawn from the
-        default CPU generator as the reference does; (zero, 0.) without a discriminator."""
+        """The adversarial generator term (M:1826-1831): -discr(frames).mean() on one random frame per clip, drawn from the
+        default CPU generator as the reference does -> (loss, (frame indices, d loss / d frames) | None); (zero, None)
+        without a discriminator."""
         if not self.has_gan:
-            return self.zero, 0.
+            return self.zero, None
+        from .gan import generator_term
         frame_indices = torch.randn((recon.shape[0], recon.shape[2])).topk(1, dim=-1).indices
-        return -self.discr(self._pick_frames(recon, frame_indices)).mean(), 1.
+        loss, info = generator_term(self.discr, self._pick_frames(recon, frame_indices))
+        return loss, (frame_indices, info["grad_images"]) if "grad_images" in info else None
+
+    def _perceptual_loss(self, target, recon):
+        """The perceptual term (M:1788-1808): F.mse_loss of the VGG features of one random frame per clip (drawn before the
+        generator term's, M:1792) of the target and the reconstruction -> (loss, (frame indices, d loss / d recon frames) |
+        None); (zero, None) without a VGG."""
+        if not self.use_vgg:
+            return self.zero, None
+        from .vgg import perceptual_loss
+        frame_indices = torch.randn((recon.shape[0], recon.shape[2])).topk(1, dim=-1).indices
+        real = self._pick_frames(target, frame_indices).to(self.dtype).contiguous()
+        loss, info = perceptual_loss(self.vgg, real, self._pick_frames(recon, frame_indices), self.channels, self._vgg_cache)
+        return loss, (frame_indices, info["grad_frames"]) if "grad_frames" in info else None
+
+    @staticmethod
+    def _scatter_frames(recon, frame_indices, g_frames):
+        """The reconstruction gradient of a loss on the picked frames (B, C, H, W): zero on every other frame."""
+        g = torch.zeros(recon.shape, device=recon.device, dtype=g_frames.dtype)
+        g.transpose(1, 2)[torch.arange(recon.shape[0], device=recon.device), frame_indices[:, 0].to(recon.device)] = g_frames
+        return g
+
+    def _adaptive_weight(self, runner, recon, g_perc, g_gen):
+        """M:1812-1841: |d perceptual / d W| / max(|d gen / d W|, 1e-3), clamped at 1e3 (NaN -> 1.), W = conv_out.conv.weight,
+        from the tokenizer's saved activations (TrainRunner.last_layer_weight_grad) -- no backward runs."""
+        norm_p = runner.last_layer_weight_grad(self._scatter_frames(recon, *g_perc)).norm(p=2)
+        norm_g = runner.last_layer_weight_grad(self._scatter_frames(recon, *g_gen)).norm(p=2)
+        w = (norm_p / norm_g.clamp(min=1e-3)).clamp(max=1e3)
+        return 1. if torch.isnan(w).any() else w.detach()
 
     def _discr_loss(self, video, ff, cond, apply_gradient_penalty):
         """``return_discr_loss`` (M:1731-1786): the tokenizer runs without gradients (as the no-grad forward, including the
@@ -668,9 +750,9 @@ class VideoTokenizer(nn.Module):
         return bool(self.channels in {1, 3, 4} and self.perceptual_loss_weight > 0.)
 
     def _needs_gan_or_vgg(self) -> bool:
-        """True when the loss needs a term this package does not build: the VGG (M:1392), multiscale discriminators (M:1435),
-        or the GAN term of a model that built no discriminator (M:1427)."""
-        return bool(self._has_vgg() or (self.use_gan and self.adversarial_loss_weight > 0. and self.discr is None)
+        """True when the loss needs a term this package does not build: the perceptual term without a VGG module (M:1392),
+        multiscale discriminators (M:1435), or the GAN term of a model that built no discriminator (M:1427)."""
+        return bool((self._has_vgg() and not self.use_vgg) or (self.use_gan and self.adversarial_loss_weight > 0. and self.discr is None)
                     or self.has_multiscale_discrs)
 
     @property

@@ -73,6 +73,52 @@ def fill_discr_(module, seed: int = 0):
     return module
 
 
+class Vgg(torch.nn.Module):
+    """torchvision.models.VGG's forward: features, avgpool, flatten, classifier."""
+
+    def __init__(self, features, avgpool, classifier):
+        super().__init__()
+        self.features, self.avgpool, self.classifier = features, avgpool, classifier
+
+    def forward(self, x):
+        return self.classifier(torch.flatten(self.avgpool(self.features(x)), 1))
+
+
+# torchvision's VGG16 feature configuration: output channels of each 3x3 conv, "M" = MaxPool2d(2, 2)
+VGG16_CFG = (64, 64, "M", 128, 128, "M", 256, 256, 256, "M", 512, 512, 512, "M", 512, 512, 512, "M")
+
+
+def build_vgg(cfg, hidden, num_classes=None, dropout=0.5, avgpool=(7, 7)):
+    """A pure ``torch.nn`` module with torchvision's VGG attribute layout (features / avgpool / classifier and their child
+    indices), so that no test needs torchvision.  num_classes=None truncates the classifier as the reference does for its
+    default VGG16 (M:1403: the last ReLU-less Linear and the Dropout before it are dropped); otherwise the full classifier."""
+    from torch import nn
+
+    layers, c = [], 3
+    for v in cfg:
+        if v == "M":
+            layers.append(nn.MaxPool2d(kernel_size=2, stride=2))
+        else:
+            layers += [nn.Conv2d(c, v, kernel_size=3, padding=1), nn.ReLU(inplace=True)]
+            c = v
+    cls = [nn.Linear(c * avgpool[0] * avgpool[1], hidden), nn.ReLU(True), nn.Dropout(p=dropout),
+           nn.Linear(hidden, hidden), nn.ReLU(True), nn.Dropout(p=dropout)]
+    cls = cls[:-1] if num_classes is None else cls + [nn.Linear(hidden, num_classes)]
+    return Vgg(nn.Sequential(*layers), nn.AdaptiveAvgPool2d(avgpool), nn.Sequential(*cls))
+
+
+@torch.no_grad()
+def fill_vgg_(vgg, seed: int = 0):
+    """Overwrite a VGG's weights in place from per-key seeded generators: He scaling (sqrt(2 / fan_in)) keeps the activations'
+    magnitude through the ReLU layers, so the features and the perceptual loss do not vanish."""
+    for k, v in vgg.state_dict().items():
+        t = synth_tensor("vgg." + k, v.shape, seed)
+        if k.endswith("weight"):
+            t = t * 2 ** 0.5
+        v.copy_(t.to(v.dtype))
+    return vgg
+
+
 def synth_video(batch, channels, frames, size, seed=1234):
     g = torch.Generator(device="cpu")
     g.manual_seed(seed)
