@@ -174,7 +174,7 @@ int mv2_geglu(const void* in, void* out, int dtype, int64_t N, int I, void* stre
 
 /* ---- quantisers (un-vendored vector-quantize-pytorch LFQ / FSQ; SURVEY.md Appendix A.1/A.2;
  * reference call sites M:1576, M:1593, M:1700, M:1705; constructor kwargs num_codebooks M:1057, lfq_spherical M:1070) ------
- * d = dims per codebook, num_codebooks = nc, D = d * nc <= 16 projected dims; one index per (token, codebook):
+ * d = dims per codebook, num_codebooks = nc, D = d * nc <= 32 projected dims; one index per (token, codebook):
  *   indices [N][nc].
  * lfq_forward : x [N][C] -> p = tanh((Win x + bin)/clamp)*clamp (fp32), per codebook (L2-normalised first when
  *               spherical != 0): bit_j = p_j > 0, index = sum bit_j << (d-1-j) (int64), quantized [N][C] = Wout (+-1) + bout.
@@ -197,16 +197,32 @@ int mv2_fsq_decode(const void* indices, int index_is_i64, int64_t N, int C, int 
  * lfq_entropy_partials: from presign [N][nc][d] (d <= 12) accumulates, for this rank,
  *   stats[0] = sum_{tokens, codebooks} H(softmax_K(2*inv_temp*<p, code_k>)), stats[1] = sum (p - sign p)^2,
  *   avg_prob[nc][K] += sum_tokens prob (un-normalised; caller divides by the token count, then the cross-rank SUM
- *   all-reduce of avg_prob -- the 4 KiB NCCL all-reduce of cfg 3).
+ *   all-reduce of avg_prob -- nc * 2^d * 4 bytes, 4 KiB at the README config).
  * stats and avg_prob must be zeroed by the caller.                                             */
 int mv2_lfq_entropy_partials(const float* presign, int64_t N, int d, int num_codebooks, float inv_temperature,
                              float* avg_prob, float* stats, void* stream);
+
+/* lfq_entropy_fact_*: the same terms for 1 <= d <= 20 (D = d * nc <= 32), factorised over bits:
+ *   prob_k = prod_i sigmoid(4 inv_temp p_i s_ki)  (s_ki = +-1: bit i of code k, MSB first), so nothing of size
+ *   [tokens][2^d] is materialised; O(N nc 2^d) work, a log only where prob > 1e-5.  Deterministic: fixed-order sums, no
+ *   float atomics, bit-identical across runs.  workspace: mv2_lfq_entropy_fact_workspace_bytes(N, d, nc) bytes (covers both).
+ * fact_partials: OVERWRITES avg_prob[nc][2^d] = sum_tokens prob and stats[2] (as lfq_entropy_partials; no zeroing needed).
+ * fact_backward: grad_presign [N][nc][d] of  coef_sample * sum_{t,c} H(prob_tc) - coef_batch * sum_{t,c,k} h'(avg_global_ck) prob_tck
+ *   (h'(x) = -(log x + 1) above 1e-5, -log 1e-5 below), i.e. the entropy part of the aux loss with the batch term taken at the
+ *   cross-rank mean avg_global [nc][2^d]: coef_sample = entropy_weight / (N nc), coef_batch = entropy_weight * diversity_gamma / (N nc).
+ *   grad = 2 inv_temp (sum_k c_k s_ki - tanh(2 inv_temp p_i) sum_k c_k),  c_k = prob_k (coef_sample h'(prob_k) - coef_batch h'(avg_k)). */
+size_t mv2_lfq_entropy_fact_workspace_bytes(int64_t n_tokens, int d, int num_codebooks);
+int mv2_lfq_entropy_fact_partials(const float* presign, int64_t N, int d, int num_codebooks, float inv_temperature,
+                                  float* avg_prob, float* stats, void* workspace, void* stream);
+int mv2_lfq_entropy_fact_backward(const float* presign, const float* avg_global, int64_t N, int d, int num_codebooks,
+                                  float inv_temperature, float coef_sample, float coef_batch, float* grad_presign,
+                                  void* workspace, void* stream);
 
 /* mv2_lfq_aux_finalize: out4 = {per_sample_entropy, batch_entropy, commitment, aux_loss} from the partial sums above
  * (A.1 steps 7-10): per_sample = stats[0] / (n_tokens nc), commitment = stats[1] / (n_tokens nc d),
  * batch_entropy = mean over codebooks of sum_k -p_k log(max(p_k, 1e-5)), p = avg_prob_sum / n_tokens_global
  * (avg_prob_sum = the cross-rank SUM), aux = (per_sample - diversity_gamma * batch_entropy) * entropy_weight
- * + commitment * commitment_weight.                                                                                    */
+ * + commitment * commitment_weight.  d <= 20 (d > 12: one 1024-thread block, fp64 sums in a fixed order).             */
 int mv2_lfq_aux_finalize(const float* avg_prob_sum, const float* stats, int d, int num_codebooks, int64_t n_tokens,
                          int64_t n_tokens_global, float diversity_gamma, float entropy_weight, float commitment_weight,
                          float* out4, void* stream);

@@ -97,6 +97,9 @@ SIGNATURES = {
     "mv2_fsq_decode": (_I, [_VP, _I, _I64, _I, _I, _I, C.POINTER(C.c_int32), _VP, _VP, _VP, _I, _VP]),
     "mv2_lfq_entropy_partials": (_I, [_VP, _I64, _I, _I, _F, _VP, _VP, _VP]),
     "mv2_lfq_aux_finalize": (_I, [_VP, _VP, _I, _I, _I64, _I64, _F, _F, _F, _VP, _VP]),
+    "mv2_lfq_entropy_fact_workspace_bytes": (_SZ, [_I64, _I, _I]),
+    "mv2_lfq_entropy_fact_partials": (_I, [_VP, _I64, _I, _I, _F, _VP, _VP, _VP, _VP]),
+    "mv2_lfq_entropy_fact_backward": (_I, [_VP, _VP, _I64, _I, _I, _F, _F, _F, _VP, _VP, _VP]),
     "mv2_gateloop_scan": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
     "mv2_mse": (_I, [_VP, _I, _VP, _I, _I64, _VP, _VP, _VP]),
     "mv2_mse_workspace_bytes": (C.c_size_t, []),

@@ -1672,18 +1672,21 @@ __global__ void geglu_kernel(const T* __restrict__ in, T* __restrict__ out, int6
 // ------------------------------------------------------------------------------------------
 // quantisers
 // ------------------------------------------------------------------------------------------
-constexpr int Q_MAXD = 16;
-struct FsqLevels { int32_t lv[Q_MAXD]; };
+// projected dims per token: D <= 16 runs the original instantiation, 17 <= D <= 32 (e.g. MAGVIT-v2's 2^18 codes, or 2 x 2^16)
+// the wide one, so the narrow configurations keep their register budget and results
+constexpr int Q_MAXD = 16, Q_MAXD_WIDE = 32;
+template <int MAXD>
+struct FsqLevelsT { int32_t lv[MAXD]; };
 
-// mode 0: LFQ, mode 1: FSQ.  One warp per token.  `d` = dims per codebook, `nc` codebooks (d * nc <= Q_MAXD projected dims,
+// mode 0: LFQ, mode 1: FSQ.  One warp per token.  `d` = dims per codebook, `nc` codebooks (d * nc <= MAXD projected dims,
 // reference kwarg num_codebooks M:1057 -> M:1367 / M:1381): one index per (token, codebook), idx[tok * nc + cb].
 // spherical (LFQ, M:1070 -> A.1 step 4): the per-codebook d-vector is L2-normalised before the sign / the auxiliary terms; the
 // quantised output (+-1) and the indices do not depend on it.
-template <typename T, int MODE>
+template <typename T, int MODE, int MAXD>
 __global__ void __launch_bounds__(256) quant_forward_kernel(const T* __restrict__ x, int64_t N, int C, int d, int nc,
                                                             const float* __restrict__ win, const float* __restrict__ bin,
                                                             const float* __restrict__ wout, const float* __restrict__ bout,
-                                                            float clamp, int spherical, FsqLevels lv, int64_t* __restrict__ idx64,
+                                                            float clamp, int spherical, FsqLevelsT<MAXD> lv, int64_t* __restrict__ idx64,
                                                             int32_t* __restrict__ idx32, T* __restrict__ quant,
                                                             float* __restrict__ aux) {
   pdl_wait();
@@ -1693,18 +1696,18 @@ __global__ void __launch_bounds__(256) quant_forward_kernel(const T* __restrict_
   if (tok >= N) return;
   const int D = d * nc;
   const T* row = x + tok * C;
-  float acc[Q_MAXD];
+  float acc[MAXD];
 #pragma unroll
-  for (int i = 0; i < Q_MAXD; ++i) acc[i] = 0.f;
+  for (int i = 0; i < MAXD; ++i) acc[i] = 0.f;
   for (int c = lane; c < C; c += 32) {
     const float xv = to_f32<T>(row[c]);
 #pragma unroll
-    for (int i = 0; i < Q_MAXD; ++i)
+    for (int i = 0; i < MAXD; ++i)
       if (i < D) acc[i] = fmaf(xv, win[(int64_t)i * C + c], acc[i]);
   }
-  float code[Q_MAXD], pv[Q_MAXD];
+  float code[MAXD], pv[MAXD];
 #pragma unroll
-  for (int i = 0; i < Q_MAXD; ++i) {
+  for (int i = 0; i < MAXD; ++i) {
     pv[i] = 0.f;
     if (i < D) {
       float p = warp_sum(acc[i]) + bin[i];
@@ -1716,11 +1719,11 @@ __global__ void __launch_bounds__(256) quant_forward_kernel(const T* __restrict_
     for (int cb = 0; cb < nc; ++cb) {
       float ss = 0.f;
 #pragma unroll
-      for (int i = 0; i < Q_MAXD; ++i)
+      for (int i = 0; i < MAXD; ++i)
         if (i >= cb * d && i < (cb + 1) * d) ss = fmaf(pv[i], pv[i], ss);
       const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
 #pragma unroll
-      for (int i = 0; i < Q_MAXD; ++i)
+      for (int i = 0; i < MAXD; ++i)
         if (i >= cb * d && i < (cb + 1) * d) pv[i] *= inv;
     }
   }
@@ -1728,7 +1731,7 @@ __global__ void __launch_bounds__(256) quant_forward_kernel(const T* __restrict_
   int32_t basis = 1;
   int j = 0, cb = 0;                      // position inside the current codebook
 #pragma unroll
-  for (int i = 0; i < Q_MAXD; ++i) {
+  for (int i = 0; i < MAXD; ++i) {
     code[i] = 0.f;
     if (i < D) {
       const float p = pv[i];
@@ -1764,16 +1767,16 @@ __global__ void __launch_bounds__(256) quant_forward_kernel(const T* __restrict_
     for (int c = lane; c < C; c += 32) {
       float o = bout[c];
 #pragma unroll
-      for (int i = 0; i < Q_MAXD; ++i)
+      for (int i = 0; i < MAXD; ++i)
         if (i < D) o = fmaf(code[i], wout[(int64_t)c * D + i], o);
       qrow[c] = from_f32<T>(o);
     }
   }
 }
 
-template <typename T, int MODE>
+template <typename T, int MODE, int MAXD>
 __global__ void __launch_bounds__(256) quant_decode_kernel(const void* __restrict__ indices, int is64, int64_t N, int C,
-                                                           int d, int nc, FsqLevels lv, const float* __restrict__ wout,
+                                                           int d, int nc, FsqLevelsT<MAXD> lv, const float* __restrict__ wout,
                                                            const float* __restrict__ bout, T* __restrict__ quant) {
   pdl_wait();
   pdl_launch_dependents();
@@ -1781,11 +1784,11 @@ __global__ void __launch_bounds__(256) quant_decode_kernel(const void* __restric
   const int64_t tok = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (tok >= N) return;
   const int D = d * nc;
-  float code[Q_MAXD];
+  float code[MAXD];
   int64_t index = 0, rem = 0;
   int j = 0, cb = 0;
 #pragma unroll
-  for (int i = 0; i < Q_MAXD; ++i) {
+  for (int i = 0; i < MAXD; ++i) {
     code[i] = 0.f;
     if (i < D) {
       if (j == 0) {
@@ -1808,7 +1811,7 @@ __global__ void __launch_bounds__(256) quant_decode_kernel(const void* __restric
   for (int c = lane; c < C; c += 32) {
     float o = bout[c];
 #pragma unroll
-    for (int i = 0; i < Q_MAXD; ++i)
+    for (int i = 0; i < MAXD; ++i)
       if (i < D) o = fmaf(code[i], wout[(int64_t)c * D + i], o);
     qrow[c] = from_f32<T>(o);
   }
@@ -1890,6 +1893,285 @@ __global__ void __launch_bounds__(256) lfq_entropy_kernel(const float* __restric
   if (tid == 0) atomicAdd(&stats[1], commit_sum);
 }
 
+
+// ------------------------------------------------------------------------------------------
+// LFQ entropy terms of large codebooks (1 <= d <= 20), factorised over bits.  The code distribution
+//   prob_k = softmax_k(2 tau <p, c_k>),  c_k in {+-1}^d,   equals   prod_i sigma(4 tau p_i s_ki)
+// (s_ki = +-1: bit i of code k, MSB first as LFQ's mask), so one (token, code) probability is the product of two or three entries
+// of small per-token tables of bit-probability products and nothing of size K is kept per token.  The clamped entropy
+// -x log max(x, 1e-5) is not a sum over bits, so both passes still visit every (token, code) pair -- but they take a log only
+// where x > 1e-5.  Every sum runs in a fixed order (per-thread registers, fixed shuffle trees, fixed-order partial reductions;
+// no float atomics), so two runs give bit-identical results.
+// ------------------------------------------------------------------------------------------
+constexpr int LF_MAXD = 20;
+constexpr int LF_TT = 32;                 // tokens staged per chunk (partials)
+constexpr int LF_R = 16;                  // codes per thread (partials)
+constexpr int LF_TARGET_BLOCKS = 264;     // partials grid: code tiles x token splits x codebooks ~ 2 waves of 132 SMs
+constexpr int LF_BW_WARPS = 4;            // backward: warps per block (~150 registers per thread: 3 blocks per SM)
+constexpr float LF_LOG_INV_EPS = 11.512925464970229f;   // -log(1e-5): -x log max(x, 1e-5) = x * this for x <= 1e-5
+
+// code bit layout of the partials kernel (LSB first): lb = min(d, 8) bits -> threadIdx.x (split into lo4 = min(lb, 4) and the rest),
+// rb = min(d - lb, 4) bits -> the thread's LF_R register codes, the top tb = d - lb - rb bits -> blockIdx.x (one code tile)
+struct LfLayout {
+  int lb, lo4, rb, tb;
+  __host__ __device__ explicit LfLayout(int d) {
+    lb = d < 8 ? d : 8;
+    lo4 = lb < 4 ? lb : 4;
+    rb = d - lb < 4 ? d - lb : 4;
+    tb = d - lb - rb;
+  }
+};
+
+struct LfSplit { int tiles, splits; int64_t per; };
+static inline LfSplit lf_split(int64_t N, int d, int nc) {
+  const LfLayout L(d);
+  LfSplit s;
+  s.tiles = 1 << L.tb;
+  const int64_t want = std::max<int64_t>(1, (LF_TARGET_BLOCKS + (int64_t)s.tiles * nc - 1) / ((int64_t)s.tiles * nc));
+  const int64_t chunks = (N + LF_TT - 1) / LF_TT;
+  const int64_t sp = std::min<int64_t>(want, chunks);
+  s.per = (chunks + sp - 1) / sp * LF_TT;           // tokens per split, a whole number of chunks
+  s.splits = (int)((N + s.per - 1) / s.per);        // no empty split
+  return s;
+}
+
+// product of the bit probabilities of `v` (nbits bits) over dims [i0, i0 + nbits): dim i0 + j <-> bit nbits - 1 - j of v
+__device__ __forceinline__ float lf_bits_prod(const float (*sg)[2], int i0, int nbits, int v) {
+  float a = 1.f;
+  for (int j = 0; j < nbits; ++j) a *= sg[i0 + j][(v >> (nbits - 1 - j)) & 1];
+  return a;
+}
+
+__device__ __forceinline__ float lf_plogp(float x) {     // -x log max(x, 1e-5)
+  return x > 1e-5f ? -x * __logf(x) : x * LF_LOG_INV_EPS;
+}
+
+// one block: one code tile (LF_R x 256 codes) of one codebook (blockIdx.z) over one token split (blockIdx.y).  Per code: the sum of
+// prob over the split's tokens; per block: the sum of the clamped entropy terms.  Both into fp64 workspace partials.
+__global__ void __launch_bounds__(256, 1) lfq_fact_partials_kernel(const float* __restrict__ presign, int64_t N, int d, int nc,
+                                                                float inv_temp, int64_t per, double* __restrict__ ws_avg,
+                                                                double* __restrict__ ws_ent) {
+  pdl_wait();
+  pdl_launch_dependents();
+  __shared__ float sg[LF_TT][LF_MAXD][2];       // sigma(-4 tau p), sigma(+4 tau p): probability of code bit 0 / 1
+  __shared__ float tab[LF_TT][3][16];           // per token: low-4-bit products, next-4-bit products, Q[r] = tile factor x r factor
+  __shared__ double red[8];
+  const LfLayout L(d);
+  const int K = 1 << d, tid = threadIdx.x, tile = blockIdx.x, split = blockIdx.y, c = blockIdx.z;
+  const int64_t tbeg = (int64_t)split * per, tend = min(N, tbeg + per);
+  double accd[LF_R], entd = 0.0;
+#pragma unroll
+  for (int r = 0; r < LF_R; ++r) accd[r] = 0.0;
+  for (int64_t t0 = tbeg; t0 < tend; t0 += LF_TT) {
+    const int nt = (int)min((int64_t)LF_TT, tend - t0);
+    for (int e = tid; e < nt * d; e += 256) {
+      const int t = e / d, i = e - t * d;
+      const float x = 4.f * inv_temp * presign[((t0 + t) * nc + c) * d + i];
+      sg[t][i][1] = 1.f / (1.f + expf(-x));
+      sg[t][i][0] = 1.f / (1.f + expf(x));
+    }
+    __syncthreads();
+    for (int e = tid; e < LF_TT * 48; e += 256) {
+      const int t = e / 48, w = e - t * 48, which = w >> 4, v = w & 15;
+      float a = 0.f;
+      if (t < nt) {
+        if (which == 0) a = v < (1 << L.lo4) ? lf_bits_prod(sg[t], d - L.lo4, L.lo4, v) : 0.f;
+        else if (which == 1) a = v < (1 << (L.lb - L.lo4)) ? lf_bits_prod(sg[t], d - L.lb, L.lb - L.lo4, v) : 0.f;
+        else a = v < (1 << L.rb) ? lf_bits_prod(sg[t], L.tb, L.rb, v) * lf_bits_prod(sg[t], 0, L.tb, tile) : 0.f;
+      }
+      tab[t][which][v] = a;
+    }
+    __syncthreads();
+    float acc[LF_R], ent = 0.f;
+#pragma unroll
+    for (int r = 0; r < LF_R; ++r) acc[r] = 0.f;
+    for (int t = 0; t < nt; ++t) {
+      const float b = tab[t][0][tid & 15] * tab[t][1][tid >> 4];     // 0 for the threads past 2^lb codes
+#pragma unroll
+      for (int r = 0; r < LF_R; ++r) {
+        const float pr = tab[t][2][r] * b;
+        acc[r] += pr;
+        ent += lf_plogp(pr);
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < LF_R; ++r) accd[r] += (double)acc[r];
+    entd += (double)ent;
+    __syncthreads();               // sg / tab are rewritten by the next chunk
+  }
+  if (tid < (1 << L.lb)) {
+    double* out = ws_avg + ((int64_t)split * nc + c) * K + ((int64_t)tile << (L.rb + L.lb)) + tid;
+#pragma unroll
+    for (int r = 0; r < LF_R; ++r)
+      if (r < (1 << L.rb)) out[(int64_t)r << L.lb] = accd[r];
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) entd += __shfl_xor_sync(0xffffffffu, entd, o);
+  if ((tid & 31) == 0) red[tid >> 5] = entd;
+  __syncthreads();
+  if (tid == 0) {
+    double s = 0.0;
+    for (int w = 0; w < 8; ++w) s += red[w];
+    ws_ent[((int64_t)split * nc + c) * gridDim.x + tile] = s;
+  }
+}
+
+// avg_prob[i] = sum over the token splits, in split order
+__global__ void __launch_bounds__(256) lfq_fact_avg_kernel(const double* __restrict__ ws_avg, int64_t n, int splits,
+                                                           float* __restrict__ avg_prob) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (i >= n) return;
+  double s = 0.0;
+  for (int k = 0; k < splits; ++k) s += ws_avg[(int64_t)k * n + i];
+  avg_prob[i] = (float)s;
+}
+
+// stats[0] = entropy partials summed in a fixed order, stats[1] = commitment sum  sum (p - sign p)^2  over [N][nc][d]
+__global__ void __launch_bounds__(256) lfq_fact_stats_kernel(const double* __restrict__ ws_ent, int n_ent, const float* __restrict__ presign,
+                                                             int64_t n_pre, float* __restrict__ stats) {
+  pdl_wait();
+  pdl_launch_dependents();
+  __shared__ double red[2][8];
+  double e = 0.0, cm = 0.0;
+  for (int i = threadIdx.x; i < n_ent; i += 256) e += ws_ent[i];
+  for (int64_t i = threadIdx.x; i < n_pre; i += 256) {
+    const float p = presign[i], q = p > 0.f ? 1.f : -1.f;
+    cm += (double)((p - q) * (p - q));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    e += __shfl_xor_sync(0xffffffffu, e, o);
+    cm += __shfl_xor_sync(0xffffffffu, cm, o);
+  }
+  if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = e; red[1][threadIdx.x >> 5] = cm; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double a = 0.0, b = 0.0;
+    for (int w = 0; w < 8; ++w) { a += red[0][w]; b += red[1][w]; }
+    stats[0] = (float)a;
+    stats[1] = (float)b;
+  }
+}
+
+// hga[i] = coef_batch * h'(avg_global[i]),  h'(x) = -(log x + 1) for x > 1e-5, -log 1e-5 below the clamp
+__global__ void __launch_bounds__(256) lfq_fact_hga_kernel(const float* __restrict__ avg, int64_t n, float coef_batch,
+                                                           float* __restrict__ hga) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+  if (i >= n) return;
+  const float a = avg[i];
+  hga[i] = coef_batch * (a > 1e-5f ? -(logf(a) + 1.f) : LF_LOG_INV_EPS);
+}
+
+// Backward of  coef_sample * sum_t H(prob_t) - coef_batch * <h'(avg_global), sum_t prob_t>  (the entropy part of LFQ's aux loss,
+// with avg entering as avg_local + (avg_global - avg_local).detach()) with respect to the pre-sign values:
+//   c_tk = prob_tk (coef_sample h'(prob_tk) - coef_batch h'(avg_global_k)),   dp_ti = 2 tau (sum_k c_tk s_ki - tanh(2 tau p_ti) sum_k c_tk)
+// One warp per (token, codebook) walks all 2^d codes.  Code bit layout (LSB first): min(d, 5) bits -> lane, the next min(d - 5, 5)
+// bits -> the warp's 32 register columns j, the rest -> the outer loop.  The bit sums come from the per-column sums M[j], the
+// per-outer-step sums and the lane's total, so the cost is O(2^d) per token, not O(2^d d).
+__global__ void __launch_bounds__(LF_BW_WARPS * 32) lfq_fact_backward_kernel(const float* __restrict__ presign, const float* __restrict__ hga,
+                                                                int64_t N, int d, int nc, float inv_temp, float coef_sample,
+                                                                float* __restrict__ grad) {
+  pdl_wait();
+  pdl_launch_dependents();
+  __shared__ float sgw[LF_BW_WARPS][LF_MAXD][2];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t pair = (int64_t)blockIdx.x * LF_BW_WARPS + warp;   // token * nc + codebook
+  if (pair >= N * nc) return;
+  const int c = (int)(pair % nc), K = 1 << d;
+  const int lbb = d < 5 ? d : 5, mbb = d - lbb < 5 ? d - lbb : 5, tbb = d - lbb - mbb;
+  const float* pp = presign + pair * d;
+  float pi = 0.f;
+  if (lane < d) {
+    pi = pp[lane];
+    const float x = 4.f * inv_temp * pi;
+    sgw[warp][lane][1] = 1.f / (1.f + expf(-x));
+    sgw[warp][lane][0] = 1.f / (1.f + expf(x));
+  }
+  __syncwarp();
+  const float (*sg)[2] = sgw[warp];
+  const float b = lane < (1 << lbb) ? lf_bits_prod(sg, d - lbb, lbb, lane) : 0.f;
+  const float am = lane < (1 << mbb) ? lf_bits_prod(sg, tbb, mbb, lane) : 0.f;
+  float P[32], M[32], Ht[LF_MAXD - 10];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) { P[j] = __shfl_sync(0xffffffffu, am, j) * b; M[j] = 0.f; }
+#pragma unroll
+  for (int i = 0; i < LF_MAXD - 10; ++i) Ht[i] = 0.f;
+  const float* hg = hga + (int64_t)c * K;
+  const bool live = lane < (1 << lbb);
+  for (int tp = 0; tp < (1 << tbb); ++tp) {
+    const float at = lf_bits_prod(sg, 0, tbb, tp);
+    const int base = (tp << (mbb + lbb)) + lane;
+    float u = 0.f;
+#pragma unroll
+    for (int j = 0; j < 32; ++j) {
+      if (j < (1 << mbb)) {
+        const float pr = at * P[j];
+        const float h = live ? __ldg(hg + base + (j << lbb)) : 0.f;
+        const float hp = pr > 1e-5f ? -(__logf(pr) + 1.f) : LF_LOG_INV_EPS;
+        const float cv = pr * fmaf(coef_sample, hp, -h);
+        M[j] += cv;
+        u += cv;
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < LF_MAXD - 10; ++i)
+      if (i < tbb) Ht[i] += ((tp >> (tbb - 1 - i)) & 1) ? u : -u;
+  }
+  float T = 0.f;
+#pragma unroll
+  for (int j = 0; j < 32; ++j) T += M[j];
+  float g = 0.f;
+#pragma unroll
+  for (int i = 0; i < LF_MAXD; ++i) {
+    if (i < d) {
+      float v = 0.f;
+      if (i < tbb) {
+        if (i < LF_MAXD - 10) v = Ht[i];
+      } else if (i < tbb + mbb) {
+        const int q = mbb - 1 - (i - tbb);
+#pragma unroll
+        for (int j = 0; j < 32; ++j) v += ((j >> q) & 1) ? M[j] : -M[j];
+      } else {
+        v = ((lane >> (d - 1 - i)) & 1) ? T : -T;
+      }
+      v = warp_sum(v);
+      if (lane == i) g = v;
+    }
+  }
+  T = warp_sum(T);
+  if (lane < d) grad[pair * d + lane] = 2.f * inv_temp * (g - tanhf(2.f * inv_temp * pi) * T);
+}
+
+// LFQ auxiliary loss for codebooks past the one-block 256-thread finalize (d > 12): the same terms, fp64 sums in a fixed order
+__global__ void __launch_bounds__(1024) lfq_aux_final_wide_kernel(const float* __restrict__ avg_prob_sum, const float* __restrict__ stats,
+                                                                  int64_t n, int nc, float inv_tokens_global, float inv_tokens,
+                                                                  float inv_elems, float gamma, float w_entropy, float w_commit,
+                                                                  float* __restrict__ out) {
+  pdl_wait();
+  pdl_launch_dependents();
+  __shared__ double sw[32];
+  double t = 0.0;
+  for (int64_t k = threadIdx.x; k < n; k += 1024) {
+    const float p = avg_prob_sum[k] * inv_tokens_global;
+    t += (double)(-p * logf(fmaxf(p, 1e-5f)));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  if ((threadIdx.x & 31) == 0) sw[threadIdx.x >> 5] = t;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double s = 0.0;
+    for (int w = 0; w < 32; ++w) s += sw[w];
+    const float be = (float)(s / nc);
+    const float ps = stats[0] * inv_tokens, cm = stats[1] * inv_elems;
+    out[0] = ps; out[1] = be; out[2] = cm;
+    out[3] = (ps - gamma * be) * w_entropy + cm * w_commit;
+  }
+}
 
 // ------------------------------------------------------------------------------------------
 // gateloop_time (reference M:1216-1222: ToTimeSequence(Residual(SimpleGateLoopLayer))): per (clip, pixel, channel) the gated
@@ -2108,6 +2390,42 @@ static int launch_attention(const mv2_attn_args* a, cudaStream_t st) {
     case 3: launch_k(attention_kernel<T, 3>, dim3(grid), dim3(128), 0, st, *a); break;
     default: set_error("dim_head %d unsupported", a->dim_head); return MV2_E_UNSUPPORTED;
   }
+  MV2_CHECK_LAUNCH();
+  return MV2_OK;
+}
+
+// quantiser launches for one max-dims instantiation (MODE 0: LFQ, 1: FSQ); `levels` (FSQ) has d entries, checked by the caller
+template <int MODE, int MAXD>
+static int launch_quant_forward(const void* x, int dtype, int64_t N, int C, int d, int nc, const float* win, const float* bin,
+                                const float* wout, const float* bout, float clamp, int spherical, const int32_t* levels,
+                                int64_t* idx64, int32_t* idx32, void* quantized, float* aux, cudaStream_t st) {
+  FsqLevelsT<MAXD> lv = {};
+  for (int i = 0; levels && i < d; ++i) lv.lv[i] = levels[i];
+  const int blocks = ceil_div(N, 8);
+  if (dtype == MV2_F32)
+    launch_k(quant_forward_kernel<float, MODE, MAXD>, dim3(blocks), dim3(256), 0, st, (const float*)x, N, C, d, nc, win, bin, wout, bout,
+             clamp, spherical, lv, idx64, idx32, (float*)quantized, aux);
+  else if (dtype == MV2_BF16)
+    launch_k(quant_forward_kernel<__nv_bfloat16, MODE, MAXD>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, N, C, d, nc, win,
+             bin, wout, bout, clamp, spherical, lv, idx64, idx32, (__nv_bfloat16*)quantized, aux);
+  else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
+  MV2_CHECK_LAUNCH();
+  return MV2_OK;
+}
+
+template <int MODE, int MAXD>
+static int launch_quant_decode(const void* indices, int is64, int64_t N, int C, int d, int nc, const int32_t* levels,
+                               const float* wout, const float* bout, void* quantized, int dtype, cudaStream_t st) {
+  FsqLevelsT<MAXD> lv = {};
+  for (int i = 0; levels && i < d; ++i) lv.lv[i] = levels[i];
+  const int blocks = ceil_div(N, 8);
+  if (dtype == MV2_F32)
+    launch_k(quant_decode_kernel<float, MODE, MAXD>, dim3(blocks), dim3(256), 0, st, indices, is64, N, C, d, nc, lv, wout, bout,
+             (float*)quantized);
+  else if (dtype == MV2_BF16)
+    launch_k(quant_decode_kernel<__nv_bfloat16, MODE, MAXD>, dim3(blocks), dim3(256), 0, st, indices, is64, N, C, d, nc, lv, wout, bout,
+             (__nv_bfloat16*)quantized);
+  else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }
@@ -2473,70 +2791,46 @@ int mv2_lfq_forward(const void* x, int dtype, int64_t N, int C, int d, int num_c
                     const float* wout, const float* bout, float clamp, int spherical, int64_t* indices, void* quantized,
                     float* presign, void* stream) {
   const int nc = num_codebooks;
-  MV2_CHECK_ARG(x && win && bin && N > 0 && C > 0 && d > 0 && nc > 0 && d * nc <= Q_MAXD);
+  MV2_CHECK_ARG(x && win && bin && N > 0 && C > 0 && d > 0 && nc > 0 && d * nc <= Q_MAXD_WIDE);
   MV2_CHECK_ARG(!quantized || (wout && bout));
-  FsqLevels lv = {};
-  const int blocks = ceil_div(N, 8);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == MV2_F32)
-    launch_k(quant_forward_kernel<float, 0>, dim3(blocks), dim3(256), 0, st, (const float*)x, N, C, d, nc, win, bin, wout, bout, clamp, spherical, lv, indices, nullptr, (float*)quantized, presign);
-  else if (dtype == MV2_BF16)
-    launch_k(quant_forward_kernel<__nv_bfloat16, 0>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, N, C, d, nc, win, bin, wout, bout, clamp, spherical, lv, indices, nullptr, (__nv_bfloat16*)quantized, presign);
-  else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
-  MV2_CHECK_LAUNCH();
-  return MV2_OK;
+  return d * nc <= Q_MAXD ? launch_quant_forward<0, Q_MAXD>(x, dtype, N, C, d, nc, win, bin, wout, bout, clamp, spherical, nullptr,
+                                                            indices, nullptr, quantized, presign, (cudaStream_t)stream)
+                          : launch_quant_forward<0, Q_MAXD_WIDE>(x, dtype, N, C, d, nc, win, bin, wout, bout, clamp, spherical, nullptr,
+                                                                 indices, nullptr, quantized, presign, (cudaStream_t)stream);
 }
 
 int mv2_lfq_decode(const void* indices, int index_is_i64, int64_t N, int C, int d, int num_codebooks, const float* wout,
                    const float* bout, void* quantized, int dtype, void* stream) {
   const int nc = num_codebooks;
-  MV2_CHECK_ARG(indices && wout && bout && quantized && N > 0 && C > 0 && d > 0 && nc > 0 && d * nc <= Q_MAXD);
-  FsqLevels lv = {};
-  const int blocks = ceil_div(N, 8);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == MV2_F32)
-    launch_k(quant_decode_kernel<float, 0>, dim3(blocks), dim3(256), 0, st, indices, index_is_i64, N, C, d, nc, lv, wout, bout, (float*)quantized);
-  else if (dtype == MV2_BF16)
-    launch_k(quant_decode_kernel<__nv_bfloat16, 0>, dim3(blocks), dim3(256), 0, st, indices, index_is_i64, N, C, d, nc, lv, wout, bout, (__nv_bfloat16*)quantized);
-  else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
-  MV2_CHECK_LAUNCH();
-  return MV2_OK;
+  MV2_CHECK_ARG(indices && wout && bout && quantized && N > 0 && C > 0 && d > 0 && nc > 0 && d * nc <= Q_MAXD_WIDE);
+  return d * nc <= Q_MAXD ? launch_quant_decode<0, Q_MAXD>(indices, index_is_i64, N, C, d, nc, nullptr, wout, bout, quantized, dtype,
+                                                           (cudaStream_t)stream)
+                          : launch_quant_decode<0, Q_MAXD_WIDE>(indices, index_is_i64, N, C, d, nc, nullptr, wout, bout, quantized, dtype,
+                                                                (cudaStream_t)stream);
 }
 
 int mv2_fsq_forward(const void* x, int dtype, int64_t N, int C, int d, int num_codebooks, const int32_t* levels, const float* win,
                     const float* bin, const float* wout, const float* bout, int32_t* indices, void* quantized,
                     float* bounded, void* stream) {
   const int nc = num_codebooks;
-  MV2_CHECK_ARG(x && levels && win && bin && N > 0 && C > 0 && d > 0 && nc > 0 && d * nc <= Q_MAXD);
+  MV2_CHECK_ARG(x && levels && win && bin && N > 0 && C > 0 && d > 0 && nc > 0 && d * nc <= Q_MAXD_WIDE);
   MV2_CHECK_ARG(!quantized || (wout && bout));
-  FsqLevels lv = {};
-  for (int i = 0; i < d; ++i) { MV2_CHECK_ARG(levels[i] >= 2); lv.lv[i] = levels[i]; }
-  const int blocks = ceil_div(N, 8);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == MV2_F32)
-    launch_k(quant_forward_kernel<float, 1>, dim3(blocks), dim3(256), 0, st, (const float*)x, N, C, d, nc, win, bin, wout, bout, 0.f, 0, lv, nullptr, indices, (float*)quantized, bounded);
-  else if (dtype == MV2_BF16)
-    launch_k(quant_forward_kernel<__nv_bfloat16, 1>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, N, C, d, nc, win, bin, wout, bout, 0.f, 0, lv, nullptr, indices, (__nv_bfloat16*)quantized, bounded);
-  else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
-  MV2_CHECK_LAUNCH();
-  return MV2_OK;
+  for (int i = 0; i < d; ++i) MV2_CHECK_ARG(levels[i] >= 2);
+  return d * nc <= Q_MAXD ? launch_quant_forward<1, Q_MAXD>(x, dtype, N, C, d, nc, win, bin, wout, bout, 0.f, 0, levels, nullptr,
+                                                            indices, quantized, bounded, (cudaStream_t)stream)
+                          : launch_quant_forward<1, Q_MAXD_WIDE>(x, dtype, N, C, d, nc, win, bin, wout, bout, 0.f, 0, levels, nullptr,
+                                                                 indices, quantized, bounded, (cudaStream_t)stream);
 }
 
 int mv2_fsq_decode(const void* indices, int index_is_i64, int64_t N, int C, int d, int num_codebooks, const int32_t* levels,
                    const float* wout, const float* bout, void* quantized, int dtype, void* stream) {
   const int nc = num_codebooks;
-  MV2_CHECK_ARG(indices && levels && wout && bout && quantized && N > 0 && C > 0 && d > 0 && nc > 0 && d * nc <= Q_MAXD);
-  FsqLevels lv = {};
-  for (int i = 0; i < d; ++i) { MV2_CHECK_ARG(levels[i] >= 2); lv.lv[i] = levels[i]; }
-  const int blocks = ceil_div(N, 8);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == MV2_F32)
-    launch_k(quant_decode_kernel<float, 1>, dim3(blocks), dim3(256), 0, st, indices, index_is_i64, N, C, d, nc, lv, wout, bout, (float*)quantized);
-  else if (dtype == MV2_BF16)
-    launch_k(quant_decode_kernel<__nv_bfloat16, 1>, dim3(blocks), dim3(256), 0, st, indices, index_is_i64, N, C, d, nc, lv, wout, bout, (__nv_bfloat16*)quantized);
-  else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
-  MV2_CHECK_LAUNCH();
-  return MV2_OK;
+  MV2_CHECK_ARG(indices && levels && wout && bout && quantized && N > 0 && C > 0 && d > 0 && nc > 0 && d * nc <= Q_MAXD_WIDE);
+  for (int i = 0; i < d; ++i) MV2_CHECK_ARG(levels[i] >= 2);
+  return d * nc <= Q_MAXD ? launch_quant_decode<1, Q_MAXD>(indices, index_is_i64, N, C, d, nc, levels, wout, bout, quantized, dtype,
+                                                           (cudaStream_t)stream)
+                          : launch_quant_decode<1, Q_MAXD_WIDE>(indices, index_is_i64, N, C, d, nc, levels, wout, bout, quantized, dtype,
+                                                                (cudaStream_t)stream);
 }
 
 int mv2_lfq_entropy_partials(const float* presign, int64_t N, int d, int num_codebooks, float inv_temperature, float* avg_prob,
@@ -2546,6 +2840,50 @@ int mv2_lfq_entropy_partials(const float* presign, int64_t N, int d, int num_cod
   const int blocks = ceil_div(N, LE_TOK);
   launch_k(lfq_entropy_kernel, dim3(dim3(blocks, num_codebooks)), dim3(256), K * sizeof(float), (cudaStream_t)stream, presign, N, d, num_codebooks,
            inv_temperature, avg_prob, stats);
+  MV2_CHECK_LAUNCH();
+  return MV2_OK;
+}
+
+size_t mv2_lfq_entropy_fact_workspace_bytes(int64_t n_tokens, int d, int num_codebooks) {
+  if (n_tokens <= 0 || d < 1 || d > LF_MAXD || num_codebooks <= 0) return 0;
+  const LfSplit s = lf_split(n_tokens, d, num_codebooks);
+  const size_t K = (size_t)1 << d, nc = (size_t)num_codebooks;
+  const size_t fwd = (size_t)s.splits * nc * (K + (size_t)s.tiles) * sizeof(double), bwd = nc * K * sizeof(float);
+  return std::max(fwd, bwd);
+}
+
+int mv2_lfq_entropy_fact_partials(const float* presign, int64_t N, int d, int num_codebooks, float inv_temperature, float* avg_prob,
+                                  float* stats, void* workspace, void* stream) {
+  const int nc = num_codebooks;
+  MV2_CHECK_ARG(presign && avg_prob && stats && workspace && N > 0 && d >= 1 && d <= LF_MAXD && nc > 0 && d * nc <= Q_MAXD_WIDE);
+  const LfSplit s = lf_split(N, d, nc);
+  cudaStream_t st = (cudaStream_t)stream;
+  double* ws_avg = (double*)workspace;
+  const int64_t n = (int64_t)nc << d;
+  double* ws_ent = ws_avg + (int64_t)s.splits * n;
+  launch_k(lfq_fact_partials_kernel, dim3(s.tiles, s.splits, nc), dim3(256), 0, st, presign, N, d, nc, inv_temperature, s.per,
+           ws_avg, ws_ent);
+  MV2_CHECK_LAUNCH();
+  launch_k(lfq_fact_avg_kernel, dim3(ceil_div(n, 256)), dim3(256), 0, st, (const double*)ws_avg, n, s.splits, avg_prob);
+  MV2_CHECK_LAUNCH();
+  launch_k(lfq_fact_stats_kernel, dim3(1), dim3(256), 0, st, (const double*)ws_ent, s.splits * nc * s.tiles, presign, N * nc * d, stats);
+  MV2_CHECK_LAUNCH();
+  return MV2_OK;
+}
+
+int mv2_lfq_entropy_fact_backward(const float* presign, const float* avg_global, int64_t N, int d, int num_codebooks,
+                                  float inv_temperature, float coef_sample, float coef_batch, float* grad_presign, void* workspace,
+                                  void* stream) {
+  const int nc = num_codebooks;
+  MV2_CHECK_ARG(presign && avg_global && grad_presign && workspace && N > 0 && d >= 1 && d <= LF_MAXD && nc > 0 &&
+                d * nc <= Q_MAXD_WIDE);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t n = (int64_t)nc << d;
+  float* hga = (float*)workspace;
+  launch_k(lfq_fact_hga_kernel, dim3(ceil_div(n, 256)), dim3(256), 0, st, avg_global, n, coef_batch, hga);
+  MV2_CHECK_LAUNCH();
+  launch_k(lfq_fact_backward_kernel, dim3(ceil_div(N * nc, LF_BW_WARPS)), dim3(LF_BW_WARPS * 32), 0, st, presign, (const float*)hga, N, d, nc, inv_temperature,
+           coef_sample, grad_presign);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }
@@ -2573,10 +2911,15 @@ size_t mv2_mse_workspace_bytes(void) { return (size_t)MSE_BLOCKS * sizeof(double
 int mv2_lfq_aux_finalize(const float* avg_prob_sum, const float* stats, int d, int num_codebooks, int64_t n_tokens, int64_t n_tokens_global,
                          float diversity_gamma, float entropy_weight, float commitment_weight, float* out4, void* stream) {
   const int nc = num_codebooks;
-  MV2_CHECK_ARG(avg_prob_sum && stats && out4 && d > 0 && d <= 12 && nc > 0 && n_tokens > 0 && n_tokens_global > 0);
-  launch_k(lfq_aux_final_kernel, dim3(1), dim3(256), 0, (cudaStream_t)stream, avg_prob_sum, stats, 1 << d, nc,
-           (float)(1.0 / (double)n_tokens_global), (float)(1.0 / ((double)n_tokens * nc)), (float)(1.0 / ((double)n_tokens * nc * d)),
-           diversity_gamma, entropy_weight, commitment_weight, out4);
+  MV2_CHECK_ARG(avg_prob_sum && stats && out4 && d > 0 && d <= LF_MAXD && nc > 0 && n_tokens > 0 && n_tokens_global > 0);
+  const float inv_g = (float)(1.0 / (double)n_tokens_global), inv_t = (float)(1.0 / ((double)n_tokens * nc)),
+              inv_e = (float)(1.0 / ((double)n_tokens * nc * d));
+  if (d <= 12)
+    launch_k(lfq_aux_final_kernel, dim3(1), dim3(256), 0, (cudaStream_t)stream, avg_prob_sum, stats, 1 << d, nc, inv_g, inv_t, inv_e,
+             diversity_gamma, entropy_weight, commitment_weight, out4);
+  else
+    launch_k(lfq_aux_final_wide_kernel, dim3(1), dim3(1024), 0, (cudaStream_t)stream, avg_prob_sum, stats, (int64_t)nc << d, nc, inv_g,
+             inv_t, inv_e, diversity_gamma, entropy_weight, commitment_weight, out4);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }

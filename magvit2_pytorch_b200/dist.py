@@ -3,8 +3,9 @@ GPUs, gloo in the CPU tests) for the plumbing.
 
 The eval forward is batch independent, so clips are simply sharded across ranks with NO data-path collective.
 The only collective on the path is LFQ's training-mode batch-entropy term (SURVEY.md Appendix A.1 step 7; reached
-from reference M:1705): every rank's mean code-probability vector ``avg_prob`` (num_codebooks x codebook_size fp32
-= 4 KiB at the README config) is summed over ranks and divided by the world size.  It is latency bound, so it is
+from reference M:1705): every rank's mean code-probability vector ``avg_prob`` (num_codebooks x codebook_size fp32:
+nc * 2^d * 4 bytes, 4 KiB at the README config, 1 MiB at MAGVIT-v2's 2^18 codes) is summed over ranks and divided by the
+world size.  It is latency bound, so it is
 issued on a side stream and overlaps whatever the caller runs next (the decoder).
 """
 from __future__ import annotations
@@ -53,10 +54,24 @@ def entropy_from_avg_prob(avg_prob: torch.Tensor, eps: float = 1e-5) -> torch.Te
     return (-avg_prob * torch.log(avg_prob.clamp(min=eps))).sum(dim=-1)
 
 
+# codebook dims per codebook (d = log2(codebook_size)) of the LFQ training-mode terms: up to LFQ_DENSE_MAX_D the per-token
+# softmax over all 2^d codes runs in shared memory (mv2_lfq_entropy_partials); above, the bit-factorised kernels take it
+# (mv2_lfq_entropy_fact_*, d <= LFQ_TRAIN_MAX_D)
+LFQ_DENSE_MAX_D = 12
+LFQ_TRAIN_MAX_D = 20
+
+
+def check_lfq_train_dim(d: int):
+    if d > LFQ_TRAIN_MAX_D:
+        raise NotImplementedError(f"LFQ training-mode losses take codebook_size <= 2^{LFQ_TRAIN_MAX_D} per codebook "
+                                  f"(got 2^{d}); tokenize / decode take any size up to 32 projected dims")
+
+
 class LfqBatchEntropy:
-    """LFQ training-mode auxiliary terms on the GPU: per-rank partials by mv2_lfq_entropy_partials, then the 4 KiB
-    all-reduce on a side stream.  start() launches; finish() returns
-    (per_sample_entropy, batch_entropy, commitment, aux_loss) as 0-d tensors."""
+    """LFQ training-mode auxiliary terms on the GPU: per-rank partials (mv2_lfq_entropy_partials for d <= 12, the
+    bit-factorised mv2_lfq_entropy_fact_partials for 12 < d <= 20), then the all-reduce of avg_prob (nc * 2^d * 4 bytes)
+    on a side stream.  start() launches; finish() returns (per_sample_entropy, batch_entropy, commitment, aux_loss) as
+    0-d tensors."""
 
     def __init__(self, engine, inv_temperature: float = 100.0, num_codebooks: int = 1):
         self.eng = engine
@@ -70,18 +85,28 @@ class LfqBatchEntropy:
         eng = self.eng
         N, D = presign.shape
         d = D // self.nc                 # presign is [N][num_codebooks][d]
+        check_lfq_train_dim(d)
         K = 1 << d
         avg = torch.zeros(self.nc * K, device=presign.device, dtype=torch.float32)
         stats = torch.zeros(2, device=presign.device, dtype=torch.float32)
+        ws = None
+        if d > LFQ_DENSE_MAX_D:
+            ws = torch.empty(eng.lib.mv2_lfq_entropy_fact_workspace_bytes(N, d, self.nc), device=presign.device, dtype=torch.uint8)
         self.side.wait_stream(torch.cuda.current_stream(eng.device))
         with torch.cuda.stream(self.side):
-            check(eng.lib.mv2_lfq_entropy_partials(presign.data_ptr(), N, d, self.nc, float(self.inv_temperature), avg.data_ptr(),
-                                                   stats.data_ptr(), C.c_void_p(self.side.cuda_stream)),
-                  "mv2_lfq_entropy_partials")
+            st = C.c_void_p(self.side.cuda_stream)
+            if ws is None:
+                check(eng.lib.mv2_lfq_entropy_partials(presign.data_ptr(), N, d, self.nc, float(self.inv_temperature), avg.data_ptr(),
+                                                       stats.data_ptr(), st), "mv2_lfq_entropy_partials")
+            else:
+                check(eng.lib.mv2_lfq_entropy_fact_partials(presign.data_ptr(), N, d, self.nc, float(self.inv_temperature),
+                                                            avg.data_ptr(), stats.data_ptr(), ws.data_ptr(), st),
+                      "mv2_lfq_entropy_fact_partials")
+                ws.record_stream(self.side)
             eng.launches += 1
             avg.div_(N)                       # local mean code probability
             if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
-                dist.all_reduce(avg, op=dist.ReduceOp.SUM, group=group)    # the one collective of the path (NCCL, 4 KiB)
+                dist.all_reduce(avg, op=dist.ReduceOp.SUM, group=group)    # the one collective of the path (NCCL, nc * 2^d * 4 bytes)
         presign.record_stream(self.side)
         self._pending = (avg, stats, N, d)
 

@@ -303,8 +303,8 @@ class LFQ(_NoForward):
         cdims = d * self.num_codebooks
         if dim == cdims:
             raise NotImplementedError("LFQ without projections (dim == log2(codebook_size) * num_codebooks) is not supported")
-        if cdims > 16:
-            raise NotImplementedError("the quantiser kernels take at most 16 projected dims (log2(codebook_size) * num_codebooks)")
+        if cdims > 32:
+            raise NotImplementedError("the quantiser kernels take at most 32 projected dims (log2(codebook_size) * num_codebooks)")
         self.project_in = nn.Linear(dim, cdims)
         self.project_out = nn.Linear(cdims, dim)
         self.register_buffer("mask", 2 ** torch.arange(d - 1, -1, -1))
@@ -322,8 +322,8 @@ class FSQ(_NoForward):
         cdims = len(levels) * self.num_codebooks
         if dim == cdims:
             raise NotImplementedError("FSQ without projections is not supported")
-        if cdims > 16:
-            raise NotImplementedError("the quantiser kernels take at most 16 projected dims (len(levels) * num_codebooks)")
+        if cdims > 32:
+            raise NotImplementedError("the quantiser kernels take at most 32 projected dims (len(levels) * num_codebooks)")
         self.project_in = nn.Linear(dim, cdims)
         self.project_out = nn.Linear(cdims, dim)
 

@@ -21,12 +21,14 @@ Reference lines: M: = magvit2_pytorch/magvit2_pytorch.py, A: = attend.py.
 """
 from __future__ import annotations
 
+import ctypes as C
 from typing import Callable, Dict, List, Sequence
 
 import torch
 import torch.nn.functional as F
 
 from ._lib import ACT_ELU
+from .dist import LFQ_DENSE_MAX_D
 from .engine import pack_conv
 
 
@@ -186,15 +188,64 @@ def _lfq_train(x, qz, avg_global, inv_temperature=100.):
     qd = torch.where(p > 0, torch.ones_like(p), -torch.ones_like(p))
     st = (p + (qd - p).detach()).reshape(*x.shape[:-1], nc * d)
     out = F.linear(st.to(x.dtype), qz.project_out.weight, qz.project_out.bias)
+    commit = ((p - qd) ** 2).mean()
+    if d > LFQ_DENSE_MAX_D:
+        ent = _LfqEntropyFact.apply(p.contiguous(), avg_global.reshape(-1).float().contiguous(), inv_temperature,
+                                    qz.entropy_loss_weight, qz.diversity_gamma)
+        return out, ent + commit * qz.commitment_loss_weight
     mask = qz.mask.to(p.device)
     codebook = ((torch.arange(2 ** d, device=p.device)[:, None] & mask) != 0).float() * 2 - 1
     prob = (2 * inv_temperature * torch.einsum("tcd,kd->tck", p, codebook)).softmax(dim=-1)      # (tokens, nc, K)
     per_sample = _entropy(prob).mean()
     avg_local = prob.mean(dim=0)                                                                  # (nc, K)
     avg = avg_local + (avg_global.reshape(nc, -1) - avg_local).detach()
-    commit = ((p - qd) ** 2).mean()
     aux = (per_sample - qz.diversity_gamma * _entropy(avg).mean()) * qz.entropy_loss_weight + commit * qz.commitment_loss_weight
     return out, aux
+
+
+class _LfqEntropyFact(torch.autograd.Function):
+    """The entropy part of LFQ's aux loss, entropy_weight * (per_sample_entropy - diversity_gamma * batch_entropy), for
+    codebooks of 2^13 .. 2^20 codes, where the dense (tokens, nc, 2^d) probabilities of _lfq_train's d <= 12 path would take
+    gigabytes.  The code distribution factorises over bits (DESIGN.md), so the value comes from mv2_lfq_entropy_fact_partials
+    and mv2_lfq_aux_finalize and the gradient of the pre-sign values from mv2_lfq_entropy_fact_backward, both O(tokens 2^d)
+    with no per-token table of size 2^d.  The batch term is taken at the cross-rank mean `avg_global`, whose gradient reaches
+    the local tokens as through _lfq_train's avg_local + (avg_global - avg_local).detach()."""
+
+    @staticmethod
+    def forward(ctx, p, avg_global, inv_temperature, entropy_weight, diversity_gamma):
+        from ._lib import check, load
+        lib = load()
+        N, nc, d = p.shape
+        dev = p.device
+        st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+        ws = torch.empty(lib.mv2_lfq_entropy_fact_workspace_bytes(N, d, nc), device=dev, dtype=torch.uint8)
+        avg_local = torch.empty(nc << d, device=dev, dtype=torch.float32)
+        stats = torch.empty(2, device=dev, dtype=torch.float32)
+        check(lib.mv2_lfq_entropy_fact_partials(p.data_ptr(), N, d, nc, float(inv_temperature), avg_local.data_ptr(), stats.data_ptr(),
+                                                ws.data_ptr(), st), "mv2_lfq_entropy_fact_partials")
+        out4 = torch.empty(4, device=dev, dtype=torch.float32)
+        # avg_global is already a mean (n_tokens_global = 1); out4 = (per_sample, batch_entropy, commitment, aux) with the
+        # commitment left to autograd (weight 0 here)
+        check(lib.mv2_lfq_aux_finalize(avg_global.data_ptr(), stats.data_ptr(), d, nc, N, 1, float(diversity_gamma), float(entropy_weight),
+                                       0.0, out4.data_ptr(), st), "mv2_lfq_aux_finalize")
+        ctx.save_for_backward(p, avg_global)
+        ctx.coefs = (float(inv_temperature), entropy_weight / (N * nc), entropy_weight * diversity_gamma / (N * nc))
+        return out4[3].clone()
+
+    @staticmethod
+    def backward(ctx, g):
+        from ._lib import check, load
+        lib = load()
+        p, avg_global = ctx.saved_tensors
+        N, nc, d = p.shape
+        inv_t, coef_sample, coef_batch = ctx.coefs
+        dev = p.device
+        ws = torch.empty(lib.mv2_lfq_entropy_fact_workspace_bytes(N, d, nc), device=dev, dtype=torch.uint8)
+        gp = torch.empty_like(p)
+        check(lib.mv2_lfq_entropy_fact_backward(p.data_ptr(), avg_global.data_ptr(), N, d, nc, inv_t, coef_sample, coef_batch, gp.data_ptr(),
+                                                ws.data_ptr(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+              "mv2_lfq_entropy_fact_backward")
+        return gp * g, None, None, None, None
 
 
 def _fsq_train(x, qz):

@@ -531,7 +531,7 @@ class VideoTokenizer(nn.Module):
     def lfq_loss_breakdown(self, video, group=None):
         """Training-mode LFQ auxiliary terms the reference computes at M:1705 (``quantizer_loss_breakdown``):
         returns ``(codes, (per_sample_entropy, batch_entropy, commitment), aux_loss)``.  ``batch_entropy`` uses the
-        cross-rank mean code probability -- the single 4 KiB all-reduce of the path (dist.LfqBatchEntropy), issued
+        cross-rank mean code probability -- the single all-reduce of the path (num_codebooks * codebook_size * 4 bytes) (dist.LfqBatchEntropy), issued
         on a side stream.  (The losses' backward and the GAN/perceptual terms are out of scope, SURVEY.md 8f N2.)"""
         from .dist import LfqBatchEntropy
         assert not self.use_fsq, "FSQ has no auxiliary loss (reference M:1702)"
@@ -550,7 +550,7 @@ class VideoTokenizer(nn.Module):
         in training mode): besides codes / reconstruction the quantiser's auxiliary terms are computed -- per-sample entropy,
         batch (codebook) entropy of the CROSS-RANK mean code probability, commitment -- and kept in
         ``self.quantizer_loss_breakdown`` = (per_sample_entropy, batch_entropy, commitment) / ``self.quantizer_aux_loss``.
-        The batch-entropy term needs the one collective of the path: a 4 KiB SUM all-reduce of avg_prob (A.1 step 7), issued
+        The batch-entropy term needs the one collective of the path: a SUM all-reduce of avg_prob (num_codebooks * codebook_size * 4 bytes) (A.1 step 7), issued
         on a side stream so that it overlaps the decoder.  The decoder is fed the quantised value q itself; the reference's
         straight-through ``x + (q - x).detach()`` equals q up to one rounding (SURVEY 8d cfg 3).  No autograd (N2)."""
         from .dist import LfqBatchEntropy
