@@ -161,6 +161,23 @@ typedef struct mv2_attn_args {
 } mv2_attn_args;
 int mv2_attention(const mv2_attn_args* a, void* stream);
 
+/* ---- attention dropout (Attend's dropout on the softmax weights in training mode, A:175 / A:239) --------------------
+ * mv2_attention_dropout: mv2_attention (same kernels choice, same arguments) with every softmax weight, memory key/values
+ *   included, kept with probability 1 - p and scaled by 1 / (1 - p); the softmax denominator is the undropped one:
+ *     o_i = fp32(1 / (1 - p)) * sum_j keep_ij softmax_ij v_j.
+ * keep_ij is a pure function of (seed, call, sequence s = o * n_inner + n, head h, query i, key j), j in [0, n_mem + L)
+ *   counting the memory slots first: with r = Philox4x32-10(counter (i, j >> 2, s, h | call << 16), key (seed low, seed
+ *   high word)), keep_ij = r[j & 3] >= floor(p * 2^32) (p the fp32 value, widened to double).
+ * mv2_attention_dropout_mask: writes that mask, uint8 keep[s][h][i][n_mem + L] (s < n_seq), including the entries a
+ *   causal mask hides.  Both need 0 < p < 1, heads < 2^16 and call < 2^16 (MV2_E_ARG otherwise).                      */
+typedef struct mv2_dropout_args {
+  uint64_t seed;
+  uint32_t call;   /* index of the attention call within one forward: distinct calls draw independent masks */
+  float p;
+} mv2_dropout_args;
+int mv2_attention_dropout(const mv2_attn_args* a, const mv2_dropout_args* d, void* stream);
+int mv2_attention_dropout_mask(int n_seq, int heads, int L, int n_mem, const mv2_dropout_args* d, uint8_t* keep, void* stream);
+
 /* ---- Taylor-series linear attention core (TaylorSeriesLinearAttn, un-vendored dependency;
  * SURVEY.md Appendix A.3; called at M:430).  q: [Ntok][heads*8], kv: [Ntok][2*heads*8] '(kv h d)',
  * out: [Ntok][heads*8]; sequences are n_seq contiguous runs of L tokens.  dim_head must be 8.

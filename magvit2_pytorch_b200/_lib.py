@@ -45,6 +45,11 @@ class AttnArgs(C.Structure):
     ]
 
 
+class DropoutArgs(C.Structure):
+    """mv2_dropout_args (attention dropout; see include/magvit2_b200.h)."""
+    _fields_ = [("seed", C.c_uint64), ("call", C.c_uint32), ("p", C.c_float)]
+
+
 class TcConvArgs(C.Structure):
     """mv2_tc_conv_args (wgmma implicit-GEMM path; see include/magvit2_b200.h)."""
     _fields_ = [
@@ -88,6 +93,8 @@ SIGNATURES = {
     "mv2_gate_residual": (_I, [_VP, _VP, _VP, _VP, _I, _I, _I, _I, _VP]),
     "mv2_rmsnorm": (_I, [_VP, _VP, _I, _VP, _I, _I, _I, _I, _I, _VP]),
     "mv2_attention": (_I, [C.POINTER(AttnArgs), _VP]),
+    "mv2_attention_dropout": (_I, [C.POINTER(AttnArgs), C.POINTER(DropoutArgs), _VP]),
+    "mv2_attention_dropout_mask": (_I, [_I, _I, _I, _I, C.POINTER(DropoutArgs), _VP, _VP]),
     "mv2_linattn_workspace_bytes": (_SZ, [_I, _I, _I]),
     "mv2_linear_attention": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _VP, _VP]),
     "mv2_geglu": (_I, [_VP, _VP, _I, _I64, _I, _VP]),

@@ -74,6 +74,34 @@ __device__ __forceinline__ float warp_max(float v) {
 
 static inline int ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 
+// ---- attention dropout: counter-based Philox4x32-10 (Salmon et al., SC'11; Random123's constants) ------------------------
+// The keep mask is a pure function of (seed, call, sequence, head, query i, key j): word j & 3 of
+// philox(counter (i, j >> 2, seq, h | call << 16), key seed) is kept iff >= thr = floor(p * 2^32).  No kernel, tiling or
+// dtype enters it, so every attention kernel, mv2_attention_dropout_mask and a numpy replica agree bit for bit.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+    const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+  }
+  return c;
+}
+
+struct AttnDrop {           // kernel-side form of mv2_dropout_args
+  uint32_t k0, k1;          // seed, low / high word
+  uint32_t call_hi;         // call << 16
+  uint32_t thr;             // keep iff word >= thr
+  float scale;              // fp32(1 / (1 - p))
+};
+
+// keep bits (bit w = word w >= thr) of the 4-key group `grp` (keys 4 grp .. 4 grp + 3) of query i
+__device__ __forceinline__ uint32_t attn_keep4(const AttnDrop& d, uint32_t i, uint32_t grp, uint32_t seq, uint32_t h) {
+  const uint4 r = philox4x32_10(make_uint4(i, grp, seq, h | d.call_hi), d.k0, d.k1);
+  return (uint32_t)(r.x >= d.thr) | (uint32_t)(r.y >= d.thr) << 1 | (uint32_t)(r.z >= d.thr) << 2 | (uint32_t)(r.w >= d.thr) << 3;
+}
+
 // ---- per-device one-time initialisation ----------------------------------------------------------------------
 // cudaFuncSetAttribute (the > 48 KB dynamic shared memory opt-in) applies to the CURRENT device only, so a process that
 // drives several GPUs must repeat it on each of them: the flag is kept per device ordinal, not per process.

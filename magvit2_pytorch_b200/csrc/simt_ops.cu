@@ -854,9 +854,12 @@ __global__ void __launch_bounds__(256) rmsnorm_bf16x8_kernel(const __nv_bfloat16
 // ------------------------------------------------------------------------------------------
 // softmax attention core
 // ------------------------------------------------------------------------------------------
+// Every softmax kernel body below takes a DROP parameter: DROP = false is the plain kernel; DROP = true drops the softmax
+// weights with the Philox mask of common.cuh (attn_keep4).  The denominator sums the undropped weights; only the P.V operand
+// is masked, and 1 / (1 - p) is folded into the final 1 / l.
 constexpr int AT_Q = 32;  // queries per block
-template <typename T, int DPL>
-__global__ void __launch_bounds__(128) attention_kernel(const mv2_attn_args a) {
+template <typename T, int DPL, bool DROP>
+__device__ __forceinline__ void attention_body(const mv2_attn_args& a, const AttnDrop& dr) {
   pdl_wait();
   pdl_launch_dependents();
   constexpr int D = DPL * 32;
@@ -932,8 +935,10 @@ __global__ void __launch_bounds__(128) attention_kernel(const mv2_attn_args a) {
       m[r] = m_new;
 #pragma unroll
       for (int dd = 0; dd < DPL; ++dd) o[r][dd] *= corr;
+      float pv = p;
+      if (DROP) pv = (attn_keep4(dr, i, jg >> 2, blockIdx.x, h) >> (jg & 3)) & 1u ? p : 0.f;
       for (int j = 0; j < 32; ++j) {
-        const float pj = __shfl_sync(0xffffffffu, p, j);
+        const float pj = __shfl_sync(0xffffffffu, pv, j);
 #pragma unroll
         for (int dd = 0; dd < DPL; ++dd) o[r][dd] = fmaf(pj, Vs[j][lane + 32 * dd], o[r][dd]);
       }
@@ -943,11 +948,17 @@ __global__ void __launch_bounds__(128) attention_kernel(const mv2_attn_args a) {
   for (int r = 0; r < 8; ++r) {
     const int i = q0 + warp * 8 + r;
     if (i >= a.L) continue;
-    const float inv = 1.f / l[r];
+    const float inv = DROP ? dr.scale / l[r] : 1.f / l[r];
     T* orow = out + (base + (int64_t)i * a.tok_stride) * HD + h * D;
 #pragma unroll
     for (int dd = 0; dd < DPL; ++dd) orow[lane + 32 * dd] = from_f32<T>(o[r][dd] * inv);
   }
+}
+template <typename T, int DPL>
+__global__ void __launch_bounds__(128) attention_kernel(const mv2_attn_args a) { attention_body<T, DPL, false>(a, AttnDrop{}); }
+template <typename T, int DPL>
+__global__ void __launch_bounds__(128) attention_dropout_kernel(const mv2_attn_args a, const AttnDrop d) {
+  attention_body<T, DPL, true>(a, d);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -957,8 +968,8 @@ __global__ void __launch_bounds__(128) attention_kernel(const mv2_attn_args a) {
 // bf16 only (the fp32 path keeps the general kernel and its summation order).
 // ------------------------------------------------------------------------------------------
 constexpr int AS_L = 8, AS_M = 8;      // max tokens / memory slots
-template <int DPL>
-__global__ void __launch_bounds__(256) attention_small_kernel(const mv2_attn_args a) {
+template <int DPL, bool DROP>
+__device__ __forceinline__ void attention_small_body(const mv2_attn_args& a, const AttnDrop& dr) {
   pdl_wait();
   pdl_launch_dependents();
   constexpr int D = DPL * 32;
@@ -997,9 +1008,18 @@ __global__ void __launch_bounds__(256) attention_small_kernel(const mv2_attn_arg
       }
       q[i][dd] = qv; k[AS_M + i][dd] = kv; v[AS_M + i][dd] = vv;
     }
+  // dropout: NM + L <= 16 keys are 4 Philox groups per query, so lane 4 i + grp draws group grp of query i once; the quad's
+  // OR leaves query i's 16 keep bits (bit = key index, memory first) in lanes 4 i .. 4 i + 3
+  uint32_t keep = 0;
+  if (DROP) {
+    keep = attn_keep4(dr, lane >> 2, lane & 3, (uint32_t)seq, h) << (4 * (lane & 3));
+    keep |= __shfl_xor_sync(0xffffffffu, keep, 1);
+    keep |= __shfl_xor_sync(0xffffffffu, keep, 2);
+  }
 #pragma unroll
   for (int i = 0; i < AS_L; ++i) {
     if (i >= L) break;
+    const uint32_t keep_i = DROP ? __shfl_sync(0xffffffffu, keep, 4 * i) : 0u;
     float sc[AS_M + AS_L], mx = -INFINITY;
 #pragma unroll
     for (int j = 0; j < AS_M + AS_L; ++j) {
@@ -1019,14 +1039,22 @@ __global__ void __launch_bounds__(256) attention_small_kernel(const mv2_attn_arg
     for (int j = 0; j < AS_M + AS_L; ++j) {
       const float e = sc[j] > -INFINITY ? __expf(sc[j] - mx) : 0.f;
       den += e;
+      float ev = e;
+      if (DROP) ev = (keep_i >> (j < AS_M ? j : NM + j - AS_M)) & 1u ? e : 0.f;
 #pragma unroll
-      for (int dd = 0; dd < DPL; ++dd) o[dd] = fmaf(e, v[j][dd], o[dd]);
+      for (int dd = 0; dd < DPL; ++dd) o[dd] = fmaf(ev, v[j][dd], o[dd]);
     }
-    const float inv = 1.f / den;
+    const float inv = DROP ? dr.scale / den : 1.f / den;
     __nv_bfloat16* orow = out + (base + (int64_t)i * a.tok_stride) * HD + h * D;
 #pragma unroll
     for (int dd = 0; dd < DPL; ++dd) orow[lane + 32 * dd] = __float2bfloat16_rn(o[dd] * inv);
   }
+}
+template <int DPL>
+__global__ void __launch_bounds__(256) attention_small_kernel(const mv2_attn_args a) { attention_small_body<DPL, false>(a, AttnDrop{}); }
+template <int DPL>
+__global__ void __launch_bounds__(256) attention_small_dropout_kernel(const mv2_attn_args a, const AttnDrop d) {
+  attention_small_body<DPL, true>(a, d);
 }
 
 
@@ -1049,8 +1077,8 @@ __device__ __forceinline__ uint32_t pack2_bf16(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-template <int D>
-__global__ void __launch_bounds__(256) attention_mma_kernel(const mv2_attn_args a) {
+template <int D, bool DROP>
+__device__ __forceinline__ void attention_mma_body(const mv2_attn_args& a, const AttnDrop& dr) {
   pdl_wait();
   pdl_launch_dependents();
   constexpr int DK = D / 16, DN = D / 8;
@@ -1176,6 +1204,19 @@ __global__ void __launch_bounds__(256) attention_mma_kernel(const mv2_attn_args 
       l0 += sfr[nt][0] + sfr[nt][1];
       l1 += sfr[nt][2] + sfr[nt][3];
     }
+    if (DROP) {
+      // keys j0 + nt*8 + 4*(t>>1) .. +3 are one Philox group, shared by threads t and t^1 for rows q0+g and q0+g+8: the even
+      // thread draws row q0+g, the odd one row q0+g+8, and each passes the partner the two keep bits it needs
+#pragma unroll
+      for (int nt = 0; nt < FA_KT / 8; ++nt) {
+        const uint32_t odd = t & 1;
+        const uint32_t kb = attn_keep4(dr, q0 + g + 8 * odd, (j0 + nt * 8) / 4 + (t >> 1), blockIdx.x, h);
+        const uint32_t other = __shfl_xor_sync(0xffffffffu, odd ? kb & 3u : kb >> 2, 1);
+        const uint32_t k0 = odd ? other : kb & 3u, k1 = odd ? kb >> 2 : other;    // row q0+g / q0+g+8: bit c = column 2t + c
+        sfr[nt][0] = k0 & 1u ? sfr[nt][0] : 0.f; sfr[nt][1] = k0 & 2u ? sfr[nt][1] : 0.f;
+        sfr[nt][2] = k1 & 1u ? sfr[nt][2] : 0.f; sfr[nt][3] = k1 & 2u ? sfr[nt][3] : 0.f;
+      }
+    }
     // ---- O += P V ----
 #pragma unroll
     for (int kk = 0; kk < FA_KT / 16; ++kk) {
@@ -1196,7 +1237,7 @@ __global__ void __launch_bounds__(256) attention_mma_kernel(const mv2_attn_args 
   l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
   l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-  const float i0 = 1.f / l0, i1 = 1.f / l1;
+  const float i0 = DROP ? dr.scale / l0 : 1.f / l0, i1 = DROP ? dr.scale / l1 : 1.f / l1;
   const int r0 = q0 + g, r1 = q0 + g + 8;
   if (r0 < a.L) {
     __nv_bfloat16* orow = out + (base + (int64_t)r0 * a.tok_stride) * HD + h * D;
@@ -1207,6 +1248,32 @@ __global__ void __launch_bounds__(256) attention_mma_kernel(const mv2_attn_args 
     __nv_bfloat16* orow = out + (base + (int64_t)r1 * a.tok_stride) * HD + h * D;
 #pragma unroll
     for (int dn = 0; dn < DN; ++dn) *reinterpret_cast<uint32_t*>(orow + dn * 8 + t * 2) = pack2_bf16(o[dn][2] * i1, o[dn][3] * i1);
+  }
+}
+template <int D>
+__global__ void __launch_bounds__(256) attention_mma_kernel(const mv2_attn_args a) { attention_mma_body<D, false>(a, AttnDrop{}); }
+template <int D>
+__global__ void __launch_bounds__(256) attention_mma_dropout_kernel(const mv2_attn_args a, const AttnDrop d) {
+  attention_mma_body<D, true>(a, d);
+}
+
+// keep mask of mv2_attention_dropout_mask: one thread per (sequence, head, query, 4-key group), keep[seq][h][i][n_mem + L]
+__global__ void __launch_bounds__(256) attention_dropout_mask_kernel(int64_t n_groups, int heads, int L, int Ltot, const AttnDrop d,
+                                                                     uint8_t* __restrict__ keep) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const int gpr = (Ltot + 3) / 4;                                  // groups per query row
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < n_groups; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int grp = (int)(idx % gpr);
+    const int64_t row = idx / gpr;                                 // (seq * heads + h) * L + i
+    const int i = (int)(row % L);
+    const int h = (int)((row / L) % heads);
+    const uint32_t seq = (uint32_t)(row / ((int64_t)L * heads));
+    const uint32_t kb = attn_keep4(d, i, grp, seq, h);
+    uint8_t* dst = keep + row * Ltot + 4 * grp;
+#pragma unroll
+    for (int w = 0; w < 4; ++w)
+      if (4 * grp + w < Ltot) dst[w] = (uint8_t)((kb >> w) & 1u);
   }
 }
 
@@ -2381,16 +2448,63 @@ __global__ void __launch_bounds__(256) maxpool2x2_backward_kernel(const T* __res
 // ==========================================================================================
 using namespace mv2;
 
+// a softmax attention kernel, or its dropout twin when d is given
+static void launch_attn_k(void (*plain)(mv2_attn_args), void (*drop)(mv2_attn_args, AttnDrop), dim3 grid, dim3 block,
+                          cudaStream_t st, const mv2_attn_args* a, const AttnDrop* d) {
+  if (d) launch_k(drop, grid, block, 0, st, *a, *d);
+  else launch_k(plain, grid, block, 0, st, *a);
+}
+
 template <typename T>
-static int launch_attention(const mv2_attn_args* a, cudaStream_t st) {
+static int launch_attention(const mv2_attn_args* a, const AttnDrop* d, cudaStream_t st) {
   dim3 grid((unsigned)((int64_t)a->n_outer * a->n_inner), a->heads, ceil_div(a->L, AT_Q));
   switch (a->dim_head / 32) {
-    case 1: launch_k(attention_kernel<T, 1>, dim3(grid), dim3(128), 0, st, *a); break;
-    case 2: launch_k(attention_kernel<T, 2>, dim3(grid), dim3(128), 0, st, *a); break;
-    case 3: launch_k(attention_kernel<T, 3>, dim3(grid), dim3(128), 0, st, *a); break;
+    case 1: launch_attn_k(attention_kernel<T, 1>, attention_dropout_kernel<T, 1>, grid, dim3(128), st, a, d); break;
+    case 2: launch_attn_k(attention_kernel<T, 2>, attention_dropout_kernel<T, 2>, grid, dim3(128), st, a, d); break;
+    case 3: launch_attn_k(attention_kernel<T, 3>, attention_dropout_kernel<T, 3>, grid, dim3(128), st, a, d); break;
     default: set_error("dim_head %d unsupported", a->dim_head); return MV2_E_UNSUPPORTED;
   }
   MV2_CHECK_LAUNCH();
+  return MV2_OK;
+}
+
+// mv2_attention's argument checks and kernel choice; d != NULL launches the dropout twins
+static int attention_dispatch(const mv2_attn_args* a, const AttnDrop* d, void* stream) {
+  MV2_CHECK_ARG(a && a->qkv && a->out && a->mem_kv);
+  MV2_CHECK_ARG(a->heads > 0 && a->dim_head > 0 && a->dim_head % 32 == 0 && a->dim_head <= 96);
+  MV2_CHECK_ARG(a->n_mem >= 0 && a->n_outer > 0 && a->n_inner > 0 && a->L > 0);
+  MV2_CHECK_ARG((int64_t)a->n_outer * a->n_inner <= 2147483647LL && ceil_div(a->L, AT_Q) <= 65535);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (a->dtype == MV2_F32) return launch_attention<float>(a, d, st);
+  if (a->dtype == MV2_BF16 && !a->causal && a->L >= 64 && (a->dim_head == 32 || a->dim_head == 64) && a->heads * a->dim_head % 8 == 0) {
+    dim3 grid((unsigned)((int64_t)a->n_outer * a->n_inner), a->heads, ceil_div(a->L, FA_Q));
+    if (a->dim_head == 32) launch_attn_k(attention_mma_kernel<32>, attention_mma_dropout_kernel<32>, grid, dim3(256), st, a, d);
+    else launch_attn_k(attention_mma_kernel<64>, attention_mma_dropout_kernel<64>, grid, dim3(256), st, a, d);
+    MV2_CHECK_LAUNCH();
+    return MV2_OK;
+  }
+  if (a->dtype == MV2_BF16 && a->L <= AS_L && a->n_mem <= AS_M && (a->dim_head == 32 || a->dim_head == 64)) {
+    const int64_t warps = (int64_t)a->n_outer * a->n_inner * a->heads;
+    const dim3 grid((unsigned)ceil_div(warps, 8));
+    if (a->dim_head == 32) launch_attn_k(attention_small_kernel<1>, attention_small_dropout_kernel<1>, grid, dim3(256), st, a, d);
+    else launch_attn_k(attention_small_kernel<2>, attention_small_dropout_kernel<2>, grid, dim3(256), st, a, d);
+    MV2_CHECK_LAUNCH();
+    return MV2_OK;
+  }
+  if (a->dtype == MV2_BF16) return launch_attention<__nv_bfloat16>(a, d, st);
+  set_error("bad dtype %d", a->dtype);
+  return MV2_E_ARG;
+}
+
+// mv2_dropout_args -> AttnDrop, after the checks both dropout entry points share
+static int attn_drop_from(const mv2_dropout_args* dp, int heads, AttnDrop* out) {
+  MV2_CHECK_ARG(dp && dp->p > 0.f && dp->p < 1.f);                 // NaN fails too
+  MV2_CHECK_ARG(heads > 0 && heads < 65536 && dp->call < 65536u);  // h | call << 16 is one 32-bit counter word
+  out->k0 = (uint32_t)dp->seed;
+  out->k1 = (uint32_t)(dp->seed >> 32);
+  out->call_hi = dp->call << 16;
+  out->thr = (uint32_t)floor((double)dp->p * 4294967296.0);        // < 2^32 for p < 1
+  out->scale = (float)(1.0 / (1.0 - (double)dp->p));
   return MV2_OK;
 }
 
@@ -2709,30 +2823,27 @@ int mv2_rmsnorm(const void* x, void* out, int dtype, const float* gamma, int B, 
   return MV2_OK;
 }
 
-int mv2_attention(const mv2_attn_args* a, void* stream) {
-  MV2_CHECK_ARG(a && a->qkv && a->out && a->mem_kv);
-  MV2_CHECK_ARG(a->heads > 0 && a->dim_head > 0 && a->dim_head % 32 == 0 && a->dim_head <= 96);
-  MV2_CHECK_ARG(a->n_mem >= 0 && a->n_outer > 0 && a->n_inner > 0 && a->L > 0);
-  MV2_CHECK_ARG((int64_t)a->n_outer * a->n_inner <= 2147483647LL && ceil_div(a->L, AT_Q) <= 65535);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (a->dtype == MV2_F32) return launch_attention<float>(a, st);
-  if (a->dtype == MV2_BF16 && !a->causal && a->L >= 64 && (a->dim_head == 32 || a->dim_head == 64) && a->heads * a->dim_head % 8 == 0) {
-    dim3 grid((unsigned)((int64_t)a->n_outer * a->n_inner), a->heads, ceil_div(a->L, FA_Q));
-    if (a->dim_head == 32) launch_k(attention_mma_kernel<32>, dim3(grid), dim3(256), 0, st, *a);
-    else launch_k(attention_mma_kernel<64>, dim3(grid), dim3(256), 0, st, *a);
-    MV2_CHECK_LAUNCH();
-    return MV2_OK;
-  }
-  if (a->dtype == MV2_BF16 && a->L <= AS_L && a->n_mem <= AS_M && (a->dim_head == 32 || a->dim_head == 64)) {
-    const int64_t warps = (int64_t)a->n_outer * a->n_inner * a->heads;
-    if (a->dim_head == 32) launch_k(attention_small_kernel<1>, dim3((unsigned)ceil_div(warps, 8)), dim3(256), 0, st, *a);
-    else launch_k(attention_small_kernel<2>, dim3((unsigned)ceil_div(warps, 8)), dim3(256), 0, st, *a);
-    MV2_CHECK_LAUNCH();
-    return MV2_OK;
-  }
-  if (a->dtype == MV2_BF16) return launch_attention<__nv_bfloat16>(a, st);
-  set_error("bad dtype %d", a->dtype);
-  return MV2_E_ARG;
+int mv2_attention(const mv2_attn_args* a, void* stream) { return attention_dispatch(a, nullptr, stream); }
+
+int mv2_attention_dropout(const mv2_attn_args* a, const mv2_dropout_args* dp, void* stream) {
+  MV2_CHECK_ARG(a);
+  AttnDrop d;
+  const int rc = attn_drop_from(dp, a->heads, &d);
+  if (rc != MV2_OK) return rc;
+  return attention_dispatch(a, &d, stream);
+}
+
+int mv2_attention_dropout_mask(int n_seq, int heads, int L, int n_mem, const mv2_dropout_args* dp, uint8_t* keep, void* stream) {
+  MV2_CHECK_ARG(keep && n_seq > 0 && L > 0 && n_mem >= 0);
+  AttnDrop d;
+  const int rc = attn_drop_from(dp, heads, &d);
+  if (rc != MV2_OK) return rc;
+  const int Ltot = n_mem + L;
+  const int64_t n_groups = (int64_t)n_seq * heads * L * ((Ltot + 3) / 4);
+  const int blocks = (int)std::min<int64_t>((n_groups + 255) / 256, 1 << 20);
+  launch_k(attention_dropout_mask_kernel, dim3(blocks), dim3(256), 0, (cudaStream_t)stream, n_groups, heads, L, Ltot, d, keep);
+  MV2_CHECK_LAUNCH();
+  return MV2_OK;
 }
 
 size_t mv2_linattn_workspace_bytes(int n_seq, int heads, int L) {

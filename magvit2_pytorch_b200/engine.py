@@ -36,6 +36,21 @@ def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else t.data_ptr()
 
 
+class AttnDropout:
+    """Attention dropout of one train-mode tokenizer forward: drop probability p, the 64-bit Philox seed of the forward and
+    the index of the next softmax attention call (its `call`, in execution order: encoder stages, then decoder stages).
+    (seed, call) selects the call's keep mask (include/magvit2_b200.h, mv2_dropout_args)."""
+
+    def __init__(self, p: float, seed: int):
+        self.p, self.seed, self.calls = float(p), int(seed), 0
+
+    def take(self) -> _lib.DropoutArgs:
+        """The dropout arguments of the next attention call."""
+        a = _lib.DropoutArgs(seed=self.seed, call=self.calls, p=self.p)
+        self.calls += 1
+        return a
+
+
 @dataclass
 class ConvPack:
     """One convolution's parameters in kernel layout."""
@@ -186,6 +201,7 @@ class Engine:
         self.taps: Optional[dict] = None  # when set, per-stage activations are recorded (tests)
         self._prof: Optional[list] = None  # when set, (event0, event1, flops) per wgmma conv launch
         self.conv_log: Optional[list] = None  # when set, one shape record per tensor-core conv launch
+        self.dropout: Optional[AttnDropout] = None  # set for the duration of a train-mode forward with attention dropout
 
     # ------------------------------------------------------------------ parameters
     def bind(self, p0: torch.Tensor, what: str):
@@ -510,8 +526,9 @@ class Engine:
         finally:
             self.use_tc = use
 
-    def attention(self, x, p, axis: str):
-        """Residual(SpaceAttention) / Residual(TokenShift(TimeAttention)) (M:444-464, M:1190, M:1235)."""
+    def attention(self, x, p, axis: str, dropout: Optional[_lib.DropoutArgs] = None):
+        """Residual(SpaceAttention) / Residual(TokenShift(TimeAttention)) (M:444-464, M:1190, M:1235).  `dropout`: drop the
+        softmax weights with that (seed, call, p) mask (Attend in training mode, A:175 / A:239)."""
         B, T, H, W, Cc = x.shape
         time_axis = axis == "time"
         xn = self.rmsnorm(x, p["gamma"], token_shift=time_axis)
@@ -527,9 +544,20 @@ class Engine:
             a = AttnArgs(qkv=_ptr(qkv), out=_ptr(o), mem_kv=_ptr(p["mem_kv"]), dtype=_dt(self.dtype), heads=heads,
                          dim_head=dh, n_mem=p["n_mem"], causal=0, n_outer=B * T, n_inner=1, L=HW,
                          outer_stride=HW, inner_stride=0, tok_stride=1)
-        check(self.lib.mv2_attention(C.byref(a), self._stream()), "mv2_attention")
+        if dropout is None:
+            check(self.lib.mv2_attention(C.byref(a), self._stream()), "mv2_attention")
+        else:
+            check(self.lib.mv2_attention_dropout(C.byref(a), C.byref(dropout), self._stream()), "mv2_attention_dropout")
         self.launches += 1
         return self.conv(o, p["out"], res=x)
+
+    def attention_dropout_mask(self, n_seq, heads, L, n_mem, dropout: _lib.DropoutArgs):
+        """The keep mask of an attention call, uint8 (n_seq, heads, L, n_mem + L) (mv2_attention_dropout_mask)."""
+        keep = torch.empty((n_seq, heads, L, n_mem + L), device=self.device, dtype=torch.uint8)
+        check(self.lib.mv2_attention_dropout_mask(n_seq, heads, L, n_mem, C.byref(dropout), _ptr(keep), self._stream()),
+              "mv2_attention_dropout_mask")
+        self.launches += 1
+        return keep
 
     def linear_attention(self, x, p):
         """Residual(LinearSpaceAttention) (M:421-442, M:1207)."""
@@ -600,12 +628,11 @@ class Engine:
                 x = self.conv(x, P[key], act=ACT_SILU, shuffle=SHUFFLE_TIME)
             else:         # TimeDownsample2x (M:796-807): pad (2, 0), Conv1d k3 s2
                 x = self.conv(x, P[key], stride=(2, 1, 1), pad=(2, 0, 0), out_spatial=((T + 2 - 3) // 2 + 1, H, W))
-        elif st.kind == "attend_space":
-            x = self.attention(x, P[key + ".attn"], "space")
-            x = self.feed_forward(x, P[key + ".ff"])
-        elif st.kind == "attend_time":
-            x = self.attention(x, P[key + ".attn"], "time")
-            x = self.feed_forward(x, P[key + ".ff"], token_shift=True)
+        elif st.kind in ("attend_space", "attend_time"):
+            time_axis = st.kind == "attend_time"
+            drop = () if self.dropout is None else (self.dropout.take(),)      # without dropout: the plain call
+            x = self.attention(x, P[key + ".attn"], "time" if time_axis else "space", *drop)
+            x = self.feed_forward(x, P[key + ".ff"], token_shift=time_axis)
         elif st.kind == "linear_attend_space":
             x = self.linear_attention(x, P[key + ".attn"])
             x = self.feed_forward(x, P[key + ".ff"])

@@ -60,18 +60,29 @@ def _squeeze_excite(y, se):
     return (yf * gate[:, None, :]).reshape(y.shape)
 
 
-def _softmax_attention(q, k, v, causal):
-    """Attend (A:218-241) with the right-aligned causal mask (A:46-47, A:123-129)."""
+def dropout_scale(p: float) -> float:
+    """fp32(1 / (1 - p)) of the fp32 value of p: the factor the attention kernels apply to the kept weights."""
+    return C.c_float(1.0 / (1.0 - C.c_float(p).value)).value
+
+
+def _softmax_attention(q, k, v, causal, dropout=None):
+    """Attend (A:218-241) with the right-aligned causal mask (A:46-47, A:123-129).  `dropout`: (keep mask (b, h, i, j) uint8, p)
+    -- the softmax weights are multiplied by keep * fp32(1 / (1 - p)) after the softmax (A:239)."""
     dots = torch.einsum("bhid,bhjd->bhij", q, k) * (q.shape[-1] ** -0.5)
     i, j = dots.shape[-2:]
     if causal and i > 1:
         mask = torch.ones((i, j), dtype=torch.bool, device=q.device).triu(j - i + 1)
         dots = dots.masked_fill(mask, -torch.finfo(dots.dtype).max)
-    return torch.einsum("bhij,bhjd->bhid", dots.softmax(dim=-1), v)
+    attn = dots.softmax(dim=-1)
+    if dropout is not None:
+        keep, p = dropout
+        attn = attn * keep.to(attn.dtype) * dropout_scale(p)
+    return torch.einsum("bhij,bhjd->bhid", attn, v)
 
 
-def _attention_block(x, at, axis):
-    """Residual(SpaceAttention) / Residual(TokenShift(TimeAttention)) (M:327-388, M:444-464, M:1190, M:1235)."""
+def _attention_block(x, at, axis, dropout=None):
+    """Residual(SpaceAttention) / Residual(TokenShift(TimeAttention)) (M:327-388, M:444-464, M:1190, M:1235).  `dropout`: as
+    _softmax_attention's, the mask laid out as mv2_attention_dropout_mask writes it."""
     B, T, H, W, Cc = x.shape
     xs = _token_shift(x) if axis == "time" else x
     xn = _rmsnorm(xs, at.norm.gamma)
@@ -82,7 +93,7 @@ def _attention_block(x, at, axis):
     mem = at.mem_kv.to(x.dtype)
     k = torch.cat((mem[0][None].expand(b, -1, -1, -1), k), dim=-2)
     v = torch.cat((mem[1][None].expand(b, -1, -1, -1), v), dim=-2)
-    o = _softmax_attention(q, k, v, causal=(axis == "time")).permute(0, 2, 1, 3).reshape(b, n, -1)
+    o = _softmax_attention(q, k, v, causal=(axis == "time"), dropout=dropout).permute(0, 2, 1, 3).reshape(b, n, -1)
     o = F.linear(o, at.to_out[1].weight)
     o = o.reshape(B, H, W, T, Cc).permute(0, 3, 1, 2, 4) if axis == "time" else o.reshape(B, T, H, W, Cc)
     return o + x
@@ -400,6 +411,16 @@ class TrainRunner(TapeRunner):
         self.tape.append(bwd)
         return out
 
+    def _attn_keep(self, x, at, axis, drop):
+        """(keep mask, p) of the attention call `drop` (its (seed, call, p)) on the block input x, regenerated by
+        mv2_attention_dropout_mask when the backward needs it; None without dropout.  The uint8 mask lives only as long as
+        the block's backward."""
+        if drop is None:
+            return None
+        B, T, H, W, _ = x.shape
+        n_seq, L = (B * H * W, T) if axis == "time" else (B * T, H * W)
+        return self.eng.attention_dropout_mask(n_seq, at.heads, L, int(at.mem_kv.shape[2]), drop), drop.p
+
     def _block(self, x, run, fn, params):
         """A light block: forward by the engine (`run`), backward by the torch restatement `fn` on the saved input."""
         out = run(x)
@@ -458,8 +479,9 @@ class TrainRunner(TapeRunner):
                                 list(at.parameters()))
             else:
                 axis = "time" if time_axis else "space"
-                x = self._block(x, lambda t: eng.attention(t, P[key + ".attn"], axis), lambda t: _attention_block(t, at, axis),
-                                list(at.parameters()))
+                drop = None if eng.dropout is None else eng.dropout.take()
+                x = self._block(x, lambda t: eng.attention(t, P[key + ".attn"], axis, *(() if drop is None else (drop,))),
+                                lambda t: _attention_block(t, at, axis, self._attn_keep(t, at, axis, drop)), list(at.parameters()))
             return self._block(x, lambda t: eng.feed_forward(t, P[key + ".ff"], token_shift=time_axis),
                                lambda t: _feed_forward_block(t, ff, time_axis), list(ff.parameters()))
         raise NotImplementedError(f"no training path for layer type {st.kind!r}")

@@ -24,6 +24,9 @@ user-supplied VGG module (``vgg=``, M:1081; nothing is downloaded): the perceptu
 (M:1788-1841) then run on the device (vgg.py).  Without one (``vgg=None``) the model builds no discriminator and
 ``return_loss`` / ``return_discr_loss`` raise.  The VGG is left out of ``state_dict``, ``copy_for_eval`` and the pickled
 config, so ``init_and_load_from`` gives a model without it.
+``attn_dropout`` (0 <= p < 1) drops the softmax attention weights of train-mode forwards (grad and no-grad) with a Philox
+mask seeded once per call from torch's default CPU generator (engine.AttnDropout, DESIGN.md 3.6); such forwards bypass the
+CUDA graphs.  Eval mode never drops.
 Out of scope (raise at construction / call; SURVEY.md 8f): multiscale discriminators and the discriminator's antialiased
 (Blur) downsampling.
 """
@@ -43,7 +46,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import modules as M
-from .engine import Engine
+from .engine import AttnDropout, Engine
 
 __version__ = "0.1.0"
 
@@ -72,6 +75,26 @@ def _on_model_device(fn):
         ctx = torch.cuda.device(dev) if dev.type == "cuda" else contextlib.nullcontext()
         with ctx:
             return fn(self, *a, **k)
+    return wrapper
+
+
+def _attn_dropout_scope(fn):
+    """Runs the method with attention dropout live when the model is in training mode and was built with attn_dropout > 0:
+    one 64-bit Philox seed per call, drawn from torch's default CPU generator (torch.manual_seed reproduces a step and nothing
+    waits on the device; nothing is drawn otherwise, so other runs' random streams are untouched)."""
+    @functools.wraps(fn)
+    def wrapper(self, *a, **k):
+        if not (self.training and self.attn_dropout > 0.):
+            return fn(self, *a, **k)
+        eng = self.engine
+        if eng.dropout is not None:           # already inside a dropout forward of this model
+            return fn(self, *a, **k)
+        hi, lo = torch.randint(0, 2 ** 32, (2,), dtype=torch.int64).tolist()
+        eng.dropout = AttnDropout(self.attn_dropout, hi << 32 | lo)
+        try:
+            return fn(self, *a, **k)
+        finally:
+            eng.dropout = None
     return wrapper
 
 
@@ -138,8 +161,11 @@ class VideoTokenizer(nn.Module):
             raise TypeError("layers must be a tuple")
         if pad_mode not in ("constant", "reflect", "replicate", "circular"):
             raise ValueError(f"unknown pad_mode {pad_mode!r}")
-        if attn_dropout != 0.:
-            raise NotImplementedError("attention dropout is a training feature")
+        if not 0. <= attn_dropout <= 1.:                                          # as nn.Dropout (A:175)
+            raise ValueError(f"dropout probability has to be between 0 and 1, but got {attn_dropout}")
+        if attn_dropout == 1.:
+            raise NotImplementedError("attn_dropout=1 would drop every attention weight; it is not supported")
+        self.attn_dropout = float(attn_dropout)
         ks = residual_conv_kernel_size
 
         self.channels = channels
@@ -408,8 +434,9 @@ class VideoTokenizer(nn.Module):
         return self._engine
 
     def _graph_call(self, name, fn, *tensors):
-        """fn(*tensors) -> tensor | tuple of tensors, replayed through a cached CUDA graph when enabled."""
-        if not self.cuda_graphs:
+        """fn(*tensors) -> tensor | tuple of tensors, replayed through a cached CUDA graph when enabled.  Forwards with live
+        attention dropout run directly: a captured graph would replay one dropout mask forever."""
+        if not self.cuda_graphs or (self._engine is not None and self._engine.dropout is not None):
             return fn(*tensors)
         eng = self.engine
         key = (name, eng._sig_id, tuple((tuple(t.shape), t.dtype) for t in tensors), self._lane)
@@ -461,6 +488,7 @@ class VideoTokenizer(nn.Module):
     # ------------------------------------------------------------------ reference API
     @torch.no_grad()
     @_on_model_device
+    @_attn_dropout_scope
     def encode(self, video, quantize=False, cond=None, video_contains_first_frame=True):
         """M:1523-1576.  Returns (B, C, T', H', W') like the reference."""
         video, ff = self._check_video(video, video_contains_first_frame)
@@ -493,6 +521,7 @@ class VideoTokenizer(nn.Module):
 
     @torch.no_grad()
     @_on_model_device
+    @_attn_dropout_scope
     def decode(self, quantized, cond=None, video_contains_first_frame=True):
         """M:1598-1649.  quantized: (B, C, T', H', W')."""
         assert quantized.ndim == 5 and quantized.shape[1] == self.quantizers.dim, \
@@ -504,6 +533,7 @@ class VideoTokenizer(nn.Module):
 
     @torch.no_grad()
     @_on_model_device
+    @_attn_dropout_scope
     def decode_from_code_indices(self, codes, cond=None, video_contains_first_frame=True):
         """M:1579-1595."""
         assert codes.dtype in (torch.long, torch.int32)                           # M:1585
@@ -528,6 +558,7 @@ class VideoTokenizer(nn.Module):
 
     @torch.no_grad()
     @_on_model_device
+    @_attn_dropout_scope
     def lfq_loss_breakdown(self, video, group=None):
         """Training-mode LFQ auxiliary terms the reference computes at M:1705 (``quantizer_loss_breakdown``):
         returns ``(codes, (per_sample_entropy, batch_entropy, commitment), aux_loss)``.  ``batch_entropy`` uses the
@@ -579,6 +610,7 @@ class VideoTokenizer(nn.Module):
         return self.forward(video, return_codes=True)
 
     @_on_model_device
+    @_attn_dropout_scope
     def forward(self, video_or_images, cond=None, return_loss=False, return_codes=False, return_recon=False,
                 return_discr_loss=False, return_recon_loss_only=False, apply_gradient_penalty=True,
                 video_contains_first_frame=True, adversarial_loss_weight=None,
