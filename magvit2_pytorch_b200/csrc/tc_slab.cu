@@ -17,13 +17,15 @@
 //     128-column divisor take 128-column tiles with a ragged last one;
 //   * the kernel is instantiated per epilogue flavour (tc_common.cuh: EPI_*) and N tile (32 / 64 / 128); the plain
 //     flavour transposes each 32 x 32 chunk through shared memory so stores / residual loads are 64-byte contiguous per row.
-// Warp roles (384 threads): w0 slab TMA producer, w2 weight TMA producer, w3 resident 1x1x1 weights (fused ResidualUnit
-// only), w4-7 / w8-11 two consumer warpgroups: each issues the wgmma of 64 of the 128 positions of every M-tile, stages
-// its accumulators in shared memory and runs the epilogue on them (one output row per thread and 32-column chunk).
+// Warp roles (384 threads): w0 slab TMA producer, w2 weight TMA producer (40 registers each, setmaxnreg), w4-7 / w8-11
+// two consumer warpgroups (232 registers): each issues the wgmma of 64 of the 128 positions of every M-tile, with one
+// commit group in flight across ring stages, stages its accumulators in shared memory and runs the epilogue on them
+// (one output row per thread and 32-column chunk).
 #include "common.cuh"
 #include "tc_common.cuh"
 #include <cuda.h>
 #include <algorithm>
+#include <type_traits>
 #include <mutex>
 #include <map>
 #include <vector>
@@ -95,28 +97,31 @@ __host__ __device__ __forceinline__ TileCoord decode_tile(const SlabParams& p, i
 
 // Shared-memory layout behind the two TMA rings (host and kernel must agree): barriers, bias, the eight 2 KB
 // epilogue transpose buffers, [fused: logit partials], the fp32 accumulator staging of both consumer warpgroups
-// (mw M-tiles x 64 rows x (bn + 4) each), [fused: the H buffer and the resident 1x1x1 weights].
-struct SlabSmem { uint32_t sbias, stage0, lpart, accstg, hbuf, w1buf, end; };
+// (mw M-tiles x 64 rows x (bn + 4) each), [fused: the H buffer].
+struct SlabSmem { uint32_t sbias, stage0, lpart, accstg, hbuf, end; };
 __host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& p, uint32_t bar0, bool fused) {
   SlabSmem m;
-  m.sbias = (bar0 + 8 * (2 * p.slab_stages + 2 * p.w_stages + 1) + 15) & ~15u;
+  m.sbias = (bar0 + 8 * (2 * p.slab_stages + 2 * p.w_stages) + 15) & ~15u;
   m.stage0 = m.sbias + (uint32_t)(p.n_tiles_n * p.bn) * 4 * (fused ? 3 : 1);   // fused: [conv3 bias][conv1 bias][SE to_k weight]
   m.lpart = m.stage0 + (fused ? 0 : 8 * 2048);   // fused: the transposes reuse the accumulator staging
   m.accstg = m.lpart + (fused ? 2048 : 0);
   m.hbuf = m.accstg + 2u * p.mw * 64 * (p.bn + 4) * 4;
   if (fused) m.hbuf = (m.hbuf + 1023u) & ~1023u;        // SWIZZLE_128B operand tiles: 1024-byte aligned
-  m.w1buf = m.hbuf + (fused ? (uint32_t)p.h_stride : 0);
-  m.end = m.w1buf + (fused ? (uint32_t)(p.kchunks * p.bn * p.row_bytes) : 0);
+  m.end = m.hbuf + (fused ? (uint32_t)p.h_stride : 0);
   return m;
 }
 
-// Every instantiation runs 384 threads: warp 0 slab TMA producer, warp 2 weight TMA producer, warp 3 (fused ResidualUnit
-// only) loads the resident 1x1x1 weights, warps 4-11 are two consumer warpgroups.  Consumer warpgroup g issues the wgmma
-// of output rows h0 + 8g .. h0 + 8g + 7 of every M-tile (64 positions) against all bn columns, keeping mw accumulators of
-// 64 x bn in registers (mw * bn <= 128: at most 64 fp32 registers per thread), then runs the epilogue on them.
+// Every instantiation runs 384 threads: warp 0 slab TMA producer, warp 2 weight TMA producer (warps 1 and 3 idle), warps
+// 4-11 are two consumer warpgroups.  Consumer warpgroup g issues the wgmma of output rows h0 + 8g .. h0 + 8g + 7 of every
+// M-tile (64 positions) against all bn columns, keeping mw accumulators of 64 x bn in registers (mw * bn <= 128: at most
+// 64 fp32 registers per thread), then runs the epilogue on them.
+// Register split: the launch gives every thread 168 registers (384 x 168 = 64,512); the producer warpgroup drops to
+// SLAB_PRODUCER_REGS and the consumers take the freed registers (128 x 40 + 256 x 232 = 64,512).
+constexpr int SLAB_PRODUCER_REGS = 40, SLAB_CONSUMER_REGS = 232;
 template <int MODE, int BN>
 __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__ SlabParams p) {
   constexpr int MWMAX = 128 / BN;
+  constexpr int KC1 = BN >= 64 ? BN / 64 : 1;   // EPI_FUSED_RU (bn = C = 64 | 128): 64-channel K-chunks of the 1x1x1 GEMM
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -130,7 +135,6 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
   // barrier table (8 bytes each)
   const uint32_t slab_full = bar0, slab_empty = slab_full + 8 * p.slab_stages;
   const uint32_t w_full = slab_empty + 8 * p.slab_stages, w_empty = w_full + 8 * p.w_stages;
-  const uint32_t w1_full = w_empty + 8 * p.w_stages;                       // EPI_FUSED_RU: 1x1x1 weights landed (once)
   const SlabSmem L = slab_smem_layout(p, bar0, MODE == EPI_FUSED_RU);
   auto gen = [&](uint32_t u) { return smem_raw + (u - smem_u32(smem_raw)); };
   float* sbias = reinterpret_cast<float*>(gen(L.sbias));   // padded Co floats, 16-byte aligned
@@ -141,12 +145,13 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
     // empty barriers: one arrival per consumer warp once its wgmma of the stage have completed
     for (int s = 0; s < p.slab_stages; ++s) { mbar_init(slab_full + 8 * s, 1); mbar_init(slab_empty + 8 * s, 8); }
     for (int s = 0; s < p.w_stages; ++s) { mbar_init(w_full + 8 * s, 1); mbar_init(w_empty + 8 * s, 8); }
-    mbar_init(w1_full, 1);
     fence_barrier_init();
   }
   if (warp == 0 && lane == 0) { tma_prefetch_desc(&p.amap); if (MODE == EPI_DOWN_SPACE) tma_prefetch_desc(&p.amap_odd); }
-  if (warp == 2 && lane == 0) { tma_prefetch_desc(&p.wmap); tma_prefetch_desc(&p.wmap2); }
-  if (MODE == EPI_FUSED_RU && warp == 3 && lane == 0) tma_prefetch_desc(&p.w1map);
+  if (warp == 2 && lane == 0) {
+    tma_prefetch_desc(&p.wmap); tma_prefetch_desc(&p.wmap2);
+    if (MODE == EPI_FUSED_RU) tma_prefetch_desc(&p.w1map);
+  }
   if (warp >= 4) {
     const int nb = p.n_tiles_n * p.bn;   // >= Co; padded columns read zeros
     for (int i = threadIdx.x - 128; i < nb; i += 256) sbias[i] = (p.epi.bias && i < p.Co) ? p.epi.bias[i] : 0.f;
@@ -163,81 +168,90 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
 
   const int taps2d = p.kh * p.kw;
 
-  if (warp == 0) {
-    // ------------------------------ slab producer ------------------------------
-    if (MODE == EPI_DOWN_SPACE) {
-      // one stage = the odd-row sub-slab (input rows 2*ho - 1: 17 rows for 16 output rows) + the even-row sub-slab (rows 2*ho)
-      // of one 64-channel chunk of the (W/2) x (2C) view; w2 starts one position to the left (the dw = 0 tap), OOB = zero pad
-      if (lane == 0) {
-        uint32_t s = 0, ph = 0;
-        for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
-          const TileCoord c = decode_tile(p, tile);
-          for (int kc = 0; kc < p.kchunks; ++kc) {
-            mbar_wait(slab_empty + 8 * s, ph ^ 1);
-            mbar_expect_tx(slab_full + 8 * s, p.slab_bytes);
-            tma_load_5d(slab0 + s * p.slab_stride, &p.amap_odd, slab_full + 8 * s, kc * bk, c.w0 - 1, c.h0 - 1, c.t, c.b);
-            tma_load_5d(slab0 + s * p.slab_stride + p.dn_e_off, &p.amap, slab_full + 8 * s, kc * bk, c.w0 - 1, c.h0, c.t, c.b);
-            if (++s == (uint32_t)p.slab_stages) { s = 0; ph ^= 1; }
+  if (warp < 4) {
+    // every warp of the producer warpgroup, the idle ones included, gives up its registers (one setmaxnreg for the
+    // warpgroup) before any of them returns: the consumers' setmaxnreg.inc waits until the SM's register file has them
+    setmaxnreg_dec<SLAB_PRODUCER_REGS>();
+    if (warp == 0) {
+      // ------------------------------ slab producer ------------------------------
+      if (MODE == EPI_DOWN_SPACE) {
+        // one stage = the odd-row sub-slab (input rows 2*ho - 1: 17 rows for 16 output rows) + the even-row sub-slab (rows 2*ho)
+        // of one 64-channel chunk of the (W/2) x (2C) view; w2 starts one position to the left (the dw = 0 tap), OOB = zero pad
+        if (lane == 0) {
+          uint32_t s = 0, ph = 0;
+          for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
+            const TileCoord c = decode_tile(p, tile);
+            for (int kc = 0; kc < p.kchunks; ++kc) {
+              mbar_wait(slab_empty + 8 * s, ph ^ 1);
+              mbar_expect_tx(slab_full + 8 * s, p.slab_bytes);
+              tma_load_5d(slab0 + s * p.slab_stride, &p.amap_odd, slab_full + 8 * s, kc * bk, c.w0 - 1, c.h0 - 1, c.t, c.b);
+              tma_load_5d(slab0 + s * p.slab_stride + p.dn_e_off, &p.amap, slab_full + 8 * s, kc * bk, c.w0 - 1, c.h0, c.t, c.b);
+              if (++s == (uint32_t)p.slab_stages) { s = 0; ph ^= 1; }
+            }
           }
         }
-      }
-    } else
-    if (lane == 0) {
-      uint32_t s = 0, ph = 0;
-      for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
-        const TileCoord c = decode_tile(p, tile);
-        const int dt0 = max(0, p.pt - c.t * p.st);
-        for (int dt = dt0; dt < p.kt; ++dt)
-          for (int kc = 0; kc < p.kchunks; ++kc) {
-            mbar_wait(slab_empty + 8 * s, ph ^ 1);
-            mbar_expect_tx(slab_full + 8 * s, p.slab_bytes);
-            tma_load_5d(slab0 + s * p.slab_stride, &p.amap, slab_full + 8 * s, kc * bk, c.w0 - p.pw, c.h0 - p.ph,
-                        c.t * p.st + dt - p.pt, c.b);
-            if (++s == (uint32_t)p.slab_stages) { s = 0; ph ^= 1; }
-          }
-      }
-    }
-  } else if (warp == 2) {
-    // ------------------------------ weight producer ------------------------------
-    if (MODE == EPI_DOWN_SPACE) {
+      } else
       if (lane == 0) {
         uint32_t s = 0, ph = 0;
-        const int C2 = p.Ci;                 // channels of the paired view (2C)
         for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
           const TileCoord c = decode_tile(p, tile);
-          for (int kc = 0; kc < p.kchunks; ++kc)
-            for (int tap = kc < p.dn_lower ? 1 : 0; tap < 6; tap += kc < p.dn_lower ? 2 : 1) {
+          const int dt0 = max(0, p.pt - c.t * p.st);
+          for (int dt = dt0; dt < p.kt; ++dt)
+            for (int kc = 0; kc < p.kchunks; ++kc) {
+              mbar_wait(slab_empty + 8 * s, ph ^ 1);
+              mbar_expect_tx(slab_full + 8 * s, p.slab_bytes);
+              tma_load_5d(slab0 + s * p.slab_stride, &p.amap, slab_full + 8 * s, kc * bk, c.w0 - p.pw, c.h0 - p.ph,
+                          c.t * p.st + dt - p.pt, c.b);
+              if (++s == (uint32_t)p.slab_stages) { s = 0; ph ^= 1; }
+            }
+        }
+      }
+    } else if (warp == 2) {
+      // ------------------------------ weight producer ------------------------------
+      if (MODE == EPI_DOWN_SPACE) {
+        if (lane == 0) {
+          uint32_t s = 0, ph = 0;
+          const int C2 = p.Ci;                 // channels of the paired view (2C)
+          for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
+            const TileCoord c = decode_tile(p, tile);
+            for (int kc = 0; kc < p.kchunks; ++kc)
+              for (int tap = kc < p.dn_lower ? 1 : 0; tap < 6; tap += kc < p.dn_lower ? 2 : 1) {
+                mbar_wait(w_empty + 8 * s, ph ^ 1);
+                mbar_expect_tx(w_full + 8 * s, w_tile);
+                tma_load_2d(wst0 + s * w_bytes, &p.wmap2, w_full + 8 * s, tap * C2 + kc * (int)bk, c.n0);
+                if (++s == (uint32_t)p.w_stages) { s = 0; ph ^= 1; }
+              }
+          }
+        }
+      } else
+      if (lane == 0) {
+        uint32_t s = 0, ph = 0;
+        for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
+          const TileCoord c = decode_tile(p, tile);
+          const int dt0 = max(0, p.pt - c.t * p.st);
+          for (int dt = dt0; dt < p.kt; ++dt)
+            for (int kc = 0; kc < p.kchunks; ++kc)
+              for (int tp = 0; tp < taps2d; tp += p.tpw) {
+                mbar_wait(w_empty + 8 * s, ph ^ 1);
+                mbar_expect_tx(w_full + 8 * s, w_bytes);
+                if (p.tpw == 1) tma_load_2d(wst0 + s * w_bytes, &p.wmap2, w_full + 8 * s, (dt * taps2d + tp) * p.Ci + kc * bk, c.n0);
+                else tma_load_3d(wst0 + s * w_bytes, &p.wmap, w_full + 8 * s, kc * bk, c.n0, dt * taps2d + tp);
+                if (++s == (uint32_t)p.w_stages) { s = 0; ph ^= 1; }
+              }
+          // EPI_FUSED_RU: the tile's last KC1 stages are the 1x1x1 weights (tpw = 1, one 64-channel K-chunk each), which
+          // the second GEMM of every M-tile of the tile reads
+          if (MODE == EPI_FUSED_RU)
+            for (int kc2 = 0; kc2 < KC1; ++kc2) {
               mbar_wait(w_empty + 8 * s, ph ^ 1);
               mbar_expect_tx(w_full + 8 * s, w_tile);
-              tma_load_2d(wst0 + s * w_bytes, &p.wmap2, w_full + 8 * s, tap * C2 + kc * (int)bk, c.n0);
+              tma_load_2d(wst0 + s * w_bytes, &p.w1map, w_full + 8 * s, kc2 * (int)bk, 0);
               if (++s == (uint32_t)p.w_stages) { s = 0; ph ^= 1; }
             }
         }
       }
-    } else
-    if (lane == 0) {
-      uint32_t s = 0, ph = 0;
-      for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
-        const TileCoord c = decode_tile(p, tile);
-        const int dt0 = max(0, p.pt - c.t * p.st);
-        for (int dt = dt0; dt < p.kt; ++dt)
-          for (int kc = 0; kc < p.kchunks; ++kc)
-            for (int tp = 0; tp < taps2d; tp += p.tpw) {
-              mbar_wait(w_empty + 8 * s, ph ^ 1);
-              mbar_expect_tx(w_full + 8 * s, w_bytes);
-              if (p.tpw == 1) tma_load_2d(wst0 + s * w_bytes, &p.wmap2, w_full + 8 * s, (dt * taps2d + tp) * p.Ci + kc * bk, c.n0);
-              else tma_load_3d(wst0 + s * w_bytes, &p.wmap, w_full + 8 * s, kc * bk, c.n0, dt * taps2d + tp);
-              if (++s == (uint32_t)p.w_stages) { s = 0; ph ^= 1; }
-            }
-      }
     }
-  } else if (warp == 3) {
-    // ------------------------------ EPI_FUSED_RU: the 1x1x1 weights, resident for the whole kernel ------------------------------
-    if (MODE == EPI_FUSED_RU && lane == 0) {
-      mbar_expect_tx(w1_full, (uint32_t)p.kchunks * w_tile);
-      for (int kc2 = 0; kc2 < p.kchunks; ++kc2) tma_load_2d(L.w1buf + kc2 * w_tile, &p.w1map, w1_full, kc2 * (int)bk, 0);
-    }
-  } else if (warp >= 4) {
+  } else {
+    setmaxnreg_inc<SLAB_CONSUMER_REGS>();
     // ------------------------------ consumer warpgroups: wgmma main loop + epilogue ------------------------------
     const int wg = (warp - 4) >> 2, wq = warp & 3, tid = threadIdx.x & 127;
     // epilogue roles: 32-row quarter `sub` of the M-tile (rows sub*32 .. +31 = output rows h0 + 4 sub .. +3, all 8 w) and
@@ -261,11 +275,35 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
     uint32_t s_idx = 0, s_par = 0;                               // slab ring
     uint32_t w_idx = 0, w_par = 0, b_lo = b_lo0;                 // weight ring
     uint32_t ecount = 0;       // EPI_FUSED_RU: M-tiles processed (selects the logit exchange buffer)
-    if (MODE == EPI_FUSED_RU) mbar_wait(w1_full, 0);
     float acc[MWMAX][BN / 2];
-    for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
-      const TileCoord c = decode_tile(p, tile);
-      uint32_t accum = 0;
+    // Main loop of one tile, compiled per M-tile count MW (= p.mw) and K steps per 64-byte half row (K4: 128-byte rows),
+    // so that every commit group is straight-line code with constant accumulator indices: ptxas closes a group early at
+    // any branch inside it, which would leave nothing but an empty MMA in flight.
+    // One commit group (the MMAs of one tap) stays in flight: after committing group g the warpgroup waits until g - 1
+    // has completed (wait_group 1).  When g - 1 was the last tap of its weight stage, that weight slot is released, and
+    // when it was also the last reading its slab stage, that slab slot too (one arrival per consumer warp and slot).
+    // The tile's last group is retired with wait_group 0.
+    auto mainloop = [&](const TileCoord& c, auto mw_c, auto k4_c) {
+      constexpr int MW = decltype(mw_c)::value;
+      constexpr bool K4 = decltype(k4_c)::value;
+      constexpr uint32_t NONE = ~0u;
+      uint32_t accum = 0, pend_w = NONE, pend_s = NONE;
+      auto release_pending = [&]() {
+        __syncwarp();
+        if (lane == 0) {
+          if (pend_w != NONE) mbar_arrive(w_empty + 8 * pend_w);
+          if (pend_s != NONE) mbar_arrive(slab_empty + 8 * pend_s);
+        }
+      };
+      // after a commit: retire the previous group, then hold the slots (or NONE) the group just committed frees once done
+      auto retire_previous = [&](uint32_t w_last, uint32_t s_last) {
+        wgmma_wait<1>();
+        release_pending();
+        pend_w = w_last; pend_s = s_last;
+      };
+      auto next_w_stage = [&]() {
+        if (++w_idx == (uint32_t)p.w_stages) { w_idx = 0; w_par ^= 1; b_lo = b_lo0; } else { b_lo += w_stage16; }
+      };
       if (MODE == EPI_DOWN_SPACE) {
         for (int kc = 0; kc < p.kchunks; ++kc) {
           mbar_wait(slab_full + 8 * s_idx, s_par);
@@ -276,8 +314,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
             wgmma_fence();
             const uint64_t bd = b_hi | (uint64_t)b_lo;
 #pragma unroll
-            for (int j = 0; j < MWMAX; ++j) {
-              if (j >= p.mw) break;
+            for (int j = 0; j < MW; ++j) {
               const uint64_t ad = a_hi | (uint64_t)(a_base + (uint32_t)p.dn_aoff[tap] + j * a_mtile);
               wgmma_bf16<BN>(acc[j], ad, bd, accum);
               wgmma_bf16<BN>(acc[j], ad + 2, bd + 2, 1u);
@@ -285,13 +322,10 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
               wgmma_bf16<BN>(acc[j], ad + 6, bd + 6, 1u);
             }
             wgmma_commit();
-            wgmma_wait_all();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(w_empty + 8 * w_idx);
+            retire_previous(w_idx, tap + tstep >= 6 ? s_idx : NONE);
             accum = 1;
-            if (++w_idx == (uint32_t)p.w_stages) { w_idx = 0; w_par ^= 1; b_lo = b_lo0; } else { b_lo += w_stage16; }
+            next_w_stage();
           }
-          if (lane == 0) mbar_arrive(slab_empty + 8 * s_idx);
           if (++s_idx == (uint32_t)p.slab_stages) { s_idx = 0; s_par ^= 1; }
         }
       } else {
@@ -303,35 +337,47 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
             int dw = 0;
             for (int tp0 = 0; tp0 < taps2d; tp0 += p.tpw) {
               mbar_wait(w_full + 8 * w_idx, w_par);
-              wgmma_fence();
+              const bool slab_last = tp0 + p.tpw >= taps2d;
               uint32_t b_cur = b_lo;
               for (int u = 0; u < p.tpw; ++u) {
+                wgmma_fence();
                 const uint64_t bd = b_hi | (uint64_t)b_cur;
 #pragma unroll
-                for (int j = 0; j < MWMAX; ++j) {
-                  if (j >= p.mw) break;
+                for (int j = 0; j < MW; ++j) {
                   const uint64_t ad = a_hi | (uint64_t)(a_lo + j * a_mtile);
                   wgmma_bf16<BN>(acc[j], ad, bd, accum);
                   wgmma_bf16<BN>(acc[j], ad + 2, bd + 2, 1u);
-                  if (k4) {
+                  if (K4) {
                     wgmma_bf16<BN>(acc[j], ad + 4, bd + 4, 1u);
                     wgmma_bf16<BN>(acc[j], ad + 6, bd + 6, 1u);
                   }
                 }
+                wgmma_commit();
+                const bool w_last = u == p.tpw - 1;
+                retire_previous(w_last ? w_idx : NONE, w_last && slab_last ? s_idx : NONE);
                 accum = 1;
                 b_cur += w_tile16;
                 if (++dw == p.kw) { dw = 0; a_lo += a_next_dh; } else { a_lo += a_row; }
               }
-              wgmma_commit();
-              wgmma_wait_all();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(w_empty + 8 * w_idx);   // the weight slot is free once these MMAs have read it
-              if (++w_idx == (uint32_t)p.w_stages) { w_idx = 0; w_par ^= 1; b_lo = b_lo0; } else { b_lo += w_stage16; }
+              next_w_stage();
             }
-            if (lane == 0) mbar_arrive(slab_empty + 8 * s_idx);
             if (++s_idx == (uint32_t)p.slab_stages) { s_idx = 0; s_par ^= 1; }
           }
       }
+      wgmma_wait<0>();
+      release_pending();
+    };
+    // 64-byte rows (k4 false) occur only in the plain slab flavours; the fused ResidualUnit and SpatialDownsample2x
+    // always read 128-byte rows
+    auto mainloop_k = [&](const TileCoord& c, auto mw_c) {
+      if (MODE != EPI_FUSED_RU && MODE != EPI_DOWN_SPACE && !k4) mainloop(c, mw_c, std::false_type());
+      else mainloop(c, mw_c, std::true_type());
+    };
+    for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
+      const TileCoord c = decode_tile(p, tile);
+      if (MWMAX >= 4 && p.mw == 4) mainloop_k(c, std::integral_constant<int, (MWMAX >= 4 ? 4 : 1)>());
+      else if (MWMAX >= 2 && p.mw == 2) mainloop_k(c, std::integral_constant<int, (MWMAX >= 2 ? 2 : 1)>());
+      else mainloop_k(c, std::integral_constant<int, 1>());
       // ---- accumulators -> shared-memory staging (one [64][BN + 4] block per M-tile), once the previous tile's epilogue
       //      of this warpgroup has read its staging ----
       named_bar_sync(wg_bar, 128);
@@ -360,7 +406,15 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
 #pragma unroll
           for (int i = 0; i < 8; ++i) run_acc[q][i] = 0.f;
         const uint64_t h_hi = gmma_desc_hi(1024, 128);
-        const uint32_t h_lo = desc_lo(L.hbuf) + (uint32_t)wg * ((64 * 128) >> 4), w1_lo = desc_lo(L.w1buf);
+        const uint32_t h_lo = desc_lo(L.hbuf) + (uint32_t)wg * ((64 * 128) >> 4);
+        // the 1x1x1 weights: the tile's last KC1 weight-ring stages (the producer appends them after the conv's stages);
+        // they stay held until the last M-tile's second GEMM has read them
+        uint32_t w1_slot[KC1], w1_par[KC1], w1_lo[KC1];
+#pragma unroll
+        for (int kc2 = 0; kc2 < KC1; ++kc2) {
+          w1_slot[kc2] = w_idx; w1_par[kc2] = w_par; w1_lo[kc2] = b_lo;
+          if (++w_idx == (uint32_t)p.w_stages) { w_idx = 0; w_par ^= 1; b_lo = b_lo0; } else { b_lo += w_stage16; }
+        }
         for (int j = 0; j < p.mw; ++j) {
           const float* srow = stg + (j * 64 + row - 64 * wg) * (BN + 4);
           // E2's transpose buffers: 2 KB per warp inside the staging rows of this warp pair, which both warps have read
@@ -384,16 +438,25 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
           fence_proxy_async();      // generic-proxy writes -> visible to the tensor core's async-proxy reads
           named_bar_sync(wg_bar, 128);
           // second GEMM: acc[0] = H (this warpgroup's 64 rows) x W1^T; the staging of M-tile j is free again afterwards
+#pragma unroll
+          for (int kc2 = 0; kc2 < KC1; ++kc2) mbar_wait(w_full + 8 * w1_slot[kc2], w1_par[kc2]);
           wgmma_fence();
-          for (int kc2 = 0; kc2 < p.kchunks; ++kc2) {
-            const uint64_t ad = h_hi | (uint64_t)(h_lo + kc2 * (16384 >> 4)), bd = h_hi | (uint64_t)(w1_lo + kc2 * (w_tile >> 4));
+#pragma unroll
+          for (int kc2 = 0; kc2 < KC1; ++kc2) {
+            const uint64_t ad = h_hi | (uint64_t)(h_lo + kc2 * (16384 >> 4)), bd = h_hi | (uint64_t)w1_lo[kc2];
             wgmma_bf16<BN>(acc[0], ad, bd, kc2 > 0 ? 1u : 0u);
             wgmma_bf16<BN>(acc[0], ad + 2, bd + 2, 1u);
             wgmma_bf16<BN>(acc[0], ad + 4, bd + 4, 1u);
             wgmma_bf16<BN>(acc[0], ad + 6, bd + 6, 1u);
           }
           wgmma_commit();
-          wgmma_wait_all();
+          wgmma_wait<0>();
+          if (j == p.mw - 1) {
+            __syncwarp();
+            if (lane == 0)
+#pragma unroll
+              for (int kc2 = 0; kc2 < KC1; ++kc2) mbar_arrive(w_empty + 8 * w1_slot[kc2]);
+          }
           stage_acc<BN>(acc[0], stg + j * 64 * (BN + 4), tid);
           named_bar_sync(wg_bar, 128);
           // E2: y = ELU(conv1 + b1) -> bf16 -> global (64-byte row pieces through the transpose buffer), and per 32-position
@@ -619,7 +682,7 @@ extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
 }
 
 // Shared memory left for the two TMA rings of a launch: 227 KB minus what follows them (barrier table sized for the deepest
-// rings, bias, transpose buffers, accumulator staging, [fused: H buffer, resident 1x1x1 weights]) and the alignment slack.
+// rings, bias, transpose buffers, accumulator staging, [fused: H buffer]) and the alignment slack.
 static int slab_ring_budget(const SlabParams& p, bool fused) {
   SlabParams q = p;
   q.slab_stages = 3; q.w_stages = 12;      // upper bounds for the barrier table
@@ -808,7 +871,7 @@ extern "C" int mv2_tc_ru_supported(const mv2_tc_ru_args* a) {
 
 // tiling + shared-memory plan of the fused kernel (host arithmetic only): the slab plan of the 3x3x3 conv (one N tile of
 // bn = C; its M-tile rule gives mw = 2 at C = 64 and 1 at C = 128), one tap per weight stage, two slab stages and as many
-// weight stages as the H buffer and the resident 1x1x1 weights leave room for
+// weight stages as the H buffer leaves room for (the 1x1x1 weights stream through the same ring, C / 64 stages per tile)
 static int ru_fill_plan(const mv2_tc_ru_args* a, SlabParams& p) {
   mv2_tc_conv_args c;
   ru_as_conv_args(a, &c);
