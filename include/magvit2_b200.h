@@ -363,6 +363,47 @@ int mv2_se_gate_records(const void* workspace, int nrec, int F, int C, int Hd,
                         const float* w1, const float* b1, const float* w2, const float* b2,
                         float* gates, void* stream);
 
+/* ---- streaming: causal state carried from one chunk of a clip to the next (magvit2_pytorch_b200/stream.py) ------------
+ * A chunked call must give exactly what the whole-clip call gives, so the kernels read the state in place instead of
+ * re-running earlier frames.
+ *
+ * mv2_conv_hist: the frames in front of a causal conv's input x.  Input frame t < 0 of clip b is history frame T_h + t,
+ *   read from h + b * clip_stride (elements) as a (T_h, Hi, Wi, Ci) block; frames older than the history (t < -T_h) are the
+ *   causal zero padding, exactly as frame t < 0 is for the entry points without history.  The history may be the tail of
+ *   the previous chunk's input itself (clip_stride = that tensor's frames per clip * Hi * Wi * Ci): nothing is copied.
+ *   T_h = 0 means no history (the plain entry point's result).
+ * mv2_conv_forward_hist / mv2_tc_conv_forward_hist / mv2_tc_slab_forward_hist / mv2_tc_ru_forward_hist: the entry point
+ *   of the same name without _hist, with that history.  Each output element accumulates the same products in the same
+ *   order as the whole-clip call; the slab kernels skip the taps older than the history as they skip the padding.
+ *   mv2_tc_conv_forward_hist takes the shapes mv2_tc_conv_hist_supported accepts (pure host arithmetic): stride 1 and an
+ *   output tile of one frame or of >= 8 positions per frame.  For the others a caller runs mv2_tc_conv_forward on a copy of
+ *   [history | x] with pt reduced by T_h, which gives the same values.                                                      */
+typedef struct mv2_conv_hist {
+  const void* h;
+  int32_t T_h;
+  int64_t clip_stride;
+} mv2_conv_hist;
+int mv2_conv_forward_hist(const mv2_conv_args* a, const mv2_conv_hist* hist, void* stream);
+int mv2_tc_conv_hist_supported(const mv2_tc_conv_args* a);
+int mv2_tc_conv_forward_hist(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream);
+int mv2_tc_slab_forward_hist(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream);
+int mv2_tc_ru_forward_hist(const mv2_tc_ru_args* a, const mv2_conv_hist* hist, void* stream);
+/* mv2_rmsnorm_prev: mv2_rmsnorm whose token shift reads frame -1 of clip b from prev + b * prev_clip_stride (elements,
+ *   a (P, C) frame) instead of zeros: the TokenShift (M:250-254) of a chunk that continues a clip.                        */
+int mv2_rmsnorm_prev(const void* x, const void* prev, int64_t prev_clip_stride, void* out, int dtype, const float* gamma,
+                     int B, int T, int P, int C, void* stream);
+/* mv2_attention_tail: rows [q_begin, a->L) of a causal mv2_attention call over L tokens (the same kernel choice for that L,
+ *   so the same values).  a->qkv is a K/V cache holding the keys and values of all L tokens, rows of 2 * heads * dim_head
+ *   laid out '(kv h d)', addressed with a's strides; the queries are rows 0 .. L - q_begin - 1 of q (the chunk's qkv rows,
+ *   '(qkv h d)', sequences q_outer_stride tokens apart, same inner / token strides) and the output rows are written alike to
+ *   out (out_outer_stride).  The cost grows with the key count only.                                                      */
+int mv2_attention_tail(const mv2_attn_args* a, const void* q, int64_t q_outer_stride, int q_begin, void* out,
+                       int64_t out_outer_stride, void* stream);
+/* mv2_gateloop_scan_state: mv2_gateloop_scan starting from s_{-1} = state (fp32 [B][P][C]) instead of 0; the state after
+ *   the last frame is written back to it.                                                                                  */
+int mv2_gateloop_scan_state(const void* qkva, const void* res, void* out, int dtype, int B, int T, int P, int C, float* state,
+                            void* stream);
+
 #ifdef __cplusplus
 }
 #endif

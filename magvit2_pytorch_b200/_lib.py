@@ -74,6 +74,11 @@ class TcRuArgs(C.Structure):
     ]
 
 
+class ConvHist(C.Structure):
+    """mv2_conv_hist (frames in front of a streamed chunk; see include/magvit2_b200.h)."""
+    _fields_ = [("h", C.c_void_p), ("T_h", C.c_int32), ("clip_stride", C.c_int64)]
+
+
 # name -> (restype, argtypes); must list every symbol include/magvit2_b200.h declares
 _VP, _I, _I64, _F, _SZ = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_size_t
 SIGNATURES = {
@@ -128,6 +133,14 @@ SIGNATURES = {
     "mv2_tc_ru_workspace_bytes": (_SZ, [C.POINTER(TcRuArgs)]),
     "mv2_tc_ru_forward": (_I, [C.POINTER(TcRuArgs), _VP]),
     "mv2_se_gate_records": (_I, [_VP, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
+    "mv2_conv_forward_hist": (_I, [C.POINTER(ConvArgs), C.POINTER(ConvHist), _VP]),
+    "mv2_tc_conv_forward_hist": (_I, [C.POINTER(TcConvArgs), C.POINTER(ConvHist), _VP]),
+    "mv2_tc_slab_forward_hist": (_I, [C.POINTER(TcConvArgs), C.POINTER(ConvHist), _VP]),
+    "mv2_tc_ru_forward_hist": (_I, [C.POINTER(TcRuArgs), C.POINTER(ConvHist), _VP]),
+    "mv2_rmsnorm_prev": (_I, [_VP, _VP, _I64, _VP, _I, _VP, _I, _I, _I, _I, _VP]),
+    "mv2_attention_tail": (_I, [C.POINTER(AttnArgs), _VP, _I64, _I, _VP, _I64, _VP]),
+    "mv2_tc_conv_hist_supported": (_I, [C.POINTER(TcConvArgs)]),
+    "mv2_gateloop_scan_state": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _VP, _VP]),
 }
 
 _lib = None

@@ -171,7 +171,7 @@ __global__ void __launch_bounds__(256) ingest_kwpack_kernel(const TS* __restrict
 constexpr int CBM = 64, CBN = 64, CBK = 16;
 
 template <typename T>
-__global__ void __launch_bounds__(256) conv_simt_kernel(const mv2_conv_args a) {
+__global__ void __launch_bounds__(256) conv_simt_kernel(const mv2_conv_args a, const mv2_conv_hist hh) {
   pdl_wait();
   pdl_launch_dependents();
   __shared__ float As[CBK][CBM + 4];
@@ -224,6 +224,8 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const mv2_conv_args a) {
           if (a.x_token_shift && c >= half_c) tt -= 1;
           if (tt >= 0 && tt < a.Ti)
             v = to_f32<T>(x[((((int64_t)lb * a.Ti + tt) * a.Hi + hi) * a.Wi + wi) * a.Ci + c]);
+          else if (tt < 0 && tt >= -hh.T_h)       // frames in front of the chunk: the carried history (T_h = 0: none)
+            v = to_f32<T>(((const T*)hh.h)[(int64_t)lb * hh.clip_stride + (((int64_t)(hh.T_h + tt) * a.Hi + hi) * a.Wi + wi) * a.Ci + c]);
         }
         As[lk + j][lp] = v;
       }
@@ -742,7 +744,8 @@ __global__ void pad_cl_kernel(const T* __restrict__ src, T* __restrict__ dst, in
 template <typename T>
 __global__ void __launch_bounds__(256) rmsnorm_kernel(const T* __restrict__ x, T* __restrict__ out,
                                                       const float* __restrict__ gamma, int64_t n_tok, int T_,
-                                                      int P, int C, int token_shift) {
+                                                      int P, int C, int token_shift, const T* __restrict__ prev,
+                                                      int64_t prev_stride) {
   pdl_wait();
   pdl_launch_dependents();
   const int lane = threadIdx.x & 31;
@@ -751,8 +754,9 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const T* __restrict__ x, T
   const int t = (int)((tok / P) % T_);
   const int half = (C + 1) >> 1;           // torch.chunk(2): the first (unshifted) half takes ceil(C / 2) channels (M:250)
   const T* row = x + tok * C;
-  const T* prow = row - (int64_t)P * C;
-  const bool has_prev = t > 0;
+  // frame -1 of a chunk that continues a clip: the previous chunk's last frame (prev), else the zero shift
+  const T* prow = t > 0 || !prev ? row - (int64_t)P * C : prev + (tok / ((int64_t)T_ * P)) * prev_stride + (tok % P) * C;
+  const bool has_prev = t > 0 || prev;
   float ss = 0.f;
   for (int c = lane; c < C; c += 32) {
     float v;
@@ -780,7 +784,8 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const T* __restrict__ x, T
 template <int NU, int RN_TPW>   // 256-channel slabs per token: C <= 256 * NU
 __global__ void __launch_bounds__(256) rmsnorm_bf16x8_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ out,
                                                              const float* __restrict__ gamma, int64_t n_tok, int T_,
-                                                             int P, int C, int token_shift) {
+                                                             int P, int C, int token_shift,
+                                                             const __nv_bfloat16* __restrict__ prev, int64_t prev_stride) {
   pdl_wait();
   pdl_launch_dependents();
   const int lane = threadIdx.x & 31;
@@ -794,8 +799,9 @@ __global__ void __launch_bounds__(256) rmsnorm_bf16x8_kernel(const __nv_bfloat16
     const bool valid = tok < n_tok;
     const int t = valid ? (int)((tok / P) % T_) : 0;
     const __nv_bfloat16* row = x + (valid ? tok : tok0) * C;
-    const __nv_bfloat16* prow = row - (int64_t)P * C;
-    const bool has_prev = t > 0;
+    const __nv_bfloat16* prow = t > 0 || !prev ? row - (int64_t)P * C
+                                               : prev + ((valid ? tok : tok0) / ((int64_t)T_ * P)) * prev_stride + ((valid ? tok : tok0) % P) * C;
+    const bool has_prev = t > 0 || prev;
 #pragma unroll
     for (int u = 0; u < NU; ++u) {
       const int c = (u * 32 + lane) * 8;
@@ -858,8 +864,12 @@ __global__ void __launch_bounds__(256) rmsnorm_bf16x8_kernel(const __nv_bfloat16
 // weights with the Philox mask of common.cuh (attn_keep4).  The denominator sums the undropped weights; only the P.V operand
 // is masked, and 1 / (1 - p) is folded into the final 1 / l.
 constexpr int AT_Q = 32;  // queries per block
+// Rows [q_begin, L) of a call (mv2_attention_tail): a.qkv is then a K/V cache ('(kv h d)' rows of 2 * heads * dim_head), the
+// queries are rows 0.. of the chunk's qkv rows q (sequences q_outer tokens apart), and the output rows are stored alike
+// (out_outer).  A whole call is {0, -1, nullptr, 0}: queries, keys and values from a.qkv.
+struct AttnTail { int q_begin; int64_t out_outer; const void* q; int64_t q_outer; };
 template <typename T, int DPL, bool DROP>
-__device__ __forceinline__ void attention_body(const mv2_attn_args& a, const AttnDrop& dr) {
+__device__ __forceinline__ void attention_body(const mv2_attn_args& a, const AttnDrop& dr, const AttnTail tl = AttnTail{0, -1, nullptr, 0}) {
   pdl_wait();
   pdl_launch_dependents();
   constexpr int D = DPL * 32;
@@ -873,9 +883,10 @@ __device__ __forceinline__ void attention_body(const mv2_attn_args& a, const Att
   const int64_t seq = blockIdx.x;
   const int64_t so = seq / a.n_inner, sn = seq % a.n_inner;
   const int64_t base = so * a.outer_stride + sn * a.inner_stride;
-  const int q0 = blockIdx.z * AT_Q;
+  const int q0 = tl.q_begin + blockIdx.z * AT_Q;
   const int HD = a.heads * D;
   const int64_t row_stride = 3 * (int64_t)HD;
+  const int64_t kv_stride = tl.q ? 2 * (int64_t)HD : row_stride, k_off = tl.q ? 0 : HD;   // K/V cache rows: '(kv h d)'
   const float scale = rsqrtf((float)D);
   const bool causal = a.causal && a.L > 1;
   const int Ltot = a.n_mem + a.L;
@@ -884,7 +895,10 @@ __device__ __forceinline__ void attention_body(const mv2_attn_args& a, const Att
     const int qi = idx / D, d = idx % D;
     const int i = q0 + qi;
     float v = 0.f;
-    if (i < a.L) v = to_f32<T>(qkv[(base + (int64_t)i * a.tok_stride) * row_stride + h * D + d]);
+    if (i < a.L) {
+      if (tl.q) v = to_f32<T>(((const T*)tl.q)[(so * tl.q_outer + sn * a.inner_stride + (int64_t)(i - tl.q_begin) * a.tok_stride) * row_stride + h * D + d]);
+      else v = to_f32<T>(qkv[(base + (int64_t)i * a.tok_stride) * row_stride + h * D + d]);
+    }
     Qs[qi][d] = v;
   }
   float m[8], l[8], o[8][DPL];
@@ -908,9 +922,9 @@ __device__ __forceinline__ void attention_body(const mv2_attn_args& a, const Att
         kv = a.mem_kv[(((int64_t)0 * a.heads + h) * a.n_mem + jg) * D + d];
         vv = a.mem_kv[(((int64_t)1 * a.heads + h) * a.n_mem + jg) * D + d];
       } else if (jg < Ltot) {
-        const int64_t tokrow = (base + (int64_t)(jg - a.n_mem) * a.tok_stride) * row_stride;
-        kv = to_f32<T>(qkv[tokrow + HD + h * D + d]);
-        vv = to_f32<T>(qkv[tokrow + 2 * HD + h * D + d]);
+        const int64_t tokrow = (base + (int64_t)(jg - a.n_mem) * a.tok_stride) * kv_stride + k_off;
+        kv = to_f32<T>(qkv[tokrow + h * D + d]);
+        vv = to_f32<T>(qkv[tokrow + HD + h * D + d]);
       }
       Ks[j][d] = kv;
       Vs[j][d] = vv;
@@ -949,13 +963,18 @@ __device__ __forceinline__ void attention_body(const mv2_attn_args& a, const Att
     const int i = q0 + warp * 8 + r;
     if (i >= a.L) continue;
     const float inv = DROP ? dr.scale / l[r] : 1.f / l[r];
-    T* orow = out + (base + (int64_t)i * a.tok_stride) * HD + h * D;
+    const int64_t obase = tl.out_outer < 0 ? base : so * tl.out_outer + sn * a.inner_stride;
+    T* orow = out + (obase + (int64_t)(i - tl.q_begin) * a.tok_stride) * HD + h * D;
 #pragma unroll
     for (int dd = 0; dd < DPL; ++dd) orow[lane + 32 * dd] = from_f32<T>(o[r][dd] * inv);
   }
 }
 template <typename T, int DPL>
 __global__ void __launch_bounds__(128) attention_kernel(const mv2_attn_args a) { attention_body<T, DPL, false>(a, AttnDrop{}); }
+template <typename T, int DPL>
+__global__ void __launch_bounds__(128) attention_tail_kernel(const mv2_attn_args a, const AttnTail tl) {
+  attention_body<T, DPL, false>(a, AttnDrop{}, tl);
+}
 template <typename T, int DPL>
 __global__ void __launch_bounds__(128) attention_dropout_kernel(const mv2_attn_args a, const AttnDrop d) {
   attention_body<T, DPL, true>(a, d);
@@ -969,7 +988,7 @@ __global__ void __launch_bounds__(128) attention_dropout_kernel(const mv2_attn_a
 // ------------------------------------------------------------------------------------------
 constexpr int AS_L = 8, AS_M = 8;      // max tokens / memory slots
 template <int DPL, bool DROP>
-__device__ __forceinline__ void attention_small_body(const mv2_attn_args& a, const AttnDrop& dr) {
+__device__ __forceinline__ void attention_small_body(const mv2_attn_args& a, const AttnDrop& dr, const AttnTail tl = AttnTail{0, -1, nullptr, 0}) {
   pdl_wait();
   pdl_launch_dependents();
   constexpr int D = DPL * 32;
@@ -1002,7 +1021,13 @@ __device__ __forceinline__ void attention_small_body(const mv2_attn_args& a, con
     for (int dd = 0; dd < DPL; ++dd) {
       const int d = lane + 32 * dd;
       float qv = 0.f, kv = 0.f, vv = 0.f;
-      if (i < L) {
+      if (i < L && tl.q) {        // K/V cache rows '(kv h d)'; the queries of rows >= q_begin from the chunk
+        const int64_t row = (base + (int64_t)i * a.tok_stride) * (2 * (int64_t)HD) + h * D + d;
+        kv = __bfloat162float(qkv[row]); vv = __bfloat162float(qkv[row + HD]);
+        if (i >= tl.q_begin)
+          qv = __bfloat162float(((const __nv_bfloat16*)tl.q)[((seq / a.n_inner) * tl.q_outer + (seq % a.n_inner) * a.inner_stride +
+                                                            (int64_t)(i - tl.q_begin) * a.tok_stride) * row_stride + h * D + d]);
+      } else if (i < L) {
         const int64_t row = (base + (int64_t)i * a.tok_stride) * row_stride + h * D + d;
         qv = __bfloat162float(qkv[row]); kv = __bfloat162float(qkv[row + HD]); vv = __bfloat162float(qkv[row + 2 * HD]);
       }
@@ -1019,6 +1044,7 @@ __device__ __forceinline__ void attention_small_body(const mv2_attn_args& a, con
 #pragma unroll
   for (int i = 0; i < AS_L; ++i) {
     if (i >= L) break;
+    if (i < tl.q_begin) continue;
     const uint32_t keep_i = DROP ? __shfl_sync(0xffffffffu, keep, 4 * i) : 0u;
     float sc[AS_M + AS_L], mx = -INFINITY;
 #pragma unroll
@@ -1045,13 +1071,18 @@ __device__ __forceinline__ void attention_small_body(const mv2_attn_args& a, con
       for (int dd = 0; dd < DPL; ++dd) o[dd] = fmaf(ev, v[j][dd], o[dd]);
     }
     const float inv = DROP ? dr.scale / den : 1.f / den;
-    __nv_bfloat16* orow = out + (base + (int64_t)i * a.tok_stride) * HD + h * D;
+    const int64_t obase = tl.out_outer < 0 ? base : (seq / a.n_inner) * tl.out_outer + (seq % a.n_inner) * a.inner_stride;
+    __nv_bfloat16* orow = out + (obase + (int64_t)(i - tl.q_begin) * a.tok_stride) * HD + h * D;
 #pragma unroll
     for (int dd = 0; dd < DPL; ++dd) orow[lane + 32 * dd] = __float2bfloat16_rn(o[dd] * inv);
   }
 }
 template <int DPL>
 __global__ void __launch_bounds__(256) attention_small_kernel(const mv2_attn_args a) { attention_small_body<DPL, false>(a, AttnDrop{}); }
+template <int DPL>
+__global__ void __launch_bounds__(256) attention_small_tail_kernel(const mv2_attn_args a, const AttnTail tl) {
+  attention_small_body<DPL, false>(a, AttnDrop{}, tl);
+}
 template <int DPL>
 __global__ void __launch_bounds__(256) attention_small_dropout_kernel(const mv2_attn_args a, const AttnDrop d) {
   attention_small_body<DPL, true>(a, d);
@@ -2248,7 +2279,7 @@ __global__ void __launch_bounds__(1024) lfq_aux_final_wide_kernel(const float* _
 // ------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(256) gateloop_scan_kernel(const T* __restrict__ qkva, const T* __restrict__ res, T* __restrict__ out,
-                                                            int Tn, int64_t PC, int C, int64_t total) {
+                                                            int Tn, int64_t PC, int C, int64_t total, float* __restrict__ state) {
   pdl_wait();
   pdl_launch_dependents();
   const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;      // over B * P * C
@@ -2257,7 +2288,7 @@ __global__ void __launch_bounds__(256) gateloop_scan_kernel(const T* __restrict_
   const int64_t p = pc / C;
   const int c = (int)(pc - p * C);
   const int64_t P = PC / C;
-  float s = 0.f;
+  float s = state ? state[i] : 0.f;
   for (int t = 0; t < Tn; ++t) {
     const int64_t pos = (b * Tn + t) * P + p;
     const T* row = qkva + pos * 3 * C;
@@ -2265,6 +2296,7 @@ __global__ void __launch_bounds__(256) gateloop_scan_kernel(const T* __restrict_
     s = fmaf(1.f / (1.f + expf(-a)), s, kv);
     out[pos * C + c] = from_f32<T>(fmaf(q, s, to_f32<T>(res[pos * C + c])));
   }
+  if (state) state[i] = s;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2603,7 +2635,12 @@ int mv2_ingest_kwpack(const void* src, int src_dtype, void* dst, int B, int C, i
 }
 
 int mv2_conv_forward(const mv2_conv_args* a, void* stream) {
-  MV2_CHECK_ARG(a && a->x && a->w && a->y);
+  const mv2_conv_hist none = {nullptr, 0, 0};
+  return mv2_conv_forward_hist(a, &none, stream);
+}
+
+int mv2_conv_forward_hist(const mv2_conv_args* a, const mv2_conv_hist* hist, void* stream) {
+  MV2_CHECK_ARG(a && a->x && a->w && a->y && hist && hist->T_h >= 0 && (hist->T_h == 0 || hist->h));
   MV2_CHECK_ARG(a->B > 0 && a->Ti > 0 && a->Hi > 0 && a->Wi > 0 && a->Ci > 0);
   MV2_CHECK_ARG(a->To > 0 && a->Ho > 0 && a->Wo > 0 && a->Co > 0);
   MV2_CHECK_ARG(a->kt > 0 && a->kh > 0 && a->kw > 0 && a->st > 0 && a->sh > 0 && a->sw > 0);
@@ -2612,8 +2649,8 @@ int mv2_conv_forward(const mv2_conv_args* a, void* stream) {
   const int64_t M = (int64_t)a->B * a->To * a->Ho * a->Wo;
   dim3 grid(ceil_div(M, CBM), ceil_div(a->Co, CBN));
   cudaStream_t st = (cudaStream_t)stream;
-  if (a->dtype == MV2_F32) launch_k(conv_simt_kernel<float>, dim3(grid), dim3(256), 0, st, *a);
-  else if (a->dtype == MV2_BF16) launch_k(conv_simt_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, *a);
+  if (a->dtype == MV2_F32) launch_k(conv_simt_kernel<float>, dim3(grid), dim3(256), 0, st, *a, *hist);
+  else if (a->dtype == MV2_BF16) launch_k(conv_simt_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, *a, *hist);
   else { set_error("bad dtype %d", a->dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -2799,31 +2836,69 @@ int mv2_gate_residual(const void* y, const void* x, const float* gates, void* ou
   return MV2_OK;
 }
 
-int mv2_rmsnorm(const void* x, void* out, int dtype, const float* gamma, int B, int T, int P, int C, int token_shift,
-                void* stream) {
+static int rmsnorm_launch(const void* x, void* out, int dtype, const float* gamma, int B, int T, int P, int C, int token_shift,
+                          const void* prev, int64_t prev_stride, void* stream) {
   MV2_CHECK_ARG(x && out && gamma && B > 0 && T > 0 && P > 0 && C > 0);
   const int64_t n_tok = (int64_t)B * T * P;
   const int blocks = ceil_div(n_tok, 8);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32)
-    launch_k(rmsnorm_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)x, (float*)out, gamma, n_tok, T, P, C, token_shift);
+    launch_k(rmsnorm_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)x, (float*)out, gamma, n_tok, T, P, C, token_shift, (const float*)prev, prev_stride);
   else if (dtype == MV2_BF16 && C % 8 == 0 && C <= 1024 && (!token_shift || (C / 2) % 8 == 0))
     {
       const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
       __nv_bfloat16* ob = (__nv_bfloat16*)out;
       // one token per warp up to C = 512 keeps the most warps in flight on the small README shapes; the widest rows take 4
-      if (C <= 256) launch_k(rmsnorm_bf16x8_kernel<1, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
-      else if (C <= 512) launch_k(rmsnorm_bf16x8_kernel<2, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
-      else launch_k(rmsnorm_bf16x8_kernel<4, 4>, dim3(ceil_div(n_tok, 8 * 4)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift);
+      if (C <= 256) launch_k(rmsnorm_bf16x8_kernel<1, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift, (const __nv_bfloat16*)prev, prev_stride);
+      else if (C <= 512) launch_k(rmsnorm_bf16x8_kernel<2, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift, (const __nv_bfloat16*)prev, prev_stride);
+      else launch_k(rmsnorm_bf16x8_kernel<4, 4>, dim3(ceil_div(n_tok, 8 * 4)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift, (const __nv_bfloat16*)prev, prev_stride);
     }
   else if (dtype == MV2_BF16)
-    launch_k(rmsnorm_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, (__nv_bfloat16*)out, gamma, n_tok, T, P, C, token_shift);
+    launch_k(rmsnorm_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, (__nv_bfloat16*)out, gamma, n_tok, T, P, C, token_shift, (const __nv_bfloat16*)prev, prev_stride);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }
 
+int mv2_rmsnorm(const void* x, void* out, int dtype, const float* gamma, int B, int T, int P, int C, int token_shift,
+                void* stream) {
+  return rmsnorm_launch(x, out, dtype, gamma, B, T, P, C, token_shift, nullptr, 0, stream);
+}
+
+int mv2_rmsnorm_prev(const void* x, const void* prev, int64_t prev_clip_stride, void* out, int dtype, const float* gamma,
+                     int B, int T, int P, int C, void* stream) {
+  MV2_CHECK_ARG(prev && prev_clip_stride >= (int64_t)P * C);
+  return rmsnorm_launch(x, out, dtype, gamma, B, T, P, C, 1, prev, prev_clip_stride, stream);
+}
+
 int mv2_attention(const mv2_attn_args* a, void* stream) { return attention_dispatch(a, nullptr, stream); }
+
+// the kernel mv2_attention picks for a causal call of this L (the tensor-core kernel is non-causal only), on rows [q_begin, L)
+int mv2_attention_tail(const mv2_attn_args* a, const void* q, int64_t q_outer_stride, int q_begin, void* out,
+                       int64_t out_outer_stride, void* stream) {
+  MV2_CHECK_ARG(a && a->qkv && q && out && a->mem_kv && a->causal && q_outer_stride >= 0);
+  MV2_CHECK_ARG(a->heads > 0 && a->dim_head > 0 && a->dim_head % 32 == 0 && a->dim_head <= 96);
+  MV2_CHECK_ARG(a->n_mem >= 0 && a->n_outer > 0 && a->n_inner > 0 && a->L > 0 && q_begin >= 0 && q_begin < a->L);
+  MV2_CHECK_ARG(out_outer_stride >= 0 && (int64_t)a->n_outer * a->n_inner <= 2147483647LL);
+  const AttnTail tl{q_begin, out_outer_stride, q, q_outer_stride};
+  mv2_attn_args o = *a;
+  o.out = out;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int dpl = a->dim_head / 32;
+  if (a->dtype == MV2_BF16 && a->L <= AS_L && a->n_mem <= AS_M && (dpl == 1 || dpl == 2)) {
+    const dim3 grid((unsigned)ceil_div((int64_t)a->n_outer * a->n_inner * a->heads, 8));
+    if (dpl == 1) launch_k(attention_small_tail_kernel<1>, grid, dim3(256), 0, st, o, tl);
+    else launch_k(attention_small_tail_kernel<2>, grid, dim3(256), 0, st, o, tl);
+  } else if (a->dtype == MV2_F32 || a->dtype == MV2_BF16) {
+    const dim3 grid((unsigned)((int64_t)a->n_outer * a->n_inner), a->heads, ceil_div(a->L - q_begin, AT_Q));
+    const bool f32 = a->dtype == MV2_F32;
+    if (dpl == 1) f32 ? launch_k(attention_tail_kernel<float, 1>, grid, dim3(128), 0, st, o, tl) : launch_k(attention_tail_kernel<__nv_bfloat16, 1>, grid, dim3(128), 0, st, o, tl);
+    else if (dpl == 2) f32 ? launch_k(attention_tail_kernel<float, 2>, grid, dim3(128), 0, st, o, tl) : launch_k(attention_tail_kernel<__nv_bfloat16, 2>, grid, dim3(128), 0, st, o, tl);
+    else f32 ? launch_k(attention_tail_kernel<float, 3>, grid, dim3(128), 0, st, o, tl) : launch_k(attention_tail_kernel<__nv_bfloat16, 3>, grid, dim3(128), 0, st, o, tl);
+  } else { set_error("bad dtype %d", a->dtype); return MV2_E_ARG; }
+  MV2_CHECK_LAUNCH();
+  return MV2_OK;
+}
 
 int mv2_attention_dropout(const mv2_attn_args* a, const mv2_dropout_args* dp, void* stream) {
   MV2_CHECK_ARG(a);
@@ -3036,15 +3111,20 @@ int mv2_lfq_aux_finalize(const float* avg_prob_sum, const float* stats, int d, i
 }
 
 int mv2_gateloop_scan(const void* qkva, const void* res, void* out, int dtype, int B, int T, int P, int C, void* stream) {
+  return mv2_gateloop_scan_state(qkva, res, out, dtype, B, T, P, C, nullptr, stream);
+}
+
+int mv2_gateloop_scan_state(const void* qkva, const void* res, void* out, int dtype, int B, int T, int P, int C, float* state,
+                            void* stream) {
   MV2_CHECK_ARG(qkva && res && out && B > 0 && T > 0 && P > 0 && C > 0);
   const int64_t total = (int64_t)B * P * C;
   const int64_t blocks = ceil_div(total, (int64_t)256);
   MV2_CHECK_ARG(blocks <= 2147483647LL);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32)
-    launch_k(gateloop_scan_kernel<float>, dim3((unsigned)blocks), dim3(256), 0, st, (const float*)qkva, (const float*)res, (float*)out, T, (int64_t)P * C, C, total);
+    launch_k(gateloop_scan_kernel<float>, dim3((unsigned)blocks), dim3(256), 0, st, (const float*)qkva, (const float*)res, (float*)out, T, (int64_t)P * C, C, total, state);
   else if (dtype == MV2_BF16)
-    launch_k(gateloop_scan_kernel<__nv_bfloat16>, dim3((unsigned)blocks), dim3(256), 0, st, (const __nv_bfloat16*)qkva, (const __nv_bfloat16*)res, (__nv_bfloat16*)out, T, (int64_t)P * C, C, total);
+    launch_k(gateloop_scan_kernel<__nv_bfloat16>, dim3((unsigned)blocks), dim3(256), 0, st, (const __nv_bfloat16*)qkva, (const __nv_bfloat16*)res, (__nv_bfloat16*)out, T, (int64_t)P * C, C, total, state);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;

@@ -35,12 +35,15 @@ constexpr int TC_BM = 128;
 
 struct alignas(64) TcParams {
   CUtensorMap amap[TC_MAX_MAPS];
+  CUtensorMap hmap;      // history frames in front of x (mv2_conv_hist; stride 1 only): used when frame_loads > 1
   CUtensorMap wmap;
   int8_t tap_map[TC_MAX_TAPS], tap_dt[TC_MAX_TAPS], tap_dh[TC_MAX_TAPS], tap_dw[TC_MAX_TAPS];
   int ntaps, kchunks, ci_pad, bk;
   int B, To, Ho, Wo, Co;
   int bt, bh, bw, tt, th, tw;
   int bn, stages;
+  int hist_T;
+  int frame_loads;       // hist_T = 0: 1 box of bt frames per stage; else bt boxes of one frame, each from x or the history
   TcEpi epi;
 };
 
@@ -98,8 +101,15 @@ __global__ void __launch_bounds__(384, 1) tc_conv_kernel(const __grid_constant__
         mbar_wait(empty0 + 8 * s, ph ^ 1);
         mbar_expect_tx(full0 + 8 * s, stage_bytes);
         const uint32_t sa = smem_base + s * stage_bytes;
-        tma_load_5d(sa, &p.amap[p.tap_map[tap]], full0 + 8 * s, kc * bk, w0 + p.tap_dw[tap], h0 + p.tap_dh[tap],
-                    t0 + p.tap_dt[tap], b);
+        if (p.hist_T == 0)
+          tma_load_5d(sa, &p.amap[p.tap_map[tap]], full0 + 8 * s, kc * bk, w0 + p.tap_dw[tap], h0 + p.tap_dh[tap],
+                      t0 + p.tap_dt[tap], b);
+        else
+          for (int lt = 0; lt < p.frame_loads; ++lt) {     // frames in front of the chunk come from the history
+            const int ti = t0 + lt + p.tap_dt[tap];
+            tma_load_5d(sa + lt * (uint32_t)(p.bw * p.bh) * row_bytes, ti >= 0 ? &p.amap[0] : &p.hmap, full0 + 8 * s, kc * bk,
+                        w0 + p.tap_dw[tap], h0 + p.tap_dh[tap], ti >= 0 ? ti : ti + p.hist_T, b);
+          }
         tma_load_2d(sa + a_bytes, &p.wmap, full0 + 8 * s, tap * p.ci_pad + kc * bk, n0);
         if (++kc == p.kchunks) { kc = 0; ++tap; }
         if (++s == (uint32_t)p.stages) { s = 0; ph ^= 1; }
@@ -166,6 +176,20 @@ using namespace mv2;
 
 extern "C" {
 
+// output tile box of a launch: bw * bh * bt = 128 positions
+static void tc_tile_box(const mv2_tc_conv_args* a, int& bw, int& bh, int& bt) {
+  bw = std::min(128, pow2_ceil(a->Wo));
+  bh = std::min(128 / bw, pow2_ceil(a->Ho));
+  bt = 128 / (bw * bh);
+}
+
+int mv2_tc_conv_hist_supported(const mv2_tc_conv_args* a) {
+  if (!mv2_tc_conv_supported(a) || a->st != 1 || a->sh != 1 || a->sw != 1) return 0;
+  int bw, bh, bt;
+  tc_tile_box(a, bw, bh, bt);
+  return bt == 1 || (bw * bh) % 8 == 0;      // one box per frame: each must start on a whole swizzle pattern (8 rows)
+}
+
 int mv2_tc_conv_supported(const mv2_tc_conv_args* a) {
   if (!a) return 0;
   if (a->Ci % 16 != 0) return 0;                    // TMA inner box = 32/64/128 B, global strides multiple of 16 B
@@ -181,8 +205,12 @@ int mv2_tc_conv_supported(const mv2_tc_conv_args* a) {
   return 1;
 }
 
-int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) {
+int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) { return mv2_tc_conv_forward_hist(a, nullptr, stream); }
+
+int mv2_tc_conv_forward_hist(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream) {
   MV2_CHECK_ARG(a && a->x && a->w && a->y);
+  MV2_CHECK_ARG(!hist || (hist->T_h >= 0 && (hist->T_h == 0 || (hist->h && hist->clip_stride > 0))));
+  const int hist_T = hist ? hist->T_h : 0;
   if (!mv2_tc_conv_supported(a)) { set_error("mv2_tc_conv_forward: unsupported shape (Ci=%d Co=%d)", a->Ci, a->Co); return MV2_E_UNSUPPORTED; }
 
   TcParams p;
@@ -194,10 +222,14 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) {
   p.kchunks = a->Ci / bk;
   p.B = a->B; p.To = a->To; p.Ho = a->Ho; p.Wo = a->Wo; p.Co = a->Co;
   // output tile box: bw * bh * bt = 128
-  p.bw = std::min(128, pow2_ceil(a->Wo));
-  p.bh = std::min(128 / p.bw, pow2_ceil(a->Ho));
-  p.bt = 128 / (p.bw * p.bh);
+  tc_tile_box(a, p.bw, p.bh, p.bt);
   p.tw = ceil_div(a->Wo, p.bw); p.th = ceil_div(a->Ho, p.bh); p.tt = ceil_div(a->To, p.bt);
+  p.hist_T = hist_T;
+  p.frame_loads = hist_T > 0 ? p.bt : 1;
+  if (hist_T > 0 && !mv2_tc_conv_hist_supported(a)) {
+    set_error("mv2_tc_conv_forward_hist: unsupported shape (mv2_tc_conv_hist_supported)");
+    return MV2_E_UNSUPPORTED;
+  }
   // N tile: 32, 64 or 128 columns (a wgmma N, 64 fp32 accumulator registers per thread at 128); wider outputs take
   // several N tiles, a ragged last one reads zero-filled weight rows and stores nothing for them
   const int bn = a->Co <= 32 ? 32 : (a->Co <= 64 ? 64 : 128);
@@ -227,12 +259,18 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) {
         const cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)nW, (cuuint64_t)nH, (cuuint64_t)nT, (cuuint64_t)a->B};
         const cuuint64_t strides[4] = {(cuuint64_t)(sw * C * 2), (cuuint64_t)(sh * W * C * 2), (cuuint64_t)(st * H * W * C * 2),
                                        (cuuint64_t)(T * H * W * C * 2)};
-        const cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)p.bw, (cuuint32_t)p.bh, (cuuint32_t)p.bt, 1};
+        const cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)p.bw, (cuuint32_t)p.bh, (cuuint32_t)(128 / (p.bw * p.bh * p.frame_loads)), 1};
         const char* base = (const char*)a->x + ((int64_t)pt * H * W + (int64_t)ph * W + pw) * C * 2;
         char what[32];
         snprintf(what, sizeof(what), "activations, phase %d", id);
         if (const int rc = encode_bf16_map(&p.amap[id], 5, base, dims, strides, box, swz, what)) return rc;
       }
+  if (hist_T > 0) {
+    const cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)hist_T, (cuuint64_t)a->B};
+    const cuuint64_t strides[4] = {(cuuint64_t)(C * 2), (cuuint64_t)(W * C * 2), (cuuint64_t)(H * W * C * 2), (cuuint64_t)(hist->clip_stride * 2)};
+    const cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)p.bw, (cuuint32_t)p.bh, 1, 1};
+    if (const int rc = encode_bf16_map(&p.hmap, 5, hist->h, dims, strides, box, swz, "history")) return rc;
+  }
   // ---- taps ----
   p.ntaps = a->kt * a->kh * a->kw;
   for (int dt = 0; dt < a->kt; ++dt)

@@ -12,7 +12,8 @@
 //     tile from shared memory, dividing weight traffic by mw (mw * bn <= 128: the mw accumulators of a consumer
 //     warpgroup fit 64 fp32 registers per thread);
 //   * CTAs are persistent with a static, cost-sorted serpentine tile schedule (slab_frame_of / slab_tile_of);
-//   * causal frames in front of the clip (t + dt - pt < 0) are all-zero and are skipped outright;
+//   * causal frames in front of the clip (t + dt - pt < 0) come from the history map (hmap: the tail of the previous chunk
+//     of a streamed clip, hist_T frames); those in front of the history are all-zero and are skipped outright;
 //   * N tiles need not divide Co (the plain / GEGLU epilogues guard every stored column): wide outputs without a
 //     128-column divisor take 128-column tiles with a ragged last one;
 //   * the kernel is instantiated per epilogue flavour (tc_common.cuh: EPI_*) and N tile (32 / 64 / 128); the plain
@@ -35,10 +36,12 @@ namespace mv2 {
 
 struct alignas(64) SlabParams {
   CUtensorMap amap;
+  CUtensorMap hmap;      // history frames in front of x (mv2_conv_hist), hist_T of them; unused when hist_T = 0
   CUtensorMap wmap;      // weights as {ci, co, tap} (3-D boxes of tpw taps)
   CUtensorMap wmap2;     // weights as {k, co} (2-D boxes, used when tpw == 1)
   int kt, kh, kw, pt, ph, pw;
   int st;                // stride along t (1, or 2: TimeDownsample2x); spatial strides are always 1 in this kernel
+  int hist_T;
   int Ci, kchunks, row_bytes;
   int B, T, H, W, Co;
   int mw, pitch, slab_h, slab_bytes, slab_stride;
@@ -147,7 +150,11 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
     for (int s = 0; s < p.w_stages; ++s) { mbar_init(w_full + 8 * s, 1); mbar_init(w_empty + 8 * s, 8); }
     fence_barrier_init();
   }
-  if (warp == 0 && lane == 0) { tma_prefetch_desc(&p.amap); if (MODE == EPI_DOWN_SPACE) tma_prefetch_desc(&p.amap_odd); }
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&p.amap);
+    if (MODE == EPI_DOWN_SPACE) tma_prefetch_desc(&p.amap_odd);
+    else if (p.hist_T > 0) tma_prefetch_desc(&p.hmap);
+  }
   if (warp == 2 && lane == 0) {
     tma_prefetch_desc(&p.wmap); tma_prefetch_desc(&p.wmap2);
     if (MODE == EPI_FUSED_RU) tma_prefetch_desc(&p.w1map);
@@ -195,13 +202,14 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
         uint32_t s = 0, ph = 0;
         for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
           const TileCoord c = decode_tile(p, tile);
-          const int dt0 = max(0, p.pt - c.t * p.st);
+          const int dt0 = max(0, p.pt - c.t * p.st - p.hist_T);
           for (int dt = dt0; dt < p.kt; ++dt)
             for (int kc = 0; kc < p.kchunks; ++kc) {
               mbar_wait(slab_empty + 8 * s, ph ^ 1);
               mbar_expect_tx(slab_full + 8 * s, p.slab_bytes);
-              tma_load_5d(slab0 + s * p.slab_stride, &p.amap, slab_full + 8 * s, kc * bk, c.w0 - p.pw, c.h0 - p.ph,
-                          c.t * p.st + dt - p.pt, c.b);
+              const int ti = c.t * p.st + dt - p.pt;
+              tma_load_5d(slab0 + s * p.slab_stride, ti >= 0 ? &p.amap : &p.hmap, slab_full + 8 * s, kc * bk, c.w0 - p.pw,
+                          c.h0 - p.ph, ti >= 0 ? ti : ti + p.hist_T, c.b);
               if (++s == (uint32_t)p.slab_stages) { s = 0; ph ^= 1; }
             }
         }
@@ -228,7 +236,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
         uint32_t s = 0, ph = 0;
         for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
           const TileCoord c = decode_tile(p, tile);
-          const int dt0 = max(0, p.pt - c.t * p.st);
+          const int dt0 = max(0, p.pt - c.t * p.st - p.hist_T);
           for (int dt = dt0; dt < p.kt; ++dt)
             for (int kc = 0; kc < p.kchunks; ++kc)
               for (int tp = 0; tp < taps2d; tp += p.tpw) {
@@ -329,7 +337,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
           if (++s_idx == (uint32_t)p.slab_stages) { s_idx = 0; s_par ^= 1; }
         }
       } else {
-        const int dt0 = max(0, p.pt - c.t * p.st);
+        const int dt0 = max(0, p.pt - c.t * p.st - p.hist_T);
         for (int dt = dt0; dt < p.kt; ++dt)
           for (int kc = 0; kc < p.kchunks; ++kc) {
             mbar_wait(slab_full + 8 * s_idx, s_par);
@@ -761,13 +769,19 @@ static int slab_fill_plan(const mv2_tc_conv_args* a, SlabParams& p) {
 
 // TMA maps of a stride-1 slab conv: the activation slab (box {bk, pitch, slab_h, 1, 1} of x as {Ci, Wi, Hi, Ti, B}) and the
 // weights [Co][tap][Ci] as {ci, co, tap} (box {bk, bn, tpw}: tpw consecutive K-major tiles) and as {k, co} (box {bk, bn}).
-static int slab_encode_maps(SlabParams& p, const mv2_tc_conv_args* a) {
+static int slab_encode_maps(SlabParams& p, const mv2_tc_conv_args* a, const mv2_conv_hist* hist = nullptr) {
   const CUtensorMapSwizzle swz = swizzle_of_row(p.row_bytes);
   const int64_t C = a->Ci, W = a->Wi, H = a->Hi, T = a->Ti;
   const cuuint64_t xdims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)T, (cuuint64_t)a->B};
   const cuuint64_t xstrides[4] = {(cuuint64_t)(C * 2), (cuuint64_t)(W * C * 2), (cuuint64_t)(H * W * C * 2), (cuuint64_t)(T * H * W * C * 2)};
   const cuuint32_t xbox[5] = {(cuuint32_t)p.row_bytes / 2, (cuuint32_t)p.pitch, (cuuint32_t)p.slab_h, 1, 1};
   if (const int rc = encode_bf16_map(&p.amap, 5, a->x, xdims, xstrides, xbox, swz, "slab")) return rc;
+  p.hist_T = hist ? hist->T_h : 0;
+  if (p.hist_T > 0) {     // the same boxes over the history: (T_h frames, clip stride of the tensor it lives in)
+    const cuuint64_t hdims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)p.hist_T, (cuuint64_t)a->B};
+    const cuuint64_t hstrides[4] = {xstrides[0], xstrides[1], xstrides[2], (cuuint64_t)(hist->clip_stride * 2)};
+    if (const int rc = encode_bf16_map(&p.hmap, 5, hist->h, hdims, hstrides, xbox, swz, "history")) return rc;
+  }
   const int64_t ntaps = (int64_t)a->kt * a->kh * a->kw, K = ntaps * C;
   const cuuint64_t wdims[3] = {(cuuint64_t)C, (cuuint64_t)a->Co, (cuuint64_t)ntaps}, kdims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
   const cuuint64_t wstrides[2] = {(cuuint64_t)(K * 2), (cuuint64_t)(C * 2)};
@@ -830,12 +844,15 @@ extern "C" int mv2_tc_slab_tile(const mv2_tc_conv_args* a, int n_sm, int cta, in
   return MV2_OK;
 }
 
-extern "C" int mv2_tc_slab_forward(const mv2_tc_conv_args* a, void* stream) {
+extern "C" int mv2_tc_slab_forward(const mv2_tc_conv_args* a, void* stream) { return mv2_tc_slab_forward_hist(a, nullptr, stream); }
+
+extern "C" int mv2_tc_slab_forward_hist(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream) {
   MV2_CHECK_ARG(a && a->x && a->w && a->y);
+  MV2_CHECK_ARG(!hist || (hist->T_h >= 0 && (hist->T_h == 0 || (hist->h && hist->clip_stride > 0))));
   if (!mv2_tc_slab_supported(a)) { set_error("mv2_tc_slab_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }
   SlabParams p;
   if (const int rc = slab_fill_plan(a, p)) return rc;
-  if (const int rc = slab_encode_maps(p, a)) return rc;
+  if (const int rc = slab_encode_maps(p, a, hist)) return rc;
   int mode = EPI_PLAIN;
   if (a->epi_mode == 1) mode = EPI_GEGLU;
   else if (a->shuffle != MV2_SHUFFLE_NONE && (a->Co / (a->shuffle == MV2_SHUFFLE_SPACE ? 4 : 2)) % 32 == 0) mode = EPI_SHUFFLE_ST;
@@ -901,14 +918,17 @@ extern "C" size_t mv2_tc_ru_workspace_bytes(const mv2_tc_ru_args* a) {
   return (F * recs * (a->C + 2) + F * (a->C + 16)) * sizeof(float);    // pool records + the SE hidden layer (mv2_se_gate_records)
 }
 
-extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, void* stream) {
+extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, void* stream) { return mv2_tc_ru_forward_hist(a, nullptr, stream); }
+
+extern "C" int mv2_tc_ru_forward_hist(const mv2_tc_ru_args* a, const mv2_conv_hist* hist, void* stream) {
   MV2_CHECK_ARG(a && a->x && a->w3 && a->w1 && a->y && a->se_wk && a->se_ws);
+  MV2_CHECK_ARG(!hist || (hist->T_h >= 0 && (hist->T_h == 0 || (hist->h && hist->clip_stride > 0))));
   if (!mv2_tc_ru_supported(a)) { set_error("mv2_tc_ru_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }
   SlabParams p;
   if (const int rc = ru_fill_plan(a, p)) return rc;
   mv2_tc_conv_args c;
   ru_as_conv_args(a, &c);
-  if (const int rc = slab_encode_maps(p, &c)) return rc;
+  if (const int rc = slab_encode_maps(p, &c, hist)) return rc;
   const cuuint64_t dims1[2] = {(cuuint64_t)a->C, (cuuint64_t)a->C};
   const cuuint64_t strides1[1] = {(cuuint64_t)a->C * 2};
   const cuuint32_t box1[2] = {64, (cuuint32_t)p.bn};

@@ -16,7 +16,7 @@ import torch
 
 from . import _lib
 from ._lib import (ACT_ELU, ACT_NONE, ACT_SILU, MV2_BF16, MV2_F32, MV2_U8, SHUFFLE_NONE, SHUFFLE_SPACE,
-                   SHUFFLE_TIME, AttnArgs, ConvArgs, TcConvArgs, TcRuArgs, check)
+                   SHUFFLE_TIME, AttnArgs, ConvArgs, ConvHist, TcConvArgs, TcRuArgs, check)
 
 
 def _dt(t: torch.dtype) -> int:
@@ -49,6 +49,29 @@ class AttnDropout:
         a = _lib.DropoutArgs(seed=self.seed, call=self.calls, p=self.p)
         self.calls += 1
         return a
+
+
+class StreamState:
+    """Causal state of a streamed clip batch (stream.py), carried from one push to the next: per layer, the history frames
+    of a causal conv, the previous frame of a token shift, the time attention's qkv cache, the gateloop scan state.  A
+    view with a key prefix (`sub`) is what the layer functions receive; None everywhere means a whole-clip call."""
+
+    def __init__(self, slots=None, prefix=""):
+        self._slots = {} if slots is None else slots
+        self._prefix = prefix
+
+    def sub(self, name) -> "StreamState":
+        return StreamState(self._slots, f"{self._prefix}{name}/")
+
+    def get(self, name):
+        return self._slots.get(self._prefix + name)
+
+    def put(self, name, value):
+        self._slots[self._prefix + name] = value
+
+
+def _sub(ss: Optional[StreamState], name):
+    return None if ss is None else ss.sub(name)
 
 
 @dataclass
@@ -318,11 +341,49 @@ class Engine:
     def _new(self, shape, dtype=None):
         return torch.empty(shape, device=self.device, dtype=dtype or self.dtype)
 
+    def _conv_hist(self, ss: Optional[StreamState], x, need: int):
+        """(mv2_conv_hist of the frames in front of x, state update to run after the launch) of a causal conv whose input
+        reaches `need` frames back; (None, None) for a whole-clip call.  The history is a frame range of an earlier input
+        (tensor, first frame, count); only when it has to span two chunks are the frames copied into a tensor of their own."""
+        if ss is None or need <= 0:
+            return None, None
+        h = ss.get("hist")
+        hist = None
+        if h is not None:
+            t, t0, n = h
+            fe = t[0, 0].numel()
+            hist = ConvHist(h=t.data_ptr() + t0 * fe * t.element_size(), T_h=n, clip_stride=t.shape[1] * fe)
+
+        def advance():
+            T = x.shape[1]
+            if T >= need or h is None:
+                keep = min(need, T)
+                ss.put("hist", (x, T - keep, keep))
+                return
+            t, t0, n = h
+            old = min(n, need - T)
+            buf = self._new((x.shape[0], old + T) + tuple(x.shape[2:]), x.dtype)
+            self.copy_frames(t, t0 + n - old, old, dst=buf, dst_t0=0)
+            self.copy_frames(x, 0, T, dst=buf, dst_t0=old)
+            ss.put("hist", (buf, 0, old + T))
+        return hist, advance
+
+    def _hist_cat(self, ss: StreamState, x):
+        """[carried history | x] as one new (B, T_h + T, ...) tensor."""
+        t, t0, n = ss.get("hist")
+        cat = self._new((x.shape[0], n + x.shape[1]) + tuple(x.shape[2:]), x.dtype)
+        self.copy_frames(t, t0, n, dst=cat, dst_t0=0)
+        self.copy_frames(x, 0, x.shape[1], dst=cat, dst_t0=n)
+        return cat
+
     def conv(self, x, pk: ConvPack, *, stride=(1, 1, 1), pad=None, out_spatial=None, act=ACT_NONE,
-             res=None, shuffle=SHUFFLE_NONE, token_shift=False, out_cf=False, oscale=None):
+             res=None, shuffle=SHUFFLE_NONE, token_shift=False, out_cf=False, oscale=None, ss: Optional[StreamState] = None):
         """x: (B,T,H,W,Ci) channels-last.  `pad` = leading (pt,ph,pw); causal default (kt-1, kh//2, kw//2).
-        out_cf (wgmma slab path, Co % 8 != 0 only): write torch's (B,Co,To,Ho,Wo) layout directly."""
+        out_cf (wgmma slab path, Co % 8 != 0 only): write torch's (B,Co,To,Ho,Wo) layout directly.
+        ss: stream state of this conv -- the frames in front of x are read from the carried history, and the last
+        k_t - 1 input frames are kept for the next chunk."""
         B, Ti, Hi, Wi, Ci = x.shape
+        hist, advance = self._conv_hist(ss, x, pk.k[0] - 1)
         tc_ok = (self.dtype == torch.bfloat16 and self.use_tc and pk.w_tc is not None and not token_shift
                  and Ci == pk.Ci_tc)
         kt, kh, kw = pk.k_tc if (tc_ok and pk.k_tc) else pk.k
@@ -364,9 +425,21 @@ class Engine:
                 if use_down:
                     check(self.lib.mv2_tc_down_space_forward(C.byref(ta), self._stream()), "mv2_tc_down_space_forward")
                     self.slab_calls += 1
+                elif use_slab and hist is not None:
+                    check(self.lib.mv2_tc_slab_forward_hist(C.byref(ta), C.byref(hist), self._stream()), "mv2_tc_slab_forward_hist")
+                    self.slab_calls += 1
                 elif use_slab:
                     check(self.lib.mv2_tc_slab_forward(C.byref(ta), self._stream()), "mv2_tc_slab_forward")
                     self.slab_calls += 1
+                elif hist is not None and self.lib.mv2_tc_conv_hist_supported(C.byref(ta)):
+                    check(self.lib.mv2_tc_conv_forward_hist(C.byref(ta), C.byref(hist), self._stream()), "mv2_tc_conv_forward_hist")
+                elif hist is not None:
+                    # shapes the history operand does not take (a strided conv, or frame tiles of < 8 positions): the same
+                    # kernel on a copy of [history | x] with the leading padding shortened by the history, which gives the
+                    # same products per output element
+                    cat = self._hist_cat(ss, x)
+                    ta.x, ta.Ti, ta.pt = _ptr(cat), cat.shape[1], pad[0] - hist.T_h
+                    check(self.lib.mv2_tc_conv_forward(C.byref(ta), self._stream()), "mv2_tc_conv_forward")
                 else:
                     check(self.lib.mv2_tc_conv_forward(C.byref(ta), self._stream()), "mv2_tc_conv_forward")
                 if self._prof is not None:
@@ -379,6 +452,8 @@ class Engine:
                                               epi_mode=pk.epi_mode, stride=tuple(stride)))
                 self.launches += 1
                 self.tc_calls += 1
+                if advance is not None:
+                    advance()
                 return y
             assert not out_cf, "channels-first output is a wgmma slab-kernel feature"
             assert pk.w is not None and pk.epi_mode in (0, 2) and Ci == pk.Ci, "wgmma-only weight pack has no CUDA-core fallback"
@@ -399,8 +474,13 @@ class Engine:
                      kt=kt, kh=kh, kw=kw, st=stride[0], sh=stride[1], sw=stride[2],
                      pt=pad[0], ph=pad[1], pw=pad[2], act=act, shuffle=shuffle, x_token_shift=int(token_shift),
                      oscale=_ptr(oscale))
-        check(self.lib.mv2_conv_forward(C.byref(a), self._stream()), "mv2_conv_forward")
+        if hist is not None:
+            check(self.lib.mv2_conv_forward_hist(C.byref(a), C.byref(hist), self._stream()), "mv2_conv_forward_hist")
+        else:
+            check(self.lib.mv2_conv_forward(C.byref(a), self._stream()), "mv2_conv_forward")
         self.launches += 1
+        if advance is not None:
+            advance()
         if pk.epi_mode == 2:          # scaled residual: the residual epilogue, then * 2^-0.5 (the reference's add-then-multiply)
             assert res is not None and shuffle == SHUFFLE_NONE
             scale = torch.full((B, pk.Co), 2 ** -0.5, device=self.device, dtype=torch.float32)
@@ -409,7 +489,7 @@ class Engine:
             self.launches += 1
         return y
 
-    def residual_unit(self, x, p):
+    def residual_unit(self, x, p, ss: Optional[StreamState] = None):
         """ResidualUnit (reference M:930-944): x + SE(ELU(conv1(ELU(causal_conv3(x)))))."""
         B, T, H, W, Cc = x.shape
         F_, Pn = B * T, H * W
@@ -421,6 +501,7 @@ class Engine:
                           se_wk=_ptr(p["wk"]), se_bk=p["bk"], y=None, se_ws=None, B=B, T=T, H=H, W=W, C=Cc,
                           kt=c3.k[0], kh=c3.k[1], kw=c3.k[2])
             if self.lib.mv2_tc_ru_supported(C.byref(ra)):
+                hist, advance = self._conv_hist(_sub(ss, "conv3"), x, c3.k[0] - 1)
                 y = self._new(x.shape)
                 ws = self._new((self.lib.mv2_tc_ru_workspace_bytes(C.byref(ra)) // 4,), torch.float32)
                 ra.y, ra.se_ws = _ptr(y), _ptr(ws)
@@ -428,7 +509,12 @@ class Engine:
                 if self._prof is not None:
                     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                     e0.record()
-                check(self.lib.mv2_tc_ru_forward(C.byref(ra), st), "mv2_tc_ru_forward")
+                if hist is not None:
+                    check(self.lib.mv2_tc_ru_forward_hist(C.byref(ra), C.byref(hist), st), "mv2_tc_ru_forward_hist")
+                else:
+                    check(self.lib.mv2_tc_ru_forward(C.byref(ra), st), "mv2_tc_ru_forward")
+                if advance is not None:
+                    advance()
                 if self._prof is not None:
                     e1.record()
                     self._prof.append((e0, e1, 2.0 * B * T * H * W * (c3.macs + c1.macs), "slab", c3.k[0] * c3.k[1] * c3.k[2]))
@@ -445,7 +531,7 @@ class Engine:
                 self.slab_calls += 1
                 self.fused_ru_calls += 1
                 return out
-        h = self.conv(x, c3, act=ACT_ELU)
+        h = self.conv(x, c3, act=ACT_ELU, ss=_sub(ss, "conv3"))
         y = self.conv(h, c1, act=ACT_ELU)
         return self.squeeze_excite_residual(y, x, p)
 
@@ -478,7 +564,7 @@ class Engine:
         p = self._packs[f"{side}_cond_in"]
         return self.dense_small(cond.float().contiguous(), p["w"], p["b"], ACT_SILU)
 
-    def residual_unit_mod(self, x, p, cond_e):
+    def residual_unit_mod(self, x, p, cond_e, ss: Optional[StreamState] = None):
         """ResidualUnitMod (M:978-988): x + ELU(conv_out(ELU(Conv3DMod(x, to_cond(cond))))).  The per-clip modulated weights
         are never built: input channels are scaled by (cond + 1), the shared-weight conv runs unchanged and the demodulation
         rsqrt(sum w_b^2) multiplies the accumulator per (clip, output channel) in the epilogue (include/magvit2_b200.h)."""
@@ -491,21 +577,31 @@ class Engine:
         xs = self._new(x.shape)
         check(self.lib.mv2_scale_channels(_ptr(x), _ptr(scale_in), _ptr(xs), _dt(self.dtype), B, T * H * W, Cc, st), "mv2_scale_channels")
         self.launches += 2
-        h = self.conv(xs, p["conv3"], act=ACT_ELU, oscale=inv_norm)
+        h = self.conv(xs, p["conv3"], act=ACT_ELU, oscale=inv_norm, ss=_sub(ss, "conv3"))
         return self.conv(h, p["conv1"], act=ACT_ELU, res=x)
 
-    def rmsnorm(self, x, gamma, token_shift=False):
+    def rmsnorm(self, x, gamma, token_shift=False, ss: Optional[StreamState] = None):
+        """ss (token shift only): the shifted channels of frame 0 come from the previous chunk's last frame."""
         B, T, H, W, Cc = x.shape
         out = self._new(x.shape)
-        check(self.lib.mv2_rmsnorm(_ptr(x), _ptr(out), _dt(self.dtype), _ptr(gamma), B, T, H * W, Cc,
-                                   int(token_shift), self._stream()), "mv2_rmsnorm")
+        prev = None if (ss is None or not token_shift) else ss.get("prev")
+        if prev is not None:
+            t, tl = prev
+            fe = t[0, 0].numel()
+            check(self.lib.mv2_rmsnorm_prev(_ptr(x), t.data_ptr() + tl * fe * t.element_size(), t.shape[1] * fe, _ptr(out),
+                                            _dt(self.dtype), _ptr(gamma), B, T, H * W, Cc, self._stream()), "mv2_rmsnorm_prev")
+        else:
+            check(self.lib.mv2_rmsnorm(_ptr(x), _ptr(out), _dt(self.dtype), _ptr(gamma), B, T, H * W, Cc,
+                                       int(token_shift), self._stream()), "mv2_rmsnorm")
+        if ss is not None and token_shift:
+            ss.put("prev", (x, T - 1))
         self.launches += 1
         return out
 
-    def feed_forward(self, x, p, token_shift=False):
+    def feed_forward(self, x, p, token_shift=False, ss: Optional[StreamState] = None):
         """Residual(FeedForward) (M:471-508, M:1191): x + fc2(geglu(fc1(rmsnorm(shift(x)))))."""
         B, T, H, W, Cc = x.shape
-        xn = self.rmsnorm(x, p["gamma"], token_shift)
+        xn = self.rmsnorm(x, p["gamma"], token_shift, ss)
         # fused fc1 + GEGLU pack is wgmma-only (K = C must be a multiple of 16); other widths take the unfused
         # CUDA-core convs + mv2_geglu below, like the fp32 path
         if self.dtype == torch.bfloat16 and self.use_tc and p["fc1"].epi_mode == 1 and Cc % 16 == 0:
@@ -526,16 +622,19 @@ class Engine:
         finally:
             self.use_tc = use
 
-    def attention(self, x, p, axis: str, dropout: Optional[_lib.DropoutArgs] = None):
+    def attention(self, x, p, axis: str, dropout: Optional[_lib.DropoutArgs] = None, ss: Optional[StreamState] = None):
         """Residual(SpaceAttention) / Residual(TokenShift(TimeAttention)) (M:444-464, M:1190, M:1235).  `dropout`: drop the
         softmax weights with that (seed, call, p) mask (Attend in training mode, A:175 / A:239)."""
         B, T, H, W, Cc = x.shape
         time_axis = axis == "time"
-        xn = self.rmsnorm(x, p["gamma"], token_shift=time_axis)
+        xn = self.rmsnorm(x, p["gamma"], token_shift=time_axis, ss=ss)
         qkv = self.conv(xn, p["qkv"])
         heads, dh = p["heads"], p["dim_head"]
         o = self._new((B, T, H, W, heads * dh))
         HW = H * W
+        if time_axis and ss is not None:
+            self._attention_tail(qkv, o, p, ss)
+            return self.conv(o, p["out"], res=x)
         if time_axis:
             a = AttnArgs(qkv=_ptr(qkv), out=_ptr(o), mem_kv=_ptr(p["mem_kv"]), dtype=_dt(self.dtype), heads=heads,
                          dim_head=dh, n_mem=p["n_mem"], causal=1, n_outer=B, n_inner=HW, L=T,
@@ -550,6 +649,32 @@ class Engine:
             check(self.lib.mv2_attention_dropout(C.byref(a), C.byref(dropout), self._stream()), "mv2_attention_dropout")
         self.launches += 1
         return self.conv(o, p["out"], res=x)
+
+    KV_CACHE_STEP = 16       # latent frames the time attention's K/V cache grows by
+
+    def _attention_tail(self, qkv, o, p, ss: StreamState):
+        """Time attention of a streamed chunk: the chunk's keys and values are appended to the stream's K/V cache (every
+        earlier frame's; it grows by KV_CACHE_STEP frames when full) and mv2_attention_tail computes the chunk's queries,
+        read from qkv, against all cached keys."""
+        B, T, H, W, C3 = qkv.shape
+        HW, HD = H * W, C3 // 3
+        cache = ss.get("kv")
+        L0 = 0 if cache is None else cache[1]
+        buf = None if cache is None else cache[0]
+        if buf is None or buf.shape[1] < L0 + T:
+            cap = _round_up(L0 + T, self.KV_CACHE_STEP)
+            nbuf = self._new((B, cap, H, W, 2 * HD))
+            if L0:
+                self.copy_frames(buf, 0, L0, dst=nbuf, dst_t0=0)
+            buf = nbuf
+        buf[:, L0:L0 + T].copy_(qkv[..., HD:])           # the '(kv h d)' two thirds of each '(qkv h d)' row
+        L = L0 + T
+        ss.put("kv", (buf, L))
+        a = AttnArgs(qkv=_ptr(buf), out=None, mem_kv=_ptr(p["mem_kv"]), dtype=_dt(self.dtype), heads=p["heads"],
+                     dim_head=p["dim_head"], n_mem=p["n_mem"], causal=1, n_outer=B, n_inner=HW, L=L,
+                     outer_stride=buf.shape[1] * HW, inner_stride=1, tok_stride=HW)
+        check(self.lib.mv2_attention_tail(C.byref(a), _ptr(qkv), T * HW, L0, _ptr(o), T * HW, self._stream()), "mv2_attention_tail")
+        self.launches += 1
 
     def attention_dropout_mask(self, n_seq, heads, L, n_mem, dropout: _lib.DropoutArgs):
         """The keep mask of an attention call, uint8 (n_seq, heads, L, n_mem + L) (mv2_attention_dropout_mask)."""
@@ -574,14 +699,22 @@ class Engine:
         self.launches += 2
         return self.conv(o, p["out"], res=x)
 
-    def gateloop(self, x, p):
+    def gateloop(self, x, p, ss: Optional[StreamState] = None):
         """ToTimeSequence(Residual(SimpleGateLoopLayer)) (M:178-191, M:1216-1222): RMSNorm, Linear(dim, 3 dim), then the gated
         recurrence over time per (pixel, channel) with the residual add fused (mv2_gateloop_scan)."""
         B, T, H, W, Cc = x.shape
         qkva = self.conv(self.rmsnorm(x, p["gamma"]), p["qkva"])
         out = self._new(x.shape)
-        check(self.lib.mv2_gateloop_scan(_ptr(qkva), _ptr(x), _ptr(out), _dt(self.dtype), B, T, H * W, Cc, self._stream()),
-              "mv2_gateloop_scan")
+        if ss is not None:            # the fp32 scan state s_{t-1} per (clip, pixel, channel) carries over to the next chunk
+            state = ss.get("s")
+            if state is None:
+                state = torch.zeros((B, H * W, Cc), device=self.device, dtype=torch.float32)
+                ss.put("s", state)
+            check(self.lib.mv2_gateloop_scan_state(_ptr(qkva), _ptr(x), _ptr(out), _dt(self.dtype), B, T, H * W, Cc, _ptr(state),
+                                                   self._stream()), "mv2_gateloop_scan_state")
+        else:
+            check(self.lib.mv2_gateloop_scan(_ptr(qkva), _ptr(x), _ptr(out), _dt(self.dtype), B, T, H * W, Cc, self._stream()),
+                  "mv2_gateloop_scan")
         self.launches += 1
         return out
 
@@ -609,14 +742,14 @@ class Engine:
         return out
 
     # ------------------------------------------------------------------ stages
-    def _stage(self, x, st, key, decoder: bool, cond_e=None):
+    def _stage(self, x, st, key, decoder: bool, cond_e=None, ss: Optional[StreamState] = None):
         P = self._packs
         B, T, H, W, Cc = x.shape
         if st.kind == "residual":
             for j in range(st.count):
-                x = self.residual_unit(x, P[f"{key}.{j}"])
+                x = self.residual_unit(x, P[f"{key}.{j}"], _sub(ss, str(j)))
         elif st.kind == "cond_residual":
-            x = self.residual_unit_mod(x, P[key], cond_e)
+            x = self.residual_unit_mod(x, P[key], cond_e, ss)
         elif st.kind == "compress_space":
             if decoder:   # SpatialUpsample2x (M:838-846)
                 x = self.conv(x, P[key], act=ACT_SILU, shuffle=SHUFFLE_SPACE)
@@ -627,17 +760,21 @@ class Engine:
             if decoder:   # TimeUpsample2x (M:875-883)
                 x = self.conv(x, P[key], act=ACT_SILU, shuffle=SHUFFLE_TIME)
             else:         # TimeDownsample2x (M:796-807): pad (2, 0), Conv1d k3 s2
-                x = self.conv(x, P[key], stride=(2, 1, 1), pad=(2, 0, 0), out_spatial=((T + 2 - 3) // 2 + 1, H, W))
+                x = self.conv(x, P[key], stride=(2, 1, 1), pad=(2, 0, 0), out_spatial=((T + 2 - 3) // 2 + 1, H, W), ss=ss)
         elif st.kind in ("attend_space", "attend_time"):
             time_axis = st.kind == "attend_time"
             drop = () if self.dropout is None else (self.dropout.take(),)      # without dropout: the plain call
-            x = self.attention(x, P[key + ".attn"], "time" if time_axis else "space", *drop)
-            x = self.feed_forward(x, P[key + ".ff"], token_shift=time_axis)
+            if time_axis and ss is not None:
+                x = self.attention(x, P[key + ".attn"], "time", ss=ss.sub("attn"))
+                x = self.feed_forward(x, P[key + ".ff"], token_shift=True, ss=ss.sub("ff"))
+            else:
+                x = self.attention(x, P[key + ".attn"], "time" if time_axis else "space", *drop)
+                x = self.feed_forward(x, P[key + ".ff"], token_shift=time_axis)
         elif st.kind == "linear_attend_space":
             x = self.linear_attention(x, P[key + ".attn"])
             x = self.feed_forward(x, P[key + ".ff"])
         elif st.kind == "gateloop_time":
-            x = self.gateloop(x, P[key])
+            x = self.gateloop(x, P[key], ss)
         else:
             raise ValueError(st.kind)
         return x
@@ -741,20 +878,27 @@ class Engine:
         return gx
 
     # ------------------------------------------------------------------ the path
-    def conv_in(self, video: torch.Tensor, first_frame: bool = True):
+    def conv_in(self, video: torch.Tensor, first_frame: bool = True, ss: Optional[StreamState] = None, sff_rest: bool = False):
         """video (B,C,T,H,W) on device -> conv_in's output (B,T+t_pad,H,W,C) channels-last.  The time_padding zero frames
-        are only prepended when the clip starts with a first frame (video_contains_first_frame, M:1534-1537)."""
+        are only prepended when the clip starts with a first frame (video_contains_first_frame, M:1534-1537).
+        sff_rest: a streamed chunk after the first frame of a separate_first_frame_encoding clip (the causal conv_in of
+        frames 1.., which the whole-clip call runs on channels-last frames)."""
         m = self.model
         t_pad = m.time_padding if first_frame else 0
         pin = self._packs.get("conv_in_tc")
-        if m.separate_first_frame_encoding and first_frame:
+        ss = _sub(ss, "conv_in")
+        if sff_rest:
+            x = self.conv(self.to_channels_last(video, 0), self._packs["conv_in"], ss=ss)
+        elif m.separate_first_frame_encoding and first_frame:
             # M:1553-1561: the first frame goes through its own 2-D conv, frames 1.. through the causal conv_in on their own,
             # then the feature map is [time_padding zero frames, first, rest]
             B, _, T, H, W = video.shape
             v_cl = self.to_channels_last(video, 0)
             parts = [(self.conv(self.copy_frames(v_cl, 0, 1), self._packs["conv_in_ff"]), t_pad)]
             if T > 1:
-                parts.append((self.causal_conv_padded(self.copy_frames(v_cl, 1, T - 1), self._packs["conv_in"], m.conv_in.pad_mode), t_pad + 1))
+                rest = self.copy_frames(v_cl, 1, T - 1)
+                parts.append((self.conv(rest, self._packs["conv_in"], ss=ss) if ss is not None else
+                              self.causal_conv_padded(rest, self._packs["conv_in"], m.conv_in.pad_mode), t_pad + 1))
             x = self._new((B, T + t_pad, H, W, parts[0][0].shape[-1]))
             for i, (part, t0) in enumerate(parts):
                 self.copy_frames(part, 0, part.shape[1], dst=x, dst_t0=t0, zero_front=(i == 0))
@@ -762,47 +906,55 @@ class Engine:
             x = self.causal_conv_padded(self.to_channels_last(video, t_pad), self._packs["conv_in"], m.conv_in.pad_mode)
         elif self.dtype == torch.bfloat16 and self.use_tc and pin is not None:
             x = self.ingest_kwpack(video, t_pad, pin)
-            x = self.conv(x, pin, pad=(pin.k_tc[0] - 1, pin.k_tc[1] // 2, 0))
+            x = self.conv(x, pin, pad=(pin.k_tc[0] - 1, pin.k_tc[1] // 2, 0), ss=ss)
         else:
             x = self.to_channels_last(video, t_pad)
-            x = self.conv(x, self._packs["conv_in"])
+            x = self.conv(x, self._packs["conv_in"], ss=ss)
         return x
 
-    def encode_cl(self, video: torch.Tensor, first_frame: bool = True, cond=None):
-        """video (B,C,T,H,W) on device -> encoder output, channels-last.  Reference encode M:1523-1576."""
+    def encode_cl(self, video: torch.Tensor, first_frame: bool = True, cond=None, ss: Optional[StreamState] = None,
+                  sff_rest: bool = False):
+        """video (B,C,T,H,W) on device -> encoder output, channels-last.  Reference encode M:1523-1576.  ss / sff_rest:
+        one chunk of a streamed clip (stream.TokenizeStream)."""
         m = self.model
-        x = self.conv_in(video, first_frame)
+        x = self.conv_in(video, first_frame, ss, sff_rest)
         self._tap("conv_in", x)
         cond_e = self.cond_stem(cond, "enc") if (m.has_cond and cond is not None) else None     # M:1544-1548
         for i, st in enumerate(m.stages):
-            x = self._stage(x, st, f"enc{i}", decoder=False, cond_e=cond_e)
+            x = self._stage(x, st, f"enc{i}", decoder=False, cond_e=cond_e, ss=_sub(ss, f"enc{i}"))
             self._tap(f"enc{i}", x)
         return x
 
-    def decode_cl(self, q: torch.Tensor, first_frame: bool = True, cond=None):
-        """quantized channels-last (B,T',H',W',C) -> video (B,3,T,H,W).  Reference decode M:1598-1649."""
+    def decode_cl(self, q: torch.Tensor, first_frame: bool = True, cond=None, ss: Optional[StreamState] = None,
+                  sff_rest: bool = False):
+        """quantized channels-last (B,T',H',W',C) -> video (B,3,T,H,W).  Reference decode M:1598-1649.  ss / sff_rest: one
+        chunk of a streamed clip (stream.DecodeStream)."""
         m = self.model
         x = q
         cond_e = self.cond_stem(cond, "dec") if (m.has_cond and cond is not None) else None     # M:1612-1616
         for j, st in enumerate(reversed(m.stages)):
-            x = self._stage(x, st, f"dec{j}", decoder=True, cond_e=cond_e)
+            x = self._stage(x, st, f"dec{j}", decoder=True, cond_e=cond_e, ss=_sub(ss, f"dec{j}"))
             self._tap(f"dec{j}", x)
-        return self.conv_out(x, first_frame)
+        return self.conv_out(x, first_frame, ss, sff_rest)
 
-    def conv_out(self, x: torch.Tensor, first_frame: bool = True):
+    def conv_out(self, x: torch.Tensor, first_frame: bool = True, ss: Optional[StreamState] = None, sff_rest: bool = False):
         """decoder output (B,T,H,W,C) channels-last -> reconstruction (B,3,T-t_pad,H,W).  The leading time_padding frames
-        are dropped only for clips that contain a first frame (M:1646-1647)."""
+        are dropped only for clips that contain a first frame (M:1646-1647).  sff_rest as in conv_in."""
         m = self.model
         pk = self._packs["conv_out"]
         B, T, H, W, Cc = x.shape
         tp = m.time_padding if first_frame else 0
+        ss = _sub(ss, "conv_out")
+        if sff_rest:
+            return self.to_channels_first(self.conv(x, pk, ss=ss))
         if m.separate_first_frame_encoding and first_frame:
             # M:1633-1639: conv_out_first_frame on frame `tp`, the causal conv_out on the frames after it, re-attached
             first = self.conv(self.copy_frames(x, tp, 1), self._packs["conv_out_ff"])
             out = self._new((B, T - tp, H, W, first.shape[-1]))
             self.copy_frames(first, 0, 1, dst=out, dst_t0=0)
             if T - tp > 1:
-                rest = self.causal_conv_padded(self.copy_frames(x, tp + 1, T - tp - 1), pk, m.conv_out.pad_mode)
+                rest = self.copy_frames(x, tp + 1, T - tp - 1)
+                rest = self.conv(rest, pk, ss=ss) if ss is not None else self.causal_conv_padded(rest, pk, m.conv_out.pad_mode)
                 self.copy_frames(rest, 0, T - tp - 1, dst=out, dst_t0=1)
             return self.to_channels_first(out)
         if m.conv_out.pad_mode != "constant":
@@ -811,8 +963,9 @@ class Engine:
                 and Cc % 64 == 0 and pk.k[2] <= 3 and T > tp):
             # conv_out writes the reconstruction in torch's (B,C,T,H,W) layout itself and never computes the time_padding
             # frames the reference drops afterwards (M:1642-1647)
-            return self.conv(x, pk, pad=(pk.k[0] - 1 - tp, pk.k[1] // 2, pk.k[2] // 2), out_spatial=(T - tp, H, W), out_cf=True)
-        x = self.conv(x, pk)
+            return self.conv(x, pk, pad=(pk.k[0] - 1 - tp, pk.k[1] // 2, pk.k[2] // 2), out_spatial=(T - tp, H, W), out_cf=True,
+                             ss=ss)
+        x = self.conv(x, pk, ss=ss)
         return self.to_channels_first(x, t_crop=tp)
 
     def quantize_cl(self, x, want_quantized=True, want_aux=False):

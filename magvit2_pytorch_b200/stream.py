@@ -1,0 +1,124 @@
+"""Streaming tokenize and decode: a clip fed in chunks gives exactly the codes and frames of one whole-clip call.
+
+The tokenizer is causal in time end to end (causal convs, TimeDownsample2x's window [2j-2, 2j], pointwise TimeUpsample2x,
+right-aligned causal time attention with TokenShift, the gateloop forward scan), so chunk k's outputs depend only on frames up
+to its own.  A stream carries what the next chunk needs from the earlier ones (engine.StreamState): per causal conv its last
+k_t - 1 input frames, per token shift the previous frame, per time attention the qkv rows of every earlier frame, per
+gateloop the fp32 scan state.  The kernels read that state in place (DESIGN.md 3.7).
+
+    enc = tok.tokenize_stream(batch_size=B)
+    codes = torch.cat([enc.push(chunk) for chunk in chunks], dim=1)      # == tok.tokenize(video)
+    dec = tok.decode_stream(batch_size=B)
+    video = torch.cat([dec.push(c) for c in codes.split(1, dim=1)], dim=2)   # == tok.decode_from_code_indices(codes)
+"""
+from __future__ import annotations
+
+import torch
+
+from .engine import StreamState
+
+
+def check_stream_model(model):
+    """Construction-time checks shared by both streams (no device needed)."""
+    for name in ("conv_in", "conv_out"):
+        mode = getattr(model, name).pad_mode
+        if mode != "constant":
+            raise NotImplementedError(
+                f"streaming needs pad_mode='constant' ({name} has '{mode}'): the other modes pad with the whole clip's "
+                "leading frames, and only when the clip is longer than the padding, which a stream cannot know")
+
+
+def encoder_chunk_frames(n: int, tdf: int, first_push: bool, first_frame: bool) -> int:
+    """Latent frames an encoder push of n frames yields; ValueError names the chunk rule when n breaks it."""
+    if first_push and first_frame:
+        if n < 1 or (n - 1) % tdf:
+            raise ValueError(f"the first push of a stream with a first frame takes 1 + k * {tdf} frames (k >= 0), got {n}")
+        return (n - 1) // tdf + 1
+    if n < tdf or n % tdf:
+        what = "every later push" if first_frame else "every push of a stream without a first frame"
+        raise ValueError(f"{what} takes k * {tdf} frames (k >= 1, the time downsample factor {tdf}), got {n}")
+    return n // tdf
+
+
+def decoder_chunk_frames(n: int, tdf: int, first_push: bool, first_frame: bool) -> int:
+    """Frames a decoder push of n latent frames yields; ValueError when n < 1."""
+    if n < 1:
+        raise ValueError(f"a decoder push takes at least one latent frame, got {n}")
+    return tdf * n - (tdf - 1 if first_push and first_frame else 0)
+
+
+class _Stream:
+    def __init__(self, model, batch_size, cond, video_contains_first_frame):
+        check_stream_model(model)
+        if int(batch_size) < 1:
+            raise ValueError(f"batch_size must be >= 1, got {batch_size}")
+        self.model = model
+        self.batch_size = int(batch_size)
+        self.first_frame = bool(video_contains_first_frame)
+        self.cond = model._check_cond(cond, self.batch_size)
+        self.state = StreamState()
+        self.pushes = 0
+        self._sig_id = None
+
+    def _engine(self):
+        """The model's engine, eval mode, checked against the parameter packs this stream started with."""
+        self.model.eval()
+        eng = self.model.engine
+        if self._sig_id is None:
+            self._sig_id = eng._sig_id
+        elif eng._sig_id != self._sig_id:
+            raise RuntimeError("the tokenizer's parameters changed while this stream was open: its carried state belongs "
+                               "to the old ones; start a new stream")
+        return eng
+
+    def _check_batch(self, t, what):
+        if t.shape[0] != self.batch_size:
+            raise ValueError(f"{what} has batch {t.shape[0]}, the stream was built for batch_size={self.batch_size}")
+        self.model._check_on_device(t, what)
+
+
+class TokenizeStream(_Stream):
+    """Encoder + quantiser of a clip fed in chunks; see push()."""
+
+    @torch.no_grad()
+    def push(self, chunk: torch.Tensor) -> torch.Tensor:
+        """chunk (B, C, n, H, W) float / bf16 / uint8 frames -> codes (B, n', H', W'[, num_codebooks]) of those frames:
+        n' = n // tdf, plus 1 on the first push of a stream with a first frame (which takes 1 + k * tdf frames)."""
+        m = self.model
+        if chunk.ndim != 5 or chunk.shape[1] != m.channels or tuple(chunk.shape[-2:]) != (m.image_size, m.image_size):
+            raise ValueError(f"chunk must be (B, {m.channels}, n, {m.image_size}, {m.image_size}), got {tuple(chunk.shape)}")
+        self._check_batch(chunk, "chunk")
+        first = self.pushes == 0
+        encoder_chunk_frames(chunk.shape[2], m.time_downsample_factor, first, self.first_frame)
+        with torch.cuda.device(m.device):
+            eng = self._engine()
+            x = eng.encode_cl(chunk.contiguous(), self.first_frame and first, self.cond, ss=self.state,
+                              sff_rest=self.first_frame and not first and m.separate_first_frame_encoding)
+            _, codes, _ = eng.quantize_cl(x, want_quantized=False)
+        self.pushes += 1
+        return codes
+
+
+class DecodeStream(_Stream):
+    """Decoder of latent codes fed in chunks; see push()."""
+
+    @torch.no_grad()
+    def push(self, codes: torch.Tensor) -> torch.Tensor:
+        """codes (B, n', H', W'[, num_codebooks]) int64 / int32 -> frames (B, C, tdf * n', H, W) in the model dtype, less the
+        time_padding frames on the first push of a stream with a first frame."""
+        m = self.model
+        nc = m.quantizers.num_codebooks
+        if codes.dtype not in (torch.long, torch.int32) or codes.ndim != (4 if nc == 1 else 5) or \
+                (nc > 1 and codes.shape[-1] != nc):
+            raise ValueError(f"codes must be int64 / int32 (B, n, H, W{'' if nc == 1 else ', num_codebooks'}), "
+                             f"got {codes.dtype} {tuple(codes.shape)}")
+        self._check_batch(codes, "codes")
+        first = self.pushes == 0
+        decoder_chunk_frames(codes.shape[1], m.time_downsample_factor, first, self.first_frame)
+        with torch.cuda.device(m.device):
+            eng = self._engine()
+            q = eng.codes_to_quantized_cl(codes)
+            out = eng.decode_cl(q, self.first_frame and first, self.cond, ss=self.state,
+                                sff_rest=self.first_frame and not first and m.separate_first_frame_encoding)
+        self.pushes += 1
+        return out

@@ -603,6 +603,16 @@ class VideoTokenizer(nn.Module):
         self.quantizer_aux_loss = aux
         return (codes, recon) if need_recon else codes
 
+    def tokenize_stream(self, batch_size, cond=None, video_contains_first_frame=True):
+        """A stream.TokenizeStream: push() chunks of a clip batch, get the codes one tokenize of the whole clip gives."""
+        from .stream import TokenizeStream
+        return TokenizeStream(self, batch_size, cond, video_contains_first_frame)
+
+    def decode_stream(self, batch_size, cond=None, video_contains_first_frame=True):
+        """A stream.DecodeStream: push() latent frames, get the frames one decode_from_code_indices of all of them gives."""
+        from .stream import DecodeStream
+        return DecodeStream(self, batch_size, cond, video_contains_first_frame)
+
     @torch.no_grad()
     def tokenize(self, video):
         """M:1651-1654."""
