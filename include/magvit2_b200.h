@@ -294,7 +294,10 @@ typedef struct mv2_tc_conv_args {
   int32_t out_layout;  /* 0: y is channels-last (B,To,Ho,Wo,Co).  1: y is torch's channels-first (B,Co,To,Ho,Wo) -- the slab
                           kernel's conv_out (Co % 8 != 0) writes the reconstruction directly in the caller's layout; with
                           To < Ti and pt = kt - 1 - (Ti - To) the leading time_padding frames are never computed
-                          (reference M:1642-1647: conv_out, then video[:, :, time_padding:]).                            */
+                          (reference M:1642-1647: conv_out, then video[:, :, time_padding:]).  pt = -(Ti - To) is the
+                          data gradient of a causal conv (the transposed conv, no leading pad) without its first Ti - To
+                          frames: the video's gradient through conv_in; with Co <= 16 and kw > 3 (up to 7) it runs on
+                          8- / 16-column N tiles.                                                                        */
 } mv2_tc_conv_args;
 int mv2_tc_conv_supported(const mv2_tc_conv_args* a);
 int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream);

@@ -67,6 +67,20 @@ template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wg
 template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_bf16<8>(float (&d)[4], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
 template <> __device__ __forceinline__ void wgmma_bf16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
@@ -146,7 +160,8 @@ struct TcEpi {
                                  // 2 scaled residual: (act(acc + bias) + res) * 2^-0.5 (DiscriminatorBlock, M:585)
   int Co;                        // packed GEMM output columns
   int To, Ho, Wo;                // output volume before any depth-to-space/time shuffle
-  int out_cf;                    // 1: y is channels-first (B, Co, To, Ho, Wo) -- EPI_RAGGED scalar stores only (conv_out)
+  int out_cf;                    // 1: y is channels-first (B, Co, To, Ho, Wo) -- EPI_RAGGED scalar stores only (conv_out,
+                                 // the video's data gradient)
   const float* oscale;           // [B][Co] or null: accumulator multiplier per (clip, output channel) before bias / activation
 };
 

@@ -18,6 +18,9 @@
 //     128-column divisor take 128-column tiles with a ragged last one;
 //   * the kernel is instantiated per epilogue flavour (tc_common.cuh: EPI_*) and N tile (32 / 64 / 128); the plain
 //     flavour transposes each 32 x 32 chunk through shared memory so stores / residual loads are 64-byte contiguous per row.
+//     The channels-first flavour (EPI_RAGGED: fewer than 32 output channels, so never a wider tile than 32) has narrow
+//     8- and 16-column tiles (wgmma m64n8k16 / m64n16k16) instead, for the data gradient of conv_in with respect to the
+//     video: 3 output channels, 7 x 7 in-plane taps (slab_narrow).
 // Warp roles (384 threads): w0 slab TMA producer, w2 weight TMA producer (40 registers each, setmaxnreg), w4-7 / w8-11
 // two consumer warpgroups (232 registers): each issues the wgmma of 64 of the 128 positions of every M-tile, with one
 // commit group in flight across ring stages, stages its accumulators in shared memory and runs the epilogue on them
@@ -123,7 +126,7 @@ __host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& 
 constexpr int SLAB_PRODUCER_REGS = 40, SLAB_CONSUMER_REGS = 232;
 template <int MODE, int BN>
 __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__ SlabParams p) {
-  constexpr int MWMAX = 128 / BN;
+  constexpr int MWMAX = BN >= 32 ? 128 / BN : 4;        // mw <= 4 (slab_default_mw)
   constexpr int KC1 = BN >= 64 ? BN / 64 : 1;   // EPI_FUSED_RU (bn = C = 64 | 128): 64-channel K-chunks of the 1x1x1 GEMM
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -651,7 +654,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
         } else {
           for (int c0 = ((j + half) & 1) * 32; c0 < p.bn; c0 += 64) {
             uint32_t r[32];
-            load_row32(srow + c0, 32, r);
+            load_row32(srow + c0, BN < 32 ? BN : 32, r);     // a narrow tile's staged rows hold BN + 4 floats
             if (row_ok) epi_chunk32<MODE>(p.epi, r, min(32, p.bn - c0), c.n0 + c0, sbias + c.n0 + c0, c.b, c.t, h, w, row_base);
           }
         }
@@ -663,6 +666,11 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
 }  // namespace mv2
 
 using namespace mv2;
+
+// Channels-first outputs of at most 16 channels whose in-plane taps are wider than 3 -- the data gradient of a 7 x 7 x 7
+// conv_in (or its 1 x 7 x 7 first-frame conv) with respect to the video -- run on the narrow N tiles (8 / 16 columns):
+// a 32-column tile would spend 29 of every 32 MMA columns and weight rows on padding.
+static bool slab_narrow(const mv2_tc_conv_args* a) { return a->out_layout == 1 && a->Co <= 16 && a->kw > 3; }
 
 extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
   if (!a) return 0;
@@ -680,11 +688,14 @@ extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
   if (a->Ci % 64 != 0 && a->kw != 1) return 0;           // 64-byte rows (32 channels): only h-shifted taps (1024 B multiples)
   if (a->res && a->Co % 8 != 0) return 0;
   if (a->shuffle != MV2_SHUFFLE_NONE && ((a->shuffle == MV2_SHUFFLE_SPACE ? a->Co / 4 : a->Co / 2) % 8 != 0 || a->Co % 32 != 0)) return 0;
-  if (a->kh > 7 || a->kw > 3 || a->kt > 8) return 0;
+  if (a->kh > 7 || a->kw > (slab_narrow(a) ? 7 : 3) || a->kt > 8) return 0;
   if (a->Ho != a->Hi || a->Wo != a->Wi) return 0;
-  if (a->out_layout == 1) {   // channels-first output: the ragged scalar-store epilogue only (conv_out); may drop leading frames
+  if (a->out_layout == 1) {   // channels-first output: the ragged scalar-store epilogue only; may drop leading frames
     if (a->Co % 8 == 0 || a->res || a->shuffle != MV2_SHUFFLE_NONE || a->epi_mode != 0) return 0;
-    if (a->To > a->Ti || a->To < 1 || a->pt != a->kt - 1 - (a->Ti - a->To)) return 0;
+    if (a->To > a->Ti || a->To < 1) return 0;
+    // conv_out (causal, the first Ti - To output frames not computed) or the data gradient of a causal conv (the transposed
+    // conv: no leading pad, output frame t reads input frames t + Ti - To ..; the first Ti - To frames not computed)
+    if (a->pt != a->kt - 1 - (a->Ti - a->To) && a->pt != -(a->Ti - a->To)) return 0;
   } else if (a->out_layout != 0 || (a->st == 1 && a->To != a->Ti)) return 0;
   return 1;
 }
@@ -703,7 +714,7 @@ static size_t slab_smem_bytes(const SlabParams& p, bool fused) {
 }
 // M-tiles side by side per weight tile: as many as the frame width uses, while their accumulators fit 64 fp32 registers
 // per consumer thread (mw * bn <= 128); this divides the weight traffic by mw
-static int slab_default_mw(int bn, int Wo) { return bn == 32 && Wo > 16 ? 4 : (bn <= 64 && Wo > 8 ? 2 : 1); }
+static int slab_default_mw(int bn, int Wo) { return bn <= 32 && Wo > 16 ? 4 : (bn <= 64 && Wo > 8 ? 2 : 1); }
 // Slab geometry of a macro tile of mw M-tiles: slab row pitch, bytes of one slab (slab_h rows) and its 1024-byte aligned
 // ring stride, tile counts.  Needs kw, slab_h, row_bytes, B, T, W, tiles_h and n_tiles_n.
 static void slab_set_geometry(SlabParams& p, int mw) {
@@ -737,8 +748,9 @@ static int slab_fill_plan(const mv2_tc_conv_args* a, SlabParams& p) {
   const bool ragged_ok = a->epi_mode == 0 && a->shuffle == MV2_SHUFFLE_NONE && a->Co % 8 == 0;
   if ((ragged_ok || a->epi_mode == 1) && best_bn <= 64 && co_pad >= 512 && (co_pad + 127) / 128 * 128 * 100 <= co_pad * 108)
     best_bn = 128;
-  p.bn = best_bn;
-  p.n_tiles_n = (co_pad + p.bn - 1) / p.bn;   // a ragged last tile reads zero-filled weight rows and stores nothing for them
+  p.bn = slab_narrow(a) ? (a->Co <= 8 ? 8 : 16) : best_bn;
+  // a ragged last tile reads zero-filled weight rows and stores nothing for them; a narrow tile covers all of Co (<= bn)
+  p.n_tiles_n = slab_narrow(a) ? 1 : (co_pad + p.bn - 1) / p.bn;
   p.tiles_h = ceil_div(a->Ho, 16);
   p.slab_h = 16 + a->kh - 1;
   int budget;
@@ -792,10 +804,12 @@ static int slab_encode_maps(SlabParams& p, const mv2_tc_conv_args* a, const mv2_
 
 // Launches one slab-kernel flavour: persistent CTAs, one per SM of the current device (fewer when there are fewer tiles)
 static int slab_launch(int mode, const SlabParams& p, void* stream) {
-  // kernel instance per (epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared memory
+  // kernel instance per (epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared memory.  The
+  // channels-first flavour EPI_RAGGED (< 32 channels) has the 32-column tile and the narrow 16- and 8-column ones.
 #define MV2_SLAB_BN(M) {tc_slab_kernel<M, 32>, tc_slab_kernel<M, 64>, tc_slab_kernel<M, 128>}
   static void (*const kernels[8][3])(SlabParams) = {
-      MV2_SLAB_BN(EPI_PLAIN), MV2_SLAB_BN(EPI_GEGLU), MV2_SLAB_BN(EPI_SHUFFLE), MV2_SLAB_BN(EPI_RAGGED),
+      MV2_SLAB_BN(EPI_PLAIN), MV2_SLAB_BN(EPI_GEGLU), MV2_SLAB_BN(EPI_SHUFFLE),
+      {tc_slab_kernel<EPI_RAGGED, 32>, tc_slab_kernel<EPI_RAGGED, 16>, tc_slab_kernel<EPI_RAGGED, 8>},
       MV2_SLAB_BN(EPI_PLAIN_RES), MV2_SLAB_BN(EPI_FUSED_RU), MV2_SLAB_BN(EPI_SHUFFLE_ST), MV2_SLAB_BN(EPI_DOWN_SPACE)};
 #undef MV2_SLAB_BN
   static PerDeviceOnce attr_once;
@@ -812,7 +826,9 @@ static int slab_launch(int mode, const SlabParams& p, void* stream) {
   int dev = 0, n_sm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
-  launch_k(kernels[mode][p.bn == 32 ? 0 : (p.bn == 64 ? 1 : 2)], dim3(std::min(p.total_tiles, n_sm)), dim3(384), smem,
+  MV2_CHECK_ARG(p.bn >= 32 || mode == EPI_RAGGED);
+  const int slot = p.bn == 32 ? 0 : (p.bn == 64 || p.bn == 16 ? 1 : 2);
+  launch_k(kernels[mode][slot], dim3(std::min(p.total_tiles, n_sm)), dim3(384), smem,
            (cudaStream_t)stream, p);
   MV2_CHECK_LAUNCH();
   return MV2_OK;

@@ -384,8 +384,7 @@ class Engine:
         k_t - 1 input frames are kept for the next chunk."""
         B, Ti, Hi, Wi, Ci = x.shape
         hist, advance = self._conv_hist(ss, x, pk.k[0] - 1)
-        tc_ok = (self.dtype == torch.bfloat16 and self.use_tc and pk.w_tc is not None and not token_shift
-                 and Ci == pk.Ci_tc)
+        tc_ok = self._tc_ok(x, pk) and not token_shift
         kt, kh, kw = pk.k_tc if (tc_ok and pk.k_tc) else pk.k
         if pad is None:
             pad = (kt - 1, kh // 2, kw // 2)
@@ -405,11 +404,7 @@ class Engine:
                 y = self._new((B, To, Ho, Wo, co_out))
             if res is not None:
                 assert res.shape == y.shape and res.dtype == y.dtype and res.is_contiguous()
-            ta = TcConvArgs(x=_ptr(x), w=_ptr(pk.w_tc), bias=_ptr(pk.bias_tc), res=_ptr(res), y=_ptr(y),
-                            B=B, Ti=Ti, Hi=Hi, Wi=Wi, Ci=Ci, To=To, Ho=Ho, Wo=Wo, Co=co_gemm,
-                            kt=kt, kh=kh, kw=kw, st=stride[0], sh=stride[1], sw=stride[2],
-                            pt=pad[0], ph=pad[1], pw=pad[2], act=act, shuffle=shuffle, epi_mode=pk.epi_mode,
-                            oscale=_ptr(oscale), out_layout=int(out_cf))
+            ta = self._tc_args(x, pk, stride, pad, out_spatial, act, shuffle, out_cf, res=res, y=y, oscale=oscale)
             # policy: the persistent slab kernel reuses each activation slab for all in-plane taps, so it takes every layer it
             # supports (incl. the 64-byte-row conv_in); the tap-wise kernel keeps the strided down-samplers.  tc_variant = "tap" forces the tap-wise kernel (tests / sweeps).
             use_slab = self.tc_variant != "tap" and bool(self.lib.mv2_tc_slab_supported(C.byref(ta)))
@@ -488,6 +483,29 @@ class Engine:
                   "mv2_scale_channels")
             self.launches += 1
         return y
+
+    def _tc_ok(self, x, pk: ConvPack) -> bool:
+        """Whether conv(x, pk) may run on the wgmma kernels: bf16 with a wgmma weight pack for x's channel count."""
+        return self.dtype == torch.bfloat16 and self.use_tc and pk.w_tc is not None and x.shape[-1] == pk.Ci_tc
+
+    def _tc_args(self, x, pk: ConvPack, stride, pad, out_spatial, act, shuffle, out_cf, res=None, y=None, oscale=None):
+        """The mv2_tc_conv_args of conv(x, pk, ...) on the wgmma kernels."""
+        B, Ti, Hi, Wi, Ci = x.shape
+        kt, kh, kw = pk.k_tc or pk.k
+        To, Ho, Wo = out_spatial
+        return TcConvArgs(x=_ptr(x), w=_ptr(pk.w_tc), bias=_ptr(pk.bias_tc), res=_ptr(res), y=_ptr(y),
+                          B=B, Ti=Ti, Hi=Hi, Wi=Wi, Ci=Ci, To=To, Ho=Ho, Wo=Wo, Co=pk.Co_tc,
+                          kt=kt, kh=kh, kw=kw, st=stride[0], sh=stride[1], sw=stride[2],
+                          pt=pad[0], ph=pad[1], pw=pad[2], act=act, shuffle=shuffle, epi_mode=pk.epi_mode,
+                          oscale=_ptr(oscale), out_layout=int(out_cf))
+
+    def conv_cf_supported(self, x, pk: ConvPack, pad, out_spatial) -> bool:
+        """True when conv(x, pk, pad=pad, out_spatial=out_spatial, out_cf=True) runs: bf16 on the slab kernel, whose
+        channels-first epilogue takes fewer than 8 (or a ragged number of) output channels."""
+        if not (self._tc_ok(x, pk) and self.tc_variant != "tap" and pk.Co % 8 != 0):
+            return False
+        ta = self._tc_args(x, pk, (1, 1, 1), pad, out_spatial, ACT_NONE, SHUFFLE_NONE, True)
+        return bool(self.lib.mv2_tc_slab_supported(C.byref(ta)))
 
     def residual_unit(self, x, p, ss: Optional[StreamState] = None):
         """ResidualUnit (reference M:930-944): x + SE(ELU(conv1(ELU(causal_conv3(x)))))."""

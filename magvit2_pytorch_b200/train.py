@@ -14,7 +14,12 @@ Division of labour
     FeedForward blocks, the two up-samplers, the quantiser with its straight-through estimator and auxiliary losses) are
     differentiated by re-evaluating a torch restatement of the block on its saved input (``_vjp``).
   There are no dedicated backward kernels (wgrad, attention backward) yet; this slice makes the drop-in claim true for the trainer's generator step,
-  it is not a speed claim for training.  Gradients are checked against the unmodified reference's autograd on the `mini`
+  it is not a speed claim for training.
+The forward is built from three pieces that each record their tape entries -- encoder (conv_in + stages), quantiser, decoder
+(stages + conv_out) -- which the training step chains whole and the differentiable encode / decode / decode_from_code_indices
+entry points chain in part (DESIGN.md 3.8), all under one autograd.Function (_TapeFn).  Those entry points also need the
+gradient wrt their inputs: the cond vector (through the cond stems) and the video, whose data gradient through conv_in runs on
+the slab kernel's narrow N tile in bf16 and on the CUDA-core conv in fp32 (_video_dgrad).  Gradients are checked against the unmodified reference's autograd on the `mini`
   config (tests/golden/mini_train.pt, tests/test_train_gpu.py).
 
 Reference lines: M: = magvit2_pytorch/magvit2_pytorch.py, A: = attend.py.
@@ -182,11 +187,8 @@ def _entropy(p, eps=1e-5):
     return (-p * torch.log(p.clamp(min=eps))).sum(dim=-1)
 
 
-def _lfq_train(x, qz, avg_global, inv_temperature=100.):
-    """LFQ training forward (SURVEY Appendix A.1 steps 2-10) on (B,T,H,W,C): -> (straight-through quantised output, aux loss).
-    `avg_global` is the cross-rank mean code probability of the forward pass; the local term enters as
-    avg_local + (avg_global - avg_local).detach(), which reproduces the gradient of the reference's autograd-aware
-    all-reduce (each rank back-propagates d H / d avg_global into its own tokens)."""
+def _lfq_project(x, qz):
+    """LFQ's pre-sign values (SURVEY Appendix A.1 steps 2-4) on (B,T,H,W,C): project_in, soft clamp, [spherical] -> fp32 (N, nc, d)."""
     d, nc = qz.codebook_dim, qz.num_codebooks
     p = F.linear(x, qz.project_in.weight, qz.project_in.bias)
     cv = qz.soft_clamp_input_value
@@ -195,7 +197,46 @@ def _lfq_train(x, qz, avg_global, inv_temperature=100.):
     p = p.reshape(-1, nc, d)
     if qz.spherical:
         p = F.normalize(p, dim=-1)
-    p = p.float()
+    return p.float()
+
+
+def _lfq_quantize(x, qz, straight_through):
+    """LFQ's quantised output without the auxiliary loss (the first element of encode(quantize=True)): project_out of the
+    signs, with the straight-through estimator x + (q - x).detach() in train mode (A.1 step 6); in eval mode the signs are a
+    constant of the input, so only project_out gets a gradient."""
+    p = _lfq_project(x, qz)
+    qd = torch.where(p > 0, torch.ones_like(p), -torch.ones_like(p))
+    st = p + (qd - p).detach() if straight_through else qd.detach()
+    return F.linear(st.reshape(*x.shape[:-1], -1).to(x.dtype), qz.project_out.weight, qz.project_out.bias)
+
+
+def _project_out(codes, qz, dtype):
+    """indices_to_codes' projection (M:1593): project_out of the code values (B,T,H,W, nc * d) -- the only parameters
+    decode_from_code_indices reaches in the quantiser."""
+    return F.linear(codes.to(dtype), qz.project_out.weight, qz.project_out.bias)
+
+
+def _code_values(codes, qz, fsq):
+    """Code values (B,T,H,W, nc * d) fp32 of indices (B,T,H,W[,nc]): LFQ's +-1 bits, FSQ's (level - half width) / half width
+    (indices_to_codes, A.1 / A.2)."""
+    ind = codes.long().reshape(*codes.shape[:4], -1)[..., None]                   # (B,T,H,W,nc,1)
+    if fsq:
+        lv = torch.tensor(qz.levels, device=codes.device, dtype=torch.long)
+        basis = torch.cumprod(torch.cat((lv.new_ones(1), lv[:-1])), dim=0)
+        half = lv // 2
+        vals = ((ind // basis) % lv - half).float() / half.float()
+    else:
+        vals = ((ind & qz.mask.to(codes.device).long()) != 0).float() * 2 - 1
+    return vals.reshape(*codes.shape[:4], -1)
+
+
+def _lfq_train(x, qz, avg_global, inv_temperature=100.):
+    """LFQ training forward (SURVEY Appendix A.1 steps 2-10) on (B,T,H,W,C): -> (straight-through quantised output, aux loss).
+    `avg_global` is the cross-rank mean code probability of the forward pass; the local term enters as
+    avg_local + (avg_global - avg_local).detach(), which reproduces the gradient of the reference's autograd-aware
+    all-reduce (each rank back-propagates d H / d avg_global into its own tokens)."""
+    d, nc = qz.codebook_dim, qz.num_codebooks
+    p = _lfq_project(x, qz)
     qd = torch.where(p > 0, torch.ones_like(p), -torch.ones_like(p))
     st = (p + (qd - p).detach()).reshape(*x.shape[:-1], nc * d)
     out = F.linear(st.to(x.dtype), qz.project_out.weight, qz.project_out.bias)
@@ -278,6 +319,14 @@ def _elu_grad(g, y):
     return g * torch.where(y > 0, torch.ones_like(y), y + 1)
 
 
+def transposed_pack(weight, k, dtype):
+    """The weight pack of a stride-1 conv's data gradient: weight (Co, Ci, *k) flipped in (t, h, w) and transposed in
+    (co, ci), so that the transposed conv is the same implicit GEMM on the engine's conv kernels."""
+    kt, kh, kw = k
+    wt = weight.detach().reshape(weight.shape[0], -1, kt, kh, kw).flip(2, 3, 4).transpose(0, 1).contiguous()
+    return pack_conv(wt, None, dtype)
+
+
 class TapeRunner:
     """A forward through the engine's kernels that records its backward on a tape, with the gradient pieces shared by the
     generator's runner (TrainRunner) and the discriminator's (gan.DiscrRunner)."""
@@ -319,9 +368,8 @@ class TapeRunner:
         leading pad in time (gx[t] = sum_e W'[e] g[t + e]; frames past the clip are the kernels' out-of-bounds zeros).
         g: (B,To,Ho,Wo,Co) channels-last; returns (B,*out_spatial,Ci) channels-last."""
         kt, kh, kw = k
-        wt = weight.detach().reshape(weight.shape[0], -1, kt, kh, kw).flip(2, 3, 4).transpose(0, 1).contiguous()
         self.own_dgrad_calls += 1
-        return self.eng.conv(g.contiguous(), pack_conv(wt, None, self.eng.dtype), pad=(0, kh // 2, kw // 2),
+        return self.eng.conv(g.contiguous(), transposed_pack(weight, k, self.eng.dtype), pad=(0, kh // 2, kw // 2),
                              out_spatial=tuple(out_spatial))
 
     def _wgrad(self, g, x_cf, weight, bias, k, stride, pad, need_gx=False):
@@ -486,67 +534,155 @@ class TrainRunner(TapeRunner):
                                lambda t: _feed_forward_block(t, ff, time_axis), list(ff.parameters()))
         raise NotImplementedError(f"no training path for layer type {st.kind!r}")
 
-    def forward(self, video, first_frame=True, group=None, cond=None):
-        """-> (recon (B,C,T,H,W), aux_loss 0-d fp32); codes / the LFQ breakdown are left in .codes / .breakdown."""
-        from .dist import LfqBatchEntropy
+    # ---- the three pieces of a forward (encoder, quantiser, decoder); each records its backward on the tape.  The training
+    #      forward chains all three, the differentiable encode / decode entry points (run_encode, run_decode, run_decode_codes)
+    #      one or two of them
+    def encoder_piece(self, video, first_frame=True, cond=None, need_gvideo=False):
+        """conv_in + the encoder stages (M:1523-1565): video (B,C,T,H,W) -> encoder output, channels-last.  need_gvideo: the
+        backward also returns the video's gradient (B,C,T,H,W) (_conv_in_bwd)."""
         m, eng = self.m, self.eng
         self.cond = cond
-        ce_enc = eng.cond_stem(cond, "enc") if m.has_cond else None            # M:1544-1548 (Linear + SiLU stems)
-        ce_dec = eng.cond_stem(cond, "dec") if m.has_cond else None            # M:1612-1616
+        ce = eng.cond_stem(cond, "enc") if m.has_cond else None            # M:1544-1548 (Linear + SiLU stem)
+        x = eng.conv_in(video, first_frame)
+        self.tape.append(self._conv_in_bwd(video, first_frame, need_gvideo))
+        for i, st in enumerate(m.stages):
+            x = self._stage(x, st, f"enc{i}", m.encoder_layers[i], decoder=False, cond_e=ce)
+        return x
+
+    def _conv_in_bwd(self, vid, first_frame, need_gvideo):
+        """conv_in's tape entry: weight / bias gradients of conv_in [and conv_in_first_frame], and with need_gvideo the gradient
+        wrt the video (B,C,T,H,W), without the time_padding frames the reference prepends as constants (M:1534-1537).  The
+        video's data gradient runs on the engine's conv kernels (_video_dgrad) except in the non-constant pad modes, where it
+        is folded back through F.pad like the other padded convs (_conv_bwd_padmode)."""
+        m, eng = self.m, self.eng
         t_pad = m.time_padding if first_frame else 0
-        cin, cout = m.conv_in.conv, m.conv_out.conv
+        cin = m.conv_in.conv
         kin = tuple(cin.weight.shape[2:])
         sff = bool(m.separate_first_frame_encoding and first_frame)
-        mode_in, mode_out = m.conv_in.pad_mode, m.conv_out.pad_mode
-        vid = video
-        x = eng.conv_in(video, first_frame)
+        mode = m.conv_in.pad_mode
 
-        def bwd_conv_in(g):     # the video needs no gradient: weight / bias only
+        def padded(frames):          # the forward pads with pad_mode (Engine.causal_conv_padded), not with zeros
+            return need_gvideo and mode != "constant" and kin[0] - 1 < frames
+
+        def bwd(g):
             # the causal conv_in's input in the pad modes: channels-last, from the same layout kernel as in the forward
             v = (vid.float() / 255. if vid.dtype == torch.uint8 else vid).to(eng.dtype)
             if sff:
                 ff = m.conv_in_first_frame
                 kff = (1,) + tuple(ff.weight.shape[2:])
-                self._conv_bwd(g[:, t_pad:t_pad + 1].contiguous(), v[:, :, 0:1], ff.weight, ff.bias, kff, pad=(0, kff[1] // 2, kff[2] // 2),
-                               need_gx=False, x_is_cf=True)
+                gv = torch.zeros(v.shape, device=v.device, dtype=eng.dtype) if need_gvideo else None
+                g0 = g[:, t_pad:t_pad + 1].contiguous()
+                self._conv_bwd(g0, v[:, :, 0:1], ff.weight, ff.bias, kff, pad=(0, kff[1] // 2, kff[2] // 2), need_gx=False, x_is_cf=True)
+                if need_gvideo:
+                    gv[:, :, 0:1] = self._video_dgrad(g0, ff.weight, kff, 0)
                 if v.shape[2] > 1:
-                    self._conv_bwd_padmode(g[:, t_pad + 1:].contiguous(), eng.to_channels_last(vid[:, :, 1:]), cin.weight, cin.bias, kin,
-                                           mode_in, need_gx=False)
+                    g1 = g[:, t_pad + 1:].contiguous()
+                    gx = self._conv_bwd_padmode(g1, eng.to_channels_last(vid[:, :, 1:]), cin.weight, cin.bias, kin, mode,
+                                                need_gx=padded(v.shape[2] - 1))
+                    if need_gvideo:
+                        gv[:, :, 1:] = gx.permute(0, 4, 1, 2, 3) if gx is not None else self._video_dgrad(g1, cin.weight, kin, 0)
+                return gv
+            if mode != "constant":
+                gx = self._conv_bwd_padmode(g, eng.to_channels_last(vid, t_pad), cin.weight, cin.bias, kin, mode,
+                                            need_gx=padded(v.shape[2] + t_pad))
+            else:
+                gx = None
+                self._conv_bwd(g, v, cin.weight, cin.bias, kin, pad=(t_pad + kin[0] - 1, kin[1] // 2, kin[2] // 2),
+                               need_gx=False, x_is_cf=True)
+            if not need_gvideo:
                 return None
-            if mode_in != "constant":
-                self._conv_bwd_padmode(g, eng.to_channels_last(vid, t_pad), cin.weight, cin.bias, kin, mode_in, need_gx=False)
-                return None
-            self._conv_bwd(g, v, cin.weight, cin.bias, kin, pad=(t_pad + kin[0] - 1, kin[1] // 2, kin[2] // 2),
-                           need_gx=False, x_is_cf=True)
-            return None
+            return gx[:, t_pad:].permute(0, 4, 1, 2, 3) if gx is not None else self._video_dgrad(g, cin.weight, kin, t_pad)
 
-        self.tape.append(bwd_conv_in)
-        for i, st in enumerate(m.stages):
-            x = self._stage(x, st, f"enc{i}", m.encoder_layers[i], decoder=False, cond_e=ce_enc)
+        return bwd
 
+    def _video_dgrad(self, g, weight, k, t_crop):
+        """Data gradient of conv_in (or its first-frame conv) wrt the video on the engine's conv kernels, like _dgrad: the same
+        implicit GEMM with flipped / transposed weights (K = taps x init_dim, N = channels), without its first t_crop frames
+        (the time_padding).  g: (B,Ti,H,W,init_dim) channels-last -> (B,channels,Ti - t_crop,H,W).  In bf16 the slab kernel's
+        narrow N tile writes torch's layout directly (Engine.conv_cf_supported); otherwise the conv's channels-last output is
+        transposed."""
+        return self.video_dgrad_packed(g, transposed_pack(weight, k, self.eng.dtype), t_crop)
+
+    def video_dgrad_packed(self, g, pk, t_crop):
+        """_video_dgrad with the transposed weight pack given (transposed_pack)."""
+        eng = self.eng
+        _, kh, kw = pk.k
+        B, Ti, H, W, _ = g.shape
+        self.own_dgrad_calls += 1
+        g = g.contiguous()
+        pad_cf, out_cf = (-t_crop, kh // 2, kw // 2), (Ti - t_crop, H, W)
+        if eng.conv_cf_supported(g, pk, pad_cf, out_cf):
+            return eng.conv(g, pk, pad=pad_cf, out_spatial=out_cf, out_cf=True)
+        return eng.to_channels_first(eng.conv(g, pk, pad=(0, kh // 2, kw // 2), out_spatial=(Ti, H, W)), t_crop=t_crop)
+
+    def quantizer_piece(self, x, mode, group=None):
+        """The quantiser on the encoder output x (channels-last); the codes are left in .codes.
+          * mode "loss" (the training forward, M:1705): -> (quantised, aux loss 0-d fp32).  LFQ with its straight-through
+            estimator and auxiliary loss (breakdown in .breakdown, batch entropy over `group`), FSQ with round_ste;
+          * mode "quantize" (encode(quantize=True), M:1567-1576): -> quantised.  LFQ is straight-through in train mode only
+            (in eval the quantised value is a constant of the input), FSQ's round_ste in both modes.  No auxiliary loss."""
+        from .dist import LfqBatchEntropy
+        m, eng = self.m, self.eng
         qz = m.quantizers
+        params = list(qz.parameters())
+        if mode == "quantize":
+            q, self.codes, _ = eng.quantize_cl(x)
+            if m.use_fsq or m.training:
+                fn = (lambda t: _fsq_train(t, qz)) if m.use_fsq else (lambda t: _lfq_quantize(t, qz, True))
+                self.tape.append(lambda g: self._vjp(fn, x, params, g))
+                return q
+
+            def bwd_eval_lfq(g):      # the signs are a constant of x: project_out's gradient only, and nothing reaches x
+                if any(p.requires_grad for p in qz.project_out.parameters()):
+                    self._vjp(lambda t: _lfq_quantize(t, qz, False), x, params, g)
+                return None
+
+            self.tape.append(bwd_eval_lfq)
+            return q
         if m.use_fsq:
-            xq = x
             q, self.codes, _ = eng.quantize_cl(x)
             aux = torch.zeros((), device=eng.device, dtype=torch.float32)
-            self._q_index = len(self.tape)
-            self.tape.append(lambda gs: self._vjp(lambda t: _fsq_train(t, qz), xq, list(qz.parameters()), gs[0]))
-        else:
-            xq = x
-            q, self.codes, pre = eng.quantize_cl(x, want_quantized=True, want_aux=True)
-            be = LfqBatchEntropy(eng, num_codebooks=qz.num_codebooks)
-            be.start(pre, group)
-            avg_sum = be.avg_prob_sum
-            ps, bent, commit, aux = be.finish(qz.diversity_gamma, qz.entropy_loss_weight, qz.commitment_loss_weight, group)
-            world = torch.distributed.get_world_size(group) if (torch.distributed.is_available() and torch.distributed.is_initialized()) else 1
-            avg_global = avg_sum / world
-            self.breakdown = (ps, bent, commit)
-            self._q_index = len(self.tape)
-            self.tape.append(lambda gs: self._vjp(lambda t: _lfq_train(t, qz, avg_global), xq, list(qz.parameters()), gs))
+            self.tape.append(lambda g: self._vjp(lambda t: _fsq_train(t, qz), x, params, g))
+            return q, aux
+        q, self.codes, pre = eng.quantize_cl(x, want_quantized=True, want_aux=True)
+        be = LfqBatchEntropy(eng, num_codebooks=qz.num_codebooks)
+        be.start(pre, group)
+        avg_sum = be.avg_prob_sum
+        ps, bent, commit, aux = be.finish(qz.diversity_gamma, qz.entropy_loss_weight, qz.commitment_loss_weight, group)
+        world = torch.distributed.get_world_size(group) if (torch.distributed.is_available() and torch.distributed.is_initialized()) else 1
+        avg_global = avg_sum / world
+        self.breakdown = (ps, bent, commit)
+        # the auxiliary loss's gradient (self._g_aux) enters here, set by backward
+        self.tape.append(lambda g: self._vjp(lambda t: _lfq_train(t, qz, avg_global), x, params, (g, self._g_aux)))
+        return q, aux
 
+    def codes_piece(self, codes):
+        """indices_to_codes (M:1593) on the engine: codes -> quantised channels-last, recording project_out's backward (a
+        torch restatement on the code values; the integer codes themselves have no gradient)."""
+        m, eng = self.m, self.eng
+        qz = m.quantizers
+        q = eng.codes_to_quantized_cl(codes)
+        vals = _code_values(codes, qz, m.use_fsq)
+
+        def bwd(g):
+            self._vjp(lambda t: _project_out(t, qz, eng.dtype), vals, list(qz.project_out.parameters()), g)
+            return None
+
+        self.tape.append(bwd)
+        return q
+
+    def decoder_piece(self, q, first_frame=True, cond=None):
+        """The decoder stages + conv_out (M:1598-1649): quantised channels-last (B,T',H',W',C) -> reconstruction (B,C,T,H,W)."""
+        m, eng = self.m, self.eng
+        self.cond = cond
+        ce = eng.cond_stem(cond, "dec") if m.has_cond else None            # M:1612-1616
+        t_pad = m.time_padding if first_frame else 0
+        cout = m.conv_out.conv
+        sff = bool(m.separate_first_frame_encoding and first_frame)
+        mode_out = m.conv_out.pad_mode
         x = q
         for j, st in enumerate(reversed(m.stages)):
-            x = self._stage(x, st, f"dec{j}", m.decoder_layers[j], decoder=True, cond_e=ce_dec)
+            x = self._stage(x, st, f"dec{j}", m.decoder_layers[j], decoder=True, cond_e=ce)
         xo = x
         kout = tuple(cout.weight.shape[2:])
         recon = eng.conv_out(xo, first_frame)
@@ -573,8 +709,34 @@ class TrainRunner(TapeRunner):
 
         self.tape.append(bwd_conv_out)
         self._bwd_conv_out = bwd_conv_out
-        self._recon_shape = tuple(recon.shape)
-        return recon, aux
+        return recon
+
+    def forward(self, video, first_frame=True, group=None, cond=None):
+        """The training forward: -> (recon (B,C,T,H,W), aux_loss 0-d fp32); codes / the LFQ breakdown are left in .codes /
+        .breakdown."""
+        x = self.encoder_piece(video, first_frame, cond)
+        q, aux = self.quantizer_piece(x, "loss", group)
+        return self.decoder_piece(q, first_frame, cond), aux
+
+    # ---- the differentiable entry points of VideoTokenizer (one piece chain each); the first tape entry returns the
+    #      gradient wrt the call's input in the caller's layout
+    def run_encode(self, video, cond, first_frame, quantize, need_gvideo):
+        """encode (M:1523-1576): video -> (B,C,T',H',W') encoder output or, quantize, the quantised value."""
+        x = self.encoder_piece(video, first_frame, cond, need_gvideo)
+        if quantize:
+            x = self.quantizer_piece(x, "quantize")
+        dt = self.eng.dtype
+        self.tape.append(lambda g: g.permute(0, 2, 3, 4, 1).to(dt).contiguous())     # from the (B,C,T',H',W') output
+        return self.eng.to_channels_first(x)
+
+    def run_decode(self, quantized, cond, first_frame):
+        """decode (M:1598-1649): quantized (B,C,T',H',W') -> reconstruction."""
+        self.tape.append(lambda g: g.permute(0, 4, 1, 2, 3))                          # to the (B,C,T',H',W') input
+        return self.decoder_piece(self.eng.to_channels_last(quantized), first_frame, cond)
+
+    def run_decode_codes(self, codes, cond, first_frame):
+        """decode_from_code_indices (M:1579-1595): codes (B,T',H',W'[,nc]) -> reconstruction."""
+        return self.decoder_piece(self.codes_piece(codes), first_frame, cond)
 
     def last_layer_weight_grad(self, g_recon):
         """The gradient of ``conv_out.conv.weight`` for a reconstruction gradient g_recon (B,C,T,H,W): the adaptive adversarial
@@ -592,54 +754,55 @@ class TrainRunner(TapeRunner):
             self.grads = grads
         return torch.zeros_like(w) if gw is None else gw
 
-    def backward(self, g_recon, g_aux):
-        """Runs the tape in reverse; returns {Parameter: grad}.  g_recon (B,C,T,H,W) or None, g_aux 0-d or None."""
+    def backward(self, g_out, g_aux=None):
+        """Runs the tape in reverse from the gradient of the last piece's output (g_out; g_aux: the auxiliary loss's, training
+        forward only) -> (gradient wrt the first piece's input | None, gradient wrt cond | None, {Parameter: grad}).  An entry
+        that returns None ends the chain: nothing before it is reached (the eval-mode LFQ quantiser)."""
         if not self.tape:
             raise RuntimeError("the tokenizer's backward ran already: the saved activations are released after one backward pass "
                                "(call the forward again; retain_graph is not supported by this path)")
-        if g_recon is None:
-            g_recon = torch.zeros(self._recon_shape, device=self.eng.device, dtype=self.eng.dtype)
-        g = g_recon.to(self.eng.dtype)
-        n = len(self.tape)
-        q_index = self._q_index                  # the quantiser's entry sits between the encoder and decoder entries
+        g = g_out.to(self.eng.dtype)
+        self._g_aux = (g_aux if g_aux is not None else torch.zeros((), device=self.eng.device)).float()
+        g_cond = None
         with torch.no_grad():
-            for i in range(n - 1, -1, -1):
-                if i == q_index:
-                    if self.m.use_fsq:
-                        g = self.tape[i]((g,))
-                    else:
-                        ga = g_aux if g_aux is not None else torch.zeros((), device=self.eng.device)
-                        g = self.tape[i]((g, ga.float()))
-                else:
-                    g = self.tape[i](g)
+            for entry in reversed(self.tape):
+                g = entry(g)
+                if g is None:
+                    break
             for side, stem in (("enc", self.m.encoder_cond_in), ("dec", self.m.decoder_cond_in)):
                 if side in self.g_cond:       # cond stems (M:1344-1352): Linear + SiLU of the raw cond vector
                     lin = stem[0]
-                    self._vjp(lambda t, lin=lin: F.silu(F.linear(t, lin.weight.float(), lin.bias.float())), self.cond.float(),
-                              list(lin.parameters()), self.g_cond[side].float())
+                    gc = self._vjp(lambda t, lin=lin: F.silu(F.linear(t, lin.weight.float(), lin.bias.float())), self.cond.float(),
+                                   list(lin.parameters()), self.g_cond[side].float())
+                    g_cond = gc if g_cond is None else g_cond + gc
         # the tape's closures and conv_out's piece of it refer to this runner: dropping them here breaks the reference cycle,
         # so the saved activations are freed with the loss graph, not at a later cyclic collection
         self.tape = []
         self._bwd_conv_out = None
-        return self.grads
+        return g, g_cond, self.grads
 
 
-class _TokenizerTrainFn(torch.autograd.Function):
-    """(video, *parameters) -> (recon, aux_loss): forward by the engine kernels, backward by TrainRunner's tape."""
+class _TapeFn(torch.autograd.Function):
+    """(x, cond, *parameters) -> the outputs of `run(x, cond)`, a chain of a runner's pieces on the engine's kernels;
+    backward by the runner's tape.  x is the call's input (video, quantised latents or integer codes); the outputs are a
+    tensor or, for the training forward, (recon, aux_loss).  Gradients go to x and cond when they are floating, and to
+    every parameter handed over."""
 
     @staticmethod
-    def forward(ctx, runner, first_frame, cond, video, *params):
-        recon, aux = runner.forward(video, first_frame, cond=cond)
+    def forward(ctx, runner, run, x, cond, *params):
+        out = run(x, cond)
         ctx.runner, ctx.params = runner, params
-        return recon, aux
+        ctx.in_dtypes = tuple(t.dtype if t is not None and t.is_floating_point() else None for t in (x, cond))
+        return out
 
     @staticmethod
-    def backward(ctx, g_recon, g_aux):
-        grads = ctx.runner.backward(g_recon, g_aux)
+    def backward(ctx, g_out, *g_more):
+        gx, gc, grads = ctx.runner.backward(g_out, g_more[0] if g_more else None)
+        g_in = tuple(None if (g is None or dt is None) else g.to(dt) for g, dt in zip((gx, gc), ctx.in_dtypes))
         # every parameter handed to the Function gets a gradient tensor (zeros if this call did not touch it, e.g. conv_in of a
         # one-frame clip with separate_first_frame_encoding): DistributedDataParallel waits for the hook of every parameter it can
         # reach from the outputs
-        return (None, None, None, None) + tuple(grads[p] if p in grads else torch.zeros_like(p) for p in ctx.params)
+        return (None, None) + g_in + tuple(grads[p] if p in grads else torch.zeros_like(p) for p in ctx.params)
 
 
 def live_parameters(model, first_frame=True):
@@ -652,10 +815,45 @@ def live_parameters(model, first_frame=True):
     return [p for p in model.parameters() if p.requires_grad and id(p) not in dead]
 
 
+def reached_parameters(model, entry, first_frame=True, frames=None, quantize=False):
+    """The parameters (requires_grad) a differentiable call reaches: those the reference's graph gives a gradient.
+      * "decode": the decoder stages, conv_out, conv_out_first_frame (separate_first_frame_encoding with a first frame),
+        decoder_cond_in;  "decode_codes": those and quantizers.project_out (indices_to_codes, M:1593);
+      * "encode": conv_in, conv_in_first_frame (as above), the encoder stages (not the final LayerNorm, see live_parameters),
+        encoder_cond_in; quantize adds the quantiser's projections -- in eval mode only LFQ's project_out, as the signs are a
+        constant of the input there.
+    frames: the clip's frames (encode) or the decoder's output frames (decode): with separate_first_frame_encoding and a
+    first frame, the causal conv_in / conv_out only run on frames after the first."""
+    m = model
+    sff = bool(m.separate_first_frame_encoding and first_frame)
+    mods = []
+    if entry == "encode":
+        qz = m.quantizers
+        if quantize and not m.use_fsq and not m.training:
+            return [p for p in qz.project_out.parameters() if p.requires_grad]
+        if not (sff and frames == 1):
+            mods.append(m.conv_in)
+        if sff:
+            mods.append(m.conv_in_first_frame)
+        mods += [m.encoder_layers[i] for i in range(len(m.stages))] + [m.encoder_cond_in]
+        if quantize:
+            mods += [qz.project_in, qz.project_out]
+    else:
+        if entry == "decode_codes":
+            mods.append(m.quantizers.project_out)
+        mods += [m.decoder_layers, m.decoder_cond_in]
+        if not (sff and frames == 1):
+            mods.append(m.conv_out)
+        if sff:
+            mods.append(m.conv_out_first_frame)
+    ids = {id(p) for mod in mods for p in mod.parameters()}
+    return [p for p in m.parameters() if p.requires_grad and id(p) in ids]
+
+
 def train_forward(model, video, first_frame=True, cond=None, runner=None):
     """-> (recon with grad_fn, aux_loss with grad_fn, codes, lfq breakdown | None).  `runner`: a fresh TrainRunner of the model
     to run on (the caller keeps it for last_layer_weight_grad)."""
     runner = runner or TrainRunner(model)
     params = live_parameters(model, first_frame)
-    recon, aux = _TokenizerTrainFn.apply(runner, first_frame, cond, video, *params)
+    recon, aux = _TapeFn.apply(runner, lambda v, c: runner.forward(v, first_frame, cond=c), video, cond, *params)
     return recon, aux, runner.codes, runner.breakdown

@@ -24,6 +24,10 @@ user-supplied VGG module (``vgg=``, M:1081; nothing is downloaded): the perceptu
 (M:1788-1841) then run on the device (vgg.py).  Without one (``vgg=None``) the model builds no discriminator and
 ``return_loss`` / ``return_discr_loss`` raise.  The VGG is left out of ``state_dict``, ``copy_for_eval`` and the pickled
 config, so ``init_and_load_from`` gives a model without it.
+``encode``, ``decode`` and ``decode_from_code_indices`` are differentiable like the reference's (M:1522-1649) when grad
+mode is on and a floating input requires grad or, in train mode, a parameter the call reaches does (_grad_params): the
+forward runs on the same kernels and train.py's tape pieces give the gradients of the video / latents, ``cond`` and the
+reached parameters; every other call takes the no-grad path unchanged.  ``tokenize`` stays no-grad, as in the reference.
 ``attn_dropout`` (0 <= p < 1) drops the softmax attention weights of train-mode forwards (grad and no-grad) with a Philox
 mask seeded once per call from torch's default CPU generator (engine.AttnDropout, DESIGN.md 3.6); such forwards bypass the
 CUDA graphs.  Eval mode never drops.
@@ -486,22 +490,53 @@ class VideoTokenizer(nn.Module):
         return v, bool(ff)
 
     # ------------------------------------------------------------------ reference API
-    @torch.no_grad()
+    def _grad_params(self, inputs, entry, *args):
+        """The parameters handed to the differentiable path when encode / decode / decode_from_code_indices take it, else
+        None.  The rule: grad mode is on, and a floating input requires grad or, in train mode, a parameter the call reaches
+        does (the rule forward applies to return_loss).  Every other call runs the no-grad path (fused ResidualUnit, CUDA
+        graphs, lanes).  entry, args: train.reached_parameters'."""
+        if not torch.is_grad_enabled():
+            return None
+        wants_input = any(t is not None and t.is_floating_point() and t.requires_grad for t in inputs)
+        if not (wants_input or self.training):
+            return None
+        from .train import reached_parameters
+        params = reached_parameters(self, entry, *args)
+        return params if (wants_input or params) else None
+
+    def _grad_call(self, method, x, cond, params, *args):
+        """One differentiable call: train.TrainRunner.<method>(x, cond, *args) under train._TapeFn."""
+        from .train import TrainRunner, _TapeFn
+        runner = TrainRunner(self)
+        run = getattr(runner, method)
+        return _TapeFn.apply(runner, lambda x_, c_: run(x_, c_, *args), x, cond, *params), runner
+
     @_on_model_device
     @_attn_dropout_scope
     def encode(self, video, quantize=False, cond=None, video_contains_first_frame=True):
-        """M:1523-1576.  Returns (B, C, T', H', W') like the reference."""
+        """M:1523-1576.  Returns (B, C, T', H', W') like the reference; quantize: (quantized, codes[, aux_loss]).
+        Differentiable (see _grad_params) wrt the video, cond and the parameters it reaches (train.reached_parameters).  With
+        quantize, LFQ passes a straight-through gradient in train mode only and FSQ in both modes; the third element keeps
+        its no-grad value (zero in eval mode) -- the train-mode entropy loss with its gradient comes from forward(return_loss=True)."""
         video, ff = self._check_video(video, video_contains_first_frame)
         cond = self._check_cond(cond, video.shape[0])
-        eng = self.engine
-        x = eng.encode_cl(video, ff, cond)
-        if quantize:
-            q, idx, _ = eng.quantize_cl(x)
-            out = eng.to_channels_first(q)
-            if self.use_fsq:
-                return out, idx
-            return out, idx, self.zero
-        return eng.to_channels_first(x)
+        params = self._grad_params((video, cond), "encode", ff, video.shape[2], quantize)
+        if params is not None:
+            need_gvideo = video.is_floating_point() and video.requires_grad
+            out, runner = self._grad_call("run_encode", video.contiguous(), cond, params, ff, quantize, need_gvideo)
+            if not quantize:
+                return out
+            return (out, runner.codes) if self.use_fsq else (out, runner.codes, self.zero)
+        with torch.no_grad():
+            eng = self.engine
+            x = eng.encode_cl(video, ff, cond)
+            if quantize:
+                q, idx, _ = eng.quantize_cl(x)
+                out = eng.to_channels_first(q)
+                if self.use_fsq:
+                    return out, idx
+                return out, idx, self.zero
+            return eng.to_channels_first(x)
 
     def _check_cond(self, cond, batch):
         """M:1542-1545 / M:1610-1613."""
@@ -519,23 +554,31 @@ class VideoTokenizer(nn.Module):
         if t.device != self.device:
             raise RuntimeError(f"{what} is on {t.device} but the tokenizer is on {self.device}")
 
-    @torch.no_grad()
+    def _decoded_frames(self, latent_frames, ff):
+        """Frames of the reconstruction of `latent_frames` latent frames."""
+        return latent_frames * self.time_downsample_factor - (self.time_padding if ff else 0)
+
     @_on_model_device
     @_attn_dropout_scope
     def decode(self, quantized, cond=None, video_contains_first_frame=True):
-        """M:1598-1649.  quantized: (B, C, T', H', W')."""
+        """M:1598-1649.  quantized: (B, C, T', H', W').  Differentiable (see _grad_params) wrt quantized, cond and the
+        decoder's parameters (train.reached_parameters)."""
         assert quantized.ndim == 5 and quantized.shape[1] == self.quantizers.dim, \
             f"quantized must be (B, {self.quantizers.dim}, T, H, W), got {tuple(quantized.shape)}"
         self._check_on_device(quantized, "quantized")
         cond = self._check_cond(cond, quantized.shape[0])
-        eng = self.engine
-        return eng.decode_cl(eng.to_channels_last(quantized), bool(video_contains_first_frame), cond)
+        ff = bool(video_contains_first_frame)
+        params = self._grad_params((quantized, cond), "decode", ff, self._decoded_frames(quantized.shape[2], ff))
+        if params is not None:
+            return self._grad_call("run_decode", quantized, cond, params, ff)[0]
+        with torch.no_grad():
+            eng = self.engine
+            return eng.decode_cl(eng.to_channels_last(quantized), ff, cond)
 
-    @torch.no_grad()
     @_on_model_device
     @_attn_dropout_scope
     def decode_from_code_indices(self, codes, cond=None, video_contains_first_frame=True):
-        """M:1579-1595."""
+        """M:1579-1595.  Differentiable (see _grad_params) wrt cond and the parameters of decode and quantizers.project_out."""
         assert codes.dtype in (torch.long, torch.int32)                           # M:1585
         if codes.ndim == 2:                                                       # M:1587-1591
             n = codes.shape[-1]
@@ -547,9 +590,16 @@ class VideoTokenizer(nn.Module):
         assert codes.ndim == (4 if nc == 1 else 5) and (nc == 1 or codes.shape[-1] == nc), \
             f"codes must be (B, T, H, W{'' if nc == 1 else ', num_codebooks'}) or flat (B, N), got {tuple(codes.shape)}"
         self._check_on_device(codes, "codes")
-        eng = self.engine
         ff = bool(video_contains_first_frame)
         cond = self._check_cond(cond, codes.shape[0])
+        params = self._grad_params((cond,), "decode_codes", ff, self._decoded_frames(codes.shape[1], ff))
+        if params is not None:
+            return self._grad_call("run_decode_codes", codes.contiguous(), cond, params, ff)[0]
+        with torch.no_grad():
+            return self._decode_codes_no_grad(codes, cond, ff)
+
+    def _decode_codes_no_grad(self, codes, cond, ff):
+        eng = self.engine
         if cond is not None:
             return self._graph_call("decode_codes_cond" + ("" if ff else "_noff"),
                                     lambda c, cd: eng.decode_cl(eng.codes_to_quantized_cl(c), ff, cd), codes.contiguous(), cond.contiguous())
