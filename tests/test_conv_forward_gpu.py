@@ -233,33 +233,39 @@ def _geometry(c):
     return pad, ((T + pad[0] - kt) // st + 1, (H + 2 * pad[1] - kh) // sh + 1, (W + 2 * pad[2] - kw) // sw + 1)
 
 
-def _forward64(c, x, w, b, os, r, wrong=None):
-    """float64 reference and allowance (module docstring) of case c; `wrong` names a defect to build into the reference."""
-    kern, kt = c.kern, c.k[0]
-    pad, out_sp = _geometry(c)
-    if c.tshift:                  # TokenShift (M:250-254): channels [ceil(C / 2), C) delayed by one frame
+def forward64(x, w, b, os, r, *, kern, stride, pad, out_sp, K, act=NONE, mode=0, shuffle=SHUFFLE_NONE, tp=None,
+              tshift=False, dtype=torch.bfloat16, wrong=None, exact=False, delta=None):
+    """float64 reference and allowance (module docstring) of one Engine.conv call: x (B,T,H,W,Ci) channels-last, w
+    (Co,Ci,kt,kh,kw) in the reference's channel order, b (Co,), per-clip oscale `os` (B,Co) or None, residual r or None;
+    `pad` / `out_sp` the call's leading pad and output extent before any shuffle, K the packed GEMM depth, `tp` the
+    channels-first conv_out's dropped leading frames.  `wrong` names a defect to build into the reference.  `exact`: the
+    accumulation and the bias add are exact (operands on a dyadic grid), so only the epilogue's errors are allowed;
+    `delta` (B,To,Ho,Wo,Co) is added to the accumulators before the epilogue."""
+    kt = w.shape[2]
+    if tshift:                    # TokenShift (M:250-254): channels [ceil(C / 2), C) delayed by one frame
         split = x.shape[-1] // 2 if wrong == "token shift split at floor(Ci / 2)" else (x.shape[-1] + 1) // 2
         x = x.clone()
         x[:, 1:, ..., split:] = x[:, :-1, ..., split:].clone()
         x[:, 0, ..., split:] = 0
     if wrong == "pad at the back":
-        pad = tuple(0 if s == 2 else p for s, p in zip(c.stride, pad))
-    if c.tp is not None:          # the full causal conv, then its first tp (or, wrongly, tp + 1) frames dropped
+        pad = tuple(0 if s == 2 else p for s, p in zip(stride, pad))
+    if tp is not None:            # the full causal conv, then its first tp (or, wrongly, tp + 1) frames dropped
         T = x.shape[1]
-        crop = c.tp + (wrong == "cropped one frame late")
+        crop = tp + (wrong == "cropped one frame late")
         full = [_conv64(v, wv, (1, 1, 1), (kt - 1,) + pad[1:], (T,) + out_sp[1:]) for v, wv in ((x, w), (x.abs(), w.abs()))]
-        acc, S = (torch.cat((f[:, crop:], torch.zeros_like(f[:, :crop - c.tp])), 1) for f in full)
+        acc, S = (torch.cat((f[:, crop:], torch.zeros_like(f[:, :crop - tp])), 1) for f in full)
     else:
-        acc = _conv64(x, w, c.stride, pad, out_sp)
-        S = _conv64(x.abs(), w.abs(), c.stride, pad, out_sp)
-    B = x.shape[0]
+        acc = _conv64(x, w, stride, pad, out_sp)
+        S = _conv64(x.abs(), w.abs(), stride, pad, out_sp)
+    if delta is not None:
+        acc = acc + delta
     if os is not None:
+        assert not exact, "a per-clip oscale product is rounded: no exact accumulation"
         osv = os.clone()
         if wrong == "oscale of clip 0 used for clip 1":
             osv[1:] = osv[0]
         osb = osv[:, None, None, None, :]
         S = S * os.abs()[:, None, None, None, :]
-    K = 12 * c.ci if kern == "down" else math.prod(c.k) * c.ci      # the packed down-space GEMM: 6 taps x 2 Ci
     gam = _gamma(K, C_KERN[kern])
     if os is not None and wrong == "oscale applied after the bias":
         z = (acc + b) * osb
@@ -269,28 +275,36 @@ def _forward64(c, x, w, b, os, r, wrong=None):
         z = acc + b
     if wrong == "bias dropped":
         z = z - b
-    e = gam * S + 3 * U * (S + b.abs())
+    e = torch.zeros_like(S) if exact else gam * S + 3 * U * (S + b.abs())
     if wrong == "bias added after the activation":
-        v = ACT64[c.act](z - b) + b
+        v = ACT64[act](z - b) + b
     else:
-        v = ACT64[c.act](z)
-    e = SLOPE[c.act] * e + _act_err(c.act, z, v, kern)
+        v = ACT64[act](z)
+    e = SLOPE[act] * e + _act_err(act, z, v, kern)
     ref = v
     if r is not None:
         t = v + r
         e = e + U * t.abs()
         ref = t
-        if c.mode == 2:
+        if mode == 2:
             ref = v * RS + r if wrong == "scaled-residual factor applied before the residual add" else t * RS
             if kern == "simt":    # rounded to the output dtype, then scaled and rounded again
-                e = RS * (0.5 * _ulp(t.abs() + e, DT[c.dt]) + e) + 2 * U * ref.abs()
+                e = RS * (0.5 * _ulp(t.abs() + e, dtype) + e) + 2 * U * ref.abs()
             else:
                 e = RS * e + 2 * U * ref.abs()
     swap = wrong == "shuffle phases swapped"
-    ref, e = _shuffle(ref, c.shuffle, swap), _shuffle(e, c.shuffle)
-    if c.tp is not None:
+    ref, e = _shuffle(ref, shuffle, swap), _shuffle(e, shuffle)
+    if tp is not None:
         ref, e = ref.permute(0, 4, 1, 2, 3), e.permute(0, 4, 1, 2, 3)
     return ref, e
+
+
+def _forward64(c, x, w, b, os, r, wrong=None):
+    """forward64 of case c."""
+    pad, out_sp = _geometry(c)
+    K = 12 * c.ci if c.kern == "down" else math.prod(c.k) * c.ci      # the packed down-space GEMM: 6 taps x 2 Ci
+    return forward64(x, w, b, os, r, kern=c.kern, stride=c.stride, pad=pad, out_sp=out_sp, K=K, act=c.act, mode=c.mode,
+                     shuffle=c.shuffle, tp=c.tp, tshift=c.tshift, dtype=DT[c.dt], wrong=wrong)
 
 
 def _wrongs(c):
@@ -520,16 +534,24 @@ def test_geglu_epilogue_vs_float64(guarded, name, C_, I, packing, variant, shape
     assert y.shape == (B, T, H, W, Ip)
     if Ip > I:                    # the hidden channels pack_ff pads in are exactly zero: gelu(0) * 0
         assert torch.equal(y[..., I:].float(), torch.zeros_like(y[..., I:].float())), f"{name}: padded channels"
-    h = x @ w1.T + b1
-    S = x.abs() @ w1.abs().T
-    e = _gamma(C_, C_KERN[kind]) * S + 3 * U * (S + b1.abs())
-    xv, gt, ex, eg = h[..., :I], h[..., I:], e[..., :I], e[..., I:]
-    ref = F.gelu(gt) * xv
-    acc = xv.abs() * (_gelu_err(gt) + GELU_SLOPE * eg) + F.gelu(gt).abs() * ex + U * ref.abs()
+    ref, acc, (xv, gt) = geglu64(x, w1, b1, kind)
     out = y[..., :I]
     _check(out, ref, torch.bfloat16, acc, name)
     _rejects(out, F.gelu(xv) * gt, torch.bfloat16, acc, f"{name}: x and gate halves swapped")
     _rejects(out, (F.gelu(gt - b1[I:]) + b1[I:]) * xv, torch.bfloat16, acc, f"{name}: gate bias added after the GELU")
+
+
+def geglu64(x, w1, b1, kern, exact=False):
+    """float64 fc1 + GEGLU of x (..., C) with fc1 (2I, C) in the reference's row order: (reference, allowance, (x half,
+    gate half)).  `exact`: fc1's accumulation and bias add are exact (dyadic operands)."""
+    I = w1.shape[0] // 2
+    h = x @ w1.T + b1
+    S = x.abs() @ w1.abs().T
+    e = torch.zeros_like(S) if exact else _gamma(w1.shape[1], C_KERN[kern]) * S + 3 * U * (S + b1.abs())
+    xv, gt, ex, eg = h[..., :I], h[..., I:], e[..., :I], e[..., I:]
+    ref = F.gelu(gt) * xv
+    acc = xv.abs() * (_gelu_err(gt) + GELU_SLOPE * eg) + F.gelu(gt).abs() * ex + U * ref.abs()
+    return ref, acc, (xv, gt)
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -592,6 +614,36 @@ RU_CASES = [
 RU_HD = 32
 
 
+def ru_y64(x, w3, b3, w1, b1, exact=False, delta=None):
+    """float64 y = ELU(conv1(round_bf16(ELU(conv3 x + b3))) + b1) of the fused ResidualUnit (module docstring): (y,
+    allowance, bf16-rounded h).  x (B,T,H,W,C), w3 (C,C,kt,kh,kw), w1 (C,C,1,1,1).  `exact`: conv3's accumulation and bias
+    add are exact (dyadic operands); `delta` is added to conv3's accumulators."""
+    B, T, H, W, C_ = x.shape
+    kt, kh, kw = w3.shape[2:]
+    K3 = kt * kh * kw * C_
+    z3 = _conv64(x, w3, (1, 1, 1), (kt - 1, kh // 2, kw // 2), (T, H, W))
+    if delta is not None:
+        z3 = z3 + delta
+    z3 = z3 + b3
+    h64 = F.elu(z3)
+    eh = _act_err(ELU, z3, h64, "slab")
+    if not exact:
+        S3 = _conv64(x.abs(), w3.abs(), (1, 1, 1), (kt - 1, kh // 2, kw // 2), (T, H, W))
+        eh = eh + _gamma(K3, 2) * S3 + 3 * U * (S3 + b3.abs())
+        del S3
+    lo, hi = (v.to(torch.bfloat16).double() for v in (h64 - eh, h64 + eh))
+    hb = h64.to(torch.bfloat16).double()
+    del h64, eh, z3
+    either = torch.where(lo != hi, _ulp(torch.maximum(lo.abs(), hi.abs()), torch.bfloat16), torch.zeros_like(hb))
+    del lo, hi
+    w1m = w1[:, :, 0, 0, 0]
+    z1 = hb @ w1m.T + b1
+    S1 = (hb.abs() + either) @ w1m.abs().T
+    y_ref = F.elu(z1)
+    ey = _gamma(C_, 2) * S1 + 3 * U * (S1 + b1.abs()) + either @ w1m.abs().T + _act_err(ELU, z1, y_ref, "slab")
+    return y_ref, ey, hb
+
+
 def _ru_targets(H, W):
     """Impulse positions per frame: the last (ragged) row's last column, elsewhere on the last row and on the last column,
     and next to a quarter boundary (rows 3 / 4 of a row tile)."""
@@ -614,19 +666,8 @@ def test_fused_residual_unit_vs_float64(guarded, name, C_, shape, plan):
     for (h, w_) in _ru_targets(H, W):
         x[:, :, h, w_] = _bfrand(C_, gen, 3.0)
     x[1:] *= 2                                                      # clip 1 scaled
-    # float64 reference of y (module docstring)
-    z3 = _conv64(x, w3, (1, 1, 1), (2, 1, 1), (T, H, W)) + b3
-    S3 = _conv64(x.abs(), w3.abs(), (1, 1, 1), (2, 1, 1), (T, H, W))
-    h64 = F.elu(z3)
-    eh = _gamma(27 * C_, 2) * S3 + 3 * U * (S3 + b3.abs()) + _act_err(ELU, z3, h64, "slab")
-    lo, hi = (v.to(torch.bfloat16).double() for v in (h64 - eh, h64 + eh))
-    hb = h64.to(torch.bfloat16).double()
-    either = torch.where(lo != hi, _ulp(torch.maximum(lo.abs(), hi.abs()), torch.bfloat16), torch.zeros_like(hb))
+    y_ref, ey, hb = ru_y64(x, w3, b3, w1, b1)
     w1m = w1[:, :, 0, 0, 0]
-    z1 = hb @ w1m.T + b1
-    S1 = (hb.abs() + either) @ w1m.abs().T
-    y_ref = F.elu(z1)
-    ey = _gamma(C_, 2) * S1 + 3 * U * (S1 + b1.abs()) + either @ w1m.abs().T + _act_err(ELU, z1, y_ref, "slab")
     # se_wk along the corner impulse's response in y, scaled until the last row and the last column each carry at least
     # 10% of every frame's softmax weight
     y_bg = y_ref[0, 0, 0, 0]                                       # no impulse reaches (0, 0): the constant background
