@@ -32,9 +32,11 @@
 extern "C" {
 #endif
 
-#define MV2_ABI_VERSION 4   /* 2: mv2_conv_args.oscale, mv2_tc_conv_args.{oscale,out_layout}; 3: num_codebooks / spherical in the quantiser entry points;
+#define MV2_ABI_VERSION 5   /* 2: mv2_conv_args.oscale, mv2_tc_conv_args.{oscale,out_layout}; 3: num_codebooks / spherical in the quantiser entry points;
                                4: the two entry points of the one-launch SqueezeExcite tail for small frames are removed: the
-                               engine never enabled it by default, so the separate pool / gate / gate_residual calls are the only SE path */
+                               engine never enabled it by default, so the separate pool / gate / gate_residual calls are the only SE path;
+                               5: the conv entry points take the streaming history (mv2_conv_hist, NULL for none) as an argument,
+                               their four _hist twins are removed */
 
 enum { MV2_F32 = 0, MV2_BF16 = 1,
        MV2_U8 = 2   /* source dtype of the two layout-in entry points only: decoded uint8 frames, normalised x / 255 */ };
@@ -53,6 +55,8 @@ int mv2_abi_version(void);
 const char* mv2_last_error(void);
 /* Compute capability of the current device as major*10+minor (90 on H100), <0 on error. */
 int mv2_device_arch(void);
+/* The frames in front of a streamed chunk that the conv entry points read (see "streaming" below); NULL: none. */
+typedef struct mv2_conv_hist mv2_conv_hist;
 /* Programmatic dependent launch: when on, every kernel is launched with
  * cudaLaunchAttributeProgrammaticStreamSerialization so its prologue (barrier init, bias staging,
  * block scheduling) overlaps the tail of the previous kernel of the stream; all kernels execute griddepcontrol.wait
@@ -120,7 +124,7 @@ typedef struct mv2_conv_args {
   const float* oscale;       /* fp32 [B][Co] or NULL: per-(clip, output channel) multiplier applied to the accumulator BEFORE
                                 bias / activation -- the demodulation factor of Conv3DMod (M:741-742), see mv2_mod_prepare */
 } mv2_conv_args;
-int mv2_conv_forward(const mv2_conv_args* a, void* stream);
+int mv2_conv_forward(const mv2_conv_args* a, const mv2_conv_hist* hist, void* stream);
 
 /* ---- SqueezeExcite (M:221-240) --------------------------------------------------
  * se_pool  : per frame f (F = B*T frames of P = H*W positions, C channels):
@@ -300,13 +304,13 @@ typedef struct mv2_tc_conv_args {
                           8- / 16-column N tiles.                                                                        */
 } mv2_tc_conv_args;
 int mv2_tc_conv_supported(const mv2_tc_conv_args* a);
-int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream);
+int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream);
 /* "Slab" variant for stride-1 convs with an in-plane kernel (the causal 3x3x3 residual convs): persistent
  * CTAs, one haloed activation slab per (frame, 64-channel slice) staged in shared memory once and reused by
  * all k_h*k_w in-plane taps, up to four 128-position M-tiles sharing each weight tile (mw * N tile <= 128 columns of
  * register accumulators).  Requirements (mv2_tc_slab_supported): stride 1, Ci % 64 == 0, Co % 32 == 0, no shuffle.   */
 int mv2_tc_slab_supported(const mv2_tc_conv_args* a);
-int mv2_tc_slab_forward(const mv2_tc_conv_args* a, void* stream);
+int mv2_tc_slab_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream);
 /* SpatialDownsample2x (M:770-780: per-frame Conv2d k3 s2 p1) on the slab design: the input is read as (W/2) x (2C) with
  * row-parity sub-slabs, so no tap reloads its tile from L2.  `a` describes the conv as usual (kh = kw = 3, sh = sw = 2,
  * ph = pw = 1, kt = 1), but w is packed as bf16 [Co][6][2*Ci]: tap' = dh * 2 + q, q = 0: [zeros(Ci) | w[:, :, dh, 0]],
@@ -358,7 +362,7 @@ typedef struct mv2_tc_ru_args {
 int mv2_tc_ru_supported(const mv2_tc_ru_args* a);
 int mv2_tc_ru_records(const mv2_tc_ru_args* a);
 size_t mv2_tc_ru_workspace_bytes(const mv2_tc_ru_args* a);
-int mv2_tc_ru_forward(const mv2_tc_ru_args* a, void* stream);
+int mv2_tc_ru_forward(const mv2_tc_ru_args* a, const mv2_conv_hist* hist, void* stream);
 /* SE gate from pool records in the (max, sum, acc[C]) format, nrec records per frame laid out [F][nrec][C + 2], with the
  * hidden layer scratch (F * Hd floats) right behind them: gate[f,:] = sigmoid(W2 leaky_relu_0.1(W1 pooled + b1) + b2).
  * mv2_tc_ru_workspace_bytes reserves F * (C + 16) floats for that scratch: Hd <= C + 16, else MV2_E_ARG.                  */
@@ -372,25 +376,20 @@ int mv2_se_gate_records(const void* workspace, int nrec, int F, int C, int Hd,
  *
  * mv2_conv_hist: the frames in front of a causal conv's input x.  Input frame t < 0 of clip b is history frame T_h + t,
  *   read from h + b * clip_stride (elements) as a (T_h, Hi, Wi, Ci) block; frames older than the history (t < -T_h) are the
- *   causal zero padding, exactly as frame t < 0 is for the entry points without history.  The history may be the tail of
- *   the previous chunk's input itself (clip_stride = that tensor's frames per clip * Hi * Wi * Ci): nothing is copied.
- *   T_h = 0 means no history (the plain entry point's result).
- * mv2_conv_forward_hist / mv2_tc_conv_forward_hist / mv2_tc_slab_forward_hist / mv2_tc_ru_forward_hist: the entry point
- *   of the same name without _hist, with that history.  Each output element accumulates the same products in the same
- *   order as the whole-clip call; the slab kernels skip the taps older than the history as they skip the padding.
- *   mv2_tc_conv_forward_hist takes the shapes mv2_tc_conv_hist_supported accepts (pure host arithmetic): stride 1 and an
- *   output tile of one frame or of >= 8 positions per frame.  For the others a caller runs mv2_tc_conv_forward on a copy of
- *   [history | x] with pt reduced by T_h, which gives the same values.                                                      */
-typedef struct mv2_conv_hist {
+ *   causal zero padding, exactly as frame t < 0 is without history.  The history may be the tail of the previous chunk's
+ *   input itself (clip_stride = that tensor's frames per clip * Hi * Wi * Ci): nothing is copied.
+ * The `hist` argument of mv2_conv_forward, mv2_tc_conv_forward, mv2_tc_slab_forward and mv2_tc_ru_forward: NULL or T_h = 0
+ *   means no history.  Each output element accumulates the same products in the same order as the whole-clip call; the
+ *   slab kernels skip the taps older than the history as they skip the padding.  mv2_tc_conv_forward takes a history only
+ *   on the shapes mv2_tc_conv_hist_supported accepts (pure host arithmetic): stride 1 and an output tile of one frame or of
+ *   >= 8 positions per frame.  For the others a caller runs it without history on a copy of [history | x] with pt reduced
+ *   by T_h, which gives the same values.                                                                                    */
+struct mv2_conv_hist {
   const void* h;
   int32_t T_h;
   int64_t clip_stride;
-} mv2_conv_hist;
-int mv2_conv_forward_hist(const mv2_conv_args* a, const mv2_conv_hist* hist, void* stream);
+};
 int mv2_tc_conv_hist_supported(const mv2_tc_conv_args* a);
-int mv2_tc_conv_forward_hist(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream);
-int mv2_tc_slab_forward_hist(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream);
-int mv2_tc_ru_forward_hist(const mv2_tc_ru_args* a, const mv2_conv_hist* hist, void* stream);
 /* mv2_rmsnorm_prev: mv2_rmsnorm whose token shift reads frame -1 of clip b from prev + b * prev_clip_stride (elements,
  *   a (P, C) frame) instead of zeros: the TokenShift (M:250-254) of a chunk that continues a clip.                        */
 int mv2_rmsnorm_prev(const void* x, const void* prev, int64_t prev_clip_stride, void* out, int dtype, const float* gamma,

@@ -91,7 +91,7 @@ SIGNATURES = {
     "mv2_ingest_kwpack": (_I, [_VP, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _VP]),
     "mv2_copy_frames": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _SZ, _I, _VP]),
     "mv2_pad_cl": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _VP]),
-    "mv2_conv_forward": (_I, [C.POINTER(ConvArgs), _VP]),
+    "mv2_conv_forward": (_I, [C.POINTER(ConvArgs), C.POINTER(ConvHist), _VP]),
     "mv2_se_workspace_bytes": (_SZ, [_I, _I, _I]),
     "mv2_se_pool": (_I, [_VP, _I, _I, _I, _I, _VP, _F, _VP, _VP]),
     "mv2_se_gate": (_I, [_VP, _I, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
@@ -118,9 +118,9 @@ SIGNATURES = {
     "mv2_maxpool2x2": (_I, [_VP, _VP, _I, _I, _I, _I, _I, _VP]),
     "mv2_maxpool2x2_backward": (_I, [_VP, _VP, _VP, _I, _I, _I, _I, _I, _VP]),
     "mv2_tc_conv_supported": (_I, [C.POINTER(TcConvArgs)]),
-    "mv2_tc_conv_forward": (_I, [C.POINTER(TcConvArgs), _VP]),
+    "mv2_tc_conv_forward": (_I, [C.POINTER(TcConvArgs), C.POINTER(ConvHist), _VP]),
     "mv2_tc_slab_supported": (_I, [C.POINTER(TcConvArgs)]),
-    "mv2_tc_slab_forward": (_I, [C.POINTER(TcConvArgs), _VP]),
+    "mv2_tc_slab_forward": (_I, [C.POINTER(TcConvArgs), C.POINTER(ConvHist), _VP]),
     "mv2_tc_down_space_supported": (_I, [C.POINTER(TcConvArgs)]),
     "mv2_tc_down_space_forward": (_I, [C.POINTER(TcConvArgs), _VP]),
     "mv2_tc_slab_plan": (_I, [C.POINTER(TcConvArgs), _I, C.POINTER(C.c_int32)]),
@@ -131,12 +131,8 @@ SIGNATURES = {
     "mv2_tc_ru_supported": (_I, [C.POINTER(TcRuArgs)]),
     "mv2_tc_ru_records": (_I, [C.POINTER(TcRuArgs)]),
     "mv2_tc_ru_workspace_bytes": (_SZ, [C.POINTER(TcRuArgs)]),
-    "mv2_tc_ru_forward": (_I, [C.POINTER(TcRuArgs), _VP]),
+    "mv2_tc_ru_forward": (_I, [C.POINTER(TcRuArgs), C.POINTER(ConvHist), _VP]),
     "mv2_se_gate_records": (_I, [_VP, _I, _I, _I, _I, _VP, _VP, _VP, _VP, _VP, _VP]),
-    "mv2_conv_forward_hist": (_I, [C.POINTER(ConvArgs), C.POINTER(ConvHist), _VP]),
-    "mv2_tc_conv_forward_hist": (_I, [C.POINTER(TcConvArgs), C.POINTER(ConvHist), _VP]),
-    "mv2_tc_slab_forward_hist": (_I, [C.POINTER(TcConvArgs), C.POINTER(ConvHist), _VP]),
-    "mv2_tc_ru_forward_hist": (_I, [C.POINTER(TcRuArgs), C.POINTER(ConvHist), _VP]),
     "mv2_rmsnorm_prev": (_I, [_VP, _VP, _I64, _VP, _I, _VP, _I, _I, _I, _I, _VP]),
     "mv2_attention_tail": (_I, [C.POINTER(AttnArgs), _VP, _I64, _I, _VP, _I64, _VP]),
     "mv2_tc_conv_hist_supported": (_I, [C.POINTER(TcConvArgs)]),
@@ -164,8 +160,8 @@ def load():
         fn.restype = res
         fn.argtypes = args
     ver = lib.mv2_abi_version()
-    if ver != 4:
-        raise Mv2Error(f"ABI version mismatch: library {ver}, binding 4")
+    if ver != 5:
+        raise Mv2Error(f"ABI version mismatch: library {ver}, binding 5")
     _lib = lib
     return lib
 

@@ -2634,13 +2634,10 @@ int mv2_ingest_kwpack(const void* src, int src_dtype, void* dst, int B, int C, i
   return MV2_OK;
 }
 
-int mv2_conv_forward(const mv2_conv_args* a, void* stream) {
+int mv2_conv_forward(const mv2_conv_args* a, const mv2_conv_hist* hist, void* stream) {
   const mv2_conv_hist none = {nullptr, 0, 0};
-  return mv2_conv_forward_hist(a, &none, stream);
-}
-
-int mv2_conv_forward_hist(const mv2_conv_args* a, const mv2_conv_hist* hist, void* stream) {
-  MV2_CHECK_ARG(a && a->x && a->w && a->y && hist && hist->T_h >= 0 && (hist->T_h == 0 || hist->h));
+  if (!hist) hist = &none;
+  MV2_CHECK_ARG(a && a->x && a->w && a->y && hist->T_h >= 0 && (hist->T_h == 0 || hist->h));
   MV2_CHECK_ARG(a->B > 0 && a->Ti > 0 && a->Hi > 0 && a->Wi > 0 && a->Ci > 0);
   MV2_CHECK_ARG(a->To > 0 && a->Ho > 0 && a->Wo > 0 && a->Co > 0);
   MV2_CHECK_ARG(a->kt > 0 && a->kh > 0 && a->kw > 0 && a->st > 0 && a->sh > 0 && a->sw > 0);

@@ -205,9 +205,7 @@ int mv2_tc_conv_supported(const mv2_tc_conv_args* a) {
   return 1;
 }
 
-int mv2_tc_conv_forward(const mv2_tc_conv_args* a, void* stream) { return mv2_tc_conv_forward_hist(a, nullptr, stream); }
-
-int mv2_tc_conv_forward_hist(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream) {
+int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream) {
   MV2_CHECK_ARG(a && a->x && a->w && a->y);
   MV2_CHECK_ARG(!hist || (hist->T_h >= 0 && (hist->T_h == 0 || (hist->h && hist->clip_stride > 0))));
   const int hist_T = hist ? hist->T_h : 0;
@@ -227,7 +225,7 @@ int mv2_tc_conv_forward_hist(const mv2_tc_conv_args* a, const mv2_conv_hist* his
   p.hist_T = hist_T;
   p.frame_loads = hist_T > 0 ? p.bt : 1;
   if (hist_T > 0 && !mv2_tc_conv_hist_supported(a)) {
-    set_error("mv2_tc_conv_forward_hist: unsupported shape (mv2_tc_conv_hist_supported)");
+    set_error("mv2_tc_conv_forward: unsupported shape with history (mv2_tc_conv_hist_supported)");
     return MV2_E_UNSUPPORTED;
   }
   // N tile: 32, 64 or 128 columns (a wgmma N, 64 fp32 accumulator registers per thread at 128); wider outputs take

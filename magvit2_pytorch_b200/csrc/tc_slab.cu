@@ -860,9 +860,7 @@ extern "C" int mv2_tc_slab_tile(const mv2_tc_conv_args* a, int n_sm, int cta, in
   return MV2_OK;
 }
 
-extern "C" int mv2_tc_slab_forward(const mv2_tc_conv_args* a, void* stream) { return mv2_tc_slab_forward_hist(a, nullptr, stream); }
-
-extern "C" int mv2_tc_slab_forward_hist(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream) {
+extern "C" int mv2_tc_slab_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream) {
   MV2_CHECK_ARG(a && a->x && a->w && a->y);
   MV2_CHECK_ARG(!hist || (hist->T_h >= 0 && (hist->T_h == 0 || (hist->h && hist->clip_stride > 0))));
   if (!mv2_tc_slab_supported(a)) { set_error("mv2_tc_slab_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }
@@ -934,9 +932,7 @@ extern "C" size_t mv2_tc_ru_workspace_bytes(const mv2_tc_ru_args* a) {
   return (F * recs * (a->C + 2) + F * (a->C + 16)) * sizeof(float);    // pool records + the SE hidden layer (mv2_se_gate_records)
 }
 
-extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, void* stream) { return mv2_tc_ru_forward_hist(a, nullptr, stream); }
-
-extern "C" int mv2_tc_ru_forward_hist(const mv2_tc_ru_args* a, const mv2_conv_hist* hist, void* stream) {
+extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, const mv2_conv_hist* hist, void* stream) {
   MV2_CHECK_ARG(a && a->x && a->w3 && a->w1 && a->y && a->se_wk && a->se_ws);
   MV2_CHECK_ARG(!hist || (hist->T_h >= 0 && (hist->T_h == 0 || (hist->h && hist->clip_stride > 0))));
   if (!mv2_tc_ru_supported(a)) { set_error("mv2_tc_ru_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }

@@ -9,6 +9,7 @@ fallback: every op is a library call and a missing library is an error.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Tuple
 
@@ -139,11 +140,15 @@ def _round_up(v, m):
 def pack_ff(fc1_w, fc1_b, fc2_w, fc2_b, dtype):
     """FeedForward weights (reference M:492-496).  wgmma layout: the hidden width I is padded to a multiple of 64,
     fc1's rows are re-paired as [8 x-rows, their 8 gate-rows] per group of 16 so GEGLU (M:466-469) fuses into fc1's
-    epilogue, and fc2's K is zero-padded to match."""
+    epilogue, and fc2's K is zero-padded to match.  The fused fc1 needs K = C a multiple of 16; for other widths there
+    are no wgmma packs, and fc1, GEGLU and fc2 run unfused on the CUDA cores."""
     fc1 = pack_conv(fc1_w, fc1_b, dtype)
     fc2 = pack_conv(fc2_w, fc2_b, dtype)
-    if dtype == torch.bfloat16:
-        two_i, C_ = fc1_w.shape[:2]
+    two_i, C_ = fc1_w.shape[:2]
+    if dtype == torch.bfloat16 and C_ % 16 != 0:
+        for pk in (fc1, fc2):
+            pk.w_tc = pk.bias_tc = None
+    elif dtype == torch.bfloat16:
         I = two_i // 2
         Ip = _round_up(I, 64)
         w1 = fc1_w.detach().reshape(two_i, C_).float()
@@ -215,7 +220,7 @@ class Engine:
         self._sig_id = 0             # bumped whenever parameters are re-packed (invalidates cached CUDA graphs)
         self.launches = 0            # kernels launched through the C ABI (bench's gpu_launches)
         self.use_tc = True           # bf16: dense contractions on wgmma (False -> CUDA-core cross-check path)
-        self.tc_variant = "auto"     # "auto" | "tap" (tc_conv.cu only) | "slab" (prefer tc_slab.cu)
+        self.tc_variant = "auto"     # "auto" (Engine.conv_kernel's choice) | "tap" (tc_conv.cu only)
         self.fuse_ru = True          # bf16: conv3x3x3 + ELU + conv1x1x1 + ELU + SE pool partials in one wgmma launch (C = 64 / 128)
         self.fused_ru_calls = 0
         self.tc_calls = 0
@@ -223,7 +228,7 @@ class Engine:
         self.simt_conv_calls = 0
         self.taps: Optional[dict] = None  # when set, per-stage activations are recorded (tests)
         self._prof: Optional[list] = None  # when set, (event0, event1, flops) per wgmma conv launch
-        self.conv_log: Optional[list] = None  # when set, one shape record per tensor-core conv launch
+        self.conv_log: Optional[list] = None  # when set, one record per tensor-core conv launch (Engine._conv_launch)
         self.dropout: Optional[AttnDropout] = None  # set for the duration of a train-mode forward with attention dropout
 
     # ------------------------------------------------------------------ parameters
@@ -384,99 +389,50 @@ class Engine:
         k_t - 1 input frames are kept for the next chunk."""
         B, Ti, Hi, Wi, Ci = x.shape
         hist, advance = self._conv_hist(ss, x, pk.k[0] - 1)
-        tc_ok = self._tc_ok(x, pk) and not token_shift
-        kt, kh, kw = pk.k_tc if (tc_ok and pk.k_tc) else pk.k
-        if pad is None:
-            pad = (kt - 1, kh // 2, kw // 2)
-        if out_spatial is None:
-            out_spatial = (Ti, Hi, Wi)
-        To, Ho, Wo = out_spatial
-        if tc_ok:
-            co_gemm = pk.Co_tc
-            co_out = co_gemm // 2 if pk.epi_mode == 1 else co_gemm
-            if shuffle == SHUFFLE_SPACE:
-                y = self._new((B, To, 2 * Ho, 2 * Wo, co_out // 4))
-            elif shuffle == SHUFFLE_TIME:
-                y = self._new((B, 2 * To, Ho, Wo, co_out // 2))
-            elif out_cf:
-                y = self._new((B, co_out, To, Ho, Wo))
-            else:
-                y = self._new((B, To, Ho, Wo, co_out))
-            if res is not None:
-                assert res.shape == y.shape and res.dtype == y.dtype and res.is_contiguous()
-            ta = self._tc_args(x, pk, stride, pad, out_spatial, act, shuffle, out_cf, res=res, y=y, oscale=oscale)
-            # policy: the persistent slab kernel reuses each activation slab for all in-plane taps, so it takes every layer it
-            # supports (incl. the 64-byte-row conv_in); the tap-wise kernel keeps the strided down-samplers.  tc_variant = "tap" forces the tap-wise kernel (tests / sweeps).
-            use_slab = self.tc_variant != "tap" and bool(self.lib.mv2_tc_slab_supported(C.byref(ta)))
-            use_down = (not use_slab and self.tc_variant != "tap" and pk.w_down is not None and stride == (1, 2, 2)
-                        and bool(self.lib.mv2_tc_down_space_supported(C.byref(ta))))
-            if use_down:
-                ta.w = _ptr(pk.w_down)
-                use_slab = True
-            if use_slab or self.lib.mv2_tc_conv_supported(C.byref(ta)):
-                if self._prof is not None:
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    e0.record()
-                if use_down:
-                    check(self.lib.mv2_tc_down_space_forward(C.byref(ta), self._stream()), "mv2_tc_down_space_forward")
-                    self.slab_calls += 1
-                elif use_slab and hist is not None:
-                    check(self.lib.mv2_tc_slab_forward_hist(C.byref(ta), C.byref(hist), self._stream()), "mv2_tc_slab_forward_hist")
-                    self.slab_calls += 1
-                elif use_slab:
-                    check(self.lib.mv2_tc_slab_forward(C.byref(ta), self._stream()), "mv2_tc_slab_forward")
-                    self.slab_calls += 1
-                elif hist is not None and self.lib.mv2_tc_conv_hist_supported(C.byref(ta)):
-                    check(self.lib.mv2_tc_conv_forward_hist(C.byref(ta), C.byref(hist), self._stream()), "mv2_tc_conv_forward_hist")
-                elif hist is not None:
-                    # shapes the history operand does not take (a strided conv, or frame tiles of < 8 positions): the same
-                    # kernel on a copy of [history | x] with the leading padding shortened by the history, which gives the
-                    # same products per output element
-                    cat = self._hist_cat(ss, x)
-                    ta.x, ta.Ti, ta.pt = _ptr(cat), cat.shape[1], pad[0] - hist.T_h
-                    check(self.lib.mv2_tc_conv_forward(C.byref(ta), self._stream()), "mv2_tc_conv_forward")
-                else:
-                    check(self.lib.mv2_tc_conv_forward(C.byref(ta), self._stream()), "mv2_tc_conv_forward")
-                if self._prof is not None:
-                    e1.record()
-                    self._prof.append((e0, e1, 2.0 * B * To * Ho * Wo * pk.macs,
-                                       "slab" if use_slab else "tap", pk.k[1] * pk.k[2] * pk.k[0]))
-                if self.conv_log is not None:
-                    self.conv_log.append(dict(kind="slab" if use_slab else "tap", Ci=Ci, Co=co_out, k=tuple(pk.k), out=(B, To, Ho, Wo),
-                                              geglu=pk.epi_mode == 1, shuffle=shuffle, res=res is not None, act=act,
-                                              epi_mode=pk.epi_mode, stride=tuple(stride)))
-                self.launches += 1
-                self.tc_calls += 1
-                if advance is not None:
-                    advance()
-                return y
-            assert not out_cf, "channels-first output is a wgmma slab-kernel feature"
-            assert pk.w is not None and pk.epi_mode in (0, 2) and Ci == pk.Ci, "wgmma-only weight pack has no CUDA-core fallback"
-            kt, kh, kw = pk.k
-        assert Ci == pk.Ci, (Ci, pk.Ci)
-        assert pk.w is not None and not out_cf
-        if shuffle == SHUFFLE_SPACE:
-            y = self._new((B, To, 2 * Ho, 2 * Wo, pk.Co // 4))
-        elif shuffle == SHUFFLE_TIME:
-            y = self._new((B, 2 * To, Ho, Wo, pk.Co // 2))
+        ta = self._tc_args(x, pk, stride, pad, out_spatial, act, shuffle, out_cf, res=res, oscale=oscale)
+        kind = self.conv_kernel(ta, pk, 0 if hist is None else hist.T_h, token_shift)
+        To, Ho, Wo = ta.To, ta.Ho, ta.Wo
+        if kind == "simt":
+            assert Ci == pk.Ci and pk.w is not None and not out_cf, "wgmma-only weight pack or layout has no CUDA-core path"
+            co = pk.Co
         else:
-            y = self._new((B, To, Ho, Wo, pk.Co))
+            co = pk.Co_tc // 2 if pk.epi_mode == 1 else pk.Co_tc
+        if shuffle == SHUFFLE_SPACE:
+            y = self._new((B, To, 2 * Ho, 2 * Wo, co // 4))
+        elif shuffle == SHUFFLE_TIME:
+            y = self._new((B, 2 * To, Ho, Wo, co // 2))
+        elif out_cf:
+            y = self._new((B, co, To, Ho, Wo))
+        else:
+            y = self._new((B, To, Ho, Wo, co))
         if res is not None:
             assert res.shape == y.shape and res.dtype == y.dtype and res.is_contiguous()
-        self.simt_conv_calls += 1
-        a = ConvArgs(x=_ptr(x), w=_ptr(pk.w), bias=_ptr(pk.bias), res=_ptr(res), y=_ptr(y), dtype=_dt(self.dtype),
-                     B=B, Ti=Ti, Hi=Hi, Wi=Wi, Ci=Ci, To=To, Ho=Ho, Wo=Wo, Co=pk.Co,
-                     kt=kt, kh=kh, kw=kw, st=stride[0], sh=stride[1], sw=stride[2],
-                     pt=pad[0], ph=pad[1], pw=pad[2], act=act, shuffle=shuffle, x_token_shift=int(token_shift),
-                     oscale=_ptr(oscale))
-        if hist is not None:
-            check(self.lib.mv2_conv_forward_hist(C.byref(a), C.byref(hist), self._stream()), "mv2_conv_forward_hist")
+        hist_p = None if hist is None else C.byref(hist)
+        if kind == "simt":
+            a = ConvArgs(x=_ptr(x), w=_ptr(pk.w), bias=_ptr(pk.bias), res=_ptr(res), y=_ptr(y), dtype=_dt(self.dtype),
+                         B=B, Ti=Ti, Hi=Hi, Wi=Wi, Ci=Ci, To=To, Ho=Ho, Wo=Wo, Co=pk.Co,
+                         kt=ta.kt, kh=ta.kh, kw=ta.kw, st=ta.st, sh=ta.sh, sw=ta.sw, pt=ta.pt, ph=ta.ph, pw=ta.pw,
+                         act=act, shuffle=shuffle, x_token_shift=int(token_shift), oscale=_ptr(oscale))
+            entry, args = "mv2_conv_forward", (C.byref(a), hist_p)
+        elif kind == "down":
+            ta.y, ta.w = _ptr(y), _ptr(pk.w_down)
+            entry, args = "mv2_tc_down_space_forward", (C.byref(ta),)
         else:
-            check(self.lib.mv2_conv_forward(C.byref(a), self._stream()), "mv2_conv_forward")
-        self.launches += 1
+            ta.y = _ptr(y)
+            if kind == "tap_cat":
+                # shapes the history operand does not take (a strided conv, or frame tiles of < 8 positions): the same
+                # kernel on a copy of [history | x] with the leading padding shortened by the history, which gives the
+                # same products per output element
+                cat = self._hist_cat(ss, x)
+                ta.x, ta.Ti, ta.pt = _ptr(cat), cat.shape[1], ta.pt - hist.T_h
+                kind, hist_p = "tap", None
+            entry = "mv2_tc_slab_forward" if kind == "slab" else "mv2_tc_conv_forward"
+            args = (C.byref(ta), hist_p)
+        self._conv_launch(kind, entry, args, Ci=Ci, Co=co, k=tuple(pk.k), out=(B, To, Ho, Wo), macs=pk.macs, act=act,
+                          shuffle=shuffle, res=res is not None, epi_mode=pk.epi_mode, stride=tuple(stride))
         if advance is not None:
             advance()
-        if pk.epi_mode == 2:          # scaled residual: the residual epilogue, then * 2^-0.5 (the reference's add-then-multiply)
+        if kind == "simt" and pk.epi_mode == 2:   # scaled residual: the residual epilogue, then * 2^-0.5 (the reference's add-then-multiply)
             assert res is not None and shuffle == SHUFFLE_NONE
             scale = torch.full((B, pk.Co), 2 ** -0.5, device=self.device, dtype=torch.float32)
             check(self.lib.mv2_scale_channels(_ptr(y), _ptr(scale), _ptr(y), _dt(self.dtype), B, To * Ho * Wo, pk.Co, self._stream()),
@@ -484,28 +440,70 @@ class Engine:
             self.launches += 1
         return y
 
-    def _tc_ok(self, x, pk: ConvPack) -> bool:
-        """Whether conv(x, pk) may run on the wgmma kernels: bf16 with a wgmma weight pack for x's channel count."""
-        return self.dtype == torch.bfloat16 and self.use_tc and pk.w_tc is not None and x.shape[-1] == pk.Ci_tc
+    def conv_kernel(self, ta: TcConvArgs, pk: ConvPack, hist_T: int = 0, token_shift: bool = False) -> str:
+        """The kernel conv() runs for the call `ta` (its mv2_tc_conv_args) with hist_T history frames: "slab" (tc_slab.cu),
+        "down" (its SpatialDownsample2x flavour, on pk.w_down), "tap" (tc_conv.cu), "tap_cat" (tc_conv.cu on a copy of
+        [history | x]) or "simt" (the CUDA-core conv).  Host-side shape queries only: it launches nothing and needs no device."""
+        if not (self.dtype == torch.bfloat16 and self.use_tc and pk.w_tc is not None and ta.Ci == pk.Ci_tc and not token_shift):
+            return "simt"
+        lib = self.lib
+        # the persistent slab kernel reuses each activation slab for all in-plane taps, so it takes every layer it supports
+        # (incl. the 64-byte-row conv_in); the tap-wise kernel keeps the strided down-samplers that have no down-space pack.
+        # tc_variant = "tap" forces the tap-wise kernel (tests / sweeps).
+        if self.tc_variant != "tap":
+            if lib.mv2_tc_slab_supported(C.byref(ta)):
+                return "slab"
+            if pk.w_down is not None and lib.mv2_tc_down_space_supported(C.byref(ta)):
+                return "down"
+        if not lib.mv2_tc_conv_supported(C.byref(ta)):
+            return "simt"
+        return "tap_cat" if hist_T > 0 and not lib.mv2_tc_conv_hist_supported(C.byref(ta)) else "tap"
 
-    def _tc_args(self, x, pk: ConvPack, stride, pad, out_spatial, act, shuffle, out_cf, res=None, y=None, oscale=None):
-        """The mv2_tc_conv_args of conv(x, pk, ...) on the wgmma kernels."""
-        B, Ti, Hi, Wi, Ci = x.shape
+    def _conv_launch(self, kind, entry, args, *, Ci, Co, k, out, macs, act, shuffle=SHUFFLE_NONE, res=False, epi_mode=0,
+                     stride=(1, 1, 1), fused_ru=False):
+        """Launches conv kernel `entry`(*args, stream) of `kind` ("slab", "down", "tap" or "simt") and accounts for it: the
+        counters, CUDA events around it inside profile_convs and, for the tensor-core kernels, a conv_log record.  out:
+        (B, To, Ho, Wo) output positions; macs: multiply-accumulates per position.  The down-space kernel is a flavour of the
+        slab kernel: it counts, profiles and logs as "slab", and its record has down_space=True."""
+        down_space = kind == "down"
+        kind = "slab" if down_space else kind
+        prof = self._prof is not None and kind != "simt"
+        if prof:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+        check(getattr(self.lib, entry)(*args, self._stream()), entry)
+        self.launches += 1
+        if kind == "simt":
+            self.simt_conv_calls += 1
+            return
+        if prof:
+            e1.record()
+            self._prof.append((e0, e1, 2.0 * math.prod(out) * macs, kind, math.prod(k)))
+        if self.conv_log is not None:
+            self.conv_log.append(dict(kind=kind, Ci=Ci, Co=Co, k=k, out=out, geglu=epi_mode == 1, shuffle=shuffle, res=res,
+                                      act=act, epi_mode=epi_mode, stride=stride, fused_ru=fused_ru, down_space=down_space))
+        self.tc_calls += 1
+        self.slab_calls += kind != "tap"
+        self.fused_ru_calls += fused_ru
+
+    def _tc_args(self, x, pk: ConvPack, stride=(1, 1, 1), pad=None, out_spatial=None, act=ACT_NONE, shuffle=SHUFFLE_NONE,
+                 out_cf=False, res=None, y=None, oscale=None):
+        """The mv2_tc_conv_args of conv(x, pk, ...) on the wgmma kernels, with conv's defaults for pad and out_spatial.  x may
+        be the input's shape instead, for a conv_kernel query before the input exists."""
+        B, Ti, Hi, Wi, Ci = x.shape if isinstance(x, torch.Tensor) else x
         kt, kh, kw = pk.k_tc or pk.k
-        To, Ho, Wo = out_spatial
-        return TcConvArgs(x=_ptr(x), w=_ptr(pk.w_tc), bias=_ptr(pk.bias_tc), res=_ptr(res), y=_ptr(y),
-                          B=B, Ti=Ti, Hi=Hi, Wi=Wi, Ci=Ci, To=To, Ho=Ho, Wo=Wo, Co=pk.Co_tc,
+        pt, ph, pw = (kt - 1, kh // 2, kw // 2) if pad is None else pad
+        To, Ho, Wo = (Ti, Hi, Wi) if out_spatial is None else out_spatial
+        return TcConvArgs(x=_ptr(x) if isinstance(x, torch.Tensor) else None, w=_ptr(pk.w_tc), bias=_ptr(pk.bias_tc),
+                          res=_ptr(res), y=_ptr(y), B=B, Ti=Ti, Hi=Hi, Wi=Wi, Ci=Ci, To=To, Ho=Ho, Wo=Wo, Co=pk.Co_tc,
                           kt=kt, kh=kh, kw=kw, st=stride[0], sh=stride[1], sw=stride[2],
-                          pt=pad[0], ph=pad[1], pw=pad[2], act=act, shuffle=shuffle, epi_mode=pk.epi_mode,
+                          pt=pt, ph=ph, pw=pw, act=act, shuffle=shuffle, epi_mode=pk.epi_mode,
                           oscale=_ptr(oscale), out_layout=int(out_cf))
 
     def conv_cf_supported(self, x, pk: ConvPack, pad, out_spatial) -> bool:
         """True when conv(x, pk, pad=pad, out_spatial=out_spatial, out_cf=True) runs: bf16 on the slab kernel, whose
         channels-first epilogue takes fewer than 8 (or a ragged number of) output channels."""
-        if not (self._tc_ok(x, pk) and self.tc_variant != "tap" and pk.Co % 8 != 0):
-            return False
-        ta = self._tc_args(x, pk, (1, 1, 1), pad, out_spatial, ACT_NONE, SHUFFLE_NONE, True)
-        return bool(self.lib.mv2_tc_slab_supported(C.byref(ta)))
+        return self.conv_kernel(self._tc_args(x, pk, pad=pad, out_spatial=out_spatial, out_cf=True), pk) == "slab"
 
     def residual_unit(self, x, p, ss: Optional[StreamState] = None):
         """ResidualUnit (reference M:930-944): x + SE(ELU(conv1(ELU(causal_conv3(x)))))."""
@@ -514,7 +512,7 @@ class Engine:
         st = self._stream()
         dt = _dt(self.dtype)
         c3, c1 = p["conv3"], p["conv1"]
-        if self.dtype == torch.bfloat16 and self.use_tc and self.fuse_ru and c3.w_tc is not None and self.tc_variant != "tap":
+        if self.fuse_ru and self.conv_kernel(self._tc_args(x, c3, act=ACT_ELU), c3) == "slab":
             ra = TcRuArgs(x=_ptr(x), w3=_ptr(c3.w_tc), b3=_ptr(c3.bias_tc), w1=_ptr(c1.w_tc), b1=_ptr(c1.bias_tc),
                           se_wk=_ptr(p["wk"]), se_bk=p["bk"], y=None, se_ws=None, B=B, T=T, H=H, W=W, C=Cc,
                           kt=c3.k[0], kh=c3.k[1], kw=c3.k[2])
@@ -524,30 +522,16 @@ class Engine:
                 ws = self._new((self.lib.mv2_tc_ru_workspace_bytes(C.byref(ra)) // 4,), torch.float32)
                 ra.y, ra.se_ws = _ptr(y), _ptr(ws)
                 nrec = self.lib.mv2_tc_ru_records(C.byref(ra))
-                if self._prof is not None:
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    e0.record()
-                if hist is not None:
-                    check(self.lib.mv2_tc_ru_forward_hist(C.byref(ra), C.byref(hist), st), "mv2_tc_ru_forward_hist")
-                else:
-                    check(self.lib.mv2_tc_ru_forward(C.byref(ra), st), "mv2_tc_ru_forward")
+                self._conv_launch("slab", "mv2_tc_ru_forward", (C.byref(ra), None if hist is None else C.byref(hist)), Ci=Cc,
+                                  Co=Cc, k=tuple(c3.k), out=(B, T, H, W), macs=c3.macs + c1.macs, act=ACT_ELU, fused_ru=True)
                 if advance is not None:
                     advance()
-                if self._prof is not None:
-                    e1.record()
-                    self._prof.append((e0, e1, 2.0 * B * T * H * W * (c3.macs + c1.macs), "slab", c3.k[0] * c3.k[1] * c3.k[2]))
-                if self.conv_log is not None:
-                    self.conv_log.append(dict(kind="slab", Ci=Cc, Co=Cc, k=tuple(c3.k), out=(B, T, H, W), geglu=False, shuffle=0,
-                                              res=False, fused_ru=True))
                 gates = self._new((F_, Cc), torch.float32)
                 check(self.lib.mv2_se_gate_records(_ptr(ws), nrec, F_, Cc, p["hidden"], _ptr(p["w1"]), _ptr(p["b1"]), _ptr(p["w2"]),
                                                    _ptr(p["b2"]), _ptr(gates), st), "mv2_se_gate_records")
                 out = self._new(x.shape)
                 check(self.lib.mv2_gate_residual(_ptr(y), _ptr(x), _ptr(gates), _ptr(out), dt, F_, Pn, Cc, st), "mv2_gate_residual")
-                self.launches += 4
-                self.tc_calls += 1
-                self.slab_calls += 1
-                self.fused_ru_calls += 1
+                self.launches += 3                # mv2_se_gate_records: two kernels; mv2_gate_residual: one
                 return out
         h = self.conv(x, c3, act=ACT_ELU, ss=_sub(ss, "conv3"))
         y = self.conv(h, c1, act=ACT_ELU)
@@ -620,25 +604,16 @@ class Engine:
         """Residual(FeedForward) (M:471-508, M:1191): x + fc2(geglu(fc1(rmsnorm(shift(x)))))."""
         B, T, H, W, Cc = x.shape
         xn = self.rmsnorm(x, p["gamma"], token_shift, ss)
-        # fused fc1 + GEGLU pack is wgmma-only (K = C must be a multiple of 16); other widths take the unfused
-        # CUDA-core convs + mv2_geglu below, like the fp32 path
-        if self.dtype == torch.bfloat16 and self.use_tc and p["fc1"].epi_mode == 1 and Cc % 16 == 0:
-            g = self.conv(xn, p["fc1"])                       # fc1 + bias + GEGLU fused, hidden width padded to 64
-            return self.conv(g, p["fc2"], res=x)
         fc1 = p["fc1"]
-        hdn = self._conv_simt_only(xn, fc1)
+        if self.conv_kernel(self._tc_args(xn, fc1), fc1) != "simt":
+            g = self.conv(xn, fc1)                            # fc1 + bias + GEGLU fused, hidden width padded to 64
+            return self.conv(g, p["fc2"], res=x)
+        hdn = self.conv(xn, fc1)
         I = p["inner"]
         g = self._new((B, T, H, W, I))
         check(self.lib.mv2_geglu(_ptr(hdn), _ptr(g), _dt(self.dtype), B * T * H * W, I, self._stream()), "mv2_geglu")
         self.launches += 1
-        return self._conv_simt_only(g, p["fc2"], res=x)
-
-    def _conv_simt_only(self, x, pk, **kw):
-        use, self.use_tc = self.use_tc, False
-        try:
-            return self.conv(x, pk, **kw)
-        finally:
-            self.use_tc = use
+        return self.conv(g, p["fc2"], res=x)
 
     def attention(self, x, p, axis: str, dropout: Optional[_lib.DropoutArgs] = None, ss: Optional[StreamState] = None):
         """Residual(SpaceAttention) / Residual(TokenShift(TimeAttention)) (M:444-464, M:1190, M:1235).  `dropout`: drop the
@@ -905,12 +880,12 @@ class Engine:
         t_pad = m.time_padding if first_frame else 0
         pin = self._packs.get("conv_in_tc")
         ss = _sub(ss, "conv_in")
+        B, _, T, H, W = video.shape
         if sff_rest:
             x = self.conv(self.to_channels_last(video, 0), self._packs["conv_in"], ss=ss)
         elif m.separate_first_frame_encoding and first_frame:
             # M:1553-1561: the first frame goes through its own 2-D conv, frames 1.. through the causal conv_in on their own,
             # then the feature map is [time_padding zero frames, first, rest]
-            B, _, T, H, W = video.shape
             v_cl = self.to_channels_last(video, 0)
             parts = [(self.conv(self.copy_frames(v_cl, 0, 1), self._packs["conv_in_ff"]), t_pad)]
             if T > 1:
@@ -922,7 +897,7 @@ class Engine:
                 self.copy_frames(part, 0, part.shape[1], dst=x, dst_t0=t0, zero_front=(i == 0))
         elif m.conv_in.pad_mode != "constant":
             x = self.causal_conv_padded(self.to_channels_last(video, t_pad), self._packs["conv_in"], m.conv_in.pad_mode)
-        elif self.dtype == torch.bfloat16 and self.use_tc and pin is not None:
+        elif pin is not None and self.conv_kernel(self._tc_args((B, T + t_pad, H, W, pin.Ci_tc), pin), pin) != "simt":
             x = self.ingest_kwpack(video, t_pad, pin)
             x = self.conv(x, pin, pad=(pin.k_tc[0] - 1, pin.k_tc[1] // 2, 0), ss=ss)
         else:
@@ -977,12 +952,13 @@ class Engine:
             return self.to_channels_first(out)
         if m.conv_out.pad_mode != "constant":
             return self.to_channels_first(self.causal_conv_padded(x, pk, m.conv_out.pad_mode), t_crop=tp)
-        if (self.dtype == torch.bfloat16 and self.use_tc and self.tc_variant != "tap" and pk.w_tc is not None and pk.Co % 8 != 0
-                and Cc % 64 == 0 and pk.k[2] <= 3 and T > tp):
-            # conv_out writes the reconstruction in torch's (B,C,T,H,W) layout itself and never computes the time_padding
-            # frames the reference drops afterwards (M:1642-1647)
-            return self.conv(x, pk, pad=(pk.k[0] - 1 - tp, pk.k[1] // 2, pk.k[2] // 2), out_spatial=(T - tp, H, W), out_cf=True,
-                             ss=ss)
+        # conv_out writes the reconstruction in torch's (B,C,T,H,W) layout itself and never computes the time_padding frames
+        # the reference drops afterwards (M:1642-1647)
+        pad, out_sp = (pk.k[0] - 1 - tp, pk.k[1] // 2, pk.k[2] // 2), (T - tp, H, W)
+        if (pk.k[2] <= 3            # wider in-plane taps would take the narrow N tiles, which are meant for the video's data gradient
+                and Cc % 64 == 0    # 128-byte rows only: a kw = 1 conv_out on 32-channel rows keeps the channels-last conv
+                and T > tp and self.conv_cf_supported(x, pk, pad, out_sp)):
+            return self.conv(x, pk, pad=pad, out_spatial=out_sp, out_cf=True, ss=ss)
         x = self.conv(x, pk, ss=ss)
         return self.to_channels_first(x, t_crop=tp)
 

@@ -31,12 +31,12 @@ def test_every_declared_symbol_is_exported_and_bound():
         assert name in declared, f"{name} bound in _lib.py but not declared in the header"
 
 
-def test_load_and_abi_version():
-    """ABI version 4: the library, the header's MV2_ABI_VERSION and the ctypes binding agree (load() checks the binding)."""
+def test_load_and_abi_version_5():
+    """ABI version 5: the library, the header's MV2_ABI_VERSION and the ctypes binding agree (load() checks the binding)."""
     lib = _lib.load()
-    assert lib.mv2_abi_version() == 4
+    assert lib.mv2_abi_version() == 5
     header = open(os.path.join(ROOT, "include", "magvit2_b200.h")).read()
-    assert int(re.search(r"#define\s+MV2_ABI_VERSION\s+(\d+)", header).group(1)) == 4
+    assert int(re.search(r"#define\s+MV2_ABI_VERSION\s+(\d+)", header).group(1)) == 5
     assert lib.mv2_se_workspace_bytes(2, 256, 64) == (2 * 8 * 66 + 2 * 80) * 4
     assert lib.mv2_linattn_workspace_bytes(3, 16, 1024) == 3 * 16 * 4 * 657 * 4 + 3 * 16 * 2 * 16 * 88 * 2
 

@@ -143,8 +143,8 @@ def _ran(eng, fn):
     kind = {(1, 1, 0, 0): "slab", (0, 1, 0, 0): "tap", (0, 0, 1, 0): "simt", (1, 1, 0, 1): "ru"}.get(d, f"counters moved by {d}")
     if kind in ("slab", "tap"):
         assert len(eng.conv_log) == n_log + 1 and eng.conv_log[-1]["kind"] == kind
-        if kind == "slab" and eng.conv_log[-1]["stride"] == (1, 2, 2):
-            kind = "down"        # the slab kernel itself takes no spatial stride: only the down-space variant does
+        if eng.conv_log[-1]["down_space"]:
+            kind = "down"        # a flavour of the slab kernel: counted and logged as "slab", flagged in its record
     return kind, out
 
 

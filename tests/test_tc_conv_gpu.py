@@ -172,7 +172,7 @@ def test_slab_matches_cuda_core(case):
     pk = pack_conv(w, bias, torch.bfloat16, k=k3, shuffle_q=kw.pop("q", 1))
     want_res = kw.pop("res", False)
     res = torch.randn((B, T, H, W, wshape[0]), generator=g).cuda().to(torch.bfloat16) if want_res else None
-    eng.use_tc, eng.tc_variant, eng.slab_calls = True, "slab", 0
+    eng.use_tc, eng.tc_variant, eng.slab_calls = True, "auto", 0
     y_slab = eng.conv(x, pk, res=res, **kw)
     assert eng.slab_calls == 1, "slab kernel was not taken"
     eng.tc_variant = "tap"
@@ -217,7 +217,7 @@ def test_fused_geglu_feed_forward_matches_cuda_core(C_, tshift):
     assert (a - b).abs().mean().item() <= 0.004 * b.abs().mean().item() + 1e-4
 
 
-@pytest.mark.parametrize("variant", ["tap", "slab"])
+@pytest.mark.parametrize("variant", ["tap", "auto"])
 def test_conv_in_kwpack_matches_cuda_core(variant):
     """conv_in (7x7x7, C_in=3) through mv2_ingest_kwpack + wgmma (49 taps x 32 packed channels) vs the CUDA-core conv."""
     assert torch.cuda.is_available()
@@ -230,7 +230,7 @@ def test_conv_in_kwpack_matches_cuda_core(variant):
     eng.use_tc, eng.tc_calls, eng.slab_calls, eng.tc_variant = True, 0, 0, variant
     x = eng.ingest_kwpack(v, 2, pin)
     y_tc = eng.conv(x, pin, pad=(6, 3, 0))
-    assert eng.tc_calls == 1 and eng.slab_calls == (1 if variant == "slab" else 0)
+    assert eng.tc_calls == 1 and eng.slab_calls == (1 if variant == "auto" else 0)
     eng.use_tc = False
     y_ref = eng.conv(eng.to_channels_last(v, 2), eng._packs["conv_in"])
     torch.cuda.synchronize()

@@ -43,10 +43,10 @@ class _RecordingLib:
         if name not in LAUNCHES:
             return fn
 
-        def launch(args_ref, stream):
+        def launch(args_ref, *rest):          # (hist, stream), or (stream,) for the down-space conv
             a = args_ref._obj
             self.calls.append((name, type(a).from_buffer_copy(a)))
-            return fn(args_ref, stream)
+            return fn(args_ref, *rest)
         return launch
 
 
