@@ -11,7 +11,13 @@ clip through each network):
     arithmetic and by fp32 sums in shuffled orders against float64.
 
 readme_table() is the table the GPU test asserts its recorded calls against: a later dispatch change cannot silently move one of
-these calls off the kernel the GPU test checks."""
+these calls off the kernel the GPU test checks.
+
+tokenizer_table() / tokenizer_counts() are the same for the tokenizer's own calls in that step
+(tests/test_train_tokenizer_calls_gpu.py): every conv of the training forward (ResidualUnits unfused) and every data
+gradient, the calls per kind, and the premises of its replays (the deepest GEMM within the replay grid's exact depth, the
+weight-gradient replay's integer sums below 2^24, the slab plans and defect tiles on 132 SMs)."""
+import ctypes as C
 import math
 
 import numpy as np
@@ -19,12 +25,14 @@ import pytest
 import torch
 
 import synth_data
-from tests.test_bench_calls_gpu import REPLAY_GRID
+from tests.test_bench_calls_cpu import N_SM
+from tests.test_bench_calls_gpu import REPLAY_GRID, last_cta
 from tests.util import README_LAYERS
 
 from magvit2_pytorch_b200 import VideoTokenizer
-from magvit2_pytorch_b200._lib import ACT_LEAKY_RELU, ACT_RELU, SHUFFLE_SPACE
-from magvit2_pytorch_b200.engine import Engine, pack_conv, pack_conv_in_kwpack, pack_feed_forward
+from magvit2_pytorch_b200._lib import ACT_ELU, ACT_LEAKY_RELU, ACT_RELU, ACT_SILU, SHUFFLE_SPACE, SHUFFLE_TIME
+from magvit2_pytorch_b200.engine import (Engine, pack_conv, pack_conv_down_space, pack_conv_in_kwpack, pack_feed_forward,
+                                         pack_linear_attention)
 from magvit2_pytorch_b200.gan import logits_conv_weight, stride2_1x1_dgrad_weight, unshuffle_conv_weight, unshuffle_dgrad_weight
 from magvit2_pytorch_b200.train import transposed_pack
 from magvit2_pytorch_b200.vgg import adaptive_pool_matrix, fold_avgpool_linear
@@ -303,3 +311,211 @@ def test_fold_error_allowance(fmap):
                         *(adaptive_pool_matrix(n, 7) for n in fmap))
     wf = fold_avgpool_linear(w, 8, fmap, (7, 7)).to(BF).double()
     assert ((wf - wf64).abs() <= (2.0 ** -8 + 2.0 ** -23) * wf64.abs()).all()
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the tokenizer's own calls (tests/test_train_tokenizer_calls_gpu.py)
+# ------------------------------------------------------------------------------------------------------------------
+FRAMES = 17
+# the tokenizer call that runs on the CUDA-core conv by design: conv_out's data gradient, a transposed conv with 3 input
+# channels (the reconstruction's), below the wgmma kernels' channel granularity
+TOK_SIMT_BY_DESIGN = {("tok", "dgrad k333", "conv_out")}
+
+
+def _tok_dgrad(block, w, k, g_shape, kind):
+    """TapeRunner._dgrad of a stride-1 causal conv with weight w and kernel k: the transposed conv on g (B, T, H, W, Co)."""
+    return _c("tok", f"dgrad k{''.join(map(str, k))}", block, g_shape, transposed_pack(w, k, BF),
+              dict(pad=(0, k[1] // 2, k[2] // 2), out_spatial=g_shape[1:4]), kind)
+
+
+def _attn_calls(calls, key, mod, st, x):
+    """The convs of an attention-type stage: its projections, then the feed-forward's fc1 (GEGLU) and fc2."""
+    time_axis = st.kind == "attend_time"
+    if st.kind == "linear_attend_space":
+        p = pack_linear_attention(mod[0].fn, BF)
+        inner = p["heads"] * p["dim_head"]
+        calls += [_c("tok", "q", key, x, p["q"], {}, "slab"), _c("tok", "kv", key, x, p["kv"], {}, "slab"),
+                  _c("tok", "attn_out", key, x[:-1] + (inner,), p["out"], dict(res=True), "slab")]
+        ff = mod[1].fn
+    else:
+        at = mod[0].fn.fn if time_axis else mod[0].fn
+        inner = at.heads * at.dim_head
+        calls += [_c("tok", "qkv", key, x, pack_conv(at.to_qkv[0].weight[:, :, None, None, None], None, BF), {}, "slab"),
+                  _c("tok", "attn_out", key, x[:-1] + (inner,),
+                     pack_conv(at.to_out[1].weight[:, :, None, None, None], None, BF), dict(res=True), "slab")]
+        ff = mod[1].fn.fn if time_axis else mod[1].fn
+    p = pack_feed_forward(ff, BF)
+    calls += [_c("tok", "fc1", key, x, p["fc1"], {}, "slab"),
+              _c("tok", "fc2", key, x[:-1] + (p["fc1"].Co_tc // 2,), p["fc2"], dict(res=True), "slab")]
+
+
+def tokenizer_calls(m, B, frames=FRAMES, size=128):
+    """Every engine conv of one TrainRunner forward and backward of the tokenizer (train.py), in the order of the forward,
+    then the data gradients: dict(net, role, block, x_shape, pk, kw, kind) as discr_calls.  The ResidualUnits run unfused
+    (conv3 with ELU, conv1 with ELU); the backward runs two data gradients per ResidualUnit and conv_out's."""
+    T, S = frames + m.time_padding, size
+    cin = m.conv_in.conv
+    pin = pack_conv_in_kwpack(cin.weight, cin.bias)
+    kt, kh = pin.k_tc[:2]
+    calls = [_c("tok", "conv_in_kw", "conv_in", (B, T, S, S, pin.Ci_tc), pin, dict(pad=(kt - 1, kh // 2, 0)), "slab")]
+    dgrads = []
+
+    def residual(key, mod, st, x):
+        for j, ru in enumerate(list(mod) if st.nested else [mod]):
+            seq = ru.fn
+            c3, c1 = seq[0].conv, seq[2]
+            k3 = tuple(c3.weight.shape[2:])
+            calls.append(_c("tok", "conv3", f"{key}.{j}", x, pack_conv(c3.weight, c3.bias, BF), dict(act=ACT_ELU), "slab"))
+            calls.append(_c("tok", "conv1", f"{key}.{j}", x, pack_conv(c1.weight, c1.bias, BF), dict(act=ACT_ELU), "slab"))
+            dgrads.append(_tok_dgrad(f"{key}.{j}", c1.weight, (1, 1, 1), x, "slab"))
+            dgrads.append(_tok_dgrad(f"{key}.{j}", c3.weight, k3, x, "slab"))
+
+    C_ = cin.weight.shape[0]
+    for i, st in enumerate(m.stages):
+        mod, key, x = m.encoder_layers[i], f"enc{i}", (B, T, S, S, C_)
+        if st.kind == "residual":
+            residual(key, mod, st, x)
+        elif st.kind == "compress_space":
+            pk = pack_conv(mod.conv.weight, mod.conv.bias, BF)
+            pack_conv_down_space(pk, mod.conv.weight)
+            S //= 2
+            calls.append(_c("tok", "down_space", key, x, pk, dict(stride=(1, 2, 2), pad=(0, 1, 1), out_spatial=(T, S, S)),
+                            "down"))
+            C_ = pk.Co
+        elif st.kind == "compress_time":
+            pk = pack_conv(mod.conv.weight, mod.conv.bias, BF, k=(3, 1, 1))
+            T //= 2
+            calls.append(_c("tok", "down_time", key, x, pk, dict(stride=(2, 1, 1), pad=(2, 0, 0), out_spatial=(T, S, S)),
+                            "slab"))
+            C_ = pk.Co
+        else:
+            _attn_calls(calls, key, mod, st, x)
+    for j, st in enumerate(reversed(m.stages)):
+        mod, key, x = m.decoder_layers[j], f"dec{j}", (B, T, S, S, C_)
+        if st.kind == "residual":
+            residual(key, mod, st, x)
+        elif st.kind == "compress_space":
+            pk = pack_conv(mod.net[0].weight, mod.net[0].bias, BF, shuffle_q=4)
+            calls.append(_c("tok", "up_space", key, x, pk, dict(act=ACT_SILU, shuffle=SHUFFLE_SPACE), "slab"))
+            S, C_ = 2 * S, pk.Co // 4
+        elif st.kind == "compress_time":
+            pk = pack_conv(mod.net[0].weight, mod.net[0].bias, BF, k=(1, 1, 1), shuffle_q=2)
+            calls.append(_c("tok", "up_time", key, x, pk, dict(act=ACT_SILU, shuffle=SHUFFLE_TIME), "slab"))
+            T, C_ = 2 * T, pk.Co // 2
+        else:
+            _attn_calls(calls, key, mod, st, x)
+    cout = m.conv_out.conv
+    kout, tp = tuple(cout.weight.shape[2:]), m.time_padding
+    x = (B, T, S, S, C_)
+    calls.append(_c("tok", "conv_out", "conv_out", x, pack_conv(cout.weight, cout.bias, BF),
+                    dict(pad=(kout[0] - 1 - tp, kout[1] // 2, kout[2] // 2), out_spatial=(T - tp, S, S), out_cf=True), "slab"))
+    dgrads.append(_tok_dgrad("conv_out", cout.weight, kout, x[:-1] + (cout.weight.shape[0],), "simt"))
+    return calls + dgrads
+
+
+def tokenizer_table(B=CLIPS):
+    """(calls, {call_key: (kind, block)}, model) of the README training step's tokenizer calls."""
+    m = readme_train_model()
+    calls = tokenizer_calls(m, B)
+    return calls, {call_key(c): (c["kind"], c["block"]) for c in calls}, m
+
+
+def _n_residual_units(m):
+    return sum(st.count for st in m.stages if st.kind == "residual")
+
+
+def tokenizer_counts(m):
+    """Calls per kind of the tokenizer in one generator step (TrainRunner forward, backward and the adaptive weight's two
+    last_layer_weight_grad calls): per ResidualUnit two convs, one squeeze_excite_residual, two data gradients and two
+    _conv_bwd; per attention-type stage (each side) the projections (3 for the linear attention, 2 otherwise), fc1, fc2 and
+    two rmsnorms; one conv per down- or up-sampler and one _conv_bwd per down-sampler (its weight and data gradient); conv_in
+    and conv_out, conv_in's _conv_bwd (weights only), conv_out's data gradient and three _conv_bwd through
+    _conv_bwd_padmode (the backward, and weights only for each last_layer_weight_grad); one quantize_cl and one batch-entropy
+    start / finish."""
+    n_ru = 2 * _n_residual_units(m)
+    n = dict(conv=2 + 2 * n_ru, se=n_ru, rmsnorm=0, dgrad=2 * n_ru + 1, conv_bwd=2 * n_ru + 1 + 3, padmode=3,
+             quantize=1, entropy=1)
+    for st in m.stages:
+        if st.kind in ("compress_space", "compress_time"):
+            n["conv"] += 2
+            n["conv_bwd"] += 1
+        elif st.kind in ("attend_space", "attend_time", "linear_attend_space"):
+            n["conv"] += 2 * ((3 if st.kind == "linear_attend_space" else 2) + 2)
+            n["rmsnorm"] += 4
+    return n
+
+
+def test_readme_train_tokenizer_call_kernels():
+    """Every tokenizer conv and data gradient of the README training step runs the kernel of the table: the slab kernel,
+    its down-space flavour for the three SpatialDownsample2x, and the CUDA-core conv only for conv_out's data gradient."""
+    eng = _engine()
+    calls, table, _ = tokenizer_table()
+    got = {}
+    for c in calls:
+        kw = dict(c["kw"])
+        res = kw.pop("res", False)
+        ta = eng._tc_args(c["x_shape"], c["pk"], res=torch.empty(1) if res else None, **kw)
+        got[call_key(c)] = eng.conv_kernel(ta, c["pk"])
+    assert got == {k: v[0] for k, v in table.items()}
+    assert {(c["net"], c["role"], c["block"]) for c in calls if c["kind"] == "simt"} == TOK_SIMT_BY_DESIGN
+    assert {c["block"] for c in calls if c["kind"] == "down"} == {"enc1", "enc3", "enc6"}
+
+
+def test_readme_train_tokenizer_call_counts():
+    """The count formulas on the README modules: 11 ResidualUnits per side, three space and two time samplers, one
+    linear, one space and one time attention stage."""
+    calls, table, m = tokenizer_table()
+    assert _n_residual_units(m) == 11 and m.time_padding == 3
+    n = tokenizer_counts(m)
+    assert n == dict(conv=82, se=22, rmsnorm=12, dgrad=45, conv_bwd=53, padmode=3, quantize=1, entropy=1), n
+    assert sum(not c["role"].startswith("dgrad") for c in calls) == n["conv"]
+    assert sum(c["role"].startswith("dgrad") for c in calls) == n["dgrad"]
+
+
+def test_tokenizer_replay_premises():
+    """The exact replays of tests/test_train_tokenizer_calls_gpu.py:
+      * the deepest wgmma GEMM is the 512-channel 3x3x3 conv and its data gradient, K = 13824, within the depth up to which
+        tests/test_bench_calls_cpu.py shows REPLAY_GRID exact (27 x 1024);
+      * the weight-gradient replays take operands in {-1, 0, 1}: at the deepest summation, 4 clips x 20 frames x 128^2
+        positions, every partial sum is an integer of magnitude below 2^24, exact in fp32 in any order;
+      * mv2_tc_slab_plan on 132 SMs: the 64-channel 128^2 unfused ResidualUnit convs and their data gradients plan 5120 tiles
+        on a grid of 132 (39 per CTA, rounded up), the 512-channel 16^2 calls at 5 frames 160 tiles on 132 CTAs, and every
+        slab call plans more tiles than CTAs;
+      * the schedule's last tile of every slab call has a predecessor on its CTA whose output region does not overlap it,
+        so a previous tile's accumulators left in place are visible there."""
+    calls, _, _ = tokenizer_table()
+    ks = {math.prod(c["pk"].k_tc) * c["pk"].Ci_tc for c in calls if c["kind"] != "simt"}
+    assert max(ks) == 27 * 512 <= 27 * 1024
+    assert {c["role"] for c in calls if c["kind"] != "simt" and math.prod(c["pk"].k_tc) * c["pk"].Ci_tc == max(ks)} == {
+        "conv3", "dgrad k333"}
+    assert CLIPS * (FRAMES + 3) * 128 * 128 == 1310720 < 2 ** 24
+    eng, lib = _engine(), Engine(None).lib
+    out = (C.c_int32 * 6)()
+    n_slab = 0
+    for c in calls:
+        if c["kind"] != "slab":
+            continue
+        kw = dict(c["kw"])
+        res = kw.pop("res", False)
+        ta = eng._tc_args(c["x_shape"], c["pk"], res=torch.empty(1) if res else None, **kw)
+        ta.x = ta.w = ta.y = 1
+        assert lib.mv2_tc_slab_plan(C.byref(ta), N_SM, out) == 0, lib.mv2_last_error()
+        mw, bn, total, grid = out[0], out[1], out[3], out[4]
+        assert total > grid == N_SM, (call_key(c), total, grid)
+        if c["role"] in ("conv3", "conv1", "dgrad k333", "dgrad k111") and c["x_shape"][1:] == (20, 128, 128, 64):
+            assert (total, grid, -(-total // grid)) == (5120, 132, 39), call_key(c)
+        if c["x_shape"][1:4] == (5, 16, 16) and c["pk"].Co_tc == 512:
+            assert (total, grid) == (160, 132), call_key(c)
+        tiles, k = [], 0
+        while True:
+            assert lib.mv2_tc_slab_tile(C.byref(ta), N_SM, last_cta(total, grid), k, out) == 0
+            if out[0] < 0:
+                break
+            tiles.append(tuple(out))
+            k += 1
+        assert len(tiles) >= 2 and tiles[-1][0] == total - 1, (call_key(c), tiles)
+        (_, b0, t0, h0, w0, n0), (_, b1, t1, h1, w1, n1) = tiles[-2:]
+        assert not (b0 == b1 and t0 == t1 and abs(h0 - h1) < 16 and abs(w0 - w1) < 8 * mw and abs(n0 - n1) < bn), (
+            call_key(c), tiles[-2:])
+        n_slab += 1
+    assert n_slab == sum(c["kind"] == "slab" for c in calls)

@@ -8,7 +8,7 @@ one warm-up step (so that the discriminator's and the VGG's packs and engines ex
 discriminator forward and backward with the image gradient, the VGG on the real and the reconstructed frames, the VGG's
 data gradient) and a discriminator step (two discriminator forwards and backwards, no gradient penalty).  The
 discriminator's widths are 3 -> 512 -> 512 ... 512 (its `dim` is the tokenizer's last stage width), six blocks, last map
-4 x 4.  The tokenizer's own engine is checked by tests/test_bench_calls_gpu.py and tests/test_conv_grad_gpu.py.
+4 x 4.  The tokenizer's own engine is checked by tests/test_train_tokenizer_calls_gpu.py.
 
 Part 1, real data.  The entry points of the discriminator's and the VGG's engine instances (conv, ingest_kwpack, rmsnorm,
 maxpool2x2, maxpool2x2_backward, mse) and the runners' TapeRunner._dgrad / DiscrRunner._dgrad_s2 are wrapped; each call
@@ -386,7 +386,7 @@ class _Recorder:
 
         def wrapped(runner, g, w, *args):
             eng = runner.eng
-            if id(eng) not in rec_.net:       # the tokenizer's own runner
+            if id(eng) not in rec_.net:       # the tokenizer's runner: tests/test_train_tokenizer_calls_gpu.py
                 return fn(runner, g, w, *args)
             n0 = len(rec_.guard[id(eng)].allocs)
             rec_.nested = inner = {}
