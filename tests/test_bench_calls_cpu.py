@@ -1,7 +1,8 @@
-"""Host-side premises of tests/test_bench_calls_gpu.py, without a GPU:
+"""Host-side premises of tests/test_bench_calls_gpu.py (and of tests/test_video_dgrad_gpu.py, which replays and plants
+defects the same way), without a GPU:
 
   * the exact-replay grid: at every GEMM depth K the benchmark's workloads run (README up to 27 x 512 and the GEGLU
-    widths, cfg4 up to 27 x 1024), every product and partial sum of grid operands is a multiple of 2^-8 below 2^14 (22
+    widths, cfg4 up to 27 x 1024) and the video's data gradient runs (init_dim x taps, up to 128 x 343), every product and partial sum of grid operands is a multiple of 2^-8 below 2^14 (22
     significant bits), so an fp32 accumulation is exact in any order, even with an adder that truncates.  Checked by the
     arithmetic and by fp32 sums in shuffled orders against float64;
   * the defect tile choice: the schedule's last tile (mv2_tc_slab_tile) has a predecessor on the same CTA whose output
@@ -15,11 +16,14 @@ import torch
 
 from bench import FRAMES, WORKLOADS
 from tests.test_bench_calls_gpu import REPLAY_GRID, last_cta
+from tests.test_slab_plan_narrow import VIDEO_DGRAD_SLAB, video_dgrad_args
 
 from magvit2_pytorch_b200 import VideoTokenizer, _lib
 from magvit2_pytorch_b200.engine import _round_up
 
 N_SM = 132
+# the depths of the video's data gradient: init_dim x the taps of conv_in (7x7x7, 5x5x5, 3x3x3) or of its first-frame conv
+VIDEO_DGRAD_DEPTHS = [64 * 343, 128 * 343, 64 * 125, 64 * 49, 64 * 27]
 
 
 def _gemm_depths(kw):
@@ -39,11 +43,15 @@ def _gemm_depths(kw):
     return m, sorted(ks)
 
 
-@pytest.mark.parametrize("workload", ["readme", "cfg4"])
+@pytest.mark.parametrize("workload", ["readme", "cfg4", "video_dgrad"])
 def test_replay_grid_is_exact_at_every_depth(workload):
     (nx, ex), (nw, ew), (nb, eb) = REPLAY_GRID["x"], REPLAY_GRID["w"], REPLAY_GRID["b"]
-    m, ks = _gemm_depths(WORKLOADS[workload]["kw"])
-    assert max(ks) == 27 * (1024 if workload == "cfg4" else 512)
+    if workload == "video_dgrad":
+        ks = VIDEO_DGRAD_DEPTHS
+        assert max(ks) == 128 * 343 > 27 * 1024
+    else:
+        _, ks = _gemm_depths(WORKLOADS[workload]["kw"])
+        assert max(ks) == 27 * (1024 if workload == "cfg4" else 512)
     # the arithmetic: products are multiples of 2^-(ex + ew); the bias is a multiple of 2^-eb with eb <= ex + ew; the
     # largest partial sum (all products of one sign at their largest, plus the bias) stays below 2^(22 - ex - ew)
     m_ = ex + ew
@@ -82,7 +90,10 @@ def _args(B, T, H, W, Ci, Co, k, pad, To):
 
 def _defect_shapes(workload):
     """(name, TcConvArgs) of the calls the replay plants its defects in: the fused RU (C = 64 and 128, at the first
-    encoder / last decoder resolution), the widest 3x3x3 EPI_PLAIN conv at each frame count, conv_out."""
+    encoder / last decoder resolution), the widest 3x3x3 EPI_PLAIN conv at each frame count, conv_out; for "video_dgrad"
+    every slab case of tests/test_video_dgrad_gpu.py."""
+    if workload == "video_dgrad":
+        return [(name, video_dgrad_args(*shape)) for name, (shape, _) in VIDEO_DGRAD_SLAB.items()]
     kw, clips = WORKLOADS[workload]["kw"], WORKLOADS[workload]["clips"] if workload == "readme" else 1
     s, top = kw["image_size"], kw["max_dim"]
     T = FRAMES + 3
@@ -93,7 +104,7 @@ def _defect_shapes(workload):
             ("conv_out", _args(clips, T, s, s, 64, 3, (3, 3, 3), (-1, 1, 1), FRAMES))]
 
 
-@pytest.mark.parametrize("workload", ["readme", "cfg4"])
+@pytest.mark.parametrize("workload", ["readme", "cfg4", "video_dgrad"])
 def test_defect_tile_has_a_disjoint_predecessor(workload):
     lib = _lib.load()
     out = (C.c_int32 * 6)()

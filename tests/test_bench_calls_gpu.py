@@ -109,14 +109,17 @@ def _last_tiles(lib, ta, n_sm):
 
 
 def _region(tile, plan, shape):
-    """Index of one tile's outputs in a (1, To, Ho, Wo, Co) accumulator."""
+    """Index of one tile's outputs in a (1, To, Ho, Wo, Co) accumulator.  The accumulators are channels-last whatever the
+    output's layout: a channels-first output (out_layout 1) compares with them permuted to (1, Co, To, Ho, Wo)."""
     _, _, t, h0, w0, n0 = tile
     _, To, Ho, Wo, Co = shape
     return (0, t, slice(h0, min(h0 + 16, Ho)), slice(w0, min(w0 + 8 * plan["mw"], Wo)), slice(n0, min(n0 + plan["bn"], Co)))
 
 
 def _acc64(x, w, pad, out_sp, tp):
-    """The conv's accumulators (no bias) as forward64 builds them: stride 1, tp leading output frames dropped."""
+    """The conv's accumulators (no bias) as forward64 builds them: stride 1, tp leading output frames dropped.  With tp None
+    the leading time pad may be negative: the transposed conv of a data gradient with its first -pad[0] output frames
+    cropped (output frame t reads input frames t - pad[0] ..)."""
     if tp is None:
         return _conv64(x, w, (1, 1, 1), pad, out_sp)
     kt = w.shape[2]
@@ -124,13 +127,18 @@ def _acc64(x, w, pad, out_sp, tp):
 
 
 def _defect_deltas(lib, ta, n_sm, xs, w, pad, out_sp, tp, plan):
-    """{defect: (clip, delta)} at the schedule's last tile: one ring stage (the last frame tap, the centre in-plane tap, input
-    channels 0..63) missing, and the previous tile's accumulators added.  xs(b) gives clip b's float64 operand."""
+    """{defect: (clip, delta)} at the schedule's last tile: one ring stage (the centre in-plane tap, input channels 0..63,
+    of the last frame tap that reads inside the clip at that tile's frame) missing, and the previous tile's accumulators
+    added.  xs(b) gives clip b's float64 operand.  Output frame t reads input frames t - pad[0] + d (pad[0] = kt - 1 - tp
+    for a conv with tp cropped frames): a causal conv's last frame reads its last frame at tap kt - 1, a data gradient's
+    (the transposed conv, pad[0] <= 0) only at tap 0."""
     prev, last = _last_tiles(lib, ta, n_sm)
     b = last[1]
     kt, kh, kw = w.shape[2:]
+    ft = min(kt - 1, xs(b).shape[1] - 1 - last[2] + pad[0])
+    assert ft >= 0, (last, pad)
     ws = torch.zeros_like(w)
-    ws[:, :64, kt - 1, kh // 2, kw // 2] = w[:, :64, kt - 1, kh // 2, kw // 2]
+    ws[:, :64, ft, kh // 2, kw // 2] = w[:, :64, ft, kh // 2, kw // 2]
     stage = _acc64(xs(b), ws, pad, out_sp, tp)
     r = _region(last, plan, stage.shape)
     d_stage = torch.zeros_like(stage)
@@ -141,7 +149,7 @@ def _defect_deltas(lib, ta, n_sm, xs, w, pad, out_sp, tp, plan):
     a, p_ = d_reset[r], acc_prev[rp]
     n = [min(u, v) for u, v in zip(a.shape, p_.shape)]
     d_reset[r][:n[0], :n[1], :n[2]] = p_[:n[0], :n[1], :n[2]]
-    assert (prev[2:] != last[2:] or prev[1] != b) and d_reset.abs().max() > 0
+    assert (prev[2:] != last[2:] or prev[1] != b) and d_reset.abs().max() > 0 and d_stage.abs().max() > 0
     return {"one ring stage missing": (b, d_stage), "previous tile's accumulators not reset": (b, d_reset)}
 
 

@@ -1,12 +1,12 @@
 """Differentiable encode / decode / decode_from_code_indices on the device: fp32 losses and gradients against the unmodified
-reference's autograd (tests/golden/*_io_grad.pt, oracle/make_io_grad_golden.py), bf16 against fp32, the video's data gradient
-against a float64 conv at its edges, and the no-grad path left as it was."""
+reference's autograd (tests/golden/*_io_grad.pt, oracle/make_io_grad_golden.py), bf16 against fp32, the video's gradient on the
+engine's kernels (its float64 checks are tests/test_video_dgrad_gpu.py), and the no-grad path left as it was."""
 import pytest
 import torch
 import torch.nn.functional as F
 
 from magvit2_pytorch_b200 import VideoTokenizer
-from magvit2_pytorch_b200.train import TrainRunner, _code_values
+from magvit2_pytorch_b200.train import _code_values
 from oracle.make_io_grad_golden import _cotangent
 from tests.test_io_grad_cpu import CASES, IO_GOLDENS
 from tests.test_oracle import grad_digest_close
@@ -114,47 +114,6 @@ def _dgrad_model(dtype, kin=(7, 7, 7)):
     m = VideoTokenizer(image_size=32, init_dim=64, codebook_size=1024, layers=("residual", "compress_time"),
                        input_conv_kernel_size=kin, use_gan=False, perceptual_loss_weight=0.)
     return m.cuda().to(dtype)
-
-
-@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
-@pytest.mark.parametrize("B,T,t_pad,H,W,first_frame", [
-    (1, 1, 0, 16, 16, False), (1, 1, 1, 16, 16, False), (2, 3, 1, 20, 27, False), (1, 2, 0, 13, 9, False),
-    (2, 1, 1, 21, 18, True), (1, 1, 0, 16, 40, True)])
-def test_video_dgrad_against_float64(dtype, B, T, t_pad, H, W, first_frame):
-    """TrainRunner._video_dgrad (the video's gradient through conv_in, or its 1 x 7 x 7 first-frame conv) against float64
-    autograd of the same conv: T = 1 and 1 + time_padding frames, frame sizes that are not tile multiples, B > 1.  bf16 runs
-    on the slab kernel's narrow N tile (conv_log), fp32 on the CUDA-core conv."""
-    _require_cuda()
-    torch.manual_seed(0)
-    m = _dgrad_model(dtype)
-    w = m.conv_in.conv.weight
-    k = (7, 7, 7)
-    if first_frame:
-        w = torch.randn(64, 3, 7, 7, device="cuda").to(dtype) * 0.05
-        k = (1, 7, 7)
-    eng = m.engine
-    Ti = T + t_pad
-    g = torch.randn(B, Ti, H, W, 64, device="cuda").to(dtype)
-    runner = TrainRunner(m)
-    eng.conv_log = []
-    calls0 = eng.simt_conv_calls
-    with torch.no_grad():
-        got = runner._video_dgrad(g, w, k, t_pad)
-    torch.cuda.synchronize()
-    # float64: y = conv(video behind t_pad zero frames, causal time pad, symmetric H / W pad); d/d video of (y * g).sum()
-    v = torch.zeros(B, 3, T, H, W, dtype=torch.float64, device="cuda", requires_grad=True)
-    w64 = w.double().reshape(64, 3, *k)
-    x = F.pad(v, (k[2] // 2, k[2] // 2, k[1] // 2, k[1] // 2, t_pad + k[0] - 1, 0))
-    (F.conv3d(x, w64) * g.double().permute(0, 4, 1, 2, 3)).sum().backward()
-    ref = v.grad
-    assert got.shape == ref.shape
-    err = float((got.double() - ref).abs().max()) / float(ref.abs().max())
-    assert err < (1e-5 if dtype == torch.float32 else 1e-2), err
-    if dtype == torch.bfloat16:
-        recs = [r for r in eng.conv_log if r["Co"] == 3 and r["k"] == k]
-        assert recs and all(r["kind"] == "slab" for r in recs), eng.conv_log
-    else:
-        assert eng.simt_conv_calls > calls0
 
 
 def test_video_gradient_runs_on_the_engine_kernels():

@@ -78,7 +78,7 @@ import torch.nn.functional as F
 
 import synth_data
 from tests.test_bench_calls_gpu import _Recorder as _BenchRecorder
-from tests.test_bench_calls_gpu import _acc64, _defect_deltas, _grid, _last_tiles, _lib_plan, _region, _replay_key
+from tests.test_bench_calls_gpu import _defect_deltas, _grid, _lib_plan, _replay_key
 from tests.test_conv_forward_gpu import _ran, forward64
 from tests.test_conv_grad_gpu import C_OF, _conv64_grads, _dgrad64, _gamma
 from tests.test_simt_ops_gpu import U, _check, _lfq_entropy64, _rejects
@@ -201,21 +201,9 @@ class _Recorder(_BenchRecorder):
             rec["rejected"] = self._defects(rec, xs, w, b, y, kw, res)
 
     def _defects(self, rec, xs, w, b, y, kw, res):
-        """_defect_deltas at the schedule's last tile, each rejected by the exact bound."""
+        """_defect_deltas at the schedule's last tile, each rejected by the exact bound.  A data gradient reads frames
+        t .. t + kt - 1, so at the clip's last frame its missing ring stage is frame tap 0's."""
         deltas = _defect_deltas(self.lib, rec["ta"], self.n_sm, xs, w, kw["pad"], kw["out_sp"], kw.get("tp"), rec["plan"])
-        kt, kh, kw_ = w.shape[2:]
-        if kw["pad"][0] == 0 and kt > 1:
-            # a data gradient reads frames t .. t + kt - 1: at the clip's last frame only frame tap 0 is in range, so the
-            # missing ring stage is that tap's (the centre in-plane tap, input channels 0..63)
-            _, last = _last_tiles(self.lib, rec["ta"], self.n_sm)
-            ws = torch.zeros_like(w)
-            ws[:, :64, 0, kh // 2, kw_ // 2] = w[:, :64, 0, kh // 2, kw_ // 2]
-            stage = _acc64(xs(last[1]), ws, kw["pad"], kw["out_sp"], kw.get("tp"))
-            r = _region(last, rec["plan"], stage.shape)
-            d = torch.zeros_like(stage)
-            d[r] = -stage[r]
-            assert d.abs().max() > 0
-            deltas[STAGE] = (last[1], d)
         for defect, (i, delta) in deltas.items():
             r = None if res is None else res[i:i + 1].double()
             ref, acc = forward64(xs(i), w, b, None, r, dtype=BF, exact=True, **kw)
