@@ -45,13 +45,18 @@ def _gemm_depths(kw):
 
 @pytest.mark.parametrize("workload", ["readme", "cfg4", "video_dgrad"])
 def test_replay_grid_is_exact_at_every_depth(workload):
-    (nx, ex), (nw, ew), (nb, eb) = REPLAY_GRID["x"], REPLAY_GRID["w"], REPLAY_GRID["b"]
     if workload == "video_dgrad":
         ks = VIDEO_DGRAD_DEPTHS
         assert max(ks) == 128 * 343 > 27 * 1024
     else:
         _, ks = _gemm_depths(WORKLOADS[workload]["kw"])
         assert max(ks) == 27 * (1024 if workload == "cfg4" else 512)
+    assert_replay_grid_exact(ks)
+
+
+def assert_replay_grid_exact(ks):
+    """REPLAY_GRID operands accumulate exactly in fp32, in any order, at every GEMM depth in ks."""
+    (nx, ex), (nw, ew), (nb, eb) = REPLAY_GRID["x"], REPLAY_GRID["w"], REPLAY_GRID["b"]
     # the arithmetic: products are multiples of 2^-(ex + ew); the bias is a multiple of 2^-eb with eb <= ex + ew; the
     # largest partial sum (all products of one sign at their largest, plus the bias) stays below 2^(22 - ex - ew)
     m_ = ex + ew

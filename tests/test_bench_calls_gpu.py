@@ -56,8 +56,9 @@ from magvit2_pytorch_b200.engine import pack_conv, pack_conv_down_space, pack_co
 pytestmark = pytest.mark.gpu
 
 BF = torch.bfloat16
-# the replay grid: x, residual and video in {-8..8} / 2^2, weights in {-8..8} / 2^6, biases in {-64..64} / 2^8
-REPLAY_GRID = dict(x=(8, 2), w=(8, 6), b=(64, 8))
+# the replay grid: x, residual and video in {-8..8} / 2^2, weights in {-8..8} / 2^6, biases in {-64..64} / 2^8; a conv's
+# per-clip oscale (the Conv3DMod's demodulation) in {1..8} / 2^3
+REPLAY_GRID = dict(x=(8, 2), w=(8, 6), b=(64, 8), os=(8, 3))
 FLAVOURS = ("ru_c64", "ru_c128", "plain", "plain_res", "geglu", "down", "time_stride", "shuffle", "ragged_cf", "conv_in")
 _EAGER = {}          # workload -> (codes, reconstruction) of the checked eager step, for the launch-mode test
 
@@ -193,14 +194,15 @@ class _Recorder:
         what = f"call {len(self.calls)}: conv {kind} x {tuple(x.shape)} -> {tuple(y.shape)}"
         self._done(n0, what)
         rec = self._conv_record(x, pk, kw, y, kind)
-        self._check_conv(rec, x, y, what, res=kw.get("res"), video=self.ingest[0] if rec["conv_in"] else None)
+        self._check_conv(rec, x, y, what, res=kw.get("res"), video=self.ingest[0] if rec["conv_in"] else None,
+                         os=kw.get("oscale"))
         self.calls.append(rec)
         return y
 
     def _conv_record(self, x, pk, kw, y, kind):
-        assert kw.get("oscale") is None and not kw.get("token_shift") and kw.get("ss") is None
+        assert not kw.get("token_shift") and kw.get("ss") is None
         kt, kh, kw_ = pk.k_tc or pk.k
-        d = dict(op="conv", kind=kind, pk=pk, x_shape=tuple(x.shape), y_shape=tuple(y.shape),
+        d = dict(op="conv", kind=kind, pk=pk, x_shape=tuple(x.shape), y_shape=tuple(y.shape), os=kw.get("oscale") is not None,
                  stride=tuple(kw.get("stride", (1, 1, 1))), act=kw.get("act", ACT_NONE),
                  shuffle=kw.get("shuffle", SHUFFLE_NONE), res=kw.get("res") is not None, out_cf=bool(kw.get("out_cf")),
                  pad=tuple(kw.get("pad") or (kt - 1, kh // 2, kw_ // 2)),
@@ -209,7 +211,7 @@ class _Recorder:
         if d["conv_in"]:
             d["t_pad"] = self.ingest[1]
         ta = self.eng._tc_args(x, pk, d["stride"], d["pad"], d["out_sp"], d["act"], d["shuffle"], d["out_cf"],
-                               res=kw.get("res"), y=y)
+                               res=kw.get("res"), y=y, oscale=kw.get("oscale"))
         d["ta"] = ta
         if kind == "slab":
             d["plan"] = _lib_plan(self.lib, ta, self.n_sm)
@@ -249,9 +251,12 @@ class _Recorder:
         return xs, w, b, dict(kern=rec["kind"], stride=rec["stride"], pad=rec["pad"], out_sp=rec["out_sp"], K=K,
                               act=rec["act"], mode=pk.epi_mode, shuffle=rec["shuffle"], tp=tp)
 
-    def _check_conv(self, rec, x, y, what, exact=False, w=None, b=None, res=None, video=None, defects=False):
+    def _check_conv(self, rec, x, y, what, exact=False, w=None, b=None, res=None, video=None, defects=False, os=None):
+        """os: the call's per-clip oscale (B, Co), or None.  A call on the CUDA-core conv fails unless its record names it
+        as meant to run there (simt_ok)."""
         pk, B = rec["pk"], rec["x_shape"][0]
-        assert rec["kind"] != "simt", f"{what}: a bf16 conv fell back to the CUDA-core kernel"
+        assert rec["kind"] != "simt" or rec.get("simt_ok"), f"{what}: a bf16 conv fell back to the CUDA-core kernel"
+        osc = (lambda i: None) if os is None else (lambda i: os[i:i + 1].double())
         if pk.epi_mode == 1:      # fc1 + GEGLU; the hidden channels pack_ff pads in are exactly zero
             w1 = pk.w.double()[0].T if w is None else w
             b1 = pk.bias.double() if b is None else b
@@ -264,14 +269,14 @@ class _Recorder:
         xs, w, b, kw = self._conv_ref_args(rec, video if rec["conv_in"] else x, w, b)
         for i in range(B):
             r = None if res is None else res[i:i + 1].double()
-            ref, acc = forward64(xs(i), w, b, None, r, dtype=BF, exact=exact, **kw)
+            ref, acc = forward64(xs(i), w, b, osc(i), r, dtype=BF, exact=exact, **kw)
             _check(y[i:i + 1], ref, BF, acc, f"{what}, clip {i}")
             del ref
         if defects:
             for defect, (i, delta) in _defect_deltas(self.lib, rec["ta"], self.n_sm, xs, w, kw["pad"], kw["out_sp"],
                                                      kw["tp"], rec["plan"]).items():
-                ref, acc = forward64(xs(i), w, b, None, None, dtype=BF, exact=True, **kw)
-                wrong, _ = forward64(xs(i), w, b, None, None, dtype=BF, exact=True, delta=delta, **kw)
+                ref, acc = forward64(xs(i), w, b, osc(i), None, dtype=BF, exact=True, **kw)
+                wrong, _ = forward64(xs(i), w, b, osc(i), None, dtype=BF, exact=True, delta=delta, **kw)
                 _rejects(y[i:i + 1], wrong, BF, acc, f"{what}: {defect}")
                 rec.setdefault("rejected", []).append(defect)
 
@@ -448,12 +453,17 @@ class _Recorder:
         if rec["res"]:
             res = _grid(rec["y_shape"], "x", gen)
             kw["res"] = res.to(BF).contiguous()
+        os = None
+        if rec.get("os"):         # a per-clip oscale on its own dyadic grid
+            n, e = REPLAY_GRID["os"]
+            os = torch.randint(1, n + 1, (x_shape[0], pk.Co), generator=gen, device="cuda").double() * 2.0 ** -e
+            kw["oscale"] = os.float()
         kind2, y = _ran(self.eng, lambda: self.orig["conv"](x.to(BF).contiguous(), pk2, **kw))
         what = f"replay of {rec['flavour']} conv x {x_shape}"
         assert kind2 == kind, f"{what}: ran {kind2}, the recorded call ran {kind}"
         self._done(n0, what)
         rec2 = dict(rec, pk=pk2)
-        self._check_conv(rec2, x, y, what, exact=True, w=w, b=b, res=res, video=video, defects=defects)
+        self._check_conv(rec2, x, y, what, exact=True, w=w, b=b, res=res, video=video, defects=defects, os=os)
         rec.setdefault("rejected", []).extend(rec2.get("rejected", []))
 
     def _replay_ru(self, rec, gen, defects):

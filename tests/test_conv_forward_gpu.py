@@ -239,7 +239,8 @@ def forward64(x, w, b, os, r, *, kern, stride, pad, out_sp, K, act=NONE, mode=0,
     (Co,Ci,kt,kh,kw) in the reference's channel order, b (Co,), per-clip oscale `os` (B,Co) or None, residual r or None;
     `pad` / `out_sp` the call's leading pad and output extent before any shuffle, K the packed GEMM depth, `tp` the
     channels-first conv_out's dropped leading frames.  `wrong` names a defect to build into the reference.  `exact`: the
-    accumulation and the bias add are exact (operands on a dyadic grid), so only the epilogue's errors are allowed;
+    accumulation and the bias add are exact (operands on a dyadic grid), so only the epilogue's errors are allowed (with
+    oscale, the oscale product and the bias add after it round);
     `delta` (B,To,Ho,Wo,Co) is added to the accumulators before the epilogue."""
     kt = w.shape[2]
     if tshift:                    # TokenShift (M:250-254): channels [ceil(C / 2), C) delayed by one frame
@@ -260,7 +261,6 @@ def forward64(x, w, b, os, r, *, kern, stride, pad, out_sp, K, act=NONE, mode=0,
     if delta is not None:
         acc = acc + delta
     if os is not None:
-        assert not exact, "a per-clip oscale product is rounded: no exact accumulation"
         osv = os.clone()
         if wrong == "oscale of clip 0 used for clip 1":
             osv[1:] = osv[0]
@@ -275,7 +275,10 @@ def forward64(x, w, b, os, r, *, kern, stride, pad, out_sp, K, act=NONE, mode=0,
         z = acc + b
     if wrong == "bias dropped":
         z = z - b
-    e = torch.zeros_like(S) if exact else gam * S + 3 * U * (S + b.abs())
+    if exact:                     # with oscale the product and the bias add still round: 3 u (S |os| + |b|) covers both
+        e = torch.zeros_like(S) if os is None else 3 * U * (S + b.abs())
+    else:
+        e = gam * S + 3 * U * (S + b.abs())
     if wrong == "bias added after the activation":
         v = ACT64[act](z - b) + b
     else:

@@ -342,6 +342,20 @@ def _proj_err(x, prm):
     return (-(-C_ // 32) + 6) * U * (x.abs() @ prm["win"].abs().T + prm["bin"].abs())
 
 
+def lfq_presign64(p64, err, nc, d, spherical):
+    """(reference, allowance) of the LFQ kernel's fp32 pre-sign values from the float64 projection p64 (N, nc d) and its
+    error bound err: p64 itself, or per codebook L2-normalised when spherical (a zero vector stays zero)."""
+    if not spherical:
+        return p64, err
+    N = p64.shape[0]
+    pc = p64.reshape(N, nc, d)
+    nrm = pc.norm(dim=-1, keepdim=True)
+    pn = torch.where(nrm > 0, pc / nrm.clamp(min=1e-300), torch.zeros_like(pc))
+    en = torch.where(nrm > 0, 2 * err.reshape(N, nc, d).max(dim=-1, keepdim=True).values * d ** 0.5 / nrm.clamp(min=1e-300)
+                     + (d + 8) * U, torch.zeros_like(nrm))
+    return pn.reshape(N, nc * d), en.expand(N, nc, d).reshape(N, nc * d)
+
+
 LFQ_CASES = [
     # code, d, nc, spherical, clamp, zero bias, C
     (BF16, 16, 1, 0, 10.0, 1, 40), (F32, 16, 1, 1, 10.0, 0, 40),
@@ -389,15 +403,8 @@ def test_lfq(code, d, nc, sph, clamp, zb, C_):
         rev |= ((idx_ref >> j) & 1) << (d - 1 - j)
     assert (idx != rev).sum().item() > ambiguous.sum().item()
     # pre-sign values: fp32 projection (+ tanh clamp), per codebook L2-normalised when spherical
-    if sph:
-        pc = p64.reshape(N, nc, d)
-        nrm = pc.norm(dim=-1, keepdim=True)
-        pn = torch.where(nrm > 0, pc / nrm.clamp(min=1e-300), torch.zeros_like(pc))
-        en = torch.where(nrm > 0, 2 * err.reshape(N, nc, d).max(dim=-1, keepdim=True).values * d ** 0.5 / nrm.clamp(min=1e-300)
-                         + (d + 8) * U, torch.zeros_like(nrm))
-        _check(pre, pn.reshape(N, D), torch.float32, en.expand(N, nc, d).reshape(N, D), "lfq presign (spherical)")
-    else:
-        _check(pre, p64, torch.float32, err, "lfq presign")
+    pre_ref, pre_acc = lfq_presign64(p64, err, nc, d, sph)
+    _check(pre, pre_ref, torch.float32, pre_acc, "lfq presign" + (" (spherical)" if sph else ""))
     # quantized: bout + Wout (+-1) as a D-term fp32 fma chain, rounded once
     acc = (D + 1) * U * (prm["wout"].abs().sum(dim=1) + prm["bout"].abs())
     ok = ~ambiguous.any(dim=1)
@@ -423,6 +430,31 @@ def test_lfq(code, d, nc, sph, clamp, zb, C_):
         outs.append(qd)
     assert torch.equal(outs[0], outs[1])
     _check(outs[0], want, DT[code], acc.expand(M, C_), "lfq decode")
+
+
+def fsq64(x64, prm, levels, nc):
+    """float64 FSQ of tokens x64 (N, C) with projections prm (oracle.restated.fsq_quantize) and the kernel's allowances:
+    dict(q, idx (N, nc), bounded (N, nc d), err: the allowance of the fp32 bounded values, ambiguous (N, nc): a bounded
+    value within err of a .5 rounding point (its digit may round either way), reversed: the indices with the mixed-radix
+    digits in reverse order (first dimension most significant), acc_q: the allowance of the quantized output per channel
+    before its rounding)."""
+    N, C_ = x64.shape
+    d = len(levels)
+    D = d * nc
+    sd = {k: v.cpu() for k, v in _quant_sd(prm, d).items()}        # R's FSQ constants are CPU tensors
+    q_ref, idx_ref, b_ref = R.fsq_quantize(x64.T.reshape(1, C_, N, 1, 1).cpu(), sd, levels, nc)
+    q_ref, idx_ref, b_ref = q_ref.reshape(C_, N).T.cuda(), idx_ref.reshape(N, nc).cuda(), b_ref.reshape(N, D).cuda()
+    # bounded = tanh(z + shift) * half_l - offset: the projection error, scaled by half_l, plus a few roundings
+    half_l = torch.tensor([(l - 1) * 1.001 / 2 for l in levels] * nc, device="cuda", dtype=torch.float64)
+    lin = x64 @ prm["win"].T + prm["bin"]
+    err = half_l * (_proj_err(x64, prm) + 8 * U * (1 + lin.abs()))
+    frac = b_ref - torch.floor(b_ref)
+    ambiguous = ((frac - 0.5).abs() < err).reshape(N, nc, d).any(dim=-1)
+    digits = torch.round(b_ref).reshape(N, nc, d) + torch.tensor([l // 2 for l in levels], device="cuda")
+    rbasis = [math.prod(levels[j + 1:]) for j in range(d)]
+    rev = (digits * torch.tensor(rbasis, device="cuda", dtype=torch.float64)).sum(dim=-1).to(torch.int32)
+    acc = (D + 2) * U * (prm["wout"].abs().sum(dim=1) + prm["bout"].abs())
+    return dict(q=q_ref, idx=idx_ref, bounded=b_ref, err=err, ambiguous=ambiguous, reversed=rev, acc_q=acc)
 
 
 FSQ_CASES = [
@@ -453,26 +485,17 @@ def test_fsq(code, levels, nc):
     _ok(lib.mv2_fsq_forward(x.data_ptr(), code, N, C_, d, nc, lv, w["win"].data_ptr(), w["bin"].data_ptr(),
                             w["wout"].data_ptr(), w["bout"].data_ptr(), idx.data_ptr(), q.data_ptr(), bnd.data_ptr(), _st()),
         "mv2_fsq_forward")
+    f = fsq64(x64, prm, levels, nc)
     sd = {k: v.cpu() for k, v in _quant_sd(prm, d).items()}        # R's FSQ constants are CPU tensors
-    q_ref, idx_ref, b_ref = R.fsq_quantize(x64.T.reshape(1, C_, N, 1, 1).cpu(), sd, levels, nc)
-    q_ref, idx_ref, b_ref = q_ref.reshape(C_, N).T.cuda(), idx_ref.reshape(N, nc).cuda(), b_ref.reshape(N, D).cuda()
-    # bounded = tanh(z + shift) * half_l - offset: the projection error, scaled by half_l, plus a few roundings
-    half_l = torch.tensor([(l - 1) * 1.001 / 2 for l in levels] * nc, device="cuda", dtype=torch.float64)
-    lin = x64 @ prm["win"].T + prm["bin"]
-    err = half_l * (_proj_err(x64, prm) + 8 * U * (1 + lin.abs()))
-    _check(bnd, b_ref, torch.float32, err, "fsq bounded")
-    frac = b_ref - torch.floor(b_ref)
-    ambiguous = ((frac - 0.5).abs() < err).reshape(N, nc, d).any(dim=-1)    # within fp32 noise of a .5 rounding point
+    _check(bnd, f["bounded"], torch.float32, f["err"], "fsq bounded")
+    ambiguous = f["ambiguous"]
     assert ambiguous.sum().item() <= max(2, N // 100)
-    assert torch.equal(idx[~ambiguous], idx_ref[~ambiguous])
+    assert torch.equal(idx[~ambiguous], f["idx"][~ambiguous])
     # the bound rejects the mixed-radix digits taken in reversed order (first dimension most significant)
-    digits = torch.round(b_ref).reshape(N, nc, d) + torch.tensor([l // 2 for l in levels], device="cuda")
-    rbasis = [math.prod(levels[j + 1:]) for j in range(d)]
-    rev = (digits * torch.tensor(rbasis, device="cuda", dtype=torch.float64)).sum(dim=-1).to(torch.int32)
-    assert (idx != rev).sum().item() > ambiguous.sum().item()
-    acc = (D + 2) * U * (prm["wout"].abs().sum(dim=1) + prm["bout"].abs())
+    assert (idx != f["reversed"]).sum().item() > ambiguous.sum().item()
+    acc = f["acc_q"]
     ok = ~ambiguous.any(dim=1)
-    _check(q[ok], q_ref[ok], DT[code], acc.expand(N, C_)[ok], "fsq quantized")
+    _check(q[ok], f["q"][ok], DT[code], acc.expand(N, C_)[ok], "fsq quantized")
     for is64, ii in ((0, idx), (1, idx.long().contiguous())):
         qd = torch.empty_like(q)
         _ok(lib.mv2_fsq_decode(ii.data_ptr(), is64, N, C_, d, nc, lv, w["wout"].data_ptr(), w["bout"].data_ptr(), qd.data_ptr(),
@@ -599,6 +622,25 @@ def test_mse(ad, bd, n):
 # ------------------------------------------------------------------------------------------------------------------
 # gateloop scan
 # ------------------------------------------------------------------------------------------------------------------
+def gateloop64(qkva, res):
+    """float64 gateloop recurrence of mv2_gateloop_scan on (B, T, P, 3C) qkva and (B, T, P, C) res: s_t = sigmoid(a_t) s_{t-1}
+    + kv_t, out_t = q_t s_t + res_t.  Returns (reference, allowance, wrong): the allowance carries a running bound on the
+    fp32 state error; `wrong` takes each output from the state before that step's update."""
+    C_, T = res.shape[-1], res.shape[1]
+    q, kv, sg = qkva[..., :C_], qkva[..., C_:2 * C_], torch.sigmoid(qkva[..., 2 * C_:])
+    s = torch.zeros_like(q[:, 0])
+    mag, err = torch.zeros_like(s), torch.zeros_like(s)
+    ref, acc, wrong = torch.empty_like(res), torch.empty_like(res), torch.empty_like(res)
+    for t in range(T):
+        wrong[:, t] = q[:, t] * s + res[:, t]
+        s = sg[:, t] * s + kv[:, t]
+        mag = sg[:, t] * mag + kv[:, t].abs()
+        err = sg[:, t] * err + 6 * U * mag                     # sigmoid (expf, add, divide) and the fma, per step
+        ref[:, t] = q[:, t] * s + res[:, t]
+        acc[:, t] = q[:, t].abs() * err + U * ((q[:, t] * s).abs() + res[:, t].abs())
+    return ref, acc, wrong
+
+
 GL_CASES = [(F32, 2, 1, 37, 7), (BF16, 1, 1, 45, 13), (F32, 2, 17, 100, 24), (BF16, 1, 17, 45, 13), (BF16, 2, 5, 300, 40)]
 
 
@@ -614,18 +656,7 @@ def test_gateloop_scan(code, B, T, P, C_):
     res = _randn((B, T, P, C_), g)
     qd, rd, out = _dev(qkva, code), _dev(res, code), torch.empty((B, T, P, C_), device="cuda", dtype=DT[code])
     _ok(_lib().mv2_gateloop_scan(qd.data_ptr(), rd.data_ptr(), out.data_ptr(), code, B, T, P, C_, _st()), "mv2_gateloop_scan")
-    q, kv, sg = qkva[..., :C_], qkva[..., C_:2 * C_], torch.sigmoid(qkva[..., 2 * C_:])
-    # s_t = sigmoid(a_t) s_{t-1} + kv_t, out_t = q_t s_t + res_t, with a running bound on the fp32 state error
-    s = torch.zeros_like(q[:, 0])
-    mag, err = torch.zeros_like(s), torch.zeros_like(s)
-    ref, acc, wrong = torch.empty_like(res), torch.empty_like(res), torch.empty_like(res)
-    for t in range(T):
-        wrong[:, t] = q[:, t] * s + res[:, t]                  # perturbed: the state before this step's update
-        s = sg[:, t] * s + kv[:, t]
-        mag = sg[:, t] * mag + kv[:, t].abs()
-        err = sg[:, t] * err + 6 * U * mag                     # sigmoid (expf, add, divide) and the fma, per step
-        ref[:, t] = q[:, t] * s + res[:, t]
-        acc[:, t] = q[:, t].abs() * err + U * ((q[:, t] * s).abs() + res[:, t].abs())
+    ref, acc, wrong = gateloop64(qkva, res)
     _check(out, ref, DT[code], acc, "gateloop")
     if T > 1:
         _rejects(out, wrong, DT[code], acc, "gateloop with the output taken from the previous state")
@@ -721,6 +752,33 @@ def test_pad_cl(mode, shape, pad, code):
 ACTS = {0: lambda v: v, 1: F.elu, 2: F.silu, 3: lambda v: F.leaky_relu(v, 0.1)}
 
 
+def dense_small64(x, w, b, act):
+    """(reference, allowance, pre-activation) of mv2_dense_small: act(x w^T + b) in float64 (b may be None); the
+    allowance covers the lane fma chain, shuffle tree and bias, then the activation (Lipschitz <= 1.1, a few ulp of libm)."""
+    K = x.shape[1]
+    lin = x @ w.T + (0 if b is None else b)
+    ref = ACTS[act](lin)
+    acc = 1.1 * (-(-K // 32) + 7) * U * ((x.abs() @ w.abs().T) + (0 if b is None else b.abs())) + 4 * U * ref.abs()
+    return ref, acc, lin
+
+
+def mod_prepare64(cond, S, eps):
+    """(scale_in, inv_norm, inv_norm allowance, the wrong inv_norm with eps on the norm) of mv2_mod_prepare in float64 from
+    its fp32 inputs: scale_in = cond + 1 (one fp32 rounding), inv_norm = rsqrt(max((cond + 1)^2 . S, eps)); the allowance
+    covers (cond + 1)^2, the fma chain relative to a positive sum, and rsqrtf."""
+    ssum = ((cond + 1) ** 2) @ S.T
+    ref = torch.rsqrt(ssum.clamp(min=eps))
+    acc = (-(-cond.shape[1] // 32) + 12) * U * ref
+    return cond + 1, ref, acc, 1 / ssum.sqrt().clamp(min=eps)
+
+
+def scale_channels64(x, sc, dtype):
+    """(reference, allowance) of mv2_scale_channels: x (B, P, C) times the per-clip channel scale sc (B, C), one fp32
+    product rounded to dtype (the fp32 output rounds exactly once, the bf16 one after the fp32 product)."""
+    ref = x * sc[:, None, :]
+    return ref, (U * ref.abs() if dtype == torch.bfloat16 else 0.0)
+
+
 @pytest.mark.parametrize("bias", [True, False], ids=["bias", "nobias"])
 @pytest.mark.parametrize("act", [0, 1, 2, 3], ids=["none", "elu", "silu", "leaky"])
 def test_dense_small(act, bias):
@@ -732,10 +790,7 @@ def test_dense_small(act, bias):
     x32, w32, b32 = _f32(x), _f32(w), (_f32(b) if bias else None)
     _ok(_lib().mv2_dense_small(x32.data_ptr(), w32.data_ptr(), b32.data_ptr() if bias else None, y.data_ptr(), B, K, N, act,
                                _st()), "mv2_dense_small")
-    lin = x @ w.T + (b if bias else 0)
-    ref = ACTS[act](lin)
-    # lane fma chain + shuffle tree + bias, then the activation (Lipschitz <= 1.1, a few ulp of libm)
-    acc = 1.1 * (-(-K // 32) + 7) * U * ((x.abs() @ w.abs().T) + (b.abs() if bias else 0)) + 4 * U * ref.abs()
+    ref, acc, lin = dense_small64(x, w, b, act)
     _check(y, ref, torch.float32, acc, "dense_small")
     if act == 3:
         _rejects(y, F.leaky_relu(lin, 0.01), torch.float32, acc, "dense_small with torch's default leaky slope")
@@ -752,13 +807,11 @@ def test_mod_prepare():
     c32, s32 = _f32(cond), _f32(S)
     _ok(_lib().mv2_mod_prepare(c32.data_ptr(), s32.data_ptr(), eps, si.data_ptr(), inv.data_ptr(), B, Ci, Co, _st()),
         "mv2_mod_prepare")
-    _check(si, cond + 1, torch.float32, 0.0, "mod_prepare scale_in")
-    ssum = ((cond + 1) ** 2) @ S.T
-    ref = torch.rsqrt(ssum.clamp(min=eps))
-    acc = (-(-Ci // 32) + 12) * U * ref                  # (cond + 1)^2 and the fma chain relative to a positive sum; rsqrtf
+    si_ref, ref, acc, wrong = mod_prepare64(cond, S, eps)
+    _check(si, si_ref, torch.float32, 0.0, "mod_prepare scale_in")
     _check(inv, ref, torch.float32, acc, "mod_prepare inv_norm")
     assert abs(inv[0, 5].item() - eps ** -0.5) <= 8 * U * eps ** -0.5
-    _rejects(inv, 1 / ssum.sqrt().clamp(min=eps), torch.float32, acc, "mod_prepare with eps on the norm")
+    _rejects(inv, wrong, torch.float32, acc, "mod_prepare with eps on the norm")
 
 
 @pytest.mark.parametrize("code", [F32, BF16], ids=["f32", "bf16"])
@@ -770,8 +823,7 @@ def test_scale_channels_above_grid_cap(code):
     sc = _randn((B, C_), g)
     xd, s32, out = _dev(x, code), _f32(sc), torch.empty((B, Pn, C_), device="cuda", dtype=DT[code])
     _ok(_lib().mv2_scale_channels(xd.data_ptr(), s32.data_ptr(), out.data_ptr(), code, B, Pn, C_, _st()), "mv2_scale_channels")
-    ref = x * sc[:, None, :]
-    acc = U * ref.abs() if code == BF16 else 0.0
+    ref, acc = scale_channels64(x, sc, DT[code])
     _check(out, ref, DT[code], acc, "scale_channels")
     _rejects(out, x * sc[:1, None, :], DT[code], acc, "scale_channels with clip 0's scale everywhere")
 

@@ -193,8 +193,8 @@ class _Recorder(_BenchRecorder):
         self._table(self.calls[n], role, x.shape, pk.Co)
         return y
 
-    def _check_conv(self, rec, x, y, what, exact=False, w=None, b=None, res=None, video=None, defects=False):
-        super()._check_conv(rec, x, y, what, exact=exact, w=w, b=b, res=res, video=video)
+    def _check_conv(self, rec, x, y, what, exact=False, w=None, b=None, res=None, video=None, defects=False, os=None):
+        super()._check_conv(rec, x, y, what, exact=exact, w=w, b=b, res=res, video=video, os=os)
         if defects and rec["kind"] == "slab" and rec["pk"].epi_mode == 0 and rec["shuffle"] == SHUFFLE_NONE and \
                 not rec["conv_in"]:
             xs, w, b, kw = self._conv_ref_args(rec, video if rec["conv_in"] else x, w, b)
