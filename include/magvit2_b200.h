@@ -53,6 +53,11 @@ enum {
 
 int mv2_abi_version(void);
 const char* mv2_last_error(void);
+/* Number of kernels the library has launched from the calling thread (thread-local, from 0).  A kernel counts when its
+ * launch is accepted, including a launch into a stream under graph capture; a call refused by its argument checks adds
+ * nothing.  Memsets and copies are not kernels and are not counted: the copy of mv2_copy_frames and the zero-filled
+ * t_pad frames of mv2_to_channels_last. */
+uint64_t mv2_launch_count(void);
 /* Compute capability of the current device as major*10+minor (90 on H100), <0 on error. */
 int mv2_device_arch(void);
 /* The frames in front of a streamed chunk that the conv entry points read (see "streaming" below); NULL: none. */

@@ -84,6 +84,7 @@ _VP, _I, _I64, _F, _SZ = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_size_t
 SIGNATURES = {
     "mv2_abi_version": (_I, []),
     "mv2_last_error": (C.c_char_p, []),
+    "mv2_launch_count": (C.c_uint64, []),
     "mv2_device_arch": (_I, []),
     "mv2_set_pdl": (_I, [_I]),
     "mv2_to_channels_last": (_I, [_VP, _I, _VP, _I, _I, _I, _I, _I, _I, _I, _VP]),

@@ -127,6 +127,8 @@ struct PerDeviceOnce {
 // after, so the next kernel's CTAs move in as this kernel's CTAs retire.  Without the launch attribute both
 // instructions are no-ops.  mv2_set_pdl(1) turns the attribute on for all launches.
 extern int g_pdl;
+// kernels launched from this thread (mv2_launch_count)
+extern thread_local uint64_t g_launches;
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
@@ -142,7 +144,8 @@ static inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   attr.val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = &attr;
   cfg.numAttrs = g_pdl ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);   // errors surface through MV2_CHECK_LAUNCH
+  // a refused launch is not counted; its error surfaces through MV2_CHECK_LAUNCH
+  if (cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...) == cudaSuccess) ++g_launches;
 }
 
 }  // namespace mv2

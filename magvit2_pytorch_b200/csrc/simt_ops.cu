@@ -29,6 +29,7 @@ static int grid_cap(int per_sm) {
   return n_sm * per_sm;
 }
 static thread_local char g_err[512] = "";
+thread_local uint64_t g_launches = 0;
 void set_error(const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
@@ -2580,6 +2581,7 @@ extern "C" {
 
 int mv2_abi_version(void) { return MV2_ABI_VERSION; }
 const char* mv2_last_error(void) { return mv2::g_err; }
+uint64_t mv2_launch_count(void) { return mv2::g_launches; }
 
 int mv2_set_pdl(int on) {
   const int prev = mv2::g_pdl;

@@ -81,7 +81,6 @@ class LfqBatchEntropy:
         self._pending = None
 
     def start(self, presign: torch.Tensor, group=None):
-        from ._lib import check
         eng = self.eng
         N, D = presign.shape
         d = D // self.nc                 # presign is [N][num_codebooks][d]
@@ -96,14 +95,12 @@ class LfqBatchEntropy:
         with torch.cuda.stream(self.side):
             st = C.c_void_p(self.side.cuda_stream)
             if ws is None:
-                check(eng.lib.mv2_lfq_entropy_partials(presign.data_ptr(), N, d, self.nc, float(self.inv_temperature), avg.data_ptr(),
-                                                       stats.data_ptr(), st), "mv2_lfq_entropy_partials")
+                eng._call("mv2_lfq_entropy_partials", presign.data_ptr(), N, d, self.nc, float(self.inv_temperature), avg.data_ptr(),
+                          stats.data_ptr(), stream=st)
             else:
-                check(eng.lib.mv2_lfq_entropy_fact_partials(presign.data_ptr(), N, d, self.nc, float(self.inv_temperature),
-                                                            avg.data_ptr(), stats.data_ptr(), ws.data_ptr(), st),
-                      "mv2_lfq_entropy_fact_partials")
+                eng._call("mv2_lfq_entropy_fact_partials", presign.data_ptr(), N, d, self.nc, float(self.inv_temperature),
+                          avg.data_ptr(), stats.data_ptr(), ws.data_ptr(), stream=st)
                 ws.record_stream(self.side)
-            eng.launches += 1
             avg.div_(N)                       # local mean code probability
             if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
                 dist.all_reduce(avg, op=dist.ReduceOp.SUM, group=group)    # the one collective of the path (NCCL, nc * 2^d * 4 bytes)
@@ -120,16 +117,13 @@ class LfqBatchEntropy:
         """-> (per_sample_entropy, batch_entropy, commitment, aux_loss) as 0-d fp32 tensors (views of one 4-float result of
         mv2_lfq_aux_finalize).  `avg` holds the SUM over ranks of the per-rank mean code probabilities (start() divides by the
         local token count before the all-reduce, as the reference's maybe_distributed_mean does), so p = avg / world."""
-        from ._lib import check
         avg, stats, N, d = self._pending
         eng = self.eng
-        cur = torch.cuda.current_stream(eng.device)
-        cur.wait_stream(self.side)
+        torch.cuda.current_stream(eng.device).wait_stream(self.side)
         world = dist.get_world_size(group) if (dist.is_available() and dist.is_initialized()) else 1
         out = torch.empty(4, device=avg.device, dtype=torch.float32)
         # avg is already a per-rank mean: "tokens_global" = number of ranks summed; per-rank terms use the local N
-        check(eng.lib.mv2_lfq_aux_finalize(avg.data_ptr(), stats.data_ptr(), d, self.nc, N, world, float(diversity_gamma), float(entropy_w),
-                                           float(commit_w), out.data_ptr(), C.c_void_p(cur.cuda_stream)), "mv2_lfq_aux_finalize")
-        eng.launches += 1
+        eng._call("mv2_lfq_aux_finalize", avg.data_ptr(), stats.data_ptr(), d, self.nc, N, world, float(diversity_gamma),
+                  float(entropy_w), float(commit_w), out.data_ptr())
         self._pending = None
         return out[0], out[1], out[2], out[3]

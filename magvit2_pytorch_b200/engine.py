@@ -343,6 +343,13 @@ class Engine:
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
+    def _call(self, entry, *args, stream=None):
+        """Calls launching entry point `entry`(*args, stream) (the current stream by default), raises on its error code and
+        adds the kernels it launched, as the library counts them, to `launches`."""
+        n0 = self.lib.mv2_launch_count()
+        check(getattr(self.lib, entry)(*args, self._stream() if stream is None else stream), entry)
+        self.launches += self.lib.mv2_launch_count() - n0
+
     def _new(self, shape, dtype=None):
         return torch.empty(shape, device=self.device, dtype=dtype or self.dtype)
 
@@ -435,9 +442,7 @@ class Engine:
         if kind == "simt" and pk.epi_mode == 2:   # scaled residual: the residual epilogue, then * 2^-0.5 (the reference's add-then-multiply)
             assert res is not None and shuffle == SHUFFLE_NONE
             scale = torch.full((B, pk.Co), 2 ** -0.5, device=self.device, dtype=torch.float32)
-            check(self.lib.mv2_scale_channels(_ptr(y), _ptr(scale), _ptr(y), _dt(self.dtype), B, To * Ho * Wo, pk.Co, self._stream()),
-                  "mv2_scale_channels")
-            self.launches += 1
+            self._call("mv2_scale_channels", _ptr(y), _ptr(scale), _ptr(y), _dt(self.dtype), B, To * Ho * Wo, pk.Co)
         return y
 
     def conv_kernel(self, ta: TcConvArgs, pk: ConvPack, hist_T: int = 0, token_shift: bool = False) -> str:
@@ -471,8 +476,7 @@ class Engine:
         if prof:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        check(getattr(self.lib, entry)(*args, self._stream()), entry)
-        self.launches += 1
+        self._call(entry, *args)
         if kind == "simt":
             self.simt_conv_calls += 1
             return
@@ -509,7 +513,6 @@ class Engine:
         """ResidualUnit (reference M:930-944): x + SE(ELU(conv1(ELU(causal_conv3(x)))))."""
         B, T, H, W, Cc = x.shape
         F_, Pn = B * T, H * W
-        st = self._stream()
         dt = _dt(self.dtype)
         c3, c1 = p["conv3"], p["conv1"]
         if self.fuse_ru and self.conv_kernel(self._tc_args(x, c3, act=ACT_ELU), c3) == "slab":
@@ -527,11 +530,10 @@ class Engine:
                 if advance is not None:
                     advance()
                 gates = self._new((F_, Cc), torch.float32)
-                check(self.lib.mv2_se_gate_records(_ptr(ws), nrec, F_, Cc, p["hidden"], _ptr(p["w1"]), _ptr(p["b1"]), _ptr(p["w2"]),
-                                                   _ptr(p["b2"]), _ptr(gates), st), "mv2_se_gate_records")
+                self._call("mv2_se_gate_records", _ptr(ws), nrec, F_, Cc, p["hidden"], _ptr(p["w1"]), _ptr(p["b1"]), _ptr(p["w2"]),
+                           _ptr(p["b2"]), _ptr(gates))
                 out = self._new(x.shape)
-                check(self.lib.mv2_gate_residual(_ptr(y), _ptr(x), _ptr(gates), _ptr(out), dt, F_, Pn, Cc, st), "mv2_gate_residual")
-                self.launches += 3                # mv2_se_gate_records: two kernels; mv2_gate_residual: one
+                self._call("mv2_gate_residual", _ptr(y), _ptr(x), _ptr(gates), _ptr(out), dt, F_, Pn, Cc)
                 return out
         h = self.conv(x, c3, act=ACT_ELU, ss=_sub(ss, "conv3"))
         y = self.conv(h, c1, act=ACT_ELU)
@@ -541,16 +543,14 @@ class Engine:
         """x + SqueezeExcite(y) (M:221-240) of an unfused ResidualUnit: softmax pool of y per frame, gate MLP, gated residual."""
         B, T, H, W, Cc = x.shape
         F_, Pn = B * T, H * W
-        st = self._stream()
         dt = _dt(self.dtype)
         ws = self._new((self.lib.mv2_se_workspace_bytes(F_, Pn, Cc) // 4,), torch.float32)
         gates = self._new((F_, Cc), torch.float32)
-        check(self.lib.mv2_se_pool(_ptr(y), dt, F_, Pn, Cc, _ptr(p["wk"]), p["bk"], _ptr(ws), st), "mv2_se_pool")
-        check(self.lib.mv2_se_gate(_ptr(ws), dt, F_, Pn, Cc, p["hidden"], _ptr(p["w1"]), _ptr(p["b1"]), _ptr(p["w2"]),
-                                   _ptr(p["b2"]), _ptr(gates), st), "mv2_se_gate")
+        self._call("mv2_se_pool", _ptr(y), dt, F_, Pn, Cc, _ptr(p["wk"]), p["bk"], _ptr(ws))
+        self._call("mv2_se_gate", _ptr(ws), dt, F_, Pn, Cc, p["hidden"], _ptr(p["w1"]), _ptr(p["b1"]), _ptr(p["w2"]),
+                   _ptr(p["b2"]), _ptr(gates))
         out = self._new(x.shape)
-        check(self.lib.mv2_gate_residual(_ptr(y), _ptr(x), _ptr(gates), _ptr(out), dt, F_, Pn, Cc, st), "mv2_gate_residual")
-        self.launches += 3
+        self._call("mv2_gate_residual", _ptr(y), _ptr(x), _ptr(gates), _ptr(out), dt, F_, Pn, Cc)
         return out
 
     def dense_small(self, x, w, b, act=ACT_NONE):
@@ -558,8 +558,7 @@ class Engine:
         Bx, K = x.shape
         N = w.shape[0]
         y = self._new((Bx, N), torch.float32)
-        check(self.lib.mv2_dense_small(_ptr(x), _ptr(w), _ptr(b), _ptr(y), Bx, K, N, act, self._stream()), "mv2_dense_small")
-        self.launches += 1
+        self._call("mv2_dense_small", _ptr(x), _ptr(w), _ptr(b), _ptr(y), Bx, K, N, act)
         return y
 
     def cond_stem(self, cond, side):
@@ -574,11 +573,9 @@ class Engine:
         c = self.dense_small(cond_e, p["wc"], p["bc"])
         scale_in = self._new((B, Cc), torch.float32)
         inv_norm = self._new((B, Cc), torch.float32)
-        st = self._stream()
-        check(self.lib.mv2_mod_prepare(_ptr(c), _ptr(p["S"]), p["eps"], _ptr(scale_in), _ptr(inv_norm), B, Cc, Cc, st), "mv2_mod_prepare")
+        self._call("mv2_mod_prepare", _ptr(c), _ptr(p["S"]), p["eps"], _ptr(scale_in), _ptr(inv_norm), B, Cc, Cc)
         xs = self._new(x.shape)
-        check(self.lib.mv2_scale_channels(_ptr(x), _ptr(scale_in), _ptr(xs), _dt(self.dtype), B, T * H * W, Cc, st), "mv2_scale_channels")
-        self.launches += 2
+        self._call("mv2_scale_channels", _ptr(x), _ptr(scale_in), _ptr(xs), _dt(self.dtype), B, T * H * W, Cc)
         h = self.conv(xs, p["conv3"], act=ACT_ELU, oscale=inv_norm, ss=_sub(ss, "conv3"))
         return self.conv(h, p["conv1"], act=ACT_ELU, res=x)
 
@@ -590,14 +587,12 @@ class Engine:
         if prev is not None:
             t, tl = prev
             fe = t[0, 0].numel()
-            check(self.lib.mv2_rmsnorm_prev(_ptr(x), t.data_ptr() + tl * fe * t.element_size(), t.shape[1] * fe, _ptr(out),
-                                            _dt(self.dtype), _ptr(gamma), B, T, H * W, Cc, self._stream()), "mv2_rmsnorm_prev")
+            self._call("mv2_rmsnorm_prev", _ptr(x), t.data_ptr() + tl * fe * t.element_size(), t.shape[1] * fe, _ptr(out),
+                       _dt(self.dtype), _ptr(gamma), B, T, H * W, Cc)
         else:
-            check(self.lib.mv2_rmsnorm(_ptr(x), _ptr(out), _dt(self.dtype), _ptr(gamma), B, T, H * W, Cc,
-                                       int(token_shift), self._stream()), "mv2_rmsnorm")
+            self._call("mv2_rmsnorm", _ptr(x), _ptr(out), _dt(self.dtype), _ptr(gamma), B, T, H * W, Cc, int(token_shift))
         if ss is not None and token_shift:
             ss.put("prev", (x, T - 1))
-        self.launches += 1
         return out
 
     def feed_forward(self, x, p, token_shift=False, ss: Optional[StreamState] = None):
@@ -611,8 +606,7 @@ class Engine:
         hdn = self.conv(xn, fc1)
         I = p["inner"]
         g = self._new((B, T, H, W, I))
-        check(self.lib.mv2_geglu(_ptr(hdn), _ptr(g), _dt(self.dtype), B * T * H * W, I, self._stream()), "mv2_geglu")
-        self.launches += 1
+        self._call("mv2_geglu", _ptr(hdn), _ptr(g), _dt(self.dtype), B * T * H * W, I)
         return self.conv(g, p["fc2"], res=x)
 
     def attention(self, x, p, axis: str, dropout: Optional[_lib.DropoutArgs] = None, ss: Optional[StreamState] = None):
@@ -637,10 +631,9 @@ class Engine:
                          dim_head=dh, n_mem=p["n_mem"], causal=0, n_outer=B * T, n_inner=1, L=HW,
                          outer_stride=HW, inner_stride=0, tok_stride=1)
         if dropout is None:
-            check(self.lib.mv2_attention(C.byref(a), self._stream()), "mv2_attention")
+            self._call("mv2_attention", C.byref(a))
         else:
-            check(self.lib.mv2_attention_dropout(C.byref(a), C.byref(dropout), self._stream()), "mv2_attention_dropout")
-        self.launches += 1
+            self._call("mv2_attention_dropout", C.byref(a), C.byref(dropout))
         return self.conv(o, p["out"], res=x)
 
     KV_CACHE_STEP = 16       # latent frames the time attention's K/V cache grows by
@@ -666,15 +659,12 @@ class Engine:
         a = AttnArgs(qkv=_ptr(buf), out=None, mem_kv=_ptr(p["mem_kv"]), dtype=_dt(self.dtype), heads=p["heads"],
                      dim_head=p["dim_head"], n_mem=p["n_mem"], causal=1, n_outer=B, n_inner=HW, L=L,
                      outer_stride=buf.shape[1] * HW, inner_stride=1, tok_stride=HW)
-        check(self.lib.mv2_attention_tail(C.byref(a), _ptr(qkv), T * HW, L0, _ptr(o), T * HW, self._stream()), "mv2_attention_tail")
-        self.launches += 1
+        self._call("mv2_attention_tail", C.byref(a), _ptr(qkv), T * HW, L0, _ptr(o), T * HW)
 
     def attention_dropout_mask(self, n_seq, heads, L, n_mem, dropout: _lib.DropoutArgs):
         """The keep mask of an attention call, uint8 (n_seq, heads, L, n_mem + L) (mv2_attention_dropout_mask)."""
         keep = torch.empty((n_seq, heads, L, n_mem + L), device=self.device, dtype=torch.uint8)
-        check(self.lib.mv2_attention_dropout_mask(n_seq, heads, L, n_mem, C.byref(dropout), _ptr(keep), self._stream()),
-              "mv2_attention_dropout_mask")
-        self.launches += 1
+        self._call("mv2_attention_dropout_mask", n_seq, heads, L, n_mem, C.byref(dropout), _ptr(keep))
         return keep
 
     def linear_attention(self, x, p):
@@ -687,9 +677,7 @@ class Engine:
         n_seq, L = B * T, H * W
         ws = self._new((self.lib.mv2_linattn_workspace_bytes(n_seq, heads, L) // 4,), torch.float32)
         o = self._new((B, T, H, W, heads * dh))
-        check(self.lib.mv2_linear_attention(_ptr(q), _ptr(kv), _ptr(o), _dt(self.dtype), n_seq, L, heads, dh,
-                                            _ptr(ws), self._stream()), "mv2_linear_attention")
-        self.launches += 2
+        self._call("mv2_linear_attention", _ptr(q), _ptr(kv), _ptr(o), _dt(self.dtype), n_seq, L, heads, dh, _ptr(ws))
         return self.conv(o, p["out"], res=x)
 
     def gateloop(self, x, p, ss: Optional[StreamState] = None):
@@ -703,12 +691,9 @@ class Engine:
             if state is None:
                 state = torch.zeros((B, H * W, Cc), device=self.device, dtype=torch.float32)
                 ss.put("s", state)
-            check(self.lib.mv2_gateloop_scan_state(_ptr(qkva), _ptr(x), _ptr(out), _dt(self.dtype), B, T, H * W, Cc, _ptr(state),
-                                                   self._stream()), "mv2_gateloop_scan_state")
+            self._call("mv2_gateloop_scan_state", _ptr(qkva), _ptr(x), _ptr(out), _dt(self.dtype), B, T, H * W, Cc, _ptr(state))
         else:
-            check(self.lib.mv2_gateloop_scan(_ptr(qkva), _ptr(x), _ptr(out), _dt(self.dtype), B, T, H * W, Cc, self._stream()),
-                  "mv2_gateloop_scan")
-        self.launches += 1
+            self._call("mv2_gateloop_scan", _ptr(qkva), _ptr(x), _ptr(out), _dt(self.dtype), B, T, H * W, Cc)
         return out
 
     def profile_convs(self, fn, steps: int = 3):
@@ -785,9 +770,7 @@ class Engine:
         v = v.contiguous()
         B, Cc, T, H, W = v.shape
         out = self._new((B, T + t_pad, H, W, Cc))
-        check(self.lib.mv2_to_channels_last(_ptr(v), _src_dt(v.dtype), _ptr(out), _dt(self.dtype), B, Cc, T, H, W, t_pad,
-                                            self._stream()), "mv2_to_channels_last")
-        self.launches += 1
+        self._call("mv2_to_channels_last", _ptr(v), _src_dt(v.dtype), _ptr(out), _dt(self.dtype), B, Cc, T, H, W, t_pad)
         return out
 
     def ingest_kwpack(self, v: torch.Tensor, t_pad: int, pin):
@@ -797,9 +780,8 @@ class Engine:
         v = v.contiguous()
         B, Cc, T, H, W = v.shape
         out = self._new((B, T + t_pad, H, W, pin.Ci_tc), torch.bfloat16)
-        check(self.lib.mv2_ingest_kwpack(_ptr(v), _src_dt(v.dtype), _ptr(out), B, Cc, T, H, W, t_pad, pin.kw_orig,
-                                         pin.kw_orig // 2, pin.Ci_tc, self._stream()), "mv2_ingest_kwpack")
-        self.launches += 1
+        self._call("mv2_ingest_kwpack", _ptr(v), _src_dt(v.dtype), _ptr(out), B, Cc, T, H, W, t_pad, pin.kw_orig,
+                   pin.kw_orig // 2, pin.Ci_tc)
         return out
 
     _PAD_MODES = {"reflect": 1, "replicate": 2, "circular": 3}
@@ -812,9 +794,8 @@ class Engine:
         if pad_mode == "constant" or kt - 1 >= T:
             return self.conv(x, pk)
         xp = self._new((B, T + kt - 1, H + 2 * (kh // 2), W + 2 * (kw // 2), Cc))
-        check(self.lib.mv2_pad_cl(_ptr(x), _ptr(xp), _dt(self.dtype), B, T, H, W, Cc, kt - 1, kh // 2, kw // 2,
-                                  self._PAD_MODES[pad_mode], self._stream()), "mv2_pad_cl")
-        self.launches += 1
+        self._call("mv2_pad_cl", _ptr(x), _ptr(xp), _dt(self.dtype), B, T, H, W, Cc, kt - 1, kh // 2, kw // 2,
+                   self._PAD_MODES[pad_mode])
         return self.conv(xp, pk, pad=(0, 0, 0), out_spatial=(T, H, W))
 
     def copy_frames(self, src, t0, n, dst=None, dst_t0=0, zero_front=False):
@@ -824,17 +805,14 @@ class Engine:
             dst = self._new((B, n) + tuple(src.shape[2:]), src.dtype)
         frame_bytes = src[0, 0].numel() * src.element_size()
         assert dst[0, 0].numel() * dst.element_size() == frame_bytes and src.is_contiguous() and dst.is_contiguous()
-        check(self.lib.mv2_copy_frames(_ptr(src), _ptr(dst), B, Ts, dst.shape[1], t0, dst_t0, n, frame_bytes, int(zero_front),
-                                       self._stream()), "mv2_copy_frames")
+        self._call("mv2_copy_frames", _ptr(src), _ptr(dst), B, Ts, dst.shape[1], t0, dst_t0, n, frame_bytes, int(zero_front))
         return dst
 
     def to_channels_first(self, x: torch.Tensor, t_crop: int = 0, out_dtype=None):
         B, T, H, W, Cc = x.shape
         out_dtype = out_dtype or self.dtype
         out = torch.empty((B, Cc, T - t_crop, H, W), device=self.device, dtype=out_dtype)
-        check(self.lib.mv2_to_channels_first(_ptr(x), _dt(x.dtype), _ptr(out), _dt(out_dtype), B, Cc, T, H, W, t_crop,
-                                             self._stream()), "mv2_to_channels_first")
-        self.launches += 1
+        self._call("mv2_to_channels_first", _ptr(x), _dt(x.dtype), _ptr(out), _dt(out_dtype), B, Cc, T, H, W, t_crop)
         return out
 
     def mse(self, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
@@ -846,16 +824,14 @@ class Engine:
         a, b = a.contiguous(), b.contiguous()
         ws = self._new((self.lib.mv2_mse_workspace_bytes() // 4,), torch.float32)
         out = self._new((1,), torch.float32)
-        check(self.lib.mv2_mse(_ptr(a), _src_dt(a.dtype), _ptr(b), _dt(b.dtype), a.numel(), _ptr(ws), _ptr(out), self._stream()), "mv2_mse")
-        self.launches += 2
+        self._call("mv2_mse", _ptr(a), _src_dt(a.dtype), _ptr(b), _dt(b.dtype), a.numel(), _ptr(ws), _ptr(out))
         return out[0]
 
     def maxpool2x2(self, x):
         """nn.MaxPool2d(2, 2) (floor mode) of a channels-last (B, T, H, W, C) map -> (B, T, H // 2, W // 2, C)."""
         B, T, H, W, Cc = x.shape
         y = self._new((B, T, H // 2, W // 2, Cc), x.dtype)
-        check(self.lib.mv2_maxpool2x2(_ptr(x), _ptr(y), _dt(x.dtype), B * T, H, W, Cc, self._stream()), "mv2_maxpool2x2")
-        self.launches += 1
+        self._call("mv2_maxpool2x2", _ptr(x), _ptr(y), _dt(x.dtype), B * T, H, W, Cc)
         return y
 
     def maxpool2x2_backward(self, g, x):
@@ -865,9 +841,7 @@ class Engine:
         g = g.to(x.dtype).contiguous()
         assert tuple(g.shape) == (B, T, H // 2, W // 2, Cc), (g.shape, x.shape)
         gx = self._new(x.shape, x.dtype)
-        check(self.lib.mv2_maxpool2x2_backward(_ptr(g), _ptr(x), _ptr(gx), _dt(x.dtype), B * T, H, W, Cc, self._stream()),
-              "mv2_maxpool2x2_backward")
-        self.launches += 1
+        self._call("mv2_maxpool2x2_backward", _ptr(g), _ptr(x), _ptr(gx), _dt(x.dtype), B * T, H, W, Cc)
         return gx
 
     # ------------------------------------------------------------------ the path
@@ -976,16 +950,14 @@ class Engine:
         if m.use_fsq:
             idx = torch.empty(ishape, device=self.device, dtype=torch.int32)
             lv = (C.c_int32 * d)(*qz.levels)
-            check(self.lib.mv2_fsq_forward(_ptr(x), _dt(self.dtype), N, Cc, d, nc, lv, _ptr(P["win"]), _ptr(P["bin"]),
-                                           _ptr(P["wout"]), _ptr(P["bout"]), _ptr(idx), _ptr(q), _ptr(aux),
-                                           self._stream()), "mv2_fsq_forward")
+            self._call("mv2_fsq_forward", _ptr(x), _dt(self.dtype), N, Cc, d, nc, lv, _ptr(P["win"]), _ptr(P["bin"]),
+                       _ptr(P["wout"]), _ptr(P["bout"]), _ptr(idx), _ptr(q), _ptr(aux))
         else:
             idx = torch.empty(ishape, device=self.device, dtype=torch.int64)
             clamp = qz.soft_clamp_input_value
-            check(self.lib.mv2_lfq_forward(_ptr(x), _dt(self.dtype), N, Cc, d, nc, _ptr(P["win"]), _ptr(P["bin"]),
-                                           _ptr(P["wout"]), _ptr(P["bout"]), float(clamp) if clamp else 0.0, int(qz.spherical),
-                                           _ptr(idx), _ptr(q), _ptr(aux), self._stream()), "mv2_lfq_forward")
-        self.launches += 1
+            self._call("mv2_lfq_forward", _ptr(x), _dt(self.dtype), N, Cc, d, nc, _ptr(P["win"]), _ptr(P["bin"]),
+                       _ptr(P["wout"]), _ptr(P["bout"]), float(clamp) if clamp else 0.0, int(qz.spherical),
+                       _ptr(idx), _ptr(q), _ptr(aux))
         return q, idx, aux
 
     def codes_to_quantized_cl(self, codes: torch.Tensor):
@@ -1002,10 +974,9 @@ class Engine:
         is64 = int(codes.dtype == torch.int64)
         if m.use_fsq:
             lv = (C.c_int32 * d)(*qz.levels)
-            check(self.lib.mv2_fsq_decode(_ptr(codes), is64, N, Cc, d, nc, lv, _ptr(P["wout"]), _ptr(P["bout"]), _ptr(q),
-                                          _dt(self.dtype), self._stream()), "mv2_fsq_decode")
+            self._call("mv2_fsq_decode", _ptr(codes), is64, N, Cc, d, nc, lv, _ptr(P["wout"]), _ptr(P["bout"]), _ptr(q),
+                       _dt(self.dtype))
         else:
-            check(self.lib.mv2_lfq_decode(_ptr(codes), is64, N, Cc, d, nc, _ptr(P["wout"]), _ptr(P["bout"]), _ptr(q),
-                                          _dt(self.dtype), self._stream()), "mv2_lfq_decode")
-        self.launches += 1
+            self._call("mv2_lfq_decode", _ptr(codes), is64, N, Cc, d, nc, _ptr(P["wout"]), _ptr(P["bout"]), _ptr(q),
+                       _dt(self.dtype))
         return q

@@ -34,7 +34,7 @@ import torch.nn.functional as F
 
 from ._lib import ACT_ELU
 from .dist import LFQ_DENSE_MAX_D
-from .engine import pack_conv
+from .engine import Engine, pack_conv
 
 
 # --------------------------------------------------------------------------------------------
@@ -230,11 +230,12 @@ def _code_values(codes, qz, fsq):
     return vals.reshape(*codes.shape[:4], -1)
 
 
-def _lfq_train(x, qz, avg_global, inv_temperature=100.):
+def _lfq_train(x, qz, avg_global, eng=None, inv_temperature=100.):
     """LFQ training forward (SURVEY Appendix A.1 steps 2-10) on (B,T,H,W,C): -> (straight-through quantised output, aux loss).
     `avg_global` is the cross-rank mean code probability of the forward pass; the local term enters as
     avg_local + (avg_global - avg_local).detach(), which reproduces the gradient of the reference's autograd-aware
-    all-reduce (each rank back-propagates d H / d avg_global into its own tokens)."""
+    all-reduce (each rank back-propagates d H / d avg_global into its own tokens).  `eng`: the Engine that launches (and
+    counts) the bit-factorised entropy kernels of codebooks past 2^LFQ_DENSE_MAX_D codes; None: an engine of the call's own."""
     d, nc = qz.codebook_dim, qz.num_codebooks
     p = _lfq_project(x, qz)
     qd = torch.where(p > 0, torch.ones_like(p), -torch.ones_like(p))
@@ -242,7 +243,10 @@ def _lfq_train(x, qz, avg_global, inv_temperature=100.):
     out = F.linear(st.to(x.dtype), qz.project_out.weight, qz.project_out.bias)
     commit = ((p - qd) ** 2).mean()
     if d > LFQ_DENSE_MAX_D:
-        ent = _LfqEntropyFact.apply(p.contiguous(), avg_global.reshape(-1).float().contiguous(), inv_temperature,
+        if eng is None:
+            eng = Engine(None)
+            eng.bind(p, "the LFQ entropy terms")
+        ent = _LfqEntropyFact.apply(eng, p.contiguous(), avg_global.reshape(-1).float().contiguous(), inv_temperature,
                                     qz.entropy_loss_weight, qz.diversity_gamma)
         return out, ent + commit * qz.commitment_loss_weight
     mask = qz.mask.to(p.device)
@@ -264,40 +268,35 @@ class _LfqEntropyFact(torch.autograd.Function):
     the local tokens as through _lfq_train's avg_local + (avg_global - avg_local).detach()."""
 
     @staticmethod
-    def forward(ctx, p, avg_global, inv_temperature, entropy_weight, diversity_gamma):
-        from ._lib import check, load
-        lib = load()
+    def forward(ctx, eng, p, avg_global, inv_temperature, entropy_weight, diversity_gamma):
         N, nc, d = p.shape
         dev = p.device
-        st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        ws = torch.empty(lib.mv2_lfq_entropy_fact_workspace_bytes(N, d, nc), device=dev, dtype=torch.uint8)
+        ws = torch.empty(eng.lib.mv2_lfq_entropy_fact_workspace_bytes(N, d, nc), device=dev, dtype=torch.uint8)
         avg_local = torch.empty(nc << d, device=dev, dtype=torch.float32)
         stats = torch.empty(2, device=dev, dtype=torch.float32)
-        check(lib.mv2_lfq_entropy_fact_partials(p.data_ptr(), N, d, nc, float(inv_temperature), avg_local.data_ptr(), stats.data_ptr(),
-                                                ws.data_ptr(), st), "mv2_lfq_entropy_fact_partials")
+        eng._call("mv2_lfq_entropy_fact_partials", p.data_ptr(), N, d, nc, float(inv_temperature), avg_local.data_ptr(),
+                  stats.data_ptr(), ws.data_ptr())
         out4 = torch.empty(4, device=dev, dtype=torch.float32)
         # avg_global is already a mean (n_tokens_global = 1); out4 = (per_sample, batch_entropy, commitment, aux) with the
         # commitment left to autograd (weight 0 here)
-        check(lib.mv2_lfq_aux_finalize(avg_global.data_ptr(), stats.data_ptr(), d, nc, N, 1, float(diversity_gamma), float(entropy_weight),
-                                       0.0, out4.data_ptr(), st), "mv2_lfq_aux_finalize")
+        eng._call("mv2_lfq_aux_finalize", avg_global.data_ptr(), stats.data_ptr(), d, nc, N, 1, float(diversity_gamma),
+                  float(entropy_weight), 0.0, out4.data_ptr())
         ctx.save_for_backward(p, avg_global)
+        ctx.eng = eng
         ctx.coefs = (float(inv_temperature), entropy_weight / (N * nc), entropy_weight * diversity_gamma / (N * nc))
         return out4[3].clone()
 
     @staticmethod
     def backward(ctx, g):
-        from ._lib import check, load
-        lib = load()
+        eng = ctx.eng
         p, avg_global = ctx.saved_tensors
         N, nc, d = p.shape
         inv_t, coef_sample, coef_batch = ctx.coefs
-        dev = p.device
-        ws = torch.empty(lib.mv2_lfq_entropy_fact_workspace_bytes(N, d, nc), device=dev, dtype=torch.uint8)
+        ws = torch.empty(eng.lib.mv2_lfq_entropy_fact_workspace_bytes(N, d, nc), device=p.device, dtype=torch.uint8)
         gp = torch.empty_like(p)
-        check(lib.mv2_lfq_entropy_fact_backward(p.data_ptr(), avg_global.data_ptr(), N, d, nc, inv_t, coef_sample, coef_batch, gp.data_ptr(),
-                                                ws.data_ptr(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
-              "mv2_lfq_entropy_fact_backward")
-        return gp * g, None, None, None, None
+        eng._call("mv2_lfq_entropy_fact_backward", p.data_ptr(), avg_global.data_ptr(), N, d, nc, inv_t, coef_sample, coef_batch,
+                  gp.data_ptr(), ws.data_ptr())
+        return None, gp * g, None, None, None, None
 
 
 def _fsq_train(x, qz):
@@ -653,7 +652,7 @@ class TrainRunner(TapeRunner):
         avg_global = avg_sum / world
         self.breakdown = (ps, bent, commit)
         # the auxiliary loss's gradient (self._g_aux) enters here, set by backward
-        self.tape.append(lambda g: self._vjp(lambda t: _lfq_train(t, qz, avg_global), x, params, (g, self._g_aux)))
+        self.tape.append(lambda g: self._vjp(lambda t: _lfq_train(t, qz, avg_global, eng), x, params, (g, self._g_aux)))
         return q, aux
 
     def codes_piece(self, codes):

@@ -41,6 +41,27 @@ def test_load_and_abi_version_5():
     assert lib.mv2_linattn_workspace_bytes(3, 16, 1024) == 3 * 16 * 4 * 657 * 4 + 3 * 16 * 2 * 16 * 88 * 2
 
 
+def test_launch_count_is_per_thread_and_skips_refused_calls():
+    """mv2_launch_count is exported and bound, reads 0 on a freshly started thread, and a call refused by its argument
+    check (mv2_rmsnorm with x = NULL touches no CUDA API) returns MV2_E_ARG without counting a launch."""
+    import threading
+    lib = _lib.load()
+    assert _lib.SIGNATURES["mv2_launch_count"] == (ctypes.c_uint64, [])
+    assert hasattr(ctypes.CDLL(_lib.LIB_PATH), "mv2_launch_count")
+    seen = {}
+
+    def run():
+        seen["fresh"] = lib.mv2_launch_count()
+        buf = (ctypes.c_float * 8)()
+        seen["rc"] = lib.mv2_rmsnorm(None, ctypes.addressof(buf), _lib.MV2_F32, ctypes.addressof(buf), 1, 1, 1, 8, 0, None)
+        seen["after"] = lib.mv2_launch_count()
+
+    t = threading.Thread(target=run)
+    t.start()
+    t.join()
+    assert seen == {"fresh": 0, "rc": -1, "after": 0}, seen       # MV2_E_ARG = -1
+
+
 def test_struct_sizes_match_header_layout():
     # 5 pointers + 22 int32 (conv), 3 pointers + 8 int32 + 3 int64 (attention)
     assert ctypes.sizeof(_lib.ConvArgs) == 5 * 8 + 22 * 4 + 8            # + oscale pointer
