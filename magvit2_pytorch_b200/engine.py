@@ -209,6 +209,34 @@ def param_signature(module):
     return (tuple((p.data_ptr(), p._version) for p in ps), ps[0].dtype, ps[0].device)
 
 
+class PackCache:
+    """The engine and weight packs of a module that runs on an engine of its own (the discriminator, the VGG,
+    CausalConvTranspose3d).  The engine outlives re-packs, so its `launches` keep counting; copies and pickles start empty,
+    as its ctypes handles belong to this instance."""
+
+    def __init__(self):
+        self.engine: Optional[Engine] = None
+        self.packs = None
+        self._sig = None
+
+    def get(self, module, what, build, key=()):
+        """-> (engine, packs): re-packs with build(engine), under no_grad, when the module's parameters (param_signature) or
+        `key` changed, after binding the engine to them (Engine.bind; `what` names the module in its errors)."""
+        sig = (param_signature(module), key)
+        if sig != self._sig:
+            self._sig = None
+            if self.engine is None:
+                self.engine = Engine(None)
+            self.engine.bind(next(iter(module.parameters())), what)
+            with torch.no_grad():
+                self.packs = build(self.engine)
+            self._sig = sig
+        return self.engine, self.packs
+
+    def __reduce__(self):         # pickle, copy and deepcopy
+        return PackCache, ()
+
+
 class Engine:
     """Executes the inference path of one VideoTokenizer on its parameters' device/dtype."""
 

@@ -28,7 +28,7 @@ import torch.nn.functional as F
 from torch.autograd.function import once_differentiable
 
 from ._lib import ACT_LEAKY_RELU, ACT_NONE, SHUFFLE_SPACE
-from .engine import Engine, pack_conv, pack_conv_in_kwpack, pack_feed_forward, pack_linear_attention, param_signature
+from .engine import pack_conv, pack_conv_in_kwpack, pack_feed_forward, pack_linear_attention
 from .train import TapeRunner, _feed_forward_block, _linear_attention_block
 
 # reference M:1039-1043
@@ -102,37 +102,30 @@ def gradient_penalty(d, images):
 # --------------------------------------------------------------------------------------------
 # device path
 # --------------------------------------------------------------------------------------------
-def _packs(d):
-    """(engine, packs) of the Discriminator, re-packed when its parameters changed."""
-    sig = param_signature(d)
-    if d._pack is not None and d._pack[0] == sig:
-        return d._pack[1], d._pack[2]
-    eng = d._pack[1] if d._pack is not None else Engine(None)
-    eng.bind(d.to_logits[0].weight, "the discriminator")
+def _packs(d, eng):
+    """The weight packs of the Discriminator d on engine eng."""
     dt = eng.dtype
     P = []
-    with torch.no_grad():
-        for block, attn in d.blocks:
-            n0, n2, cr = block.net[0], block.net[2], block.conv_res
-            e = dict(net0=pack_conv(n0.weight, n0.bias, dt), net2=pack_conv(n2.weight, n2.bias, dt),
-                     res=pack_conv(cr.weight, cr.bias, dt), attn=pack_linear_attention(attn[0].fn, dt),
-                     ff=pack_feed_forward(attn[1].fn, dt))
-            if dt == torch.bfloat16 and n0.weight.shape[1] * 3 <= 32:       # 3-channel first conv: conv_in's kw-packed ingest
-                e["net0_kw"] = pack_conv_in_kwpack(n0.weight[:, :, None], n0.bias)
-            # the block output (branch + conv_res(x)) * 2^-0.5 is the epilogue of the block's last conv: the unshuffle conv
-            # with conv_res(x) as residual, or -- without downsample -- conv_res with the branch as residual
-            if block.downsample is not None:
-                ds = block.downsample[1]
-                e["down"] = pack_conv(unshuffle_conv_weight(ds.weight), ds.bias, dt)
-                e["down"].epi_mode = 2
-            else:
-                e["res"].epi_mode = 2
-            P.append(e)
-        tl = d.to_logits
-        logits = dict(conv=pack_conv(tl[0].weight, tl[0].bias, dt),
-                      lin=pack_conv(logits_conv_weight(tl[3], tl[0].weight.shape[0], d.last_fmap), tl[3].bias, dt))
-    d._pack = (sig, eng, (P, logits))
-    return eng, (P, logits)
+    for block, attn in d.blocks:
+        n0, n2, cr = block.net[0], block.net[2], block.conv_res
+        e = dict(net0=pack_conv(n0.weight, n0.bias, dt), net2=pack_conv(n2.weight, n2.bias, dt),
+                 res=pack_conv(cr.weight, cr.bias, dt), attn=pack_linear_attention(attn[0].fn, dt),
+                 ff=pack_feed_forward(attn[1].fn, dt))
+        if dt == torch.bfloat16 and n0.weight.shape[1] * 3 <= 32:       # 3-channel first conv: conv_in's kw-packed ingest
+            e["net0_kw"] = pack_conv_in_kwpack(n0.weight[:, :, None], n0.bias)
+        # the block output (branch + conv_res(x)) * 2^-0.5 is the epilogue of the block's last conv: the unshuffle conv
+        # with conv_res(x) as residual, or -- without downsample -- conv_res with the branch as residual
+        if block.downsample is not None:
+            ds = block.downsample[1]
+            e["down"] = pack_conv(unshuffle_conv_weight(ds.weight), ds.bias, dt)
+            e["down"].epi_mode = 2
+        else:
+            e["res"].epi_mode = 2
+        P.append(e)
+    tl = d.to_logits
+    logits = dict(conv=pack_conv(tl[0].weight, tl[0].bias, dt),
+                  lin=pack_conv(logits_conv_weight(tl[3], tl[0].weight.shape[0], d.last_fmap), tl[3].bias, dt))
+    return P, logits
 
 
 def _leaky_grad(g, y):
@@ -144,7 +137,7 @@ class DiscrRunner(TapeRunner):
     """One discriminator forward through the engine's kernels, recording what the backward needs."""
 
     def __init__(self, d):
-        eng, (self.P, self.logits_pk) = _packs(d)
+        eng, (self.P, self.logits_pk) = d._pack_cache.get(d, "the discriminator", lambda eng: _packs(d, eng))
         super().__init__(eng)
         self.d = d
 
@@ -240,13 +233,8 @@ class DiscrRunner(TapeRunner):
 
     def backward(self, g_logits):
         """-> (gradient wrt the images (B, C, H, W) | None, {Parameter: grad})."""
-        if not self.tape:
-            raise RuntimeError("the discriminator's backward ran already (retain_graph is not supported by this path)")
-        g = g_logits.to(self.eng.dtype)
-        with torch.no_grad():
-            for fn in reversed(self.tape):
-                g = fn(g)
-        self.tape = []
+        g = self._run_tape(g_logits.to(self.eng.dtype),
+                           "the discriminator's backward ran already (retain_graph is not supported by this path)")
         gx = None if g is None else g[:, 0].permute(0, 3, 1, 2).contiguous()
         return gx, self.grads
 

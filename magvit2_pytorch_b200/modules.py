@@ -15,6 +15,9 @@ import math
 import torch
 from torch import nn
 
+from ._lib import SHUFFLE_NONE, SHUFFLE_TIME
+from .engine import PackCache, pack_conv
+
 
 class _NoForward(nn.Module):
     def forward(self, *a, **k):
@@ -271,12 +274,7 @@ class Discriminator(_NoForward):
         latent = self.last_fmap[0] * self.last_fmap[1] * dim_last
         self.to_logits = nn.Sequential(nn.Conv2d(dim_last, dim_last, 3, padding=1), Marker("LeakyReLU(0.1)"),
                                        Marker("'b ... -> b (...)'"), nn.Linear(latent, 1), Marker("'b 1 -> b'"))
-        self._pack = None         # (parameter signature, engine, weight packs) of the device path (gan.py)
-
-    def __getstate__(self):       # the packs and the engine belong to this instance: copies and pickles re-pack on first use
-        st = dict(self.__dict__)
-        st["_pack"] = None
-        return st
+        self._pack_cache = PackCache()       # engine and weight packs of the device path (gan.py)
 
     def forward(self, images):
         from .gan import discriminator_forward
@@ -346,7 +344,7 @@ class CausalConvTranspose3d(nn.Module):
             raise NotImplementedError("CausalConvTranspose3d on the device supports time_stride 1 and 2")
         self.upsample_factor = time_stride
         self.conv = nn.ConvTranspose3d(chan_in, chan_out, ks, (time_stride, 1, 1), padding=(0, ks[1] // 2, ks[2] // 2), **kwargs)
-        self._pack = None
+        self._pack_cache = PackCache()
 
     def equivalent_conv_weight(self):
         """-> (weight (s*Co, Ci, ceil(kt/s), kh, kw), bias (s*Co) | None) of the causal conv described above."""
@@ -365,22 +363,13 @@ class CausalConvTranspose3d(nn.Module):
         return weq.reshape(Co * s, Ci, ktp, kh, kw), beq
 
     def forward(self, x):
-        from .engine import Engine, pack_conv
-        from ._lib import SHUFFLE_NONE, SHUFFLE_TIME
         assert x.ndim == 5
         w = self.conv.weight
         if w.device.type != "cuda" or x.device != w.device:
             raise RuntimeError("CausalConvTranspose3d runs on CUDA (sm_90a) only, input and parameters on the same device")
-        if w.dtype not in (torch.float32, torch.bfloat16):
-            raise TypeError("parameters must be float32 or bfloat16")
-        sig = (w.data_ptr(), w._version, w.dtype, w.device, None if self.conv.bias is None else self.conv.bias._version)
         with torch.no_grad(), torch.cuda.device(w.device):
-            if self._pack is None or self._pack[0] != sig:
-                eng = Engine(None)
-                eng.dtype, eng.device = w.dtype, w.device
-                weq, beq = self.equivalent_conv_weight()
-                self._pack = (sig, eng, pack_conv(weq, beq, w.dtype, shuffle_q=self.upsample_factor))
-            _, eng, pk = self._pack
+            eng, pk = self._pack_cache.get(self, "CausalConvTranspose3d", lambda eng: pack_conv(
+                *self.equivalent_conv_weight(), eng.dtype, shuffle_q=self.upsample_factor))
             y = eng.conv(eng.to_channels_last(x), pk, shuffle=SHUFFLE_TIME if self.upsample_factor == 2 else SHUFFLE_NONE)
             out = eng.to_channels_first(y)
             n = self.output_frames(x.shape[2])

@@ -327,8 +327,9 @@ def transposed_pack(weight, k, dtype):
 
 
 class TapeRunner:
-    """A forward through the engine's kernels that records its backward on a tape, with the gradient pieces shared by the
-    generator's runner (TrainRunner) and the discriminator's (gan.DiscrRunner)."""
+    """A forward through the engine's kernels that records its backward on a tape, with the tape loop and the gradient
+    pieces shared by the generator's runner (TrainRunner), the discriminator's (gan.DiscrRunner) and the VGG's
+    (vgg.VggRunner)."""
 
     def __init__(self, eng):
         self.eng = eng
@@ -336,6 +337,20 @@ class TapeRunner:
         self.grads: Dict[torch.nn.Parameter, torch.Tensor] = {}
         self.own_dgrad = True            # data gradient of the stride-1 convs through the engine's own conv kernels
         self.own_dgrad_calls = 0
+
+    def _run_tape(self, g, msg):
+        """Runs the tape in reverse from g under no_grad, up to an entry that returns None, then drops it: its closures refer
+        to this runner, so the saved activations are freed with the loss graph, not at a later cyclic collection.  `msg`:
+        the error of a second backward."""
+        if not self.tape:
+            raise RuntimeError(msg)
+        with torch.no_grad():
+            for entry in reversed(self.tape):
+                g = entry(g)
+                if g is None:
+                    break
+        self.tape = []
+        return g
 
     # ---- gradient bookkeeping
     def _acc(self, param, g):
@@ -755,29 +770,20 @@ class TrainRunner(TapeRunner):
 
     def backward(self, g_out, g_aux=None):
         """Runs the tape in reverse from the gradient of the last piece's output (g_out; g_aux: the auxiliary loss's, training
-        forward only) -> (gradient wrt the first piece's input | None, gradient wrt cond | None, {Parameter: grad}).  An entry
-        that returns None ends the chain: nothing before it is reached (the eval-mode LFQ quantiser)."""
-        if not self.tape:
-            raise RuntimeError("the tokenizer's backward ran already: the saved activations are released after one backward pass "
-                               "(call the forward again; retain_graph is not supported by this path)")
-        g = g_out.to(self.eng.dtype)
+        forward only) -> (gradient wrt the first piece's input | None, gradient wrt cond | None, {Parameter: grad}).  The
+        eval-mode LFQ quantiser's entry returns None: nothing before it is reached."""
         self._g_aux = (g_aux if g_aux is not None else torch.zeros((), device=self.eng.device)).float()
+        g = self._run_tape(g_out.to(self.eng.dtype),
+                           "the tokenizer's backward ran already: the saved activations are released after one backward pass "
+                           "(call the forward again; retain_graph is not supported by this path)")
+        self._bwd_conv_out = None          # conv_out's piece of the tape, released with it
         g_cond = None
-        with torch.no_grad():
-            for entry in reversed(self.tape):
-                g = entry(g)
-                if g is None:
-                    break
-            for side, stem in (("enc", self.m.encoder_cond_in), ("dec", self.m.decoder_cond_in)):
-                if side in self.g_cond:       # cond stems (M:1344-1352): Linear + SiLU of the raw cond vector
-                    lin = stem[0]
-                    gc = self._vjp(lambda t, lin=lin: F.silu(F.linear(t, lin.weight.float(), lin.bias.float())), self.cond.float(),
-                                   list(lin.parameters()), self.g_cond[side].float())
-                    g_cond = gc if g_cond is None else g_cond + gc
-        # the tape's closures and conv_out's piece of it refer to this runner: dropping them here breaks the reference cycle,
-        # so the saved activations are freed with the loss graph, not at a later cyclic collection
-        self.tape = []
-        self._bwd_conv_out = None
+        for side, stem in (("enc", self.m.encoder_cond_in), ("dec", self.m.decoder_cond_in)):
+            if side in self.g_cond:       # cond stems (M:1344-1352): Linear + SiLU of the raw cond vector
+                lin = stem[0]
+                gc = self._vjp(lambda t, lin=lin: F.silu(F.linear(t, lin.weight.float(), lin.bias.float())), self.cond.float(),
+                               list(lin.parameters()), self.g_cond[side].float())
+                g_cond = gc if g_cond is None else g_cond + gc
         return g, g_cond, self.grads
 
 

@@ -31,7 +31,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from ._lib import ACT_NONE, ACT_RELU
-from .engine import Engine, pack_conv, pack_conv_in_kwpack, param_signature
+from .engine import PackCache, pack_conv, pack_conv_in_kwpack
 from .train import TapeRunner
 
 
@@ -123,53 +123,39 @@ def first_conv_weight(w, channels):
     return w
 
 
-def _build_packs(vgg, eng, fmap_in, channels):
+def vgg_packs(vgg, eng, fmap_in, channels):
+    """The weight packs of the VGG on engine eng for `channels`-channel frames of size fmap_in."""
     dt = eng.dtype
     feats = []                                     # {"pk", "w", "pool", ["kw"]} per conv
     h, w = fmap_in
-    with torch.no_grad():
-        for m in vgg.features:
-            if isinstance(m, nn.Conv2d):
-                wt = first_conv_weight(m.weight, channels) if not feats else m.weight.detach()
-                e = dict(pk=pack_conv(wt, m.bias, dt), w=wt, pool=False)
-                if not feats and dt == torch.bfloat16 and wt.shape[1] * 3 <= 32:    # 3-channel first conv: kw-packed ingest
-                    e["kw"] = pack_conv_in_kwpack(wt[:, :, None], m.bias)
-                feats.append(e)
-            elif isinstance(m, nn.MaxPool2d):
-                feats[-1]["pool"] = True
-                h, w = h // 2, w // 2
-        c_last = feats[-1]["w"].shape[0]
-        ops = []
-        for m in vgg.classifier:
-            if isinstance(m, nn.Linear):
-                if not ops:              # the first Linear with the average pool folded in: a conv covering the (h, w) map
-                    wf = fold_avgpool_linear(m.weight, c_last, (h, w), _out_size(vgg.avgpool, (h, w)))
-                    pk = pack_conv(wf, m.bias, dt)
-                    # its data gradient: a 1x1 conv O -> (h w c), whose output is the channels-last map gradient
-                    pk_t = pack_conv(wf.permute(2, 3, 1, 0).reshape(h * w * c_last, -1)[:, :, None, None], None, dt)
-                else:
-                    pk = pack_conv(m.weight[:, :, None, None], m.bias, dt)
-                    pk_t = pack_conv(m.weight.detach().t()[:, :, None, None], None, dt)
-                ops.append(dict(kind="linear", pk=pk, pk_t=pk_t))
-            elif isinstance(m, nn.ReLU):
-                ops.append(dict(kind="relu"))
+    for m in vgg.features:
+        if isinstance(m, nn.Conv2d):
+            wt = first_conv_weight(m.weight, channels) if not feats else m.weight.detach()
+            e = dict(pk=pack_conv(wt, m.bias, dt), w=wt, pool=False)
+            if not feats and dt == torch.bfloat16 and wt.shape[1] * 3 <= 32:    # 3-channel first conv: kw-packed ingest
+                e["kw"] = pack_conv_in_kwpack(wt[:, :, None], m.bias)
+            feats.append(e)
+        elif isinstance(m, nn.MaxPool2d):
+            feats[-1]["pool"] = True
+            h, w = h // 2, w // 2
+    c_last = feats[-1]["w"].shape[0]
+    ops = []
+    for m in vgg.classifier:
+        if isinstance(m, nn.Linear):
+            if not ops:              # the first Linear with the average pool folded in: a conv covering the (h, w) map
+                wf = fold_avgpool_linear(m.weight, c_last, (h, w), _out_size(vgg.avgpool, (h, w)))
+                pk = pack_conv(wf, m.bias, dt)
+                # its data gradient: a 1x1 conv O -> (h w c), whose output is the channels-last map gradient
+                pk_t = pack_conv(wf.permute(2, 3, 1, 0).reshape(h * w * c_last, -1)[:, :, None, None], None, dt)
             else:
-                ops.append(dict(kind="dropout", mod=m))
+                pk = pack_conv(m.weight[:, :, None, None], m.bias, dt)
+                pk_t = pack_conv(m.weight.detach().t()[:, :, None, None], None, dt)
+            ops.append(dict(kind="linear", pk=pk, pk_t=pk_t))
+        elif isinstance(m, nn.ReLU):
+            ops.append(dict(kind="relu"))
+        else:
+            ops.append(dict(kind="dropout", mod=m))
     return dict(feats=feats, ops=ops, fmap=(h, w), c_last=c_last)
-
-
-def vgg_packs(vgg, fmap_in, channels, cache=None):
-    """(engine, packs) of the VGG for `channels`-channel frames of size fmap_in, re-packed when its parameters, the frame
-    size or the channel count changed.  `cache`: a dict kept by the caller (None: no caching)."""
-    sig = (param_signature(vgg), tuple(fmap_in), int(channels))
-    if cache is not None and cache.get("sig") == sig:
-        return cache["eng"], cache["packs"]
-    eng = (cache or {}).get("eng") or Engine(None)
-    eng.bind(vgg.features[0].weight, "the VGG")
-    packs = _build_packs(vgg, eng, fmap_in, channels)
-    if cache is not None:
-        cache.update(sig=sig, eng=eng, packs=packs)
-    return eng, packs
 
 
 # --------------------------------------------------------------------------------------------
@@ -213,7 +199,9 @@ class VggRunner(TapeRunner):
     """One VGG forward through the engine's kernels on (B, channels, H, W) frames, recording its data gradient."""
 
     def __init__(self, vgg, fmap_in, channels=3, cache=None):
-        eng, self.P = vgg_packs(vgg, fmap_in, channels, cache)
+        """`cache`: the PackCache the VGG's packs are kept in (None: packs of this runner's own)."""
+        eng, self.P = (cache or PackCache()).get(vgg, "the VGG", lambda eng: vgg_packs(vgg, eng, fmap_in, channels),
+                                                 key=(tuple(fmap_in), int(channels)))
         super().__init__(eng)
         self.vgg = vgg
         self.masks = []          # per classifier Dropout: the scaled keep-mask drawn, or None when inactive
@@ -281,13 +269,8 @@ class VggRunner(TapeRunner):
 
     def backward(self, g_feats):
         """g_feats (B, F) -> the data gradient wrt the images (B, channels, H, W).  Single use: the tape is released."""
-        if not self.tape:
-            raise RuntimeError("the VGG's backward ran already, or its forward kept no tape")
-        g = g_feats.to(self.eng.dtype).reshape(g_feats.shape[0], 1, 1, 1, -1)
-        with torch.no_grad():
-            for fn in reversed(self.tape):
-                g = fn(g)
-        self.tape = []
+        g = self._run_tape(g_feats.to(self.eng.dtype).reshape(g_feats.shape[0], 1, 1, 1, -1),
+                           "the VGG's backward ran already, or its forward kept no tape")
         return g[:, 0].permute(0, 3, 1, 2).contiguous()
 
 

@@ -50,7 +50,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import modules as M
-from .engine import AttnDropout, Engine
+from .engine import AttnDropout, Engine, PackCache
 
 __version__ = "0.1.0"
 
@@ -294,7 +294,7 @@ class VideoTokenizer(nn.Module):
         # the loss has a perceptual term without a VGG module (M:1415-1427, gan.py); multiscale discriminators are not built
         self.vgg = None
         self.use_vgg = False
-        self._vgg_cache = {}                    # the VGG's weight packs (vgg.vgg_packs): per model, like _engine
+        self._vgg_cache = PackCache()           # the VGG's engine and weight packs (vgg.vgg_packs): per model, like _engine
         self.perceptual_loss_weight = perceptual_loss_weight
         if isinstance(vgg, nn.Module) and self._has_vgg():
             from .vgg import check_vgg
@@ -369,7 +369,6 @@ class VideoTokenizer(nn.Module):
         # to THIS instance: a copy starts without them and re-packs / re-captures on first use
         eng, self._engine = self._engine, None
         graphs, self._graphs = self._graphs, {}
-        vgg_cache, self._vgg_cache = self._vgg_cache, {}
         try:
             cls = self.__class__
             new = cls.__new__(cls)
@@ -379,14 +378,12 @@ class VideoTokenizer(nn.Module):
         finally:
             self._engine = eng
             self._graphs = graphs
-            self._vgg_cache = vgg_cache
         return new
 
     def __getstate__(self):
         st = dict(self.__dict__)
         st["_engine"] = None
         st["_graphs"] = {}
-        st["_vgg_cache"] = {}
         return st
 
     def copy_for_eval(self):

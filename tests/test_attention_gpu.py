@@ -676,11 +676,11 @@ def test_discriminator_attention_calls(monkeypatch):
     from magvit2_pytorch_b200.modules import Discriminator
     torch.manual_seed(0)
     d = Discriminator(dim=16, image_size=128, max_dim=128).cuda().bfloat16()
-    eng, _ = gan._packs(d)
-    calls = _record(monkeypatch, eng)
+    runner = gan.DiscrRunner(d)
+    calls = _record(monkeypatch, runner.eng)
     images = torch.randn((2, 3, 128, 128), generator=_gen("discr"), device=DEV).bfloat16()
     with torch.no_grad():
-        gan.DiscrRunner(d).forward(images)
+        runner.forward(images)
     torch.cuda.synchronize()
     assert [c["args"]["L"] for c in calls] == [4096, 1024, 256, 64, 16, 16][:len(d.blocks)]
     assert len(calls) == len(d.blocks) and all(c["args"]["heads"] == 16 for c in calls)

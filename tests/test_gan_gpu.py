@@ -137,7 +137,7 @@ def test_bf16_discriminator_convs_run_on_tensor_cores():
     m = _model(g, torch.bfloat16)
     with torch.no_grad():
         m.discr(_images(g, torch.bfloat16))               # packs, engine
-        eng = m.discr._pack[1]
+        eng = m.discr._pack_cache.engine
         eng.conv_log, eng.simt_conv_calls = [], 0
         m.discr(_images(g, torch.bfloat16))
     log, eng.conv_log = eng.conv_log, None

@@ -158,6 +158,17 @@ def test_causal_conv_transpose3d_equivalent_causal_conv(kt, stride):
         m(x)                                                        # CPU-resident: no kernels to run, no eager fallback
 
 
+def test_pack_cache_copies_and_pickles_start_empty():
+    """A filled PackCache holds an engine whose ctypes handles cannot be copied: its copies and pickles are empty caches."""
+    from magvit2_pytorch_b200.engine import Engine, PackCache
+    c = PackCache()
+    c.engine, c.packs, c._sig = Engine(None), {"w": torch.ones(2)}, ("sig", ())
+    for d in (copy.copy(c), copy.deepcopy(c), pickle.loads(pickle.dumps(c))):
+        assert type(d) is PackCache and (d.engine, d.packs, d._sig) == (None, None, None)
+    with pytest.raises(RuntimeError):                               # bound on the module's parameters: CUDA only
+        c.get(torch.nn.Linear(2, 2), "a CPU module", lambda eng: pytest.fail("packed for a CPU module"))
+
+
 def test_stream_lanes_and_round_trip_refuse_cpu_models():
     """The stream front ends are CUDA-only like the model itself: a CPU-resident tokenizer is refused up front."""
     from magvit2_pytorch_b200 import HostRoundTrip, StreamLanes

@@ -97,7 +97,7 @@ def case_train_step():
     torch.manual_seed(1)
     step()                      # warm-up: the discriminator's and the VGG's packs and engines
     torch.manual_seed(2)
-    return _profiled([m.engine, m.discr._pack[1], m._vgg_cache["eng"]], step)
+    return _profiled([m.engine, m.discr._pack_cache.engine, m._vgg_cache.engine], step)
 
 
 def case_lfq_2_18_train():

@@ -521,24 +521,45 @@ def test_attention_small_sequences_kernel(T, HW, D, heads, causal, n_mem):
     assert (a_ - o_).abs().max().item() < 2.0 ** -8 * o_.abs().max().item() + 2e-3     # one bf16 rounding of the output
 
 
+# (kt, stride, cin, cout, then): `then` is done after a first forward and before the checked one -- "new_bias": a bias
+# assigned through .data (new storage, same version counter); "copy": the module deep-copied and pickled
+CONV_T_CASES = [(3, 2, 64, 64, None), (4, 2, 64, 32, None), (3, 1, 64, 64, None), (3, 2, 5, 4, None),
+                (3, 2, 64, 64, "new_bias"), (3, 2, 64, 64, "copy")]
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
-@pytest.mark.parametrize("kt,stride,cin,cout", [(3, 2, 64, 64), (4, 2, 64, 32), (3, 1, 64, 64), (3, 2, 5, 4)])
-def test_causal_conv_transpose3d_vs_oracle(dtype, kt, stride, cin, cout):
+@pytest.mark.parametrize("kt,stride,cin,cout,then",
+                         [pytest.param(*c, id="-".join(str(v) for v in c if v is not None)) for c in CONV_T_CASES])
+def test_causal_conv_transpose3d_vs_oracle(dtype, kt, stride, cin, cout, then):
     """CausalConvTranspose3d (M:990-1024) on the device (one causal conv + depth-to-time) against the CPU restatement."""
     if not torch.cuda.is_available():
         pytest.skip("needs a CUDA device")
+    import copy
+    import pickle
     from magvit2_pytorch_b200.modules import CausalConvTranspose3d
     from oracle.restated import causal_conv_transpose3d
     torch.manual_seed(kt + stride + cin)
     m = CausalConvTranspose3d(cin, cout, (kt, 3, 3), time_stride=stride)
     x = torch.randn(2, cin, 5, 16, 16)
+    bias = torch.randn(cout)
     if dtype == torch.bfloat16:                # identical bf16-representable operands on both sides
         with torch.no_grad():
             m.conv.weight.copy_(m.conv.weight.bfloat16().float()); m.conv.bias.copy_(m.conv.bias.bfloat16().float())
-        x = x.bfloat16().float()
-    want = causal_conv_transpose3d(x, m.conv.weight.detach(), m.conv.bias.detach(), stride)
-    got = m.cuda().to(dtype)(x.cuda().to(dtype)).float().cpu()
-    assert got.shape == want.shape
+        x, bias = x.bfloat16().float(), bias.bfloat16().float()
+    m = m.cuda().to(dtype)
+    xd = x.cuda().to(dtype)
+    mods = [m]
+    if then is not None:
+        m(xd)                                  # packs
+    if then == "new_bias":
+        m.conv.bias.data = bias.cuda().to(dtype)
+    elif then == "copy":
+        mods = [copy.deepcopy(m), pickle.loads(pickle.dumps(m))]
+    want = causal_conv_transpose3d(x, m.conv.weight.detach().float().cpu(), m.conv.bias.detach().float().cpu(), stride)
+    outs = [mod(xd).float().cpu() for mod in mods]
     tol = 1e-5 if dtype == torch.float32 else 2e-2
-    assert (got - want).abs().max().item() < tol * max(1.0, want.abs().max().item())
+    for got in outs:
+        assert got.shape == want.shape
+        assert (got - want).abs().max().item() < tol * max(1.0, want.abs().max().item())
+        assert torch.equal(got, outs[0])

@@ -119,7 +119,7 @@ class _Recorder:
 
     def __init__(self, monkeypatch, m):
         self.m, self.d, self.vgg = m, m.discr, m.vgg
-        engs = {"discr": m.discr._pack[1], "vgg": m._vgg_cache["eng"]}
+        engs = {"discr": m.discr._pack_cache.engine, "vgg": m._vgg_cache.engine}
         self.net = {id(e): n for n, e in engs.items()}
         self.guard = {id(e): _Guard(e) for e in engs.values()}
         self.lib, self.n_sm = engs["discr"].lib, _n_sm()
@@ -137,7 +137,7 @@ class _Recorder:
         monkeypatch.setattr(TapeRunner, "_dgrad", self._dgrad_wrapper(TapeRunner._dgrad, "dgrad"))
         monkeypatch.setattr(DiscrRunner, "_dgrad_s2", self._dgrad_wrapper(DiscrRunner._dgrad_s2, "dgrad_s2"))
         # the packs of the forward convs -> (net, role) of the table
-        P, logits = self.d._pack[2]
+        P, logits = self.d._pack_cache.packs
         self.roles = {id(logits["conv"]): "logits_conv", id(logits["lin"]): "logits_lin"}
         for e in P:
             for k, role in (("net0_kw", "net0_kw"), ("net0", "net0"), ("net2", "net2"), ("down", "down")):
@@ -148,7 +148,7 @@ class _Recorder:
                 self.roles[id(e["attn"][k])] = k
             for k in ("fc1", "fc2"):
                 self.roles[id(e["ff"][k])] = k
-        vp = m._vgg_cache["packs"]
+        vp = m._vgg_cache.packs
         for i, e in enumerate(vp["feats"]):
             self.roles[id(e["pk"])] = "conv"
             if "kw" in e:
@@ -332,7 +332,7 @@ class _Recorder:
         if rec["role"] == "linear2_t":
             _check(y.reshape(B, -1), gx, BF, _gamma(K, C_OF[rec["kind"]]) * S, what)
             return
-        fmap, c_last = self.m._vgg_cache["packs"]["fmap"], self.m._vgg_cache["packs"]["c_last"]
+        fmap, c_last = self.m._vgg_cache.packs["fmap"], self.m._vgg_cache.packs["c_last"]
         out_size = self.vgg.avgpool.output_size
         gm = _pool_adjoint(gx.reshape(B, c_last, *out_size), fmap, out_size).permute(0, 2, 3, 1)
         Sm = _pool_adjoint(S.reshape(B, c_last, *out_size), fmap, out_size).permute(0, 2, 3, 1)
@@ -517,7 +517,7 @@ class _Recorder:
         if rec["op"] != "conv":
             return self._replay_dgrad(rec, gen, defects)
         pk, role = rec["pk"], rec["role"]
-        eng = self.d._pack[1] if rec["net"] == "discr" else self.m._vgg_cache["eng"]
+        eng = self.d._pack_cache.engine if rec["net"] == "discr" else self.m._vgg_cache.engine
         conv = self.orig[(id(eng), "conv")]
         kw = dict(stride=rec["stride"], pad=rec["pad"], out_spatial=rec["out_sp"], act=rec["act"])
         video = res = None
@@ -641,7 +641,7 @@ def test_readme_train_step_calls_vs_float64(monkeypatch):
     seen = {c["key"] for c in calls if "key" in c}
     assert seen == set(rec.table), (set(rec.table) - seen, seen - set(rec.table))
     for eng_id in rec.net:
-        eng = rec.d._pack[1] if rec.net[eng_id] == "discr" else m._vgg_cache["eng"]
+        eng = rec.d._pack_cache.engine if rec.net[eng_id] == "discr" else m._vgg_cache.engine
         assert eng.simt_conv_calls - rec.simt0[eng_id] == sum(c["kind"] == "simt" and c["op"] in ("conv", "dgrad", "dgrad_s2") and
                                           c["net"] == rec.net[eng_id] for c in calls)
     big = [c for c in calls if c["kind"] == "slab" and c["x_shape"][2] == 128]
@@ -658,7 +658,7 @@ def test_readme_train_step_calls_vs_float64(monkeypatch):
             continue
         rejected[c["key"]] = (c["kind"], c.get("plan"), rec.replay(c, gen, defects=True))
     for eng_id, guard in rec.guard.items():
-        eng = rec.d._pack[1] if rec.net[eng_id] == "discr" else m._vgg_cache["eng"]
+        eng = rec.d._pack_cache.engine if rec.net[eng_id] == "discr" else m._vgg_cache.engine
         rec._done(eng, 0, "allocations outside the checked calls")
     n_tap = n_slab = 0
     for key, (kind, plan, got) in rejected.items():

@@ -9,7 +9,7 @@ import synth_data
 from magvit2_pytorch_b200 import VideoTokenizer
 from magvit2_pytorch_b200 import vgg as V
 from magvit2_pytorch_b200._lib import ACT_RELU
-from magvit2_pytorch_b200.engine import Engine, pack_conv
+from magvit2_pytorch_b200.engine import Engine, PackCache, pack_conv
 from tests.test_oracle import grad_digest_close
 from tests.util import golden_video, load_golden
 
@@ -219,9 +219,9 @@ def test_bf16_within_reference_bf16_error_budget(name):
 def test_bf16_vgg_convs_run_on_tensor_cores():
     g = load_golden("mini_vgg16")
     vgg = _vgg(g).cuda().bfloat16().eval()
-    cache = {}
+    cache = PackCache()
     V.VggRunner(vgg, (32, 32), cache=cache).forward(_images(g, torch.bfloat16), record=False)       # packs
-    eng = cache["eng"]
+    eng = cache.engine
     eng.conv_log, eng.simt_conv_calls = [], 0
     r = V.VggRunner(vgg, (32, 32), cache=cache)
     feats = r.forward(_images(g, torch.bfloat16))
@@ -318,12 +318,12 @@ def test_one_and_four_channel_frames_match_reference_repeat_and_slice(channels, 
     gen = torch.Generator(device="cpu").manual_seed(channels)
     x = torch.randn(2, channels, 32, 32, generator=gen).to(dtype)
     gf = torch.randn(2, 32, generator=gen).to(dtype)
-    cache = {}
+    cache = PackCache()
     r = V.VggRunner(vgg, (32, 32), channels, cache)
     feats = r.forward(x.cuda())
     gx = r.backward(gf.cuda())
     if dtype == torch.bfloat16:
-        assert "kw" in cache["packs"]["feats"][0]
+        assert "kw" in cache.packs["feats"][0]
     xr = x.double().requires_grad_(True)
     ref = V.vgg_torch(vgg64, xr.repeat(1, 3, 1, 1) if channels == 1 else xr[:, :3])
     gref, = torch.autograd.grad(ref, xr, gf.double())

@@ -90,7 +90,7 @@ def main():
     with torch.no_grad():
         t_fwd = _time(lambda: d(frames), args.iters * 4)
     # FLOPs of the discriminator's convs (3x3, 1x1 / 2x2 stride 2, to_logits) per forward, from the shapes
-    eng = d._pack[1]
+    eng = d._pack_cache.engine
     eng._prof = []
     with torch.no_grad():
         d(frames)

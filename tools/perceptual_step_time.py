@@ -78,7 +78,7 @@ def main():
             vgg_bwd_prep()
         t_bwd = _time(vgg_bwd, args.iters * 4)
         # FLOPs of the VGG's convs per forward on 8 frames, from the shapes (every wgmma launch: 3x3 convs and the Linears)
-        eng = cache["eng"]
+        eng = cache.engine
         eng._prof = []
         vgg_fwd()
         torch.cuda.synchronize()
