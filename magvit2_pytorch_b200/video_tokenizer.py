@@ -31,8 +31,14 @@ reached parameters; every other call takes the no-grad path unchanged.  ``tokeni
 ``attn_dropout`` (0 <= p < 1) drops the softmax attention weights of train-mode forwards (grad and no-grad) with a Philox
 mask seeded once per call from torch's default CPU generator (engine.AttnDropout, DESIGN.md 3.6); such forwards bypass the
 CUDA graphs.  Eval mode never drops.
-Out of scope (raise at construction / call; SURVEY.md 8f): multiscale discriminators and the discriminator's antialiased
-(Blur) downsampling.
+Multiscale discriminators (``multiscale_discrs=``, M:1085, M:1429-1441) are the user's own torch modules on whole videos and
+torch runs them, as in the reference: ``return_discr_loss`` adds their hinge losses on the video and the detached
+reconstruction (M:1752-1765).  The generator term reproduces the reference's quirk (M:1846-1866): its loop never calls the
+discriminators -- each multiscale generator loss is ``-frames.mean()`` of the image-GAN term's picked reconstruction frames
+(the perceptual term's without an image GAN), and its adaptive weight, with a VGG, is the perceptual gradient norm over that
+loss's (clamped at 1e-5, no NaN fallback).  They are left out of ``parameters()``, ``discr_parameters()``, ``copy_for_eval``
+and the pickled config (the reference trainer builds their optimizers itself), and kept in ``state_dict``.
+Out of scope (raise at construction; SURVEY.md 8f): the discriminator's antialiased (Blur) downsampling.
 """
 from __future__ import annotations
 
@@ -59,6 +65,11 @@ __version__ = "0.1.0"
 LossBreakdown = namedtuple("LossBreakdown", [
     "recon_loss", "lfq_aux_loss", "quantizer_loss_breakdown", "perceptual_loss", "adversarial_gen_loss",
     "adaptive_adversarial_weight", "multiscale_gen_losses", "multiscale_gen_adaptive_weights"])
+
+
+def _hinge_discr_loss(fake, real):
+    """hinge_discr_loss (M:120-121)."""
+    return (F.relu(1 + fake) + F.relu(1 - real)).mean()
 
 
 @dataclass
@@ -291,7 +302,8 @@ class VideoTokenizer(nn.Module):
 
         # training-only branches of the reference.  The perceptual term runs when a VGG module is passed (vgg.py; this
         # package never downloads torchvision's weights, M:1397-1405); the image discriminator is built for the GAN term unless
-        # the loss has a perceptual term without a VGG module (M:1415-1427, gan.py); multiscale discriminators are not built
+        # the loss has a perceptual term without a VGG module (M:1415-1427, gan.py); the multiscale discriminators are the
+        # user's modules, held even when the flags are off (M:1429-1441)
         self.vgg = None
         self.use_vgg = False
         self._vgg_cache = PackCache()           # the VGG's engine and weight packs (vgg.vgg_packs): per model, like _engine
@@ -308,9 +320,9 @@ class VideoTokenizer(nn.Module):
             kw = dict(dim=dim, image_size=image_size, channels=channels, max_dim=512) if discr_kwargs is None else dict(discr_kwargs)
             self.discr = M.Discriminator(**kw)
             self.has_gan = True
-        self.has_multiscale_gan = False
-        self.has_multiscale_discrs = False
-        self.multiscale_discrs = nn.ModuleList([])
+        self.has_multiscale_gan = bool(use_gan and multiscale_adversarial_loss_weight > 0.)
+        self.multiscale_discrs = nn.ModuleList([*multiscale_discrs])
+        self.has_multiscale_discrs = bool(self.has_multiscale_gan and len(multiscale_discrs) > 0)
         self.adversarial_loss_weight = adversarial_loss_weight
         self.grad_penalty_loss_weight = grad_penalty_loss_weight
         self.multiscale_adversarial_loss_weight = multiscale_adversarial_loss_weight
@@ -356,10 +368,12 @@ class VideoTokenizer(nn.Module):
 
     def load_state_dict(self, state_dict, strict: bool = True, **kw):
         # reference checkpoints carry discriminator weights (always constructed, M:1422); a model that built no
-        # discriminator drops them, as it drops the multiscale discriminators'.  Checkpoints carry no VGG weights (M:1491-1493):
-        # any in `state_dict` are ignored and the VGG keeps its own, which stand in for its keys under strict loading.
+        # discriminator drops them, and a model that holds no multiscale discriminators drops theirs (init_and_load_from builds
+        # none).  Checkpoints carry no VGG weights (M:1491-1493): any in `state_dict` are ignored and the VGG keeps its own,
+        # which stand in for its keys under strict loading.
         sd = {k: v for k, v in state_dict.items()
-              if not ((self.discr is None and k.startswith("discr.")) or k.startswith("multiscale_discrs.") or k.startswith("vgg."))}
+              if not ((self.discr is None and k.startswith("discr.")) or k.startswith("vgg.")
+                      or (len(self.multiscale_discrs) == 0 and k.startswith("multiscale_discrs.")))}
         if self.vgg is not None:
             sd.update(("vgg." + k, v) for k, v in self.vgg.state_dict(keep_vars=True).items())
         return super().load_state_dict(sd, strict=strict, **kw)
@@ -387,24 +401,31 @@ class VideoTokenizer(nn.Module):
         return st
 
     def copy_for_eval(self):
-        """An eval-mode copy without the VGG (M:1476-1485): its return_loss raises like a model built with vgg=None."""
+        """An eval-mode copy without the VGG and the multiscale discriminators (M:1476-1485): its return_loss raises like a
+        model built with vgg=None, and has no multiscale terms."""
         dev = self.device
-        memo = {} if self.vgg is None else {id(self.vgg): None}      # the copy's `vgg` entry is None: the VGG is not copied
+        memo = {id(self.multiscale_discrs): nn.ModuleList()}          # neither the multiscale discriminators ...
+        if self.vgg is not None:
+            memo[id(self.vgg)] = None                                 # ... nor the VGG is copied: the copy's `vgg` entry is None
         c = copy.deepcopy(self.cpu(), memo)
         self.to(dev)
         c.vgg, c.use_vgg = None, False
+        c.has_multiscale_discrs = False
         c.eval()
         return c.to(dev)
 
     @classmethod
     def init_and_load_from(cls, path, strict=True):
+        """M:1447-1458: a model built from the checkpoint's pickled config, which stores neither the VGG nor the multiscale
+        discriminators: the model has neither, and the checkpoint's multiscale discriminator weights are dropped."""
         path = Path(path)
         assert path.exists()
         pkg = torch.load(str(path), map_location="cpu", weights_only=False)
         assert "config" in pkg, "model configs were not found in this saved checkpoint"
         config = pickle.loads(pkg["config"])
         # reference checkpoints pickle module-valued kwargs we do not build; the VGG is never saved, so a model loaded here
-        # has none (vgg=None): pass the VGG module to the constructor and load_state_dict to train with the perceptual term
+        # has none (vgg=None): pass the VGG module to the constructor and load_state_dict to train with the perceptual term;
+        # likewise the multiscale discriminators
         for k in ("vgg", "lfq_activation"):
             config[k] = None
         config["multiscale_discrs"] = tuple()
@@ -675,9 +696,11 @@ class VideoTokenizer(nn.Module):
         """The reference forward (M:1657-1896): inference returns (codes / reconstruction), ``return_recon_loss_only``,
         ``return_discr_loss`` and ``return_loss``: ``(total_loss, LossBreakdown)`` with ``total_loss = recon_loss + aux_loss *
         quantizer_aux_loss_weight + perceptual_loss * perceptual_loss_weight + gen_loss * adaptive_weight *
-        adversarial_loss_weight`` (M:1868-1896).  The perceptual term needs a ``vgg=`` module; the adaptive weight is the ratio
-        of the perceptual and adversarial terms' gradient norms at ``conv_out.conv.weight`` in a train-mode step (M:1812-1841),
-        1 in eval mode."""
+        adversarial_loss_weight + sum(multiscale_gen_losses * multiscale weights) * multiscale_adversarial_loss_weight``
+        (M:1868-1896).  The perceptual term needs a ``vgg=`` module; the adaptive weights are the ratio of the perceptual and
+        adversarial terms' gradient norms at ``conv_out.conv.weight`` in a train-mode step (M:1812-1868), 1 in eval mode.  The
+        call-site ``adversarial_loss_weight`` / ``multiscale_adversarial_loss_weight`` default to the attributes; the
+        discriminator step's total uses the attribute (M:1776-1779)."""
         assert (return_loss + return_codes + return_discr_loss) <= 1               # M:1674
         if return_discr_loss and self.discr is None:
             raise NotImplementedError("return_discr_loss needs the image discriminator, which is built for use_gan=True, "
@@ -685,18 +708,23 @@ class VideoTokenizer(nn.Module):
                                       "(SURVEY.md 8f N2)")
         if return_loss and self._needs_gan_or_vgg():
             raise NotImplementedError(
-                "return_loss with the perceptual term needs a `vgg=` module (this package downloads no VGG weights), and "
-                "multiscale discriminators (reference M:1846-1866) are outside the accelerated path (SURVEY.md 8f N2): pass "
+                "return_loss with the perceptual term needs a `vgg=` module (this package downloads no VGG weights): pass "
                 "vgg=<module> or construct with perceptual_loss_weight=0.")
+        if return_loss and self.has_multiscale_discrs and not (self.has_gan or self.use_vgg):
+            raise ValueError("the multiscale generator terms are taken on the image discriminator's or the perceptual term's "
+                             "frame pick (M:1846-1850), and this model has neither (the reference fails with UnboundLocalError "
+                             "here): construct with adversarial_loss_weight > 0 or pass a `vgg=` module")
         grad_step = (return_loss and self.training and torch.is_grad_enabled()
                      and any(p.requires_grad for p in self.parameters()))
-        if return_loss and self.training and self.use_vgg and self.has_gan and not grad_step:
+        if return_loss and self.training and self.use_vgg and (self.has_gan or self.has_multiscale_discrs) and not grad_step:
             raise RuntimeError("a train-mode return_loss with a VGG and a GAN needs gradients: the adaptive adversarial weight is "
                                "a ratio of gradient norms (M:1812-1841; the reference fails in torch.autograd.grad here)")
         video, ff = self._check_video(video_or_images, video_contains_first_frame)
         cond = self._check_cond(cond, video.shape[0])
-        if adversarial_loss_weight is None:                                        # the call-site weight wins (M:1674-1680)
+        if adversarial_loss_weight is None:                                        # the call-site weights win (M:1671-1672)
             adversarial_loss_weight = self.adversarial_loss_weight
+        if multiscale_adversarial_loss_weight is None:
+            multiscale_adversarial_loss_weight = self.multiscale_adversarial_loss_weight
         if return_discr_loss:
             return self._discr_loss(video, ff, cond, apply_gradient_penalty)
         if grad_step:
@@ -710,15 +738,26 @@ class VideoTokenizer(nn.Module):
             aux_losses = aux.to(recon_loss.dtype)
             total_loss = recon_loss + aux_losses * self.quantizer_aux_loss_weight                # M:1868-1871
             perceptual_loss, g_perc = self._perceptual_loss(target, recon)
+            # the perceptual gradient norm at the last decoder layer, for the adaptive weights (M:1817-1820)
+            norm_p = None
+            if self.use_vgg and (self.has_gan or self.has_multiscale_discrs):
+                norm_p = self._last_layer_grad_norm(runner, recon, *g_perc)
             gen_loss, g_gen = self._gen_loss(recon)
             adaptive_weight = 0.
             if self.has_gan:
-                adaptive_weight = self._adaptive_weight(runner, recon, g_perc, g_gen) if self.use_vgg else 1.
+                adaptive_weight = 1.
+                if norm_p is not None:                                                             # M:1833-1841
+                    w = self._adaptive_weight(norm_p, self._last_layer_grad_norm(runner, recon, *g_gen), 1e-3)
+                    adaptive_weight = 1. if torch.isnan(w).any() else w
+            ms_losses, ms_weights = self._multiscale_gen_terms(recon, g_gen if self.has_gan else g_perc, runner, norm_p)
             if self.use_vgg:
                 total_loss = total_loss + perceptual_loss * self.perceptual_loss_weight
             if self.has_gan:
                 total_loss = total_loss + gen_loss * adaptive_weight * adversarial_loss_weight   # M:1872-1875
-            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, perceptual_loss, gen_loss, adaptive_weight, [], [])
+            if self.has_multiscale_discrs:                                                         # M:1877-1881
+                total_loss = total_loss + sum(l * w for l, w in zip(ms_losses, ms_weights)) * multiscale_adversarial_loss_weight
+            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, perceptual_loss, gen_loss, adaptive_weight,
+                                             ms_losses, ms_weights)
         with torch.no_grad():
             eng = self.engine
             need_recon = return_recon or return_recon_loss_only or return_loss or not return_codes
@@ -733,20 +772,24 @@ class VideoTokenizer(nn.Module):
             recon_loss = eng.mse(video, recon).to(self.dtype)                      # M:1722
             if return_recon_loss_only:                                             # M:1726-1727
                 return recon_loss, recon
-            # M:1868-1896 without multiscale discriminators: perceptual_loss = zero without a VGG; gen_loss = zero and
-            # adaptive_weight = 0. without a discriminator, adaptive_weight = 1. with one (no gradients here, M:1833)
+            # M:1868-1896: perceptual_loss = zero without a VGG; gen_loss = zero and adaptive_weight = 0. without a
+            # discriminator, adaptive_weight = 1. with one, and every multiscale weight 1. (no gradients here, M:1833, M:1861)
             zero = self.zero
             aux_losses = zero if aux is None else aux.to(recon_loss.dtype)         # eval mode / FSQ: M:1700-1703
             total_loss = recon_loss + aux_losses * self.quantizer_aux_loss_weight
-            perceptual_loss, _ = self._perceptual_loss(video.float() / 255. if video.dtype == torch.uint8 else video, recon)
+            perceptual_loss, g_perc = self._perceptual_loss(video.float() / 255. if video.dtype == torch.uint8 else video, recon)
             if self.use_vgg:
                 total_loss = total_loss + perceptual_loss * self.perceptual_loss_weight
-            gen_loss, _ = self._gen_loss(recon)
+            gen_loss, g_gen = self._gen_loss(recon)
             adaptive_weight = 1. if self.has_gan else 0.
             if self.has_gan:
                 total_loss = total_loss + gen_loss * adaptive_weight * adversarial_loss_weight
+            ms_losses, ms_weights = self._multiscale_gen_terms(recon, g_gen if self.has_gan else g_perc)
+            if self.has_multiscale_discrs:
+                total_loss = total_loss + sum(l * w for l, w in zip(ms_losses, ms_weights)) * multiscale_adversarial_loss_weight
             qlb = None if (self.use_fsq or aux is None) else self.quantizer_loss_breakdown
-            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, perceptual_loss, gen_loss, adaptive_weight, [], [])
+            return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, perceptual_loss, gen_loss, adaptive_weight,
+                                             ms_losses, ms_weights)
 
     def _no_grad_forward(self, eng, video, ff, cond, need_recon):
         """The tokenizer forward without gradients -> (codes | (codes, recon), train-mode LFQ aux loss | None)."""
@@ -777,26 +820,26 @@ class VideoTokenizer(nn.Module):
 
     def _gen_loss(self, recon):
         """The adversarial generator term (M:1826-1831): -discr(frames).mean() on one random frame per clip, drawn from the
-        default CPU generator as the reference does -> (loss, (frame indices, d loss / d frames) | None); (zero, None)
+        default CPU generator as the reference does -> (loss, (frame indices, d loss / d frames | None)); (zero, None)
         without a discriminator."""
         if not self.has_gan:
             return self.zero, None
         from .gan import generator_term
         frame_indices = torch.randn((recon.shape[0], recon.shape[2])).topk(1, dim=-1).indices
         loss, info = generator_term(self.discr, self._pick_frames(recon, frame_indices))
-        return loss, (frame_indices, info["grad_images"]) if "grad_images" in info else None
+        return loss, (frame_indices, info.get("grad_images"))
 
     def _perceptual_loss(self, target, recon):
         """The perceptual term (M:1788-1808): F.mse_loss of the VGG features of one random frame per clip (drawn before the
-        generator term's, M:1792) of the target and the reconstruction -> (loss, (frame indices, d loss / d recon frames) |
-        None); (zero, None) without a VGG."""
+        generator term's, M:1792) of the target and the reconstruction -> (loss, (frame indices, d loss / d recon frames |
+        None)); (zero, None) without a VGG."""
         if not self.use_vgg:
             return self.zero, None
         from .vgg import perceptual_loss
         frame_indices = torch.randn((recon.shape[0], recon.shape[2])).topk(1, dim=-1).indices
         real = self._pick_frames(target, frame_indices).to(self.dtype).contiguous()
         loss, info = perceptual_loss(self.vgg, real, self._pick_frames(recon, frame_indices), self.channels, self._vgg_cache)
-        return loss, (frame_indices, info["grad_frames"]) if "grad_frames" in info else None
+        return loss, (frame_indices, info.get("grad_frames"))
 
     @staticmethod
     def _scatter_frames(recon, frame_indices, g_frames):
@@ -805,18 +848,41 @@ class VideoTokenizer(nn.Module):
         g.transpose(1, 2)[torch.arange(recon.shape[0], device=recon.device), frame_indices[:, 0].to(recon.device)] = g_frames
         return g
 
-    def _adaptive_weight(self, runner, recon, g_perc, g_gen):
-        """M:1812-1841: |d perceptual / d W| / max(|d gen / d W|, 1e-3), clamped at 1e3 (NaN -> 1.), W = conv_out.conv.weight,
+    def _last_layer_grad_norm(self, runner, recon, frame_indices, g_frames):
+        """|d loss / d W|, W = conv_out.conv.weight, for a loss on the picked reconstruction frames with gradient g_frames,
         from the tokenizer's saved activations (TrainRunner.last_layer_weight_grad) -- no backward runs."""
-        norm_p = runner.last_layer_weight_grad(self._scatter_frames(recon, *g_perc)).norm(p=2)
-        norm_g = runner.last_layer_weight_grad(self._scatter_frames(recon, *g_gen)).norm(p=2)
-        w = (norm_p / norm_g.clamp(min=1e-3)).clamp(max=1e3)
-        return 1. if torch.isnan(w).any() else w.detach()
+        return runner.last_layer_weight_grad(self._scatter_frames(recon, frame_indices, g_frames)).norm(p=2)
+
+    @staticmethod
+    def _adaptive_weight(norm_p, norm_g, eps):
+        """M:1836-1838 / M:1864-1866: norm_p / max(norm_g, eps), clamped at 1e3."""
+        return (norm_p / norm_g.clamp(min=eps)).clamp(max=1e3).detach()
+
+    def _multiscale_gen_terms(self, recon, picked, runner=None, norm_p=None):
+        """The multiscale generator terms (M:1846-1866) -> (losses, adaptive weights), one of each per multiscale
+        discriminator; ([], []) without them.  The reference's loop sets ``fake_logits = recon_video_frames`` and never calls
+        the discriminator, so every loss is hinge_gen_loss(frames) = -frames.mean() of the same picked reconstruction frames
+        (picked: the image-GAN term's (frame indices, ...), or the perceptual term's without an image GAN) -- no new random
+        draw.  Every weight is then the same: norm_p over the loss's last-layer gradient norm (clamped at 1e-5, no NaN
+        fallback) when the perceptual norm norm_p exists, else 1."""
+        if not self.has_multiscale_discrs:
+            return [], []
+        frame_indices = picked[0]
+        frames = self._pick_frames(recon, frame_indices)
+        loss = -frames.mean()
+        weight = 1.
+        if norm_p is not None:
+            g_frames = torch.full(frames.shape, -1. / frames.numel(), device=recon.device, dtype=recon.dtype)
+            weight = self._adaptive_weight(norm_p, self._last_layer_grad_norm(runner, recon, frame_indices, g_frames), 1e-5)
+        n = len(self.multiscale_discrs)
+        return [loss] * n, [weight] * n
 
     def _discr_loss(self, video, ff, cond, apply_gradient_penalty):
         """``return_discr_loss`` (M:1731-1786): the tokenizer runs without gradients (as the no-grad forward, including the
         train-mode LFQ all-reduce), then the hinge loss of the device discriminator on one real and one reconstructed frame
-        per clip, plus the gradient penalty (gan.gradient_penalty) when asked for."""
+        per clip, the hinge loss of each multiscale discriminator on the whole real and reconstructed videos (torch runs the
+        user's modules; a uint8 video is passed as x / 255 in the model's dtype), plus the image discriminator's gradient
+        penalty (gan.gradient_penalty) when asked for."""
         from .gan import DiscrLossBreakdown, gradient_penalty
         with torch.no_grad():
             (_, recon), _ = self._no_grad_forward(self.engine, video, ff, cond, True)
@@ -825,12 +891,19 @@ class VideoTokenizer(nn.Module):
         real = self._pick_frames(frames, frame_indices).to(self.dtype).contiguous()
         fake = self._pick_frames(recon, frame_indices).detach().contiguous()
         real_logits, fake_logits = self.discr(real), self.discr(fake)
-        discr_loss = (F.relu(1 + fake_logits) + F.relu(1 - real_logits)).mean()           # hinge_discr_loss (M:120-121)
+        discr_loss = _hinge_discr_loss(fake_logits, real_logits)
+        multiscale = [self.zero]
+        if self.has_multiscale_discrs:                                                     # M:1752-1765
+            real_video = frames.to(self.dtype) if video.dtype == torch.uint8 else video
+            fake_video = recon.detach()
+            multiscale = []
+            for d in self.multiscale_discrs:
+                real_ms = d(real_video)
+                multiscale.append(_hinge_discr_loss(d(fake_video), real_ms))
         if apply_gradient_penalty:
             gp = gradient_penalty(self.discr, real) + gradient_penalty(self.discr, fake)
         else:
             gp = self.zero
-        multiscale = [self.zero]
         total = discr_loss + gp * self.grad_penalty_loss_weight + sum(multiscale) * self.multiscale_adversarial_loss_weight
         return total, DiscrLossBreakdown(discr_loss, multiscale, gp)
 
@@ -840,9 +913,8 @@ class VideoTokenizer(nn.Module):
 
     def _needs_gan_or_vgg(self) -> bool:
         """True when the loss needs a term this package does not build: the perceptual term without a VGG module (M:1392),
-        multiscale discriminators (M:1435), or the GAN term of a model that built no discriminator (M:1427)."""
-        return bool((self._has_vgg() and not self.use_vgg) or (self.use_gan and self.adversarial_loss_weight > 0. and self.discr is None)
-                    or self.has_multiscale_discrs)
+        or the GAN term of a model that built no discriminator (M:1427)."""
+        return bool((self._has_vgg() and not self.use_vgg) or (self.use_gan and self.adversarial_loss_weight > 0. and self.discr is None))
 
     @property
     def dtype(self):
