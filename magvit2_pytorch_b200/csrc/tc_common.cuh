@@ -49,6 +49,16 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
+// shared -> global box store, completed through this thread's bulk async-groups
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// waits until this thread's bulk stores have read their shared-memory sources (the buffers may be written again)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// waits until this thread's bulk stores are complete
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
@@ -174,16 +184,17 @@ __device__ __forceinline__ void store8_bf16(__nv_bfloat16* dst, const float (&v)
 
 // Epilogue flavours are compile-time so each kernel instance carries only the code it runs (the generic version was
 // ~2300 SASS instructions per 32-column chunk and thrashed the instruction cache of the 8 epilogue warps).
-// EPI_PLAIN (slab kernel only) additionally requires Co % 8 == 0 and stores through a shared-memory transpose;
+// EPI_PLAIN (slab kernel only) additionally requires Co % 8 == 0; its epilogue runs on the accumulator fragments and
+// stores through TMA (tc_slab.cu: slab_epi_fragment);
 // EPI_RAGGED is the direct per-row path with scalar tails (conv_out's 3 channels, and the tap kernel's plain mode).
-// EPI_PLAIN_RES is EPI_PLAIN with a residual input: each lane reads its own row's residual (64 contiguous bytes per chunk)
-// and act(conv + bias) + res is summed in fp32 and rounded to bf16 ONCE (the reference's bf16 `fn(x) + x` rounds twice; the
-// single rounding is strictly closer to the fp32 result).
+// EPI_PLAIN_RES is EPI_PLAIN with a residual input (TMA-loaded into shared memory under the main loop): act(conv + bias)
+// + res is summed in fp32 and rounded to bf16 ONCE (the reference's bf16 `fn(x) + x` rounds twice; the single rounding
+// is strictly closer to the fp32 result).
 // EPI_FUSED_RU (slab kernel only): the whole conv half of a ResidualUnit in one launch -- the ELU'd 3x3x3 tile goes to
 // shared memory as the A operand of a second wgmma against the 1x1x1 weights, and the second epilogue emits the
 // SqueezeExcite online-softmax pool partials next to y (see tc_slab.cu).
-// EPI_SHUFFLE_ST (slab kernel only): depth-to-space / depth-to-time stores through the same shared-memory transpose as
-// EPI_PLAIN (64 contiguous bytes per output position and store instruction); needs Cy % 32 == 0 so that a 32-column chunk
+// EPI_SHUFFLE_ST (slab kernel only): depth-to-space / depth-to-time stores through a shared-memory transpose of the
+// staged accumulators (64 contiguous bytes per output position and store instruction); needs Cy % 32 == 0 so that a 32-column chunk
 // stays inside one sub-pixel phase.  EPI_SHUFFLE is the direct 16-byte-piece path for the other widths.
 // EPI_DOWN_SPACE (slab kernel only): SpatialDownsample2x (3x3, stride 2) -- plain epilogue, but the slab is two row-parity
 // sub-slabs of the input viewed as (W/2) x (2C) and the taps follow a small offset table (see tc_slab.cu).
@@ -336,24 +347,6 @@ __device__ __forceinline__ void epi_pack32_t(const uint32_t (&r)[32], const floa
     pk[2 * g] = pack_bf16x2(act_ct<ACT>(__uint_as_float(r[4 * g]) + b.x, relu), act_ct<ACT>(__uint_as_float(r[4 * g + 1]) + b.y, relu));
     pk[2 * g + 1] = pack_bf16x2(act_ct<ACT>(__uint_as_float(r[4 * g + 2]) + b.z, relu), act_ct<ACT>(__uint_as_float(r[4 * g + 3]) + b.w, relu));
   }
-}
-// bias + activation of one 32-column chunk, kept in fp32 (for the fp32-staged residual epilogue)
-template <int ACT>
-__device__ __forceinline__ void epi_act32_t(uint32_t (&r)[32], const float* sb, bool relu = false) {
-#pragma unroll
-  for (int g = 0; g < 8; ++g) {
-    const float4 b = *reinterpret_cast<const float4*>(sb + g * 4);
-    r[4 * g] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g]) + b.x, relu));
-    r[4 * g + 1] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g + 1]) + b.y, relu));
-    r[4 * g + 2] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g + 2]) + b.z, relu));
-    r[4 * g + 3] = __float_as_uint(act_ct<ACT>(__uint_as_float(r[4 * g + 3]) + b.w, relu));
-  }
-}
-__device__ __forceinline__ void epi_act32(int act, uint32_t (&r)[32], const float* sb) {
-  if (act == MV2_ACT_ELU) epi_act32_t<MV2_ACT_ELU>(r, sb);
-  else if (act == MV2_ACT_SILU) epi_act32_t<MV2_ACT_SILU>(r, sb);
-  else if (act == MV2_ACT_LEAKY_RELU || act == MV2_ACT_RELU) epi_act32_t<MV2_ACT_LEAKY_RELU>(r, sb, act == MV2_ACT_RELU);
-  else epi_act32_t<MV2_ACT_NONE>(r, sb);
 }
 __device__ __forceinline__ void epi_pack32(int act, const uint32_t (&r)[32], const float* sb, uint32_t (&pk)[16]) {
   if (act == MV2_ACT_ELU) epi_pack32_t<MV2_ACT_ELU>(r, sb, pk);

@@ -14,17 +14,17 @@
 //   * CTAs are persistent with a static, cost-sorted serpentine tile schedule (slab_frame_of / slab_tile_of);
 //   * causal frames in front of the clip (t + dt - pt < 0) come from the history map (hmap: the tail of the previous chunk
 //     of a streamed clip, hist_T frames); those in front of the history are all-zero and are skipped outright;
-//   * N tiles need not divide Co (the plain / GEGLU epilogues guard every stored column): wide outputs without a
+//   * N tiles need not divide Co (TMA clips the plain / GEGLU stores at Co): wide outputs without a
 //     128-column divisor take 128-column tiles with a ragged last one;
-//   * the kernel is instantiated per epilogue flavour (tc_common.cuh: EPI_*) and N tile (32 / 64 / 128); the plain
-//     flavour transposes each 32 x 32 chunk through shared memory so stores / residual loads are 64-byte contiguous per row.
+//   * the kernel is instantiated per epilogue flavour (tc_common.cuh: EPI_*) and N tile (32 / 64 / 128); the plain,
+//     residual, GEGLU and SpatialDownsample2x flavours run the epilogue on the accumulator fragments and store bf16
+//     boxes through TMA (slab_epi_fragment), the others stage the accumulators in shared memory first.
 //     The channels-first flavour (EPI_RAGGED: fewer than 32 output channels, so never a wider tile than 32) has narrow
 //     8- and 16-column tiles (wgmma m64n8k16 / m64n16k16) instead, for the data gradient of conv_in with respect to the
 //     video: 3 output channels, 7 x 7 in-plane taps (slab_narrow).
-// Warp roles (384 threads): w0 slab TMA producer, w2 weight TMA producer (40 registers each, setmaxnreg), w4-7 / w8-11
-// two consumer warpgroups (232 registers): each issues the wgmma of 64 of the 128 positions of every M-tile, with one
-// commit group in flight across ring stages, stages its accumulators in shared memory and runs the epilogue on them
-// (one output row per thread and 32-column chunk).
+// Warp roles (384 threads): w0 slab TMA producer, w1 residual TMA producer (EPI_PLAIN_RES), w2 weight TMA producer
+// (40 registers each, setmaxnreg), w4-7 / w8-11 two consumer warpgroups (232 registers): each issues the wgmma of 64 of
+// the 128 positions of every M-tile, with one commit group in flight across ring stages, and runs the epilogue.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include <cuda.h>
@@ -64,7 +64,22 @@ struct alignas(64) SlabParams {
   int dn_aoff[6];        // per tap' = dh * 2 + (dw2 + 1): A-descriptor start offset inside the stage, in 16-byte units
   int dn_lower;          // K-chunks of the lower (pw = 0) half of the 2C axis: they only see the dw2 = 0 taps
   int h_stride;          // bytes of the shared-memory H buffer (ELU'd 3x3x3 tile of one M-tile) = kchunks * 16 KB
+  // ---- TMA-store flavours (slab_tma_epi: EPI_PLAIN, EPI_PLAIN_RES, EPI_GEGLU, EPI_DOWN_SPACE) ----
+  CUtensorMap ymap;      // y as {Co (GEGLU: Co / 2), W, H, T, B}: boxes {cb, 8, 8, 1, 1}, one per 64 positions and cb channels
+  CUtensorMap rmap;      // EPI_PLAIN_RES: the residual, same view and boxes as ymap
 };
+
+// Flavours whose epilogue runs on the accumulator fragments and stores through TMA; the others stage the accumulators in
+// shared memory first (the fused ResidualUnit's second GEMM reads the staged tile, the channels-first and shuffled stores
+// need a row per thread).
+__host__ __device__ constexpr bool slab_tma_epi(int mode) {
+  return mode == EPI_PLAIN || mode == EPI_PLAIN_RES || mode == EPI_GEGLU || mode == EPI_DOWN_SPACE;
+}
+// Channels of one output box of a TMA-store flavour with an N tile of bn columns: one 128-byte swizzled row (64
+// channels), or the whole tile when its output is narrower (GEGLU writes bn / 2 channels)
+__host__ __device__ constexpr int slab_out_box_ch(int mode, int bn) {
+  return (mode == EPI_GEGLU ? bn / 2 : bn) < 64 ? (mode == EPI_GEGLU ? bn / 2 : bn) : 64;
+}
 
 // Frames are enumerated most-expensive first: the B * (T - pt) frames that see all kt frame taps, then the frames
 // t = pt-1, pt-2, ..., 0 of every clip (their leading taps fall into the causal padding and are skipped, so their tiles
@@ -104,7 +119,12 @@ __host__ __device__ __forceinline__ TileCoord decode_tile(const SlabParams& p, i
 // Shared-memory layout behind the two TMA rings (host and kernel must agree): barriers, bias, the eight 2 KB
 // epilogue transpose buffers, [fused: logit partials], the fp32 accumulator staging of both consumer warpgroups
 // (mw M-tiles x 64 rows x (bn + 4) each), [fused: the H buffer].
-struct SlabSmem { uint32_t sbias, stage0, lpart, accstg, hbuf, end; };
+// The TMA-store flavours use the span of the transpose buffers and the staging for other things: the residual
+// full / empty barriers of both warpgroups, then (1024-byte aligned, for the swizzled boxes) the bf16 output tiles and
+// the residual tiles of both warpgroups, 2 x mw x 64 x bn x 2 bytes each.  Together they take at most
+// 32 + 1023 + 512 mw bn bytes of the 16 KB + 512 mw (bn + 4) the span has, so the span, and with it every launch's
+// plan, is the same for all flavours but the fused one.
+struct SlabSmem { uint32_t sbias, stage0, lpart, accstg, hbuf, end, rbar, otile, rtile; };
 __host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& p, uint32_t bar0, bool fused) {
   SlabSmem m;
   m.sbias = (bar0 + 8 * (2 * p.slab_stages + 2 * p.w_stages) + 15) & ~15u;
@@ -114,10 +134,79 @@ __host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& 
   m.hbuf = m.accstg + 2u * p.mw * 64 * (p.bn + 4) * 4;
   if (fused) m.hbuf = (m.hbuf + 1023u) & ~1023u;        // SWIZZLE_128B operand tiles: 1024-byte aligned
   m.end = m.hbuf + (fused ? (uint32_t)p.h_stride : 0);
+  m.rbar = m.stage0;
+  m.otile = (m.rbar + 32 + 1023u) & ~1023u;
+  m.rtile = m.otile + 2u * p.mw * 64 * p.bn * 2;
   return m;
 }
 
-// Every instantiation runs 384 threads: warp 0 slab TMA producer, warp 2 weight TMA producer (warps 1 and 3 idle), warps
+// Epilogue of the TMA-store flavours on one consumer warpgroup's accumulators, in fragment layout: thread (warp wq of
+// the warpgroup, lane) holds rows m0 = 16 wq + lane / 4 and m0 + 8 of every M-tile (row m = output position
+// (h0 + 8 wg + m / 8, w0 + 8 j + m % 8)) and columns 8 g + 2 (lane % 4) + {0, 1}.  The math per element is that of the
+// staged epilogue, in the same order: x oscale, + bias and activation, [+ residual in fp32, x 2^-0.5 in mode 2], one
+// rounding to bf16; GEGLU pairs packed column 16 g + c (x) with 16 g + 8 + c (its gate), which the same thread holds.
+// Results go to the output tile `ot` as [mw][boxes][64 rows][cb channels] bf16 boxes in the swizzle TMA uses for their
+// row width; the residual is read from `rt` in the same layout.  Bank-conflict free: the 8 rows of a warp's access
+// fall on 8 different 16-byte units of the swizzle.
+template <int MODE, int BN, int ACT, int MWMAX>
+__device__ __forceinline__ void slab_epi_fragment(const SlabParams& p, const float (&acc)[MWMAX][BN / 2], const TileCoord& c,
+                                                  const float* sbias, uint32_t ot, uint32_t rt, int wq, int lane, bool relu) {
+  constexpr int OC = MODE == EPI_GEGLU ? BN / 2 : BN, CB = slab_out_box_ch(MODE, BN), NB = OC / CB;
+  constexpr uint32_t RB = CB * 2, BOX = 64 * RB, SWZ = (RB / 16 - 1) << 4;
+  const uint32_t m0 = 16 * wq + (lane >> 2), q4 = (lane & 3) * 4;
+  auto at = [&](int j, int col, uint32_t m) {        // byte offset of (row m, output columns col, col + 1) of M-tile j
+    const uint32_t off = m * RB + (uint32_t)(col % CB) * 2 + q4;
+    return (uint32_t)(j * NB + col / CB) * BOX + (off ^ ((off >> 3) & SWZ));
+  };
+  auto st32 = [](uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); };
+  const float* os = (MODE == EPI_PLAIN || MODE == EPI_PLAIN_RES) && p.epi.oscale ? p.epi.oscale + (int64_t)c.b * p.Co : nullptr;
+  const float rs = MODE == EPI_PLAIN_RES && p.epi.mode == 2 ? 0.70710678118654752440f : 1.f;
+#pragma unroll
+  for (int j = 0; j < MWMAX; ++j) {
+    if (j >= p.mw) break;
+    if (MODE == EPI_GEGLU) {
+#pragma unroll
+      for (int g = 0; g < BN / 16; ++g) {
+        const int n = c.n0 + 16 * g + 2 * (lane & 3);
+        const float2 bx = *reinterpret_cast<const float2*>(sbias + n), bg = *reinterpret_cast<const float2*>(sbias + n + 8);
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          const float* xv = &acc[j][8 * g + 2 * hr];
+          const float* gv = &acc[j][8 * g + 4 + 2 * hr];
+          const float v0 = gelu_fast(gv[0] + bg.x) * (xv[0] + bx.x);
+          const float v1 = gelu_fast(gv[1] + bg.y) * (xv[1] + bx.y);
+          st32(ot + at(j, 8 * g, m0 + 8 * hr), pack_bf16x2(v0, v1));
+        }
+      }
+    } else {
+#pragma unroll
+      for (int g = 0; g < BN / 8; ++g) {
+        const int col = 8 * g, n = c.n0 + col + 2 * (lane & 3);
+        const float2 b = *reinterpret_cast<const float2*>(sbias + n);
+        float o0 = 1.f, o1 = 1.f;
+        if (os) { o0 = n < p.Co ? os[n] : 0.f; o1 = n + 1 < p.Co ? os[n + 1] : 0.f; }
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+          float v0 = acc[j][4 * g + 2 * hr], v1 = acc[j][4 * g + 2 * hr + 1];
+          if (os) { v0 *= o0; v1 *= o1; }
+          v0 = act_ct<ACT>(v0 + b.x, relu);
+          v1 = act_ct<ACT>(v1 + b.y, relu);
+          const uint32_t a = at(j, col, m0 + 8 * hr);
+          if (MODE == EPI_PLAIN_RES) {
+            uint32_t r;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(rt + a) : "memory");
+            v0 = (v0 + __uint_as_float(r << 16)) * rs;
+            v1 = (v1 + __uint_as_float(r & 0xffff0000u)) * rs;
+          }
+          st32(ot + a, pack_bf16x2(v0, v1));
+        }
+      }
+    }
+  }
+}
+
+// Every instantiation runs 384 threads: warp 0 slab TMA producer, warp 2 weight TMA producer, warp 1 residual TMA producer
+// (EPI_PLAIN_RES; otherwise idle, as is warp 3), warps
 // 4-11 are two consumer warpgroups.  Consumer warpgroup g issues the wgmma of output rows h0 + 8g .. h0 + 8g + 7 of every
 // M-tile (64 positions) against all bn columns, keeping mw accumulators of 64 x bn in registers (mw * bn <= 128: at most
 // 64 fp32 registers per thread), then runs the epilogue on them.
@@ -151,6 +240,9 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
     // empty barriers: one arrival per consumer warp once its wgmma of the stage have completed
     for (int s = 0; s < p.slab_stages; ++s) { mbar_init(slab_full + 8 * s, 1); mbar_init(slab_empty + 8 * s, 8); }
     for (int s = 0; s < p.w_stages; ++s) { mbar_init(w_full + 8 * s, 1); mbar_init(w_empty + 8 * s, 8); }
+    // residual tile of each consumer warpgroup: full = the producer's TMA loads, empty = one arrival per consumer warp
+    if (MODE == EPI_PLAIN_RES)
+      for (int g = 0; g < 2; ++g) { mbar_init(L.rbar + 8 * g, 1); mbar_init(L.rbar + 16 + 8 * g, 4); }
     fence_barrier_init();
   }
   if (warp == 0 && lane == 0) {
@@ -161,6 +253,10 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
   if (warp == 2 && lane == 0) {
     tma_prefetch_desc(&p.wmap); tma_prefetch_desc(&p.wmap2);
     if (MODE == EPI_FUSED_RU) tma_prefetch_desc(&p.w1map);
+  }
+  if (slab_tma_epi(MODE) && warp == 1 && lane == 0) {
+    tma_prefetch_desc(&p.ymap);
+    if (MODE == EPI_PLAIN_RES) tma_prefetch_desc(&p.rmap);
   }
   if (warp >= 4) {
     const int nb = p.n_tiles_n * p.bn;   // >= Co; padded columns read zeros
@@ -215,6 +311,31 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
                           c.h0 - p.ph, ti >= 0 ? ti : ti + p.hist_T, c.b);
               if (++s == (uint32_t)p.slab_stages) { s = 0; ph ^= 1; }
             }
+        }
+      }
+    } else if (warp == 1) {
+      // ------------------------------ residual producer (EPI_PLAIN_RES) ------------------------------
+      // loads the boxes of a tile's residual that hold output positions and channels (the boxes of slab_epi_fragment)
+      // as soon as the warpgroup has read the previous tile's, so that they arrive under the tile's main loop
+      if (MODE == EPI_PLAIN_RES && lane == 0) {
+        constexpr int CB = slab_out_box_ch(MODE, BN), NB = BN / CB;
+        uint32_t ph = 0;
+        for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
+          const TileCoord c = decode_tile(p, tile);
+          for (int g = 0; g < 2; ++g) {
+            const uint32_t rt = L.rtile + (uint32_t)(g * p.mw * NB) * 64 * CB * 2;
+            const int h = c.h0 + 8 * g;
+            int nbox = 0;
+            for (int j = 0; j < p.mw; ++j)
+              for (int b = 0; b < NB; ++b) nbox += h < p.H && c.w0 + 8 * j < p.W && c.n0 + b * CB < p.Co;
+            mbar_wait(L.rbar + 16 + 8 * g, ph ^ 1);
+            mbar_expect_tx(L.rbar + 8 * g, (uint32_t)nbox * 64 * CB * 2);
+            for (int j = 0; j < p.mw; ++j)
+              for (int b = 0; b < NB; ++b)
+                if (h < p.H && c.w0 + 8 * j < p.W && c.n0 + b * CB < p.Co)
+                  tma_load_5d(rt + (uint32_t)(j * NB + b) * 64 * CB * 2, &p.rmap, L.rbar + 8 * g, c.n0 + b * CB, c.w0 + 8 * j, h, c.t, c.b);
+          }
+          ph ^= 1;
         }
       }
     } else if (warp == 2) {
@@ -286,6 +407,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
     uint32_t s_idx = 0, s_par = 0;                               // slab ring
     uint32_t w_idx = 0, w_par = 0, b_lo = b_lo0;                 // weight ring
     uint32_t ecount = 0;       // EPI_FUSED_RU: M-tiles processed (selects the logit exchange buffer)
+    uint32_t r_par = 0;        // EPI_PLAIN_RES: parity of the residual tile's full barrier
     float acc[MWMAX][BN / 2];
     // Main loop of one tile, compiled per M-tile count MW (= p.mw) and K steps per 64-byte half row (K4: 128-byte rows),
     // so that every commit group is straight-line code with constant accumulator indices: ptxas closes a group early at
@@ -389,6 +511,39 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
       if (MWMAX >= 4 && p.mw == 4) mainloop_k(c, std::integral_constant<int, (MWMAX >= 4 ? 4 : 1)>());
       else if (MWMAX >= 2 && p.mw == 2) mainloop_k(c, std::integral_constant<int, (MWMAX >= 2 ? 2 : 1)>());
       else mainloop_k(c, std::integral_constant<int, 1>());
+      if (slab_tma_epi(MODE)) {
+        // ---- register epilogue: bf16 results -> this warpgroup's output tile -> TMA box stores ----
+        constexpr int CB = slab_out_box_ch(MODE, BN), NB = (MODE == EPI_GEGLU ? BN / 2 : BN) / CB;
+        constexpr uint32_t BOX = 64 * CB * 2;
+        const uint32_t ot = L.otile + (uint32_t)(wg * p.mw * NB) * BOX, rt = L.rtile + (uint32_t)(wg * p.mw) * 64 * BN * 2;
+        if (tid == 0) bulk_wait_read_all();     // the previous tile's stores have read the output tile
+        named_bar_sync(wg_bar, 128);
+        if (MODE == EPI_PLAIN_RES) mbar_wait(L.rbar + 8 * wg, r_par);
+        const int act = p.epi.act;
+        if (MODE == EPI_GEGLU || act == MV2_ACT_NONE)
+          slab_epi_fragment<MODE, BN, MV2_ACT_NONE>(p, acc, c, sbias, ot, rt, wq, lane, false);
+        else if (act == MV2_ACT_ELU) slab_epi_fragment<MODE, BN, MV2_ACT_ELU>(p, acc, c, sbias, ot, rt, wq, lane, false);
+        else if (act == MV2_ACT_SILU) slab_epi_fragment<MODE, BN, MV2_ACT_SILU>(p, acc, c, sbias, ot, rt, wq, lane, false);
+        else slab_epi_fragment<MODE, BN, MV2_ACT_LEAKY_RELU>(p, acc, c, sbias, ot, rt, wq, lane, act == MV2_ACT_RELU);
+        if (MODE == EPI_PLAIN_RES) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(L.rbar + 16 + 8 * wg);
+          r_par ^= 1;
+        }
+        fence_proxy_async();                    // generic-proxy writes -> visible to the TMA engine's reads
+        named_bar_sync(wg_bar, 128);
+        if (tid == 0) {
+          // boxes without an output position or channel are skipped; TMA clips the others at the H, W and Co edges
+          const int oc0 = MODE == EPI_GEGLU ? c.n0 / 2 : c.n0, oco = MODE == EPI_GEGLU ? p.Co / 2 : p.Co;
+          const int h = c.h0 + 8 * wg;
+          for (int j = 0; j < p.mw; ++j)
+            for (int b = 0; b < NB; ++b)
+              if (h < p.H && c.w0 + 8 * j < p.W && oc0 + b * CB < oco)
+                tma_store_5d(&p.ymap, ot + (uint32_t)(j * NB + b) * BOX, oc0 + b * CB, c.w0 + 8 * j, h, c.t, c.b);
+          bulk_commit();
+        }
+        continue;
+      }
       // ---- accumulators -> shared-memory staging (one [64][BN + 4] block per M-tile), once the previous tile's epilogue
       //      of this warpgroup has read its staging ----
       named_bar_sync(wg_bar, 128);
@@ -571,50 +726,19 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
         const float* srow = stg + (j * 64 + row - 64 * wg) * (BN + 4);
         const int64_t row_base = ((((int64_t)c.b * p.T + c.t) * p.H + h) * p.W + w) * p.Co;
         // column chunks are dealt round-robin to the two warps that share this lane quarter
-        if (MODE == EPI_PLAIN || MODE == EPI_PLAIN_RES || MODE == EPI_SHUFFLE_ST || MODE == EPI_DOWN_SPACE) {
+        if (MODE == EPI_SHUFFLE_ST) {
           // Row-per-lane results are transposed through shared memory so that every store instruction writes 8 rows
-          // x 64 contiguous bytes (full sectors; the 8 rows are neighbours along w, i.e. one contiguous run when the
-          // tile spans all of Co) instead of 32 scattered 16-byte pieces.  The residual is read with the same mapping.
+          // x 64 contiguous bytes (full sectors; the 8 rows are neighbours along w) instead of 32 scattered 16-byte pieces.
           const uint32_t stg = stage0 + (uint32_t)ew * 2048;
           const uint32_t wr = stg + lane * 64, wsw = (lane >> 1) & 3;
           const int rl = lane >> 2, piece = lane & 3;                 // read side: row within an 8-row group, 16-byte piece
           const int w2 = c.w0 + 8 * j + rl;
           const uint32_t rd = stg + rl * 64;
-          // output addressing is hoisted out of the chunk loop: element offset of (row k = 0, column piece) and the
-          // stride between the four h rows a warp stores per chunk
           const int h20 = c.h0 + sub * 4;
-          const int64_t row0 = ((((int64_t)c.b * p.T + c.t) * p.H + h20) * p.W + w2) * p.Co + c.n0 + piece * 8;
-          const int64_t kstride = (int64_t)p.W * p.Co;
           const int kmax = w2 < p.W ? p.H - h20 : 0;                   // rows k < kmax are inside the frame
           for (int c0 = ((j + half) & 1) * 32; c0 < p.bn; c0 += 64) {
             uint32_t r[32], pk[16];
-            uint4 rv[4];
-            if (MODE == EPI_PLAIN_RES) {
-              // residual: this lane's own row, 64 contiguous bytes (two full sectors), requested before the staged accumulators are read;
-              // it is added in fp32 BEFORE the single rounding to bf16 (the reference's bf16 `fn(x) + x` rounds twice)
-              const __nv_bfloat16* rr = p.epi.res + row_base + c.n0 + c0;
-#pragma unroll
-              for (int g = 0; g < 4; ++g)
-                rv[g] = (row_ok && c.n0 + c0 + g * 8 < p.Co && c0 + g * 8 < p.bn) ? *reinterpret_cast<const uint4*>(rr + g * 8) : make_uint4(0, 0, 0, 0);
-            }
             load_row32(srow + c0, 32, r);
-            if ((MODE == EPI_PLAIN || MODE == EPI_PLAIN_RES) && p.epi.oscale) {   // Conv3DMod demodulation (M:741-742)
-              const float* os = p.epi.oscale + (int64_t)c.b * p.Co + c.n0 + c0;
-#pragma unroll
-              for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * (c.n0 + c0 + i < p.Co ? os[i] : 0.f));
-            }
-            if (MODE == EPI_PLAIN_RES) {
-              epi_act32(p.epi.act, r, sbias + c.n0 + c0);
-              const float rs = p.epi.mode == 2 ? 0.70710678118654752440f : 1.f;     // scaled residual (DiscriminatorBlock, M:585)
-#pragma unroll
-              for (int g = 0; g < 4; ++g) {
-                const uint32_t w4[4] = {rv[g].x, rv[g].y, rv[g].z, rv[g].w};
-#pragma unroll
-                for (int q = 0; q < 4; ++q)
-                  pk[4 * g + q] = pack_bf16x2((__uint_as_float(r[8 * g + 2 * q]) + __uint_as_float(w4[q] << 16)) * rs,
-                                              (__uint_as_float(r[8 * g + 2 * q + 1]) + __uint_as_float(w4[q] & 0xffff0000u)) * rs);
-              }
-            } else
             epi_pack32(p.epi.act, r, sbias + c.n0 + c0, pk);
 #pragma unroll
             for (int g = 0; g < 4; ++g)
@@ -623,24 +747,19 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
             __syncwarp();
             const bool col_ok = c.n0 + c0 + piece * 8 < p.Co && c0 + piece * 8 < p.bn;
             const int klim = col_ok ? kmax : 0;
+            // packed GEMM columns are (q, c): this chunk's 32 columns share one sub-pixel phase q (Cy % 32 == 0), so a
+            // row's 64 bytes land contiguously at its shuffled position (reference M:824 / M:861 rearranges)
             __nv_bfloat16* yp;
             int64_t ks;
-            if (MODE == EPI_SHUFFLE_ST) {
-              // packed GEMM columns are (q, c): this chunk's 32 columns share one sub-pixel phase q (Cy % 32 == 0), so a
-              // row's 64 bytes land contiguously at its shuffled position (reference M:824 / M:861 rearranges)
-              const int n = c.n0 + c0;
-              if (p.epi.shuffle == MV2_SHUFFLE_SPACE) {
-                const int cy = p.Co >> 2, qd = n / cy, cb = n - qd * cy;
-                yp = p.epi.y + ((((int64_t)c.b * p.T + c.t) * (2 * p.H) + (2 * h20 + (qd >> 1))) * (2 * p.W) + (2 * w2 + (qd & 1))) * cy + cb + piece * 8;
-                ks = (int64_t)4 * p.W * cy;          // next h row = two output rows further
-              } else {
-                const int cy = p.Co >> 1, qd = n / cy, cb = n - qd * cy;
-                yp = p.epi.y + ((((int64_t)c.b * (2 * p.T) + (2 * c.t + qd)) * p.H + h20) * p.W + w2) * cy + cb + piece * 8;
-                ks = (int64_t)p.W * cy;
-              }
+            const int n = c.n0 + c0;
+            if (p.epi.shuffle == MV2_SHUFFLE_SPACE) {
+              const int cy = p.Co >> 2, qd = n / cy, cb = n - qd * cy;
+              yp = p.epi.y + ((((int64_t)c.b * p.T + c.t) * (2 * p.H) + (2 * h20 + (qd >> 1))) * (2 * p.W) + (2 * w2 + (qd & 1))) * cy + cb + piece * 8;
+              ks = (int64_t)4 * p.W * cy;          // next h row = two output rows further
             } else {
-              yp = p.epi.y + row0 + c0;
-              ks = kstride;
+              const int cy = p.Co >> 1, qd = n / cy, cb = n - qd * cy;
+              yp = p.epi.y + ((((int64_t)c.b * (2 * p.T) + (2 * c.t + qd)) * p.H + h20) * p.W + w2) * cy + cb + piece * 8;
+              ks = (int64_t)p.W * cy;
             }
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
@@ -660,6 +779,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
         }
       }
     }
+    if (slab_tma_epi(MODE) && tid == 0) bulk_wait_all();   // the output is written before the CTA exits
   }
 }
 
@@ -801,6 +921,20 @@ static int slab_encode_maps(SlabParams& p, const mv2_tc_conv_args* a, const mv2_
   if (const int rc = encode_bf16_map(&p.wmap, 3, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
   return encode_bf16_map(&p.wmap2, 2, a->w, kdims, wstrides, wbox, swz, "weights 2-D");
 }
+// Output (and residual) maps of the TMA-store flavours: y as {oc, W, H, T, B} (oc = Co, or Co / 2 for GEGLU), boxes of
+// slab_out_box_ch channels x 8 (w) x 8 (h) in the swizzle of their row width
+static int slab_encode_out_maps(SlabParams& p, int mode) {
+  const int cb = slab_out_box_ch(mode, p.bn);
+  const int64_t oc = mode == EPI_GEGLU ? p.Co / 2 : p.Co;
+  const cuuint64_t dims[5] = {(cuuint64_t)oc, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.T, (cuuint64_t)p.B};
+  const cuuint64_t strides[4] = {(cuuint64_t)(oc * 2), (cuuint64_t)(p.W * oc * 2), (cuuint64_t)(p.H * p.W * oc * 2),
+                                 (cuuint64_t)(p.T * p.H * p.W * oc * 2)};
+  const cuuint32_t box[5] = {(cuuint32_t)cb, 8, 8, 1, 1};
+  const CUtensorMapSwizzle swz = swizzle_of_row(cb * 2);
+  if (const int rc = encode_bf16_map(&p.ymap, 5, p.epi.y, dims, strides, box, swz, "output")) return rc;
+  if (mode != EPI_PLAIN_RES) return MV2_OK;
+  return encode_bf16_map(&p.rmap, 5, p.epi.res, dims, strides, box, swz, "residual");
+}
 
 // Launches one slab-kernel flavour: persistent CTAs, one per SM of the current device (fewer when there are fewer tiles)
 static int slab_launch(int mode, const SlabParams& p, void* stream) {
@@ -873,6 +1007,8 @@ extern "C" int mv2_tc_slab_forward(const mv2_tc_conv_args* a, const mv2_conv_his
   else if (a->shuffle != MV2_SHUFFLE_NONE) mode = EPI_SHUFFLE;
   else if (a->Co % 8 != 0) mode = EPI_RAGGED;
   else if (a->res) mode = EPI_PLAIN_RES;
+  if (slab_tma_epi(mode))
+    if (const int rc = slab_encode_out_maps(p, mode)) return rc;
   return slab_launch(mode, p, stream);
 }
 
@@ -1013,5 +1149,6 @@ extern "C" int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream
   const cuuint32_t wbox[2] = {(cuuint32_t)bk, (cuuint32_t)bn};
   if (const int rc = encode_bf16_map(&p.wmap2, 2, a->w, wdims, wstrides, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "weights")) return rc;
   p.wmap = p.wmap2;
+  if (const int rc = slab_encode_out_maps(p, EPI_DOWN_SPACE)) return rc;
   return slab_launch(EPI_DOWN_SPACE, p, stream);
 }

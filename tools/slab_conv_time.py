@@ -4,8 +4,11 @@ events around every wgmma conv launch (slab, fused ResidualUnit, SpatialDownsamp
 repetition is queued behind a GPU spin so the events bracket kernel time rather than host launch gaps.
 
 One row per launch: kernel, shape, slab plan (mw, bn, slab stages; mv2_tc_slab_plan of the conv, for the fused
-ResidualUnit that of its 3x3x3 conv), median microseconds and TFLOP/s from the shapes.  The card's name, power limit and
-the median SM clock during the timed repetitions are printed with the numbers.
+ResidualUnit that of its 3x3x3 conv), median microseconds and TFLOP/s from the shapes, the bytes the algorithm has to
+move (input, weights and output once each, and the residual) and the launch's floor max(FLOP / 989 TFLOP/s, bytes /
+3.35 TB/s).  Both rates of the floor are H100 SXM data-sheet figures (dense BF16, HBM3), not measured ones.  Subtotals
+split the launches into one-tap ones (1x1x1 convs, Linear layers, the decoder's up-samplers) and the rest.  The card's
+name, power limit and the median SM clock during the timed repetitions are printed with the numbers.
 
     python tools/slab_conv_time.py [--reps 60]
 """
@@ -86,6 +89,20 @@ def _describe(lib, name, a):
     return shape, plan
 
 
+PEAK_FLOPS, PEAK_BYTES = 989e12, 3.35e12        # H100 SXM data sheet: dense BF16 tensor core, HBM3 bandwidth
+
+
+def _bytes_and_taps(name, a):
+    """bf16 bytes a launch has to move at least (input, weights, output once each, and the residual), and its taps"""
+    if name == "mv2_tc_ru_forward":                     # x, the 3x3x3 and 1x1x1 weights, y
+        taps = a.kt * a.kh * a.kw
+        return 2 * (2 * a.B * a.T * a.H * a.W * a.C + (taps + 1) * a.C * a.C), taps + 1
+    taps = a.kt * a.kh * a.kw
+    out = a.B * a.To * a.Ho * a.Wo * (a.Co // 2 if a.epi_mode == 1 else a.Co)
+    n = a.B * a.Ti * a.Hi * a.Wi * a.Ci + taps * a.Ci * a.Co + out + (out if a.res else 0)
+    return 2 * n, taps
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=60, help="timed repetitions of the step (>= 50)")
@@ -135,15 +152,25 @@ def main():
     print(f"card: {_card()}  (name, power limit, max SM clock)")
     print(f"SM clock during the timed repetitions: median {clocks.get('sm_mhz')} MHz of {clocks.get('sm_max_mhz')} "
           f"({clocks.get('samples')} samples, reasons {clocks.get('reasons')}); {args.reps} repetitions, median per launch")
-    print(f"{'#':>3} {'kernel':<10} {'shape':<36} {'plan':<16} {'us':>8} {'TFLOP/s':>8}")
-    tot_us = tot_fl = 0.0
+    print(f"{'#':>3} {'kernel':<10} {'shape':<36} {'plan':<16} {'us':>8} {'TFLOP/s':>8} {'MB':>8} {'floor us':>9}")
+    groups = {"one-tap": [0, 0.0, 0.0, 0.0, 0.0], "multi-tap": [0, 0.0, 0.0, 0.0, 0.0]}   # launches, us, FLOP, bytes, floor
     for i, (name, a) in enumerate(calls):
         samples = [prof[r * n + i][0].elapsed_time(prof[r * n + i][1]) * 1e3 for r in range(args.reps)]
         us, flops = statistics.median(samples), prof[i][2]
-        tot_us += us
-        tot_fl += flops
+        nbytes, taps = _bytes_and_taps(name, a)
+        floor = max(flops / PEAK_FLOPS, nbytes / PEAK_BYTES) * 1e6
+        g = groups["one-tap" if taps == 1 else "multi-tap"]
+        for k, v in enumerate((1, us, flops, nbytes, floor)):
+            g[k] += v
         shape, plan = _describe(lib, name, a)
-        print(f"{i:>3} {KIND[name]:<10} {shape:<36} {plan:<16} {us:>8.1f} {flops / us / 1e6:>8.1f}")
+        print(f"{i:>3} {KIND[name]:<10} {shape:<36} {plan:<16} {us:>8.1f} {flops / us / 1e6:>8.1f} {nbytes / 1e6:>8.1f} "
+              f"{floor:>9.1f}")
+    print("floor: max(FLOP / 989 TFLOP/s, bytes / 3.35 TB/s), H100 SXM data-sheet rates, not measured ones")
+    for label, (cnt, us, fl, nb, floor) in groups.items():
+        print(f"{label} launches ({cnt}): {us / 1e3:.3f} ms, {fl / 1e12:.3f} TFLOP, {fl / us / 1e6:.1f} TFLOP/s, "
+              f"{nb / 1e9:.3f} GB, floor {floor / 1e3:.3f} ms")
+    tot_us = sum(g[1] for g in groups.values())
+    tot_fl = sum(g[2] for g in groups.values())
     print(f"all {n} launches: {tot_us / 1e3:.3f} ms, {tot_fl / 1e12:.3f} TFLOP, {tot_fl / tot_us / 1e6:.1f} TFLOP/s")
 
 
