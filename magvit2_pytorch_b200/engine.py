@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes as C
 import math
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Tuple
+from typing import Callable, Dict, List, Optional, Tuple
 
 import torch
 
@@ -54,8 +54,11 @@ class AttnDropout:
 
 class StreamState:
     """Causal state of a streamed clip batch (stream.py), carried from one push to the next: per layer, the history frames
-    of a causal conv, the previous frame of a token shift, the time attention's qkv cache, the gateloop scan state.  A
-    view with a key prefix (`sub`) is what the layer functions receive; None everywhere means a whole-clip call."""
+    of a causal conv, the previous frame of a token shift, the time attention's K/V cache and output buffers, the gateloop
+    scan state.  A view with a key prefix (`sub`) is what the layer functions receive; None everywhere means a whole-clip
+    call.  Every buffer a push's kernels read or write across pushes is allocated once and updated in place, so a push
+    captured as a CUDA graph (stream.PushPlan) can be replayed on later pushes; only the K/V cache moves when it grows, and
+    the host steps that use it are not captured."""
 
     def __init__(self, slots=None, prefix=""):
         self._slots = {} if slots is None else slots
@@ -69,6 +72,11 @@ class StreamState:
 
     def put(self, name, value):
         self._slots[self._prefix + name] = value
+
+    def history_counts(self):
+        """The frame count of every conv history, in layer order: with the chunk's shape, what a push's launches depend on
+        besides the time attention's K/V cache length."""
+        return tuple(v[1] for k, v in self._slots.items() if k.rsplit("/", 1)[-1] == "hist")
 
 
 def _sub(ss: Optional[StreamState], name):
@@ -258,6 +266,9 @@ class Engine:
         self._prof: Optional[list] = None  # when set, (event0, event1, flops) per wgmma conv launch
         self.conv_log: Optional[list] = None  # when set, one record per tensor-core conv launch (Engine._conv_launch)
         self.dropout: Optional[AttnDropout] = None  # set for the duration of a train-mode forward with attention dropout
+        # set while a stream push is captured (stream.PushPlan): host_step(step) runs step(), a piece of the push that a
+        # CUDA graph cannot replay, between two captured segments and returns its result
+        self.host_step: Optional[Callable] = None
 
     # ------------------------------------------------------------------ parameters
     def bind(self, p0: torch.Tensor, what: str):
@@ -383,36 +394,36 @@ class Engine:
 
     def _conv_hist(self, ss: Optional[StreamState], x, need: int):
         """(mv2_conv_hist of the frames in front of x, state update to run after the launch) of a causal conv whose input
-        reaches `need` frames back; (None, None) for a whole-clip call.  The history is a frame range of an earlier input
-        (tensor, first frame, count); only when it has to span two chunks are the frames copied into a tensor of their own."""
+        reaches `need` frames back; (None, None) for a whole-clip call.  The history is (buffer, count): a (B, need, ...)
+        buffer the stream owns, holding the last `count` frames in front of x at its end (count < need only until the
+        stream has seen `need` frames at this layer).  The update keeps its last need frames of [history | x] there."""
         if ss is None or need <= 0:
             return None, None
         h = ss.get("hist")
         hist = None
         if h is not None:
-            t, t0, n = h
-            fe = t[0, 0].numel()
-            hist = ConvHist(h=t.data_ptr() + t0 * fe * t.element_size(), T_h=n, clip_stride=t.shape[1] * fe)
+            buf, n = h
+            fe = buf[0, 0].numel()
+            hist = ConvHist(h=buf.data_ptr() + (need - n) * fe * buf.element_size(), T_h=n, clip_stride=need * fe)
 
         def advance():
             T = x.shape[1]
-            if T >= need or h is None:
-                keep = min(need, T)
-                ss.put("hist", (x, T - keep, keep))
-                return
-            t, t0, n = h
-            old = min(n, need - T)
-            buf = self._new((x.shape[0], old + T) + tuple(x.shape[2:]), x.dtype)
-            self.copy_frames(t, t0 + n - old, old, dst=buf, dst_t0=0)
-            self.copy_frames(x, 0, T, dst=buf, dst_t0=old)
-            ss.put("hist", (buf, 0, old + T))
+            buf, n = h if h is not None else (self._new((x.shape[0], need) + tuple(x.shape[2:]), x.dtype), 0)
+            keep = min(T, need)
+            old = min(n, need - keep)
+            # the older frames move T places towards the front, one frame per copy in increasing order: source and
+            # destination ranges overlap when T < old
+            for i in range(old):
+                self.copy_frames(buf, need - old + i, 1, dst=buf, dst_t0=need - keep - old + i)
+            self.copy_frames(x, T - keep, keep, dst=buf, dst_t0=need - keep)
+            ss.put("hist", (buf, old + keep))
         return hist, advance
 
     def _hist_cat(self, ss: StreamState, x):
         """[carried history | x] as one new (B, T_h + T, ...) tensor."""
-        t, t0, n = ss.get("hist")
+        buf, n = ss.get("hist")
         cat = self._new((x.shape[0], n + x.shape[1]) + tuple(x.shape[2:]), x.dtype)
-        self.copy_frames(t, t0, n, dst=cat, dst_t0=0)
+        self.copy_frames(buf, buf.shape[1] - n, n, dst=cat, dst_t0=0)
         self.copy_frames(x, 0, x.shape[1], dst=cat, dst_t0=n)
         return cat
 
@@ -608,19 +619,21 @@ class Engine:
         return self.conv(h, p["conv1"], act=ACT_ELU, res=x)
 
     def rmsnorm(self, x, gamma, token_shift=False, ss: Optional[StreamState] = None):
-        """ss (token shift only): the shifted channels of frame 0 come from the previous chunk's last frame."""
+        """ss (token shift only): the shifted channels of frame 0 come from the previous chunk's last frame, which the
+        stream keeps in a (B, 1, ...) buffer of its own."""
         B, T, H, W, Cc = x.shape
         out = self._new(x.shape)
         prev = None if (ss is None or not token_shift) else ss.get("prev")
         if prev is not None:
-            t, tl = prev
-            fe = t[0, 0].numel()
-            self._call("mv2_rmsnorm_prev", _ptr(x), t.data_ptr() + tl * fe * t.element_size(), t.shape[1] * fe, _ptr(out),
-                       _dt(self.dtype), _ptr(gamma), B, T, H * W, Cc)
+            self._call("mv2_rmsnorm_prev", _ptr(x), _ptr(prev), prev[0, 0].numel(), _ptr(out), _dt(self.dtype), _ptr(gamma),
+                       B, T, H * W, Cc)
         else:
             self._call("mv2_rmsnorm", _ptr(x), _ptr(out), _dt(self.dtype), _ptr(gamma), B, T, H * W, Cc, int(token_shift))
         if ss is not None and token_shift:
-            ss.put("prev", (x, T - 1))
+            if prev is None:
+                prev = self._new((B, 1, H, W, Cc), x.dtype)
+                ss.put("prev", prev)
+            self.copy_frames(x, T - 1, 1, dst=prev)
         return out
 
     def feed_forward(self, x, p, token_shift=False, ss: Optional[StreamState] = None):
@@ -644,12 +657,13 @@ class Engine:
         time_axis = axis == "time"
         xn = self.rmsnorm(x, p["gamma"], token_shift=time_axis, ss=ss)
         qkv = self.conv(xn, p["qkv"])
+        if time_axis and ss is not None:
+            step = lambda: self._attention_tail(qkv, p, ss)     # noqa: E731
+            o = step() if self.host_step is None else self.host_step(step)
+            return self.conv(o, p["out"], res=x)
         heads, dh = p["heads"], p["dim_head"]
         o = self._new((B, T, H, W, heads * dh))
         HW = H * W
-        if time_axis and ss is not None:
-            self._attention_tail(qkv, o, p, ss)
-            return self.conv(o, p["out"], res=x)
         if time_axis:
             a = AttnArgs(qkv=_ptr(qkv), out=_ptr(o), mem_kv=_ptr(p["mem_kv"]), dtype=_dt(self.dtype), heads=heads,
                          dim_head=dh, n_mem=p["n_mem"], causal=1, n_outer=B, n_inner=HW, L=T,
@@ -666,12 +680,21 @@ class Engine:
 
     KV_CACHE_STEP = 16       # latent frames the time attention's K/V cache grows by
 
-    def _attention_tail(self, qkv, o, p, ss: StreamState):
-        """Time attention of a streamed chunk: the chunk's keys and values are appended to the stream's K/V cache (every
-        earlier frame's; it grows by KV_CACHE_STEP frames when full) and mv2_attention_tail computes the chunk's queries,
-        read from qkv, against all cached keys."""
+    def _attention_tail(self, qkv, p, ss: StreamState):
+        """Time attention of a streamed chunk -> its output o, a buffer the stream keeps per chunk length: the chunk's keys
+        and values are appended to the stream's K/V cache (every earlier frame's; it grows by KV_CACHE_STEP frames when
+        full) and mv2_attention_tail computes the chunk's queries, read from qkv, against all cached keys.  Its launch
+        arguments change with every push (the cache length, the kernel chosen for it, the cache's address after a growth),
+        so a captured push runs it as a host step between two graph segments (host_step)."""
         B, T, H, W, C3 = qkv.shape
         HW, HD = H * W, C3 // 3
+        outs = ss.get("o")
+        if outs is None:
+            outs = {}
+            ss.put("o", outs)
+        o = outs.get(T)
+        if o is None:
+            o = outs[T] = self._new((B, T, H, W, HD))
         cache = ss.get("kv")
         L0 = 0 if cache is None else cache[1]
         buf = None if cache is None else cache[0]
@@ -688,6 +711,7 @@ class Engine:
                      dim_head=p["dim_head"], n_mem=p["n_mem"], causal=1, n_outer=B, n_inner=HW, L=L,
                      outer_stride=buf.shape[1] * HW, inner_stride=1, tok_stride=HW)
         self._call("mv2_attention_tail", C.byref(a), _ptr(qkv), T * HW, L0, _ptr(o), T * HW)
+        return o
 
     def attention_dropout_mask(self, n_seq, heads, L, n_mem, dropout: _lib.DropoutArgs):
         """The keep mask of an attention call, uint8 (n_seq, heads, L, n_mem + L) (mv2_attention_dropout_mask)."""

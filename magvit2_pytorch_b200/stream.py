@@ -10,6 +10,8 @@ gateloop the fp32 scan state.  The kernels read that state in place (DESIGN.md 3
     codes = torch.cat([enc.push(chunk) for chunk in chunks], dim=1)      # == tok.tokenize(video)
     dec = tok.decode_stream(batch_size=B)
     video = torch.cat([dec.push(c) for c in codes.split(1, dim=1)], dim=2)   # == tok.decode_from_code_indices(codes)
+
+With tok.cuda_graphs set, a stream replays its pushes as CUDA graphs (PushPlan) once it has seen a push of the same shape.
 """
 from __future__ import annotations
 
@@ -47,6 +49,63 @@ def decoder_chunk_frames(n: int, tdf: int, first_push: bool, first_frame: bool) 
     return tdf * n - (tdf - 1 if first_push and first_frame else 0)
 
 
+class PushPlan:
+    """One push captured as CUDA graph segments, split where the push runs a host step (Engine.host_step: the streamed
+    time attention, whose launch arguments change with every push).  A replay runs segment 0, host step 0, segment 1, ...
+    on the current stream; the host steps read the stream's state as it is at that push.  All segments allocate from one
+    private memory pool, so a segment may read what an earlier one wrote."""
+
+    def __init__(self, eng, fn, x):
+        """Captures fn(x), the push of input x (static copy: `x`), running each segment once as soon as it is captured so
+        that the host step after it reads real values; the push's state update takes effect as in an eager push."""
+        self.x = x.clone()
+        self._eng = eng
+        self._pool = torch.cuda.graph_pool_handle()
+        self.graphs, self.launches, self.steps = [], [], []
+        self._capture = None
+        eng.host_step = self._split
+        try:
+            self._begin()
+            self.out = fn(self.x)
+            self._end()
+        except BaseException:
+            if self._capture is not None:
+                self._capture.__exit__(None, None, None)
+            raise
+        finally:
+            eng.host_step = None
+
+    def _begin(self):
+        g = torch.cuda.CUDAGraph()
+        self._capture = torch.cuda.graph(g, pool=self._pool)
+        self._capture.__enter__()
+        self.graphs.append(g)
+        self.launches.append(self._eng.launches)
+
+    def _end(self):
+        capture, self._capture = self._capture, None
+        capture.__exit__(None, None, None)
+        self.launches[-1] = self._eng.launches - self.launches[-1]
+        self.graphs[-1].replay()
+
+    def _split(self, step):
+        self._end()
+        out = step()
+        self.steps.append(step)
+        self._begin()
+        return out
+
+    def replay(self, x):
+        """The push of input x -> its output (the plan's static output tensor)."""
+        self.x.copy_(x, non_blocking=True)
+        for i, (g, n) in enumerate(zip(self.graphs, self.launches)):
+            if i:
+                self.steps[i - 1]()
+            g.replay()
+            self._eng.launches += n
+        return self.out
+
+
 class _Stream:
     def __init__(self, model, batch_size, cond, video_contains_first_frame):
         check_stream_model(model)
@@ -59,6 +118,8 @@ class _Stream:
         self.state = StreamState()
         self.pushes = 0
         self._sig_id = None
+        self._plans = {}             # push signature -> "warm" | PushPlan (model.cuda_graphs)
+        self.captures = 0            # PushPlans captured
 
     def _engine(self):
         """The model's engine, eval mode, checked against the parameter packs this stream started with."""
@@ -70,6 +131,31 @@ class _Stream:
             raise RuntimeError("the tokenizer's parameters changed while this stream was open: its carried state belongs "
                                "to the old ones; start a new stream")
         return eng
+
+    def _run(self, eng, fn, x, first, sff_rest):
+        """fn(x), the push of input x.  With model.cuda_graphs set it goes through this stream's PushPlans, with the rule
+        VideoTokenizer._graph_call follows: the first push of a signature runs eagerly, the second is captured, later ones
+        replay.  The signature is what the push's launches depend on besides the K/V cache length its host steps read: the
+        input's shape and dtype, the first-push flags and every conv history's frame count.  A replay does not update the
+        counts, so only pushes that leave them unchanged are captured; the others (the first few, while the histories
+        fill up) run eagerly, and their signatures do not recur."""
+        if not self.model.cuda_graphs:
+            return fn(x)
+        counts = self.state.history_counts()
+        key = (tuple(x.shape), x.dtype, first, sff_rest, counts)
+        plan = self._plans.get(key)
+        if plan is None:
+            out = fn(x)
+            if self.state.history_counts() == counts:
+                self._plans[key] = "warm"
+            return out
+        if plan == "warm":
+            plan = self._plans[key] = PushPlan(eng, fn, x)
+            self.captures += 1
+            out = plan.out
+        else:
+            out = plan.replay(x)
+        return out.clone()
 
     def _check_batch(self, t, what):
         if t.shape[0] != self.batch_size:
@@ -90,11 +176,14 @@ class TokenizeStream(_Stream):
         self._check_batch(chunk, "chunk")
         first = self.pushes == 0
         encoder_chunk_frames(chunk.shape[2], m.time_downsample_factor, first, self.first_frame)
+        ff, sff_rest = self.first_frame and first, self.first_frame and not first and m.separate_first_frame_encoding
         with torch.cuda.device(m.device):
             eng = self._engine()
-            x = eng.encode_cl(chunk.contiguous(), self.first_frame and first, self.cond, ss=self.state,
-                              sff_rest=self.first_frame and not first and m.separate_first_frame_encoding)
-            _, codes, _ = eng.quantize_cl(x, want_quantized=False)
+
+            def fn(v):
+                return eng.quantize_cl(eng.encode_cl(v, ff, self.cond, ss=self.state, sff_rest=sff_rest),
+                                       want_quantized=False)[1]
+            codes = self._run(eng, fn, chunk.contiguous(), first, sff_rest)
         self.pushes += 1
         return codes
 
@@ -115,10 +204,12 @@ class DecodeStream(_Stream):
         self._check_batch(codes, "codes")
         first = self.pushes == 0
         decoder_chunk_frames(codes.shape[1], m.time_downsample_factor, first, self.first_frame)
+        ff, sff_rest = self.first_frame and first, self.first_frame and not first and m.separate_first_frame_encoding
         with torch.cuda.device(m.device):
             eng = self._engine()
-            q = eng.codes_to_quantized_cl(codes)
-            out = eng.decode_cl(q, self.first_frame and first, self.cond, ss=self.state,
-                                sff_rest=self.first_frame and not first and m.separate_first_frame_encoding)
+
+            def fn(c):
+                return eng.decode_cl(eng.codes_to_quantized_cl(c), ff, self.cond, ss=self.state, sff_rest=sff_rest)
+            out = self._run(eng, fn, codes.contiguous(), first, sff_rest)
         self.pushes += 1
         return out
