@@ -17,8 +17,8 @@
 //   * N tiles need not divide Co (TMA clips the plain / GEGLU stores at Co): wide outputs without a
 //     128-column divisor take 128-column tiles with a ragged last one;
 //   * the kernel is instantiated per epilogue flavour (tc_common.cuh: EPI_*) and N tile (32 / 64 / 128); the plain,
-//     residual, GEGLU and SpatialDownsample2x flavours run the epilogue on the accumulator fragments and store bf16
-//     boxes through TMA (slab_epi_fragment), the others stage the accumulators in shared memory first.
+//     residual, GEGLU, SpatialDownsample2x and fused ResidualUnit flavours run the epilogue on the accumulator fragments
+//     and store bf16 boxes through TMA (slab_epi_mtile), the others stage the accumulators in shared memory first.
 //     The channels-first flavour (EPI_RAGGED: fewer than 32 output channels, so never a wider tile than 32) has narrow
 //     8- and 16-column tiles (wgmma m64n8k16 / m64n16k16) instead, for the data gradient of conv_in with respect to the
 //     video: 3 output channels, 7 x 7 in-plane taps (slab_narrow).
@@ -64,14 +64,14 @@ struct alignas(64) SlabParams {
   int dn_aoff[6];        // per tap' = dh * 2 + (dw2 + 1): A-descriptor start offset inside the stage, in 16-byte units
   int dn_lower;          // K-chunks of the lower (pw = 0) half of the 2C axis: they only see the dw2 = 0 taps
   int h_stride;          // bytes of the shared-memory H buffer (ELU'd 3x3x3 tile of one M-tile) = kchunks * 16 KB
-  // ---- TMA-store flavours (slab_tma_epi: EPI_PLAIN, EPI_PLAIN_RES, EPI_GEGLU, EPI_DOWN_SPACE) ----
+  // ---- TMA-store flavours (slab_tma_epi: EPI_PLAIN, EPI_PLAIN_RES, EPI_GEGLU, EPI_DOWN_SPACE; and EPI_FUSED_RU) ----
   CUtensorMap ymap;      // y as {Co (GEGLU: Co / 2), W, H, T, B}: boxes {cb, 8, 8, 1, 1}, one per 64 positions and cb channels
   CUtensorMap rmap;      // EPI_PLAIN_RES: the residual, same view and boxes as ymap
 };
 
-// Flavours whose epilogue runs on the accumulator fragments and stores through TMA; the others stage the accumulators in
-// shared memory first (the fused ResidualUnit's second GEMM reads the staged tile, the channels-first and shuffled stores
-// need a row per thread).
+// Flavours whose epilogue runs on the accumulator fragments and stores through TMA (slab_epi_fragment).  The fused
+// ResidualUnit does both too, with its own epilogue around the second GEMM; the others stage the accumulators in shared
+// memory first (the channels-first and shuffled stores need a row per thread).
 __host__ __device__ constexpr bool slab_tma_epi(int mode) {
   return mode == EPI_PLAIN || mode == EPI_PLAIN_RES || mode == EPI_GEGLU || mode == EPI_DOWN_SPACE;
 }
@@ -117,91 +117,105 @@ __host__ __device__ __forceinline__ TileCoord decode_tile(const SlabParams& p, i
 }
 
 // Shared-memory layout behind the two TMA rings (host and kernel must agree): barriers, bias, the eight 2 KB
-// epilogue transpose buffers, [fused: logit partials], the fp32 accumulator staging of both consumer warpgroups
-// (mw M-tiles x 64 rows x (bn + 4) each), [fused: the H buffer].
+// epilogue transpose buffers, the fp32 accumulator staging of both consumer warpgroups (mw M-tiles x 64 rows x (bn + 4)
+// each).
 // The TMA-store flavours use the span of the transpose buffers and the staging for other things: the residual
 // full / empty barriers of both warpgroups, then (1024-byte aligned, for the swizzled boxes) the bf16 output tiles and
 // the residual tiles of both warpgroups, 2 x mw x 64 x bn x 2 bytes each.  Together they take at most
 // 32 + 1023 + 512 mw bn bytes of the 16 KB + 512 mw (bn + 4) the span has, so the span, and with it every launch's
 // plan, is the same for all flavours but the fused one.
+// The fused ResidualUnit stages nothing: bias, logit partials, then (1024-byte aligned) the H buffer and the bf16 output
+// tiles of both warpgroups.
 struct SlabSmem { uint32_t sbias, stage0, lpart, accstg, hbuf, end, rbar, otile, rtile; };
 __host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& p, uint32_t bar0, bool fused) {
-  SlabSmem m;
+  SlabSmem m = {};
   m.sbias = (bar0 + 8 * (2 * p.slab_stages + 2 * p.w_stages) + 15) & ~15u;
   m.stage0 = m.sbias + (uint32_t)(p.n_tiles_n * p.bn) * 4 * (fused ? 3 : 1);   // fused: [conv3 bias][conv1 bias][SE to_k weight]
-  m.lpart = m.stage0 + (fused ? 0 : 8 * 2048);   // fused: the transposes reuse the accumulator staging
-  m.accstg = m.lpart + (fused ? 2048 : 0);
-  m.hbuf = m.accstg + 2u * p.mw * 64 * (p.bn + 4) * 4;
-  if (fused) m.hbuf = (m.hbuf + 1023u) & ~1023u;        // SWIZZLE_128B operand tiles: 1024-byte aligned
-  m.end = m.hbuf + (fused ? (uint32_t)p.h_stride : 0);
+  if (fused) {
+    m.lpart = m.stage0;
+    m.hbuf = (m.lpart + 2048 + 1023u) & ~1023u;          // SWIZZLE_128B tiles: 1024-byte aligned
+    m.otile = m.hbuf + (uint32_t)p.h_stride;
+    m.end = m.otile + 2u * p.mw * 64 * p.bn * 2;
+    return m;
+  }
+  m.accstg = m.stage0 + 8 * 2048;
+  m.end = m.accstg + 2u * p.mw * 64 * (p.bn + 4) * 4;
   m.rbar = m.stage0;
   m.otile = (m.rbar + 32 + 1023u) & ~1023u;
   m.rtile = m.otile + 2u * p.mw * 64 * p.bn * 2;
   return m;
 }
 
-// Epilogue of the TMA-store flavours on one consumer warpgroup's accumulators, in fragment layout: thread (warp wq of
-// the warpgroup, lane) holds rows m0 = 16 wq + lane / 4 and m0 + 8 of every M-tile (row m = output position
+// Epilogue of the TMA-store flavours on one M-tile of a consumer warpgroup's accumulators, in fragment layout: thread
+// (warp wq of the warpgroup, lane) holds rows m0 = 16 wq + lane / 4 and m0 + 8 of the M-tile (row m = output position
 // (h0 + 8 wg + m / 8, w0 + 8 j + m % 8)) and columns 8 g + 2 (lane % 4) + {0, 1}.  The math per element is that of the
 // staged epilogue, in the same order: x oscale, + bias and activation, [+ residual in fp32, x 2^-0.5 in mode 2], one
 // rounding to bf16; GEGLU pairs packed column 16 g + c (x) with 16 g + 8 + c (its gate), which the same thread holds.
-// Results go to the output tile `ot` as [mw][boxes][64 rows][cb channels] bf16 boxes in the swizzle TMA uses for their
-// row width; the residual is read from `rt` in the same layout.  Bank-conflict free: the 8 rows of a warp's access
-// fall on 8 different 16-byte units of the swizzle.
-template <int MODE, int BN, int ACT, int MWMAX>
-__device__ __forceinline__ void slab_epi_fragment(const SlabParams& p, const float (&acc)[MWMAX][BN / 2], const TileCoord& c,
-                                                  const float* sbias, uint32_t ot, uint32_t rt, int wq, int lane, bool relu) {
-  constexpr int OC = MODE == EPI_GEGLU ? BN / 2 : BN, CB = slab_out_box_ch(MODE, BN), NB = OC / CB;
+// Results go to `ot` as [boxes][64 rows][cb channels] bf16 boxes in the swizzle TMA uses for their row width; the
+// residual is read from `rt` in the same layout.  Bank-conflict free: the 8 rows of a warp's access fall on 8 different
+// 16-byte units of the swizzle.  With 128-byte rows this is also the layout of a K-major SWIZZLE_128B wgmma operand of
+// 64 rows (one 8 KB K-chunk per box), which the fused ResidualUnit's second GEMM reads.
+template <int MODE, int BN, int ACT>
+__device__ __forceinline__ void slab_epi_mtile(const SlabParams& p, const float (&acc)[BN / 2], const TileCoord& c,
+                                               const float* sbias, uint32_t ot, uint32_t rt, int wq, int lane, bool relu) {
+  constexpr int CB = slab_out_box_ch(MODE, BN);
   constexpr uint32_t RB = CB * 2, BOX = 64 * RB, SWZ = (RB / 16 - 1) << 4;
   const uint32_t m0 = 16 * wq + (lane >> 2), q4 = (lane & 3) * 4;
-  auto at = [&](int j, int col, uint32_t m) {        // byte offset of (row m, output columns col, col + 1) of M-tile j
+  auto at = [&](int col, uint32_t m) {               // byte offset of (row m, output columns col, col + 1)
     const uint32_t off = m * RB + (uint32_t)(col % CB) * 2 + q4;
-    return (uint32_t)(j * NB + col / CB) * BOX + (off ^ ((off >> 3) & SWZ));
+    return (uint32_t)(col / CB) * BOX + (off ^ ((off >> 3) & SWZ));
   };
   auto st32 = [](uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); };
   const float* os = (MODE == EPI_PLAIN || MODE == EPI_PLAIN_RES) && p.epi.oscale ? p.epi.oscale + (int64_t)c.b * p.Co : nullptr;
   const float rs = MODE == EPI_PLAIN_RES && p.epi.mode == 2 ? 0.70710678118654752440f : 1.f;
+  if (MODE == EPI_GEGLU) {
+#pragma unroll
+    for (int g = 0; g < BN / 16; ++g) {
+      const int n = c.n0 + 16 * g + 2 * (lane & 3);
+      const float2 bx = *reinterpret_cast<const float2*>(sbias + n), bg = *reinterpret_cast<const float2*>(sbias + n + 8);
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const float* xv = &acc[8 * g + 2 * hr];
+        const float* gv = &acc[8 * g + 4 + 2 * hr];
+        const float v0 = gelu_fast(gv[0] + bg.x) * (xv[0] + bx.x);
+        const float v1 = gelu_fast(gv[1] + bg.y) * (xv[1] + bx.y);
+        st32(ot + at(8 * g, m0 + 8 * hr), pack_bf16x2(v0, v1));
+      }
+    }
+  } else {
+#pragma unroll
+    for (int g = 0; g < BN / 8; ++g) {
+      const int col = 8 * g, n = c.n0 + col + 2 * (lane & 3);
+      const float2 b = *reinterpret_cast<const float2*>(sbias + n);
+      float o0 = 1.f, o1 = 1.f;
+      if (os) { o0 = n < p.Co ? os[n] : 0.f; o1 = n + 1 < p.Co ? os[n + 1] : 0.f; }
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        float v0 = acc[4 * g + 2 * hr], v1 = acc[4 * g + 2 * hr + 1];
+        if (os) { v0 *= o0; v1 *= o1; }
+        v0 = act_ct<ACT>(v0 + b.x, relu);
+        v1 = act_ct<ACT>(v1 + b.y, relu);
+        const uint32_t a = at(col, m0 + 8 * hr);
+        if (MODE == EPI_PLAIN_RES) {
+          uint32_t r;
+          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(rt + a) : "memory");
+          v0 = (v0 + __uint_as_float(r << 16)) * rs;
+          v1 = (v1 + __uint_as_float(r & 0xffff0000u)) * rs;
+        }
+        st32(ot + a, pack_bf16x2(v0, v1));
+      }
+    }
+  }
+}
+// All M-tiles of a warpgroup: output and residual tiles as [mw][boxes][64 rows][cb channels]
+template <int MODE, int BN, int ACT, int MWMAX>
+__device__ __forceinline__ void slab_epi_fragment(const SlabParams& p, const float (&acc)[MWMAX][BN / 2], const TileCoord& c,
+                                                  const float* sbias, uint32_t ot, uint32_t rt, int wq, int lane, bool relu) {
+  constexpr uint32_t MTILE = (MODE == EPI_GEGLU ? BN / 2 : BN) * 64 * 2;   // bytes of one M-tile's boxes
 #pragma unroll
   for (int j = 0; j < MWMAX; ++j) {
     if (j >= p.mw) break;
-    if (MODE == EPI_GEGLU) {
-#pragma unroll
-      for (int g = 0; g < BN / 16; ++g) {
-        const int n = c.n0 + 16 * g + 2 * (lane & 3);
-        const float2 bx = *reinterpret_cast<const float2*>(sbias + n), bg = *reinterpret_cast<const float2*>(sbias + n + 8);
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-          const float* xv = &acc[j][8 * g + 2 * hr];
-          const float* gv = &acc[j][8 * g + 4 + 2 * hr];
-          const float v0 = gelu_fast(gv[0] + bg.x) * (xv[0] + bx.x);
-          const float v1 = gelu_fast(gv[1] + bg.y) * (xv[1] + bx.y);
-          st32(ot + at(j, 8 * g, m0 + 8 * hr), pack_bf16x2(v0, v1));
-        }
-      }
-    } else {
-#pragma unroll
-      for (int g = 0; g < BN / 8; ++g) {
-        const int col = 8 * g, n = c.n0 + col + 2 * (lane & 3);
-        const float2 b = *reinterpret_cast<const float2*>(sbias + n);
-        float o0 = 1.f, o1 = 1.f;
-        if (os) { o0 = n < p.Co ? os[n] : 0.f; o1 = n + 1 < p.Co ? os[n + 1] : 0.f; }
-#pragma unroll
-        for (int hr = 0; hr < 2; ++hr) {
-          float v0 = acc[j][4 * g + 2 * hr], v1 = acc[j][4 * g + 2 * hr + 1];
-          if (os) { v0 *= o0; v1 *= o1; }
-          v0 = act_ct<ACT>(v0 + b.x, relu);
-          v1 = act_ct<ACT>(v1 + b.y, relu);
-          const uint32_t a = at(j, col, m0 + 8 * hr);
-          if (MODE == EPI_PLAIN_RES) {
-            uint32_t r;
-            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(rt + a) : "memory");
-            v0 = (v0 + __uint_as_float(r << 16)) * rs;
-            v1 = (v1 + __uint_as_float(r & 0xffff0000u)) * rs;
-          }
-          st32(ot + a, pack_bf16x2(v0, v1));
-        }
-      }
-    }
+    slab_epi_mtile<MODE, BN, ACT>(p, acc[j], c, sbias, ot + j * MTILE, rt + j * MTILE, wq, lane, relu);
   }
 }
 
@@ -217,6 +231,7 @@ template <int MODE, int BN>
 __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__ SlabParams p) {
   constexpr int MWMAX = BN >= 32 ? 128 / BN : 4;        // mw <= 4 (slab_default_mw)
   constexpr int KC1 = BN >= 64 ? BN / 64 : 1;   // EPI_FUSED_RU (bn = C = 64 | 128): 64-channel K-chunks of the 1x1x1 GEMM
+  constexpr bool TMA_STORE = slab_tma_epi(MODE) || MODE == EPI_FUSED_RU;   // y leaves through TMA box stores
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -254,7 +269,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
     tma_prefetch_desc(&p.wmap); tma_prefetch_desc(&p.wmap2);
     if (MODE == EPI_FUSED_RU) tma_prefetch_desc(&p.w1map);
   }
-  if (slab_tma_epi(MODE) && warp == 1 && lane == 0) {
+  if (TMA_STORE && warp == 1 && lane == 0) {
     tma_prefetch_desc(&p.ymap);
     if (MODE == EPI_PLAIN_RES) tma_prefetch_desc(&p.rmap);
   }
@@ -544,25 +559,22 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
         }
         continue;
       }
-      // ---- accumulators -> shared-memory staging (one [64][BN + 4] block per M-tile), once the previous tile's epilogue
-      //      of this warpgroup has read its staging ----
-      named_bar_sync(wg_bar, 128);
-#pragma unroll
-      for (int j = 0; j < MWMAX; ++j) {
-        if (j >= p.mw) break;
-        stage_acc<BN>(acc[j], stg + j * 64 * (BN + 4), tid);
-      }
-      named_bar_sync(wg_bar, 128);
-      const int h = c.h0 + lh;
       if (MODE == EPI_FUSED_RU) {
-        // ---------------- fused ResidualUnit epilogue (reference M:937-941 + the pooling half of M:229-233) ----------------
+        // ---------------- fused ResidualUnit epilogue (reference M:937-941 + the pooling half of M:229-233), per M-tile j
+        //      on the accumulator fragments: E1 writes h = bf16(ELU(conv3 + b3)) into the H buffer, the A operand of the
+        //      1x1x1 GEMM; E2 writes y = bf16(ELU(conv1 + b1)) into this warpgroup's output tile, TMA stores it and the
+        //      SE pooling reads it back.  H and the output tiles are laid out as slab_epi_mtile writes them (bn = C = 64 |
+        //      128: 128-byte rows, one 8 KB box per 64 channels); each warpgroup has its own 64 rows of both ----------------
+        constexpr int CB = slab_out_box_ch(MODE, BN), NB = BN / CB;
+        constexpr uint32_t BOX = 64 * CB * 2;
         const float* sb1 = sbias + nbias;
         const float* swk = sbias + 2 * nbias;
         float* lpart = reinterpret_cast<float*>(gen(L.lpart));
-        const int64_t kstride = (int64_t)p.W * p.Co;
-        const uint32_t wsw = (lane >> 1) & 3;
+        const uint32_t hb = L.hbuf + (uint32_t)wg * KC1 * BOX, ot = L.otile + (uint32_t)(wg * p.mw * NB) * BOX;
+        const int h = c.h0 + lh;
         const int rl = lane >> 2, piece = lane & 3;
-        const int h20 = c.h0 + sub * 4;
+        // rows of the warpgroup's 64 this thread reads back: its own (the logit), and 8 k + rl of its warp's 32 (pooling)
+        const uint32_t mrow = (uint32_t)(row & 63), mq = mrow & ~31u;
         // one record per (tile, lane quarter): the M-tiles of the tile are folded in registers (online softmax over j)
         const int recs_per_frame = p.tiles_h * p.tiles_w * 4;
         float* rec = p.se_ws + ((int64_t)(c.b * p.T + c.t) * recs_per_frame + ((c.h0 >> 4) * p.tiles_w + c.w0 / (8 * p.mw)) * 4 + sub) * (p.Co + 2);
@@ -572,7 +584,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
 #pragma unroll
           for (int i = 0; i < 8; ++i) run_acc[q][i] = 0.f;
         const uint64_t h_hi = gmma_desc_hi(1024, 128);
-        const uint32_t h_lo = desc_lo(L.hbuf) + (uint32_t)wg * ((64 * 128) >> 4);
+        const uint32_t h_lo = desc_lo(hb);
         // the 1x1x1 weights: the tile's last KC1 weight-ring stages (the producer appends them after the conv's stages);
         // they stay held until the last M-tile's second GEMM has read them
         uint32_t w1_slot[KC1], w1_par[KC1], w1_lo[KC1];
@@ -581,35 +593,22 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
           w1_slot[kc2] = w_idx; w1_par[kc2] = w_par; w1_lo[kc2] = b_lo;
           if (++w_idx == (uint32_t)p.w_stages) { w_idx = 0; w_par ^= 1; b_lo = b_lo0; } else { b_lo += w_stage16; }
         }
-        for (int j = 0; j < p.mw; ++j) {
-          const float* srow = stg + (j * 64 + row - 64 * wg) * (BN + 4);
-          // E2's transpose buffers: 2 KB per warp inside the staging rows of this warp pair, which both warps have read
-          // by the time they exchange their logit partials
-          const uint32_t stg2 = smem_u32(stg + (j * 64 + (sub & 1) * 32) * (BN + 4)) + (uint32_t)half * 2048;
-          const uint32_t wr = stg2 + lane * 64, rd = stg2 + rl * 64;
-          // E1: h = ELU(conv3 + b3) -> bf16 -> shared memory, K-major SWIZZLE_128B (128 rows x 64 channels per 16 KB K-chunk):
-          //     the A operand of the 1x1x1 GEMM; each warpgroup writes (and multiplies) its own 64 rows
-          const uint32_t hb = L.hbuf + (uint32_t)row * 128;
-          for (int c0 = half * 32; c0 < p.bn; c0 += 64) {
-            uint32_t r[32], pk[16];
-            load_row32(srow + c0, 32, r);
-            epi_pack32_t<MV2_ACT_ELU>(r, sbias + c0, pk);
-            const uint32_t hrow = hb + (uint32_t)(c0 >> 6) * 16384;
-            const uint32_t p0 = (uint32_t)(c0 & 63) >> 3;
+        // the previous tile's y stores have read the output tile (E2 writes it after the barrier that follows E1)
+        if (tid == 0) bulk_wait_read_all();
 #pragma unroll
-            for (int g = 0; g < 4; ++g)
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(hrow + (((p0 + g) ^ ((uint32_t)row & 7u)) << 4)),
-                           "r"(pk[4 * g]), "r"(pk[4 * g + 1]), "r"(pk[4 * g + 2]), "r"(pk[4 * g + 3]) : "memory");
-          }
+        for (int j = 0; j < MWMAX; ++j) {
+          if (j >= p.mw) break;
+          // E1 (H is free: the previous second GEMM completed before the barrier that follows its E2)
+          slab_epi_mtile<MODE, BN, MV2_ACT_ELU>(p, acc[j], c, sbias, hb, 0, wq, lane, false);
           fence_proxy_async();      // generic-proxy writes -> visible to the tensor core's async-proxy reads
           named_bar_sync(wg_bar, 128);
-          // second GEMM: acc[0] = H (this warpgroup's 64 rows) x W1^T; the staging of M-tile j is free again afterwards
+          // second GEMM: acc[0] = H (this warpgroup's 64 rows) x W1^T
 #pragma unroll
           for (int kc2 = 0; kc2 < KC1; ++kc2) mbar_wait(w_full + 8 * w1_slot[kc2], w1_par[kc2]);
           wgmma_fence();
 #pragma unroll
           for (int kc2 = 0; kc2 < KC1; ++kc2) {
-            const uint64_t ad = h_hi | (uint64_t)(h_lo + kc2 * (16384 >> 4)), bd = h_hi | (uint64_t)w1_lo[kc2];
+            const uint64_t ad = h_hi | (uint64_t)(h_lo + kc2 * (BOX >> 4)), bd = h_hi | (uint64_t)w1_lo[kc2];
             wgmma_bf16<BN>(acc[0], ad, bd, kc2 > 0 ? 1u : 0u);
             wgmma_bf16<BN>(acc[0], ad + 2, bd + 2, 1u);
             wgmma_bf16<BN>(acc[0], ad + 4, bd + 4, 1u);
@@ -623,31 +622,45 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
 #pragma unroll
               for (int kc2 = 0; kc2 < KC1; ++kc2) mbar_arrive(w_empty + 8 * w1_slot[kc2]);
           }
-          stage_acc<BN>(acc[0], stg + j * 64 * (BN + 4), tid);
+          // E2 -> output tile of M-tile j -> TMA box stores (boxes without an output position are skipped; TMA clips
+          // the others at the H and W edges)
+          const uint32_t otj = ot + (uint32_t)(j * NB) * BOX;
+          slab_epi_mtile<MODE, BN, MV2_ACT_ELU>(p, acc[0], c, sb1, otj, 0, wq, lane, false);
+          fence_proxy_async();
           named_bar_sync(wg_bar, 128);
-          // E2: y = ELU(conv1 + b1) -> bf16 -> global (64-byte row pieces through the transpose buffer), and per 32-position
-          //     row group (this warp's lane quarter) one SE pool record (max, sum e, sum e * y[C]) with e = exp(logit - max).
+          if (tid == 0) {
+            if (c.h0 + 8 * wg < p.H && c.w0 + 8 * j < p.W)
+#pragma unroll
+              for (int b = 0; b < NB; ++b) tma_store_5d(&p.ymap, otj + (uint32_t)b * BOX, b * CB, c.w0 + 8 * j, c.h0 + 8 * wg, c.t, c.b);
+            bulk_commit();
+          }
+          // SE logit of this thread's row on the bf16 y, like the unfused path reads it: channels half * 32 + 64 q + 0..31
+          // in order, one fma chain
+          auto ld_y = [&](int q, uint32_t m, uint32_t u) {   // 16-byte unit u (channels 8 u ..) of row m, box q
+            uint4 v;
+            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+                         : "r"(otj + (uint32_t)q * BOX + m * 128 + ((u ^ (m & 7)) << 4)) : "memory");
+            return v;
+          };
           const int w = c.w0 + 8 * j + lw;
           const bool row_ok = h < p.H && w < p.W;
-          uint32_t pk2[2][16];
           float lp = 0.f;
 #pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            const int c0 = half * 32 + 64 * q;
-            if (c0 < p.bn) {
-              uint32_t r[32];
-              load_row32(srow + c0, 32, r);
-              epi_pack32_t<MV2_ACT_ELU>(r, sb1 + c0, pk2[q]);
+          for (int q = 0; q < NB; ++q)
 #pragma unroll
-              for (int i = 0; i < 16; i += 2) {          // SE logit on the bf16-rounded y, like the unfused path reads it
-                const float4 wv = *reinterpret_cast<const float4*>(swk + c0 + 2 * i);
-                lp = fmaf(__uint_as_float(pk2[q][i] << 16), wv.x, lp);
-                lp = fmaf(__uint_as_float(pk2[q][i] & 0xffff0000u), wv.y, lp);
-                lp = fmaf(__uint_as_float(pk2[q][i + 1] << 16), wv.z, lp);
-                lp = fmaf(__uint_as_float(pk2[q][i + 1] & 0xffff0000u), wv.w, lp);
-              }
+            for (int g = 0; g < 4; ++g) {
+              const uint4 v = ld_y(q, mrow, 4 * half + g);
+              const float4 wa = *reinterpret_cast<const float4*>(swk + half * 32 + 64 * q + 8 * g);
+              const float4 wb = *reinterpret_cast<const float4*>(swk + half * 32 + 64 * q + 8 * g + 4);
+              lp = fmaf(__uint_as_float(v.x << 16), wa.x, lp);
+              lp = fmaf(__uint_as_float(v.x & 0xffff0000u), wa.y, lp);
+              lp = fmaf(__uint_as_float(v.y << 16), wa.z, lp);
+              lp = fmaf(__uint_as_float(v.y & 0xffff0000u), wa.w, lp);
+              lp = fmaf(__uint_as_float(v.z << 16), wb.x, lp);
+              lp = fmaf(__uint_as_float(v.z & 0xffff0000u), wb.y, lp);
+              lp = fmaf(__uint_as_float(v.w << 16), wb.z, lp);
+              lp = fmaf(__uint_as_float(v.w & 0xffff0000u), wb.w, lp);
             }
-          }
           // the two warps of this lane quarter hold the two halves of every row's channels: exchange the logit partials
           float* lpb = lpart + (ecount & 1u) * 256;
           ++ecount;
@@ -666,60 +679,53 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
           const float cb = mx > -INFINITY ? ex2_approx((mx - new_m) * 1.4426950408889634f) : 0.f;         // weights this M-tile
           run_s = fmaf(run_s, ca, es * cb);
           run_m = new_m;
-          const int w2 = c.w0 + 8 * j + rl;
-          const int64_t row0 = ((((int64_t)c.b * p.T + c.t) * p.H + h20) * p.W + w2) * p.Co + piece * 8;
-          const int kmax = w2 < p.W ? p.H - h20 : 0;
+          // pool sums: this lane's 8 channels (16-byte piece) of rows 8 k + rl (output rows h0 + 4 sub + k, w = w0 + 8 j + rl)
 #pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            const int c0 = half * 32 + 64 * q;
-            if (c0 < p.bn) {
+          for (int q = 0; q < NB; ++q) {
+            float t[8];
 #pragma unroll
-              for (int g = 0; g < 4; ++g)
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(wr + ((g ^ wsw) << 4)), "r"(pk2[q][4 * g]),
-                             "r"(pk2[q][4 * g + 1]), "r"(pk2[q][4 * g + 2]), "r"(pk2[q][4 * g + 3]) : "memory");
-              __syncwarp();
-              __nv_bfloat16* yp = p.epi.y + row0 + c0;
-              float t[8];
+            for (int i = 0; i < 8; ++i) t[i] = 0.f;
 #pragma unroll
-              for (int i = 0; i < 8; ++i) t[i] = 0.f;
+            for (int k = 0; k < 4; ++k) {
+              const uint4 v = ld_y(q, mq + 8 * k + rl, 4 * half + piece);
+              const uint32_t vv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                uint4 v;
-                asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
-                             : "r"(rd + k * 512 + ((piece ^ (((8 * k + rl) >> 1) & 3)) << 4)));
-                if (k < kmax) *reinterpret_cast<uint4*>(yp + k * kstride) = v;
-                const uint32_t vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  t[2 * i] = fmaf(e4[k], __uint_as_float(vv[i] << 16), t[2 * i]);
-                  t[2 * i + 1] = fmaf(e4[k], __uint_as_float(vv[i] & 0xffff0000u), t[2 * i + 1]);
-                }
+              for (int i = 0; i < 4; ++i) {
+                t[2 * i] = fmaf(e4[k], __uint_as_float(vv[i] << 16), t[2 * i]);
+                t[2 * i + 1] = fmaf(e4[k], __uint_as_float(vv[i] & 0xffff0000u), t[2 * i + 1]);
               }
-              __syncwarp();
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                t[i] += __shfl_xor_sync(0xffffffffu, t[i], 4);
-                t[i] += __shfl_xor_sync(0xffffffffu, t[i], 8);
-                t[i] += __shfl_xor_sync(0xffffffffu, t[i], 16);
-              }
-#pragma unroll
-              for (int i = 0; i < 8; ++i) run_acc[q][i] = fmaf(run_acc[q][i], ca, t[i] * cb);
             }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              t[i] += __shfl_xor_sync(0xffffffffu, t[i], 4);
+              t[i] += __shfl_xor_sync(0xffffffffu, t[i], 8);
+              t[i] += __shfl_xor_sync(0xffffffffu, t[i], 16);
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) run_acc[q][i] = fmaf(run_acc[q][i], ca, t[i] * cb);
           }
         }
         if (half == 0 && lane == 0) { rec[0] = run_m; rec[1] = run_s; }
         if (rl == 0) {
 #pragma unroll
-          for (int q = 0; q < 2; ++q) {
-            const int c0 = half * 32 + 64 * q;
-            if (c0 < p.bn) {
-              float2* dst = reinterpret_cast<float2*>(rec + 2 + c0 + piece * 8);
-              dst[0] = make_float2(run_acc[q][0], run_acc[q][1]); dst[1] = make_float2(run_acc[q][2], run_acc[q][3]);
-              dst[2] = make_float2(run_acc[q][4], run_acc[q][5]); dst[3] = make_float2(run_acc[q][6], run_acc[q][7]);
-            }
+          for (int q = 0; q < NB; ++q) {
+            float2* dst = reinterpret_cast<float2*>(rec + 2 + half * 32 + 64 * q + piece * 8);
+            dst[0] = make_float2(run_acc[q][0], run_acc[q][1]); dst[1] = make_float2(run_acc[q][2], run_acc[q][3]);
+            dst[2] = make_float2(run_acc[q][4], run_acc[q][5]); dst[3] = make_float2(run_acc[q][6], run_acc[q][7]);
           }
         }
-      } else
+        continue;
+      }
+      // ---- accumulators -> shared-memory staging (one [64][BN + 4] block per M-tile), once the previous tile's epilogue
+      //      of this warpgroup has read its staging ----
+      named_bar_sync(wg_bar, 128);
+#pragma unroll
+      for (int j = 0; j < MWMAX; ++j) {
+        if (j >= p.mw) break;
+        stage_acc<BN>(acc[j], stg + j * 64 * (BN + 4), tid);
+      }
+      named_bar_sync(wg_bar, 128);
+      const int h = c.h0 + lh;
       for (int j = 0; j < p.mw; ++j) {
         const int w = c.w0 + 8 * j + lw;
         const bool row_ok = h < p.H && w < p.W;
@@ -779,7 +785,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
         }
       }
     }
-    if (slab_tma_epi(MODE) && tid == 0) bulk_wait_all();   // the output is written before the CTA exits
+    if (TMA_STORE && tid == 0) bulk_wait_all();   // the output is written before the CTA exits
   }
 }
 
@@ -821,7 +827,8 @@ extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
 }
 
 // Shared memory left for the two TMA rings of a launch: 227 KB minus what follows them (barrier table sized for the deepest
-// rings, bias, transpose buffers, accumulator staging, [fused: H buffer]) and the alignment slack.
+// rings, bias, transpose buffers, accumulator staging or, fused, logit partials, H buffer and output tiles) and the
+// alignment slack.
 static int slab_ring_budget(const SlabParams& p, bool fused) {
   SlabParams q = p;
   q.slab_stages = 3; q.w_stages = 12;      // upper bounds for the barrier table
@@ -1037,8 +1044,9 @@ extern "C" int mv2_tc_ru_supported(const mv2_tc_ru_args* a) {
 }
 
 // tiling + shared-memory plan of the fused kernel (host arithmetic only): the slab plan of the 3x3x3 conv (one N tile of
-// bn = C; its M-tile rule gives mw = 2 at C = 64 and 1 at C = 128), one tap per weight stage, two slab stages and as many
-// weight stages as the H buffer leaves room for (the 1x1x1 weights stream through the same ring, C / 64 stages per tile)
+// bn = C; its M-tile rule gives mw = 2 at C = 64 and 1 at C = 128), one tap per weight stage, three slab stages when they
+// leave room for two weight stages next to the H buffer and the output tiles, and as many weight stages as then fit (the
+// 1x1x1 weights stream through the same ring, C / 64 stages per tile): 3 + 6 at C = 64, 3 + 5 at C = 128 (3x3x3)
 static int ru_fill_plan(const mv2_tc_ru_args* a, SlabParams& p) {
   mv2_tc_conv_args c;
   ru_as_conv_args(a, &c);
@@ -1046,9 +1054,9 @@ static int ru_fill_plan(const mv2_tc_ru_args* a, SlabParams& p) {
   MV2_CHECK_ARG(p.bn == a->C && p.n_tiles_n == 1 && p.row_bytes == 128);
   p.tpw = 1;
   p.h_stride = p.kchunks * 16384;
-  const int budget = slab_ring_budget(p, true);
-  p.slab_stages = 2;
-  p.w_stages = std::min(12, (budget - 2 * p.slab_stride) / (p.bn * p.row_bytes));
+  const int budget = slab_ring_budget(p, true), w_bytes = p.bn * p.row_bytes;
+  p.slab_stages = 3 * p.slab_stride + 2 * w_bytes <= budget ? 3 : 2;
+  p.w_stages = std::min(12, (budget - p.slab_stages * p.slab_stride) / w_bytes);
   MV2_CHECK_ARG(p.w_stages >= 2);
   p.bias1 = a->b1; p.se_wk = a->se_wk; p.se_bk = a->se_bk; p.se_ws = a->se_ws;
   return MV2_OK;
@@ -1081,6 +1089,7 @@ extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, const mv2_conv_hist* h
   const cuuint64_t strides1[1] = {(cuuint64_t)a->C * 2};
   const cuuint32_t box1[2] = {64, (cuuint32_t)p.bn};
   if (const int rc = encode_bf16_map(&p.w1map, 2, a->w1, dims1, strides1, box1, CU_TENSOR_MAP_SWIZZLE_128B, "w1")) return rc;
+  if (const int rc = slab_encode_out_maps(p, EPI_FUSED_RU)) return rc;
   return slab_launch(EPI_FUSED_RU, p, stream);
 }
 
