@@ -17,9 +17,10 @@
  *     never allocates device memory: the caller supplies workspaces.
  *   - stream ordered, no implicit synchronisation; `stream` is a cudaStream_t passed
  *     as void*.
- *   - activations are channels-last ("NDHWC"): x[b][t][h][w][c], dtype MV2_F32 or
- *     MV2_BF16; accumulation is always fp32; biases / gammas / tiny SE + quantiser
- *     weights are fp32.
+ *   - activations are channels-last ("NDHWC"): x[b][t][h][w][c], dtype MV2_F32, MV2_BF16
+ *     or MV2_F16 (wherever MV2_BF16 is accepted for activations, so is MV2_F16: same
+ *     kernels, fp16 storage with one round-to-nearest-even per stored value);
+ *     accumulation is always fp32; biases / gammas / tiny SE + quantiser weights are fp32.
  *   - there is NO CPU fallback: every function launches sm_90a kernels.
  */
 #ifndef MAGVIT2_B200_H
@@ -39,7 +40,11 @@ extern "C" {
                                their four _hist twins are removed */
 
 enum { MV2_F32 = 0, MV2_BF16 = 1,
-       MV2_U8 = 2   /* source dtype of the two layout-in entry points only: decoded uint8 frames, normalised x / 255 */ };
+       MV2_U8 = 2,  /* source dtype of the two layout-in entry points and of mv2_mse only: decoded uint8 frames, x / 255 */
+       MV2_F16 = 3  /* IEEE half: fp16 storage, fp32 accumulation */ };
+/* The tensor-core conv structs (mv2_tc_conv_args, mv2_tc_ru_args) carry their element type in a `dtype` field that sits
+ * in what was padding before fp16 existed: 0 there means bf16, so a zero-initialised struct of an older caller keeps its
+ * meaning.  MV2_F32 (also 0) is therefore not a distinct value there; the tensor-core kernels have no fp32 form anyway. */
 enum { MV2_ACT_NONE = 0, MV2_ACT_ELU = 1, MV2_ACT_SILU = 2,
        MV2_ACT_LEAKY_RELU = 3,  /* LeakyReLU(0.1), the discriminator's activation (M:117-118) */
        MV2_ACT_RELU = 4         /* ReLU, the activation of a VGG feature extractor (perceptual loss, M:1397-1405) */ };
@@ -80,7 +85,8 @@ int mv2_to_channels_first(const void* src, int src_dtype, void* dst, int dst_dty
                           int B, int C, int T, int H, int W, int t_crop, void* stream);
 /* mv2_ingest_kwpack: ingest for the tensor-core conv_in (M:1109, 7x7x7 with C_in = 3): besides the layout change and
  *   the time_padding zero frames it packs the k_w taps into the channel axis,
- *   dst[b][t+t_pad][h][w][dw*C + c] = src[b][c][t][h][w + dw - pw]  (bf16, cpack channels, zero padded),
+ *   dst[b][t+t_pad][h][w][dw*C + c] = src[b][c][t][h][w + dw - pw]  (cpack channels, zero padded; fp16 for an MV2_F16
+ *   source, bf16 for the others),
  *   so conv_in becomes a (k_t x k_h x 1)-tap implicit GEMM over cpack = 32 channels.                            */
 int mv2_ingest_kwpack(const void* src, int src_dtype, void* dst, int B, int C, int T, int H, int W,
                       int t_pad, int kw, int pw, int cpack, void* stream);
@@ -274,8 +280,8 @@ size_t mv2_mse_workspace_bytes(void);
 int mv2_maxpool2x2(const void* x, void* y, int dtype, int N, int H, int W, int C, void* stream);
 int mv2_maxpool2x2_backward(const void* gy, const void* x, void* gx, int dtype, int N, int H, int W, int C, void* stream);
 
-/* ---- wgmma / TMA implicit-GEMM convolution (bf16 in, fp32 accumulate in registers) ------------
- * Same operator family and epilogue as mv2_conv_forward, for bf16 activations, executed on the
+/* ---- wgmma / TMA implicit-GEMM convolution (bf16 or fp16 in, fp32 accumulate in registers) ------------
+ * Same operator family and epilogue as mv2_conv_forward, for bf16 or fp16 activations (mv2_tc_conv_args.dtype), executed on the
  * Hopper tensor cores (wgmma): TMA box loads with out-of-bounds zero fill implement the causal /
  * spatial halo (no padded copy, reference M:924-928), strided convs read through stride-phase
  * tensor maps, accumulators live in registers.  Weights are packed K-major: w[co][tap][ci] (bf16);
@@ -307,6 +313,8 @@ typedef struct mv2_tc_conv_args {
                           data gradient of a causal conv (the transposed conv, no leading pad) without its first Ti - To
                           frames: the video's gradient through conv_in; with Co <= 16 and kw > 3 (up to 7) it runs on
                           8- / 16-column N tiles.                                                                        */
+  int32_t dtype;       /* element type of x, w, res and y: MV2_F16, or MV2_BF16 (0, as in a zero-initialised struct, also
+                          means MV2_BF16).  It sits in what was the struct's tail padding: size and offsets are unchanged */
 } mv2_tc_conv_args;
 int mv2_tc_conv_supported(const mv2_tc_conv_args* a);
 int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream);
@@ -359,7 +367,8 @@ typedef struct mv2_tc_ru_args {
   const void* w3; const float* b3;
   const void* w1; const float* b1;
   const float* se_wk; float se_bk;
-  void* y;              /* bf16 (B, T, H, W, C) */
+  int32_t dtype;        /* element type of x, w3, w1 and y, as mv2_tc_conv_args.dtype (in what was padding) */
+  void* y;              /* bf16 / fp16 (B, T, H, W, C) */
   float* se_ws;
   int32_t B, T, H, W, C;
   int32_t kt, kh, kw;

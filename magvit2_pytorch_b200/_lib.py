@@ -12,7 +12,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MV2_LIB_PATH") or os.path.join(_HERE, "libmagvit2_b200.so")   # env override: A/B builds
 
-MV2_F32, MV2_BF16, MV2_U8 = 0, 1, 2
+MV2_F32, MV2_BF16, MV2_U8, MV2_F16 = 0, 1, 2, 3
 ACT_NONE, ACT_ELU, ACT_SILU, ACT_LEAKY_RELU, ACT_RELU = 0, 1, 2, 3, 4
 SHUFFLE_NONE, SHUFFLE_SPACE, SHUFFLE_TIME = 0, 1, 2
 
@@ -61,6 +61,7 @@ class TcConvArgs(C.Structure):
         ("pt", C.c_int32), ("ph", C.c_int32), ("pw", C.c_int32),
         ("act", C.c_int32), ("shuffle", C.c_int32), ("epi_mode", C.c_int32),
         ("oscale", C.c_void_p), ("out_layout", C.c_int32),
+        ("dtype", C.c_int32),    # MV2_F16, or MV2_BF16 (also 0)
     ]
 
 
@@ -68,7 +69,7 @@ class TcRuArgs(C.Structure):
     """mv2_tc_ru_args (fused ResidualUnit front half; see include/magvit2_b200.h)."""
     _fields_ = [
         ("x", C.c_void_p), ("w3", C.c_void_p), ("b3", C.c_void_p), ("w1", C.c_void_p), ("b1", C.c_void_p),
-        ("se_wk", C.c_void_p), ("se_bk", C.c_float), ("y", C.c_void_p), ("se_ws", C.c_void_p),
+        ("se_wk", C.c_void_p), ("se_bk", C.c_float), ("dtype", C.c_int32), ("y", C.c_void_p), ("se_ws", C.c_void_p),
         ("B", C.c_int32), ("T", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("C", C.c_int32),
         ("kt", C.c_int32), ("kh", C.c_int32), ("kw", C.c_int32),
     ]

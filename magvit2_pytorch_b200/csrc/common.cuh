@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
@@ -48,6 +49,20 @@ template <> __device__ __forceinline__ float to_f32<uint8_t>(uint8_t v) { return
 template <typename T> __device__ __forceinline__ T from_f32(float v);
 template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
 template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+template <> __device__ __forceinline__ float to_f32<__half>(__half v) { return __half2float(v); }
+template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
+
+// The two 16-bit activation dtypes (MV2_BF16, MV2_F16): fp32 accumulation, one round-to-nearest-even per stored value.
+// pair_t<T> is the 2-element vector type of T; pair_to_f2 / f2_to_pair convert it to and from fp32.
+template <typename T> struct pair_of;
+template <> struct pair_of<__nv_bfloat16> { typedef __nv_bfloat162 type; };
+template <> struct pair_of<__half> { typedef __half2 type; };
+template <typename T> using pair_t = typename pair_of<T>::type;
+__device__ __forceinline__ float2 pair_to_f2(__nv_bfloat162 v) { return __bfloat1622float2(v); }
+__device__ __forceinline__ float2 pair_to_f2(__half2 v) { return __half22float2(v); }
+template <typename T> __device__ __forceinline__ pair_t<T> f2_to_pair(float a, float b);
+template <> __device__ __forceinline__ __nv_bfloat162 f2_to_pair<__nv_bfloat16>(float a, float b) { return __floats2bfloat162_rn(a, b); }
+template <> __device__ __forceinline__ __half2 f2_to_pair<__half>(float a, float b) { return __floats2half2_rn(a, b); }
 
 // Activations.  expm1f / expf (not the fast intrinsics): the fp32 path must track the
 // reference's libm-based CPU results to ~1 ulp.

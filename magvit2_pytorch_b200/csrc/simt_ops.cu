@@ -8,6 +8,7 @@
 //
 // Reference semantics are cited per entry point in include/magvit2_b200.h.
 #include "common.cuh"
+#include <type_traits>
 #include <math.h>
 #include <stdlib.h>
 #include <mutex>
@@ -116,6 +117,14 @@ static int dispatch_transpose(const void* src, int sd, void* dst, int dd, int B,
     return launch_transpose<uint8_t, float>(src, dst, B, R, S, src_S_total, dst_S_total, s_off_src, s_off_dst, src_is_rs, st);
   if (sd == MV2_U8 && dd == MV2_BF16)
     return launch_transpose<uint8_t, __nv_bfloat16>(src, dst, B, R, S, src_S_total, dst_S_total, s_off_src, s_off_dst, src_is_rs, st);
+  if (sd == MV2_F32 && dd == MV2_F16)
+    return launch_transpose<float, __half>(src, dst, B, R, S, src_S_total, dst_S_total, s_off_src, s_off_dst, src_is_rs, st);
+  if (sd == MV2_F16 && dd == MV2_F32)
+    return launch_transpose<__half, float>(src, dst, B, R, S, src_S_total, dst_S_total, s_off_src, s_off_dst, src_is_rs, st);
+  if (sd == MV2_F16 && dd == MV2_F16)
+    return launch_transpose<__half, __half>(src, dst, B, R, S, src_S_total, dst_S_total, s_off_src, s_off_dst, src_is_rs, st);
+  if (sd == MV2_U8 && dd == MV2_F16)
+    return launch_transpose<uint8_t, __half>(src, dst, B, R, S, src_S_total, dst_S_total, s_off_src, s_off_dst, src_is_rs, st);
   set_error("unsupported dtype pair %d -> %d", sd, dd);
   return MV2_E_ARG;
 }
@@ -126,8 +135,8 @@ static int dispatch_transpose(const void* src, int sd, void* dst, int dd, int B,
 //   dst[b][t + t_pad][h][w][dw * C + c] = src[b][c][t][h][w + dw - pw]   (0 outside the image / for padded channels)
 // One block per (b, t, h) image row: the C source rows are staged in shared memory with a zero halo (coalesced
 // loads, each source element read once), then every thread assembles 16-byte groups of 8 packed channels from them.
-template <typename TS>
-__global__ void __launch_bounds__(256) ingest_kwpack_kernel(const TS* __restrict__ src, __nv_bfloat16* __restrict__ dst,
+template <typename TS, typename TD>
+__global__ void __launch_bounds__(256) ingest_kwpack_kernel(const TS* __restrict__ src, TD* __restrict__ dst,
                                                             int B, int C, int T, int H, int W, int t_pad, int kw, int pw,
                                                             int cpack) {
   pdl_wait();
@@ -147,7 +156,7 @@ __global__ void __launch_bounds__(256) ingest_kwpack_kernel(const TS* __restrict
     srow[i] = x;
   }
   __syncthreads();
-  __nv_bfloat16* drow = dst + (((int64_t)b * (T + t_pad) + t) * H + h) * (int64_t)W * cpack;
+  TD* drow = dst + (((int64_t)b * (T + t_pad) + t) * H + h) * (int64_t)W * cpack;
   for (int i = threadIdx.x; i < W * groups; i += blockDim.x) {
     const int g = i % groups, w = i / groups;
     int dw = (g * 8) / C, c = g * 8 - dw * C;
@@ -158,8 +167,8 @@ __global__ void __launch_bounds__(256) ingest_kwpack_kernel(const TS* __restrict
       if (++c == C) { c = 0; ++dw; }
     }
     uint4 o;
-    __nv_bfloat162 p0 = __floats2bfloat162_rn(v[0], v[1]), p1 = __floats2bfloat162_rn(v[2], v[3]);
-    __nv_bfloat162 p2 = __floats2bfloat162_rn(v[4], v[5]), p3 = __floats2bfloat162_rn(v[6], v[7]);
+    pair_t<TD> p0 = f2_to_pair<TD>(v[0], v[1]), p1 = f2_to_pair<TD>(v[2], v[3]);
+    pair_t<TD> p2 = f2_to_pair<TD>(v[4], v[5]), p3 = f2_to_pair<TD>(v[6], v[7]);
     o.x = *reinterpret_cast<uint32_t*>(&p0); o.y = *reinterpret_cast<uint32_t*>(&p1);
     o.z = *reinterpret_cast<uint32_t*>(&p2); o.w = *reinterpret_cast<uint32_t*>(&p3);
     *reinterpret_cast<uint4*>(drow + (int64_t)i * 8) = o;
@@ -394,8 +403,8 @@ __device__ __forceinline__ void se_bulk_load(uint32_t dst, const void* src, uint
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
-template <int VEC, int G>   // G = C / VEC lanes per row (compile time: the shuffle reductions unroll)
-__global__ void __launch_bounds__(256) se_pool_online_kernel(const __nv_bfloat16* __restrict__ y, int P, int C,
+template <typename T, int VEC, int G>   // G = C / VEC lanes per row (compile time: the shuffle reductions unroll)
+__global__ void __launch_bounds__(256) se_pool_online_kernel(const T* __restrict__ y, int P, int C,
                                                              const float* __restrict__ wk, float bk,
                                                              float* __restrict__ ws, int n_chunks, int chunk_rows) {
   extern __shared__ __align__(128) float dyn[];   // ring of SE_STAGES batches; reused as [R][C + 2] + [R] for the merge
@@ -412,7 +421,7 @@ __global__ void __launch_bounds__(256) se_pool_online_kernel(const __nv_bfloat16
   const int n_batches = (cnt + batch_rows - 1) / batch_rows;
   const uint32_t ring = (uint32_t)__cvta_generic_to_shared(dyn);
   const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(full_bar);
-  const __nv_bfloat16* ychunk = y + ((int64_t)f * P + p0) * C;
+  const T* ychunk = y + ((int64_t)f * P + p0) * C;
   if (tid == 0) {
     for (int s_ = 0; s_ < SE_STAGES; ++s_) se_mbar_init(bar0 + 8 * s_, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -462,10 +471,10 @@ __global__ void __launch_bounds__(256) se_pool_online_kernel(const __nv_bfloat16
       float dot = 0.f;
 #pragma unroll
       for (int u = 0; u < VEC / 8; ++u) {
-        const __nv_bfloat162* vb = reinterpret_cast<const __nv_bfloat162*>(&raw[uu][u]);
+        const pair_t<T>* vb = reinterpret_cast<const pair_t<T>*>(&raw[uu][u]);
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const float2 fv = __bfloat1622float2(vb[q]);
+          const float2 fv = pair_to_f2(vb[q]);
           v[uu][u * 8 + 2 * q] = fv.x;
           v[uu][u * 8 + 2 * q + 1] = fv.y;
         }
@@ -635,7 +644,8 @@ __global__ void gate_residual_kernel(const T* __restrict__ y, const T* __restric
 }
 
 // 8 bf16 per thread (16-byte accesses); requires C % 8 == 0
-__global__ void gate_residual_bf16x8_kernel(const uint4* __restrict__ y, const uint4* __restrict__ x,
+template <typename T>
+__global__ void gate_residual_x8_kernel(const uint4* __restrict__ y, const uint4* __restrict__ x,
                                             const float* __restrict__ gates, uint4* __restrict__ out,
                                             int64_t total8, int64_t PC8, int C8) {
   pdl_wait();
@@ -646,15 +656,15 @@ __global__ void gate_residual_bf16x8_kernel(const uint4* __restrict__ y, const u
     const uint4 yv = y[i], xv = x[i];
     const float4 g0 = *reinterpret_cast<const float4*>(gates + f * (C8 * 8) + c);
     const float4 g1 = *reinterpret_cast<const float4*>(gates + f * (C8 * 8) + c + 4);
-    const __nv_bfloat162* yb = reinterpret_cast<const __nv_bfloat162*>(&yv);
-    const __nv_bfloat162* xb = reinterpret_cast<const __nv_bfloat162*>(&xv);
+    const pair_t<T>* yb = reinterpret_cast<const pair_t<T>*>(&yv);
+    const pair_t<T>* xb = reinterpret_cast<const pair_t<T>*>(&xv);
     const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
     uint4 o;
     uint32_t* ob = reinterpret_cast<uint32_t*>(&o);
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      const float2 yf = __bfloat1622float2(yb[q]), xf = __bfloat1622float2(xb[q]);
-      __nv_bfloat162 r = __floats2bfloat162_rn(fmaf(gg[2 * q], yf.x, xf.x), fmaf(gg[2 * q + 1], yf.y, xf.y));
+      const float2 yf = pair_to_f2(yb[q]), xf = pair_to_f2(xb[q]);
+      pair_t<T> r = f2_to_pair<T>(fmaf(gg[2 * q], yf.x, xf.x), fmaf(gg[2 * q + 1], yf.y, xf.y));
       ob[q] = *reinterpret_cast<uint32_t*>(&r);
     }
     out[i] = o;
@@ -782,11 +792,11 @@ __global__ void __launch_bounds__(256) rmsnorm_kernel(const T* __restrict__ x, T
 // (C <= 1024: at most 4 uint4 per lane).
 // One warp normalises RN_TPW (template) tokens: all of their 16-byte loads are issued before the first reduction (one token per
 // warp left a single load in flight per lane and ran at a third of the HBM rate).
-template <int NU, int RN_TPW>   // 256-channel slabs per token: C <= 256 * NU
-__global__ void __launch_bounds__(256) rmsnorm_bf16x8_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ out,
+template <typename T, int NU, int RN_TPW>   // 256-channel slabs per token: C <= 256 * NU
+__global__ void __launch_bounds__(256) rmsnorm_x8_kernel(const T* __restrict__ x, T* __restrict__ out,
                                                              const float* __restrict__ gamma, int64_t n_tok, int T_,
                                                              int P, int C, int token_shift,
-                                                             const __nv_bfloat16* __restrict__ prev, int64_t prev_stride) {
+                                                             const T* __restrict__ prev, int64_t prev_stride) {
   pdl_wait();
   pdl_launch_dependents();
   const int lane = threadIdx.x & 31;
@@ -799,8 +809,8 @@ __global__ void __launch_bounds__(256) rmsnorm_bf16x8_kernel(const __nv_bfloat16
     const int64_t tok = tok0 + i;
     const bool valid = tok < n_tok;
     const int t = valid ? (int)((tok / P) % T_) : 0;
-    const __nv_bfloat16* row = x + (valid ? tok : tok0) * C;
-    const __nv_bfloat16* prow = t > 0 || !prev ? row - (int64_t)P * C
+    const T* row = x + (valid ? tok : tok0) * C;
+    const T* prow = t > 0 || !prev ? row - (int64_t)P * C
                                                : prev + ((valid ? tok : tok0) / ((int64_t)T_ * P)) * prev_stride + ((valid ? tok : tok0) % P) * C;
     const bool has_prev = t > 0 || prev;
 #pragma unroll
@@ -819,10 +829,10 @@ __global__ void __launch_bounds__(256) rmsnorm_bf16x8_kernel(const __nv_bfloat16
     float a = 0.f;
 #pragma unroll
     for (int u = 0; u < NU; ++u) {
-      const __nv_bfloat162* vb = reinterpret_cast<const __nv_bfloat162*>(&v[i][u]);
+      const pair_t<T>* vb = reinterpret_cast<const pair_t<T>*>(&v[i][u]);
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const float2 f = __bfloat1622float2(vb[q]);
+        const float2 f = pair_to_f2(vb[q]);
         a = fmaf(f.x, f.x, a);
         a = fmaf(f.y, f.y, a);
       }
@@ -842,13 +852,13 @@ __global__ void __launch_bounds__(256) rmsnorm_bf16x8_kernel(const __nv_bfloat16
       for (int i = 0; i < RN_TPW; ++i) {
         if (tok0 + i < n_tok) {
           const float rinv = 1.f / fmaxf(sqrtf(ss[i]), 1e-12f);   // x / max(|x|, eps) as one reciprocal per token
-          const __nv_bfloat162* vb = reinterpret_cast<const __nv_bfloat162*>(&v[i][u]);
+          const pair_t<T>* vb = reinterpret_cast<const pair_t<T>*>(&v[i][u]);
           uint4 o;
           uint32_t* ob = reinterpret_cast<uint32_t*>(&o);
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
-            const float2 f = __bfloat1622float2(vb[q]);
-            __nv_bfloat162 r = __floats2bfloat162_rn(((f.x * rinv) * scale) * gg[2 * q], ((f.y * rinv) * scale) * gg[2 * q + 1]);
+            const float2 f = pair_to_f2(vb[q]);
+            pair_t<T> r = f2_to_pair<T>(((f.x * rinv) * scale) * gg[2 * q], ((f.y * rinv) * scale) * gg[2 * q + 1]);
             ob[q] = *reinterpret_cast<uint32_t*>(&r);
           }
           *reinterpret_cast<uint4*>(out + (tok0 + i) * C + c) = o;
@@ -988,13 +998,13 @@ __global__ void __launch_bounds__(128) attention_dropout_kernel(const mv2_attn_a
 // bf16 only (the fp32 path keeps the general kernel and its summation order).
 // ------------------------------------------------------------------------------------------
 constexpr int AS_L = 8, AS_M = 8;      // max tokens / memory slots
-template <int DPL, bool DROP>
+template <typename T, int DPL, bool DROP>
 __device__ __forceinline__ void attention_small_body(const mv2_attn_args& a, const AttnDrop& dr, const AttnTail tl = AttnTail{0, -1, nullptr, 0}) {
   pdl_wait();
   pdl_launch_dependents();
   constexpr int D = DPL * 32;
-  const __nv_bfloat16* __restrict__ qkv = (const __nv_bfloat16*)a.qkv;
-  __nv_bfloat16* __restrict__ out = (__nv_bfloat16*)a.out;
+  const T* __restrict__ qkv = (const T*)a.qkv;
+  T* __restrict__ out = (T*)a.out;
   const int lane = threadIdx.x & 31;
   const int64_t wid = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);       // (sequence, head)
   const int64_t n_seq = (int64_t)a.n_outer * a.n_inner;
@@ -1024,13 +1034,13 @@ __device__ __forceinline__ void attention_small_body(const mv2_attn_args& a, con
       float qv = 0.f, kv = 0.f, vv = 0.f;
       if (i < L && tl.q) {        // K/V cache rows '(kv h d)'; the queries of rows >= q_begin from the chunk
         const int64_t row = (base + (int64_t)i * a.tok_stride) * (2 * (int64_t)HD) + h * D + d;
-        kv = __bfloat162float(qkv[row]); vv = __bfloat162float(qkv[row + HD]);
+        kv = to_f32(qkv[row]); vv = to_f32(qkv[row + HD]);
         if (i >= tl.q_begin)
-          qv = __bfloat162float(((const __nv_bfloat16*)tl.q)[((seq / a.n_inner) * tl.q_outer + (seq % a.n_inner) * a.inner_stride +
+          qv = to_f32(((const T*)tl.q)[((seq / a.n_inner) * tl.q_outer + (seq % a.n_inner) * a.inner_stride +
                                                             (int64_t)(i - tl.q_begin) * a.tok_stride) * row_stride + h * D + d]);
       } else if (i < L) {
         const int64_t row = (base + (int64_t)i * a.tok_stride) * row_stride + h * D + d;
-        qv = __bfloat162float(qkv[row]); kv = __bfloat162float(qkv[row + HD]); vv = __bfloat162float(qkv[row + 2 * HD]);
+        qv = to_f32(qkv[row]); kv = to_f32(qkv[row + HD]); vv = to_f32(qkv[row + 2 * HD]);
       }
       q[i][dd] = qv; k[AS_M + i][dd] = kv; v[AS_M + i][dd] = vv;
     }
@@ -1073,20 +1083,31 @@ __device__ __forceinline__ void attention_small_body(const mv2_attn_args& a, con
     }
     const float inv = DROP ? dr.scale / den : 1.f / den;
     const int64_t obase = tl.out_outer < 0 ? base : (seq / a.n_inner) * tl.out_outer + (seq % a.n_inner) * a.inner_stride;
-    __nv_bfloat16* orow = out + (obase + (int64_t)(i - tl.q_begin) * a.tok_stride) * HD + h * D;
+    T* orow = out + (obase + (int64_t)(i - tl.q_begin) * a.tok_stride) * HD + h * D;
 #pragma unroll
-    for (int dd = 0; dd < DPL; ++dd) orow[lane + 32 * dd] = __float2bfloat16_rn(o[dd] * inv);
+    for (int dd = 0; dd < DPL; ++dd) orow[lane + 32 * dd] = from_f32<T>(o[dd] * inv);
   }
 }
+// bf16 kernels keep their names; the fp16 ones are the _f16_ twins of the same bodies (AttnK16<T> picks one)
 template <int DPL>
-__global__ void __launch_bounds__(256) attention_small_kernel(const mv2_attn_args a) { attention_small_body<DPL, false>(a, AttnDrop{}); }
+__global__ void __launch_bounds__(256) attention_small_kernel(const mv2_attn_args a) { attention_small_body<__nv_bfloat16, DPL, false>(a, AttnDrop{}); }
 template <int DPL>
 __global__ void __launch_bounds__(256) attention_small_tail_kernel(const mv2_attn_args a, const AttnTail tl) {
-  attention_small_body<DPL, false>(a, AttnDrop{}, tl);
+  attention_small_body<__nv_bfloat16, DPL, false>(a, AttnDrop{}, tl);
 }
 template <int DPL>
 __global__ void __launch_bounds__(256) attention_small_dropout_kernel(const mv2_attn_args a, const AttnDrop d) {
-  attention_small_body<DPL, true>(a, d);
+  attention_small_body<__nv_bfloat16, DPL, true>(a, d);
+}
+template <int DPL>
+__global__ void __launch_bounds__(256) attention_small_f16_kernel(const mv2_attn_args a) { attention_small_body<__half, DPL, false>(a, AttnDrop{}); }
+template <int DPL>
+__global__ void __launch_bounds__(256) attention_small_tail_f16_kernel(const mv2_attn_args a, const AttnTail tl) {
+  attention_small_body<__half, DPL, false>(a, AttnDrop{}, tl);
+}
+template <int DPL>
+__global__ void __launch_bounds__(256) attention_small_dropout_f16_kernel(const mv2_attn_args a, const AttnDrop d) {
+  attention_small_body<__half, DPL, true>(a, d);
 }
 
 
@@ -1098,26 +1119,35 @@ __global__ void __launch_bounds__(256) attention_small_dropout_kernel(const mv2_
 // ------------------------------------------------------------------------------------------
 constexpr int FA_Q = 128, FA_KT = 64;     // 8 warps x 16 queries per block; keys / values staged 64 at a time
 
-__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+// T = __nv_bfloat16 or __half selects the operand type of the MMA (ldmatrix and the fragment layouts are the same)
+template <typename T>
+__device__ __forceinline__ void mma_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  if constexpr (std::is_same<T, __half>::value)
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+  else
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-__device__ __forceinline__ uint32_t pack2_bf16(float lo, float hi) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
+template <typename T>
+__device__ __forceinline__ uint32_t pack2_16(float lo, float hi) {
+  pair_t<T> v = f2_to_pair<T>(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-template <int D, bool DROP>
+template <typename T, int D, bool DROP>
 __device__ __forceinline__ void attention_mma_body(const mv2_attn_args& a, const AttnDrop& dr) {
   pdl_wait();
   pdl_launch_dependents();
   constexpr int DK = D / 16, DN = D / 8;
-  __shared__ __align__(16) __nv_bfloat16 Ks[FA_KT][D + 8];
-  __shared__ __align__(16) __nv_bfloat16 Vt[D][FA_KT + 8];
-  const __nv_bfloat16* __restrict__ qkv = (const __nv_bfloat16*)a.qkv;
-  __nv_bfloat16* __restrict__ out = (__nv_bfloat16*)a.out;
+  __shared__ __align__(16) T Ks[FA_KT][D + 8];
+  __shared__ __align__(16) T Vt[D][FA_KT + 8];
+  const T* __restrict__ qkv = (const T*)a.qkv;
+  T* __restrict__ out = (T*)a.out;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t = lane & 3;
   const int h = blockIdx.y;
@@ -1134,8 +1164,8 @@ __device__ __forceinline__ void attention_mma_body(const mv2_attn_args& a, const
   uint32_t qa[DK][4];
   {
     const int r0 = q0 + g, r1 = q0 + g + 8;
-    const __nv_bfloat16* p0 = qkv + (base + (int64_t)min(r0, a.L - 1) * a.tok_stride) * row_stride + h * D;
-    const __nv_bfloat16* p1 = qkv + (base + (int64_t)min(r1, a.L - 1) * a.tok_stride) * row_stride + h * D;
+    const T* p0 = qkv + (base + (int64_t)min(r0, a.L - 1) * a.tok_stride) * row_stride + h * D;
+    const T* p1 = qkv + (base + (int64_t)min(r1, a.L - 1) * a.tok_stride) * row_stride + h * D;
 #pragma unroll
     for (int k = 0; k < DK; ++k) {
       qa[k][0] = *reinterpret_cast<const uint32_t*>(p0 + k * 16 + t * 2);
@@ -1165,12 +1195,12 @@ __device__ __forceinline__ void attention_mma_body(const mv2_attn_args& a, const
       if (jg < a.n_mem) {
         const float* mk = a.mem_kv + (((int64_t)0 * a.heads + h) * a.n_mem + jg) * D + c;
         const float* mv = a.mem_kv + (((int64_t)1 * a.heads + h) * a.n_mem + jg) * D + c;
-        kv4.x = pack2_bf16(mk[0], mk[1]); kv4.y = pack2_bf16(mk[2], mk[3]);
-        kv4.z = pack2_bf16(mk[4], mk[5]); kv4.w = pack2_bf16(mk[6], mk[7]);
-        vv4.x = pack2_bf16(mv[0], mv[1]); vv4.y = pack2_bf16(mv[2], mv[3]);
-        vv4.z = pack2_bf16(mv[4], mv[5]); vv4.w = pack2_bf16(mv[6], mv[7]);
+        kv4.x = pack2_16<T>(mk[0], mk[1]); kv4.y = pack2_16<T>(mk[2], mk[3]);
+        kv4.z = pack2_16<T>(mk[4], mk[5]); kv4.w = pack2_16<T>(mk[6], mk[7]);
+        vv4.x = pack2_16<T>(mv[0], mv[1]); vv4.y = pack2_16<T>(mv[2], mv[3]);
+        vv4.z = pack2_16<T>(mv[4], mv[5]); vv4.w = pack2_16<T>(mv[6], mv[7]);
       } else if (jg < Ltot) {
-        const __nv_bfloat16* row = qkv + (base + (int64_t)(jg - a.n_mem) * a.tok_stride) * row_stride;
+        const T* row = qkv + (base + (int64_t)(jg - a.n_mem) * a.tok_stride) * row_stride;
         kv4 = *reinterpret_cast<const uint4*>(row + HD + h * D + c);
         vv4 = *reinterpret_cast<const uint4*>(row + 2 * HD + h * D + c);
       }
@@ -1187,7 +1217,7 @@ __device__ __forceinline__ void attention_mma_body(const mv2_attn_args& a, const
       const int idx = tid + it * 256;
       const int j = idx / (D / 8), c = (idx % (D / 8)) * 8;
       *reinterpret_cast<uint4*>(&Ks[j][c]) = kr[it];
-      const __nv_bfloat16* vb = reinterpret_cast<const __nv_bfloat16*>(&vr[it]);
+      const T* vb = reinterpret_cast<const T*>(&vr[it]);
 #pragma unroll
       for (int q = 0; q < 8; ++q) Vt[c + q][j] = vb[q];
     }
@@ -1203,7 +1233,7 @@ __device__ __forceinline__ void attention_mma_body(const mv2_attn_args& a, const
       for (int k = 0; k < DK; ++k) {
         const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&Ks[nt * 8 + g][k * 16 + t * 2]);
         const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&Ks[nt * 8 + g][k * 16 + 8 + t * 2]);
-        mma_bf16_16816(sfr[nt], qa[k], b0, b1);
+        mma_16816<T>(sfr[nt], qa[k], b0, b1);
       }
     }
     // ---- online softmax ----
@@ -1253,15 +1283,15 @@ __device__ __forceinline__ void attention_mma_body(const mv2_attn_args& a, const
 #pragma unroll
     for (int kk = 0; kk < FA_KT / 16; ++kk) {
       uint32_t pa[4];
-      pa[0] = pack2_bf16(sfr[2 * kk][0], sfr[2 * kk][1]);
-      pa[1] = pack2_bf16(sfr[2 * kk][2], sfr[2 * kk][3]);
-      pa[2] = pack2_bf16(sfr[2 * kk + 1][0], sfr[2 * kk + 1][1]);
-      pa[3] = pack2_bf16(sfr[2 * kk + 1][2], sfr[2 * kk + 1][3]);
+      pa[0] = pack2_16<T>(sfr[2 * kk][0], sfr[2 * kk][1]);
+      pa[1] = pack2_16<T>(sfr[2 * kk][2], sfr[2 * kk][3]);
+      pa[2] = pack2_16<T>(sfr[2 * kk + 1][0], sfr[2 * kk + 1][1]);
+      pa[3] = pack2_16<T>(sfr[2 * kk + 1][2], sfr[2 * kk + 1][3]);
 #pragma unroll
       for (int dn = 0; dn < DN; ++dn) {
         const uint32_t b0 = *reinterpret_cast<const uint32_t*>(&Vt[dn * 8 + g][kk * 16 + t * 2]);
         const uint32_t b1 = *reinterpret_cast<const uint32_t*>(&Vt[dn * 8 + g][kk * 16 + 8 + t * 2]);
-        mma_bf16_16816(o[dn], pa, b0, b1);
+        mma_16816<T>(o[dn], pa, b0, b1);
       }
     }
   }
@@ -1272,22 +1302,45 @@ __device__ __forceinline__ void attention_mma_body(const mv2_attn_args& a, const
   const float i0 = DROP ? dr.scale / l0 : 1.f / l0, i1 = DROP ? dr.scale / l1 : 1.f / l1;
   const int r0 = q0 + g, r1 = q0 + g + 8;
   if (r0 < a.L) {
-    __nv_bfloat16* orow = out + (base + (int64_t)r0 * a.tok_stride) * HD + h * D;
+    T* orow = out + (base + (int64_t)r0 * a.tok_stride) * HD + h * D;
 #pragma unroll
-    for (int dn = 0; dn < DN; ++dn) *reinterpret_cast<uint32_t*>(orow + dn * 8 + t * 2) = pack2_bf16(o[dn][0] * i0, o[dn][1] * i0);
+    for (int dn = 0; dn < DN; ++dn) *reinterpret_cast<uint32_t*>(orow + dn * 8 + t * 2) = pack2_16<T>(o[dn][0] * i0, o[dn][1] * i0);
   }
   if (r1 < a.L) {
-    __nv_bfloat16* orow = out + (base + (int64_t)r1 * a.tok_stride) * HD + h * D;
+    T* orow = out + (base + (int64_t)r1 * a.tok_stride) * HD + h * D;
 #pragma unroll
-    for (int dn = 0; dn < DN; ++dn) *reinterpret_cast<uint32_t*>(orow + dn * 8 + t * 2) = pack2_bf16(o[dn][2] * i1, o[dn][3] * i1);
+    for (int dn = 0; dn < DN; ++dn) *reinterpret_cast<uint32_t*>(orow + dn * 8 + t * 2) = pack2_16<T>(o[dn][2] * i1, o[dn][3] * i1);
   }
 }
 template <int D>
-__global__ void __launch_bounds__(256) attention_mma_kernel(const mv2_attn_args a) { attention_mma_body<D, false>(a, AttnDrop{}); }
+__global__ void __launch_bounds__(256) attention_mma_kernel(const mv2_attn_args a) { attention_mma_body<__nv_bfloat16, D, false>(a, AttnDrop{}); }
 template <int D>
 __global__ void __launch_bounds__(256) attention_mma_dropout_kernel(const mv2_attn_args a, const AttnDrop d) {
-  attention_mma_body<D, true>(a, d);
+  attention_mma_body<__nv_bfloat16, D, true>(a, d);
 }
+template <int D>
+__global__ void __launch_bounds__(256) attention_mma_f16_kernel(const mv2_attn_args a) { attention_mma_body<__half, D, false>(a, AttnDrop{}); }
+template <int D>
+__global__ void __launch_bounds__(256) attention_mma_dropout_f16_kernel(const mv2_attn_args a, const AttnDrop d) {
+  attention_mma_body<__half, D, true>(a, d);
+}
+
+// the kernels of one 16-bit element type
+template <typename T> struct AttnK16;
+template <> struct AttnK16<__nv_bfloat16> {
+  template <int D> static constexpr auto mma() { return attention_mma_kernel<D>; }
+  template <int D> static constexpr auto mma_drop() { return attention_mma_dropout_kernel<D>; }
+  template <int P> static constexpr auto small() { return attention_small_kernel<P>; }
+  template <int P> static constexpr auto small_drop() { return attention_small_dropout_kernel<P>; }
+  template <int P> static constexpr auto small_tail() { return attention_small_tail_kernel<P>; }
+};
+template <> struct AttnK16<__half> {
+  template <int D> static constexpr auto mma() { return attention_mma_f16_kernel<D>; }
+  template <int D> static constexpr auto mma_drop() { return attention_mma_dropout_f16_kernel<D>; }
+  template <int P> static constexpr auto small() { return attention_small_f16_kernel<P>; }
+  template <int P> static constexpr auto small_drop() { return attention_small_dropout_f16_kernel<P>; }
+  template <int P> static constexpr auto small_tail() { return attention_small_tail_f16_kernel<P>; }
+};
 
 // keep mask of mv2_attention_dropout_mask: one thread per (sequence, head, query, 4-key group), keep[seq][h][i][n_mem + L]
 __global__ void __launch_bounds__(256) attention_dropout_mask_kernel(int64_t n_groups, int heads, int L, int Ltot, const AttnDrop d,
@@ -1509,12 +1562,16 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], const void* 
 
 constexpr int LAM_RS = LAM_F + 8;                                            // bf16 elements per token row (176 B: conflict-free)
 constexpr size_t LAM_REDUCE_SMEM = (size_t)2 * LAM_TB * LAM_RS * 2 + (size_t)16 * (LAM_TB + 8) * 2;   // phi hi + lo, v^T
+constexpr size_t LAM_REDUCE_SMEM_F16 = LAM_REDUCE_SMEM + (size_t)16 * (LAM_TB + 8) * 2;                // + the v^T lo part
 
-__global__ void __launch_bounds__(128) linattn_reduce_mma_kernel(const __nv_bfloat16* __restrict__ kv, float* __restrict__ ws,
-                                                                 int L, int heads, int n_chunks) {
-  pdl_wait();
-  pdl_launch_dependents();
-  // phi is carried as a bf16 hi + lo pair (two MMAs) so the quadratic features keep ~16 mantissa bits; v is bf16 already.
+// T: element type of kv (bf16 or fp16).  The MMA operands are bf16 in both cases: the values are widened to fp32 at the
+// load and split into bf16 hi + lo pairs, so only the loads depend on T.
+template <typename T>
+__device__ __forceinline__ void linattn_reduce_mma_body(const T* __restrict__ kv, float* __restrict__ ws, int L, int heads,
+                                                        int n_chunks) {
+  constexpr bool V_LO = std::is_same<T, __half>::value;
+  // phi is carried as a bf16 hi + lo pair (two MMAs) so the quadratic features keep ~16 mantissa bits; a bf16 v is exact in
+  // bf16, an fp16 v (11 significant bits) is exact as a bf16 hi + lo pair (a third MMA: phi hi x v lo).
   // Token-major staging [token][feature] (one token per thread, 16-byte stores: a 176-byte row pitch puts the 32 rows of a warp
   // in 8 distinct bank groups = the minimal 4 wavefronts per store); the MMA wants A = phi^T [feature][token], which
   // ldmatrix.trans delivers straight from the token-major tile.  (The former feature-major layout needed 160 two-byte stores
@@ -1523,6 +1580,7 @@ __global__ void __launch_bounds__(128) linattn_reduce_mma_kernel(const __nv_bflo
   __nv_bfloat16 (*phi_s)[LAM_RS] = reinterpret_cast<__nv_bfloat16 (*)[LAM_RS]>(lam_dyn);                                // [token][feature] hi
   __nv_bfloat16 (*phi_l)[LAM_RS] = reinterpret_cast<__nv_bfloat16 (*)[LAM_RS]>(lam_dyn + (size_t)LAM_TB * LAM_RS * 2);  // lo
   __nv_bfloat16 (*vt)[LAM_TB + 8] = reinterpret_cast<__nv_bfloat16 (*)[LAM_TB + 8]>(lam_dyn + (size_t)2 * LAM_TB * LAM_RS * 2);   // [e][token]; e = 8: ones
+  __nv_bfloat16 (*vtl)[LAM_TB + 8] = reinterpret_cast<__nv_bfloat16 (*)[LAM_TB + 8]>(lam_dyn + LAM_REDUCE_SMEM);   // V_LO: lo part
   const int chunk = blockIdx.x, h = blockIdx.y;
   const int64_t seq = blockIdx.z;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1537,6 +1595,8 @@ __global__ void __launch_bounds__(128) linattn_reduce_mma_kernel(const __nv_bflo
       for (int c = 0; c < 4; ++c) acc[a][b][c] = 0.f;
 #pragma unroll
   for (int e = LA_D + 1; e < 16; ++e) vt[e][tid] = __float2bfloat16_rn(0.f);      // padding rows of the B operand: written once
+  if (V_LO)
+    for (int e = LA_D; e < 16; ++e) vtl[e][tid] = __float2bfloat16_rn(0.f);       // the ones row is exact: its lo part is 0
   const int t_begin = chunk * LA_CHUNK, t_end = min(L, t_begin + LA_CHUNK);
   // ldmatrix row address of this lane inside a 16-token x 16-feature block: tile j = lane / 8 covers tokens (j & 2 ? 8 : 0) + r,
   // features (j & 1 ? 8 : 0) .. +7   ->   a[0], a[1], a[2], a[3] of the m16n8k16 A fragment (rows = features, k = tokens)
@@ -1548,14 +1608,14 @@ __global__ void __launch_bounds__(128) linattn_reduce_mma_kernel(const __nv_bflo
       const bool ok = tok < t_end;
       float kk[LA_D], vv[LA_D];
       if (ok) {
-        const __nv_bfloat16* row = kv + (seq * L + tok) * (2 * (int64_t)HD);
+        const T* row = kv + (seq * L + tok) * (2 * (int64_t)HD);
         const uint4 kr = *reinterpret_cast<const uint4*>(row + h * LA_D);
         const uint4 vr = *reinterpret_cast<const uint4*>(row + HD + h * LA_D);
-        const __nv_bfloat162* kb = reinterpret_cast<const __nv_bfloat162*>(&kr);
-        const __nv_bfloat162* vb = reinterpret_cast<const __nv_bfloat162*>(&vr);
+        const pair_t<T>* kb = reinterpret_cast<const pair_t<T>*>(&kr);
+        const pair_t<T>* vb = reinterpret_cast<const pair_t<T>*>(&vr);
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const float2 a = __bfloat1622float2(kb[q]), b = __bfloat1622float2(vb[q]);
+          const float2 a = pair_to_f2(kb[q]), b = pair_to_f2(vb[q]);
           kk[2 * q] = a.x; kk[2 * q + 1] = a.y; vv[2 * q] = b.x; vv[2 * q + 1] = b.y;
         }
       } else {
@@ -1569,7 +1629,7 @@ __global__ void __launch_bounds__(128) linattn_reduce_mma_kernel(const __nv_bflo
         const __nv_bfloat16 ah = __float2bfloat16_rn(a), bh = __float2bfloat16_rn(b);
         __nv_bfloat162 hi; hi.x = ah; hi.y = bh;
         fh[f >> 1] = *reinterpret_cast<uint32_t*>(&hi);
-        fl[f >> 1] = pack2_bf16(a - __bfloat162float(ah), b - __bfloat162float(bh));
+        fl[f >> 1] = pack2_16<__nv_bfloat16>(a - __bfloat162float(ah), b - __bfloat162float(bh));
       });
 #pragma unroll
       for (int v = 0; v < LAM_F / 8; ++v) {
@@ -1577,7 +1637,11 @@ __global__ void __launch_bounds__(128) linattn_reduce_mma_kernel(const __nv_bflo
         *reinterpret_cast<uint4*>(&phi_l[tid][v * 8]) = make_uint4(fl[4 * v], fl[4 * v + 1], fl[4 * v + 2], fl[4 * v + 3]);
       }
 #pragma unroll
-      for (int e = 0; e < LA_D; ++e) vt[e][tid] = __float2bfloat16_rn(vv[e]);
+      for (int e = 0; e < LA_D; ++e) {
+        const __nv_bfloat16 vh = __float2bfloat16_rn(vv[e]);
+        vt[e][tid] = vh;
+        if (V_LO) vtl[e][tid] = __float2bfloat16_rn(vv[e] - __bfloat162float(vh));
+      }
       vt[LA_D][tid] = __float2bfloat16_rn(ok ? 1.f : 0.f);
     }
     __syncthreads();
@@ -1585,21 +1649,29 @@ __global__ void __launch_bounds__(128) linattn_reduce_mma_kernel(const __nv_bflo
 #pragma unroll
     for (int ks = 0; ks < 2; ++ks) {
       const int n0 = warp * 32 + ks * 16;
-      uint32_t b[2][2];
+      uint32_t b[2][2], bl[2][2];
 #pragma unroll
       for (int nt = 0; nt < 2; ++nt) {
         b[nt][0] = *reinterpret_cast<const uint32_t*>(&vt[nt * 8 + g][n0 + t * 2]);
         b[nt][1] = *reinterpret_cast<const uint32_t*>(&vt[nt * 8 + g][n0 + 8 + t * 2]);
+        if (V_LO) {
+          bl[nt][0] = *reinterpret_cast<const uint32_t*>(&vtl[nt * 8 + g][n0 + t * 2]);
+          bl[nt][1] = *reinterpret_cast<const uint32_t*>(&vtl[nt * 8 + g][n0 + 8 + t * 2]);
+        }
       }
 #pragma unroll
       for (int mt = 0; mt < 5; ++mt) {
         uint32_t a[4];
         ldmatrix_x4_trans(a, &phi_s[n0 + lm_tok][mt * 16 + lm_feat]);
-        mma_bf16_16816(acc[mt][0], a, b[0][0], b[0][1]);
-        mma_bf16_16816(acc[mt][1], a, b[1][0], b[1][1]);
+        mma_16816<__nv_bfloat16>(acc[mt][0], a, b[0][0], b[0][1]);
+        mma_16816<__nv_bfloat16>(acc[mt][1], a, b[1][0], b[1][1]);
+        if (V_LO) {
+          mma_16816<__nv_bfloat16>(acc[mt][0], a, bl[0][0], bl[0][1]);
+          mma_16816<__nv_bfloat16>(acc[mt][1], a, bl[1][0], bl[1][1]);
+        }
         ldmatrix_x4_trans(a, &phi_l[n0 + lm_tok][mt * 16 + lm_feat]);
-        mma_bf16_16816(acc[mt][0], a, b[0][0], b[0][1]);
-        mma_bf16_16816(acc[mt][1], a, b[1][0], b[1][1]);
+        mma_16816<__nv_bfloat16>(acc[mt][0], a, b[0][0], b[0][1]);
+        mma_16816<__nv_bfloat16>(acc[mt][1], a, b[1][0], b[1][1]);
       }
     }
   }
@@ -1624,6 +1696,19 @@ __global__ void __launch_bounds__(128) linattn_reduce_mma_kernel(const __nv_bflo
     const int si = f * 16 + e;
     o[idx] = red[si] + red[LAM_F * 16 + si] + red[2 * LAM_F * 16 + si] + red[3 * LAM_F * 16 + si];
   }
+}
+// bf16 keeps the kernel's name; the fp16 form is its _f16_ twin
+__global__ void __launch_bounds__(128) linattn_reduce_mma_kernel(const __nv_bfloat16* __restrict__ kv, float* __restrict__ ws,
+                                                                 int L, int heads, int n_chunks) {
+  pdl_wait();
+  pdl_launch_dependents();
+  linattn_reduce_mma_body(kv, ws, L, heads, n_chunks);
+}
+__global__ void __launch_bounds__(128) linattn_reduce_mma_f16_kernel(const __half* __restrict__ kv, float* __restrict__ ws,
+                                                                     int L, int heads, int n_chunks) {
+  pdl_wait();
+  pdl_launch_dependents();
+  linattn_reduce_mma_body(kv, ws, L, heads, n_chunks);
 }
 
 constexpr int LAM_AT = 64;     // tokens per block in the apply kernel (2 warps x 32)
@@ -1651,10 +1736,10 @@ __global__ void __launch_bounds__(128) linattn_finalize_kernel(const float* __re
 }
 
 constexpr int LAM_AB = 4;      // 64-token sub-blocks per apply block: the 5.6 KB state operand is loaded once per 256 tokens
-__global__ void __launch_bounds__(64) linattn_apply_mma_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ sw,
-                                                               __nv_bfloat16* __restrict__ out, int L, int heads) {
-  pdl_wait();
-  pdl_launch_dependents();
+// T: element type of q and out (bf16 or fp16); the MMA operands are bf16 hi + lo pairs of fp32 values either way
+template <typename T>
+__device__ __forceinline__ void linattn_apply_mma_body(const T* __restrict__ q, const __nv_bfloat16* __restrict__ sw,
+                                                       T* __restrict__ out, int L, int heads) {
   // both operands are carried as bf16 hi + lo pairs (3 MMAs: hi*hi + lo*hi + hi*lo) -> ~fp32-level accuracy
   __shared__ __align__(16) __nv_bfloat16 phi_s[LAM_AT][LAM_F + 8];   // [token][feature] hi
   __shared__ __align__(16) __nv_bfloat16 phi_l[LAM_AT][LAM_F + 8];   // lo
@@ -1682,11 +1767,11 @@ __global__ void __launch_bounds__(64) linattn_apply_mma_kernel(const __nv_bfloat
       float qq[LA_D];
       if (ok) {
         const uint4 qr = *reinterpret_cast<const uint4*>(q + (seq * L + tok) * HD + h * LA_D);
-        const __nv_bfloat162* qb = reinterpret_cast<const __nv_bfloat162*>(&qr);
+        const pair_t<T>* qb = reinterpret_cast<const pair_t<T>*>(&qr);
         const float qs = rsqrtf((float)LA_D);
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          const float2 a = __bfloat1622float2(qb[i]);
+          const float2 a = pair_to_f2(qb[i]);
           qq[2 * i] = a.x * qs; qq[2 * i + 1] = a.y * qs;
         }
       } else {
@@ -1701,7 +1786,7 @@ __global__ void __launch_bounds__(64) linattn_apply_mma_kernel(const __nv_bfloat
         const __nv_bfloat16 ah = __float2bfloat16_rn(a), bh = __float2bfloat16_rn(b);
         __nv_bfloat162 hi; hi.x = ah; hi.y = bh;
         fh[f >> 1] = *reinterpret_cast<uint32_t*>(&hi);
-        fl[f >> 1] = pack2_bf16(a - __bfloat162float(ah), b - __bfloat162float(bh));
+        fl[f >> 1] = pack2_16<__nv_bfloat16>(a - __bfloat162float(ah), b - __bfloat162float(bh));
       });
 #pragma unroll
       for (int v = 0; v < LAM_F / 8; ++v) {
@@ -1735,19 +1820,31 @@ __global__ void __launch_bounds__(64) linattn_apply_mma_kernel(const __nv_bfloat
           const uint32_t bh1 = *reinterpret_cast<const uint32_t*>(&st[nt * 8 + g][ks * 16 + 8 + t * 2]);
           const uint32_t bl0 = *reinterpret_cast<const uint32_t*>(&sl[nt * 8 + g][ks * 16 + t * 2]);
           const uint32_t bl1 = *reinterpret_cast<const uint32_t*>(&sl[nt * 8 + g][ks * 16 + 8 + t * 2]);
-          mma_bf16_16816(c[nt], ah, bh0, bh1);
-          mma_bf16_16816(c[nt], al, bh0, bh1);
-          mma_bf16_16816(c[nt], ah, bl0, bl1);
+          mma_16816<__nv_bfloat16>(c[nt], ah, bh0, bh1);
+          mma_16816<__nv_bfloat16>(c[nt], al, bh0, bh1);
+          mma_16816<__nv_bfloat16>(c[nt], ah, bl0, bl1);
         }
       }
       // denominator = column 8 = c[1][0] (row g) / c[1][2] (row g+8) of the quad's t == 0 lane
       const float d0 = fmaxf(__shfl_sync(0xffffffffu, c[1][0], lane & ~3), 1e-5f);
       const float d1 = fmaxf(__shfl_sync(0xffffffffu, c[1][2], lane & ~3), 1e-5f);
       const int r0 = blk * LAM_AT + n0 + g, r1 = r0 + 8;
-      if (r0 < L) *reinterpret_cast<uint32_t*>(out + (seq * L + r0) * HD + h * LA_D + t * 2) = pack2_bf16(c[0][0] / d0, c[0][1] / d0);
-      if (r1 < L) *reinterpret_cast<uint32_t*>(out + (seq * L + r1) * HD + h * LA_D + t * 2) = pack2_bf16(c[0][2] / d1, c[0][3] / d1);
+      if (r0 < L) *reinterpret_cast<uint32_t*>(out + (seq * L + r0) * HD + h * LA_D + t * 2) = pack2_16<T>(c[0][0] / d0, c[0][1] / d0);
+      if (r1 < L) *reinterpret_cast<uint32_t*>(out + (seq * L + r1) * HD + h * LA_D + t * 2) = pack2_16<T>(c[0][2] / d1, c[0][3] / d1);
     }
   }
+}
+__global__ void __launch_bounds__(64) linattn_apply_mma_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ sw,
+                                                               __nv_bfloat16* __restrict__ out, int L, int heads) {
+  pdl_wait();
+  pdl_launch_dependents();
+  linattn_apply_mma_body(q, sw, out, L, heads);
+}
+__global__ void __launch_bounds__(64) linattn_apply_mma_f16_kernel(const __half* __restrict__ q, const __nv_bfloat16* __restrict__ sw,
+                                                                   __half* __restrict__ out, int L, int heads) {
+  pdl_wait();
+  pdl_launch_dependents();
+  linattn_apply_mma_body(q, sw, out, L, heads);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2501,6 +2598,29 @@ static int launch_attention(const mv2_attn_args* a, const AttnDrop* d, cudaStrea
   return MV2_OK;
 }
 
+// kernel choice of the 16-bit dtypes (T = __nv_bfloat16 or __half)
+template <typename T>
+static int attention_dispatch16(const mv2_attn_args* a, const AttnDrop* d, cudaStream_t st) {
+  if (!a->causal && a->L >= 64 && (a->dim_head == 32 || a->dim_head == 64) && a->heads * a->dim_head % 8 == 0) {
+    dim3 grid((unsigned)((int64_t)a->n_outer * a->n_inner), a->heads, ceil_div(a->L, FA_Q));
+    using K = AttnK16<T>;
+    if (a->dim_head == 32) launch_attn_k(K::template mma<32>(), K::template mma_drop<32>(), grid, dim3(256), st, a, d);
+    else launch_attn_k(K::template mma<64>(), K::template mma_drop<64>(), grid, dim3(256), st, a, d);
+    MV2_CHECK_LAUNCH();
+    return MV2_OK;
+  }
+  if (a->L <= AS_L && a->n_mem <= AS_M && (a->dim_head == 32 || a->dim_head == 64)) {
+    const int64_t warps = (int64_t)a->n_outer * a->n_inner * a->heads;
+    const dim3 grid((unsigned)ceil_div(warps, 8));
+    using K = AttnK16<T>;
+    if (a->dim_head == 32) launch_attn_k(K::template small<1>(), K::template small_drop<1>(), grid, dim3(256), st, a, d);
+    else launch_attn_k(K::template small<2>(), K::template small_drop<2>(), grid, dim3(256), st, a, d);
+    MV2_CHECK_LAUNCH();
+    return MV2_OK;
+  }
+  return launch_attention<T>(a, d, st);
+}
+
 // mv2_attention's argument checks and kernel choice; d != NULL launches the dropout twins
 static int attention_dispatch(const mv2_attn_args* a, const AttnDrop* d, void* stream) {
   MV2_CHECK_ARG(a && a->qkv && a->out && a->mem_kv);
@@ -2509,22 +2629,8 @@ static int attention_dispatch(const mv2_attn_args* a, const AttnDrop* d, void* s
   MV2_CHECK_ARG((int64_t)a->n_outer * a->n_inner <= 2147483647LL && ceil_div(a->L, AT_Q) <= 65535);
   cudaStream_t st = (cudaStream_t)stream;
   if (a->dtype == MV2_F32) return launch_attention<float>(a, d, st);
-  if (a->dtype == MV2_BF16 && !a->causal && a->L >= 64 && (a->dim_head == 32 || a->dim_head == 64) && a->heads * a->dim_head % 8 == 0) {
-    dim3 grid((unsigned)((int64_t)a->n_outer * a->n_inner), a->heads, ceil_div(a->L, FA_Q));
-    if (a->dim_head == 32) launch_attn_k(attention_mma_kernel<32>, attention_mma_dropout_kernel<32>, grid, dim3(256), st, a, d);
-    else launch_attn_k(attention_mma_kernel<64>, attention_mma_dropout_kernel<64>, grid, dim3(256), st, a, d);
-    MV2_CHECK_LAUNCH();
-    return MV2_OK;
-  }
-  if (a->dtype == MV2_BF16 && a->L <= AS_L && a->n_mem <= AS_M && (a->dim_head == 32 || a->dim_head == 64)) {
-    const int64_t warps = (int64_t)a->n_outer * a->n_inner * a->heads;
-    const dim3 grid((unsigned)ceil_div(warps, 8));
-    if (a->dim_head == 32) launch_attn_k(attention_small_kernel<1>, attention_small_dropout_kernel<1>, grid, dim3(256), st, a, d);
-    else launch_attn_k(attention_small_kernel<2>, attention_small_dropout_kernel<2>, grid, dim3(256), st, a, d);
-    MV2_CHECK_LAUNCH();
-    return MV2_OK;
-  }
-  if (a->dtype == MV2_BF16) return launch_attention<__nv_bfloat16>(a, d, st);
+  if (a->dtype == MV2_BF16) return attention_dispatch16<__nv_bfloat16>(a, d, st);
+  if (a->dtype == MV2_F16) return attention_dispatch16<__half>(a, d, st);
   set_error("bad dtype %d", a->dtype);
   return MV2_E_ARG;
 }
@@ -2555,6 +2661,9 @@ static int launch_quant_forward(const void* x, int dtype, int64_t N, int C, int 
   else if (dtype == MV2_BF16)
     launch_k(quant_forward_kernel<__nv_bfloat16, MODE, MAXD>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, N, C, d, nc, win,
              bin, wout, bout, clamp, spherical, lv, idx64, idx32, (__nv_bfloat16*)quantized, aux);
+  else if (dtype == MV2_F16)
+    launch_k(quant_forward_kernel<__half, MODE, MAXD>, dim3(blocks), dim3(256), 0, st, (const __half*)x, N, C, d, nc, win,
+             bin, wout, bout, clamp, spherical, lv, idx64, idx32, (__half*)quantized, aux);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -2572,6 +2681,9 @@ static int launch_quant_decode(const void* indices, int is64, int64_t N, int C, 
   else if (dtype == MV2_BF16)
     launch_k(quant_decode_kernel<__nv_bfloat16, MODE, MAXD>, dim3(blocks), dim3(256), 0, st, indices, is64, N, C, d, nc, lv, wout, bout,
              (__nv_bfloat16*)quantized);
+  else if (dtype == MV2_F16)
+    launch_k(quant_decode_kernel<__half, MODE, MAXD>, dim3(blocks), dim3(256), 0, st, indices, is64, N, C, d, nc, lv, wout, bout,
+             (__half*)quantized);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -2626,11 +2738,13 @@ int mv2_ingest_kwpack(const void* src, int src_dtype, void* dst, int B, int C, i
   const int blocks = (int)rows;
   cudaStream_t st = (cudaStream_t)stream;
   if (src_dtype == MV2_F32)
-    launch_k(ingest_kwpack_kernel<float>, dim3(blocks), dim3(256), smem, st, (const float*)src, (__nv_bfloat16*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
+    launch_k(ingest_kwpack_kernel<float, __nv_bfloat16>, dim3(blocks), dim3(256), smem, st, (const float*)src, (__nv_bfloat16*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
   else if (src_dtype == MV2_BF16)
-    launch_k(ingest_kwpack_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), smem, st, (const __nv_bfloat16*)src, (__nv_bfloat16*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
+    launch_k(ingest_kwpack_kernel<__nv_bfloat16, __nv_bfloat16>, dim3(blocks), dim3(256), smem, st, (const __nv_bfloat16*)src, (__nv_bfloat16*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
+  else if (src_dtype == MV2_F16)
+    launch_k(ingest_kwpack_kernel<__half, __half>, dim3(blocks), dim3(256), smem, st, (const __half*)src, (__half*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
   else if (src_dtype == MV2_U8)
-    launch_k(ingest_kwpack_kernel<uint8_t>, dim3(blocks), dim3(256), smem, st, (const uint8_t*)src, (__nv_bfloat16*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
+    launch_k(ingest_kwpack_kernel<uint8_t, __nv_bfloat16>, dim3(blocks), dim3(256), smem, st, (const uint8_t*)src, (__nv_bfloat16*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
   else { set_error("bad dtype %d", src_dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -2650,6 +2764,7 @@ int mv2_conv_forward(const mv2_conv_args* a, const mv2_conv_hist* hist, void* st
   cudaStream_t st = (cudaStream_t)stream;
   if (a->dtype == MV2_F32) launch_k(conv_simt_kernel<float>, dim3(grid), dim3(256), 0, st, *a, *hist);
   else if (a->dtype == MV2_BF16) launch_k(conv_simt_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, *a, *hist);
+  else if (a->dtype == MV2_F16) launch_k(conv_simt_kernel<__half>, dim3(grid), dim3(256), 0, st, *a, *hist);
   else { set_error("bad dtype %d", a->dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -2673,7 +2788,7 @@ static int se_online_vec(int C) {
 static int se_rows_per_block(int dtype, int F, int P, int C) {
   (void)F;   // deliberately NOT a function of the frame count: the chunking fixes the summation order of the pooled vector, and
              // a clip's tokens must not depend on how many other clips share its batch (tests: ..._batch_independence)
-  if (!(dtype == MV2_BF16 && se_online_vec(C) != 0)) return SE_CHUNK;
+  if (!((dtype == MV2_BF16 || dtype == MV2_F16) && se_online_vec(C) != 0)) return SE_CHUNK;
   // small (L2-resident) frames take 64 - 128-row chunks: fewer, longer bulk-copy pipelines and fewer records to merge than
   // 32-row chunks; large frames amortise the per-block merge over longer chunks
   if (P <= 256) return 64;
@@ -2687,12 +2802,42 @@ static cudaError_t se_pool_smem_optin() {
   return once.run([] {
     cudaError_t err = cudaSuccess;
     auto set = [&](const void* fn) { if (err == cudaSuccess) err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024); };
-    set((const void*)se_pool_online_kernel<8, 1>); set((const void*)se_pool_online_kernel<8, 2>); set((const void*)se_pool_online_kernel<8, 4>);
-    set((const void*)se_pool_online_kernel<8, 8>); set((const void*)se_pool_online_kernel<8, 16>); set((const void*)se_pool_online_kernel<8, 32>);
-    set((const void*)se_pool_online_kernel<16, 32>); set((const void*)se_pool_online_kernel<32, 32>);
+    auto set_all = [&](auto tag) {
+      using T = decltype(tag);
+      set((const void*)se_pool_online_kernel<T, 8, 1>); set((const void*)se_pool_online_kernel<T, 8, 2>); set((const void*)se_pool_online_kernel<T, 8, 4>);
+      set((const void*)se_pool_online_kernel<T, 8, 8>); set((const void*)se_pool_online_kernel<T, 8, 16>); set((const void*)se_pool_online_kernel<T, 8, 32>);
+      set((const void*)se_pool_online_kernel<T, 16, 32>); set((const void*)se_pool_online_kernel<T, 32, 32>);
+    };
+    set_all(__nv_bfloat16());
+    set_all(__half());
     return err;
   });
 }
+
+extern "C++" {
+// the single-pass kernel of a 16-bit y (T = __nv_bfloat16 or __half)
+template <typename T>
+static int se_pool_online_launch(const void* y, int P, int C, const float* wk, float bk, void* workspace, dim3 grid, int nc,
+                                 int rows, cudaStream_t st) {
+  const int vec = se_online_vec(C);
+  const int R_ = 256 / (C / vec), U_ = vec == 8 ? 4 : 2;
+  // SE_STAGES batches of R * U rows, reused afterwards for R records of (m, s, acc[C]) + R merge coefficients
+  const size_t dsm = std::max((size_t)SE_STAGES * R_ * U_ * C * 2, (size_t)R_ * (C + 3) * sizeof(float));
+  if (dsm > 96 * 1024) { set_error("se_pool: C = %d needs %zu bytes of shared memory", C, dsm); return MV2_E_ARG; }
+  const T* yb = (const T*)y;
+  if (const cudaError_t e = se_pool_smem_optin()) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(e)); return MV2_E_CUDA; }
+  const int G_ = C / vec;
+#define MV2_SE_POOL_CASE(V, GG) \
+  else if (vec == V && G_ == GG) launch_k(se_pool_online_kernel<T, V, GG>, dim3(grid), dim3(256), dsm, st, yb, P, C, wk, bk, (float*)workspace, nc, rows)
+  if (false) {}
+  MV2_SE_POOL_CASE(8, 1); MV2_SE_POOL_CASE(8, 2); MV2_SE_POOL_CASE(8, 4); MV2_SE_POOL_CASE(8, 8); MV2_SE_POOL_CASE(8, 16);
+  MV2_SE_POOL_CASE(8, 32); MV2_SE_POOL_CASE(16, 32); MV2_SE_POOL_CASE(32, 32);
+  else { set_error("se_pool: no kernel for C = %d", C); return MV2_E_UNSUPPORTED; }
+#undef MV2_SE_POOL_CASE
+  MV2_CHECK_LAUNCH();
+  return MV2_OK;
+}
+}  // extern "C++"
 
 int mv2_se_pool(const void* y, int dtype, int F, int P, int C, const float* wk, float bk, void* workspace,
                 void* stream) {
@@ -2702,23 +2847,11 @@ int mv2_se_pool(const void* y, int dtype, int F, int P, int C, const float* wk, 
   dim3 grid(nc, F);
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32) launch_k(se_pool_kernel<float>, dim3(grid), dim3(256), 0, st, (const float*)y, P, C, wk, bk, (float*)workspace, nc);
-  else if (dtype == MV2_BF16 && se_online_vec(C) != 0) {
-    const int vec = se_online_vec(C);
-    const int R_ = 256 / (C / vec), U_ = vec == 8 ? 4 : 2;
-    // SE_STAGES batches of R * U rows, reused afterwards for R records of (m, s, acc[C]) + R merge coefficients
-    const size_t dsm = std::max((size_t)SE_STAGES * R_ * U_ * C * 2, (size_t)R_ * (C + 3) * sizeof(float));
-    MV2_CHECK_ARG(dsm <= 96 * 1024);
-    const __nv_bfloat16* yb = (const __nv_bfloat16*)y;
-    MV2_CHECK_CUDA(se_pool_smem_optin());
-    const int G_ = C / vec;
-#define MV2_SE_POOL_CASE(V, GG) \
-    else if (vec == V && G_ == GG) launch_k(se_pool_online_kernel<V, GG>, dim3(grid), dim3(256), dsm, st, yb, P, C, wk, bk, (float*)workspace, nc, rows)
-    if (false) {}
-    MV2_SE_POOL_CASE(8, 1); MV2_SE_POOL_CASE(8, 2); MV2_SE_POOL_CASE(8, 4); MV2_SE_POOL_CASE(8, 8); MV2_SE_POOL_CASE(8, 16);
-    MV2_SE_POOL_CASE(8, 32); MV2_SE_POOL_CASE(16, 32); MV2_SE_POOL_CASE(32, 32);
-    else { set_error("se_pool: no kernel for C = %d", C); return MV2_E_UNSUPPORTED; }
-#undef MV2_SE_POOL_CASE
-  } else if (dtype == MV2_BF16) launch_k(se_pool_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, (const __nv_bfloat16*)y, P, C, wk, bk, (float*)workspace, nc);
+  else if ((dtype == MV2_BF16 || dtype == MV2_F16) && se_online_vec(C) != 0)
+    return dtype == MV2_F16 ? se_pool_online_launch<__half>(y, P, C, wk, bk, workspace, grid, nc, rows, st)
+                            : se_pool_online_launch<__nv_bfloat16>(y, P, C, wk, bk, workspace, grid, nc, rows, st);
+  else if (dtype == MV2_BF16) launch_k(se_pool_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, (const __nv_bfloat16*)y, P, C, wk, bk, (float*)workspace, nc);
+  else if (dtype == MV2_F16) launch_k(se_pool_kernel<__half>, dim3(grid), dim3(256), 0, st, (const __half*)y, P, C, wk, bk, (float*)workspace, nc);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -2782,6 +2915,7 @@ int mv2_scale_channels(const void* x, const float* scale, void* out, int dtype, 
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32) launch_k(scale_channels_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)x, scale, (float*)out, total, per_clip, C);
   else if (dtype == MV2_BF16) launch_k(scale_channels_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, scale, (__nv_bfloat16*)out, total, per_clip, C);
+  else if (dtype == MV2_F16) launch_k(scale_channels_kernel<__half>, dim3(blocks), dim3(256), 0, st, (const __half*)x, scale, (__half*)out, total, per_clip, C);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -2811,6 +2945,7 @@ int mv2_pad_cl(const void* src, void* dst, int dtype, int B, int T, int H, int W
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32) launch_k(pad_cl_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)src, (float*)dst, B, T, H, W, C, pt, ph, pw, mode);
   else if (dtype == MV2_BF16) launch_k(pad_cl_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)src, (__nv_bfloat16*)dst, B, T, H, W, C, pt, ph, pw, mode);
+  else if (dtype == MV2_F16) launch_k(pad_cl_kernel<__half>, dim3(blocks), dim3(256), 0, st, (const __half*)src, (__half*)dst, B, T, H, W, C, pt, ph, pw, mode);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -2824,16 +2959,34 @@ int mv2_gate_residual(const void* y, const void* x, const float* gates, void* ou
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32)
     launch_k(gate_residual_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)y, (const float*)x, gates, (float*)out, total, (int64_t)P * C, C);
-  else if (dtype == MV2_BF16 && C % 8 == 0) {
+  else if ((dtype == MV2_BF16 || dtype == MV2_F16) && C % 8 == 0) {
     const int64_t total8 = total / 8;
     const int b8 = (int)std::min<int64_t>((total8 + 255) / 256, grid_cap(16));
-    launch_k(gate_residual_bf16x8_kernel, dim3(b8), dim3(256), 0, st, (const uint4*)y, (const uint4*)x, gates, (uint4*)out, total8, (int64_t)P * C / 8, C / 8);
+    launch_k(dtype == MV2_F16 ? gate_residual_x8_kernel<__half> : gate_residual_x8_kernel<__nv_bfloat16>, dim3(b8), dim3(256), 0, st,
+             (const uint4*)y, (const uint4*)x, gates, (uint4*)out, total8, (int64_t)P * C / 8, C / 8);
   } else if (dtype == MV2_BF16)
     launch_k(gate_residual_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)y, (const __nv_bfloat16*)x, gates, (__nv_bfloat16*)out, total, (int64_t)P * C, C);
+  else if (dtype == MV2_F16)
+    launch_k(gate_residual_kernel<__half>, dim3(blocks), dim3(256), 0, st, (const __half*)y, (const __half*)x, gates, (__half*)out, total, (int64_t)P * C, C);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }
+
+extern "C++" {
+// the one-warp-per-token kernel of a 16-bit x (T = __nv_bfloat16 or __half), C % 8 == 0, C <= 1024
+template <typename T>
+static void rmsnorm_x8_launch(const void* x, void* out, const float* gamma, int64_t n_tok, int Tn, int P, int C, int token_shift,
+                              const void* prev, int64_t prev_stride, cudaStream_t st) {
+  const T* xb = (const T*)x;
+  T* ob = (T*)out;
+  const T* pb = (const T*)prev;
+  // one token per warp up to C = 512 keeps the most warps in flight on the small README shapes; the widest rows take 4
+  if (C <= 256) launch_k(rmsnorm_x8_kernel<T, 1, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, Tn, P, C, token_shift, pb, prev_stride);
+  else if (C <= 512) launch_k(rmsnorm_x8_kernel<T, 2, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, Tn, P, C, token_shift, pb, prev_stride);
+  else launch_k(rmsnorm_x8_kernel<T, 4, 4>, dim3(ceil_div(n_tok, 8 * 4)), dim3(256), 0, st, xb, ob, gamma, n_tok, Tn, P, C, token_shift, pb, prev_stride);
+}
+}  // extern "C++"
 
 static int rmsnorm_launch(const void* x, void* out, int dtype, const float* gamma, int B, int T, int P, int C, int token_shift,
                           const void* prev, int64_t prev_stride, void* stream) {
@@ -2843,17 +2996,14 @@ static int rmsnorm_launch(const void* x, void* out, int dtype, const float* gamm
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32)
     launch_k(rmsnorm_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)x, (float*)out, gamma, n_tok, T, P, C, token_shift, (const float*)prev, prev_stride);
-  else if (dtype == MV2_BF16 && C % 8 == 0 && C <= 1024 && (!token_shift || (C / 2) % 8 == 0))
-    {
-      const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
-      __nv_bfloat16* ob = (__nv_bfloat16*)out;
-      // one token per warp up to C = 512 keeps the most warps in flight on the small README shapes; the widest rows take 4
-      if (C <= 256) launch_k(rmsnorm_bf16x8_kernel<1, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift, (const __nv_bfloat16*)prev, prev_stride);
-      else if (C <= 512) launch_k(rmsnorm_bf16x8_kernel<2, 1>, dim3(ceil_div(n_tok, 8 * 1)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift, (const __nv_bfloat16*)prev, prev_stride);
-      else launch_k(rmsnorm_bf16x8_kernel<4, 4>, dim3(ceil_div(n_tok, 8 * 4)), dim3(256), 0, st, xb, ob, gamma, n_tok, T, P, C, token_shift, (const __nv_bfloat16*)prev, prev_stride);
-    }
+  else if ((dtype == MV2_BF16 || dtype == MV2_F16) && C % 8 == 0 && C <= 1024 && (!token_shift || (C / 2) % 8 == 0)) {
+    if (dtype == MV2_F16) rmsnorm_x8_launch<__half>(x, out, gamma, n_tok, T, P, C, token_shift, prev, prev_stride, st);
+    else rmsnorm_x8_launch<__nv_bfloat16>(x, out, gamma, n_tok, T, P, C, token_shift, prev, prev_stride, st);
+  }
   else if (dtype == MV2_BF16)
     launch_k(rmsnorm_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)x, (__nv_bfloat16*)out, gamma, n_tok, T, P, C, token_shift, (const __nv_bfloat16*)prev, prev_stride);
+  else if (dtype == MV2_F16)
+    launch_k(rmsnorm_kernel<__half>, dim3(blocks), dim3(256), 0, st, (const __half*)x, (__half*)out, gamma, n_tok, T, P, C, token_shift, (const __half*)prev, prev_stride);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -2884,17 +3034,24 @@ int mv2_attention_tail(const mv2_attn_args* a, const void* q, int64_t q_outer_st
   o.out = out;
   cudaStream_t st = (cudaStream_t)stream;
   const int dpl = a->dim_head / 32;
-  if (a->dtype == MV2_BF16 && a->L <= AS_L && a->n_mem <= AS_M && (dpl == 1 || dpl == 2)) {
-    const dim3 grid((unsigned)ceil_div((int64_t)a->n_outer * a->n_inner * a->heads, 8));
-    if (dpl == 1) launch_k(attention_small_tail_kernel<1>, grid, dim3(256), 0, st, o, tl);
-    else launch_k(attention_small_tail_kernel<2>, grid, dim3(256), 0, st, o, tl);
-  } else if (a->dtype == MV2_F32 || a->dtype == MV2_BF16) {
-    const dim3 grid((unsigned)((int64_t)a->n_outer * a->n_inner), a->heads, ceil_div(a->L - q_begin, AT_Q));
-    const bool f32 = a->dtype == MV2_F32;
-    if (dpl == 1) f32 ? launch_k(attention_tail_kernel<float, 1>, grid, dim3(128), 0, st, o, tl) : launch_k(attention_tail_kernel<__nv_bfloat16, 1>, grid, dim3(128), 0, st, o, tl);
-    else if (dpl == 2) f32 ? launch_k(attention_tail_kernel<float, 2>, grid, dim3(128), 0, st, o, tl) : launch_k(attention_tail_kernel<__nv_bfloat16, 2>, grid, dim3(128), 0, st, o, tl);
-    else f32 ? launch_k(attention_tail_kernel<float, 3>, grid, dim3(128), 0, st, o, tl) : launch_k(attention_tail_kernel<__nv_bfloat16, 3>, grid, dim3(128), 0, st, o, tl);
-  } else { set_error("bad dtype %d", a->dtype); return MV2_E_ARG; }
+  if (a->dtype != MV2_F32 && a->dtype != MV2_BF16 && a->dtype != MV2_F16) { set_error("bad dtype %d", a->dtype); return MV2_E_ARG; }
+  auto go = [&](auto tag) {
+    using T = decltype(tag);
+    if (!std::is_same<T, float>::value && a->L <= AS_L && a->n_mem <= AS_M && (dpl == 1 || dpl == 2)) {
+      using T16 = typename std::conditional<std::is_same<T, float>::value, __nv_bfloat16, T>::type;
+      const dim3 grid((unsigned)ceil_div((int64_t)a->n_outer * a->n_inner * a->heads, 8));
+      if (dpl == 1) launch_k(AttnK16<T16>::template small_tail<1>(), grid, dim3(256), 0, st, o, tl);
+      else launch_k(AttnK16<T16>::template small_tail<2>(), grid, dim3(256), 0, st, o, tl);
+    } else {
+      const dim3 grid((unsigned)((int64_t)a->n_outer * a->n_inner), a->heads, ceil_div(a->L - q_begin, AT_Q));
+      if (dpl == 1) launch_k(attention_tail_kernel<T, 1>, grid, dim3(128), 0, st, o, tl);
+      else if (dpl == 2) launch_k(attention_tail_kernel<T, 2>, grid, dim3(128), 0, st, o, tl);
+      else launch_k(attention_tail_kernel<T, 3>, grid, dim3(128), 0, st, o, tl);
+    }
+  };
+  if (a->dtype == MV2_F32) go(float());
+  else if (a->dtype == MV2_BF16) go(__nv_bfloat16());
+  else go(__half());
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }
@@ -2937,24 +3094,39 @@ int mv2_linear_attention(const void* q, const void* kv, void* out, int dtype, in
     launch_k(linattn_reduce_kernel<float>, dim3(grid), dim3(256), 0, st, (const float*)kv, (float*)workspace, L, heads, nc);
     MV2_CHECK_LAUNCH();
     launch_k(linattn_apply_kernel<float>, dim3(grid), dim3(64), 0, st, (const float*)q, (const float*)workspace, (float*)out, L, heads, nc);
-  } else if (dtype == MV2_BF16 && (heads * LA_D) % 8 == 0) {
+  } else if ((dtype == MV2_BF16 || dtype == MV2_F16) && (heads * LA_D) % 8 == 0) {
+    const bool f16 = dtype == MV2_F16;
     {
       static PerDeviceOnce once;
-      MV2_CHECK_CUDA(once.run([] { return cudaFuncSetAttribute(linattn_reduce_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAM_REDUCE_SMEM); }));
+      MV2_CHECK_CUDA(once.run([] {
+        cudaError_t e = cudaFuncSetAttribute(linattn_reduce_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAM_REDUCE_SMEM);
+        if (e == cudaSuccess)
+          e = cudaFuncSetAttribute(linattn_reduce_mma_f16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LAM_REDUCE_SMEM_F16);
+        return e;
+      }));
     }
-    launch_k(linattn_reduce_mma_kernel, dim3(grid), dim3(128), LAM_REDUCE_SMEM, st, (const __nv_bfloat16*)kv, (float*)workspace, L, heads, nc);
-    MV2_CHECK_LAUNCH();
+    if (f16)
+      launch_k(linattn_reduce_mma_f16_kernel, dim3(grid), dim3(128), LAM_REDUCE_SMEM_F16, st, (const __half*)kv, (float*)workspace, L, heads, nc);
+    else
+      launch_k(linattn_reduce_mma_kernel, dim3(grid), dim3(128), LAM_REDUCE_SMEM, st, (const __nv_bfloat16*)kv, (float*)workspace, L, heads, nc);
     MV2_CHECK_LAUNCH();
     const size_t part_bytes = ((size_t)n_seq * heads * nc * LA_ST * sizeof(float) + 15) / 16 * 16;
     __nv_bfloat16* sw = reinterpret_cast<__nv_bfloat16*>((char*)workspace + part_bytes);
     launch_k(linattn_finalize_kernel, dim3(heads, n_seq), dim3(128), 0, st, (const float*)workspace, sw, heads, nc);
     MV2_CHECK_LAUNCH();
     dim3 grid2(ceil_div(L, LAM_AT * LAM_AB), heads, n_seq);
-    launch_k(linattn_apply_mma_kernel, dim3(grid2), dim3(64), 0, st, (const __nv_bfloat16*)q, (const __nv_bfloat16*)sw, (__nv_bfloat16*)out, L, heads);
+    if (f16)
+      launch_k(linattn_apply_mma_f16_kernel, dim3(grid2), dim3(64), 0, st, (const __half*)q, (const __nv_bfloat16*)sw, (__half*)out, L, heads);
+    else
+      launch_k(linattn_apply_mma_kernel, dim3(grid2), dim3(64), 0, st, (const __nv_bfloat16*)q, (const __nv_bfloat16*)sw, (__nv_bfloat16*)out, L, heads);
   } else if (dtype == MV2_BF16) {
     launch_k(linattn_reduce_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, (const __nv_bfloat16*)kv, (float*)workspace, L, heads, nc);
     MV2_CHECK_LAUNCH();
     launch_k(linattn_apply_kernel<__nv_bfloat16>, dim3(grid), dim3(64), 0, st, (const __nv_bfloat16*)q, (const float*)workspace, (__nv_bfloat16*)out, L, heads, nc);
+  } else if (dtype == MV2_F16) {
+    launch_k(linattn_reduce_kernel<__half>, dim3(grid), dim3(256), 0, st, (const __half*)kv, (float*)workspace, L, heads, nc);
+    MV2_CHECK_LAUNCH();
+    launch_k(linattn_apply_kernel<__half>, dim3(grid), dim3(64), 0, st, (const __half*)q, (const float*)workspace, (__half*)out, L, heads, nc);
   } else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -2967,6 +3139,7 @@ int mv2_geglu(const void* in, void* out, int dtype, int64_t N, int I, void* stre
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == MV2_F32) launch_k(geglu_kernel<float>, dim3(blocks), dim3(256), 0, st, (const float*)in, (float*)out, N, I);
   else if (dtype == MV2_BF16) launch_k(geglu_kernel<__nv_bfloat16>, dim3(blocks), dim3(256), 0, st, (const __nv_bfloat16*)in, (__nv_bfloat16*)out, N, I);
+  else if (dtype == MV2_F16) launch_k(geglu_kernel<__half>, dim3(blocks), dim3(256), 0, st, (const __half*)in, (__half*)out, N, I);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -3084,6 +3257,8 @@ int mv2_mse(const void* a, int a_dtype, const void* b, int b_dtype, int64_t n, v
   MV2_MSE_CASE(MV2_F32, float, MV2_F32, float); MV2_MSE_CASE(MV2_F32, float, MV2_BF16, __nv_bfloat16);
   MV2_MSE_CASE(MV2_BF16, __nv_bfloat16, MV2_F32, float); MV2_MSE_CASE(MV2_BF16, __nv_bfloat16, MV2_BF16, __nv_bfloat16);
   MV2_MSE_CASE(MV2_U8, uint8_t, MV2_F32, float); MV2_MSE_CASE(MV2_U8, uint8_t, MV2_BF16, __nv_bfloat16);
+  MV2_MSE_CASE(MV2_F32, float, MV2_F16, __half); MV2_MSE_CASE(MV2_F16, __half, MV2_F32, float);
+  MV2_MSE_CASE(MV2_F16, __half, MV2_F16, __half); MV2_MSE_CASE(MV2_U8, uint8_t, MV2_F16, __half);
   else { set_error("mse: unsupported dtype pair %d, %d", a_dtype, b_dtype); return MV2_E_ARG; }
 #undef MV2_MSE_CASE
   MV2_CHECK_LAUNCH();
@@ -3124,6 +3299,8 @@ int mv2_gateloop_scan_state(const void* qkva, const void* res, void* out, int dt
     launch_k(gateloop_scan_kernel<float>, dim3((unsigned)blocks), dim3(256), 0, st, (const float*)qkva, (const float*)res, (float*)out, T, (int64_t)P * C, C, total, state);
   else if (dtype == MV2_BF16)
     launch_k(gateloop_scan_kernel<__nv_bfloat16>, dim3((unsigned)blocks), dim3(256), 0, st, (const __nv_bfloat16*)qkva, (const __nv_bfloat16*)res, (__nv_bfloat16*)out, T, (int64_t)P * C, C, total, state);
+  else if (dtype == MV2_F16)
+    launch_k(gateloop_scan_kernel<__half>, dim3((unsigned)blocks), dim3(256), 0, st, (const __half*)qkva, (const __half*)res, (__half*)out, T, (int64_t)P * C, C, total, state);
   else { set_error("bad dtype %d", dtype); return MV2_E_ARG; }
   MV2_CHECK_LAUNCH();
   return MV2_OK;

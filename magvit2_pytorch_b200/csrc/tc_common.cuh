@@ -4,6 +4,7 @@
 #include "common.cuh"
 #include <cuda.h>
 #include <mutex>
+#include <type_traits>
 
 namespace mv2 {
 
@@ -63,7 +64,7 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-// ---- wgmma (sm_90a warpgroup MMA): D[regs] (+)= A[smem] * B[smem], bf16 in, fp32 accumulate ----
+// ---- wgmma (sm_90a warpgroup MMA): D[regs] (+)= A[smem] * B[smem], bf16 or fp16 in, fp32 accumulate ----
 // Every wgmma instruction is issued by all 128 threads of a warpgroup; the 64 x N fp32 accumulator lives in their
 // registers (m64nNk16 fragment: thread t holds rows 16 (t / 32) + (t % 32) / 4 (+ 8), columns 8 j + 2 (t % 4) (+ 1)).
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -76,42 +77,30 @@ template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wg
 // its producer warpgroup's budget so that its consumer warpgroups can raise theirs within the SM's 64 K registers.
 template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-template <int N> __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
-template <> __device__ __forceinline__ void wgmma_bf16<8>(float (&d)[4], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
-template <> __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(da), "l"(db), "r"(scale_d));
-}
+// One specialisation per (element type, N): the element type selects the PTX operand type, .bf16 or .f16 (the same
+// tensor-core rate on sm_90a; fp16 keeps 3 more mantissa bits, bf16 8 more exponent bits).
+template <typename T, int N> __device__ __forceinline__ void wgmma_mma(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+#define MV2_WGMMA_DEF(T, TY, N, REGS, DA, DB, P, ...)                                                            \
+  template <> __device__ __forceinline__ void wgmma_mma<T, N>(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) { \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " P ", 0;\n\t"                                           \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." TY "." TY " " REGS ", " DA ", " DB ", p, 1, 1, 0, 0;\n\t}" \
+                 : __VA_ARGS__ : "l"(da), "l"(db), "r"(scale_d));                                                     \
+  }
+#define MV2_WGMMA_N8(T, TY) MV2_WGMMA_DEF(T, TY, 8, "{%0, %1, %2, %3}", "%4", "%5", "%6", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]))
+#define MV2_WGMMA_N16(T, TY) MV2_WGMMA_DEF(T, TY, 16, "{%0, %1, %2, %3, %4, %5, %6, %7}", "%8", "%9", "%10", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]))
+#define MV2_WGMMA_N32(T, TY) MV2_WGMMA_DEF(T, TY, 32, "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}", "%16", "%17", "%18", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]))
+#define MV2_WGMMA_N64(T, TY) MV2_WGMMA_DEF(T, TY, 64, "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}", "%32", "%33", "%34", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]))
+#define MV2_WGMMA_N128(T, TY) MV2_WGMMA_DEF(T, TY, 128, "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}", "%64", "%65", "%66", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]))
+#define MV2_WGMMA_ALL(T, TY) MV2_WGMMA_N8(T, TY) MV2_WGMMA_N16(T, TY) MV2_WGMMA_N32(T, TY) MV2_WGMMA_N64(T, TY) MV2_WGMMA_N128(T, TY)
+MV2_WGMMA_ALL(__nv_bfloat16, "bf16")
+MV2_WGMMA_ALL(__half, "f16")
+#undef MV2_WGMMA_ALL
+#undef MV2_WGMMA_N8
+#undef MV2_WGMMA_N16
+#undef MV2_WGMMA_N32
+#undef MV2_WGMMA_N64
+#undef MV2_WGMMA_N128
+#undef MV2_WGMMA_DEF
 
 // wgmma shared-memory matrix descriptor, K-major operand with hardware swizzle (128 B rows -> SWIZZLE_128B, 64 B ->
 // SWIZZLE_64B, 32 B -> SWIZZLE_32B), without the start address:
@@ -152,20 +141,25 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 
-__device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
-  __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
+// Two fp32 values rounded (RN) into one 32-bit word of the element type T, and the two halves of such a word back in fp32
+template <typename T> __device__ __forceinline__ uint32_t pack2(float a, float b) {
+  pair_t<T> v = f2_to_pair<T>(a, b);
   return *reinterpret_cast<uint32_t*>(&v);
+}
+template <typename T> __device__ __forceinline__ float2 unpack2(uint32_t r) {
+  if constexpr (std::is_same<T, __nv_bfloat16>::value) return make_float2(__uint_as_float(r << 16), __uint_as_float(r & 0xffff0000u));
+  else return pair_to_f2(*reinterpret_cast<const pair_t<T>*>(&r));
 }
 
 
 
 // ------------------------------------------------------------------------------------------
-// shared epilogue: fp32 accumulator chunk -> bias -> activation -> (GEGLU | shuffle) -> residual -> bf16 store
+// shared epilogue: fp32 accumulator chunk -> bias -> activation -> (GEGLU | shuffle) -> residual -> bf16 / fp16 store
 // ------------------------------------------------------------------------------------------
 struct TcEpi {
   const float* bias;             // global, packed column order (only used to decide has-bias; values come from smem)
-  const __nv_bfloat16* res;
-  __nv_bfloat16* y;
+  const void* res;               // element type of the kernel (bf16 / fp16)
+  void* y;
   int act, shuffle, mode;        // mode 0 plain; 1 GEGLU: packed cols [16g, 16g+8) = x, [16g+8, 16g+16) = gate (M:466-469);
                                  // 2 scaled residual: (act(acc + bias) + res) * 2^-0.5 (DiscriminatorBlock, M:585)
   int Co;                        // packed GEMM output columns
@@ -175,10 +169,10 @@ struct TcEpi {
   const float* oscale;           // [B][Co] or null: accumulator multiplier per (clip, output channel) before bias / activation
 };
 
-__device__ __forceinline__ void store8_bf16(__nv_bfloat16* dst, const float (&v)[8]) {
+template <typename T> __device__ __forceinline__ void store8(T* dst, const float (&v)[8]) {
   uint4 o;
-  o.x = pack_bf16x2(v[0], v[1]); o.y = pack_bf16x2(v[2], v[3]);
-  o.z = pack_bf16x2(v[4], v[5]); o.w = pack_bf16x2(v[6], v[7]);
+  o.x = pack2<T>(v[0], v[1]); o.y = pack2<T>(v[2], v[3]);
+  o.z = pack2<T>(v[4], v[5]); o.w = pack2<T>(v[6], v[7]);
   *reinterpret_cast<uint4*>(dst) = o;
 }
 
@@ -258,7 +252,7 @@ __device__ __forceinline__ float act_ct(float x, bool relu = false) {
 // r: 32 raw accumulator columns of ONE output row (position b,to,ho,wo); n = first packed column; sb = smem bias of
 // these columns (always valid memory; zeros when there is no bias).
 // row_base = linear position index * Co (plain mode), computed once per row by the caller.
-template <int MODE, int ACT>
+template <typename T, int MODE, int ACT>
 __device__ __forceinline__ void epi_chunk32_t(const TcEpi& e, const uint32_t (&r)[32], int ncols, int n, const float* sb,
                                               int b, int to, int ho, int wo, int64_t row_base, bool relu = false) {
   if (MODE == EPI_GEGLU) {
@@ -274,7 +268,7 @@ __device__ __forceinline__ void epi_chunk32_t(const TcEpi& e, const uint32_t (&r
         const float gt = __uint_as_float(r[g * 16 + 8 + q]) + sb[g * 16 + 8 + q];
         v[q] = gelu_fast(gt) * xv;
       }
-      store8_bf16(e.y + pos * I + ((n + g * 16) >> 1), v);
+      store8<T>((T*)e.y + pos * I + ((n + g * 16) >> 1), v);
     }
     return;
   }
@@ -313,58 +307,59 @@ __device__ __forceinline__ void epi_chunk32_t(const TcEpi& e, const uint32_t (&r
     const float rscale = e.mode == 2 ? 0.70710678118654752440f : 1.f;
     if (vec_ok && ng + 8 <= e.Co) {
       if (e.res) {
-        const uint4 rv = *reinterpret_cast<const uint4*>(e.res + off);
-        const __nv_bfloat162* rb = reinterpret_cast<const __nv_bfloat162*>(&rv);
+        const uint4 rv = *reinterpret_cast<const uint4*>((const T*)e.res + off);
+        const pair_t<T>* rb = reinterpret_cast<const pair_t<T>*>(&rv);
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const float2 f = __bfloat1622float2(rb[q]);
+          const float2 f = pair_to_f2(rb[q]);
           v[2 * q] = (v[2 * q] + f.x) * rscale;
           v[2 * q + 1] = (v[2 * q + 1] + f.y) * rscale;
         }
       }
-      store8_bf16(e.y + off, v);
+      store8<T>((T*)e.y + off, v);
     } else {
       if (MODE == EPI_RAGGED && e.out_cf) {            // conv_out: the reconstruction goes out in torch's (B, C, T, H, W)
         const int64_t plane = (int64_t)e.Ho * e.Wo;
         const int64_t o0 = ((int64_t)b * e.Co * e.To + to) * plane + (int64_t)ho * e.Wo + wo;
-        for (int q = 0; q < 8 && ng + q < e.Co; ++q) e.y[o0 + (int64_t)(ng + q) * e.To * plane] = __float2bfloat16_rn(v[q]);
+        for (int q = 0; q < 8 && ng + q < e.Co; ++q) ((T*)e.y)[o0 + (int64_t)(ng + q) * e.To * plane] = from_f32<T>(v[q]);
       } else
       for (int q = 0; q < 8 && ng + q < e.Co; ++q) {   // scalar tail (Co % 8 != 0, e.g. conv_out's 3 channels)
         float x = v[q];
-        if (e.res) x = (x + __bfloat162float(e.res[off + q])) * rscale;
-        e.y[off + q] = __float2bfloat16_rn(x);
+        if (e.res) x = (x + to_f32(((const T*)e.res)[off + q])) * rscale;
+        ((T*)e.y)[off + q] = from_f32<T>(x);
       }
     }
   }
 }
 
-// bias + activation + bf16 packing of one 32-column chunk (row-per-lane), for the staged epilogue
-template <int ACT>
+// bias + activation + packing into T of one 32-column chunk (row-per-lane), for the staged epilogue
+template <typename T, int ACT>
 __device__ __forceinline__ void epi_pack32_t(const uint32_t (&r)[32], const float* sb, uint32_t (&pk)[16], bool relu = false) {
 #pragma unroll
   for (int g = 0; g < 8; ++g) {
     const float4 b = *reinterpret_cast<const float4*>(sb + g * 4);
-    pk[2 * g] = pack_bf16x2(act_ct<ACT>(__uint_as_float(r[4 * g]) + b.x, relu), act_ct<ACT>(__uint_as_float(r[4 * g + 1]) + b.y, relu));
-    pk[2 * g + 1] = pack_bf16x2(act_ct<ACT>(__uint_as_float(r[4 * g + 2]) + b.z, relu), act_ct<ACT>(__uint_as_float(r[4 * g + 3]) + b.w, relu));
+    pk[2 * g] = pack2<T>(act_ct<ACT>(__uint_as_float(r[4 * g]) + b.x, relu), act_ct<ACT>(__uint_as_float(r[4 * g + 1]) + b.y, relu));
+    pk[2 * g + 1] = pack2<T>(act_ct<ACT>(__uint_as_float(r[4 * g + 2]) + b.z, relu), act_ct<ACT>(__uint_as_float(r[4 * g + 3]) + b.w, relu));
   }
 }
+template <typename T>
 __device__ __forceinline__ void epi_pack32(int act, const uint32_t (&r)[32], const float* sb, uint32_t (&pk)[16]) {
-  if (act == MV2_ACT_ELU) epi_pack32_t<MV2_ACT_ELU>(r, sb, pk);
-  else if (act == MV2_ACT_SILU) epi_pack32_t<MV2_ACT_SILU>(r, sb, pk);
-  else if (act == MV2_ACT_LEAKY_RELU || act == MV2_ACT_RELU) epi_pack32_t<MV2_ACT_LEAKY_RELU>(r, sb, pk, act == MV2_ACT_RELU);
-  else epi_pack32_t<MV2_ACT_NONE>(r, sb, pk);
+  if (act == MV2_ACT_ELU) epi_pack32_t<T, MV2_ACT_ELU>(r, sb, pk);
+  else if (act == MV2_ACT_SILU) epi_pack32_t<T, MV2_ACT_SILU>(r, sb, pk);
+  else if (act == MV2_ACT_LEAKY_RELU || act == MV2_ACT_RELU) epi_pack32_t<T, MV2_ACT_LEAKY_RELU>(r, sb, pk, act == MV2_ACT_RELU);
+  else epi_pack32_t<T, MV2_ACT_NONE>(r, sb, pk);
 }
 
 // activation is a kernel argument; dispatch once per chunk (warp uniform) into the compile-time variants
-template <int MODE>
+template <typename T, int MODE>
 __device__ __forceinline__ void epi_chunk32(const TcEpi& e, const uint32_t (&r)[32], int ncols, int n, const float* sb,
                                             int b, int to, int ho, int wo, int64_t row_base) {
-  if (MODE == EPI_GEGLU) { epi_chunk32_t<EPI_GEGLU, MV2_ACT_NONE>(e, r, ncols, n, sb, b, to, ho, wo, row_base); return; }
-  if (e.act == MV2_ACT_ELU) epi_chunk32_t<MODE, MV2_ACT_ELU>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
-  else if (e.act == MV2_ACT_SILU) epi_chunk32_t<MODE, MV2_ACT_SILU>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
+  if (MODE == EPI_GEGLU) { epi_chunk32_t<T, EPI_GEGLU, MV2_ACT_NONE>(e, r, ncols, n, sb, b, to, ho, wo, row_base); return; }
+  if (e.act == MV2_ACT_ELU) epi_chunk32_t<T, MODE, MV2_ACT_ELU>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
+  else if (e.act == MV2_ACT_SILU) epi_chunk32_t<T, MODE, MV2_ACT_SILU>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
   else if (e.act == MV2_ACT_LEAKY_RELU || e.act == MV2_ACT_RELU)
-    epi_chunk32_t<MODE, MV2_ACT_LEAKY_RELU>(e, r, ncols, n, sb, b, to, ho, wo, row_base, e.act == MV2_ACT_RELU);
-  else epi_chunk32_t<MODE, MV2_ACT_NONE>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
+    epi_chunk32_t<T, MODE, MV2_ACT_LEAKY_RELU>(e, r, ncols, n, sb, b, to, ho, wo, row_base, e.act == MV2_ACT_RELU);
+  else epi_chunk32_t<T, MODE, MV2_ACT_NONE>(e, r, ncols, n, sb, b, to, ho, wo, row_base);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -389,14 +384,16 @@ static inline CUtensorMapSwizzle swizzle_of_row(int row_bytes) {
   return row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
-// One bf16 tiled tensor map: dims and box innermost first, byte strides of dims 1 .. rank-1, unit element strides,
-// 256-byte L2 promotion; box elements outside the tensor are zero-filled.  `what` names the map in the error message.
-static inline int encode_bf16_map(CUtensorMap* map, int rank, const void* base, const cuuint64_t* dims,
-                                  const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swz, const char* what) {
+// One tiled tensor map of 16-bit elements (dtype MV2_BF16 or MV2_F16): dims and box innermost first, byte strides of dims
+// 1 .. rank-1, unit element strides, 256-byte L2 promotion; box elements outside the tensor are zero-filled.  `what` names
+// the map in the error message.
+static inline int encode_map16(CUtensorMap* map, int dtype, int rank, const void* base, const cuuint64_t* dims,
+                               const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swz, const char* what) {
   const EncodeTiledFn enc = get_encode_fn();
   if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return MV2_E_CUDA; }
   const cuuint32_t es[5] = {1, 1, 1, 1, 1};
-  const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, es,
+  const CUtensorMapDataType dt = dtype == MV2_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  const CUresult r = enc(map, dt, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, es,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r); return MV2_E_CUDA; }
   return MV2_OK;
@@ -405,11 +402,16 @@ static inline int encode_bf16_map(CUtensorMap* map, int rank, const void* base, 
 // Epilogue arguments of a tensor-core conv launch
 static inline TcEpi tc_epi_of(const mv2_tc_conv_args* a) {
   TcEpi e = {};
-  e.bias = a->bias; e.res = (const __nv_bfloat16*)a->res; e.y = (__nv_bfloat16*)a->y;
+  e.bias = a->bias; e.res = a->res; e.y = a->y;
   e.act = a->act; e.shuffle = a->shuffle; e.mode = a->epi_mode; e.Co = a->Co;
   e.To = a->To; e.Ho = a->Ho; e.Wo = a->Wo; e.out_cf = a->out_layout == 1; e.oscale = a->oscale;
   return e;
 }
+
+// Element type of a tensor-core conv launch: MV2_BF16 (also for 0, the value of a zero-initialised struct) or MV2_F16;
+// -1 for anything else
+static inline int tc_dtype_of(int32_t d) { return d == 0 || d == MV2_BF16 ? MV2_BF16 : (d == MV2_F16 ? MV2_F16 : -1); }
+static inline int tc_dtype(const mv2_tc_conv_args* a) { return tc_dtype_of(a->dtype); }
 
 static inline int pow2_ceil(int v) { int r = 1; while (r < v) r <<= 1; return r; }
 static inline int floor_div(int a, int b) { int q = a / b; if ((a % b != 0) && ((a < 0) != (b < 0))) --q; return q; }

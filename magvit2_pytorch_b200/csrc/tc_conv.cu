@@ -1,4 +1,4 @@
-// wgmma / TMA implicit-GEMM convolution for sm_90a (bf16 in, fp32 accumulate in registers).
+// wgmma / TMA implicit-GEMM convolution for sm_90a (bf16 or fp16 in, fp32 accumulate in registers).
 //
 // One kernel covers the whole dense-contraction family of the VideoTokenizer forward path:
 // causal 3x3x3 convs, 1x1x1 convs / Linear layers, the strided compress_space / compress_time
@@ -47,8 +47,8 @@ struct alignas(64) TcParams {
   TcEpi epi;
 };
 
-template <int MODE, int BN>
-__global__ void __launch_bounds__(384, 1) tc_conv_kernel(const __grid_constant__ TcParams p) {
+template <typename T, int MODE, int BN>
+__device__ __forceinline__ void tc_conv_body(const TcParams& p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -129,11 +129,11 @@ __global__ void __launch_bounds__(384, 1) tc_conv_kernel(const __grid_constant__
       wgmma_fence();
       const uint64_t ad = d_hi | (uint64_t)(lo + wg16);
       const uint64_t bd = d_hi | (uint64_t)(lo + a16);
-      wgmma_bf16<BN>(acc, ad, bd, i > 0 ? 1u : 0u);
-      if (ksteps > 1) wgmma_bf16<BN>(acc, ad + 2, bd + 2, 1u);
+      wgmma_mma<T, BN>(acc, ad, bd, i > 0 ? 1u : 0u);
+      if (ksteps > 1) wgmma_mma<T, BN>(acc, ad + 2, bd + 2, 1u);
       if (ksteps > 2) {
-        wgmma_bf16<BN>(acc, ad + 4, bd + 4, 1u);
-        wgmma_bf16<BN>(acc, ad + 6, bd + 6, 1u);
+        wgmma_mma<T, BN>(acc, ad + 4, bd + 4, 1u);
+        wgmma_mma<T, BN>(acc, ad + 6, bd + 6, 1u);
       }
       wgmma_commit();
       wgmma_wait_all();
@@ -156,7 +156,7 @@ __global__ void __launch_bounds__(384, 1) tc_conv_kernel(const __grid_constant__
     for (int c0 = half * 32; c0 < BN; c0 += 64) {
       uint32_t r[32];
       load_row32(srow + c0, 32, r);
-      if (row_ok) epi_chunk32<MODE>(p.epi, r, 32, n0 + c0, sbias + c0, b, to, ho, wo, row_base);
+      if (row_ok) epi_chunk32<T, MODE>(p.epi, r, 32, n0 + c0, sbias + c0, b, to, ho, wo, row_base);
     }
   }
 }
@@ -164,10 +164,17 @@ __global__ void __launch_bounds__(384, 1) tc_conv_kernel(const __grid_constant__
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-// kernel instance per (epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared memory.
-// Rows: ragged (plain) stores, GEGLU, depth-to-space / depth-to-time shuffle.
-#define MV2_TC_BN(M) {tc_conv_kernel<M, 32>, tc_conv_kernel<M, 64>, tc_conv_kernel<M, 128>}
-static void (*const g_tc_kernels[3][3])(TcParams) = {MV2_TC_BN(EPI_RAGGED), MV2_TC_BN(EPI_GEGLU), MV2_TC_BN(EPI_SHUFFLE)};
+// kernel instance per (element type, epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared
+// memory.  [0] bf16, [1] fp16; rows: ragged (plain) stores, GEGLU, depth-to-space / depth-to-time shuffle.
+// One kernel per element type (the names of the bf16 instances are those of the library before fp16 existed)
+template <int MODE, int BN>
+__global__ void __launch_bounds__(384, 1) tc_conv_kernel(const __grid_constant__ TcParams p) { tc_conv_body<__nv_bfloat16, MODE, BN>(p); }
+template <int MODE, int BN>
+__global__ void __launch_bounds__(384, 1) tc_conv_f16_kernel(const __grid_constant__ TcParams p) { tc_conv_body<__half, MODE, BN>(p); }
+#define MV2_TC_BN(K, M) {K<M, 32>, K<M, 64>, K<M, 128>}
+#define MV2_TC_FLAVOURS(K) {MV2_TC_BN(K, EPI_RAGGED), MV2_TC_BN(K, EPI_GEGLU), MV2_TC_BN(K, EPI_SHUFFLE)}
+static void (*const g_tc_kernels[2][3][3])(TcParams) = {MV2_TC_FLAVOURS(tc_conv_kernel), MV2_TC_FLAVOURS(tc_conv_f16_kernel)};
+#undef MV2_TC_FLAVOURS
 #undef MV2_TC_BN
 
 }  // namespace mv2
@@ -192,6 +199,7 @@ int mv2_tc_conv_hist_supported(const mv2_tc_conv_args* a) {
 
 int mv2_tc_conv_supported(const mv2_tc_conv_args* a) {
   if (!a) return 0;
+  if (tc_dtype(a) < 0) return 0;
   if (a->Ci % 16 != 0) return 0;                    // TMA inner box = 32/64/128 B, global strides multiple of 16 B
   if (a->kt * a->kh * a->kw > TC_MAX_TAPS) return 0;
   if (a->st < 1 || a->st > 2 || a->sh < 1 || a->sh > 2 || a->sw < 1 || a->sw > 2) return 0;
@@ -211,6 +219,7 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, vo
   const int hist_T = hist ? hist->T_h : 0;
   if (!mv2_tc_conv_supported(a)) { set_error("mv2_tc_conv_forward: unsupported shape (Ci=%d Co=%d)", a->Ci, a->Co); return MV2_E_UNSUPPORTED; }
 
+  const int dt = tc_dtype(a);
   TcParams p;
   memset(&p, 0, sizeof(p));
   const int bk = (a->Ci % 64 == 0) ? 64 : ((a->Ci % 32 == 0) ? 32 : 16);
@@ -261,13 +270,13 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, vo
         const char* base = (const char*)a->x + ((int64_t)pt * H * W + (int64_t)ph * W + pw) * C * 2;
         char what[32];
         snprintf(what, sizeof(what), "activations, phase %d", id);
-        if (const int rc = encode_bf16_map(&p.amap[id], 5, base, dims, strides, box, swz, what)) return rc;
+        if (const int rc = encode_map16(&p.amap[id], dt, 5, base, dims, strides, box, swz, what)) return rc;
       }
   if (hist_T > 0) {
     const cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)hist_T, (cuuint64_t)a->B};
     const cuuint64_t strides[4] = {(cuuint64_t)(C * 2), (cuuint64_t)(W * C * 2), (cuuint64_t)(H * W * C * 2), (cuuint64_t)(hist->clip_stride * 2)};
     const cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)p.bw, (cuuint32_t)p.bh, 1, 1};
-    if (const int rc = encode_bf16_map(&p.hmap, 5, hist->h, dims, strides, box, swz, "history")) return rc;
+    if (const int rc = encode_map16(&p.hmap, dt, 5, hist->h, dims, strides, box, swz, "history")) return rc;
   }
   // ---- taps ----
   p.ntaps = a->kt * a->kh * a->kw;
@@ -287,22 +296,23 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, vo
   const cuuint64_t wdims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
   const cuuint64_t wstrides[1] = {(cuuint64_t)(K * 2)};
   const cuuint32_t wbox[2] = {(cuuint32_t)bk, (cuuint32_t)bn};
-  if (const int rc = encode_bf16_map(&p.wmap, 2, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
+  if (const int rc = encode_map16(&p.wmap, dt, 2, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
 
   const size_t smem = 1024 + (size_t)stages * stage_bytes + 16 * stages + 16 + (size_t)bn * 4 + stg_bytes;
   static PerDeviceOnce attr_once;
   const cudaError_t attr_err = attr_once.run([] {
     cudaError_t e = cudaSuccess;
-    for (auto& row : g_tc_kernels)
-      for (auto k : row)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    for (auto& type : g_tc_kernels)
+      for (auto& row : type)
+        for (auto k : row)
+          if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     return e;
   });
   if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
   MV2_CHECK_ARG(smem <= 227 * 1024);
   dim3 grid((unsigned)((int64_t)a->B * p.tt * p.th * p.tw), (unsigned)ceil_div(a->Co, bn));
   const int flavour = a->epi_mode == 1 ? 1 : (a->shuffle != MV2_SHUFFLE_NONE ? 2 : 0);   // row of g_tc_kernels
-  launch_k(g_tc_kernels[flavour][bn == 32 ? 0 : (bn == 64 ? 1 : 2)], grid, dim3(384), smem, (cudaStream_t)stream, p);
+  launch_k(g_tc_kernels[dt == MV2_F16][flavour][bn == 32 ? 0 : (bn == 64 ? 1 : 2)], grid, dim3(384), smem, (cudaStream_t)stream, p);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }

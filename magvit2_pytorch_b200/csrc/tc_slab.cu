@@ -1,5 +1,6 @@
 // wgmma / TMA "slab" implicit-GEMM kernel for stride-1 k_t x k_h x k_w convolutions (the causal 3x3x3 residual
-// convs carry most of the path's FLOPs), bf16 in / fp32 accumulate in registers, persistent CTAs, sm_90a.
+// convs carry most of the path's FLOPs), bf16 or fp16 in (the element type T is a template parameter
+// of every kernel) / fp32 accumulate in registers, persistent CTAs, sm_90a.
 //
 // Why a second kernel: tc_conv.cu reloads the activation tile from L2 once per tap (27x) and the weight tile once per
 // 128 output positions.  Here
@@ -18,7 +19,7 @@
 //     128-column divisor take 128-column tiles with a ragged last one;
 //   * the kernel is instantiated per epilogue flavour (tc_common.cuh: EPI_*) and N tile (32 / 64 / 128); the plain,
 //     residual, GEGLU, SpatialDownsample2x and fused ResidualUnit flavours run the epilogue on the accumulator fragments
-//     and store bf16 boxes through TMA (slab_epi_mtile), the others stage the accumulators in shared memory first.
+//     and store bf16 / fp16 boxes through TMA (slab_epi_mtile), the others stage the accumulators in shared memory first.
 //     The channels-first flavour (EPI_RAGGED: fewer than 32 output channels, so never a wider tile than 32) has narrow
 //     8- and 16-column tiles (wgmma m64n8k16 / m64n16k16) instead, for the data gradient of conv_in with respect to the
 //     video: 3 output channels, 7 x 7 in-plane taps (slab_narrow).
@@ -52,6 +53,7 @@ struct alignas(64) SlabParams {
   int slab_stages, w_stages;
   int tpw;               // in-plane taps per weight stage (one 3-D TMA box {bk, bn, tpw})
   TcEpi epi;
+  int dtype;             // host side: MV2_BF16 or MV2_F16, selects the kernel instance and the tensor maps' element type
   // ---- EPI_FUSED_RU only (mv2_tc_ru_forward) ----
   CUtensorMap w1map;     // 1x1x1 weights [Co][Ci] as {ci, co}: 2-D boxes {64, bn}
   const float* bias1;    // 1x1x1 bias [C]
@@ -151,11 +153,11 @@ __host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& 
 // (h0 + 8 wg + m / 8, w0 + 8 j + m % 8)) and columns 8 g + 2 (lane % 4) + {0, 1}.  The math per element is that of the
 // staged epilogue, in the same order: x oscale, + bias and activation, [+ residual in fp32, x 2^-0.5 in mode 2], one
 // rounding to bf16; GEGLU pairs packed column 16 g + c (x) with 16 g + 8 + c (its gate), which the same thread holds.
-// Results go to `ot` as [boxes][64 rows][cb channels] bf16 boxes in the swizzle TMA uses for their row width; the
+// Results go to `ot` as [boxes][64 rows][cb channels] 16-bit boxes in the swizzle TMA uses for their row width; the
 // residual is read from `rt` in the same layout.  Bank-conflict free: the 8 rows of a warp's access fall on 8 different
 // 16-byte units of the swizzle.  With 128-byte rows this is also the layout of a K-major SWIZZLE_128B wgmma operand of
 // 64 rows (one 8 KB K-chunk per box), which the fused ResidualUnit's second GEMM reads.
-template <int MODE, int BN, int ACT>
+template <typename T, int MODE, int BN, int ACT>
 __device__ __forceinline__ void slab_epi_mtile(const SlabParams& p, const float (&acc)[BN / 2], const TileCoord& c,
                                                const float* sbias, uint32_t ot, uint32_t rt, int wq, int lane, bool relu) {
   constexpr int CB = slab_out_box_ch(MODE, BN);
@@ -179,7 +181,7 @@ __device__ __forceinline__ void slab_epi_mtile(const SlabParams& p, const float 
         const float* gv = &acc[8 * g + 4 + 2 * hr];
         const float v0 = gelu_fast(gv[0] + bg.x) * (xv[0] + bx.x);
         const float v1 = gelu_fast(gv[1] + bg.y) * (xv[1] + bx.y);
-        st32(ot + at(8 * g, m0 + 8 * hr), pack_bf16x2(v0, v1));
+        st32(ot + at(8 * g, m0 + 8 * hr), pack2<T>(v0, v1));
       }
     }
   } else {
@@ -199,23 +201,24 @@ __device__ __forceinline__ void slab_epi_mtile(const SlabParams& p, const float 
         if (MODE == EPI_PLAIN_RES) {
           uint32_t r;
           asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(rt + a) : "memory");
-          v0 = (v0 + __uint_as_float(r << 16)) * rs;
-          v1 = (v1 + __uint_as_float(r & 0xffff0000u)) * rs;
+          const float2 rf = unpack2<T>(r);
+          v0 = (v0 + rf.x) * rs;
+          v1 = (v1 + rf.y) * rs;
         }
-        st32(ot + a, pack_bf16x2(v0, v1));
+        st32(ot + a, pack2<T>(v0, v1));
       }
     }
   }
 }
 // All M-tiles of a warpgroup: output and residual tiles as [mw][boxes][64 rows][cb channels]
-template <int MODE, int BN, int ACT, int MWMAX>
+template <typename T, int MODE, int BN, int ACT, int MWMAX>
 __device__ __forceinline__ void slab_epi_fragment(const SlabParams& p, const float (&acc)[MWMAX][BN / 2], const TileCoord& c,
                                                   const float* sbias, uint32_t ot, uint32_t rt, int wq, int lane, bool relu) {
   constexpr uint32_t MTILE = (MODE == EPI_GEGLU ? BN / 2 : BN) * 64 * 2;   // bytes of one M-tile's boxes
 #pragma unroll
   for (int j = 0; j < MWMAX; ++j) {
     if (j >= p.mw) break;
-    slab_epi_mtile<MODE, BN, ACT>(p, acc[j], c, sbias, ot + j * MTILE, rt + j * MTILE, wq, lane, relu);
+    slab_epi_mtile<T, MODE, BN, ACT>(p, acc[j], c, sbias, ot + j * MTILE, rt + j * MTILE, wq, lane, relu);
   }
 }
 
@@ -227,8 +230,8 @@ __device__ __forceinline__ void slab_epi_fragment(const SlabParams& p, const flo
 // Register split: the launch gives every thread 168 registers (384 x 168 = 64,512); the producer warpgroup drops to
 // SLAB_PRODUCER_REGS and the consumers take the freed registers (128 x 40 + 256 x 232 = 64,512).
 constexpr int SLAB_PRODUCER_REGS = 40, SLAB_CONSUMER_REGS = 232;
-template <int MODE, int BN>
-__global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__ SlabParams p) {
+template <typename T, int MODE, int BN>
+__device__ __forceinline__ void tc_slab_body(const SlabParams& p) {
   constexpr int MWMAX = BN >= 32 ? 128 / BN : 4;        // mw <= 4 (slab_default_mw)
   constexpr int KC1 = BN >= 64 ? BN / 64 : 1;   // EPI_FUSED_RU (bn = C = 64 | 128): 64-channel K-chunks of the 1x1x1 GEMM
   constexpr bool TMA_STORE = slab_tma_epi(MODE) || MODE == EPI_FUSED_RU;   // y leaves through TMA box stores
@@ -464,10 +467,10 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
 #pragma unroll
             for (int j = 0; j < MW; ++j) {
               const uint64_t ad = a_hi | (uint64_t)(a_base + (uint32_t)p.dn_aoff[tap] + j * a_mtile);
-              wgmma_bf16<BN>(acc[j], ad, bd, accum);
-              wgmma_bf16<BN>(acc[j], ad + 2, bd + 2, 1u);
-              wgmma_bf16<BN>(acc[j], ad + 4, bd + 4, 1u);
-              wgmma_bf16<BN>(acc[j], ad + 6, bd + 6, 1u);
+              wgmma_mma<T, BN>(acc[j], ad, bd, accum);
+              wgmma_mma<T, BN>(acc[j], ad + 2, bd + 2, 1u);
+              wgmma_mma<T, BN>(acc[j], ad + 4, bd + 4, 1u);
+              wgmma_mma<T, BN>(acc[j], ad + 6, bd + 6, 1u);
             }
             wgmma_commit();
             retire_previous(w_idx, tap + tstep >= 6 ? s_idx : NONE);
@@ -493,11 +496,11 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
 #pragma unroll
                 for (int j = 0; j < MW; ++j) {
                   const uint64_t ad = a_hi | (uint64_t)(a_lo + j * a_mtile);
-                  wgmma_bf16<BN>(acc[j], ad, bd, accum);
-                  wgmma_bf16<BN>(acc[j], ad + 2, bd + 2, 1u);
+                  wgmma_mma<T, BN>(acc[j], ad, bd, accum);
+                  wgmma_mma<T, BN>(acc[j], ad + 2, bd + 2, 1u);
                   if (K4) {
-                    wgmma_bf16<BN>(acc[j], ad + 4, bd + 4, 1u);
-                    wgmma_bf16<BN>(acc[j], ad + 6, bd + 6, 1u);
+                    wgmma_mma<T, BN>(acc[j], ad + 4, bd + 4, 1u);
+                    wgmma_mma<T, BN>(acc[j], ad + 6, bd + 6, 1u);
                   }
                 }
                 wgmma_commit();
@@ -527,7 +530,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
       else if (MWMAX >= 2 && p.mw == 2) mainloop_k(c, std::integral_constant<int, (MWMAX >= 2 ? 2 : 1)>());
       else mainloop_k(c, std::integral_constant<int, 1>());
       if (slab_tma_epi(MODE)) {
-        // ---- register epilogue: bf16 results -> this warpgroup's output tile -> TMA box stores ----
+        // ---- register epilogue: 16-bit results -> this warpgroup's output tile -> TMA box stores ----
         constexpr int CB = slab_out_box_ch(MODE, BN), NB = (MODE == EPI_GEGLU ? BN / 2 : BN) / CB;
         constexpr uint32_t BOX = 64 * CB * 2;
         const uint32_t ot = L.otile + (uint32_t)(wg * p.mw * NB) * BOX, rt = L.rtile + (uint32_t)(wg * p.mw) * 64 * BN * 2;
@@ -536,10 +539,10 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
         if (MODE == EPI_PLAIN_RES) mbar_wait(L.rbar + 8 * wg, r_par);
         const int act = p.epi.act;
         if (MODE == EPI_GEGLU || act == MV2_ACT_NONE)
-          slab_epi_fragment<MODE, BN, MV2_ACT_NONE>(p, acc, c, sbias, ot, rt, wq, lane, false);
-        else if (act == MV2_ACT_ELU) slab_epi_fragment<MODE, BN, MV2_ACT_ELU>(p, acc, c, sbias, ot, rt, wq, lane, false);
-        else if (act == MV2_ACT_SILU) slab_epi_fragment<MODE, BN, MV2_ACT_SILU>(p, acc, c, sbias, ot, rt, wq, lane, false);
-        else slab_epi_fragment<MODE, BN, MV2_ACT_LEAKY_RELU>(p, acc, c, sbias, ot, rt, wq, lane, act == MV2_ACT_RELU);
+          slab_epi_fragment<T, MODE, BN, MV2_ACT_NONE>(p, acc, c, sbias, ot, rt, wq, lane, false);
+        else if (act == MV2_ACT_ELU) slab_epi_fragment<T, MODE, BN, MV2_ACT_ELU>(p, acc, c, sbias, ot, rt, wq, lane, false);
+        else if (act == MV2_ACT_SILU) slab_epi_fragment<T, MODE, BN, MV2_ACT_SILU>(p, acc, c, sbias, ot, rt, wq, lane, false);
+        else slab_epi_fragment<T, MODE, BN, MV2_ACT_LEAKY_RELU>(p, acc, c, sbias, ot, rt, wq, lane, act == MV2_ACT_RELU);
         if (MODE == EPI_PLAIN_RES) {
           __syncwarp();
           if (lane == 0) mbar_arrive(L.rbar + 16 + 8 * wg);
@@ -599,7 +602,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
         for (int j = 0; j < MWMAX; ++j) {
           if (j >= p.mw) break;
           // E1 (H is free: the previous second GEMM completed before the barrier that follows its E2)
-          slab_epi_mtile<MODE, BN, MV2_ACT_ELU>(p, acc[j], c, sbias, hb, 0, wq, lane, false);
+          slab_epi_mtile<T, MODE, BN, MV2_ACT_ELU>(p, acc[j], c, sbias, hb, 0, wq, lane, false);
           fence_proxy_async();      // generic-proxy writes -> visible to the tensor core's async-proxy reads
           named_bar_sync(wg_bar, 128);
           // second GEMM: acc[0] = H (this warpgroup's 64 rows) x W1^T
@@ -609,10 +612,10 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
 #pragma unroll
           for (int kc2 = 0; kc2 < KC1; ++kc2) {
             const uint64_t ad = h_hi | (uint64_t)(h_lo + kc2 * (BOX >> 4)), bd = h_hi | (uint64_t)w1_lo[kc2];
-            wgmma_bf16<BN>(acc[0], ad, bd, kc2 > 0 ? 1u : 0u);
-            wgmma_bf16<BN>(acc[0], ad + 2, bd + 2, 1u);
-            wgmma_bf16<BN>(acc[0], ad + 4, bd + 4, 1u);
-            wgmma_bf16<BN>(acc[0], ad + 6, bd + 6, 1u);
+            wgmma_mma<T, BN>(acc[0], ad, bd, kc2 > 0 ? 1u : 0u);
+            wgmma_mma<T, BN>(acc[0], ad + 2, bd + 2, 1u);
+            wgmma_mma<T, BN>(acc[0], ad + 4, bd + 4, 1u);
+            wgmma_mma<T, BN>(acc[0], ad + 6, bd + 6, 1u);
           }
           wgmma_commit();
           wgmma_wait<0>();
@@ -625,7 +628,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
           // E2 -> output tile of M-tile j -> TMA box stores (boxes without an output position are skipped; TMA clips
           // the others at the H and W edges)
           const uint32_t otj = ot + (uint32_t)(j * NB) * BOX;
-          slab_epi_mtile<MODE, BN, MV2_ACT_ELU>(p, acc[0], c, sb1, otj, 0, wq, lane, false);
+          slab_epi_mtile<T, MODE, BN, MV2_ACT_ELU>(p, acc[0], c, sb1, otj, 0, wq, lane, false);
           fence_proxy_async();
           named_bar_sync(wg_bar, 128);
           if (tid == 0) {
@@ -634,7 +637,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
               for (int b = 0; b < NB; ++b) tma_store_5d(&p.ymap, otj + (uint32_t)b * BOX, b * CB, c.w0 + 8 * j, c.h0 + 8 * wg, c.t, c.b);
             bulk_commit();
           }
-          // SE logit of this thread's row on the bf16 y, like the unfused path reads it: channels half * 32 + 64 q + 0..31
+          // SE logit of this thread's row on the rounded y, like the unfused path reads it: channels half * 32 + 64 q + 0..31
           // in order, one fma chain
           auto ld_y = [&](int q, uint32_t m, uint32_t u) {   // 16-byte unit u (channels 8 u ..) of row m, box q
             uint4 v;
@@ -652,14 +655,15 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
               const uint4 v = ld_y(q, mrow, 4 * half + g);
               const float4 wa = *reinterpret_cast<const float4*>(swk + half * 32 + 64 * q + 8 * g);
               const float4 wb = *reinterpret_cast<const float4*>(swk + half * 32 + 64 * q + 8 * g + 4);
-              lp = fmaf(__uint_as_float(v.x << 16), wa.x, lp);
-              lp = fmaf(__uint_as_float(v.x & 0xffff0000u), wa.y, lp);
-              lp = fmaf(__uint_as_float(v.y << 16), wa.z, lp);
-              lp = fmaf(__uint_as_float(v.y & 0xffff0000u), wa.w, lp);
-              lp = fmaf(__uint_as_float(v.z << 16), wb.x, lp);
-              lp = fmaf(__uint_as_float(v.z & 0xffff0000u), wb.y, lp);
-              lp = fmaf(__uint_as_float(v.w << 16), wb.z, lp);
-              lp = fmaf(__uint_as_float(v.w & 0xffff0000u), wb.w, lp);
+              const float2 f0 = unpack2<T>(v.x), f1 = unpack2<T>(v.y), f2 = unpack2<T>(v.z), f3 = unpack2<T>(v.w);
+              lp = fmaf(f0.x, wa.x, lp);
+              lp = fmaf(f0.y, wa.y, lp);
+              lp = fmaf(f1.x, wa.z, lp);
+              lp = fmaf(f1.y, wa.w, lp);
+              lp = fmaf(f2.x, wb.x, lp);
+              lp = fmaf(f2.y, wb.y, lp);
+              lp = fmaf(f3.x, wb.z, lp);
+              lp = fmaf(f3.y, wb.w, lp);
             }
           // the two warps of this lane quarter hold the two halves of every row's channels: exchange the logit partials
           float* lpb = lpart + (ecount & 1u) * 256;
@@ -691,8 +695,9 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
               const uint32_t vv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
               for (int i = 0; i < 4; ++i) {
-                t[2 * i] = fmaf(e4[k], __uint_as_float(vv[i] << 16), t[2 * i]);
-                t[2 * i + 1] = fmaf(e4[k], __uint_as_float(vv[i] & 0xffff0000u), t[2 * i + 1]);
+                const float2 f = unpack2<T>(vv[i]);
+                t[2 * i] = fmaf(e4[k], f.x, t[2 * i]);
+                t[2 * i + 1] = fmaf(e4[k], f.y, t[2 * i + 1]);
               }
             }
 #pragma unroll
@@ -745,7 +750,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
           for (int c0 = ((j + half) & 1) * 32; c0 < p.bn; c0 += 64) {
             uint32_t r[32], pk[16];
             load_row32(srow + c0, 32, r);
-            epi_pack32(p.epi.act, r, sbias + c.n0 + c0, pk);
+            epi_pack32<T>(p.epi.act, r, sbias + c.n0 + c0, pk);
 #pragma unroll
             for (int g = 0; g < 4; ++g)
               asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(wr + ((g ^ wsw) << 4)), "r"(pk[4 * g]),
@@ -755,16 +760,16 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
             const int klim = col_ok ? kmax : 0;
             // packed GEMM columns are (q, c): this chunk's 32 columns share one sub-pixel phase q (Cy % 32 == 0), so a
             // row's 64 bytes land contiguously at its shuffled position (reference M:824 / M:861 rearranges)
-            __nv_bfloat16* yp;
+            T* yp;
             int64_t ks;
             const int n = c.n0 + c0;
             if (p.epi.shuffle == MV2_SHUFFLE_SPACE) {
               const int cy = p.Co >> 2, qd = n / cy, cb = n - qd * cy;
-              yp = p.epi.y + ((((int64_t)c.b * p.T + c.t) * (2 * p.H) + (2 * h20 + (qd >> 1))) * (2 * p.W) + (2 * w2 + (qd & 1))) * cy + cb + piece * 8;
+              yp = (T*)p.epi.y + ((((int64_t)c.b * p.T + c.t) * (2 * p.H) + (2 * h20 + (qd >> 1))) * (2 * p.W) + (2 * w2 + (qd & 1))) * cy + cb + piece * 8;
               ks = (int64_t)4 * p.W * cy;          // next h row = two output rows further
             } else {
               const int cy = p.Co >> 1, qd = n / cy, cb = n - qd * cy;
-              yp = p.epi.y + ((((int64_t)c.b * (2 * p.T) + (2 * c.t + qd)) * p.H + h20) * p.W + w2) * cy + cb + piece * 8;
+              yp = (T*)p.epi.y + ((((int64_t)c.b * (2 * p.T) + (2 * c.t + qd)) * p.H + h20) * p.W + w2) * cy + cb + piece * 8;
               ks = (int64_t)p.W * cy;
             }
 #pragma unroll
@@ -780,7 +785,7 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
           for (int c0 = ((j + half) & 1) * 32; c0 < p.bn; c0 += 64) {
             uint32_t r[32];
             load_row32(srow + c0, BN < 32 ? BN : 32, r);     // a narrow tile's staged rows hold BN + 4 floats
-            if (row_ok) epi_chunk32<MODE>(p.epi, r, min(32, p.bn - c0), c.n0 + c0, sbias + c.n0 + c0, c.b, c.t, h, w, row_base);
+            if (row_ok) epi_chunk32<T, MODE>(p.epi, r, min(32, p.bn - c0), c.n0 + c0, sbias + c.n0 + c0, c.b, c.t, h, w, row_base);
           }
         }
       }
@@ -788,6 +793,12 @@ __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__
     if (TMA_STORE && tid == 0) bulk_wait_all();   // the output is written before the CTA exits
   }
 }
+
+// One kernel per element type (the names of the bf16 instances are those of the library before fp16 existed)
+template <int MODE, int BN>
+__global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__ SlabParams p) { tc_slab_body<__nv_bfloat16, MODE, BN>(p); }
+template <int MODE, int BN>
+__global__ void __launch_bounds__(384, 1) tc_slab_f16_kernel(const __grid_constant__ SlabParams p) { tc_slab_body<__half, MODE, BN>(p); }
 
 }  // namespace mv2
 
@@ -799,7 +810,7 @@ using namespace mv2;
 static bool slab_narrow(const mv2_tc_conv_args* a) { return a->out_layout == 1 && a->Co <= 16 && a->kw > 3; }
 
 extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
-  if (!a) return 0;
+  if (!a || tc_dtype(a) < 0) return 0;
   if (a->sh != 1 || a->sw != 1) return 0;
   if (a->st != 1) {      // TimeDownsample2x (M:796-807): stride 2 along t only, plain epilogue
     if (a->st != 2 || a->out_layout != 0 || a->epi_mode != 0 || a->shuffle != MV2_SHUFFLE_NONE) return 0;
@@ -863,6 +874,7 @@ static int slab_fill_plan(const mv2_tc_conv_args* a, SlabParams& p) {
   p.Ci = a->Ci; p.kchunks = a->Ci / (p.row_bytes / 2);
   p.B = a->B; p.T = a->To; p.H = a->Ho; p.W = a->Wo; p.Co = a->Co;
   p.epi = tc_epi_of(a);
+  p.dtype = tc_dtype(a);
 
   // ---- tiling: widest N tile (<= 128 columns), then as many M-tiles per weight tile as slab_default_mw allows ----
   const int co_pad = (a->Co + 31) / 32 * 32;
@@ -914,19 +926,19 @@ static int slab_encode_maps(SlabParams& p, const mv2_tc_conv_args* a, const mv2_
   const cuuint64_t xdims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)T, (cuuint64_t)a->B};
   const cuuint64_t xstrides[4] = {(cuuint64_t)(C * 2), (cuuint64_t)(W * C * 2), (cuuint64_t)(H * W * C * 2), (cuuint64_t)(T * H * W * C * 2)};
   const cuuint32_t xbox[5] = {(cuuint32_t)p.row_bytes / 2, (cuuint32_t)p.pitch, (cuuint32_t)p.slab_h, 1, 1};
-  if (const int rc = encode_bf16_map(&p.amap, 5, a->x, xdims, xstrides, xbox, swz, "slab")) return rc;
+  if (const int rc = encode_map16(&p.amap, p.dtype, 5, a->x, xdims, xstrides, xbox, swz, "slab")) return rc;
   p.hist_T = hist ? hist->T_h : 0;
   if (p.hist_T > 0) {     // the same boxes over the history: (T_h frames, clip stride of the tensor it lives in)
     const cuuint64_t hdims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)p.hist_T, (cuuint64_t)a->B};
     const cuuint64_t hstrides[4] = {xstrides[0], xstrides[1], xstrides[2], (cuuint64_t)(hist->clip_stride * 2)};
-    if (const int rc = encode_bf16_map(&p.hmap, 5, hist->h, hdims, hstrides, xbox, swz, "history")) return rc;
+    if (const int rc = encode_map16(&p.hmap, p.dtype, 5, hist->h, hdims, hstrides, xbox, swz, "history")) return rc;
   }
   const int64_t ntaps = (int64_t)a->kt * a->kh * a->kw, K = ntaps * C;
   const cuuint64_t wdims[3] = {(cuuint64_t)C, (cuuint64_t)a->Co, (cuuint64_t)ntaps}, kdims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
   const cuuint64_t wstrides[2] = {(cuuint64_t)(K * 2), (cuuint64_t)(C * 2)};
   const cuuint32_t wbox[3] = {(cuuint32_t)p.row_bytes / 2, (cuuint32_t)p.bn, (cuuint32_t)p.tpw};
-  if (const int rc = encode_bf16_map(&p.wmap, 3, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
-  return encode_bf16_map(&p.wmap2, 2, a->w, kdims, wstrides, wbox, swz, "weights 2-D");
+  if (const int rc = encode_map16(&p.wmap, p.dtype, 3, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
+  return encode_map16(&p.wmap2, p.dtype, 2, a->w, kdims, wstrides, wbox, swz, "weights 2-D");
 }
 // Output (and residual) maps of the TMA-store flavours: y as {oc, W, H, T, B} (oc = Co, or Co / 2 for GEGLU), boxes of
 // slab_out_box_ch channels x 8 (w) x 8 (h) in the swizzle of their row width
@@ -938,27 +950,31 @@ static int slab_encode_out_maps(SlabParams& p, int mode) {
                                  (cuuint64_t)(p.T * p.H * p.W * oc * 2)};
   const cuuint32_t box[5] = {(cuuint32_t)cb, 8, 8, 1, 1};
   const CUtensorMapSwizzle swz = swizzle_of_row(cb * 2);
-  if (const int rc = encode_bf16_map(&p.ymap, 5, p.epi.y, dims, strides, box, swz, "output")) return rc;
+  if (const int rc = encode_map16(&p.ymap, p.dtype, 5, p.epi.y, dims, strides, box, swz, "output")) return rc;
   if (mode != EPI_PLAIN_RES) return MV2_OK;
-  return encode_bf16_map(&p.rmap, 5, p.epi.res, dims, strides, box, swz, "residual");
+  return encode_map16(&p.rmap, p.dtype, 5, p.epi.res, dims, strides, box, swz, "residual");
 }
 
 // Launches one slab-kernel flavour: persistent CTAs, one per SM of the current device (fewer when there are fewer tiles)
 static int slab_launch(int mode, const SlabParams& p, void* stream) {
   // kernel instance per (epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared memory.  The
   // channels-first flavour EPI_RAGGED (< 32 channels) has the 32-column tile and the narrow 16- and 8-column ones.
-#define MV2_SLAB_BN(M) {tc_slab_kernel<M, 32>, tc_slab_kernel<M, 64>, tc_slab_kernel<M, 128>}
-  static void (*const kernels[8][3])(SlabParams) = {
-      MV2_SLAB_BN(EPI_PLAIN), MV2_SLAB_BN(EPI_GEGLU), MV2_SLAB_BN(EPI_SHUFFLE),
-      {tc_slab_kernel<EPI_RAGGED, 32>, tc_slab_kernel<EPI_RAGGED, 16>, tc_slab_kernel<EPI_RAGGED, 8>},
-      MV2_SLAB_BN(EPI_PLAIN_RES), MV2_SLAB_BN(EPI_FUSED_RU), MV2_SLAB_BN(EPI_SHUFFLE_ST), MV2_SLAB_BN(EPI_DOWN_SPACE)};
+  // [0] bf16, [1] fp16.
+#define MV2_SLAB_BN(K, M) {K<M, 32>, K<M, 64>, K<M, 128>}
+#define MV2_SLAB_FLAVOURS(K)                                                                                             \
+  {MV2_SLAB_BN(K, EPI_PLAIN), MV2_SLAB_BN(K, EPI_GEGLU), MV2_SLAB_BN(K, EPI_SHUFFLE),                                 \
+   {K<EPI_RAGGED, 32>, K<EPI_RAGGED, 16>, K<EPI_RAGGED, 8>},                                                           \
+   MV2_SLAB_BN(K, EPI_PLAIN_RES), MV2_SLAB_BN(K, EPI_FUSED_RU), MV2_SLAB_BN(K, EPI_SHUFFLE_ST), MV2_SLAB_BN(K, EPI_DOWN_SPACE)}
+  static void (*const kernels[2][8][3])(SlabParams) = {MV2_SLAB_FLAVOURS(tc_slab_kernel), MV2_SLAB_FLAVOURS(tc_slab_f16_kernel)};
+#undef MV2_SLAB_FLAVOURS
 #undef MV2_SLAB_BN
   static PerDeviceOnce attr_once;
   const cudaError_t attr_err = attr_once.run([] {
     cudaError_t e = cudaSuccess;
-    for (auto& row : kernels)
-      for (auto k : row)
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    for (auto& type : kernels)
+      for (auto& row : type)
+        for (auto k : row)
+          if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     return e;
   });
   if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
@@ -969,7 +985,7 @@ static int slab_launch(int mode, const SlabParams& p, void* stream) {
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   MV2_CHECK_ARG(p.bn >= 32 || mode == EPI_RAGGED);
   const int slot = p.bn == 32 ? 0 : (p.bn == 64 || p.bn == 16 ? 1 : 2);
-  launch_k(kernels[mode][slot], dim3(std::min(p.total_tiles, n_sm)), dim3(384), smem,
+  launch_k(kernels[p.dtype == MV2_F16][mode][slot], dim3(std::min(p.total_tiles, n_sm)), dim3(384), smem,
            (cudaStream_t)stream, p);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
@@ -1030,6 +1046,7 @@ static void ru_as_conv_args(const mv2_tc_ru_args* a, mv2_tc_conv_args* c) {
   c->kt = a->kt; c->kh = a->kh; c->kw = a->kw; c->st = c->sh = c->sw = 1;
   c->pt = a->kt - 1; c->ph = a->kh / 2; c->pw = a->kw / 2;
   c->act = MV2_ACT_ELU; c->shuffle = MV2_SHUFFLE_NONE; c->epi_mode = 0;
+  c->dtype = a->dtype;
 }
 
 extern "C" int mv2_tc_ru_supported(const mv2_tc_ru_args* a) {
@@ -1088,7 +1105,7 @@ extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, const mv2_conv_hist* h
   const cuuint64_t dims1[2] = {(cuuint64_t)a->C, (cuuint64_t)a->C};
   const cuuint64_t strides1[1] = {(cuuint64_t)a->C * 2};
   const cuuint32_t box1[2] = {64, (cuuint32_t)p.bn};
-  if (const int rc = encode_bf16_map(&p.w1map, 2, a->w1, dims1, strides1, box1, CU_TENSOR_MAP_SWIZZLE_128B, "w1")) return rc;
+  if (const int rc = encode_map16(&p.w1map, p.dtype, 2, a->w1, dims1, strides1, box1, CU_TENSOR_MAP_SWIZZLE_128B, "w1")) return rc;
   if (const int rc = slab_encode_out_maps(p, EPI_FUSED_RU)) return rc;
   return slab_launch(EPI_FUSED_RU, p, stream);
 }
@@ -1104,7 +1121,7 @@ extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, const mv2_conv_hist* h
 // tap' = dh * 2 + (dw2 + 1), lower half of the dw2 = -1 taps zero (and never loaded).
 // =====================================================================================================================
 extern "C" int mv2_tc_down_space_supported(const mv2_tc_conv_args* a) {
-  if (!a) return 0;
+  if (!a || tc_dtype(a) < 0) return 0;
   if (a->kt != 1 || a->kh != 3 || a->kw != 3 || a->st != 1 || a->sh != 2 || a->sw != 2) return 0;
   if (a->pt != 0 || a->ph != 1 || a->pw != 1) return 0;
   if ((a->Hi & 1) || (a->Wi & 1) || a->Ho != a->Hi / 2 || a->Wo != a->Wi / 2 || a->To != a->Ti) return 0;
@@ -1123,6 +1140,7 @@ extern "C" int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream
   p.row_bytes = 128; p.Ci = C2; p.kchunks = C2 / bk; p.dn_lower = a->Ci / bk;
   p.B = a->B; p.T = a->To; p.H = a->Ho; p.W = a->Wo; p.Co = a->Co;
   p.epi = tc_epi_of(a);
+  p.dtype = tc_dtype(a);
   int bn = 32;
   for (int c = 128; c >= 32; c >>= 1) if (a->Co % c == 0) { bn = c; break; }
   const int w_bytes = bn * 128;
@@ -1150,13 +1168,13 @@ extern "C" int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream
   const cuuint64_t dims[5] = {(cuuint64_t)C2, (cuuint64_t)(a->Wi / 2), (cuuint64_t)(a->Hi / 2), (cuuint64_t)a->Ti, (cuuint64_t)a->B};
   const cuuint64_t strides[4] = {(cuuint64_t)(C2 * 2), (cuuint64_t)(2 * rowb), (cuuint64_t)(a->Hi * rowb), (cuuint64_t)(a->Ti * a->Hi * rowb)};
   const cuuint32_t box_e[5] = {(cuuint32_t)bk, (cuuint32_t)p.pitch, 16, 1, 1}, box_o[5] = {(cuuint32_t)bk, (cuuint32_t)p.pitch, 17, 1, 1};
-  if (const int rc = encode_bf16_map(&p.amap, 5, a->x, dims, strides, box_e, CU_TENSOR_MAP_SWIZZLE_128B, "even rows")) return rc;
-  if (const int rc = encode_bf16_map(&p.amap_odd, 5, (const char*)a->x + rowb, dims, strides, box_o, CU_TENSOR_MAP_SWIZZLE_128B, "odd rows")) return rc;
+  if (const int rc = encode_map16(&p.amap, p.dtype, 5, a->x, dims, strides, box_e, CU_TENSOR_MAP_SWIZZLE_128B, "even rows")) return rc;
+  if (const int rc = encode_map16(&p.amap_odd, p.dtype, 5, (const char*)a->x + rowb, dims, strides, box_o, CU_TENSOR_MAP_SWIZZLE_128B, "odd rows")) return rc;
   const int64_t K = 6 * (int64_t)C2;
   const cuuint64_t wdims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
   const cuuint64_t wstrides[1] = {(cuuint64_t)(K * 2)};
   const cuuint32_t wbox[2] = {(cuuint32_t)bk, (cuuint32_t)bn};
-  if (const int rc = encode_bf16_map(&p.wmap2, 2, a->w, wdims, wstrides, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "weights")) return rc;
+  if (const int rc = encode_map16(&p.wmap2, p.dtype, 2, a->w, wdims, wstrides, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "weights")) return rc;
   p.wmap = p.wmap2;
   if (const int rc = slab_encode_out_maps(p, EPI_DOWN_SPACE)) return rc;
   return slab_launch(EPI_DOWN_SPACE, p, stream);

@@ -3,7 +3,7 @@ kernels of libmagvit2_b200.so through the C ABI (ctypes).  PyTorch is used only 
 memory (caching allocator), streams and parameter storage.
 
 Activations are channels-last (B, T, H, W, C) tensors in the compute dtype (fp32 -> CUDA-core
-path, bf16 -> wgmma tensor-core path for the dense contractions).  There is no eager / CPU
+path, bf16 or fp16 -> wgmma tensor-core path for the dense contractions, tensor_core_dtype).  There is no eager / CPU
 fallback: every op is a library call and a missing library is an error.
 """
 from __future__ import annotations
@@ -16,7 +16,7 @@ from typing import Callable, Dict, List, Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import (ACT_ELU, ACT_NONE, ACT_SILU, MV2_BF16, MV2_F32, MV2_U8, SHUFFLE_NONE, SHUFFLE_SPACE,
+from ._lib import (ACT_ELU, ACT_NONE, ACT_SILU, MV2_BF16, MV2_F16, MV2_F32, MV2_U8, SHUFFLE_NONE, SHUFFLE_SPACE,
                    SHUFFLE_TIME, AttnArgs, ConvArgs, ConvHist, TcConvArgs, TcRuArgs, check)
 
 
@@ -25,7 +25,15 @@ def _dt(t: torch.dtype) -> int:
         return MV2_F32
     if t == torch.bfloat16:
         return MV2_BF16
-    raise TypeError(f"unsupported dtype {t} (only float32 and bfloat16)")
+    if t == torch.float16:
+        return MV2_F16
+    raise TypeError(f"unsupported dtype {t} (only float32, bfloat16 and float16)")
+
+
+def tensor_core_dtype(t: torch.dtype) -> bool:
+    """True for the parameter dtypes whose dense contractions run on the wgmma tensor cores (bf16 and fp16: 16-bit
+    storage, fp32 accumulation); fp32 runs on the CUDA cores."""
+    return t in (torch.bfloat16, torch.float16)
 
 
 def _src_dt(t: torch.dtype) -> int:
@@ -91,14 +99,14 @@ class ConvPack:
     k: Tuple[int, int, int]
     Ci: int
     Co: int
-    w_tc: Optional[torch.Tensor] = None      # [Co][taps*Ci] bf16, K-major (wgmma path); rows permuted for shuffles
+    w_tc: Optional[torch.Tensor] = None      # [Co][taps*Ci] bf16 / fp16, K-major (wgmma path); rows permuted for shuffles
     bias_tc: Optional[torch.Tensor] = None   # bias in w_tc's row order
     Ci_tc: int = 0                           # GEMM dims of the wgmma call (may be padded / re-paired)
     Co_tc: int = 0
     epi_mode: int = 0                        # 1: fused GEGLU (output has Co_tc // 2 channels); 2: (act(conv) + res) * 2^-0.5
     k_tc: Optional[Tuple[int, int, int]] = None
     macs: int = 0                            # algorithmic multiply-accumulates per output position (Co * Ci * taps, unpadded)
-    w_down: Optional[torch.Tensor] = None    # SpatialDownsample2x pack for mv2_tc_down_space_forward ([Co][6][2*Ci] bf16)
+    w_down: Optional[torch.Tensor] = None    # SpatialDownsample2x pack for mv2_tc_down_space_forward ([Co][6][2*Ci], as w_tc)
 
 
 def pack_conv(weight: torch.Tensor, bias: Optional[torch.Tensor], dtype, k=None, shuffle_q: int = 1) -> ConvPack:
@@ -114,14 +122,14 @@ def pack_conv(weight: torch.Tensor, bias: Optional[torch.Tensor], dtype, k=None,
     b = None if bias is None else bias.detach().float().contiguous()
     pk = ConvPack(w=w, bias=b, k=tuple(int(v) for v in k), Ci=int(Ci), Co=int(Co))
     pk.macs = int(Co) * int(Ci) * int(w3.shape[2])
-    if dtype == torch.bfloat16:
+    if tensor_core_dtype(dtype):
         wt = w3.permute(0, 2, 1).reshape(Co, -1)                      # [Co][tap*Ci + ci]
         bt = b
         if shuffle_q > 1:
             cy = Co // shuffle_q
             wt = wt.reshape(cy, shuffle_q, -1).permute(1, 0, 2).reshape(Co, -1)
             bt = None if b is None else b.reshape(cy, shuffle_q).t().reshape(Co).contiguous()
-        pk.w_tc = wt.contiguous().to(torch.bfloat16)
+        pk.w_tc = wt.contiguous().to(dtype)
         pk.bias_tc = bt
         pk.Ci_tc, pk.Co_tc, pk.k_tc = pk.Ci, pk.Co, pk.k
     return pk
@@ -138,7 +146,7 @@ def pack_conv_down_space(pk: ConvPack, weight):
     wd[:, :, 0, Ci:] = w[:, :, :, 0].permute(0, 2, 1)
     wd[:, :, 1, :Ci] = w[:, :, :, 1].permute(0, 2, 1)
     wd[:, :, 1, Ci:] = w[:, :, :, 2].permute(0, 2, 1)
-    pk.w_down = wd.reshape(Co, 6 * 2 * Ci).contiguous().to(torch.bfloat16)
+    pk.w_down = wd.reshape(Co, 6 * 2 * Ci).contiguous().to(pk.w_tc.dtype)
 
 
 def _round_up(v, m):
@@ -153,10 +161,10 @@ def pack_ff(fc1_w, fc1_b, fc2_w, fc2_b, dtype):
     fc1 = pack_conv(fc1_w, fc1_b, dtype)
     fc2 = pack_conv(fc2_w, fc2_b, dtype)
     two_i, C_ = fc1_w.shape[:2]
-    if dtype == torch.bfloat16 and C_ % 16 != 0:
+    if tensor_core_dtype(dtype) and C_ % 16 != 0:
         for pk in (fc1, fc2):
             pk.w_tc = pk.bias_tc = None
-    elif dtype == torch.bfloat16:
+    elif tensor_core_dtype(dtype):
         I = two_i // 2
         Ip = _round_up(I, 64)
         w1 = fc1_w.detach().reshape(two_i, C_).float()
@@ -168,12 +176,12 @@ def pack_ff(fc1_w, fc1_b, fc2_w, fc2_b, dtype):
         wx[:I], wg[:I], bx[:I], bg[:I] = w1[:I], w1[I:], b1[:I], b1[I:]
         wp = torch.stack((wx.reshape(Ip // 8, 8, C_), wg.reshape(Ip // 8, 8, C_)), dim=1).reshape(2 * Ip, C_)
         bp = torch.stack((bx.reshape(Ip // 8, 8), bg.reshape(Ip // 8, 8)), dim=1).reshape(2 * Ip)
-        fc1.w_tc, fc1.bias_tc = wp.contiguous().to(torch.bfloat16), bp.contiguous()
+        fc1.w_tc, fc1.bias_tc = wp.contiguous().to(dtype), bp.contiguous()
         fc1.Ci_tc, fc1.Co_tc, fc1.epi_mode = int(C_), 2 * Ip, 1
         w2 = fc2_w.detach().reshape(fc2_w.shape[0], I).float()
         w2p = torch.zeros((w2.shape[0], Ip), device=w2.device)
         w2p[:, :I] = w2
-        fc2.w_tc = w2p.contiguous().to(torch.bfloat16)
+        fc2.w_tc = w2p.contiguous().to(dtype)
         fc2.Ci_tc, fc2.Co_tc = Ip, int(w2.shape[0])
     return fc1, fc2
 
@@ -193,7 +201,7 @@ def pack_feed_forward(ff, dt):
     return dict(gamma=ff.norm.gamma.detach().float().reshape(-1).contiguous(), fc1=fc1, fc2=fc2, inner=ff.dim_inner)
 
 
-def pack_conv_in_kwpack(weight, bias, cpack=32):
+def pack_conv_in_kwpack(weight, bias, cpack=32, dtype=torch.bfloat16):
     """conv_in (M:1109) for the wgmma path: (Co, Cin, kt, kh, kw) -> [Co][(dt, dh)][dw * Cin + c], zero padded to
     `cpack` channels -- pairs with mv2_ingest_kwpack."""
     Co, Cin, kt, kh, kw = weight.shape
@@ -203,7 +211,7 @@ def pack_conv_in_kwpack(weight, bias, cpack=32):
     wp = torch.zeros((Co, kt * kh, cpack), device=w.device)
     wp[:, :, :kw * Cin] = w
     pk = ConvPack(w=None, bias=None, k=(kt, kh, 1), Ci=cpack, Co=int(Co))
-    pk.w_tc = wp.reshape(Co, kt * kh * cpack).contiguous().to(torch.bfloat16)
+    pk.w_tc = wp.reshape(Co, kt * kh * cpack).contiguous().to(dtype)
     pk.bias_tc = None if bias is None else bias.detach().float().contiguous()
     pk.Ci_tc, pk.Co_tc, pk.k_tc = cpack, int(Co), (kt, kh, 1)
     pk.kw_orig, pk.cin_orig = int(kw), int(Cin)
@@ -227,15 +235,16 @@ class PackCache:
         self.packs = None
         self._sig = None
 
-    def get(self, module, what, build, key=()):
+    def get(self, module, what, build, key=(), half=False):
         """-> (engine, packs): re-packs with build(engine), under no_grad, when the module's parameters (param_signature) or
-        `key` changed, after binding the engine to them (Engine.bind; `what` names the module in its errors)."""
+        `key` changed, after binding the engine to them (Engine.bind; `what` names the module in its errors, `half` admits
+        fp16 parameters)."""
         sig = (param_signature(module), key)
         if sig != self._sig:
             self._sig = None
             if self.engine is None:
                 self.engine = Engine(None)
-            self.engine.bind(next(iter(module.parameters())), what)
+            self.engine.bind(next(iter(module.parameters())), what, half)
             with torch.no_grad():
                 self.packs = build(self.engine)
             self._sig = sig
@@ -255,9 +264,9 @@ class Engine:
         self._sig = None
         self._sig_id = 0             # bumped whenever parameters are re-packed (invalidates cached CUDA graphs)
         self.launches = 0            # kernels launched through the C ABI (bench's gpu_launches)
-        self.use_tc = True           # bf16: dense contractions on wgmma (False -> CUDA-core cross-check path)
+        self.use_tc = True           # bf16 / fp16: dense contractions on wgmma (False -> CUDA-core cross-check path)
         self.tc_variant = "auto"     # "auto" (Engine.conv_kernel's choice) | "tap" (tc_conv.cu only)
-        self.fuse_ru = True          # bf16: conv3x3x3 + ELU + conv1x1x1 + ELU + SE pool partials in one wgmma launch (C = 64 / 128)
+        self.fuse_ru = True          # bf16 / fp16: conv3x3x3 + ELU + conv1x1x1 + ELU + SE pool partials in one wgmma launch (C = 64 / 128)
         self.fused_ru_calls = 0
         self.tc_calls = 0
         self.slab_calls = 0
@@ -271,13 +280,16 @@ class Engine:
         self.host_step: Optional[Callable] = None
 
     # ------------------------------------------------------------------ parameters
-    def bind(self, p0: torch.Tensor, what: str):
+    def bind(self, p0: torch.Tensor, what: str, half: bool = True):
         """Runs on the device and in the dtype of parameter p0, after checking that they are an sm_90 CUDA device and
-        fp32 / bf16.  `what` names the model in the error messages."""
+        fp32 / bf16 / fp16 (fp16 only with `half`: the modules that only train, the discriminator and the VGG, have no
+        fp16 path).  `what` names the model in the error messages."""
         if p0.device.type != "cuda":
             raise RuntimeError(f"{what} runs on CUDA (sm_90a) only; move the model with .cuda() -- there is no CPU fallback")
-        if p0.dtype not in (torch.float32, torch.bfloat16):
-            raise TypeError("parameters must be float32 or bfloat16")
+        if p0.dtype == torch.float16 and not half:
+            raise TypeError(f"{what} does not run in float16 (its training path has no fp16 support): use float32 or bfloat16")
+        if p0.dtype not in (torch.float32, torch.bfloat16, torch.float16):
+            raise TypeError("parameters must be float32, bfloat16 or float16")
         arch = self.lib.mv2_device_arch()
         if arch != 90:
             raise RuntimeError(f"libmagvit2_b200.so targets sm_90a (H100); device reports sm_{arch}")
@@ -294,7 +306,8 @@ class Engine:
         dt = self.dtype
         P: Dict[str, object] = {}
         P["conv_in"] = pack_conv(m.conv_in.conv.weight, m.conv_in.conv.bias, dt)
-        P["conv_in_tc"] = pack_conv_in_kwpack(m.conv_in.conv.weight, m.conv_in.conv.bias) if dt == torch.bfloat16 else None
+        P["conv_in_tc"] = (pack_conv_in_kwpack(m.conv_in.conv.weight, m.conv_in.conv.bias, dtype=dt) if tensor_core_dtype(dt)
+                           else None)
         P["conv_out"] = pack_conv(m.conv_out.conv.weight, m.conv_out.conv.bias, dt)
         if m.separate_first_frame_encoding:       # SameConv2d (M:887-890): a (1, kh, kw) conv on the single first frame
             P["conv_in_ff"] = pack_conv(m.conv_in_first_frame.weight, m.conv_in_first_frame.bias, dt)
@@ -346,7 +359,7 @@ class Engine:
                 elif st.kind == "compress_space":
                     if side == "enc":
                         P[key] = pack_conv(mod.conv.weight, mod.conv.bias, dt)                     # (Co,Ci,3,3) -> k=(1,3,3)
-                        if dt == torch.bfloat16:
+                        if tensor_core_dtype(dt):
                             pack_conv_down_space(P[key], mod.conv.weight)
                     else:
                         P[key] = pack_conv(mod.net[0].weight, mod.net[0].bias, dt, shuffle_q=4)    # (4Co,Ci,1,1)
@@ -488,7 +501,7 @@ class Engine:
         """The kernel conv() runs for the call `ta` (its mv2_tc_conv_args) with hist_T history frames: "slab" (tc_slab.cu),
         "down" (its SpatialDownsample2x flavour, on pk.w_down), "tap" (tc_conv.cu), "tap_cat" (tc_conv.cu on a copy of
         [history | x]) or "simt" (the CUDA-core conv).  Host-side shape queries only: it launches nothing and needs no device."""
-        if not (self.dtype == torch.bfloat16 and self.use_tc and pk.w_tc is not None and ta.Ci == pk.Ci_tc and not token_shift):
+        if not (tensor_core_dtype(self.dtype) and self.use_tc and pk.w_tc is not None and ta.Ci == pk.Ci_tc and not token_shift):
             return "simt"
         lib = self.lib
         # the persistent slab kernel reuses each activation slab for all in-plane taps, so it takes every layer it supports
@@ -541,10 +554,10 @@ class Engine:
                           res=_ptr(res), y=_ptr(y), B=B, Ti=Ti, Hi=Hi, Wi=Wi, Ci=Ci, To=To, Ho=Ho, Wo=Wo, Co=pk.Co_tc,
                           kt=kt, kh=kh, kw=kw, st=stride[0], sh=stride[1], sw=stride[2],
                           pt=pt, ph=ph, pw=pw, act=act, shuffle=shuffle, epi_mode=pk.epi_mode,
-                          oscale=_ptr(oscale), out_layout=int(out_cf))
+                          oscale=_ptr(oscale), out_layout=int(out_cf), dtype=_dt(self.dtype))
 
     def conv_cf_supported(self, x, pk: ConvPack, pad, out_spatial) -> bool:
-        """True when conv(x, pk, pad=pad, out_spatial=out_spatial, out_cf=True) runs: bf16 on the slab kernel, whose
+        """True when conv(x, pk, pad=pad, out_spatial=out_spatial, out_cf=True) runs: bf16 / fp16 on the slab kernel, whose
         channels-first epilogue takes fewer than 8 (or a ragged number of) output channels."""
         return self.conv_kernel(self._tc_args(x, pk, pad=pad, out_spatial=out_spatial, out_cf=True), pk) == "slab"
 
@@ -557,7 +570,7 @@ class Engine:
         if self.fuse_ru and self.conv_kernel(self._tc_args(x, c3, act=ACT_ELU), c3) == "slab":
             ra = TcRuArgs(x=_ptr(x), w3=_ptr(c3.w_tc), b3=_ptr(c3.bias_tc), w1=_ptr(c1.w_tc), b1=_ptr(c1.bias_tc),
                           se_wk=_ptr(p["wk"]), se_bk=p["bk"], y=None, se_ws=None, B=B, T=T, H=H, W=W, C=Cc,
-                          kt=c3.k[0], kh=c3.k[1], kw=c3.k[2])
+                          kt=c3.k[0], kh=c3.k[1], kw=c3.k[2], dtype=dt)
             if self.lib.mv2_tc_ru_supported(C.byref(ra)):
                 hist, advance = self._conv_hist(_sub(ss, "conv3"), x, c3.k[0] - 1)
                 y = self._new(x.shape)
@@ -817,7 +830,7 @@ class Engine:
     def to_channels_last(self, v: torch.Tensor, t_pad: int = 0):
         """(B,C,T,H,W) torch tensor (fp32, bf16, or uint8 frames: normalised x / 255 as the reference's data loaders do,
         D:103, D:188) -> (B,T+t_pad,H,W,C) compute dtype."""
-        if v.dtype not in (torch.float32, torch.bfloat16, torch.uint8):
+        if v.dtype not in self._src_dtypes():
             v = v.float()
         v = v.contiguous()
         B, Cc, T, H, W = v.shape
@@ -825,13 +838,23 @@ class Engine:
         self._call("mv2_to_channels_last", _ptr(v), _src_dt(v.dtype), _ptr(out), _dt(self.dtype), B, Cc, T, H, W, t_pad)
         return out
 
+    def _src_dtypes(self):
+        """Video dtypes the layout-in kernels read directly (others are converted to fp32 first)."""
+        return (torch.float32, torch.bfloat16, torch.uint8) + ((torch.float16,) if self.dtype == torch.float16 else ())
+
     def ingest_kwpack(self, v: torch.Tensor, t_pad: int, pin):
-        """(B,C,T,H,W) -> (B,T+t_pad,H,W,32) bf16 with the k_w taps packed into channels (mv2_ingest_kwpack)."""
-        if v.dtype not in (torch.float32, torch.bfloat16, torch.uint8):
+        """(B,C,T,H,W) -> (B,T+t_pad,H,W,32) with the k_w taps packed into channels (mv2_ingest_kwpack), in the compute
+        dtype: mv2_ingest_kwpack writes fp16 for an fp16 source and bf16 for the others, so an fp16 model's uint8 / fp32
+        video is first rounded to fp16 in place of layout (mv2_to_channels_last of single-channel frames: a plain copy)."""
+        if v.dtype not in self._src_dtypes():
             v = v.float()
         v = v.contiguous()
         B, Cc, T, H, W = v.shape
-        out = self._new((B, T + t_pad, H, W, pin.Ci_tc), torch.bfloat16)
+        if self.dtype == torch.float16 and v.dtype != torch.float16:
+            v16 = self._new(tuple(v.shape), torch.float16)
+            self._call("mv2_to_channels_last", _ptr(v), _src_dt(v.dtype), _ptr(v16), MV2_F16, B * Cc * T, 1, 1, H, W, 0)
+            v = v16
+        out = self._new((B, T + t_pad, H, W, pin.Ci_tc), self.dtype)
         self._call("mv2_ingest_kwpack", _ptr(v), _src_dt(v.dtype), _ptr(out), B, Cc, T, H, W, t_pad, pin.kw_orig,
                    pin.kw_orig // 2, pin.Ci_tc)
         return out
@@ -871,7 +894,7 @@ class Engine:
         """F.mse_loss(a, b) of two same-layout tensors (reference M:1722: video vs reconstruction, both (B,C,T,H,W)) as a 0-d
         fp32 tensor; `a` may hold uint8 frames (x / 255)."""
         assert a.shape == b.shape, (a.shape, b.shape)
-        if a.dtype not in (torch.float32, torch.bfloat16, torch.uint8):
+        if a.dtype not in self._src_dtypes():
             a = a.float()
         a, b = a.contiguous(), b.contiguous()
         ws = self._new((self.lib.mv2_mse_workspace_bytes() // 4,), torch.float32)

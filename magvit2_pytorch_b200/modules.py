@@ -369,7 +369,7 @@ class CausalConvTranspose3d(nn.Module):
             raise RuntimeError("CausalConvTranspose3d runs on CUDA (sm_90a) only, input and parameters on the same device")
         with torch.no_grad(), torch.cuda.device(w.device):
             eng, pk = self._pack_cache.get(self, "CausalConvTranspose3d", lambda eng: pack_conv(
-                *self.equivalent_conv_weight(), eng.dtype, shuffle_q=self.upsample_factor))
+                *self.equivalent_conv_weight(), eng.dtype, shuffle_q=self.upsample_factor), half=True)
             y = eng.conv(eng.to_channels_last(x), pk, shuffle=SHUFFLE_TIME if self.upsample_factor == 2 else SHUFFLE_NONE)
             out = eng.to_channels_first(y)
             n = self.output_frames(x.shape[2])

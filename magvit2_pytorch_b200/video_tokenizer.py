@@ -9,7 +9,8 @@ M:): the keyword-only constructor and ``layers=(...)`` spec (M:1047-1092, M:1138
 
 All arithmetic runs in hand-written sm_90a kernels behind the C ABI of libmagvit2_b200.so;
 the compute dtype follows the parameters' dtype (``.float()`` -> fp32 CUDA-core path,
-``.bfloat16()`` -> bf16 wgmma path).  There is no CPU / eager fallback.
+``.bfloat16()`` -> bf16 wgmma path, ``.half()`` -> the same wgmma kernels in fp16: no-grad calls only, no discriminator /
+VGG).  There is no CPU / eager fallback.
 
 ``cond_residual`` layers (ResidualUnitMod / Conv3DMod, M:680-753, M:946-988) run on the device through the
 factorisation in include/magvit2_b200.h; the other ``cond_*`` types raise in the reference itself.
@@ -520,7 +521,13 @@ class VideoTokenizer(nn.Module):
             return None
         from .train import reached_parameters
         params = reached_parameters(self, entry, *args)
-        return params if (wants_input or params) else None
+        if not (wants_input or params):
+            return None
+        if self.dtype == torch.float16:
+            raise TypeError(f"{entry} with gradients is not supported for float16 models (fp16 runs the no-grad path only): "
+                            "call it under torch.no_grad() / in eval mode with inputs that do not require grad, or use "
+                            "float32 / bfloat16 parameters")
+        return params
 
     def _grad_call(self, method, x, cond, params, *args):
         """One differentiable call: train.TrainRunner.<method>(x, cond, *args) under train._TapeFn."""
@@ -716,6 +723,16 @@ class VideoTokenizer(nn.Module):
                              "here): construct with adversarial_loss_weight > 0 or pass a `vgg=` module")
         grad_step = (return_loss and self.training and torch.is_grad_enabled()
                      and any(p.requires_grad for p in self.parameters()))
+        if self.dtype == torch.float16:
+            # fp16 runs the no-grad tokenizer only: no gradients, and no discriminator or VGG (their paths train)
+            if return_discr_loss:
+                raise TypeError("return_discr_loss is not supported for float16 models: the discriminator has no fp16 path")
+            if return_loss and (self.has_gan or self.use_vgg or self.has_multiscale_discrs):
+                raise TypeError("return_loss is not supported for float16 models with a discriminator or a VGG: those modules "
+                                "have no fp16 path")
+            if grad_step:
+                raise TypeError("a train-mode return_loss step with gradients is not supported for float16 models: run it under "
+                                "torch.no_grad() or use float32 / bfloat16 parameters")
         if return_loss and self.training and self.use_vgg and (self.has_gan or self.has_multiscale_discrs) and not grad_step:
             raise RuntimeError("a train-mode return_loss with a VGG and a GAN needs gradients: the adaptive adversarial weight is "
                                "a ratio of gradient norms (M:1812-1841; the reference fails in torch.autograd.grad here)")
