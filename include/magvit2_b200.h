@@ -41,10 +41,13 @@ extern "C" {
 
 enum { MV2_F32 = 0, MV2_BF16 = 1,
        MV2_U8 = 2,  /* source dtype of the two layout-in entry points and of mv2_mse only: decoded uint8 frames, x / 255 */
-       MV2_F16 = 3  /* IEEE half: fp16 storage, fp32 accumulation */ };
+       MV2_F16 = 3, /* IEEE half: fp16 storage, fp32 accumulation */
+       MV2_TF32 = 4 /* tensor-core convs only: fp32 storage, TF32 multiply (the top 19 bits of each fp32 operand),
+                       fp32 accumulation */ };
 /* The tensor-core conv structs (mv2_tc_conv_args, mv2_tc_ru_args) carry their element type in a `dtype` field that sits
  * in what was padding before fp16 existed: 0 there means bf16, so a zero-initialised struct of an older caller keeps its
- * meaning.  MV2_F32 (also 0) is therefore not a distinct value there; the tensor-core kernels have no fp32 form anyway. */
+ * meaning.  MV2_F32 (also 0) is therefore not a distinct value there: fp32 activations run on the tensor cores as
+ * MV2_TF32 (the tap-wise and slab convs, SpatialDownsample2x; not the fused ResidualUnit, whose _supported refuses it). */
 enum { MV2_ACT_NONE = 0, MV2_ACT_ELU = 1, MV2_ACT_SILU = 2,
        MV2_ACT_LEAKY_RELU = 3,  /* LeakyReLU(0.1), the discriminator's activation (M:117-118) */
        MV2_ACT_RELU = 4         /* ReLU, the activation of a VGG feature extractor (perceptual loss, M:1397-1405) */ };
@@ -90,6 +93,9 @@ int mv2_to_channels_first(const void* src, int src_dtype, void* dst, int dst_dty
  *   so conv_in becomes a (k_t x k_h x 1)-tap implicit GEMM over cpack = 32 channels.                            */
 int mv2_ingest_kwpack(const void* src, int src_dtype, void* dst, int B, int C, int T, int H, int W,
                       int t_pad, int kw, int pw, int cpack, void* stream);
+/* MV2_KWPACK_F32_DST OR'd into mv2_ingest_kwpack's src_dtype (MV2_F32, MV2_BF16 or MV2_U8) writes fp32 instead: the
+ *   ingest of the TF32 conv_in, 7 x 3 packed channels zero padded to cpack = 32, one 128-byte K row.                  */
+#define MV2_KWPACK_F32_DST 0x100
 
 /* mv2_copy_frames: frame-range copy between channels-last clips (device memcpy2D, no kernel):
  *   dst[b][dst_t0 + i] = src[b][src_t0 + i], i < n_frames; zero_front != 0 also zero-fills dst frames [0, dst_t0).
@@ -280,14 +286,16 @@ size_t mv2_mse_workspace_bytes(void);
 int mv2_maxpool2x2(const void* x, void* y, int dtype, int N, int H, int W, int C, void* stream);
 int mv2_maxpool2x2_backward(const void* gy, const void* x, void* gx, int dtype, int N, int H, int W, int C, void* stream);
 
-/* ---- wgmma / TMA implicit-GEMM convolution (bf16 or fp16 in, fp32 accumulate in registers) ------------
- * Same operator family and epilogue as mv2_conv_forward, for bf16 or fp16 activations (mv2_tc_conv_args.dtype), executed on the
+/* ---- wgmma / TMA implicit-GEMM convolution (bf16, fp16 or TF32 in, fp32 accumulate in registers) ------------
+ * Same operator family and epilogue as mv2_conv_forward, for bf16, fp16 or fp32 (TF32 multiply) activations
+ * (mv2_tc_conv_args.dtype), executed on the
  * Hopper tensor cores (wgmma): TMA box loads with out-of-bounds zero fill implement the causal /
  * spatial halo (no padded copy, reference M:924-928), strided convs read through stride-phase
  * tensor maps, accumulators live in registers.  Weights are packed K-major: w[co][tap][ci] (bf16);
  * for depth-to-space / depth-to-time stores the host permutes the Co rows to co' = q*Cy + c
  * (q = p1*2+p2 or p) so that the shuffled stores are channel-contiguous; bias is permuted alike.
- * Requirements (mv2_tc_conv_supported): Ci % 16 == 0, strides in {1,2}, <= 64 taps.            */
+ * Requirements (mv2_tc_conv_supported): Ci * element size % 32 == 0 (Ci % 16 for 16-bit, Ci % 8 for fp32), strides in
+ * {1,2}, <= 64 taps.                                                                                                  */
 typedef struct mv2_tc_conv_args {
   const void* x;       /* bf16 (B, Ti, Hi, Wi, Ci) */
   const void* w;       /* bf16 [Co][kt*kh*kw*Ci] */
@@ -313,8 +321,10 @@ typedef struct mv2_tc_conv_args {
                           data gradient of a causal conv (the transposed conv, no leading pad) without its first Ti - To
                           frames: the video's gradient through conv_in; with Co <= 16 and kw > 3 (up to 7) it runs on
                           8- / 16-column N tiles.                                                                        */
-  int32_t dtype;       /* element type of x, w, res and y: MV2_F16, or MV2_BF16 (0, as in a zero-initialised struct, also
-                          means MV2_BF16).  It sits in what was the struct's tail padding: size and offsets are unchanged */
+  int32_t dtype;       /* element type of x, w, res and y: MV2_F16, MV2_TF32 (fp32), or MV2_BF16 (0, as in a
+                          zero-initialised struct, also means MV2_BF16).  It sits in what was the struct's tail padding:
+                          size and offsets are unchanged.  Channel rules are rules on bytes: a K row is 32 / 64 / 128 bytes,
+                          16 / 32 / 64 16-bit or 8 / 16 / 32 fp32 channels */
 } mv2_tc_conv_args;
 int mv2_tc_conv_supported(const mv2_tc_conv_args* a);
 int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, void* stream);

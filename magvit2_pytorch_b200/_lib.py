@@ -12,7 +12,8 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MV2_LIB_PATH") or os.path.join(_HERE, "libmagvit2_b200.so")   # env override: A/B builds
 
-MV2_F32, MV2_BF16, MV2_U8, MV2_F16 = 0, 1, 2, 3
+MV2_F32, MV2_BF16, MV2_U8, MV2_F16, MV2_TF32 = 0, 1, 2, 3, 4
+MV2_KWPACK_F32_DST = 0x100     # OR'd into mv2_ingest_kwpack's source dtype: fp32 destination (the TF32 conv_in)
 ACT_NONE, ACT_ELU, ACT_SILU, ACT_LEAKY_RELU, ACT_RELU = 0, 1, 2, 3, 4
 SHUFFLE_NONE, SHUFFLE_SPACE, SHUFFLE_TIME = 0, 1, 2
 
@@ -61,7 +62,7 @@ class TcConvArgs(C.Structure):
         ("pt", C.c_int32), ("ph", C.c_int32), ("pw", C.c_int32),
         ("act", C.c_int32), ("shuffle", C.c_int32), ("epi_mode", C.c_int32),
         ("oscale", C.c_void_p), ("out_layout", C.c_int32),
-        ("dtype", C.c_int32),    # MV2_F16, or MV2_BF16 (also 0)
+        ("dtype", C.c_int32),    # MV2_F16, MV2_TF32, or MV2_BF16 (also 0)
     ]
 
 

@@ -134,7 +134,8 @@ static int dispatch_transpose(const void* src, int sd, void* dst, int dd, int B,
 // 7x7x7, C_in = 3 conv becomes a (7x7x1)-tap conv over 32 "channels":
 //   dst[b][t + t_pad][h][w][dw * C + c] = src[b][c][t][h][w + dw - pw]   (0 outside the image / for padded channels)
 // One block per (b, t, h) image row: the C source rows are staged in shared memory with a zero halo (coalesced
-// loads, each source element read once), then every thread assembles 16-byte groups of 8 packed channels from them.
+// loads, each source element read once), then every thread assembles groups of 8 packed channels from them (16 bytes of
+// bf16 / fp16, 32 bytes of fp32).
 template <typename TS, typename TD>
 __global__ void __launch_bounds__(256) ingest_kwpack_kernel(const TS* __restrict__ src, TD* __restrict__ dst,
                                                             int B, int C, int T, int H, int W, int t_pad, int kw, int pw,
@@ -166,12 +167,18 @@ __global__ void __launch_bounds__(256) ingest_kwpack_kernel(const TS* __restrict
       v[q] = dw < kw ? srow[c * pitch + w + dw] : 0.f;     // srow index w + dw  <->  source column w + dw - pw
       if (++c == C) { c = 0; ++dw; }
     }
-    uint4 o;
-    pair_t<TD> p0 = f2_to_pair<TD>(v[0], v[1]), p1 = f2_to_pair<TD>(v[2], v[3]);
-    pair_t<TD> p2 = f2_to_pair<TD>(v[4], v[5]), p3 = f2_to_pair<TD>(v[6], v[7]);
-    o.x = *reinterpret_cast<uint32_t*>(&p0); o.y = *reinterpret_cast<uint32_t*>(&p1);
-    o.z = *reinterpret_cast<uint32_t*>(&p2); o.w = *reinterpret_cast<uint32_t*>(&p3);
-    *reinterpret_cast<uint4*>(drow + (int64_t)i * 8) = o;
+    if constexpr (std::is_same<TD, float>::value) {
+      float4* d4 = reinterpret_cast<float4*>(drow + (int64_t)i * 8);
+      d4[0] = make_float4(v[0], v[1], v[2], v[3]);
+      d4[1] = make_float4(v[4], v[5], v[6], v[7]);
+    } else {
+      uint4 o;
+      pair_t<TD> p0 = f2_to_pair<TD>(v[0], v[1]), p1 = f2_to_pair<TD>(v[2], v[3]);
+      pair_t<TD> p2 = f2_to_pair<TD>(v[4], v[5]), p3 = f2_to_pair<TD>(v[6], v[7]);
+      o.x = *reinterpret_cast<uint32_t*>(&p0); o.y = *reinterpret_cast<uint32_t*>(&p1);
+      o.z = *reinterpret_cast<uint32_t*>(&p2); o.w = *reinterpret_cast<uint32_t*>(&p3);
+      *reinterpret_cast<uint4*>(drow + (int64_t)i * 8) = o;
+    }
   }
 }
 
@@ -2737,7 +2744,16 @@ int mv2_ingest_kwpack(const void* src, int src_dtype, void* dst, int B, int C, i
   MV2_CHECK_ARG(rows <= 2147483647LL && smem <= 48 * 1024);
   const int blocks = (int)rows;
   cudaStream_t st = (cudaStream_t)stream;
-  if (src_dtype == MV2_F32)
+  if (src_dtype & MV2_KWPACK_F32_DST) {        // fp32 destination: the TF32 conv_in
+    src_dtype &= ~MV2_KWPACK_F32_DST;
+    if (src_dtype == MV2_F32)
+      launch_k(ingest_kwpack_kernel<float, float>, dim3(blocks), dim3(256), smem, st, (const float*)src, (float*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
+    else if (src_dtype == MV2_BF16)
+      launch_k(ingest_kwpack_kernel<__nv_bfloat16, float>, dim3(blocks), dim3(256), smem, st, (const __nv_bfloat16*)src, (float*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
+    else if (src_dtype == MV2_U8)
+      launch_k(ingest_kwpack_kernel<uint8_t, float>, dim3(blocks), dim3(256), smem, st, (const uint8_t*)src, (float*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
+    else { set_error("bad dtype %d", src_dtype); return MV2_E_ARG; }
+  } else if (src_dtype == MV2_F32)
     launch_k(ingest_kwpack_kernel<float, __nv_bfloat16>, dim3(blocks), dim3(256), smem, st, (const float*)src, (__nv_bfloat16*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);
   else if (src_dtype == MV2_BF16)
     launch_k(ingest_kwpack_kernel<__nv_bfloat16, __nv_bfloat16>, dim3(blocks), dim3(256), smem, st, (const __nv_bfloat16*)src, (__nv_bfloat16*)dst, B, C, T, H, W, t_pad, kw, pw, cpack);

@@ -64,9 +64,9 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-// ---- wgmma (sm_90a warpgroup MMA): D[regs] (+)= A[smem] * B[smem], bf16 or fp16 in, fp32 accumulate ----
+// ---- wgmma (sm_90a warpgroup MMA): D[regs] (+)= A[smem] * B[smem], bf16, fp16 or tf32 in, fp32 accumulate ----
 // Every wgmma instruction is issued by all 128 threads of a warpgroup; the 64 x N fp32 accumulator lives in their
-// registers (m64nNk16 fragment: thread t holds rows 16 (t / 32) + (t % 32) / 4 (+ 8), columns 8 j + 2 (t % 4) (+ 1)).
+// registers (m64nNk16 / m64nNk8 fragment: thread t holds rows 16 (t / 32) + (t % 32) / 4 (+ 8), columns 8 j + 2 (t % 4) (+ 1)).
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
@@ -78,22 +78,27 @@ template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wg
 template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 // One specialisation per (element type, N): the element type selects the PTX operand type, .bf16 or .f16 (the same
-// tensor-core rate on sm_90a; fp16 keeps 3 more mantissa bits, bf16 8 more exponent bits).
+// tensor-core rate on sm_90a; fp16 keeps 3 more mantissa bits, bf16 8 more exponent bits), or .tf32 for fp32 storage.
+// One MMA reads 32 bytes of K either way: k16 of a 16-bit type, k8 of tf32 (which has no transpose operands: both are
+// K-major, as here).  The tensor core reads a tf32 operand as the top 19 bits of its fp32 word (sign, 8-bit exponent,
+// 10-bit mantissa): the low 13 mantissa bits are dropped, not rounded.
 template <typename T, int N> __device__ __forceinline__ void wgmma_mma(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
-#define MV2_WGMMA_DEF(T, TY, N, REGS, DA, DB, P, ...)                                                            \
+#define MV2_WGMMA_DEF(T, TY, K, TR, N, REGS, DA, DB, P, ...)                                                     \
   template <> __device__ __forceinline__ void wgmma_mma<T, N>(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) { \
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " P ", 0;\n\t"                                           \
-                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." TY "." TY " " REGS ", " DA ", " DB ", p, 1, 1, 0, 0;\n\t}" \
+                 "wgmma.mma_async.sync.aligned.m64n" #N K ".f32." TY "." TY " " REGS ", " DA ", " DB ", p, 1, 1" TR ";\n\t}" \
                  : __VA_ARGS__ : "l"(da), "l"(db), "r"(scale_d));                                                     \
   }
-#define MV2_WGMMA_N8(T, TY) MV2_WGMMA_DEF(T, TY, 8, "{%0, %1, %2, %3}", "%4", "%5", "%6", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]))
-#define MV2_WGMMA_N16(T, TY) MV2_WGMMA_DEF(T, TY, 16, "{%0, %1, %2, %3, %4, %5, %6, %7}", "%8", "%9", "%10", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]))
-#define MV2_WGMMA_N32(T, TY) MV2_WGMMA_DEF(T, TY, 32, "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}", "%16", "%17", "%18", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]))
-#define MV2_WGMMA_N64(T, TY) MV2_WGMMA_DEF(T, TY, 64, "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}", "%32", "%33", "%34", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]))
-#define MV2_WGMMA_N128(T, TY) MV2_WGMMA_DEF(T, TY, 128, "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}", "%64", "%65", "%66", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]))
-#define MV2_WGMMA_ALL(T, TY) MV2_WGMMA_N8(T, TY) MV2_WGMMA_N16(T, TY) MV2_WGMMA_N32(T, TY) MV2_WGMMA_N64(T, TY) MV2_WGMMA_N128(T, TY)
-MV2_WGMMA_ALL(__nv_bfloat16, "bf16")
-MV2_WGMMA_ALL(__half, "f16")
+#define MV2_WGMMA_N8(T, TY, K, TR) MV2_WGMMA_DEF(T, TY, K, TR, 8, "{%0, %1, %2, %3}", "%4", "%5", "%6", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]))
+#define MV2_WGMMA_N16(T, TY, K, TR) MV2_WGMMA_DEF(T, TY, K, TR, 16, "{%0, %1, %2, %3, %4, %5, %6, %7}", "%8", "%9", "%10", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]))
+#define MV2_WGMMA_N32(T, TY, K, TR) MV2_WGMMA_DEF(T, TY, K, TR, 32, "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}", "%16", "%17", "%18", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]))
+#define MV2_WGMMA_N64(T, TY, K, TR) MV2_WGMMA_DEF(T, TY, K, TR, 64, "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}", "%32", "%33", "%34", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]))
+#define MV2_WGMMA_N128(T, TY, K, TR) MV2_WGMMA_DEF(T, TY, K, TR, 128, "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}", "%64", "%65", "%66", "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]))
+#define MV2_WGMMA_ALL(T, TY, K, TR) MV2_WGMMA_N8(T, TY, K, TR) MV2_WGMMA_N16(T, TY, K, TR) MV2_WGMMA_N32(T, TY, K, TR) \
+  MV2_WGMMA_N64(T, TY, K, TR) MV2_WGMMA_N128(T, TY, K, TR)
+MV2_WGMMA_ALL(__nv_bfloat16, "bf16", "k16", ", 0, 0")
+MV2_WGMMA_ALL(__half, "f16", "k16", ", 0, 0")
+MV2_WGMMA_ALL(float, "tf32", "k8", "")
 #undef MV2_WGMMA_ALL
 #undef MV2_WGMMA_N8
 #undef MV2_WGMMA_N16
@@ -154,11 +159,11 @@ template <typename T> __device__ __forceinline__ float2 unpack2(uint32_t r) {
 
 
 // ------------------------------------------------------------------------------------------
-// shared epilogue: fp32 accumulator chunk -> bias -> activation -> (GEGLU | shuffle) -> residual -> bf16 / fp16 store
+// shared epilogue: fp32 accumulator chunk -> bias -> activation -> (GEGLU | shuffle) -> residual -> bf16 / fp16 / fp32 store
 // ------------------------------------------------------------------------------------------
 struct TcEpi {
   const float* bias;             // global, packed column order (only used to decide has-bias; values come from smem)
-  const void* res;               // element type of the kernel (bf16 / fp16)
+  const void* res;               // element type of the kernel (bf16 / fp16 / fp32)
   void* y;
   int act, shuffle, mode;        // mode 0 plain; 1 GEGLU: packed cols [16g, 16g+8) = x, [16g+8, 16g+16) = gate (M:466-469);
                                  // 2 scaled residual: (act(acc + bias) + res) * 2^-0.5 (DiscriminatorBlock, M:585)
@@ -169,11 +174,31 @@ struct TcEpi {
   const float* oscale;           // [B][Co] or null: accumulator multiplier per (clip, output channel) before bias / activation
 };
 
+// 8 consecutive elements of T from / to fp32: 16 bytes of bf16 / fp16 (one rounding each), 32 bytes of fp32
 template <typename T> __device__ __forceinline__ void store8(T* dst, const float (&v)[8]) {
-  uint4 o;
-  o.x = pack2<T>(v[0], v[1]); o.y = pack2<T>(v[2], v[3]);
-  o.z = pack2<T>(v[4], v[5]); o.w = pack2<T>(v[6], v[7]);
-  *reinterpret_cast<uint4*>(dst) = o;
+  if constexpr (std::is_same<T, float>::value) {
+    reinterpret_cast<float4*>(dst)[0] = make_float4(v[0], v[1], v[2], v[3]);
+    reinterpret_cast<float4*>(dst)[1] = make_float4(v[4], v[5], v[6], v[7]);
+  } else {
+    uint4 o;
+    o.x = pack2<T>(v[0], v[1]); o.y = pack2<T>(v[2], v[3]);
+    o.z = pack2<T>(v[4], v[5]); o.w = pack2<T>(v[6], v[7]);
+    *reinterpret_cast<uint4*>(dst) = o;
+  }
+}
+template <typename T> __device__ __forceinline__ void load8(const T* src, float (&f)[8]) {
+  if constexpr (std::is_same<T, float>::value) {
+    const float4 a = reinterpret_cast<const float4*>(src)[0], b = reinterpret_cast<const float4*>(src)[1];
+    f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+  } else {
+    const uint4 rv = *reinterpret_cast<const uint4*>(src);
+    const pair_t<T>* rb = reinterpret_cast<const pair_t<T>*>(&rv);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const float2 p = pair_to_f2(rb[q]);
+      f[2 * q] = p.x; f[2 * q + 1] = p.y;
+    }
+  }
 }
 
 // Epilogue flavours are compile-time so each kernel instance carries only the code it runs (the generic version was
@@ -307,14 +332,10 @@ __device__ __forceinline__ void epi_chunk32_t(const TcEpi& e, const uint32_t (&r
     const float rscale = e.mode == 2 ? 0.70710678118654752440f : 1.f;
     if (vec_ok && ng + 8 <= e.Co) {
       if (e.res) {
-        const uint4 rv = *reinterpret_cast<const uint4*>((const T*)e.res + off);
-        const pair_t<T>* rb = reinterpret_cast<const pair_t<T>*>(&rv);
+        float rf[8];
+        load8<T>((const T*)e.res + off, rf);
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float2 f = pair_to_f2(rb[q]);
-          v[2 * q] = (v[2 * q] + f.x) * rscale;
-          v[2 * q + 1] = (v[2 * q + 1] + f.y) * rscale;
-        }
+        for (int q = 0; q < 8; ++q) v[q] = (v[q] + rf[q]) * rscale;
       }
       store8<T>((T*)e.y + off, v);
     } else {
@@ -384,15 +405,16 @@ static inline CUtensorMapSwizzle swizzle_of_row(int row_bytes) {
   return row_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
 }
 
-// One tiled tensor map of 16-bit elements (dtype MV2_BF16 or MV2_F16): dims and box innermost first, byte strides of dims
-// 1 .. rank-1, unit element strides, 256-byte L2 promotion; box elements outside the tensor are zero-filled.  `what` names
-// the map in the error message.
-static inline int encode_map16(CUtensorMap* map, int dtype, int rank, const void* base, const cuuint64_t* dims,
-                               const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swz, const char* what) {
+// One tiled tensor map of the elements of a tensor-core conv (dtype MV2_BF16, MV2_F16 or MV2_TF32: fp32): dims and box
+// innermost first, byte strides of dims 1 .. rank-1, unit element strides, 256-byte L2 promotion; box elements outside the
+// tensor are zero-filled.  `what` names the map in the error message.
+static inline int encode_tc_map(CUtensorMap* map, int dtype, int rank, const void* base, const cuuint64_t* dims,
+                                const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swz, const char* what) {
   const EncodeTiledFn enc = get_encode_fn();
   if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return MV2_E_CUDA; }
   const cuuint32_t es[5] = {1, 1, 1, 1, 1};
-  const CUtensorMapDataType dt = dtype == MV2_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  const CUtensorMapDataType dt = dtype == MV2_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                 : (dtype == MV2_TF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
   const CUresult r = enc(map, dt, (cuuint32_t)rank, const_cast<void*>(base), dims, strides, box, es,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(%s) failed: %d", what, (int)r); return MV2_E_CUDA; }
@@ -408,10 +430,14 @@ static inline TcEpi tc_epi_of(const mv2_tc_conv_args* a) {
   return e;
 }
 
-// Element type of a tensor-core conv launch: MV2_BF16 (also for 0, the value of a zero-initialised struct) or MV2_F16;
-// -1 for anything else
-static inline int tc_dtype_of(int32_t d) { return d == 0 || d == MV2_BF16 ? MV2_BF16 : (d == MV2_F16 ? MV2_F16 : -1); }
+// Element type of a tensor-core conv launch: MV2_BF16 (also for 0, the value of a zero-initialised struct), MV2_F16 or
+// MV2_TF32; -1 for anything else
+static inline int tc_dtype_of(int32_t d) {
+  return d == 0 || d == MV2_BF16 ? MV2_BF16 : (d == MV2_F16 || d == MV2_TF32 ? d : -1);
+}
 static inline int tc_dtype(const mv2_tc_conv_args* a) { return tc_dtype_of(a->dtype); }
+// Bytes per stored element of a tensor-core dtype: the host plans and maps in bytes, the kernels in elements of T
+static inline int tc_esize(int dtype) { return dtype == MV2_TF32 ? 4 : 2; }
 
 static inline int pow2_ceil(int v) { int r = 1; while (r < v) r <<= 1; return r; }
 static inline int floor_div(int a, int b) { int q = a / b; if ((a % b != 0) && ((a < 0) != (b < 0))) --q; return q; }

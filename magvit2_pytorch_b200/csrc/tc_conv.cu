@@ -1,4 +1,4 @@
-// wgmma / TMA implicit-GEMM convolution for sm_90a (bf16 or fp16 in, fp32 accumulate in registers).
+// wgmma / TMA implicit-GEMM convolution for sm_90a (bf16, fp16 or fp32 with TF32 multiply in, fp32 accumulate in registers).
 //
 // One kernel covers the whole dense-contraction family of the VideoTokenizer forward path:
 // causal 3x3x3 convs, 1x1x1 convs / Linear layers, the strided compress_space / compress_time
@@ -13,7 +13,7 @@
 // time halo, the spatial halo, ragged tile edges) are zero-filled by the TMA unit, so no padded
 // copy of the activations is ever materialised (the reference does F.pad + conv, M:924-928).
 // Strided convs read through "parity view" tensor maps (one per stride phase).  Both operands are
-// K-major in shared memory with the hardware 128B/64B/32B swizzle (BK = 64/32/16 channels).
+// K-major in shared memory with the hardware 128B/64B/32B swizzle (BK = 64/32/16 16-bit or 32/16/8 fp32 channels).
 // Warp roles (384 threads): warp 0 = TMA producer, warps 4-11 = two consumer warpgroups (rows 0-63 / 64-127 of the
 // tile): wgmma into registers, then the epilogue (accumulator -> shared-memory staging -> bias/activation/residual
 // -> global, one output row per thread and 32-column chunk).
@@ -53,7 +53,7 @@ __device__ __forceinline__ void tc_conv_body(const TcParams& p) {
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int bk = p.bk;
-  const uint32_t row_bytes = bk * 2;
+  const uint32_t row_bytes = bk * (int)sizeof(T);
   const uint32_t a_bytes = TC_BM * row_bytes;
   const uint32_t b_bytes = BN * row_bytes;
   const uint32_t stage_bytes = a_bytes + b_bytes;   // both multiples of 1024 (BN >= 32, bk >= 16)
@@ -119,8 +119,9 @@ __device__ __forceinline__ void tc_conv_body(const TcParams& p) {
     // ---------------- consumer warpgroups: wgmma main loop ----------------
     const int wg = (warp - 4) >> 2, t = threadIdx.x & 127;
     const uint64_t d_hi = gmma_desc_hi(8 * row_bytes, row_bytes);
-    const int ksteps = bk >> 4;
-    // this warpgroup's 64 rows start 64 rows into the A tile; advancing 16 bf16 along K = +32 bytes = +2 address units
+    const int ksteps = bk >> (sizeof(T) == 4 ? 3 : 4);   // 32-byte MMA K steps per K row
+    // this warpgroup's 64 rows start 64 rows into the A tile; one MMA K step (16 bf16 / fp16 or 8 fp32) = +32 bytes = +2
+    // address units
     const uint32_t stage16 = stage_bytes >> 4, a16 = a_bytes >> 4, wg16 = (uint32_t)wg * ((64 * row_bytes) >> 4);
     uint32_t s = 0, ph = 0, lo = desc_lo(smem_base);
     float acc[BN / 2];
@@ -165,15 +166,18 @@ __device__ __forceinline__ void tc_conv_body(const TcParams& p) {
 // host side
 // ------------------------------------------------------------------------------------------
 // kernel instance per (element type, epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared
-// memory.  [0] bf16, [1] fp16; rows: ragged (plain) stores, GEGLU, depth-to-space / depth-to-time shuffle.
+// memory.  [0] bf16, [1] fp16, [2] TF32; rows: ragged (plain) stores, GEGLU, depth-to-space / depth-to-time shuffle.
 // One kernel per element type (the names of the bf16 instances are those of the library before fp16 existed)
 template <int MODE, int BN>
 __global__ void __launch_bounds__(384, 1) tc_conv_kernel(const __grid_constant__ TcParams p) { tc_conv_body<__nv_bfloat16, MODE, BN>(p); }
 template <int MODE, int BN>
 __global__ void __launch_bounds__(384, 1) tc_conv_f16_kernel(const __grid_constant__ TcParams p) { tc_conv_body<__half, MODE, BN>(p); }
+template <int MODE, int BN>
+__global__ void __launch_bounds__(384, 1) tc_conv_tf32_kernel(const __grid_constant__ TcParams p) { tc_conv_body<float, MODE, BN>(p); }
 #define MV2_TC_BN(K, M) {K<M, 32>, K<M, 64>, K<M, 128>}
 #define MV2_TC_FLAVOURS(K) {MV2_TC_BN(K, EPI_RAGGED), MV2_TC_BN(K, EPI_GEGLU), MV2_TC_BN(K, EPI_SHUFFLE)}
-static void (*const g_tc_kernels[2][3][3])(TcParams) = {MV2_TC_FLAVOURS(tc_conv_kernel), MV2_TC_FLAVOURS(tc_conv_f16_kernel)};
+static void (*const g_tc_kernels[3][3][3])(TcParams) = {MV2_TC_FLAVOURS(tc_conv_kernel), MV2_TC_FLAVOURS(tc_conv_f16_kernel),
+                                                        MV2_TC_FLAVOURS(tc_conv_tf32_kernel)};
 #undef MV2_TC_FLAVOURS
 #undef MV2_TC_BN
 
@@ -200,7 +204,7 @@ int mv2_tc_conv_hist_supported(const mv2_tc_conv_args* a) {
 int mv2_tc_conv_supported(const mv2_tc_conv_args* a) {
   if (!a) return 0;
   if (tc_dtype(a) < 0) return 0;
-  if (a->Ci % 16 != 0) return 0;                    // TMA inner box = 32/64/128 B, global strides multiple of 16 B
+  if (a->Ci * tc_esize(tc_dtype(a)) % 32 != 0) return 0;   // TMA inner box = 32/64/128 B, global strides multiple of 16 B
   if (a->kt * a->kh * a->kw > TC_MAX_TAPS) return 0;
   if (a->st < 1 || a->st > 2 || a->sh < 1 || a->sh > 2 || a->sw < 1 || a->sw > 2) return 0;
   if (a->shuffle != MV2_SHUFFLE_NONE && ((a->shuffle == MV2_SHUFFLE_SPACE ? a->Co / 4 : a->Co / 2) % 8 != 0)) return 0;
@@ -219,11 +223,13 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, vo
   const int hist_T = hist ? hist->T_h : 0;
   if (!mv2_tc_conv_supported(a)) { set_error("mv2_tc_conv_forward: unsupported shape (Ci=%d Co=%d)", a->Ci, a->Co); return MV2_E_UNSUPPORTED; }
 
-  const int dt = tc_dtype(a);
+  const int dt = tc_dtype(a), es = tc_esize(dt);
   TcParams p;
   memset(&p, 0, sizeof(p));
-  const int bk = (a->Ci % 64 == 0) ? 64 : ((a->Ci % 32 == 0) ? 32 : 16);
-  const CUtensorMapSwizzle swz = swizzle_of_row(bk * 2);
+  const int ci_bytes = a->Ci * es;
+  const int row_bytes = ci_bytes % 128 == 0 ? 128 : (ci_bytes % 64 == 0 ? 64 : 32);   // one K row of the operand tiles
+  const int bk = row_bytes / es;
+  const CUtensorMapSwizzle swz = swizzle_of_row(row_bytes);
   p.bk = bk;
   p.ci_pad = a->Ci;
   p.kchunks = a->Ci / bk;
@@ -240,7 +246,6 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, vo
   // N tile: 32, 64 or 128 columns (a wgmma N, 64 fp32 accumulator registers per thread at 128); wider outputs take
   // several N tiles, a ragged last one reads zero-filled weight rows and stores nothing for them
   const int bn = a->Co <= 32 ? 32 : (a->Co <= 64 ? 64 : 128);
-  const int row_bytes = bk * 2;
   p.bn = bn;
   const int stage_bytes = TC_BM * row_bytes + bn * row_bytes;
   MV2_CHECK_ARG((TC_BM * row_bytes) % 1024 == 0 && (bn * row_bytes) % 1024 == 0);
@@ -264,19 +269,19 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, vo
         const int64_t nW = (W - pw + sw - 1) / sw, nH = (H - ph + sh - 1) / sh, nT = (T - pt + st - 1) / st;
         if (nW <= 0 || nH <= 0 || nT <= 0) { set_error("empty stride phase (dimension smaller than stride)"); return MV2_E_UNSUPPORTED; }
         const cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)nW, (cuuint64_t)nH, (cuuint64_t)nT, (cuuint64_t)a->B};
-        const cuuint64_t strides[4] = {(cuuint64_t)(sw * C * 2), (cuuint64_t)(sh * W * C * 2), (cuuint64_t)(st * H * W * C * 2),
-                                       (cuuint64_t)(T * H * W * C * 2)};
+        const cuuint64_t strides[4] = {(cuuint64_t)(sw * C * es), (cuuint64_t)(sh * W * C * es), (cuuint64_t)(st * H * W * C * es),
+                                       (cuuint64_t)(T * H * W * C * es)};
         const cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)p.bw, (cuuint32_t)p.bh, (cuuint32_t)(128 / (p.bw * p.bh * p.frame_loads)), 1};
-        const char* base = (const char*)a->x + ((int64_t)pt * H * W + (int64_t)ph * W + pw) * C * 2;
+        const char* base = (const char*)a->x + ((int64_t)pt * H * W + (int64_t)ph * W + pw) * C * es;
         char what[32];
         snprintf(what, sizeof(what), "activations, phase %d", id);
-        if (const int rc = encode_map16(&p.amap[id], dt, 5, base, dims, strides, box, swz, what)) return rc;
+        if (const int rc = encode_tc_map(&p.amap[id], dt, 5, base, dims, strides, box, swz, what)) return rc;
       }
   if (hist_T > 0) {
     const cuuint64_t dims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)hist_T, (cuuint64_t)a->B};
-    const cuuint64_t strides[4] = {(cuuint64_t)(C * 2), (cuuint64_t)(W * C * 2), (cuuint64_t)(H * W * C * 2), (cuuint64_t)(hist->clip_stride * 2)};
+    const cuuint64_t strides[4] = {(cuuint64_t)(C * es), (cuuint64_t)(W * C * es), (cuuint64_t)(H * W * C * es), (cuuint64_t)(hist->clip_stride * es)};
     const cuuint32_t box[5] = {(cuuint32_t)bk, (cuuint32_t)p.bw, (cuuint32_t)p.bh, 1, 1};
-    if (const int rc = encode_map16(&p.hmap, dt, 5, hist->h, dims, strides, box, swz, "history")) return rc;
+    if (const int rc = encode_tc_map(&p.hmap, dt, 5, hist->h, dims, strides, box, swz, "history")) return rc;
   }
   // ---- taps ----
   p.ntaps = a->kt * a->kh * a->kw;
@@ -294,9 +299,9 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, vo
   // ---- weights map: [Co][taps * Ci] K-major ----
   const int64_t K = (int64_t)p.ntaps * a->Ci;
   const cuuint64_t wdims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
-  const cuuint64_t wstrides[1] = {(cuuint64_t)(K * 2)};
+  const cuuint64_t wstrides[1] = {(cuuint64_t)(K * es)};
   const cuuint32_t wbox[2] = {(cuuint32_t)bk, (cuuint32_t)bn};
-  if (const int rc = encode_map16(&p.wmap, dt, 2, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
+  if (const int rc = encode_tc_map(&p.wmap, dt, 2, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
 
   const size_t smem = 1024 + (size_t)stages * stage_bytes + 16 * stages + 16 + (size_t)bn * 4 + stg_bytes;
   static PerDeviceOnce attr_once;
@@ -312,7 +317,7 @@ int mv2_tc_conv_forward(const mv2_tc_conv_args* a, const mv2_conv_hist* hist, vo
   MV2_CHECK_ARG(smem <= 227 * 1024);
   dim3 grid((unsigned)((int64_t)a->B * p.tt * p.th * p.tw), (unsigned)ceil_div(a->Co, bn));
   const int flavour = a->epi_mode == 1 ? 1 : (a->shuffle != MV2_SHUFFLE_NONE ? 2 : 0);   // row of g_tc_kernels
-  launch_k(g_tc_kernels[dt == MV2_F16][flavour][bn == 32 ? 0 : (bn == 64 ? 1 : 2)], grid, dim3(384), smem, (cudaStream_t)stream, p);
+  launch_k(g_tc_kernels[dt == MV2_F16 ? 1 : (dt == MV2_TF32 ? 2 : 0)][flavour][bn == 32 ? 0 : (bn == 64 ? 1 : 2)], grid, dim3(384), smem, (cudaStream_t)stream, p);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }

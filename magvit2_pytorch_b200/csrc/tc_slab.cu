@@ -1,6 +1,7 @@
 // wgmma / TMA "slab" implicit-GEMM kernel for stride-1 k_t x k_h x k_w convolutions (the causal 3x3x3 residual
-// convs carry most of the path's FLOPs), bf16 or fp16 in (the element type T is a template parameter
-// of every kernel) / fp32 accumulate in registers, persistent CTAs, sm_90a.
+// convs carry most of the path's FLOPs), bf16, fp16 or fp32 (TF32 multiply) in (the element type T is a template
+// parameter of every kernel) / fp32 accumulate in registers, persistent CTAs, sm_90a.  The host plans in bytes: a 128-byte
+// K row holds 64 bf16 / fp16 channels or 32 fp32 ones and takes the same four 32-byte MMA K steps.
 //
 // Why a second kernel: tc_conv.cu reloads the activation tile from L2 once per tap (27x) and the weight tile once per
 // 128 output positions.  Here
@@ -53,7 +54,7 @@ struct alignas(64) SlabParams {
   int slab_stages, w_stages;
   int tpw;               // in-plane taps per weight stage (one 3-D TMA box {bk, bn, tpw})
   TcEpi epi;
-  int dtype;             // host side: MV2_BF16 or MV2_F16, selects the kernel instance and the tensor maps' element type
+  int dtype;             // host side: MV2_BF16, MV2_F16 or MV2_TF32, selects the kernel instance and the tensor maps' element type
   // ---- EPI_FUSED_RU only (mv2_tc_ru_forward) ----
   CUtensorMap w1map;     // 1x1x1 weights [Co][Ci] as {ci, co}: 2-D boxes {64, bn}
   const float* bias1;    // 1x1x1 bias [C]
@@ -77,10 +78,11 @@ struct alignas(64) SlabParams {
 __host__ __device__ constexpr bool slab_tma_epi(int mode) {
   return mode == EPI_PLAIN || mode == EPI_PLAIN_RES || mode == EPI_GEGLU || mode == EPI_DOWN_SPACE;
 }
-// Channels of one output box of a TMA-store flavour with an N tile of bn columns: one 128-byte swizzled row (64
-// channels), or the whole tile when its output is narrower (GEGLU writes bn / 2 channels)
-__host__ __device__ constexpr int slab_out_box_ch(int mode, int bn) {
-  return (mode == EPI_GEGLU ? bn / 2 : bn) < 64 ? (mode == EPI_GEGLU ? bn / 2 : bn) : 64;
+// Channels of one output box of a TMA-store flavour with an N tile of bn columns and es-byte elements: one 128-byte
+// swizzled row (64 bf16 / fp16 or 32 fp32 channels), or the whole tile when its output is narrower (GEGLU writes bn / 2
+// channels)
+__host__ __device__ constexpr int slab_out_box_ch(int mode, int bn, int es) {
+  return (mode == EPI_GEGLU ? bn / 2 : bn) < 128 / es ? (mode == EPI_GEGLU ? bn / 2 : bn) : 128 / es;
 }
 
 // Frames are enumerated most-expensive first: the B * (T - pt) frames that see all kt frame taps, then the frames
@@ -122,14 +124,15 @@ __host__ __device__ __forceinline__ TileCoord decode_tile(const SlabParams& p, i
 // epilogue transpose buffers, the fp32 accumulator staging of both consumer warpgroups (mw M-tiles x 64 rows x (bn + 4)
 // each).
 // The TMA-store flavours use the span of the transpose buffers and the staging for other things: the residual
-// full / empty barriers of both warpgroups, then (1024-byte aligned, for the swizzled boxes) the bf16 output tiles and
-// the residual tiles of both warpgroups, 2 x mw x 64 x bn x 2 bytes each.  Together they take at most
-// 32 + 1023 + 512 mw bn bytes of the 16 KB + 512 mw (bn + 4) the span has, so the span, and with it every launch's
-// plan, is the same for all flavours but the fused one.
-// The fused ResidualUnit stages nothing: bias, logit partials, then (1024-byte aligned) the H buffer and the bf16 output
+// full / empty barriers of both warpgroups, then (1024-byte aligned, for the swizzled boxes) the output tiles and
+// the residual tiles of both warpgroups, 2 x mw x 64 x bn x es bytes each (es-byte elements).  With 16-bit elements
+// they take at most 32 + 1023 + 512 mw bn bytes of the 16 KB + 512 mw (bn + 4) the span has, so the span, and with it
+// every launch's plan, is the same for all flavours but the fused one.  fp32 tiles take twice that: the output tiles
+// still fit the span, the residual tiles (launches with a residual only) extend it.
+// The fused ResidualUnit stages nothing: bias, logit partials, then (1024-byte aligned) the H buffer and the output
 // tiles of both warpgroups.
 struct SlabSmem { uint32_t sbias, stage0, lpart, accstg, hbuf, end, rbar, otile, rtile; };
-__host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& p, uint32_t bar0, bool fused) {
+__host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& p, uint32_t bar0, bool fused, uint32_t es) {
   SlabSmem m = {};
   m.sbias = (bar0 + 8 * (2 * p.slab_stages + 2 * p.w_stages) + 15) & ~15u;
   m.stage0 = m.sbias + (uint32_t)(p.n_tiles_n * p.bn) * 4 * (fused ? 3 : 1);   // fused: [conv3 bias][conv1 bias][SE to_k weight]
@@ -137,14 +140,16 @@ __host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& 
     m.lpart = m.stage0;
     m.hbuf = (m.lpart + 2048 + 1023u) & ~1023u;          // SWIZZLE_128B tiles: 1024-byte aligned
     m.otile = m.hbuf + (uint32_t)p.h_stride;
-    m.end = m.otile + 2u * p.mw * 64 * p.bn * 2;
+    m.end = m.otile + 2u * p.mw * 64 * p.bn * es;
     return m;
   }
   m.accstg = m.stage0 + 8 * 2048;
   m.end = m.accstg + 2u * p.mw * 64 * (p.bn + 4) * 4;
   m.rbar = m.stage0;
   m.otile = (m.rbar + 32 + 1023u) & ~1023u;
-  m.rtile = m.otile + 2u * p.mw * 64 * p.bn * 2;
+  m.rtile = m.otile + 2u * p.mw * 64 * p.bn * es;
+  const uint32_t tiles_end = m.rtile + (p.epi.res ? 2u * p.mw * 64 * p.bn * es : 0u);   // residual tiles: EPI_PLAIN_RES only
+  if (tiles_end > m.end) m.end = tiles_end;
   return m;
 }
 
@@ -152,22 +157,27 @@ __host__ __device__ __forceinline__ SlabSmem slab_smem_layout(const SlabParams& 
 // (warp wq of the warpgroup, lane) holds rows m0 = 16 wq + lane / 4 and m0 + 8 of the M-tile (row m = output position
 // (h0 + 8 wg + m / 8, w0 + 8 j + m % 8)) and columns 8 g + 2 (lane % 4) + {0, 1}.  The math per element is that of the
 // staged epilogue, in the same order: x oscale, + bias and activation, [+ residual in fp32, x 2^-0.5 in mode 2], one
-// rounding to bf16; GEGLU pairs packed column 16 g + c (x) with 16 g + 8 + c (its gate), which the same thread holds.
-// Results go to `ot` as [boxes][64 rows][cb channels] 16-bit boxes in the swizzle TMA uses for their row width; the
+// rounding to bf16 / fp16 (fp32 is stored as computed); GEGLU pairs packed column 16 g + c (x) with 16 g + 8 + c (its
+// gate), which the same thread holds.
+// Results go to `ot` as [boxes][64 rows][cb channels] boxes of T in the swizzle TMA uses for their row width; the
 // residual is read from `rt` in the same layout.  Bank-conflict free: the 8 rows of a warp's access fall on 8 different
 // 16-byte units of the swizzle.  With 128-byte rows this is also the layout of a K-major SWIZZLE_128B wgmma operand of
 // 64 rows (one 8 KB K-chunk per box), which the fused ResidualUnit's second GEMM reads.
 template <typename T, int MODE, int BN, int ACT>
 __device__ __forceinline__ void slab_epi_mtile(const SlabParams& p, const float (&acc)[BN / 2], const TileCoord& c,
                                                const float* sbias, uint32_t ot, uint32_t rt, int wq, int lane, bool relu) {
-  constexpr int CB = slab_out_box_ch(MODE, BN);
-  constexpr uint32_t RB = CB * 2, BOX = 64 * RB, SWZ = (RB / 16 - 1) << 4;
-  const uint32_t m0 = 16 * wq + (lane >> 2), q4 = (lane & 3) * 4;
+  constexpr int ES = sizeof(T);
+  constexpr int CB = slab_out_box_ch(MODE, BN, ES);
+  constexpr uint32_t RB = CB * ES, BOX = 64 * RB, SWZ = (RB / 16 - 1) << 4;
+  const uint32_t m0 = 16 * wq + (lane >> 2), q4 = (lane & 3) * 2 * ES;
   auto at = [&](int col, uint32_t m) {               // byte offset of (row m, output columns col, col + 1)
-    const uint32_t off = m * RB + (uint32_t)(col % CB) * 2 + q4;
+    const uint32_t off = m * RB + (uint32_t)(col % CB) * ES + q4;
     return (uint32_t)(col / CB) * BOX + (off ^ ((off >> 3) & SWZ));
   };
-  auto st32 = [](uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); };
+  auto st2 = [](uint32_t a, float v0, float v1) {   // two adjacent output columns
+    if constexpr (ES == 4) asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v0), "f"(v1) : "memory");
+    else asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(pack2<T>(v0, v1)) : "memory");
+  };
   const float* os = (MODE == EPI_PLAIN || MODE == EPI_PLAIN_RES) && p.epi.oscale ? p.epi.oscale + (int64_t)c.b * p.Co : nullptr;
   const float rs = MODE == EPI_PLAIN_RES && p.epi.mode == 2 ? 0.70710678118654752440f : 1.f;
   if (MODE == EPI_GEGLU) {
@@ -181,7 +191,7 @@ __device__ __forceinline__ void slab_epi_mtile(const SlabParams& p, const float 
         const float* gv = &acc[8 * g + 4 + 2 * hr];
         const float v0 = gelu_fast(gv[0] + bg.x) * (xv[0] + bx.x);
         const float v1 = gelu_fast(gv[1] + bg.y) * (xv[1] + bx.y);
-        st32(ot + at(8 * g, m0 + 8 * hr), pack2<T>(v0, v1));
+        st2(ot + at(8 * g, m0 + 8 * hr), v0, v1);
       }
     }
   } else {
@@ -199,13 +209,18 @@ __device__ __forceinline__ void slab_epi_mtile(const SlabParams& p, const float 
         v1 = act_ct<ACT>(v1 + b.y, relu);
         const uint32_t a = at(col, m0 + 8 * hr);
         if (MODE == EPI_PLAIN_RES) {
-          uint32_t r;
-          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(rt + a) : "memory");
-          const float2 rf = unpack2<T>(r);
+          float2 rf;
+          if constexpr (ES == 4) {
+            asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(rf.x), "=f"(rf.y) : "r"(rt + a) : "memory");
+          } else {
+            uint32_t r;
+            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(rt + a) : "memory");
+            rf = unpack2<T>(r);
+          }
           v0 = (v0 + rf.x) * rs;
           v1 = (v1 + rf.y) * rs;
         }
-        st32(ot + a, pack2<T>(v0, v1));
+        st2(ot + a, v0, v1);
       }
     }
   }
@@ -214,7 +229,7 @@ __device__ __forceinline__ void slab_epi_mtile(const SlabParams& p, const float 
 template <typename T, int MODE, int BN, int ACT, int MWMAX>
 __device__ __forceinline__ void slab_epi_fragment(const SlabParams& p, const float (&acc)[MWMAX][BN / 2], const TileCoord& c,
                                                   const float* sbias, uint32_t ot, uint32_t rt, int wq, int lane, bool relu) {
-  constexpr uint32_t MTILE = (MODE == EPI_GEGLU ? BN / 2 : BN) * 64 * 2;   // bytes of one M-tile's boxes
+  constexpr uint32_t MTILE = (MODE == EPI_GEGLU ? BN / 2 : BN) * 64 * (int)sizeof(T);   // bytes of one M-tile's boxes
 #pragma unroll
   for (int j = 0; j < MWMAX; ++j) {
     if (j >= p.mw) break;
@@ -238,8 +253,8 @@ __device__ __forceinline__ void tc_slab_body(const SlabParams& p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t row_bytes = p.row_bytes;          // 128 (64 channels, SWIZZLE_128B) or 64 (32 channels, SWIZZLE_64B)
-  const uint32_t bk = row_bytes >> 1;
+  const uint32_t row_bytes = p.row_bytes;          // 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B)
+  const uint32_t bk = row_bytes / (uint32_t)sizeof(T);   // channels of one K row
   const uint32_t w_tile = p.bn * row_bytes;          // one tap's weight tile
   const uint32_t w_bytes = w_tile * p.tpw;           // one ring stage = tpw consecutive in-plane taps
   const uint32_t slab0 = smem_base;
@@ -248,7 +263,7 @@ __device__ __forceinline__ void tc_slab_body(const SlabParams& p) {
   // barrier table (8 bytes each)
   const uint32_t slab_full = bar0, slab_empty = slab_full + 8 * p.slab_stages;
   const uint32_t w_full = slab_empty + 8 * p.slab_stages, w_empty = w_full + 8 * p.w_stages;
-  const SlabSmem L = slab_smem_layout(p, bar0, MODE == EPI_FUSED_RU);
+  const SlabSmem L = slab_smem_layout(p, bar0, MODE == EPI_FUSED_RU, (uint32_t)sizeof(T));
   auto gen = [&](uint32_t u) { return smem_raw + (u - smem_u32(smem_raw)); };
   float* sbias = reinterpret_cast<float*>(gen(L.sbias));   // padded Co floats, 16-byte aligned
   const uint32_t nbias = (uint32_t)(p.n_tiles_n * p.bn);
@@ -336,22 +351,23 @@ __device__ __forceinline__ void tc_slab_body(const SlabParams& p) {
       // loads the boxes of a tile's residual that hold output positions and channels (the boxes of slab_epi_fragment)
       // as soon as the warpgroup has read the previous tile's, so that they arrive under the tile's main loop
       if (MODE == EPI_PLAIN_RES && lane == 0) {
-        constexpr int CB = slab_out_box_ch(MODE, BN), NB = BN / CB;
+        constexpr int CB = slab_out_box_ch(MODE, BN, sizeof(T)), NB = BN / CB;
+        constexpr uint32_t BOX = 64 * CB * (uint32_t)sizeof(T);
         uint32_t ph = 0;
         for (int tk = 0, tile; (tile = slab_tile_of(p, tk)) >= 0; ++tk) {
           const TileCoord c = decode_tile(p, tile);
           for (int g = 0; g < 2; ++g) {
-            const uint32_t rt = L.rtile + (uint32_t)(g * p.mw * NB) * 64 * CB * 2;
+            const uint32_t rt = L.rtile + (uint32_t)(g * p.mw * NB) * BOX;
             const int h = c.h0 + 8 * g;
             int nbox = 0;
             for (int j = 0; j < p.mw; ++j)
               for (int b = 0; b < NB; ++b) nbox += h < p.H && c.w0 + 8 * j < p.W && c.n0 + b * CB < p.Co;
             mbar_wait(L.rbar + 16 + 8 * g, ph ^ 1);
-            mbar_expect_tx(L.rbar + 8 * g, (uint32_t)nbox * 64 * CB * 2);
+            mbar_expect_tx(L.rbar + 8 * g, (uint32_t)nbox * BOX);
             for (int j = 0; j < p.mw; ++j)
               for (int b = 0; b < NB; ++b)
                 if (h < p.H && c.w0 + 8 * j < p.W && c.n0 + b * CB < p.Co)
-                  tma_load_5d(rt + (uint32_t)(j * NB + b) * 64 * CB * 2, &p.rmap, L.rbar + 8 * g, c.n0 + b * CB, c.w0 + 8 * j, h, c.t, c.b);
+                  tma_load_5d(rt + (uint32_t)(j * NB + b) * BOX, &p.rmap, L.rbar + 8 * g, c.n0 + b * CB, c.w0 + 8 * j, h, c.t, c.b);
           }
           ph ^= 1;
         }
@@ -414,7 +430,7 @@ __device__ __forceinline__ void tc_slab_body(const SlabParams& p) {
     const uint32_t sbo = (uint32_t)p.pitch * row_bytes;
     const uint64_t a_hi = gmma_desc_hi(sbo, row_bytes);
     const uint64_t b_hi = gmma_desc_hi(8 * row_bytes, row_bytes);
-    const bool k4 = bk == 64;
+    const bool k4 = row_bytes == 128;
     // All ring bookkeeping is incremental (stage index, parity, descriptor low words).
     const uint32_t a_row = row_bytes >> 4;                       // descriptor-address units per slab row
     const uint32_t a_wg = (uint32_t)wg * 8 * (sbo >> 4);         // this warpgroup's first output row: 8 slab rows (h) down
@@ -530,10 +546,10 @@ __device__ __forceinline__ void tc_slab_body(const SlabParams& p) {
       else if (MWMAX >= 2 && p.mw == 2) mainloop_k(c, std::integral_constant<int, (MWMAX >= 2 ? 2 : 1)>());
       else mainloop_k(c, std::integral_constant<int, 1>());
       if (slab_tma_epi(MODE)) {
-        // ---- register epilogue: 16-bit results -> this warpgroup's output tile -> TMA box stores ----
-        constexpr int CB = slab_out_box_ch(MODE, BN), NB = (MODE == EPI_GEGLU ? BN / 2 : BN) / CB;
-        constexpr uint32_t BOX = 64 * CB * 2;
-        const uint32_t ot = L.otile + (uint32_t)(wg * p.mw * NB) * BOX, rt = L.rtile + (uint32_t)(wg * p.mw) * 64 * BN * 2;
+        // ---- register epilogue: results -> this warpgroup's output tile -> TMA box stores ----
+        constexpr int CB = slab_out_box_ch(MODE, BN, sizeof(T)), NB = (MODE == EPI_GEGLU ? BN / 2 : BN) / CB;
+        constexpr uint32_t BOX = 64 * CB * (uint32_t)sizeof(T);
+        const uint32_t ot = L.otile + (uint32_t)(wg * p.mw * NB) * BOX, rt = L.rtile + (uint32_t)(wg * p.mw) * 64 * BN * (uint32_t)sizeof(T);
         if (tid == 0) bulk_wait_read_all();     // the previous tile's stores have read the output tile
         named_bar_sync(wg_bar, 128);
         if (MODE == EPI_PLAIN_RES) mbar_wait(L.rbar + 8 * wg, r_par);
@@ -562,13 +578,14 @@ __device__ __forceinline__ void tc_slab_body(const SlabParams& p) {
         }
         continue;
       }
-      if (MODE == EPI_FUSED_RU) {
+      if constexpr (MODE == EPI_FUSED_RU) {
         // ---------------- fused ResidualUnit epilogue (reference M:937-941 + the pooling half of M:229-233), per M-tile j
         //      on the accumulator fragments: E1 writes h = bf16(ELU(conv3 + b3)) into the H buffer, the A operand of the
         //      1x1x1 GEMM; E2 writes y = bf16(ELU(conv1 + b1)) into this warpgroup's output tile, TMA stores it and the
         //      SE pooling reads it back.  H and the output tiles are laid out as slab_epi_mtile writes them (bn = C = 64 |
         //      128: 128-byte rows, one 8 KB box per 64 channels); each warpgroup has its own 64 rows of both ----------------
-        constexpr int CB = slab_out_box_ch(MODE, BN), NB = BN / CB;
+        static_assert(sizeof(T) == 2, "the fused ResidualUnit has 16-bit instances only");
+        constexpr int CB = slab_out_box_ch(MODE, BN, 2), NB = BN / CB;
         constexpr uint32_t BOX = 64 * CB * 2;
         const float* sb1 = sbias + nbias;
         const float* swk = sbias + 2 * nbias;
@@ -737,7 +754,8 @@ __device__ __forceinline__ void tc_slab_body(const SlabParams& p) {
         const float* srow = stg + (j * 64 + row - 64 * wg) * (BN + 4);
         const int64_t row_base = ((((int64_t)c.b * p.T + c.t) * p.H + h) * p.W + w) * p.Co;
         // column chunks are dealt round-robin to the two warps that share this lane quarter
-        if (MODE == EPI_SHUFFLE_ST) {
+        if constexpr (MODE == EPI_SHUFFLE_ST) {
+          static_assert(sizeof(T) == 2, "the transposed shuffle stores have 16-bit instances only");
           // Row-per-lane results are transposed through shared memory so that every store instruction writes 8 rows
           // x 64 contiguous bytes (full sectors; the 8 rows are neighbours along w) instead of 32 scattered 16-byte pieces.
           const uint32_t stg = stage0 + (uint32_t)ew * 2048;
@@ -799,6 +817,8 @@ template <int MODE, int BN>
 __global__ void __launch_bounds__(384, 1) tc_slab_kernel(const __grid_constant__ SlabParams p) { tc_slab_body<__nv_bfloat16, MODE, BN>(p); }
 template <int MODE, int BN>
 __global__ void __launch_bounds__(384, 1) tc_slab_f16_kernel(const __grid_constant__ SlabParams p) { tc_slab_body<__half, MODE, BN>(p); }
+template <int MODE, int BN>
+__global__ void __launch_bounds__(384, 1) tc_slab_tf32_kernel(const __grid_constant__ SlabParams p) { tc_slab_body<float, MODE, BN>(p); }
 
 }  // namespace mv2
 
@@ -811,18 +831,19 @@ static bool slab_narrow(const mv2_tc_conv_args* a) { return a->out_layout == 1 &
 
 extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
   if (!a || tc_dtype(a) < 0) return 0;
+  const int ci_bytes = a->Ci * tc_esize(tc_dtype(a));      // bytes of one position's input channels
   if (a->sh != 1 || a->sw != 1) return 0;
   if (a->st != 1) {      // TimeDownsample2x (M:796-807): stride 2 along t only, plain epilogue
     if (a->st != 2 || a->out_layout != 0 || a->epi_mode != 0 || a->shuffle != MV2_SHUFFLE_NONE) return 0;
     if (a->To != (a->Ti + a->pt - a->kt) / a->st + 1 || a->To < 1) return 0;
   }
-  if (a->Ci % 32 != 0 || a->Co > 4096) return 0;
+  if (ci_bytes % 64 != 0 || a->Co > 4096) return 0;
   if (a->oscale && (a->epi_mode != 0 || a->shuffle != MV2_SHUFFLE_NONE)) return 0;   // demodulation: plain / ragged epilogues only
   if (a->epi_mode == 1 && (a->Co % 64 != 0 || a->shuffle != MV2_SHUFFLE_NONE || a->res)) return 0;   // fused GEGLU (64-column epilogue chunks)
   if (a->epi_mode == 2 && (!a->res || a->shuffle != MV2_SHUFFLE_NONE)) return 0;   // scaled residual
   if (a->epi_mode < 0 || a->epi_mode > 2) return 0;
   if (a->Co % 32 != 0 && a->Co > 32) return 0;           // ragged N only as a single (zero padded) 32-column tile
-  if (a->Ci % 64 != 0 && a->kw != 1) return 0;           // 64-byte rows (32 channels): only h-shifted taps (1024 B multiples)
+  if (ci_bytes % 128 != 0 && a->kw != 1) return 0;       // 64-byte rows: only h-shifted taps (1024 B multiples)
   if (a->res && a->Co % 8 != 0) return 0;
   if (a->shuffle != MV2_SHUFFLE_NONE && ((a->shuffle == MV2_SHUFFLE_SPACE ? a->Co / 4 : a->Co / 2) % 8 != 0 || a->Co % 32 != 0)) return 0;
   if (a->kh > 7 || a->kw > (slab_narrow(a) ? 7 : 3) || a->kt > 8) return 0;
@@ -843,12 +864,12 @@ extern "C" int mv2_tc_slab_supported(const mv2_tc_conv_args* a) {
 static int slab_ring_budget(const SlabParams& p, bool fused) {
   SlabParams q = p;
   q.slab_stages = 3; q.w_stages = 12;      // upper bounds for the barrier table
-  return 227 * 1024 - 2048 - (int)slab_smem_layout(q, 0, fused).end;
+  return 227 * 1024 - 2048 - (int)slab_smem_layout(q, 0, fused, tc_esize(p.dtype)).end;
 }
 // Dynamic shared memory of a launch: alignment slack, the slab and weight rings, then slab_smem_layout
 static size_t slab_smem_bytes(const SlabParams& p, bool fused) {
   const uint32_t rings = (uint32_t)(p.slab_stages * p.slab_stride + p.w_stages * p.bn * p.row_bytes * p.tpw);
-  return 1024 + slab_smem_layout(p, rings, fused).end;
+  return 1024 + slab_smem_layout(p, rings, fused, tc_esize(p.dtype)).end;
 }
 // M-tiles side by side per weight tile: as many as the frame width uses, while their accumulators fit 64 fp32 registers
 // per consumer thread (mw * bn <= 128); this divides the weight traffic by mw
@@ -870,11 +891,12 @@ static int slab_fill_plan(const mv2_tc_conv_args* a, SlabParams& p) {
   memset(&p, 0, sizeof(p));
   p.kt = a->kt; p.kh = a->kh; p.kw = a->kw; p.pt = a->pt; p.ph = a->ph; p.pw = a->pw;
   p.st = a->st;
-  p.row_bytes = (a->Ci % 64 == 0) ? 128 : 64;
-  p.Ci = a->Ci; p.kchunks = a->Ci / (p.row_bytes / 2);
+  p.dtype = tc_dtype(a);
+  const int ci_bytes = a->Ci * tc_esize(p.dtype);
+  p.row_bytes = ci_bytes % 128 == 0 ? 128 : 64;
+  p.Ci = a->Ci; p.kchunks = ci_bytes / p.row_bytes;
   p.B = a->B; p.T = a->To; p.H = a->Ho; p.W = a->Wo; p.Co = a->Co;
   p.epi = tc_epi_of(a);
-  p.dtype = tc_dtype(a);
 
   // ---- tiling: widest N tile (<= 128 columns), then as many M-tiles per weight tile as slab_default_mw allows ----
   const int co_pad = (a->Co + 31) / 32 * 32;
@@ -922,51 +944,59 @@ static int slab_fill_plan(const mv2_tc_conv_args* a, SlabParams& p) {
 // weights [Co][tap][Ci] as {ci, co, tap} (box {bk, bn, tpw}: tpw consecutive K-major tiles) and as {k, co} (box {bk, bn}).
 static int slab_encode_maps(SlabParams& p, const mv2_tc_conv_args* a, const mv2_conv_hist* hist = nullptr) {
   const CUtensorMapSwizzle swz = swizzle_of_row(p.row_bytes);
+  const int es = tc_esize(p.dtype);
   const int64_t C = a->Ci, W = a->Wi, H = a->Hi, T = a->Ti;
   const cuuint64_t xdims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)T, (cuuint64_t)a->B};
-  const cuuint64_t xstrides[4] = {(cuuint64_t)(C * 2), (cuuint64_t)(W * C * 2), (cuuint64_t)(H * W * C * 2), (cuuint64_t)(T * H * W * C * 2)};
-  const cuuint32_t xbox[5] = {(cuuint32_t)p.row_bytes / 2, (cuuint32_t)p.pitch, (cuuint32_t)p.slab_h, 1, 1};
-  if (const int rc = encode_map16(&p.amap, p.dtype, 5, a->x, xdims, xstrides, xbox, swz, "slab")) return rc;
+  const cuuint64_t xstrides[4] = {(cuuint64_t)(C * es), (cuuint64_t)(W * C * es), (cuuint64_t)(H * W * C * es), (cuuint64_t)(T * H * W * C * es)};
+  const cuuint32_t xbox[5] = {(cuuint32_t)(p.row_bytes / es), (cuuint32_t)p.pitch, (cuuint32_t)p.slab_h, 1, 1};
+  if (const int rc = encode_tc_map(&p.amap, p.dtype, 5, a->x, xdims, xstrides, xbox, swz, "slab")) return rc;
   p.hist_T = hist ? hist->T_h : 0;
   if (p.hist_T > 0) {     // the same boxes over the history: (T_h frames, clip stride of the tensor it lives in)
     const cuuint64_t hdims[5] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)p.hist_T, (cuuint64_t)a->B};
-    const cuuint64_t hstrides[4] = {xstrides[0], xstrides[1], xstrides[2], (cuuint64_t)(hist->clip_stride * 2)};
-    if (const int rc = encode_map16(&p.hmap, p.dtype, 5, hist->h, hdims, hstrides, xbox, swz, "history")) return rc;
+    const cuuint64_t hstrides[4] = {xstrides[0], xstrides[1], xstrides[2], (cuuint64_t)(hist->clip_stride * es)};
+    if (const int rc = encode_tc_map(&p.hmap, p.dtype, 5, hist->h, hdims, hstrides, xbox, swz, "history")) return rc;
   }
   const int64_t ntaps = (int64_t)a->kt * a->kh * a->kw, K = ntaps * C;
   const cuuint64_t wdims[3] = {(cuuint64_t)C, (cuuint64_t)a->Co, (cuuint64_t)ntaps}, kdims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
-  const cuuint64_t wstrides[2] = {(cuuint64_t)(K * 2), (cuuint64_t)(C * 2)};
-  const cuuint32_t wbox[3] = {(cuuint32_t)p.row_bytes / 2, (cuuint32_t)p.bn, (cuuint32_t)p.tpw};
-  if (const int rc = encode_map16(&p.wmap, p.dtype, 3, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
-  return encode_map16(&p.wmap2, p.dtype, 2, a->w, kdims, wstrides, wbox, swz, "weights 2-D");
+  const cuuint64_t wstrides[2] = {(cuuint64_t)(K * es), (cuuint64_t)(C * es)};
+  const cuuint32_t wbox[3] = {(cuuint32_t)(p.row_bytes / es), (cuuint32_t)p.bn, (cuuint32_t)p.tpw};
+  if (const int rc = encode_tc_map(&p.wmap, p.dtype, 3, a->w, wdims, wstrides, wbox, swz, "weights")) return rc;
+  return encode_tc_map(&p.wmap2, p.dtype, 2, a->w, kdims, wstrides, wbox, swz, "weights 2-D");
 }
 // Output (and residual) maps of the TMA-store flavours: y as {oc, W, H, T, B} (oc = Co, or Co / 2 for GEGLU), boxes of
 // slab_out_box_ch channels x 8 (w) x 8 (h) in the swizzle of their row width
 static int slab_encode_out_maps(SlabParams& p, int mode) {
-  const int cb = slab_out_box_ch(mode, p.bn);
+  const int es = tc_esize(p.dtype);
+  const int cb = slab_out_box_ch(mode, p.bn, es);
   const int64_t oc = mode == EPI_GEGLU ? p.Co / 2 : p.Co;
   const cuuint64_t dims[5] = {(cuuint64_t)oc, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.T, (cuuint64_t)p.B};
-  const cuuint64_t strides[4] = {(cuuint64_t)(oc * 2), (cuuint64_t)(p.W * oc * 2), (cuuint64_t)(p.H * p.W * oc * 2),
-                                 (cuuint64_t)(p.T * p.H * p.W * oc * 2)};
+  const cuuint64_t strides[4] = {(cuuint64_t)(oc * es), (cuuint64_t)(p.W * oc * es), (cuuint64_t)(p.H * p.W * oc * es),
+                                 (cuuint64_t)(p.T * p.H * p.W * oc * es)};
   const cuuint32_t box[5] = {(cuuint32_t)cb, 8, 8, 1, 1};
-  const CUtensorMapSwizzle swz = swizzle_of_row(cb * 2);
-  if (const int rc = encode_map16(&p.ymap, p.dtype, 5, p.epi.y, dims, strides, box, swz, "output")) return rc;
+  const CUtensorMapSwizzle swz = swizzle_of_row(cb * es);
+  if (const int rc = encode_tc_map(&p.ymap, p.dtype, 5, p.epi.y, dims, strides, box, swz, "output")) return rc;
   if (mode != EPI_PLAIN_RES) return MV2_OK;
-  return encode_map16(&p.rmap, p.dtype, 5, p.epi.res, dims, strides, box, swz, "residual");
+  return encode_tc_map(&p.rmap, p.dtype, 5, p.epi.res, dims, strides, box, swz, "residual");
 }
 
 // Launches one slab-kernel flavour: persistent CTAs, one per SM of the current device (fewer when there are fewer tiles)
 static int slab_launch(int mode, const SlabParams& p, void* stream) {
   // kernel instance per (epilogue flavour, N tile); every instance may use up to 227 KB of dynamic shared memory.  The
   // channels-first flavour EPI_RAGGED (< 32 channels) has the 32-column tile and the narrow 16- and 8-column ones.
-  // [0] bf16, [1] fp16.
+  // [0] bf16, [1] fp16, [2] TF32, which has no fused ResidualUnit and no transposed shuffle stores (null: never chosen).
 #define MV2_SLAB_BN(K, M) {K<M, 32>, K<M, 64>, K<M, 128>}
-#define MV2_SLAB_FLAVOURS(K)                                                                                             \
+#define MV2_SLAB_NONE {nullptr, nullptr, nullptr}
+#define MV2_SLAB_FLAVOURS(K, FUSED_RU, SHUFFLE_ST)                                                                       \
   {MV2_SLAB_BN(K, EPI_PLAIN), MV2_SLAB_BN(K, EPI_GEGLU), MV2_SLAB_BN(K, EPI_SHUFFLE),                                 \
    {K<EPI_RAGGED, 32>, K<EPI_RAGGED, 16>, K<EPI_RAGGED, 8>},                                                           \
-   MV2_SLAB_BN(K, EPI_PLAIN_RES), MV2_SLAB_BN(K, EPI_FUSED_RU), MV2_SLAB_BN(K, EPI_SHUFFLE_ST), MV2_SLAB_BN(K, EPI_DOWN_SPACE)}
-  static void (*const kernels[2][8][3])(SlabParams) = {MV2_SLAB_FLAVOURS(tc_slab_kernel), MV2_SLAB_FLAVOURS(tc_slab_f16_kernel)};
+   MV2_SLAB_BN(K, EPI_PLAIN_RES), FUSED_RU, SHUFFLE_ST, MV2_SLAB_BN(K, EPI_DOWN_SPACE)}
+  static void (*const kernels[3][8][3])(SlabParams) = {
+      MV2_SLAB_FLAVOURS(tc_slab_kernel, MV2_SLAB_BN(tc_slab_kernel, EPI_FUSED_RU), MV2_SLAB_BN(tc_slab_kernel, EPI_SHUFFLE_ST)),
+      MV2_SLAB_FLAVOURS(tc_slab_f16_kernel, MV2_SLAB_BN(tc_slab_f16_kernel, EPI_FUSED_RU),
+                        MV2_SLAB_BN(tc_slab_f16_kernel, EPI_SHUFFLE_ST)),
+      MV2_SLAB_FLAVOURS(tc_slab_tf32_kernel, MV2_SLAB_NONE, MV2_SLAB_NONE)};
 #undef MV2_SLAB_FLAVOURS
+#undef MV2_SLAB_NONE
 #undef MV2_SLAB_BN
   static PerDeviceOnce attr_once;
   const cudaError_t attr_err = attr_once.run([] {
@@ -974,7 +1004,7 @@ static int slab_launch(int mode, const SlabParams& p, void* stream) {
     for (auto& type : kernels)
       for (auto& row : type)
         for (auto k : row)
-          if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+          if (e == cudaSuccess && k) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     return e;
   });
   if (attr_err != cudaSuccess) { set_error("cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err)); return MV2_E_CUDA; }
@@ -985,8 +1015,9 @@ static int slab_launch(int mode, const SlabParams& p, void* stream) {
   cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
   MV2_CHECK_ARG(p.bn >= 32 || mode == EPI_RAGGED);
   const int slot = p.bn == 32 ? 0 : (p.bn == 64 || p.bn == 16 ? 1 : 2);
-  launch_k(kernels[p.dtype == MV2_F16][mode][slot], dim3(std::min(p.total_tiles, n_sm)), dim3(384), smem,
-           (cudaStream_t)stream, p);
+  const auto kernel = kernels[p.dtype == MV2_F16 ? 1 : (p.dtype == MV2_TF32 ? 2 : 0)][mode][slot];
+  MV2_CHECK_ARG(kernel != nullptr);
+  launch_k(kernel, dim3(std::min(p.total_tiles, n_sm)), dim3(384), smem, (cudaStream_t)stream, p);
   MV2_CHECK_LAUNCH();
   return MV2_OK;
 }
@@ -1026,7 +1057,8 @@ extern "C" int mv2_tc_slab_forward(const mv2_tc_conv_args* a, const mv2_conv_his
   if (const int rc = slab_encode_maps(p, a, hist)) return rc;
   int mode = EPI_PLAIN;
   if (a->epi_mode == 1) mode = EPI_GEGLU;
-  else if (a->shuffle != MV2_SHUFFLE_NONE && (a->Co / (a->shuffle == MV2_SHUFFLE_SPACE ? 4 : 2)) % 32 == 0) mode = EPI_SHUFFLE_ST;
+  else if (a->shuffle != MV2_SHUFFLE_NONE && (a->Co / (a->shuffle == MV2_SHUFFLE_SPACE ? 4 : 2)) % 32 == 0 && p.dtype != MV2_TF32)
+    mode = EPI_SHUFFLE_ST;     // TF32: a 32-column chunk of fp32 is 128 bytes per row, twice a transpose buffer's rows
   else if (a->shuffle != MV2_SHUFFLE_NONE) mode = EPI_SHUFFLE;
   else if (a->Co % 8 != 0) mode = EPI_RAGGED;
   else if (a->res) mode = EPI_PLAIN_RES;
@@ -1051,6 +1083,7 @@ static void ru_as_conv_args(const mv2_tc_ru_args* a, mv2_tc_conv_args* c) {
 
 extern "C" int mv2_tc_ru_supported(const mv2_tc_ru_args* a) {
   if (!a) return 0;
+  if (tc_dtype_of(a->dtype) == MV2_TF32) return 0;     // 16-bit only: TF32 units take the unfused convs (DESIGN.md)
   if (a->C != 64 && a->C != 128) return 0;            // all of Co in one N tile (bn = C)
   if (a->W <= 8) return 0;                            // narrow frames take the unfused path
   if (a->kt < 1 || a->kt > 8 || a->kh < 1 || a->kh > 7 || a->kw < 1 || a->kw > 3) return 0;
@@ -1105,7 +1138,7 @@ extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, const mv2_conv_hist* h
   const cuuint64_t dims1[2] = {(cuuint64_t)a->C, (cuuint64_t)a->C};
   const cuuint64_t strides1[1] = {(cuuint64_t)a->C * 2};
   const cuuint32_t box1[2] = {64, (cuuint32_t)p.bn};
-  if (const int rc = encode_map16(&p.w1map, p.dtype, 2, a->w1, dims1, strides1, box1, CU_TENSOR_MAP_SWIZZLE_128B, "w1")) return rc;
+  if (const int rc = encode_tc_map(&p.w1map, p.dtype, 2, a->w1, dims1, strides1, box1, CU_TENSOR_MAP_SWIZZLE_128B, "w1")) return rc;
   if (const int rc = slab_encode_out_maps(p, EPI_FUSED_RU)) return rc;
   return slab_launch(EPI_FUSED_RU, p, stream);
 }
@@ -1122,10 +1155,11 @@ extern "C" int mv2_tc_ru_forward(const mv2_tc_ru_args* a, const mv2_conv_hist* h
 // =====================================================================================================================
 extern "C" int mv2_tc_down_space_supported(const mv2_tc_conv_args* a) {
   if (!a || tc_dtype(a) < 0) return 0;
+  const int es = tc_esize(tc_dtype(a));
   if (a->kt != 1 || a->kh != 3 || a->kw != 3 || a->st != 1 || a->sh != 2 || a->sw != 2) return 0;
   if (a->pt != 0 || a->ph != 1 || a->pw != 1) return 0;
   if ((a->Hi & 1) || (a->Wi & 1) || a->Ho != a->Hi / 2 || a->Wo != a->Wi / 2 || a->To != a->Ti) return 0;
-  if (a->Ci % 64 != 0 || a->Co % 32 != 0 || a->Co > 4096) return 0;
+  if ((a->Ci * es) % 128 != 0 || a->Co % 32 != 0 || a->Co > 4096) return 0;    // 128-byte K rows
   if (a->res || a->shuffle != MV2_SHUFFLE_NONE || a->epi_mode != 0 || a->out_layout != 0 || a->oscale) return 0;
   return 1;
 }
@@ -1135,12 +1169,13 @@ extern "C" int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream
   if (!mv2_tc_down_space_supported(a)) { set_error("mv2_tc_down_space_forward: unsupported shape"); return MV2_E_UNSUPPORTED; }
   SlabParams p;
   memset(&p, 0, sizeof(p));
-  const int C2 = 2 * a->Ci, bk = 64;
+  p.dtype = tc_dtype(a);
+  const int es = tc_esize(p.dtype);
+  const int C2 = 2 * a->Ci, bk = 128 / es;     // channels of one 128-byte K row
   p.kt = 1; p.kh = 3; p.kw = 2; p.pt = 0; p.ph = 1; p.pw = 1; p.st = 1;
   p.row_bytes = 128; p.Ci = C2; p.kchunks = C2 / bk; p.dn_lower = a->Ci / bk;
   p.B = a->B; p.T = a->To; p.H = a->Ho; p.W = a->Wo; p.Co = a->Co;
   p.epi = tc_epi_of(a);
-  p.dtype = tc_dtype(a);
   int bn = 32;
   for (int c = 128; c >= 32; c >>= 1) if (a->Co % c == 0) { bn = c; break; }
   const int w_bytes = bn * 128;
@@ -1164,17 +1199,17 @@ extern "C" int mv2_tc_down_space_forward(const mv2_tc_conv_args* a, void* stream
   p.w_stages = std::min(12, (budget - p.slab_stages * p.slab_stride) / w_bytes);
   MV2_CHECK_ARG(p.w_stages >= 2);
 
-  const int64_t rowb = (int64_t)a->Wi * a->Ci * 2;
+  const int64_t rowb = (int64_t)a->Wi * a->Ci * es;
   const cuuint64_t dims[5] = {(cuuint64_t)C2, (cuuint64_t)(a->Wi / 2), (cuuint64_t)(a->Hi / 2), (cuuint64_t)a->Ti, (cuuint64_t)a->B};
-  const cuuint64_t strides[4] = {(cuuint64_t)(C2 * 2), (cuuint64_t)(2 * rowb), (cuuint64_t)(a->Hi * rowb), (cuuint64_t)(a->Ti * a->Hi * rowb)};
+  const cuuint64_t strides[4] = {(cuuint64_t)(C2 * es), (cuuint64_t)(2 * rowb), (cuuint64_t)(a->Hi * rowb), (cuuint64_t)(a->Ti * a->Hi * rowb)};
   const cuuint32_t box_e[5] = {(cuuint32_t)bk, (cuuint32_t)p.pitch, 16, 1, 1}, box_o[5] = {(cuuint32_t)bk, (cuuint32_t)p.pitch, 17, 1, 1};
-  if (const int rc = encode_map16(&p.amap, p.dtype, 5, a->x, dims, strides, box_e, CU_TENSOR_MAP_SWIZZLE_128B, "even rows")) return rc;
-  if (const int rc = encode_map16(&p.amap_odd, p.dtype, 5, (const char*)a->x + rowb, dims, strides, box_o, CU_TENSOR_MAP_SWIZZLE_128B, "odd rows")) return rc;
+  if (const int rc = encode_tc_map(&p.amap, p.dtype, 5, a->x, dims, strides, box_e, CU_TENSOR_MAP_SWIZZLE_128B, "even rows")) return rc;
+  if (const int rc = encode_tc_map(&p.amap_odd, p.dtype, 5, (const char*)a->x + rowb, dims, strides, box_o, CU_TENSOR_MAP_SWIZZLE_128B, "odd rows")) return rc;
   const int64_t K = 6 * (int64_t)C2;
   const cuuint64_t wdims[2] = {(cuuint64_t)K, (cuuint64_t)a->Co};
-  const cuuint64_t wstrides[1] = {(cuuint64_t)(K * 2)};
+  const cuuint64_t wstrides[1] = {(cuuint64_t)(K * es)};
   const cuuint32_t wbox[2] = {(cuuint32_t)bk, (cuuint32_t)bn};
-  if (const int rc = encode_map16(&p.wmap2, p.dtype, 2, a->w, wdims, wstrides, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "weights")) return rc;
+  if (const int rc = encode_tc_map(&p.wmap2, p.dtype, 2, a->w, wdims, wstrides, wbox, CU_TENSOR_MAP_SWIZZLE_128B, "weights")) return rc;
   p.wmap = p.wmap2;
   if (const int rc = slab_encode_out_maps(p, EPI_DOWN_SPACE)) return rc;
   return slab_launch(EPI_DOWN_SPACE, p, stream);

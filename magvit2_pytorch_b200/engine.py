@@ -3,7 +3,8 @@ kernels of libmagvit2_b200.so through the C ABI (ctypes).  PyTorch is used only 
 memory (caching allocator), streams and parameter storage.
 
 Activations are channels-last (B, T, H, W, C) tensors in the compute dtype (fp32 -> CUDA-core
-path, bf16 or fp16 -> wgmma tensor-core path for the dense contractions, tensor_core_dtype).  There is no eager / CPU
+path, or TF32 wgmma while torch allows TF32 matmuls; bf16 or fp16 -> wgmma tensor-core path for the dense contractions,
+tensor_core_dtype).  There is no eager / CPU
 fallback: every op is a library call and a missing library is an error.
 """
 from __future__ import annotations
@@ -16,7 +17,7 @@ from typing import Callable, Dict, List, Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import (ACT_ELU, ACT_NONE, ACT_SILU, MV2_BF16, MV2_F16, MV2_F32, MV2_U8, SHUFFLE_NONE, SHUFFLE_SPACE,
+from ._lib import (ACT_ELU, ACT_NONE, ACT_SILU, MV2_BF16, MV2_F16, MV2_F32, MV2_TF32, MV2_U8, SHUFFLE_NONE, SHUFFLE_SPACE,
                    SHUFFLE_TIME, AttnArgs, ConvArgs, ConvHist, TcConvArgs, TcRuArgs, check)
 
 
@@ -30,10 +31,18 @@ def _dt(t: torch.dtype) -> int:
     raise TypeError(f"unsupported dtype {t} (only float32, bfloat16 and float16)")
 
 
-def tensor_core_dtype(t: torch.dtype) -> bool:
-    """True for the parameter dtypes whose dense contractions run on the wgmma tensor cores (bf16 and fp16: 16-bit
-    storage, fp32 accumulation); fp32 runs on the CUDA cores."""
-    return t in (torch.bfloat16, torch.float16)
+def tensor_core_dtype(t: torch.dtype, tf32: bool = False) -> bool:
+    """True for the parameter dtypes whose dense contractions run on the wgmma tensor cores: bf16 and fp16 (16-bit
+    storage, fp32 accumulation) always, fp32 with `tf32` (fp32 storage, TF32 multiply, fp32 accumulation); otherwise fp32
+    runs on the CUDA cores."""
+    return t in (torch.bfloat16, torch.float16) or (tf32 and t == torch.float32)
+
+
+def tf32_matmul_enabled() -> bool:
+    """torch's TF32 switch for fp32 matmuls (torch.set_float32_matmul_precision("high" / "medium"),
+    torch.backends.cuda.matmul.allow_tf32 = True or fp32_precision = "tf32"), which an fp32 tokenizer's calls without
+    gradients follow.  cuDNN's conv switch, on by default, is not followed: it would change every fp32 result."""
+    return torch.backends.cuda.matmul.fp32_precision == "tf32"
 
 
 def _src_dt(t: torch.dtype) -> int:
@@ -99,7 +108,7 @@ class ConvPack:
     k: Tuple[int, int, int]
     Ci: int
     Co: int
-    w_tc: Optional[torch.Tensor] = None      # [Co][taps*Ci] bf16 / fp16, K-major (wgmma path); rows permuted for shuffles
+    w_tc: Optional[torch.Tensor] = None      # [Co][taps*Ci] bf16 / fp16 / fp32 (TF32), K-major (wgmma path); rows permuted for shuffles
     bias_tc: Optional[torch.Tensor] = None   # bias in w_tc's row order
     Ci_tc: int = 0                           # GEMM dims of the wgmma call (may be padded / re-paired)
     Co_tc: int = 0
@@ -109,10 +118,13 @@ class ConvPack:
     w_down: Optional[torch.Tensor] = None    # SpatialDownsample2x pack for mv2_tc_down_space_forward ([Co][6][2*Ci], as w_tc)
 
 
-def pack_conv(weight: torch.Tensor, bias: Optional[torch.Tensor], dtype, k=None, shuffle_q: int = 1) -> ConvPack:
+def pack_conv(weight: torch.Tensor, bias: Optional[torch.Tensor], dtype, k=None, shuffle_q: int = 1, tc=None) -> ConvPack:
     """weight: torch layout (Co, Ci, *kernel).  Kernel dims are mapped onto (kt, kh, kw) by `k`.
     shuffle_q = 4 / 2 for the depth-to-space / depth-to-time up-samplers: the wgmma kernel wants output
-    rows ordered (q, c) instead of the reference's (c, q) so shuffled stores are channel-contiguous."""
+    rows ordered (q, c) instead of the reference's (c, q) so shuffled stores are channel-contiguous.
+    tc: build the wgmma pack too (default: tensor_core_dtype(dtype); True for an fp32 model's TF32 pack)."""
+    if tc is None:
+        tc = tensor_core_dtype(dtype)
     Co, Ci = weight.shape[:2]
     if k is None:
         ks = tuple(weight.shape[2:])
@@ -122,7 +134,7 @@ def pack_conv(weight: torch.Tensor, bias: Optional[torch.Tensor], dtype, k=None,
     b = None if bias is None else bias.detach().float().contiguous()
     pk = ConvPack(w=w, bias=b, k=tuple(int(v) for v in k), Ci=int(Ci), Co=int(Co))
     pk.macs = int(Co) * int(Ci) * int(w3.shape[2])
-    if tensor_core_dtype(dtype):
+    if tc:
         wt = w3.permute(0, 2, 1).reshape(Co, -1)                      # [Co][tap*Ci + ci]
         bt = b
         if shuffle_q > 1:
@@ -139,7 +151,7 @@ def pack_conv_down_space(pk: ConvPack, weight):
     """SpatialDownsample2x (M:768: Conv2d k3 s2 p1) for mv2_tc_down_space_forward: w[co][tap'][2*Ci], tap' = dh * 2 + q,
     q = 0 -> [zeros | w[:, :, dh, 0]] (the column left of the pair), q = 1 -> [w[:, :, dh, 1] | w[:, :, dh, 2]]."""
     Co, Ci, kh, kw = weight.shape
-    if (kh, kw) != (3, 3) or Ci % 64 != 0 or Co % 32 != 0:
+    if (kh, kw) != (3, 3) or Ci * pk.w_tc.element_size() % 128 != 0 or Co % 32 != 0:     # 128-byte K rows
         return
     w = weight.detach().float()
     wd = torch.zeros((Co, 3, 2, 2 * Ci), device=w.device)
@@ -149,22 +161,37 @@ def pack_conv_down_space(pk: ConvPack, weight):
     pk.w_down = wd.reshape(Co, 6 * 2 * Ci).contiguous().to(pk.w_tc.dtype)
 
 
+def _adopt_tc_packs(old, new):
+    """Sets the wgmma fields of every ConvPack in the pack tree `old` to those of its counterpart in `new`, a tree of the
+    same parameters packed with them; old's CUDA-core tensors stay as they are."""
+    if isinstance(old, ConvPack):
+        for f in ("w_tc", "bias_tc", "Ci_tc", "Co_tc", "epi_mode", "k_tc", "w_down"):
+            setattr(old, f, getattr(new, f))
+    elif isinstance(old, dict):
+        for k, v in new.items():
+            if old.get(k) is None:          # a wgmma-only pack (the kw-packed conv_in)
+                old[k] = v
+            else:
+                _adopt_tc_packs(old[k], v)
+
+
 def _round_up(v, m):
     return (v + m - 1) // m * m
 
 
-def pack_ff(fc1_w, fc1_b, fc2_w, fc2_b, dtype):
+def pack_ff(fc1_w, fc1_b, fc2_w, fc2_b, dtype, tc=None):
     """FeedForward weights (reference M:492-496).  wgmma layout: the hidden width I is padded to a multiple of 64,
     fc1's rows are re-paired as [8 x-rows, their 8 gate-rows] per group of 16 so GEGLU (M:466-469) fuses into fc1's
     epilogue, and fc2's K is zero-padded to match.  The fused fc1 needs K = C a multiple of 16; for other widths there
     are no wgmma packs, and fc1, GEGLU and fc2 run unfused on the CUDA cores."""
-    fc1 = pack_conv(fc1_w, fc1_b, dtype)
-    fc2 = pack_conv(fc2_w, fc2_b, dtype)
+    tc = tensor_core_dtype(dtype) if tc is None else tc
+    fc1 = pack_conv(fc1_w, fc1_b, dtype, tc=tc)
+    fc2 = pack_conv(fc2_w, fc2_b, dtype, tc=tc)
     two_i, C_ = fc1_w.shape[:2]
-    if tensor_core_dtype(dtype) and C_ % 16 != 0:
+    if tc and C_ % 16 != 0:
         for pk in (fc1, fc2):
             pk.w_tc = pk.bias_tc = None
-    elif tensor_core_dtype(dtype):
+    elif tc:
         I = two_i // 2
         Ip = _round_up(I, 64)
         w1 = fc1_w.detach().reshape(two_i, C_).float()
@@ -186,18 +213,18 @@ def pack_ff(fc1_w, fc1_b, fc2_w, fc2_b, dtype):
     return fc1, fc2
 
 
-def pack_linear_attention(la, dt):
+def pack_linear_attention(la, dt, tc=None):
     """LinearSpaceAttention (M:390-442) for Engine.linear_attention."""
     return dict(gamma=la.norm.gamma.detach().float().contiguous(),
-                q=pack_conv(la.attn.to_q[0].weight[:, :, None, None, None], None, dt),
-                kv=pack_conv(la.attn.to_kv[0].weight[:, :, None, None, None], None, dt),
-                out=pack_conv(la.attn.to_out[0].weight[:, :, None, None, None], None, dt),
+                q=pack_conv(la.attn.to_q[0].weight[:, :, None, None, None], None, dt, tc=tc),
+                kv=pack_conv(la.attn.to_kv[0].weight[:, :, None, None, None], None, dt, tc=tc),
+                out=pack_conv(la.attn.to_out[0].weight[:, :, None, None, None], None, dt, tc=tc),
                 heads=la.heads, dim_head=la.dim_head)
 
 
-def pack_feed_forward(ff, dt):
+def pack_feed_forward(ff, dt, tc=None):
     """FeedForward (M:471-496) for Engine.feed_forward."""
-    fc1, fc2 = pack_ff(ff.net[0].weight, ff.net[0].bias, ff.net[2].weight, ff.net[2].bias, dt)
+    fc1, fc2 = pack_ff(ff.net[0].weight, ff.net[0].bias, ff.net[2].weight, ff.net[2].bias, dt, tc=tc)
     return dict(gamma=ff.norm.gamma.detach().float().reshape(-1).contiguous(), fc1=fc1, fc2=fc2, inner=ff.dim_inner)
 
 
@@ -265,6 +292,10 @@ class Engine:
         self._sig_id = 0             # bumped whenever parameters are re-packed (invalidates cached CUDA graphs)
         self.launches = 0            # kernels launched through the C ABI (bench's gpu_launches)
         self.use_tc = True           # bf16 / fp16: dense contractions on wgmma (False -> CUDA-core cross-check path)
+        # fp32: the current call runs its dense contractions on the TF32 wgmma kernels (set per call by the model, from
+        # torch's switch, for calls without gradients only; the packs they read are added by prepare(tf32_packs=True))
+        self.tf32 = False
+        self._tf32_packs = False
         self.tc_variant = "auto"     # "auto" (Engine.conv_kernel's choice) | "tap" (tc_conv.cu only)
         self.fuse_ru = True          # bf16 / fp16: conv3x3x3 + ELU + conv1x1x1 + ELU + SE pool partials in one wgmma launch (C = 64 / 128)
         self.fused_ru_calls = 0
@@ -296,22 +327,34 @@ class Engine:
         self.dtype = p0.dtype
         self.device = p0.device
 
-    def prepare(self):
-        """(Re)pack parameters into kernel layouts when they changed (load_state_dict, .to(), ...)."""
+    def prepare(self, tf32_packs: bool = False):
+        """(Re)pack parameters into kernel layouts when they changed (load_state_dict, .to(), ...).  An fp32 model's TF32
+        packs are built on the first call that needs them (tf32_packs, or self.tf32) and kept next to its CUDA-core packs
+        until the next re-pack; adding them leaves every existing pack tensor, and with it every captured graph, valid."""
         sig = param_signature(self.model)
+        tf32_packs = (tf32_packs or self.tf32) and sig[1] == torch.float32
         if sig == self._sig:
+            if tf32_packs and not self._tf32_packs:
+                _adopt_tc_packs(self._packs, self._build_packs(True))
+                self._tf32_packs = True
             return
+        self.bind(self.model.conv_in.conv.weight, "magvit2_pytorch_b200.VideoTokenizer")
+        self._packs = self._build_packs(tensor_core_dtype(self.dtype, tf32_packs))
+        self._tf32_packs = tf32_packs
+        self._sig = sig
+        self._sig_id += 1
+
+    def _build_packs(self, tc: bool) -> Dict[str, object]:
+        """Every parameter of the model in kernel layout; tc: with the wgmma packs (bf16 / fp16, or an fp32 model's TF32)."""
         m = self.model
-        self.bind(m.conv_in.conv.weight, "magvit2_pytorch_b200.VideoTokenizer")
         dt = self.dtype
         P: Dict[str, object] = {}
-        P["conv_in"] = pack_conv(m.conv_in.conv.weight, m.conv_in.conv.bias, dt)
-        P["conv_in_tc"] = (pack_conv_in_kwpack(m.conv_in.conv.weight, m.conv_in.conv.bias, dtype=dt) if tensor_core_dtype(dt)
-                           else None)
-        P["conv_out"] = pack_conv(m.conv_out.conv.weight, m.conv_out.conv.bias, dt)
+        P["conv_in"] = pack_conv(m.conv_in.conv.weight, m.conv_in.conv.bias, dt, tc=tc)
+        P["conv_in_tc"] = pack_conv_in_kwpack(m.conv_in.conv.weight, m.conv_in.conv.bias, dtype=dt) if tc else None
+        P["conv_out"] = pack_conv(m.conv_out.conv.weight, m.conv_out.conv.bias, dt, tc=tc)
         if m.separate_first_frame_encoding:       # SameConv2d (M:887-890): a (1, kh, kw) conv on the single first frame
-            P["conv_in_ff"] = pack_conv(m.conv_in_first_frame.weight, m.conv_in_first_frame.bias, dt)
-            P["conv_out_ff"] = pack_conv(m.conv_out_first_frame.weight, m.conv_out_first_frame.bias, dt)
+            P["conv_in_ff"] = pack_conv(m.conv_in_first_frame.weight, m.conv_in_first_frame.bias, dt, tc=tc)
+            P["conv_out_ff"] = pack_conv(m.conv_out_first_frame.weight, m.conv_out_first_frame.bias, dt, tc=tc)
 
         def f32(t):
             return t.detach().float().contiguous()
@@ -321,8 +364,8 @@ class Engine:
             se = seq[4]
             C_ = seq[2].weight.shape[0]
             P[key] = dict(
-                conv3=pack_conv(seq[0].conv.weight, seq[0].conv.bias, dt),
-                conv1=pack_conv(seq[2].weight, seq[2].bias, dt),
+                conv3=pack_conv(seq[0].conv.weight, seq[0].conv.bias, dt, tc=tc),
+                conv1=pack_conv(seq[2].weight, seq[2].bias, dt, tc=tc),
                 wk=f32(se.to_k.weight.reshape(-1)), bk=float(se.to_k.bias.detach().float().item()),
                 w1=f32(se.net[0].weight.reshape(se.net[0].weight.shape[0], C_)), b1=f32(se.net[0].bias),
                 w2=f32(se.net[2].weight.reshape(C_, -1)), b2=f32(se.net[2].bias),
@@ -330,16 +373,16 @@ class Engine:
             )
 
         def pack_ffn(ff, key):
-            P[key] = pack_feed_forward(ff, dt)
+            P[key] = pack_feed_forward(ff, dt, tc)
 
         def pack_attn(at, key):
-            P[key] = dict(gamma=f32(at.norm.gamma), qkv=pack_conv(at.to_qkv[0].weight[:, :, None, None, None], None, dt),
-                          out=pack_conv(at.to_out[1].weight[:, :, None, None, None], None, dt),
+            P[key] = dict(gamma=f32(at.norm.gamma), qkv=pack_conv(at.to_qkv[0].weight[:, :, None, None, None], None, dt, tc=tc),
+                          out=pack_conv(at.to_out[1].weight[:, :, None, None, None], None, dt, tc=tc),
                           mem_kv=at.mem_kv.detach().to(dt).float().contiguous(),
                           heads=at.heads, dim_head=at.dim_head, n_mem=int(at.mem_kv.shape[2]))
 
         def pack_lin(la, key):
-            P[key] = pack_linear_attention(la, dt)
+            P[key] = pack_linear_attention(la, dt, tc)
 
         for side, layers in (("enc", m.encoder_layers), ("dec", m.decoder_layers)):
             stages = m.stages if side == "enc" else list(reversed(m.stages))
@@ -353,21 +396,21 @@ class Engine:
                 elif st.kind == "cond_residual":
                     w = mod.conv.weights
                     wq = w.detach().to(dt).float()                  # the weights as the module holds them in this dtype
-                    P[key] = dict(conv3=pack_conv(w, None, dt), conv1=pack_conv(mod.conv_out.weight, mod.conv_out.bias, dt),
+                    P[key] = dict(conv3=pack_conv(w, None, dt, tc=tc), conv1=pack_conv(mod.conv_out.weight, mod.conv_out.bias, dt, tc=tc),
                                   S=(wq * wq).sum(dim=(2, 3, 4)).contiguous(), eps=float(mod.conv.eps),
                                   wc=f32(mod.to_cond.weight), bc=f32(mod.to_cond.bias))
                 elif st.kind == "compress_space":
                     if side == "enc":
-                        P[key] = pack_conv(mod.conv.weight, mod.conv.bias, dt)                     # (Co,Ci,3,3) -> k=(1,3,3)
-                        if tensor_core_dtype(dt):
+                        P[key] = pack_conv(mod.conv.weight, mod.conv.bias, dt, tc=tc)                     # (Co,Ci,3,3) -> k=(1,3,3)
+                        if tc:
                             pack_conv_down_space(P[key], mod.conv.weight)
                     else:
-                        P[key] = pack_conv(mod.net[0].weight, mod.net[0].bias, dt, shuffle_q=4)    # (4Co,Ci,1,1)
+                        P[key] = pack_conv(mod.net[0].weight, mod.net[0].bias, dt, shuffle_q=4, tc=tc)    # (4Co,Ci,1,1)
                 elif st.kind == "compress_time":
                     if side == "enc":
-                        P[key] = pack_conv(mod.conv.weight, mod.conv.bias, dt, k=(3, 1, 1))        # Conv1d (Co,Ci,3)
+                        P[key] = pack_conv(mod.conv.weight, mod.conv.bias, dt, k=(3, 1, 1), tc=tc)        # Conv1d (Co,Ci,3)
                     else:
-                        P[key] = pack_conv(mod.net[0].weight, mod.net[0].bias, dt, k=(1, 1, 1), shuffle_q=2)  # Conv1d (2Co,Ci,1)
+                        P[key] = pack_conv(mod.net[0].weight, mod.net[0].bias, dt, k=(1, 1, 1), shuffle_q=2, tc=tc)  # Conv1d (2Co,Ci,1)
                 elif st.kind == "attend_space":
                     pack_attn(mod[0].fn, key + ".attn")
                     pack_ffn(mod[1].fn, key + ".ff")
@@ -379,7 +422,7 @@ class Engine:
                     pack_ffn(mod[1].fn, key + ".ff")
                 elif st.kind == "gateloop_time":
                     gl = mod.fn.fn
-                    P[key] = dict(gamma=f32(gl.norm.gamma), qkva=pack_conv(gl.to_qkva[0].weight[:, :, None, None, None], None, dt))
+                    P[key] = dict(gamma=f32(gl.norm.gamma), qkva=pack_conv(gl.to_qkva[0].weight[:, :, None, None, None], None, dt, tc=tc))
         if m.has_cond:
             for side, stem in (("enc", m.encoder_cond_in), ("dec", m.decoder_cond_in)):
                 P[f"{side}_cond_in"] = dict(w=f32(stem[0].weight), b=f32(stem[0].bias))
@@ -387,9 +430,7 @@ class Engine:
         # the reference applies the projections in the module dtype (bf16 weights in bf16 mode)
         P["quant"] = dict(win=q.project_in.weight.detach().to(dt).float().contiguous(), bin=q.project_in.bias.detach().to(dt).float().contiguous(),
                           wout=q.project_out.weight.detach().to(dt).float().contiguous(), bout=q.project_out.bias.detach().to(dt).float().contiguous())
-        self._packs = P
-        self._sig = sig
-        self._sig_id += 1
+        return P
 
     # ------------------------------------------------------------------ primitive ops
     def _stream(self):
@@ -501,7 +542,8 @@ class Engine:
         """The kernel conv() runs for the call `ta` (its mv2_tc_conv_args) with hist_T history frames: "slab" (tc_slab.cu),
         "down" (its SpatialDownsample2x flavour, on pk.w_down), "tap" (tc_conv.cu), "tap_cat" (tc_conv.cu on a copy of
         [history | x]) or "simt" (the CUDA-core conv).  Host-side shape queries only: it launches nothing and needs no device."""
-        if not (tensor_core_dtype(self.dtype) and self.use_tc and pk.w_tc is not None and ta.Ci == pk.Ci_tc and not token_shift):
+        if not (tensor_core_dtype(self.dtype, self.tf32) and self.use_tc and pk.w_tc is not None and ta.Ci == pk.Ci_tc
+                and not token_shift):
             return "simt"
         lib = self.lib
         # the persistent slab kernel reuses each activation slab for all in-plane taps, so it takes every layer it supports
@@ -554,7 +596,11 @@ class Engine:
                           res=_ptr(res), y=_ptr(y), B=B, Ti=Ti, Hi=Hi, Wi=Wi, Ci=Ci, To=To, Ho=Ho, Wo=Wo, Co=pk.Co_tc,
                           kt=kt, kh=kh, kw=kw, st=stride[0], sh=stride[1], sw=stride[2],
                           pt=pt, ph=ph, pw=pw, act=act, shuffle=shuffle, epi_mode=pk.epi_mode,
-                          oscale=_ptr(oscale), out_layout=int(out_cf), dtype=_dt(self.dtype))
+                          oscale=_ptr(oscale), out_layout=int(out_cf), dtype=self._tc_dt())
+
+    def _tc_dt(self) -> int:
+        """Element type of this engine's wgmma launches (mv2_tc_conv_args.dtype): fp32 storage is MV2_TF32."""
+        return MV2_TF32 if self.dtype == torch.float32 else _dt(self.dtype)
 
     def conv_cf_supported(self, x, pk: ConvPack, pad, out_spatial) -> bool:
         """True when conv(x, pk, pad=pad, out_spatial=out_spatial, out_cf=True) runs: bf16 / fp16 on the slab kernel, whose
@@ -570,7 +616,7 @@ class Engine:
         if self.fuse_ru and self.conv_kernel(self._tc_args(x, c3, act=ACT_ELU), c3) == "slab":
             ra = TcRuArgs(x=_ptr(x), w3=_ptr(c3.w_tc), b3=_ptr(c3.bias_tc), w1=_ptr(c1.w_tc), b1=_ptr(c1.bias_tc),
                           se_wk=_ptr(p["wk"]), se_bk=p["bk"], y=None, se_ws=None, B=B, T=T, H=H, W=W, C=Cc,
-                          kt=c3.k[0], kh=c3.k[1], kw=c3.k[2], dtype=dt)
+                          kt=c3.k[0], kh=c3.k[1], kw=c3.k[2], dtype=self._tc_dt())
             if self.lib.mv2_tc_ru_supported(C.byref(ra)):
                 hist, advance = self._conv_hist(_sub(ss, "conv3"), x, c3.k[0] - 1)
                 y = self._new(x.shape)
@@ -845,7 +891,8 @@ class Engine:
     def ingest_kwpack(self, v: torch.Tensor, t_pad: int, pin):
         """(B,C,T,H,W) -> (B,T+t_pad,H,W,32) with the k_w taps packed into channels (mv2_ingest_kwpack), in the compute
         dtype: mv2_ingest_kwpack writes fp16 for an fp16 source and bf16 for the others, so an fp16 model's uint8 / fp32
-        video is first rounded to fp16 in place of layout (mv2_to_channels_last of single-channel frames: a plain copy)."""
+        video is first rounded to fp16 in place of layout (mv2_to_channels_last of single-channel frames: a plain copy);
+        an fp32 model's (the TF32 conv_in) is written in fp32 (MV2_KWPACK_F32_DST)."""
         if v.dtype not in self._src_dtypes():
             v = v.float()
         v = v.contiguous()
@@ -855,7 +902,8 @@ class Engine:
             self._call("mv2_to_channels_last", _ptr(v), _src_dt(v.dtype), _ptr(v16), MV2_F16, B * Cc * T, 1, 1, H, W, 0)
             v = v16
         out = self._new((B, T + t_pad, H, W, pin.Ci_tc), self.dtype)
-        self._call("mv2_ingest_kwpack", _ptr(v), _src_dt(v.dtype), _ptr(out), B, Cc, T, H, W, t_pad, pin.kw_orig,
+        dst32 = _lib.MV2_KWPACK_F32_DST if self.dtype == torch.float32 else 0
+        self._call("mv2_ingest_kwpack", _ptr(v), _src_dt(v.dtype) | dst32, _ptr(out), B, Cc, T, H, W, t_pad, pin.kw_orig,
                    pin.kw_orig // 2, pin.Ci_tc)
         return out
 

@@ -14,6 +14,8 @@ from typing import List, Optional
 
 import torch
 
+from .engine import tf32_matmul_enabled
+
 
 class StreamLanes:
     """`lanes` CUDA streams, each with its own CUDA-graph instances of the model's entry points (`VideoTokenizer._lane`).
@@ -47,7 +49,9 @@ class StreamLanes:
         s = self.streams[lane]
         # (re)pack the parameters, if they changed, on the CALLER's stream: every lane is ordered after it below, so no lane
         # can read packs that another lane's stream is still writing
-        _ = self.model.engine
+        eng = self.model.engine
+        if eng.dtype == torch.float32 and tf32_matmul_enabled():
+            eng.prepare(tf32_packs=True)        # the TF32 packs the call will add
         s.wait_stream(torch.cuda.current_stream(self.device))
         prev = self.model._lane
         self.model._lane = lane
@@ -125,7 +129,10 @@ class HostRoundTrip:
         lane = ((self.n - 1) % len(self.slots)) % len(self.lanes.streams) if self.lanes is not None else 0
         sc = self.lanes.streams[lane] if self.lanes is not None else cur
         if sc is not cur:
-            _ = self.model.engine                    # parameter (re)packing happens on `cur`, which every lane waits for
+            # parameter (re)packing, and the TF32 packs the calls may add, happen on `cur`, which every lane waits for
+            eng = self.model.engine
+            if eng.dtype == torch.float32 and tf32_matmul_enabled():
+                eng.prepare(tf32_packs=True)
             sc.wait_stream(cur)                      # whatever the caller queued before this submit (weight updates, ...)
         sc.wait_event(slot.h2d)
         if slot.used:

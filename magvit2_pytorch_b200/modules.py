@@ -16,7 +16,7 @@ import torch
 from torch import nn
 
 from ._lib import SHUFFLE_NONE, SHUFFLE_TIME
-from .engine import PackCache, pack_conv
+from .engine import PackCache, pack_conv, tf32_matmul_enabled
 
 
 class _NoForward(nn.Module):
@@ -368,8 +368,11 @@ class CausalConvTranspose3d(nn.Module):
         if w.device.type != "cuda" or x.device != w.device:
             raise RuntimeError("CausalConvTranspose3d runs on CUDA (sm_90a) only, input and parameters on the same device")
         with torch.no_grad(), torch.cuda.device(w.device):
+            # an fp32 pack carries the CUDA-core and the TF32 layouts; the call runs TF32 while torch allows TF32 matmuls
             eng, pk = self._pack_cache.get(self, "CausalConvTranspose3d", lambda eng: pack_conv(
-                *self.equivalent_conv_weight(), eng.dtype, shuffle_q=self.upsample_factor), half=True)
+                *self.equivalent_conv_weight(), eng.dtype, shuffle_q=self.upsample_factor,
+                tc=True if eng.dtype == torch.float32 else None), half=True)
+            eng.tf32 = w.dtype == torch.float32 and tf32_matmul_enabled()
             y = eng.conv(eng.to_channels_last(x), pk, shuffle=SHUFFLE_TIME if self.upsample_factor == 2 else SHUFFLE_NONE)
             out = eng.to_channels_first(y)
             n = self.output_frames(x.shape[2])

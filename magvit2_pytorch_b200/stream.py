@@ -15,9 +15,11 @@ With tok.cuda_graphs set, a stream replays its pushes as CUDA graphs (PushPlan) 
 """
 from __future__ import annotations
 
+import contextlib
+
 import torch
 
-from .engine import StreamState
+from .engine import StreamState, tf32_matmul_enabled
 
 
 def check_stream_model(model):
@@ -116,13 +118,18 @@ class _Stream:
         self.first_frame = bool(video_contains_first_frame)
         self.cond = model._check_cond(cond, self.batch_size)
         self.state = StreamState()
+        # an fp32 model's precision is read from torch's TF32 switch once, here: every push runs in it, so the pushes still
+        # give the outputs of one whole-clip call in that precision bit for bit
+        self.tf32 = model.dtype == torch.float32 and tf32_matmul_enabled()
         self.pushes = 0
         self._sig_id = None
         self._plans = {}             # push signature -> "warm" | PushPlan (model.cuda_graphs)
         self.captures = 0            # PushPlans captured
 
+    @contextlib.contextmanager
     def _engine(self):
-        """The model's engine, eval mode, checked against the parameter packs this stream started with."""
+        """The model's engine in this stream's precision for one push, eval mode, checked against the parameter packs this
+        stream started with."""
         self.model.eval()
         eng = self.model.engine
         if self._sig_id is None:
@@ -130,7 +137,13 @@ class _Stream:
         elif eng._sig_id != self._sig_id:
             raise RuntimeError("the tokenizer's parameters changed while this stream was open: its carried state belongs "
                                "to the old ones; start a new stream")
-        return eng
+        prev, eng.tf32 = eng.tf32, self.tf32
+        try:
+            if self.tf32:
+                eng.prepare()         # adds the TF32 packs on the first such push
+            yield eng
+        finally:
+            eng.tf32 = prev
 
     def _run(self, eng, fn, x, first, sff_rest):
         """fn(x), the push of input x.  With model.cuda_graphs set it goes through this stream's PushPlans, with the rule
@@ -177,9 +190,7 @@ class TokenizeStream(_Stream):
         first = self.pushes == 0
         encoder_chunk_frames(chunk.shape[2], m.time_downsample_factor, first, self.first_frame)
         ff, sff_rest = self.first_frame and first, self.first_frame and not first and m.separate_first_frame_encoding
-        with torch.cuda.device(m.device):
-            eng = self._engine()
-
+        with torch.cuda.device(m.device), self._engine() as eng:
             def fn(v):
                 return eng.quantize_cl(eng.encode_cl(v, ff, self.cond, ss=self.state, sff_rest=sff_rest),
                                        want_quantized=False)[1]
@@ -205,9 +216,7 @@ class DecodeStream(_Stream):
         first = self.pushes == 0
         decoder_chunk_frames(codes.shape[1], m.time_downsample_factor, first, self.first_frame)
         ff, sff_rest = self.first_frame and first, self.first_frame and not first and m.separate_first_frame_encoding
-        with torch.cuda.device(m.device):
-            eng = self._engine()
-
+        with torch.cuda.device(m.device), self._engine() as eng:
             def fn(c):
                 return eng.decode_cl(eng.codes_to_quantized_cl(c), ff, self.cond, ss=self.state, sff_rest=sff_rest)
             out = self._run(eng, fn, codes.contiguous(), first, sff_rest)

@@ -8,9 +8,9 @@ M:): the keyword-only constructor and ``layers=(...)`` spec (M:1047-1092, M:1138
 (M:1447-1458, M:1495-1520), ``copy_for_eval`` (M:1476), ``device`` (M:1443).
 
 All arithmetic runs in hand-written sm_90a kernels behind the C ABI of libmagvit2_b200.so;
-the compute dtype follows the parameters' dtype (``.float()`` -> fp32 CUDA-core path,
-``.bfloat16()`` -> bf16 wgmma path, ``.half()`` -> the same wgmma kernels in fp16: no-grad calls only, no discriminator /
-VGG).  There is no CPU / eager fallback.
+the compute dtype follows the parameters' dtype (``.float()`` -> fp32 CUDA-core path, or the same wgmma kernels in TF32
+for calls without gradients while torch allows TF32 matmuls, ``.bfloat16()`` -> bf16 wgmma path, ``.half()`` -> the same
+wgmma kernels in fp16: no-grad calls only, no discriminator / VGG).  There is no CPU / eager fallback.
 
 ``cond_residual`` layers (ResidualUnitMod / Conv3DMod, M:680-753, M:946-988) run on the device through the
 factorisation in include/magvit2_b200.h; the other ``cond_*`` types raise in the reference itself.
@@ -57,7 +57,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import modules as M
-from .engine import AttnDropout, Engine, PackCache
+from .engine import AttnDropout, Engine, PackCache, tf32_matmul_enabled
 
 __version__ = "0.1.0"
 
@@ -111,6 +111,23 @@ def _attn_dropout_scope(fn):
             return fn(self, *a, **k)
         finally:
             eng.dropout = None
+    return wrapper
+
+
+def _precision_scope(fn):
+    """Runs the method with the engine's fp32 precision at IEEE unless the method turns TF32 on (VideoTokenizer._tf32_engine),
+    and restores the caller's afterwards: a call that takes gradients, or a nested call, never inherits TF32."""
+    @functools.wraps(fn)
+    def wrapper(self, *a, **k):
+        eng = self._engine
+        prev = False if eng is None else eng.tf32
+        if eng is not None:
+            eng.tf32 = False
+        try:
+            return fn(self, *a, **k)
+        finally:
+            if self._engine is not None:
+                self._engine.tf32 = prev
     return wrapper
 
 
@@ -456,13 +473,23 @@ class VideoTokenizer(nn.Module):
         self._engine.lib.mv2_set_pdl(1 if self.pdl else 0)
         return self._engine
 
+    def _tf32_engine(self, follow: bool = True) -> Engine:
+        """The engine for a call without gradients, with an fp32 model's dense contractions on the TF32 tensor cores when
+        `follow` and torch allows TF32 matmuls (tf32_matmul_enabled, read once here per call); bf16 / fp16 models are not
+        affected.  Calls with gradients, and the discriminator and VGG, never come here: they stay IEEE fp32."""
+        eng = self.engine
+        eng.tf32 = bool(follow) and self.dtype == torch.float32 and tf32_matmul_enabled()
+        if eng.tf32:
+            eng.prepare()             # adds the TF32 packs on the first such call
+        return eng
+
     def _graph_call(self, name, fn, *tensors):
         """fn(*tensors) -> tensor | tuple of tensors, replayed through a cached CUDA graph when enabled.  Forwards with live
         attention dropout run directly: a captured graph would replay one dropout mask forever."""
         if not self.cuda_graphs or (self._engine is not None and self._engine.dropout is not None):
             return fn(*tensors)
         eng = self.engine
-        key = (name, eng._sig_id, tuple((tuple(t.shape), t.dtype) for t in tensors), self._lane)
+        key = (name, eng._sig_id, tuple((tuple(t.shape), t.dtype) for t in tensors), self._lane, eng.tf32)
         if any(k[1] != eng._sig_id for k in self._graphs):      # parameters were re-packed: old graphs read stale weights
             self._graphs = {k: v for k, v in self._graphs.items() if k[1] == eng._sig_id}
         ent = self._graphs.get(key)
@@ -537,6 +564,7 @@ class VideoTokenizer(nn.Module):
         return _TapeFn.apply(runner, lambda x_, c_: run(x_, c_, *args), x, cond, *params), runner
 
     @_on_model_device
+    @_precision_scope
     @_attn_dropout_scope
     def encode(self, video, quantize=False, cond=None, video_contains_first_frame=True):
         """M:1523-1576.  Returns (B, C, T', H', W') like the reference; quantize: (quantized, codes[, aux_loss]).
@@ -553,7 +581,7 @@ class VideoTokenizer(nn.Module):
                 return out
             return (out, runner.codes) if self.use_fsq else (out, runner.codes, self.zero)
         with torch.no_grad():
-            eng = self.engine
+            eng = self._tf32_engine()
             x = eng.encode_cl(video, ff, cond)
             if quantize:
                 q, idx, _ = eng.quantize_cl(x)
@@ -584,6 +612,7 @@ class VideoTokenizer(nn.Module):
         return latent_frames * self.time_downsample_factor - (self.time_padding if ff else 0)
 
     @_on_model_device
+    @_precision_scope
     @_attn_dropout_scope
     def decode(self, quantized, cond=None, video_contains_first_frame=True):
         """M:1598-1649.  quantized: (B, C, T', H', W').  Differentiable (see _grad_params) wrt quantized, cond and the
@@ -597,10 +626,11 @@ class VideoTokenizer(nn.Module):
         if params is not None:
             return self._grad_call("run_decode", quantized, cond, params, ff)[0]
         with torch.no_grad():
-            eng = self.engine
+            eng = self._tf32_engine()
             return eng.decode_cl(eng.to_channels_last(quantized), ff, cond)
 
     @_on_model_device
+    @_precision_scope
     @_attn_dropout_scope
     def decode_from_code_indices(self, codes, cond=None, video_contains_first_frame=True):
         """M:1579-1595.  Differentiable (see _grad_params) wrt cond and the parameters of decode and quantizers.project_out."""
@@ -621,6 +651,7 @@ class VideoTokenizer(nn.Module):
         if params is not None:
             return self._grad_call("run_decode_codes", codes.contiguous(), cond, params, ff)[0]
         with torch.no_grad():
+            self._tf32_engine()
             return self._decode_codes_no_grad(codes, cond, ff)
 
     def _decode_codes_no_grad(self, codes, cond, ff):
@@ -633,6 +664,7 @@ class VideoTokenizer(nn.Module):
 
     @torch.no_grad()
     @_on_model_device
+    @_precision_scope
     @_attn_dropout_scope
     def lfq_loss_breakdown(self, video, group=None):
         """Training-mode LFQ auxiliary terms the reference computes at M:1705 (``quantizer_loss_breakdown``):
@@ -642,7 +674,7 @@ class VideoTokenizer(nn.Module):
         from .dist import LfqBatchEntropy
         assert not self.use_fsq, "FSQ has no auxiliary loss (reference M:1702)"
         video, _ = self._check_video(video)
-        eng = self.engine
+        eng = self._tf32_engine()
         x = eng.encode_cl(video)
         _, codes, pre = eng.quantize_cl(x, want_quantized=False, want_aux=True)
         q = self.quantizers
@@ -695,6 +727,7 @@ class VideoTokenizer(nn.Module):
         return self.forward(video, return_codes=True)
 
     @_on_model_device
+    @_precision_scope
     @_attn_dropout_scope
     def forward(self, video_or_images, cond=None, return_loss=False, return_codes=False, return_recon=False,
                 return_discr_loss=False, return_recon_loss_only=False, apply_gradient_penalty=True,
@@ -776,7 +809,8 @@ class VideoTokenizer(nn.Module):
             return total_loss, LossBreakdown(recon_loss, aux_losses, qlb, perceptual_loss, gen_loss, adaptive_weight,
                                              ms_losses, ms_weights)
         with torch.no_grad():
-            eng = self.engine
+            # a loss with a discriminator or a VGG term stays IEEE: those modules train, and their inputs with them
+            eng = self._tf32_engine(follow=not (return_loss and (self.has_gan or self.use_vgg or self.has_multiscale_discrs)))
             need_recon = return_recon or return_recon_loss_only or return_loss or not return_codes
             out, aux = self._no_grad_forward(eng, video, ff, cond, need_recon)
             if return_codes and not return_recon:
