@@ -95,6 +95,47 @@ class StreamState:
         besides the time attention's K/V cache length."""
         return tuple(v[1] for k, v in self._slots.items() if k.rsplit("/", 1)[-1] == "hist")
 
+    def kv_capacities(self):
+        """The frame capacity of every time attention's K/V cache, in layer order."""
+        return tuple(v[0].shape[1] for k, v in self._slots.items() if k.rsplit("/", 1)[-1] == "kv")
+
+    def restart_rows(self, rows):
+        """Starts clip rows `rows` over: the next push computes for them what the first push of a new stream computes.
+        Their slices of every conv history, token-shift frame and gateloop scan state are zeroed in place (zero history
+        frames give the values of the causal padding, DESIGN.md 3.7), and each time attention's K/V cache records the
+        current end of the cache as where their keys start.  No buffer moves and no frame count changes, so a push
+        captured as a CUDA graph replays unchanged."""
+        rows = set(rows)
+        for k, v in self._slots.items():
+            leaf = k.rsplit("/", 1)[-1]
+            if leaf in ("hist", "prev", "s"):
+                buf = v[0] if leaf == "hist" else v
+                for r0, r1, hit in row_runs([r in rows for r in range(buf.shape[0])]):
+                    if hit:
+                        buf[r0:r1].zero_()
+            elif leaf == "kv":
+                buf, L, starts = v
+                self._slots[k] = (buf, L, tuple(L if r in rows else s for r, s in enumerate(starts)))
+
+
+def row_runs(starts):
+    """[(first row, end row, value)] of the runs of consecutive rows with equal `starts` values, in row order."""
+    runs = []
+    for r, s in enumerate(starts):
+        if runs and runs[-1][2] == s:
+            runs[-1] = (runs[-1][0], r + 1, s)
+        else:
+            runs.append((r, r + 1, s))
+    return runs
+
+
+def kv_cache_plan(length, T, starts, step):
+    """When a K/V cache holding `length` frames has no room for T more: (frames to drop from its front, new capacity).
+    The frames before the earliest row start belong to no live clip; the capacity is the rest plus T, rounded up to a
+    multiple of `step`."""
+    drop = min(starts)
+    return drop, _round_up(length - drop + T, step)
+
 
 def _sub(ss: Optional[StreamState], name):
     return None if ss is None else ss.sub(name)
@@ -744,7 +785,12 @@ class Engine:
         and values are appended to the stream's K/V cache (every earlier frame's; it grows by KV_CACHE_STEP frames when
         full) and mv2_attention_tail computes the chunk's queries, read from qkv, against all cached keys.  Its launch
         arguments change with every push (the cache length, the kernel chosen for it, the cache's address after a growth),
-        so a captured push runs it as a host step between two graph segments (host_step)."""
+        so a captured push runs it as a host step between two graph segments (host_step).
+
+        The cache has one time axis for all rows, and each row's clip starts at its own index of it (StreamState.restart_rows;
+        0 for a row never restarted).  Each run of consecutive rows that share a start gets its own call on the cache from
+        that start, so every row sees its own clip's keys with the kernel chosen for their count, as in a new stream.  When
+        the cache grows, the frames before the earliest start are dropped (kv_cache_plan)."""
         B, T, H, W, C3 = qkv.shape
         HW, HD = H * W, C3 // 3
         outs = ss.get("o")
@@ -754,22 +800,23 @@ class Engine:
         o = outs.get(T)
         if o is None:
             o = outs[T] = self._new((B, T, H, W, HD))
-        cache = ss.get("kv")
-        L0 = 0 if cache is None else cache[1]
-        buf = None if cache is None else cache[0]
+        buf, L0, starts = ss.get("kv") or (None, 0, (0,) * B)
         if buf is None or buf.shape[1] < L0 + T:
-            cap = _round_up(L0 + T, self.KV_CACHE_STEP)
+            drop, cap = kv_cache_plan(L0, T, starts, self.KV_CACHE_STEP)
             nbuf = self._new((B, cap, H, W, 2 * HD))
-            if L0:
-                self.copy_frames(buf, 0, L0, dst=nbuf, dst_t0=0)
-            buf = nbuf
+            if L0 > drop:
+                self.copy_frames(buf, drop, L0 - drop, dst=nbuf, dst_t0=0)
+            buf, L0, starts = nbuf, L0 - drop, tuple(s - drop for s in starts)
         buf[:, L0:L0 + T].copy_(qkv[..., HD:])           # the '(kv h d)' two thirds of each '(qkv h d)' row
         L = L0 + T
-        ss.put("kv", (buf, L))
-        a = AttnArgs(qkv=_ptr(buf), out=None, mem_kv=_ptr(p["mem_kv"]), dtype=_dt(self.dtype), heads=p["heads"],
-                     dim_head=p["dim_head"], n_mem=p["n_mem"], causal=1, n_outer=B, n_inner=HW, L=L,
-                     outer_stride=buf.shape[1] * HW, inner_stride=1, tok_stride=HW)
-        self._call("mv2_attention_tail", C.byref(a), _ptr(qkv), T * HW, L0, _ptr(o), T * HW)
+        ss.put("kv", (buf, L, starts))
+        cap, es = buf.shape[1], buf.element_size()
+        for r0, r1, s in row_runs(starts):
+            a = AttnArgs(qkv=_ptr(buf) + (r0 * cap + s) * HW * 2 * HD * es, out=None, mem_kv=_ptr(p["mem_kv"]),
+                         dtype=_dt(self.dtype), heads=p["heads"], dim_head=p["dim_head"], n_mem=p["n_mem"], causal=1,
+                         n_outer=r1 - r0, n_inner=HW, L=L - s, outer_stride=cap * HW, inner_stride=1, tok_stride=HW)
+            self._call("mv2_attention_tail", C.byref(a), _ptr(qkv) + r0 * T * HW * C3 * es, T * HW, L0 - s,
+                       _ptr(o) + r0 * T * HW * HD * es, T * HW)
         return o
 
     def attention_dropout_mask(self, n_seq, heads, L, n_mem, dropout: _lib.DropoutArgs):

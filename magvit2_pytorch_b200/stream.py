@@ -12,6 +12,11 @@ gateloop the fp32 scan state.  The kernels read that state in place (DESIGN.md 3
     video = torch.cat([dec.push(c) for c in codes.split(1, dim=1)], dim=2)   # == tok.decode_from_code_indices(codes)
 
 With tok.cuda_graphs set, a stream replays its pushes as CUDA graphs (PushPlan) once it has seen a push of the same shape.
+
+The rows of a stream are independent clips, and restart() starts single rows over, so one batched stream serves sessions
+that begin and end at different times:
+
+    dec.restart([2], cond=new_cond_row)      # row 2 starts a new clip at the next push
 """
 from __future__ import annotations
 
@@ -49,6 +54,24 @@ def decoder_chunk_frames(n: int, tdf: int, first_push: bool, first_frame: bool) 
     if n < 1:
         raise ValueError(f"a decoder push takes at least one latent frame, got {n}")
     return tdf * n - (tdf - 1 if first_push and first_frame else 0)
+
+
+def restart_rows(rows, batch_size: int) -> list:
+    """The row indices of a restart (a sequence of ints or a 1-D integer tensor) as a list; ValueError unless they are
+    distinct and in [0, batch_size)."""
+    if isinstance(rows, torch.Tensor):
+        if rows.ndim != 1 or rows.dtype.is_floating_point or rows.dtype.is_complex or rows.dtype == torch.bool:
+            raise ValueError(f"rows must be a 1-D integer tensor, got {rows.dtype} {tuple(rows.shape)}")
+        rows = rows.tolist()
+    else:
+        rows = list(rows)
+        if any(isinstance(r, bool) or not isinstance(r, int) for r in rows):
+            raise ValueError(f"rows must be integers, got {rows}")
+    if any(r < 0 or r >= batch_size for r in rows):
+        raise ValueError(f"rows must lie in [0, {batch_size}), got {rows}")
+    if len(set(rows)) != len(rows):
+        raise ValueError(f"rows must be distinct, got {rows}")
+    return rows
 
 
 class PushPlan:
@@ -116,7 +139,11 @@ class _Stream:
         self.model = model
         self.batch_size = int(batch_size)
         self.first_frame = bool(video_contains_first_frame)
-        self.cond = model._check_cond(cond, self.batch_size)
+        # the stream's own copy, in fp32 as the cond stems read it: restart() writes rows of it in place, so captured
+        # pushes keep reading it
+        cond = model._check_cond(cond, self.batch_size)
+        self.cond = None if cond is None else cond.detach().to(torch.float32, copy=True).contiguous()
+        self._restarted = set()      # rows restarted since the last push
         self.state = StreamState()
         # an fp32 model's precision is read from torch's TF32 switch once, here: every push runs in it, so the pushes still
         # give the outputs of one whole-clip call in that precision bit for bit
@@ -170,6 +197,35 @@ class _Stream:
             out = plan.replay(x)
         return out.clone()
 
+    def restart(self, rows, cond=None):
+        """Rows `rows` (distinct indices, a list or a 1-D integer tensor) start new clips at the next push; the other rows
+        carry on.  cond: (len(rows), dim_cond), the new clips' cond, required exactly when the model has cond layers.
+
+        From the next push on, a restarted row computes what a new batch_size=1 stream computes from its new clip's chunks,
+        and the other rows what they would without the restart.  Pushes keep their chunk rule: with a first frame, in a
+        restarted row's first push the first tdf - 1 frames of an encoder chunk are the clip's time padding (their values
+        are ignored, zeros are used) and the first tdf - 1 frames a decoder push returns are the padding that the
+        whole-clip decode drops.  Before the stream's first push a restart only replaces cond."""
+        m = self.model
+        if m.separate_first_frame_encoding and self.first_frame:
+            raise NotImplementedError(
+                "restart is not supported with separate_first_frame_encoding and a first frame: the first frame takes the "
+                "2-D conv for the whole push")
+        rows = restart_rows(rows, self.batch_size)
+        if m.has_cond:
+            if not isinstance(cond, torch.Tensor) or tuple(cond.shape) != (len(rows), m.dim_cond) \
+                    or not cond.dtype.is_floating_point:
+                got = f"{cond.dtype} {tuple(cond.shape)}" if isinstance(cond, torch.Tensor) else repr(cond)
+                raise ValueError(f"cond must be a float ({len(rows)}, {m.dim_cond}) tensor, got {got}")
+            if cond.device != m.device:
+                raise ValueError(f"cond is on {cond.device} but the tokenizer is on {m.device}")
+            if rows:
+                self.cond[rows] = cond.detach().to(self.cond.dtype)
+        if self.pushes and rows:
+            with torch.cuda.device(m.device):
+                self.state.restart_rows(rows)
+            self._restarted.update(rows)
+
     def _check_batch(self, t, what):
         if t.shape[0] != self.batch_size:
             raise ValueError(f"{what} has batch {t.shape[0]}, the stream was built for batch_size={self.batch_size}")
@@ -182,7 +238,8 @@ class TokenizeStream(_Stream):
     @torch.no_grad()
     def push(self, chunk: torch.Tensor) -> torch.Tensor:
         """chunk (B, C, n, H, W) float / bf16 / uint8 frames -> codes (B, n', H', W'[, num_codebooks]) of those frames:
-        n' = n // tdf, plus 1 on the first push of a stream with a first frame (which takes 1 + k * tdf frames)."""
+        n' = n // tdf, plus 1 on the first push of a stream with a first frame (which takes 1 + k * tdf frames).  With a
+        first frame, the first tdf - 1 frames of a row's chunk in its first push after a restart are read as zeros."""
         m = self.model
         if chunk.ndim != 5 or chunk.shape[1] != m.channels or tuple(chunk.shape[-2:]) != (m.image_size, m.image_size):
             raise ValueError(f"chunk must be (B, {m.channels}, n, {m.image_size}, {m.image_size}), got {tuple(chunk.shape)}")
@@ -194,8 +251,15 @@ class TokenizeStream(_Stream):
             def fn(v):
                 return eng.quantize_cl(eng.encode_cl(v, ff, self.cond, ss=self.state, sff_rest=sff_rest),
                                        want_quantized=False)[1]
-            codes = self._run(eng, fn, chunk.contiguous(), first, sff_rest)
+            x = chunk.contiguous()
+            if self._restarted and self.first_frame:
+                # the new clips' time padding, which the whole-clip call prepends as zero frames, on a copy of the chunk
+                x = x.clone()
+                for r in self._restarted:
+                    x[r, :, :m.time_padding].zero_()
+            codes = self._run(eng, fn, x, first, sff_rest)
         self.pushes += 1
+        self._restarted.clear()
         return codes
 
 
@@ -205,7 +269,8 @@ class DecodeStream(_Stream):
     @torch.no_grad()
     def push(self, codes: torch.Tensor) -> torch.Tensor:
         """codes (B, n', H', W'[, num_codebooks]) int64 / int32 -> frames (B, C, tdf * n', H, W) in the model dtype, less the
-        time_padding frames on the first push of a stream with a first frame."""
+        time_padding frames on the first push of a stream with a first frame.  With a first frame, the first tdf - 1
+        frames of a row in its first push after a restart are that padding, for the caller to drop."""
         m = self.model
         nc = m.quantizers.num_codebooks
         if codes.dtype not in (torch.long, torch.int32) or codes.ndim != (4 if nc == 1 else 5) or \
@@ -221,4 +286,5 @@ class DecodeStream(_Stream):
                 return eng.decode_cl(eng.codes_to_quantized_cl(c), ff, self.cond, ss=self.state, sff_rest=sff_rest)
             out = self._run(eng, fn, codes.contiguous(), first, sff_rest)
         self.pushes += 1
+        self._restarted.clear()
         return out
